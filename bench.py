@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- factor evals/s & GN-iters/s of the B200 hot path (BASELINE.json metric).
+"""bench.py -- factor evals/s & GN-iters/s of the H100 hot path (BASELINE.json metric).
 
 A "step" is one Levenberg-Marquardt / Gauss-Newton iteration of the sliding-window problem: evaluate
 every factor (residual + Jacobian) -> loss reweighting -> J^T J / J^T r -> landmark Schur complement
@@ -8,7 +8,7 @@ every factor (residual + Jacobian) -> loss reweighting -> J^T J / J^T r -> landm
 `value` = factors per second with everything resident in HBM; `e2e` = the same through
 hb200_optimize() with the variable blocks in pinned HOST memory (H2D + D2H inside the timed region).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--config 1] [--impl reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--config 1] [--impl reference] [--dump-outputs DIR]
 N > 1: launched by torch.distributed.run, one rank per GPU, weak scaling on the headline workload (each rank
 owns one cfg-sized factor shard of an N-times larger window) plus strong-scaling sections on the large
 BASELINE configs (cfg3: 500 k pixel factors, cfg4: 1 M factors) sharded over the N ranks.
@@ -46,6 +46,7 @@ def parse_args():
     p.add_argument("--no-large", action="store_true", help="skip the large-window sections (cfg2 / cfg3 / cfg4)")
     p.add_argument("--no-parity", action="store_true", help="skip the N-rank vs oracle check at N > 1")
     p.add_argument("--sweep", action="store_true", help="factor-count sweep of the 1 M-factor window (BASELINE config 5)")
+    p.add_argument("--dump-outputs", metavar="DIR", help="write the state the last timed step produced as DIR/<name>.npy (float64)")
     return p.parse_args()
 
 
@@ -54,7 +55,15 @@ def load_peaks():
     if os.path.exists(path):
         with open(path) as f:
             return json.load(f)["hbm_gbs"], "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
+
+
+def dump_outputs(out_dir, state):
+    """What a caller of the timed step receives: the window state after its last iteration (restored before every step,
+    so each step starts from the same inputs)."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in state.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.asarray(a, dtype=np.float64))
 
 
 def make_global_window(config, world):
@@ -293,7 +302,7 @@ def comm_entry(h, agg, reps_total=1):
     if ms:
         out["nvlink_algbw_gbs"] = pay / (ms * 1e-3) / 1e9
         out["nvlink_busbw_gbs"] = pay * 2 * (n - 1) / n / (ms * 1e-3) / 1e9
-        out["note"] = "payload is latency-bound (NVLink 5: 900 GB/s per direction); comm_ms is the launch-to-completion time of the all-reduce on the iteration stream, max wait for the slowest rank included"
+        out["note"] = "payload is latency-bound (H100 NVLink 4: 450 GB/s per direction); comm_ms is the launch-to-completion time of the all-reduce on the iteration stream, max wait for the slowest rank included"
     return out
 
 
@@ -413,7 +422,7 @@ def main():
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
 
-    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device="cuda")  # 256 MiB > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device="cuda")  # 256 MiB > 50 MB L2
     peak, peak_src = load_peaks()
 
     sampler = ClockSampler(local_rank)
@@ -429,6 +438,8 @@ def main():
     # ---- device-resident steps ---------------------------------------------------------------
     total_ms, launches = h.timed_steps(lambda: ctx.iterate(1, records=False), args.steps, max(args.warmup, 3), sampler if rank == 0 else None)
     ms_per_step = total_ms / args.steps
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, ctx.state())
     value = nf_total / (ms_per_step * 1e-3)
     info = ctx.comm_info()
 
@@ -473,22 +484,14 @@ def main():
     ab = algorithmic_bytes(win)
     dominant = max(kernel_ms, key=kernel_ms.get)
     roof_kernel = "factor_eval_kernel" if "factor_eval_kernel" in first else "pixel_eval_kernel"
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "traffic.json")
-    tj = {}
-    if os.path.exists(tpath):
-        with open(tpath) as f:
-            tj = json.load(f)
-        traffic = tj.get(roof_kernel + "_dram_bytes")
     roofline = roofline_entry(f"{roof_kernel}<{win.order},4,J,FUSE> -- the factor kernel of the timed graph (residual + Jacobian of every visual and inertial factor, fused pixel J^T J)",
                               ab[roof_kernel], first[roof_kernel], peak)
-    roofline.update(bound="hbm", peak=peak, unit="GB/s", traffic=traffic, peak_source=peak_src, dominant_kernel_by_time=dominant,
+    roofline.update(bound="hbm", peak=peak, unit="GB/s", peak_source=peak_src, dominant_kernel_by_time=dominant,
                     kernel_share_of_step=shares, launch_sequence=[n for n, _ in seq],
                     kernel_ms_source="hb200_profile_iteration: the graph's launch sequence run with a CUDA event after every launch (measured live)",
                     whole_step=dict(algorithmic_bytes=ab["factor_eval_kernel"], ms=ms_per_step, achieved=ab["factor_eval_kernel"] / (ms_per_step * 1e-3) / 1e9,
                                     frac=ab["factor_eval_kernel"] / (ms_per_step * 1e-3) / 1e9 / peak),
-                    note="cfg1 moves 7.8 MB per sweep (1.2 us at peak): latency-bound by construction (SURVEY.md 8d); large_windows holds the bandwidth-relevant fractions of the same in-iteration kernels",
-                    traffic_note="dram__bytes_read + write of one launch from the committed ncu capture (profiles/traffic.json): far below the algorithmic bytes at cfg1 because the 7 MB of residuals / Jacobians the launch writes stay in the 126 MB L2 until the J^T J / Schur kernels have consumed them; on the 1M-factor window the same kernels write through (profiles/r02_ncu_full.md)")
+                    note="cfg1 moves 7.8 MB per sweep (2.3 us at 3.35 TB/s): latency-bound by construction (SURVEY.md 8d); large_windows holds the bandwidth-relevant fractions of the same in-iteration kernels")
     try:
         roofline["fp64_peak_tflops_measured"] = ctx.measure_fp64_peak()
     except Exception as e:  # noqa: BLE001
@@ -564,8 +567,6 @@ def main():
             if rank == 0:
                 key = f"cfg{config}" + (f"_x{scale:g}" if scale != 1.0 else "")
                 large[key] = sec
-        if rank == 0 and tj.get("large_window"):
-            large["ncu_traffic"] = tj["large_window"]
 
     if rank != 0:
         if world > 1:

@@ -1,4 +1,4 @@
-// libhyperb200.so -- C-ABI (include/hyperb200.h) over the sm_100a kernels.
+// libhyperb200.so -- C-ABI (include/hyperb200.h) over the sm_90a kernels.
 // Host-side bookkeeping mirrors what the reference's CeresOptimizer keeps in ceres::Problem
 // (reference internal/hyper/optimizers/ceres/optimizer.cpp:189-382) but flattened: one set of
 // device arrays per variable family and two factor lists.
@@ -319,9 +319,9 @@ int check_launch(hb200_ctx* c, const char* what) {
 // Launch on the context's stream as a PROGRAMMATIC dependent of the previous kernel in that stream: the grid may become
 // resident while its predecessor still runs and blocks in pdl_wait() until the predecessor has completed (inside stream
 // capture the edge becomes a programmatic graph dependency).  Only for kernels whose sole dependency is that predecessor
-// and that call pdl_wait() first.  OFF by default: measured at cfg1 (profiles/r02_experiments.md) the step got slower
-// (0.164 vs 0.155 ms) with the four single-dependency edges of the iteration (knot table -> factors, solve ->
-// back-substitution -> trial factors -> accept) made programmatic; HB200_PDL=1 switches it on.
+// and that call pdl_wait() first.  OFF by default: at cfg1 the step got slower with the four single-dependency edges
+// of the iteration (knot table -> factors, solve -> back-substitution -> trial factors -> accept) made programmatic;
+// HB200_PDL=1 switches it on.
 template <typename... KArgs, typename... Args>
 cudaError_t launch_dependent(hb200_ctx* c, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, Args&&... args) {
   static const bool off = !(getenv("HB200_PDL") != nullptr && atoi(getenv("HB200_PDL")) != 0);
@@ -488,7 +488,7 @@ int launch_pixel(hb200_ctx* c, int sel, bool accumulate = false) {
   if (J && accumulate) {
     // optional (HB200_PIX_TILES): a CTA walks several consecutive tiles and flushes its J^T J accumulators once per knot base
     static const int tiles_env = getenv("HB200_PIX_TILES") ? atoi(getenv("HB200_PIX_TILES")) : 0;
-    a.tiles_per_cta = tiles_env > 0 ? tiles_env : 1;   // measured on the 1 M-factor window: 1 tile 0.41 ms, 11 tiles 0.50 ms (fewer, longer CTAs lose more than the saved atomics win)
+    a.tiles_per_cta = tiles_env > 0 ? tiles_env : 1;   // one tile per CTA: on the 1 M-factor window fewer, longer CTAs lose more than the saved atomics win
     const int grid = (c->n_pix_blocks + a.tiles_per_cta - 1) / a.tiles_per_cta;
     pixel_eval_kernel<K, J, J><<<grid, kEvalThreads, 0, c->stream>>>(a, c->basis);
   } else pixel_eval_kernel<K, J, false><<<c->n_pix_blocks, kEvalThreads, 0, c->stream>>>(a, c->basis);
@@ -593,12 +593,11 @@ int enqueue_build(hb200_ctx* c, bool pixel_fused = false) {
   { const int rf = fork_side(c); if (rf) return rf; }   // (no-op when already forked or while profiling)
   if (c->Ni) {
     // large windows (>= 16 384 inertial factors): the augmented product on the FP64 tensor cores, ~6 CTAs per SM of 8-factor
-    // chunks (1 M-factor window: 0.295 -> 0.16 ms); small windows: the scalar block-by-block kernel on short runs (cfg1, ~9
-    // factors per CTA: 16.4 vs 18.3 us).  HB200_IMU_HESS=0 / 1 forces the scalar / tensor-core kernel (A/B switch)
+    // chunks; small windows: the scalar block-by-block kernel on short runs (cfg1, ~9 factors per CTA), which is faster
+    // there.  HB200_IMU_HESS=0 / 1 forces the scalar / tensor-core kernel (A/B switch)
     static const int hess_env = getenv("HB200_IMU_HESS") != nullptr ? atoi(getenv("HB200_IMU_HESS")) : -1;
     const bool scalar_hess = hess_env >= 0 ? hess_env == 0 : c->Ni < 16384;
-    // (order 6 keeps the configuration it was measured with: 12-factor chunks, ~2 CTAs per SM -- order-6 window 0.045 ms; with
-    // 8-factor chunks and ~6 CTAs per SM 0.053 ms)
+    // (order 6 keeps 12-factor chunks at ~2 CTAs per SM, which beat 8-factor chunks at ~6 CTAs per SM on the order-6 window)
     const int splits = (scalar_hess || c->k != 4) ? c->imu_splits : c->imu_splits_mma;
     const int grid = c->nruns * splits;
     if (scalar_hess) {
@@ -900,7 +899,7 @@ int create_impl(const hb200_options* options, hb200_ctx* c) {
   HB_CUDA(cudaSetDevice(c->device));
   cudaDeviceProp prop{};
   HB_CUDA(cudaGetDeviceProperties(&prop, c->device));
-  if (prop.major < 10) return fail(-5, "device sm_%d%d is not Blackwell (built for sm_100a only)", prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) return fail(-5, "device sm_%d%d is not Hopper (built for sm_90a only)", prop.major, prop.minor);
   c->num_sms = prop.multiProcessorCount;
   c->use_graph = options ? options->use_graph != 0 : true;
   c->force_dense = options ? (options->reserved & 1) != 0 : false;

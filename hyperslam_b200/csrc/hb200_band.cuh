@@ -1,4 +1,4 @@
-// Block-banded + arrowhead Cholesky solve of the reduced system (sm_100a), one CTA.
+// Block-banded + arrowhead Cholesky solve of the reduced system (sm_90a), one CTA.
 //
 // After the landmark Schur complement the reduced system of a spline window is
 //   S = [ P  A^T ]   P: 6x6 control-point blocks, block half-bandwidth beta (= longest landmark track
@@ -475,7 +475,7 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
     t_g[1] = clock64();
     // arrow rows + the right-hand-side row (row m): one warp per row, lanes along the columns (rows of A are contiguous in
     // the packed system) -- chain 0 reads columns 0 .. N0-1, chain 1 the mirrored ones; six loads per lane in flight.
-    // (An element-indexed loop through sys_index() spent 9 of the gather's 13.6 us here at K = 50.)
+    // (An element-indexed loop through sys_index() spent most of the gather's time here at K = 50.)
     {
       const int N0 = C0.npc, n1v = 6 * C1.Ke;
       const double* Arows = sys + lay.oA;

@@ -1,8 +1,8 @@
-// Multi-CTA solve of the reduced system for LONG windows (sm_100a): block cyclic reduction.
+// Multi-CTA solve of the reduced system for LONG windows (sm_90a): block cyclic reduction.
 //
 // band_solve_kernel factors the block-banded + arrowhead system (SysLayout) in ONE CTA: K/2 + beta dependent
-// block-column steps, 0.6 ms at K = 200 and 1.4 ms at K = 500 -- more than every other kernel of the iteration
-// together, and replicated on every rank of a multi-GPU solve.  Here the chain is replaced by a tree.
+// block-column steps, which at K = 200 .. 500 takes longer than every other kernel of the iteration together,
+// and replicated on every rank of a multi-GPU solve.  Here the chain is replaced by a tree.
 // The pose part is cut into super-blocks of beta control points (nb = 6 beta dofs): a half-bandwidth of beta
 // blocks makes the super-block matrix block-TRIDIAGONAL (D_j on the diagonal, B_j = A[j+1][j] below it), with the
 // arrow rows F_j (m x nb) and the corner C (m x m) attached.  Cyclic reduction eliminates every other

@@ -1,4 +1,4 @@
-// Calibration-block Jacobians (sm_100a), produced on demand -- the sensor blocks are constant in the live
+// Calibration-block Jacobians (sm_90a), produced on demand -- the sensor blocks are constant in the live
 // configuration (reference internal/hyper/optimizers/ceres/optimizer.cpp:59-63), so the iteration kernels never
 // carry them; the reference's own gradient tests however run with every sensor manifold non-constant
 // (reference tests/internal/tests/optimizers/evaluators/pixel.cpp:57), and hb200_factor_evaluate hands these

@@ -1,4 +1,4 @@
-// Factor evaluation kernels (sm_100a): knot table, index maps, stereo-pixel and inertial
+// Factor evaluation kernels (sm_90a): knot table, index maps, stereo-pixel and inertial
 // residual + Jacobian.  One factor per thread; a CTA's knot-table tile is staged to shared memory
 // with one TMA bulk copy (cp.async.bulk + mbarrier).  Replaces, for a whole factor list at once,
 //   ExteroceptiveCost::Evaluate           reference internal/hyper/optimizers/ceres/costs/exteroceptive.cpp:101-160
@@ -237,10 +237,10 @@ HB_DI double huber_rho(double s, double delta, double* weight) {
 // ---------------------------------------------------------------------------------------------
 // Pixel factor (a5 + a3 + a7..a10 fused).  T: table origin (row r at T + r*kTabStride).
 // ---------------------------------------------------------------------------------------------
-// 256-bit global store (SASS STG.E.256): p must be 32-byte aligned.  Writes whole 32 B sectors, so a
-// thread-per-factor row store costs one L2 sector write per 32 B instead of two half-filled ones.
+// One 32-byte sector of a Jacobian row as two back-to-back 128-bit stores (STG.E.128, the widest global store
+// sm_90 has): p must be 32-byte aligned, so both halves land in the same L2 sector.
 HB_DI void st_v4(double* p, double a, double b, double c, double d) {
-  asm volatile("st.global.v4.f64 [%0], {%1, %2, %3, %4};" ::"l"(p), "d"(a), "d"(b), "d"(c), "d"(d) : "memory");
+  asm volatile("st.global.v2.f64 [%0], {%1, %2};\n\tst.global.v2.f64 [%0+16], {%3, %4};" ::"l"(p), "d"(a), "d"(b), "d"(c), "d"(d) : "memory");
 }
 
 // kind 0: pixel residual (reference pixel.cpp:16-146 + CartesianMetric); kind 1: bearing residual
@@ -409,8 +409,8 @@ struct PixelArgs {
 //     tiles (lower triangle only), the contraction runs over the rows of one knot base in steps of 4, rows
 //     of other bases inside the sub-tile are masked to zero.  Fragments: lane l holds A[m = l/4][k = l%4] =
 //     J[k][m] and B[k = l%4][n = l/4] = J[k][n] -- the same shared-memory access pattern -- and
-//     C[m = l/4][n = 2 (l%4) + {0,1}].  This replaced a scalar 3x3-register-tile loop that executed ~9 000
-//     instructions per warp (ncu smsp__inst_executed, profiles/) against ~1 400 for the factor evaluation itself.
+//     C[m = l/4][n = 2 (l%4) + {0,1}].  This replaced a scalar 3x3-register-tile loop that executed several
+//     times as many instructions per warp as the factor evaluation itself.
 // J^T J tiles / gradient entry a thread carries across the tiles of one knot base (registers)
 template <int K>
 struct PixelHessAcc {

@@ -1,4 +1,4 @@
-// Device-side fixed-size math for the sm_100a hot path (FP64, row-major 3x3, everything in
+// Device-side fixed-size math for the sm_90a hot path (FP64, row-major 3x3, everything in
 // registers after full unrolling).  Conventions are those of DESIGN.md: quaternion [x y z w],
 // global rotation tangent R <- Exp(theta) R, split SE3 tangent [theta | rho].
 #pragma once

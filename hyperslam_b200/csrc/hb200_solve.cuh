@@ -1,5 +1,5 @@
 // Normal equations, landmark Schur complement, dense Cholesky, back-substitution, retraction and
-// LM step control (sm_100a).  Replaces the inside of ceres::Solve for the reference's problem
+// LM step control (sm_90a).  Replaces the inside of ceres::Solve for the reference's problem
 // (reference internal/hyper/optimizers/ceres/optimizer.cpp:38-54,276-280): loss correction
 // (Huber 0.5 / ScaledLoss 1.6e-5, optimizer.cpp:226,267-268), J^T J / J^T r, the linear solve
 // (SPARSE_NORMAL_CHOLESKY there, landmark Schur + dense Cholesky here), Manifold::Plus

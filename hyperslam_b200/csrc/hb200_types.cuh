@@ -1,4 +1,4 @@
-// Shared host/device declarations for libhyperb200 (sm_100a).
+// Shared host/device declarations for libhyperb200 (sm_90a).
 #pragma once
 #include <cstdint>
 

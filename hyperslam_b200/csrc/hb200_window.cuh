@@ -1,4 +1,4 @@
-// Device-side sliding-window bookkeeping (sm_100a): what the reference does per message on its pointer graph --
+// Device-side sliding-window bookkeeping (sm_90a): what the reference does per message on its pointer graph --
 // appending state elements by extrapolation (reference internal/hyper/optimizers/abstract.cpp:118-144), adding
 // residual blocks (reference internal/hyper/optimizers/ceres/optimizer.cpp:189-274), dropping landmarks whose
 // observation range left the window together with their residuals (optimizer.cpp:360-382), setting state elements

@@ -1,4 +1,4 @@
-// hyper::Optimizer<B200> and the Ceres-shaped cost functor over libhyperb200
+// hyper::Optimizer<H100> and the Ceres-shaped cost functor over libhyperb200
 // (mirrors reference include/hyper/optimizers/{abstract,ceres/optimizer}.hpp and
 //  include/hyper/optimizers/ceres/costs/exteroceptive.hpp; see INTEGRATION.md).
 #pragma once
@@ -65,7 +65,7 @@ class ExteroceptiveCost final : public CostFunction {
 
 struct IterationSummary { double cost, cost_new, rho, radius; bool accepted, spd; };
 
-class Optimizer {   // OptimizerSuite::B200
+class Optimizer {   // OptimizerSuite::H100
  public:
   explicit Optimizer(int device = 0);
   ~Optimizer();

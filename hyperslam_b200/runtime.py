@@ -1,6 +1,6 @@
 """ctypes binding of libhyperb200.so (include/hyperb200.h) -- the only way Python reaches the hot path.
 
-There is no CPU fallback: constructing a Context without the built library or without a B200
+There is no CPU fallback: constructing a Context without the built library or without an H100
 raises.  The oracle under oracle/ is never imported from here.
 """
 from __future__ import annotations

@@ -1,8 +1,8 @@
-/* hyperb200.h -- C-ABI of the B200-native HyperSLAM hot path (libhyperb200.so).
+/* hyperb200.h -- C-ABI of the H100-native HyperSLAM hot path (libhyperb200.so).
  *
  * Drop-in boundary (SURVEY.md section 8b): one context owns the flattened sliding window that the
  * reference's optimizer holds as a pointer graph, and runs what ceres::Solve runs per iteration --
- * every residual block's Evaluate(), the normal equations and the linear solve -- as batched sm_100a
+ * every residual block's Evaluate(), the normal equations and the linear solve -- as batched sm_90a
  * kernels.  All pointers are plain host pointers unless a name says "device"; buffers are copied in
  * or out, never aliased across calls.  Every function returns 0 on success, <0 for an invalid
  * argument, >0 for a CUDA / numerical failure; hb200_last_error_string() describes the last one.

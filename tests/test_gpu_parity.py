@@ -1,4 +1,4 @@
-"""GPU-vs-oracle parity through the C-ABI (the parity tests proper; need a B200).
+"""GPU-vs-oracle parity through the C-ABI (the parity tests proper; need an H100).
 
 Tolerances follow BASELINE.json north_star: bit-exact factor/knot indexing, residuals within
 1e-6 relative, Jacobians within 1e-4 relative (we assert far tighter: both paths are FP64).

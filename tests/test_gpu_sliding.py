@@ -118,7 +118,11 @@ class HostWindow:
 @pytest.mark.parametrize("drop_inertial", [True, False])
 def test_sliding_sequence_matches_host_rules_and_oracle(built, drop_inertial):
     K0, frames, width = 14, (20 if drop_inertial else 8), 9
-    full = synthetic.make_window(order=4, num_knots=K0 + 20 + 2, num_landmarks=220, frames_per_landmark=5, num_imu=1500, seed=synthetic.SEED_BASE + 1234)
+    # bias knots every 1 s: with the default 10 s a sub-second window sits inside one bias segment, its four control points
+    # are nearly collinear, and once the trust region reaches its 1e16 cap a 1e-15 change of the knots moves the oracle's own
+    # accel-bias solution by up to 7e-7 relative -- any summation order other than the oracle's could then miss the 1e-6 bound
+    full = synthetic.make_window(order=4, num_knots=K0 + 20 + 2, num_landmarks=220, frames_per_landmark=5, num_imu=1500, seed=synthetic.SEED_BASE + 1234,
+                                 bias_dt=1.0)
     hw = HostWindow(full, K0)
     lo, hi = hw.valid_range()
     nv, ni, new_ids = hw.take_new(lo, hi)

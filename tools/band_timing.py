@@ -1,6 +1,6 @@
 import os, sys, ctypes as C
 os.environ["HB200_BAND_TIMING"]="1"
-sys.path.insert(0,"/root/repo")
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 from hyperslam_b200 import runtime, synthetic
 win = synthetic.make_config(int(os.environ.get("HB200_CFG", "1")), constant_knots=2)

@@ -1,5 +1,5 @@
 import os, sys, time
-sys.path.insert(0, "/root/repo")
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from hyperslam_b200 import runtime, synthetic
 win = synthetic.make_config(1, constant_knots=2)

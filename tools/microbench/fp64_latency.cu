@@ -1,6 +1,6 @@
-// Micro-benchmarks that calibrate the latency model of the single-CTA band solver on B200:
+// Micro-benchmarks that calibrate the latency model of the single-CTA band solver on H100:
 // dependent-chain latency and per-warp issue interval of DFMA, rsqrt(double), LDS, SHFL, and the cost
-// of bar.sync with 5 / 16 warps.  Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o fp64_latency fp64_latency.cu
+// of bar.sync with 5 / 16 warps.  Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o fp64_latency fp64_latency.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 
