@@ -334,6 +334,16 @@ cudaError_t launch_dependent(hb200_ctx* c, void (*kernel)(KArgs...), dim3 grid, 
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 
+// Launch configuration of the resident band solver: a grid of one 2-CTA cluster (chain r in CTA r) on the context's
+// stream, the whole workspace in each CTA's shared memory.  at: storage for the cluster-dimension attribute.
+void band_cluster_config(hb200_ctx* c, cudaLaunchConfig_t* cfg, cudaLaunchAttribute* at) {
+  cfg->gridDim = dim3(2); cfg->blockDim = dim3(kBandThreads); cfg->stream = c->stream;
+  cfg->dynamicSmemBytes = band_workspace_doubles(c->K, c->beta, c->n - 6 * c->K) * sizeof(double);
+  at[0].id = cudaLaunchAttributeClusterDimension;
+  at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+  cfg->attrs = at; cfg->numAttrs = 1;
+}
+
 cudaStream_t side(hb200_ctx* c) { return c->forked ? c->stream2 : c->stream; }
 int fork_side(hb200_ctx* c) {
   static const bool no_fork = getenv("HB200_NO_FORK") != nullptr;   // A/B switch for measurements
@@ -421,8 +431,16 @@ int ensure_system(hb200_ctx* c) {
     }
   }
   if (c->band_solver && !c->use_bcr) {
-    if (c->band_smem) HB_CUDA(cudaFuncSetAttribute(band_solve_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(ws)));
-    else {
+    if (c->band_smem) {
+      // resident workspace: one chain per CTA of a 2-CTA cluster, ws bytes of shared memory in each
+      HB_CUDA(cudaFuncSetAttribute(band_solve_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(ws)));
+      cudaLaunchConfig_t cfg{};
+      cudaLaunchAttribute at[1];
+      band_cluster_config(c, &cfg, at);
+      int nclusters = 0;
+      HB_CUDA(cudaOccupancyMaxActiveClusters(&nclusters, band_solve_kernel<true>, &cfg));
+      if (nclusters < 1) return fail(-6, "band solver: a cluster of 2 CTAs x %d threads with %zu B of shared memory each cannot be resident", kBandThreads, ws);
+    } else {
       HB_CUDA(c->band_ws.ensure(ws / sizeof(double)));
       // chunked factorisation: two shared-memory views of band_chunk_cols block columns (band + arrow + LI)
       const size_t colbytes = (static_cast<size_t>(6 + 6 * c->beta) * 6 + 6 * static_cast<size_t>(c->n - 6 * c->K + 1) + 48) * sizeof(double);
@@ -436,7 +454,7 @@ int ensure_system(hb200_ctx* c) {
   HB_CUDA(c->band_ws.ensure(1));
   if (!c->band_solver) { int rc = ensure_dense(c); if (rc) return rc; }
   if (getenv("HB200_BAND_TIMING")) {
-    HB_CUDA(c->band_dbg.ensure(72));
+    HB_CUDA(c->band_dbg.ensure(144));   // 72 per CTA of the cluster kernel
     long long variant = getenv("HB200_BCR_VARIANT") ? atoll(getenv("HB200_BCR_VARIANT")) : 0;
     HB_CUDA(cudaMemcpy(c->band_dbg.p + 71, &variant, sizeof(variant), cudaMemcpyHostToDevice));
   }
@@ -679,9 +697,12 @@ int enqueue_solve(hb200_ctx* c, bool fuse_retract = false, bool* fused = nullptr
     const SolverState* st = c->st.p;
     const unsigned char* fx = c->fixed.p;
     double* Dout = c->D.p;
-    const size_t smem = c->band_smem ? band_workspace_doubles(c->K, c->beta, c->n - 6 * c->K) * sizeof(double) : 0;
-    if (c->band_smem) band_solve_kernel<true><<<1, kBandThreads, smem, c->stream>>>(c->sys.p, c->lay, c->band_ws.p, c->dp.p, c->spd.p, c->band_dbg.p, st, fx, Dout, 0);
-    else band_solve_kernel<false><<<1, kBandThreads, c->band_chunk_smem, c->stream>>>(c->sys.p, c->lay, c->band_ws.p, c->dp.p, c->spd.p, c->band_dbg.p, st, fx, Dout, c->band_chunk_cols);
+    if (c->band_smem) {
+      cudaLaunchConfig_t cfg{};
+      cudaLaunchAttribute at[1];
+      band_cluster_config(c, &cfg, at);
+      HB_CUDA(cudaLaunchKernelEx(&cfg, band_solve_kernel<true>, static_cast<const double*>(c->sys.p), c->lay, c->band_ws.p, c->dp.p, c->spd.p, c->band_dbg.p, st, fx, Dout, 0));
+    } else band_solve_kernel<false><<<1, kBandThreads, c->band_chunk_smem, c->stream>>>(c->sys.p, c->lay, c->band_ws.p, c->dp.p, c->spd.p, c->band_dbg.p, st, fx, Dout, c->band_chunk_cols);
     HB_LAUNCH(c, "band_solve_kernel");
   } else {
     { const int rd = enqueue_densify(c); if (rd) return rd; }
@@ -2147,9 +2168,9 @@ int hb200_interpolate(hb200_ctx* c, int n, const double* stamps, double* pose, d
   return 0;
 }
 
-int hb200_debug_band_timing(hb200_ctx* c, long long* cycles /*[72]: 8 phase totals + 8 steps x 8 raw stamps*/) {
+int hb200_debug_band_timing(hb200_ctx* c, long long* cycles /*[144]: per CTA, 8 phase totals + 8 steps x 8 raw stamps*/) {
   if (!c || !c->band_dbg.p) return fail(-2, "set HB200_BAND_TIMING=1 before hb200_bind");
-  HB_CUDA(cudaMemcpy(cycles, c->band_dbg.p, 72 * sizeof(long long), cudaMemcpyDeviceToHost));
+  HB_CUDA(cudaMemcpy(cycles, c->band_dbg.p, 144 * sizeof(long long), cudaMemcpyDeviceToHost));
   return 0;
 }
 

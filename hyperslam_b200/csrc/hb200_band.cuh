@@ -1,19 +1,20 @@
-// Block-banded + arrowhead Cholesky solve of the reduced system (sm_90a), one CTA.
+// Block-banded + arrowhead Cholesky solve of the reduced system (sm_90a): a 2-CTA cluster when the workspace is
+// resident in shared memory (one elimination chain per SM), one CTA over a global-memory workspace otherwise.
 //
 // After the landmark Schur complement the reduced system of a spline window is
 //   S = [ P  A^T ]   P: 6x6 control-point blocks, block half-bandwidth beta (= longest landmark track
 //       [ A  C   ]      measured in control points, >= k-1), A: m x 6K arrow (bias knots + gravity),
 //   C: m x m.  The reference hands the same structure to CHOLMOD through SPARSE_NORMAL_CHOLESKY
 //   (reference internal/hyper/optimizers/ceres/optimizer.cpp:46-48); here the factorisation,
-//   forward and backward substitution run in a single CTA with the whole band resident in shared
-//   memory (global-memory workspace when it does not fit).
+//   forward and backward substitution run with the whole band resident in shared memory (global-memory
+//   workspace, one CTA, when it does not fit).
 //
 // Two-sided elimination.  The factorisation is a chain of K dependent block-column steps, each bounded
 // by FP64 dependent-issue latency (a 6x6 potf2 plus a panel solve), not by throughput.  The chain is cut
 // in two: a separator of beta block columns in the middle decouples the columns above it from the
 // columns below it, so chain 0 eliminates block columns 0 .. Kt-1 top-down while chain 1 eliminates
-// K-1 .. Kt+beta bottom-up IN THE SAME STEPS (same barriers, disjoint warps, one look-ahead warp per
-// chain on its own scheduler).  Chain 1 runs the very same code on the index-reversed matrix J P J
+// K-1 .. Kt+beta bottom-up IN THE SAME STEPS (resident: chain r on CTA r of a cluster; global workspace:
+// same barriers, disjoint warps; one look-ahead warp per chain on its own scheduler).  Chain 1 runs the very same code on the index-reversed matrix J P J
 // (still block-banded) and accumulates its Schur updates of the separator and of the separator's
 // arrow columns into a private, zero-initialised copy.  The copies are then merged into chain 0, which
 // eliminates the beta separator columns, and the back substitution runs outwards from the separator
@@ -111,6 +112,34 @@ HB_DI long long clock_after(double dep) {
 // Named barriers (ids 1..15; id 0 is __syncthreads): only the warps of one chain's pipeline take part.
 HB_DI void nbar_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 HB_DI void nbar_arrive(int id, int count) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory"); }
+
+// 2-CTA cluster of the resident solver.  The cluster barrier orders shared-memory accesses across the cluster
+// (release on arrive, acquire on wait); a peer CTA's shared memory is read through mapa + ld.shared::cluster.
+HB_DI int cluster_rank() { unsigned r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return static_cast<int>(r); }
+HB_DI void cluster_arrive() { asm volatile("barrier.cluster.arrive.release;" ::: "memory"); }
+HB_DI void cluster_wait() { asm volatile("barrier.cluster.wait.acquire;" ::: "memory"); }
+HB_DI unsigned peer_addr(const void* p, int rank) {
+  unsigned a;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(a) : "r"(static_cast<unsigned>(__cvta_generic_to_shared(p))), "r"(rank));
+  return a;
+}
+HB_DI double ld_peer(const double* p, int rank) {
+  double v;
+  asm volatile("ld.shared::cluster.f64 %0, [%1];" : "=d"(v) : "r"(peer_addr(p, rank)));
+  return v;
+}
+HB_DI void st_peer(double* p, int rank, double v) {
+  asm volatile("st.shared::cluster.f64 [%0], %1;" ::"r"(peer_addr(p, rank)), "d"(v) : "memory");
+}
+HB_DI int ld_peer(const int* p, int rank) {
+  int v;
+  asm volatile("ld.shared::cluster.s32 %0, [%1];" : "=r"(v) : "r"(peer_addr(p, rank)));
+  return v;
+}
+
+// Update warps per CTA of the cluster kernel (schedulers 0..2; the look-ahead warp has scheduler 3 to itself).  At cfg1
+// on an H100, 4 and 8 update warps gave the same step time within noise and 6 was ~1 us slower per solve.
+constexpr int kBandUpdWarps = 4;
 
 struct BandChain {
   double *W, *AR, *LI, *X;
@@ -324,17 +353,27 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
   extern __shared__ double s_band[];
   pdl_launch_dependents();   // the back-substitution grid behind the solve may become resident (it waits for this grid's completion)
   const long long t_entry = clock64();
+  // SMEM: the workspace is resident in shared memory and the kernel runs as a 2-CTA cluster, chain r in CTA r, each
+  // chain on its own SM (its own shared-memory crossbar and four schedulers).  Both CTAs lay out the whole workspace
+  // identically, so a peer's copy of anything sits at the local address mapped to the peer's rank.  CTA 0 also owns
+  // the corner.  !SMEM: one CTA runs both chains on chunked shared-memory views of a global workspace.
+  constexpr bool CL = SMEM;
+  const int rank = CL ? cluster_rank() : 0;
+  const bool has0 = !CL || rank == 0, has1 = !CL || rank == 1;
+  if (CL && dbg) dbg += 72 * rank;
   double* ws = SMEM ? s_band : ws_global;
   const int n = lay.n, K = lay.K, beta = lay.beta;
   const int np = 6 * K, m = n - np, h = 6 + 6 * beta, h6 = h * 6;
   const BandPlan pl = band_plan(K, beta);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  // Roles.  Each chain owns one scheduler for its latency-critical work (the arbiter favours the highest
+  // Roles (!CL).  Each chain owns one scheduler for its latency-critical work (the arbiter favours the highest
   // warp id of a scheduler): scheduler 0 = chain 0 (warp 12 look-ahead, warp 8 lane 0 block inverses),
   // scheduler 1 = chain 1 (warp 13, warp 9 lane 0); their other warps idle during the update phase.
   // The warps of schedulers 2 and 3 do the trailing updates: 2,3,6,7 -> chain 0, 10,11,14,15 -> chain 1.
+  // Roles (CL).  Warp 15 is the look-ahead warp, alone on scheduler 3 (warps 3, 7, 11 idle in the step loop); the
+  // first kBandUpdWarps warps of schedulers 0..2, in the order 0, 1, 2, 4, 5, 6, 8, ..., do panel rows and updates.
   const int sched = warp & 3;
-  const int my_chain = (sched < 2) ? sched : (warp >> 3);
+  const int my_chain = CL ? rank : ((sched < 2) ? sched : (warp >> 3));
   BandChain C0, C1;
   {
     double* p = ws;
@@ -373,7 +412,7 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
       const double dcl = damp ? fmin(fmax(diagH[a], 1e-6), 1e32) : 0.0;
       s_dmp[a] = mu * dcl;
       s_fix[a] = damp ? fixed[a] : 0;
-      if (damp) Dout[a] = dcl;
+      if (damp && has0) Dout[a] = dcl;
     }
   }
   __syncthreads();
@@ -394,7 +433,7 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
   {
     // Each element is one dependent L2 access; four per thread are kept in flight (values first, stores after):
     // a one-load-at-a-time loop spent 250 us here at K = 500.
-    const int N1 = C1.npc;
+    const int N1 = has1 ? C1.npc : 0;   // (CL: each CTA gathers its own chain only)
     auto gather4 = [&](int total, auto value, auto store) {
       for (int e0 = tid; e0 < total; e0 += 4 * kBandThreads) {
         double v[4];
@@ -428,9 +467,9 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
       // 6-row group q of block column c of the reversed band; its six entries are S[a][b0 .. b0+5] (a = np-1-(6c+j), b
       // descending with the row), contiguous in S.  Two units of each chain per thread and pass: twelve 128-bit loads in
       // flight before the first store.
-      const int nu0 = C0.ncol * h;
-      const int hq = h / 6, nu1 = C1.Ke * hq * 6;
-      for (int e = tid; e < (C1.ncol - C1.Ke) * h6; e += kBandThreads) C1.W[static_cast<size_t>(C1.Ke) * h6 + e] = 0.0;   // separator copy
+      const int nu0 = has0 ? C0.ncol * h : 0;
+      const int hq = h / 6, nu1 = has1 ? C1.Ke * hq * 6 : 0;
+      for (int e = tid; has1 && e < (C1.ncol - C1.Ke) * h6; e += kBandThreads) C1.W[static_cast<size_t>(C1.Ke) * h6 + e] = 0.0;   // separator copy
       for (int u0 = tid; u0 < max(nu0, nu1); u0 += 2 * kBandThreads) {
         double v[2][6], v1[2][6];
         int rowv[2], cv[2], av[2], b0v[2];
@@ -477,7 +516,7 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
     // the packed system) -- chain 0 reads columns 0 .. N0-1, chain 1 the mirrored ones; six loads per lane in flight.
     // (An element-indexed loop through sys_index() spent most of the gather's time here at K = 50.)
     {
-      const int N0 = C0.npc, n1v = 6 * C1.Ke;
+      const int N0 = has0 ? C0.npc : 0, n1v = has1 ? 6 * C1.Ke : 0;
       const double* Arows = sys + lay.oA;
       constexpr int NW = kBandThreads / 32;
       for (int r0 = warp; r0 <= m; r0 += 2 * NW) {   // two rows per warp and pass: 24 loads per lane in flight
@@ -513,7 +552,7 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
     }
     t_g[2] = clock64();
     t_g[3] = clock64();
-    for (int e = tid; e < (m + 1) * m; e += kBandThreads) {
+    for (int e = tid; has0 && e < (m + 1) * m; e += kBandThreads) {
       const int r = e / m, q = e - r * m;
       CC[static_cast<size_t>(r) * LDc + q] = (r < m) ? ((q <= r) ? Sval(np + r, np + q) : 0.0) : bval(np + q);
     }
@@ -526,11 +565,11 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
   // ---- two-sided factorisation + forward substitution: step s eliminates block column s of BOTH chains.
   // The 6x6 Cholesky of a chain's NEXT diagonal block is done by its look-ahead warp inside the
   // trailing-update phase, as soon as that block has received its update: off the critical path. ----
-  if (tid == 0 && C0.Ke > 0) { if (!chol6(C0.W, 6, C0.LI)) s_ok = 0; }
-  if (tid == 32 && C1.Ke > 0) { if (!chol6(C1.W, 6, C1.LI)) s_ok = 0; }
+  if (tid == 0 && has0 && C0.Ke > 0) { if (!chol6(C0.W, 6, C0.LI)) s_ok = 0; }
+  if (tid == 32 && has1 && C1.Ke > 0) { if (!chol6(C1.W, 6, C1.LI)) s_ok = 0; }
   __syncthreads();
   HB_TICK(0);
-  // Pipeline of one chain: 4 update warps (128 threads: panel rows, then trailing-update tiles) + its
+  // Pipeline of one chain: kWorkers update threads (panel rows, then trailing-update tiles) + its
   // look-ahead warp.  Barrier A: panel of step s complete (update warps sync, look-ahead warp arrives after
   // its first panel block); barrier B: step s complete.  The chains never synchronise with each other.
   __shared__ unsigned char s_tile[2 * 192];
@@ -551,16 +590,19 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
     }
   }
   __syncthreads();
-  const bool is_la = (sched < 2) && (warp >> 2) == 3;
-  const bool is_worker = sched >= 2;
-  const int wid = (((warp >> 2) & 1) * 2 + (sched - 2)) * 32 + lane;   // 0..127 within the chain's update warps
-  const int barA = 1 + 2 * my_chain, barB = 2 + 2 * my_chain;
+  const int uidx = (warp >> 2) * 3 + sched;   // CL: rank of a scheduler-0..2 warp among the update warps
+  const bool is_la = CL ? warp == 15 : (sched < 2) && (warp >> 2) == 3;
+  const bool is_worker = CL ? sched < 3 && uidx < kBandUpdWarps : sched >= 2;
+  const int wid = CL ? uidx * 32 + lane : (((warp >> 2) & 1) * 2 + (sched - 2)) * 32 + lane;   // 0..kWorkers-1
+  constexpr int kWorkers = CL ? 32 * kBandUpdWarps : 128;
+  const int barA = 1 + 2 * my_chain, barB = 2 + 2 * my_chain, nbar = kWorkers + 32;
+  const int rec_upd = CL ? 0 : 2, rec_la = CL ? 15 : 12;   // the update warp and the look-ahead warp whose steps are stamped
   __shared__ long long s_ts[8][8];
   // Two-sided phase: every step has the full band below it (the separator follows the last eliminated
   // column), so a worker's items are the same every step and their addresses are affine in s: decode once.
   constexpr int kMaxRounds = 3;
   const int nitems_full = ntiles_full * 6 - 6;   // tile 0 belongs to the look-ahead warp
-  const bool fast = have_table && pl.Kb > 0 && nitems_full <= kMaxRounds * 128;
+  const bool fast = have_table && pl.Kb > 0 && nitems_full <= kMaxRounds * kWorkers;
   // !SMEM: the workspace lives in global memory (it does not fit); the factorisation then runs chunk by chunk
   // on shared-memory VIEWS of chunk_cols block columns per chain (loaded, eliminated, written back), so its
   // steps see shared-memory latency instead of L2 latency.  V0 / V1 are the views, F the chain structure the
@@ -582,7 +624,7 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
   const double* f_u[kMaxRounds]; const double* f_v[kMaxRounds]; double* f_t[kMaxRounds]; int f_su[kMaxRounds]; bool f_ok[kMaxRounds];
 #pragma unroll
   for (int r = 0; r < kMaxRounds; ++r) {
-    const int t = 6 + wid + 128 * r;
+    const int t = 6 + wid + kWorkers * r;
     f_ok[r] = fast && is_worker && t < ntiles_full * 6;
     f_u[r] = F.W; f_v[r] = F.W; f_t[r] = F.W; f_su[r] = 0;
     if (f_ok[r]) {
@@ -621,22 +663,22 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
   // chol_last: the look-ahead of the last step also factors the next diagonal block (more columns follow)
   auto run_steps = [&](const BandChain& Q, int s0, int s1, bool use_fast, bool chol_last) {
     for (int s = s0; s < s1; ++s) {
-      const bool rec = dbg && my_chain == 0 && s >= 4 && s < 12 && lane == 0 && (warp == 2 || warp == 12);
-      if (rec) s_ts[s - 4][warp == 2 ? 0 : 4] = clock_after(Q.LI[static_cast<size_t>(s) * 48]);   // released (chol(s) visible)
+      const bool rec = dbg && (CL || my_chain == 0) && s >= 4 && s < 12 && lane == 0 && (warp == rec_upd || warp == rec_la);
+      if (rec) s_ts[s - 4][warp == rec_upd ? 0 : 4] = clock_after(Q.LI[static_cast<size_t>(s) * 48]);   // released (chol(s) visible)
       if (is_worker) {
         const int nb = min(h - 6, Q.npc - 6 * (s + 1));
-        band_panel(Q, s, h, m, wid, 128, nb >= 6 ? 6 : 0);
+        band_panel(Q, s, h, m, wid, kWorkers, nb >= 6 ? 6 : 0);
         if (rec) s_ts[s - 4][1] = clock_after(Q.AR[6 * s]);           // own panel row (arrow row 0... wid 0 -> band row 6) done
-        nbar_sync(barA, 160);
+        nbar_sync(barA, nbar);
         if (rec) s_ts[s - 4][2] = clock_after(Q.W[static_cast<size_t>(s) * h6 + 36]);   // A released
         if (use_fast) fast_update(s);
-        else band_update(Q, s, h, m, 6, wid, 128, have_table ? s_tile : nullptr, beta);
+        else band_update(Q, s, h, m, 6, wid, kWorkers, have_table ? s_tile : nullptr, beta);
         if (rec) s_ts[s - 4][3] = clock_after(Q.W[static_cast<size_t>(s + 1) * h6 + 36]);  // update done (approx)
       } else {
-        if (!band_la_step(Q, s, h, lane, s + 1 < s1 || chol_last, barA, 160)) s_ok = 0;
+        if (!band_la_step(Q, s, h, lane, s + 1 < s1 || chol_last, barA, nbar)) s_ok = 0;
         if (rec) s_ts[s - 4][5] = clock_after(Q.LI[static_cast<size_t>(s + 1) * 48]);      // chol(s+1) done
       }
-      nbar_sync(barB, 160);
+      nbar_sync(barB, nbar);
     }
   };
   // chunk transfer between a chain's global workspace G (columns c0 .. c0 + nview) and its view V, by the
@@ -682,10 +724,31 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
   else run_chunked(0, C0.Ke, C1.Ke, fast);
   __syncthreads();
   if (dbg && tid < 64) dbg[8 + tid] = s_ts[tid >> 3][tid & 7];
-  HB_TICKD(1, C0.W);
+  HB_TICKD(1, C.W);
+  // CL: CTA 1 stores chain 1's separator copy and its separator arrow columns into CTA 0's (unused) chain-1 storage at
+  // the same addresses: remote stores do not stall the way remote loads in the merge would.  Both chains are then
+  // eliminated (cluster barrier 1).  CTA 0 arrives on barrier 2 at once: it waits there for CTA 1's part of the corner
+  // update, and CTA 1 has nothing to wait for from CTA 0 until the corner is solved (barrier 3).
+  if (CL) {
+    if (rank == 1 && pl.Kb) {
+      const int nsep = 6 * pl.bs;
+      double* w = C1.W + static_cast<size_t>(C1.Ke) * h6;
+      for (int e = tid; e < pl.bs * h6; e += kBandThreads) st_peer(w + e, 0, w[e]);
+      for (int e = tid; e < (m + 1) * nsep; e += kBandThreads) {
+        const int r = e / nsep, v = e - r * nsep;
+        double* a = C1.AR + static_cast<size_t>(r) * C1.npc + 6 * C1.Ke + v;
+        st_peer(a, 0, *a);
+      }
+    }
+    cluster_arrive(); cluster_wait();
+    if (rank == 0) {
+      if (tid == 0 && !ld_peer(&s_ok, 1)) s_ok = 0;   // chain 1's SPD flag
+      cluster_arrive();
+    }
+  }
   // ---- merge chain 1's copy of the separator (index-reversed) and of its arrow columns into chain 0,
   // then chain 0's pipeline eliminates the separator columns ----
-  if (pl.Kb) {
+  if (pl.Kb && has0) {
     const int nsep = 6 * pl.bs, N1 = C1.npc;
     for (int e = tid; e < nsep * nsep; e += kBandThreads) {
       const int u = e / nsep, v = e - u * nsep;
@@ -719,12 +782,14 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
     if (ncc + C0.npc + C1.npc <= avail) { C0.X = p; C1.X = p + C0.npc; }
     __syncthreads();
   }
-  // ---- block inverses of every eliminated column (one thread each), and the deferred corner update
-  // C -= sum over all eliminated columns of (arrow panel)(arrow panel)^T, rhs row included (row m):
-  // one (u, v) pair per warp pass, lanes stride the columns (conflict-free), butterfly reduction ----
-  {
+  // ---- the deferred corner update C -= sum over all eliminated columns of (arrow panel)(arrow panel)^T, rhs row
+  // included (row m).  CL: each CTA contracts its own chain's columns; CTA 1 stores its partial sum in its (otherwise
+  // unused) corner storage, CTA 0 waits for it (cluster barrier 2) and subtracts its own partial, then CTA 1's, in
+  // this fixed order (no atomics across the cluster: replicas of the solve stay bit-identical) ----
+  if (CL && rank == 0) cluster_wait();
+  if (!CL || rank == 0 || pl.Kb) {
     // FP64 tensor-core tiles (mma.sync m8n8k4 -> SASS DMMA.8x8x4): output tile (ub, vb) of 8 x 8 corner entries,
-    // K = the eliminated columns of both chains in steps of 4.  Operand fragments: lane l holds
+    // K = the eliminated columns in steps of 4.  Operand fragments: lane l holds
     // A[row l/4][k l%4] and B[k l%4][col l/4] -- both are AR[row][col0 + l%4] -- and C[row l/4][col 2(l%4)+{0,1}].
     const int nrb = (m + 1 + 7) / 8, ncb = (m + 7) / 8;
     const int lr = lane >> 2, lk = lane & 3;
@@ -736,6 +801,7 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
       double c0 = 0.0, c1 = 0.0;
 #pragma unroll
       for (int ci = 0; ci < 2; ++ci) {
+        if (CL && ci != rank) continue;
         const BandChain& Q = ci ? C1 : C0;
         const int nused = ci ? 6 * C1.Ke : C0.npc;
         const int per = ((nused + 4 * nks - 1) / (4 * nks)) * 4;          // columns of this part (multiple of 4)
@@ -756,17 +822,28 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
         }
       }
       const int u = 8 * ub + lr, v = 8 * vb + 2 * lk;
-      if (u <= m && v < m && v <= u) atomicAdd(&CC[static_cast<size_t>(u) * LDc + v], -c0);
-      if (u <= m && v + 1 < m && v + 1 <= u) atomicAdd(&CC[static_cast<size_t>(u) * LDc + v + 1], -c1);
+      double* cu = CC + static_cast<size_t>(u) * LDc + v;
+      const bool in0 = u <= m && v < m && v <= u, in1 = u <= m && v + 1 < m && v + 1 <= u;
+      if (!CL) {
+        if (in0) atomicAdd(cu, -c0);
+        if (in1) atomicAdd(cu + 1, -c1);
+      } else if (rank == 1) {   // every corner entry belongs to one lane of one tile
+        if (in0) cu[0] = c0;
+        if (in1) cu[1] = c1;
+      } else {
+        if (in0) cu[0] = (cu[0] - c0) - (pl.Kb ? ld_peer(cu, 1) : 0.0);
+        if (in1) cu[1] = (cu[1] - c1) - (pl.Kb ? ld_peer(cu + 1, 1) : 0.0);
+      }
     }
   }
   __syncthreads();
   HB_TICKD(3, CC);
+  if (CL && rank == 1) cluster_arrive();
   // ---- corner (m x m, rhs carried as row m): right-looking Cholesky by the whole CTA with FIXED element
   // ownership (element (u, v), v <= min(u, m-1), decoded once), two barriers per column and no
   // division / modulo in the column loop.  The pivot's square root goes to XA's neighbour array DG so
   // that nobody overwrites CC[q][q] while others still read it. ----
-  {
+  if (has0) {
     double* DG = XA + m;   // diagonal of the corner factor
     const int ntri = m * (m + 1) / 2, nel = ntri + m;
     auto decode = [&](int e, int* pu, int* pv) {
@@ -861,10 +938,34 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
     }
   }
   __syncthreads();
+  // row transform of the eliminated columns (one row per thread): panel rows B <- B L^-1 and/or the rhs y <- y L^-1
+  auto row_transform = [&](bool panel, bool rhs) {
+    const int rows_per_col = (h - 6) + 1;
+    const int nc0 = has0 ? C0.ncol : 0, ncols = nc0 + (has1 ? C1.Ke : 0);
+    for (int e = tid; e < ncols * rows_per_col; e += kBandThreads) {
+      const int cc = e / rows_per_col, t = e - cc * rows_per_col;
+      const BandChain& Q = cc < nc0 ? C0 : C1;
+      const int c = cc < nc0 ? cc : cc - nc0;
+      const int nb = min(h - 6, Q.npc - 6 * (c + 1));
+      const double* L = Q.W + static_cast<size_t>(c) * h6;
+      const double* rd = Q.LI + static_cast<size_t>(c) * 48;
+      if (t < nb) { if (panel) band_transform_row(Q.W + (static_cast<size_t>(c) * h + 6 + t) * 6, L, rd); }
+      else if (t == h - 6 && rhs) band_transform_row(Q.AR + static_cast<size_t>(m) * Q.npc + 6 * c, L, rd);
+    }
+  };
+  if (CL && rank == 1) {
+    // chain 1's panel rows do not depend on the corner solution: transform them while CTA 0 solves the corner; CTA 0
+    // then stores the corner solution and the separator part of chain 0's solution here (cluster barrier 3)
+    row_transform(true, false);
+    __syncthreads();
+    HB_TICK(4);
+    cluster_wait();
+    cluster_arrive(); cluster_wait();
+  }
   HB_TICKD(5, XA);
   // arrow contribution to every eliminated block's right-hand side, all at once: y_p -= AR^T x_a (row m of AR = y)
   {
-    const int n0 = C0.npc, n1 = 6 * C1.Ke;
+    const int n0 = has0 ? C0.npc : 0, n1 = has1 ? 6 * C1.Ke : 0;
     for (int e = tid; e < n0 + n1; e += kBandThreads) {
       const BandChain& Q = e < n0 ? C0 : C1;
       const int col = e < n0 ? e : e - n0;
@@ -874,41 +975,41 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
     }
   }
   __syncthreads();
-  {
-    // row transform of every eliminated column: panel rows B <- B L^-1 and rhs y <- y L^-1 (one row per thread)
-    const int rows_per_col = (h - 6) + 1;
-    const int ncols = C0.ncol + C1.Ke;
-    for (int e = tid; e < ncols * rows_per_col; e += kBandThreads) {
-      const int cc = e / rows_per_col, t = e - cc * rows_per_col;
-      const BandChain& Q = cc < C0.ncol ? C0 : C1;
-      const int c = cc < C0.ncol ? cc : cc - C0.ncol;
-      const int nb = min(h - 6, Q.npc - 6 * (c + 1));
-      const double* L = Q.W + static_cast<size_t>(c) * h6;
-      const double* rd = Q.LI + static_cast<size_t>(c) * 48;
-      if (t < nb) band_transform_row(Q.W + (static_cast<size_t>(c) * h + 6 + t) * 6, L, rd);
-      else if (t == h - 6) band_transform_row(Q.AR + static_cast<size_t>(m) * Q.npc + 6 * c, L, rd);
-    }
-    __syncthreads();
-  }
-  HB_TICKD(7, C0.AR);
-  // separator columns first (chain 0, warp 0), then outwards: chain 0 in warp 0, chain 1 in warp 1
-  if (warp == 0 && C0.ncol > C0.Ke) band_backsub_chain(C0, C0.ncol - 1, C0.Ke, h, m, lane);
+  row_transform(!CL || rank == 0, true);
   __syncthreads();
-  if (pl.Kb) {
+  HB_TICKD(7, C.AR);
+  // separator columns first (chain 0, warp 0), then outwards: chain 0 in warp 0, chain 1 in warp 1 (CL: warp 0 of CTA 1)
+  if (has0 && warp == 0 && C0.ncol > C0.Ke) band_backsub_chain(C0, C0.ncol - 1, C0.Ke, h, m, lane);
+  __syncthreads();
+  if (CL && rank == 0) {   // barrier 3: the corner solution and the separator solution, in CTA 1's XA and X
+    if (pl.Kb) {
+      for (int e = tid; e < m; e += kBandThreads) st_peer(XA + e, 1, XA[e]);
+      for (int v = tid; v < 6 * pl.bs; v += kBandThreads) st_peer(C1.X + C1.npc - 1 - v, 1, C0.X[6 * C0.Ke + v]);
+    }
+    cluster_arrive();
+  }
+  if (!CL && pl.Kb) {
     for (int v = tid; v < 6 * pl.bs; v += kBandThreads) C1.X[C1.npc - 1 - v] = C0.X[6 * C0.Ke + v];
     __syncthreads();
   }
-  if (warp < 2) {
-    const BandChain& Q = warp ? C1 : C0;
+  if (CL ? warp == 0 : warp < 2) {
+    const BandChain& Q = (CL ? rank : warp) ? C1 : C0;
     band_backsub_chain(Q, Q.Ke - 1, 0, h, m, lane);
   }
   __syncthreads();
-  HB_TICKD(6, C0.X);
-  for (int e = tid; e < C0.npc; e += kBandThreads) x_out[e] = C0.X[e];
-  for (int e = tid; e < 6 * C1.Ke; e += kBandThreads) x_out[np - 1 - e] = C1.X[e];
-  for (int e = tid; e < m; e += kBandThreads) x_out[np + e] = XA[e];
+  HB_TICKD(6, C.X);
+  if (has0) {
+    for (int e = tid; e < C0.npc; e += kBandThreads) x_out[e] = C0.X[e];
+    for (int e = tid; e < m; e += kBandThreads) x_out[np + e] = XA[e];
+  }
+  if (has1) for (int e = tid; e < 6 * C1.Ke; e += kBandThreads) x_out[np - 1 - e] = C1.X[e];
   if (dbg && tid == 0) { for (int i = 0; i < 8; ++i) dbg[i] = t_acc[i]; dbg[8 + 6] = t_staged - t_entry; dbg[8 + 7] = t_gathered - t_staged; dbg[8 + 14] = clock64() - t_entry; dbg[8 + 15] = t_g[0] - t_staged; dbg[8 + 22] = t_g[1] - t_g[0]; dbg[8 + 23] = t_g[2] - t_g[1]; dbg[8 + 30] = t_g[3] - t_g[2]; dbg[8 + 31] = t_gathered - t_g[3]; }
-  if (tid == 0) *spd_flag = s_ok;
+  if (tid == 0 && has0) *spd_flag = s_ok;
+  // neither CTA may exit while the other can still read its shared memory (barrier 4)
+  if (CL) {
+    if (rank == 0) cluster_wait();
+    cluster_arrive(); cluster_wait();
+  }
 }
 
 }  // namespace hb

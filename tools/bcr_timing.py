@@ -13,7 +13,7 @@ ctx = runtime.Context(0)
 ctx.load_window(win)
 ctx.iterate(2)
 ctx.synchronize()
-buf = (C.c_longlong * 72)()
+buf = (C.c_longlong * 144)()
 ctx.lib.hb200_debug_band_timing(ctx.h, buf)
 n = buf[0]
 t = [buf[1 + i] for i in range(n)]
