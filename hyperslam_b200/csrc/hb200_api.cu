@@ -193,13 +193,13 @@ struct hb200_ctx {
   DevBuf<int4> v_idx, i_idx;
   std::vector<int4> h_v_idx, h_i_idx;       // bound order
   std::vector<int> v_perm, i_perm;          // bound position -> user index
-  DevBuf<int> seg_off, run_off, lm_off, lm_obs, d_invalid;
+  DevBuf<int> run_off, lm_off, lm_obs, d_invalid;
   // large windows: landmarks ordered by first knot base and cut into groups for schur_group_kernel
   DevBuf<int> lm_order, lm_group_off;
   int n_lm_groups = 0, schur_rt = 0;
   bool schur_groups = false;
-  int nseg = 0, nruns = 0, max_rows = 6;
-  int pix_splits = 1, imu_splits = 1, imu_splits_mma = 1;
+  int nruns = 0, max_rows = 6;
+  int imu_splits = 1, imu_splits_mma = 1;
   int beta = 3, min_beta = 0;   // min_beta: lower bound agreed across ranks (the packed layout must be identical everywhere)
   bool band_solver = true, band_smem = true, force_dense = false;
   DevBuf<double> band_ws;
@@ -316,24 +316,6 @@ int check_launch(hb200_ctx* c, const char* what) {
     if (rc__) return rc__;                         \
   } while (0)
 
-// Launch on the context's stream as a PROGRAMMATIC dependent of the previous kernel in that stream: the grid may become
-// resident while its predecessor still runs and blocks in pdl_wait() until the predecessor has completed (inside stream
-// capture the edge becomes a programmatic graph dependency).  Only for kernels whose sole dependency is that predecessor
-// and that call pdl_wait() first.  OFF by default: at cfg1 the step got slower with the four single-dependency edges
-// of the iteration (knot table -> factors, solve -> back-substitution -> trial factors -> accept) made programmatic;
-// HB200_PDL=1 switches it on.
-template <typename... KArgs, typename... Args>
-cudaError_t launch_dependent(hb200_ctx* c, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, Args&&... args) {
-  static const bool off = !(getenv("HB200_PDL") != nullptr && atoi(getenv("HB200_PDL")) != 0);
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = c->stream;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at; cfg.numAttrs = (off || c->profiling) ? 0 : 1;
-  return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
-}
-
 // Launch configuration of the resident band solver: a grid of one 2-CTA cluster (chain r in CTA r) on the context's
 // stream, the whole workspace in each CTA's shared memory.  at: storage for the cluster-dimension attribute.
 void band_cluster_config(hb200_ctx* c, cudaLaunchConfig_t* cfg, cudaLaunchAttribute* at) {
@@ -346,8 +328,7 @@ void band_cluster_config(hb200_ctx* c, cudaLaunchConfig_t* cfg, cudaLaunchAttrib
 
 cudaStream_t side(hb200_ctx* c) { return c->forked ? c->stream2 : c->stream; }
 int fork_side(hb200_ctx* c) {
-  static const bool no_fork = getenv("HB200_NO_FORK") != nullptr;   // A/B switch for measurements
-  if (c->profiling || c->forked || !c->stream2 || no_fork) return 0;   // the per-launch profile wants a serial timeline
+  if (c->profiling || c->forked || !c->stream2) return 0;   // the per-launch profile wants a serial timeline
   HB_CUDA(cudaEventRecord(c->ev_fork, c->stream));
   HB_CUDA(cudaStreamWaitEvent(c->stream2, c->ev_fork, 0));
   c->forked = true;
@@ -406,7 +387,7 @@ int ensure_system(hb200_ctx* c) {
   c->band_solver = !c->force_dense && ((c->n <= 512) || (12 * (c->beta + 1) <= 6 * c->K));
   c->band_smem = ws <= 220 * 1024;
   c->use_bcr = false;
-  if (c->band_solver && !c->band_smem && 6 * c->beta <= kBcrMaxNb && c->n - 6 * c->K <= 54 && !getenv("HB200_NO_BCR")) {
+  if (c->band_solver && !c->band_smem && 6 * c->beta <= kBcrMaxNb && c->n - 6 * c->K <= 54) {
     // the band does not fit one CTA's shared memory: cyclic reduction over super-blocks of beta control points
     const int m = c->n - 6 * c->K;
     const int nsb = (c->K + c->beta - 1) / c->beta;
@@ -453,20 +434,13 @@ int ensure_system(hb200_ctx* c) {
   }
   HB_CUDA(c->band_ws.ensure(1));
   if (!c->band_solver) { int rc = ensure_dense(c); if (rc) return rc; }
-  if (getenv("HB200_BAND_TIMING")) {
-    HB_CUDA(c->band_dbg.ensure(144));   // 72 per CTA of the cluster kernel
-    long long variant = getenv("HB200_BCR_VARIANT") ? atoll(getenv("HB200_BCR_VARIANT")) : 0;
-    HB_CUDA(cudaMemcpy(c->band_dbg.p + 71, &variant, sizeof(variant), cudaMemcpyHostToDevice));
-  }
-  // parallelism of the J^T J kernels: aim at ~2 CTAs per SM
-  c->pix_splits = std::max(1, std::min((2 * c->num_sms + std::max(c->nseg, 1) - 1) / std::max(c->nseg, 1), std::max(1, c->Nv / (16 * std::max(c->nseg, 1)))));
-  {
-    static const int min_chunk = getenv("HB200_IMU_MIN_CHUNK") ? std::max(1, atoi(getenv("HB200_IMU_MIN_CHUNK"))) : 8;   // factors per CTA at least
-    c->imu_splits = std::max(1, std::min((2 * c->num_sms + std::max(c->nruns, 1) - 1) / std::max(c->nruns, 1), std::max(1, c->Ni / (min_chunk * std::max(c->nruns, 1)))));
-    // tensor-core kernel (large windows): ~6 CTAs per SM, at least two 8-factor chunks per CTA
-    static const int per_sm = getenv("HB200_IMU_CTAS_PER_SM") ? std::max(1, atoi(getenv("HB200_IMU_CTAS_PER_SM"))) : 6;
-    c->imu_splits_mma = std::max(1, std::min((per_sm * c->num_sms + std::max(c->nruns, 1) - 1) / std::max(c->nruns, 1), std::max(1, c->Ni / (16 * std::max(c->nruns, 1)))));
-  }
+  if (getenv("HB200_BAND_TIMING")) HB_CUDA(c->band_dbg.ensure(144));   // 72 per CTA of the cluster kernel
+  // parallelism of the inertial J^T J kernels.  Scalar kernel: ~2 CTAs per SM, at least kImuMinChunk factors per CTA
+  constexpr int kImuMinChunk = 8;
+  c->imu_splits = std::max(1, std::min((2 * c->num_sms + std::max(c->nruns, 1) - 1) / std::max(c->nruns, 1), std::max(1, c->Ni / (kImuMinChunk * std::max(c->nruns, 1)))));
+  // tensor-core kernel (large windows): ~kImuCtasPerSm CTAs per SM, at least two 8-factor chunks per CTA
+  constexpr int kImuCtasPerSm = 6;
+  c->imu_splits_mma = std::max(1, std::min((kImuCtasPerSm * c->num_sms + std::max(c->nruns, 1) - 1) / std::max(c->nruns, 1), std::max(1, c->Ni / (16 * std::max(c->nruns, 1)))));
   return 0;
 }
 
@@ -503,13 +477,8 @@ template <int K, bool J>
 int launch_pixel(hb200_ctx* c, int sel, bool accumulate = false) {
   if (c->Nv == 0) return 0;
   PixelArgs a = pixel_args<J>(c, sel, accumulate);
-  if (J && accumulate) {
-    // optional (HB200_PIX_TILES): a CTA walks several consecutive tiles and flushes its J^T J accumulators once per knot base
-    static const int tiles_env = getenv("HB200_PIX_TILES") ? atoi(getenv("HB200_PIX_TILES")) : 0;
-    a.tiles_per_cta = tiles_env > 0 ? tiles_env : 1;   // one tile per CTA: on the 1 M-factor window fewer, longer CTAs lose more than the saved atomics win
-    const int grid = (c->n_pix_blocks + a.tiles_per_cta - 1) / a.tiles_per_cta;
-    pixel_eval_kernel<K, J, J><<<grid, kEvalThreads, 0, c->stream>>>(a, c->basis);
-  } else pixel_eval_kernel<K, J, false><<<c->n_pix_blocks, kEvalThreads, 0, c->stream>>>(a, c->basis);
+  if (J && accumulate) pixel_eval_kernel<K, J, J><<<c->n_pix_blocks, kEvalThreads, 0, c->stream>>>(a, c->basis);
+  else pixel_eval_kernel<K, J, false><<<c->n_pix_blocks, kEvalThreads, 0, c->stream>>>(a, c->basis);
   HB_LAUNCH(c, "pixel_eval_kernel");
   return 0;
 }
@@ -528,8 +497,8 @@ int launch_factors_merged(hb200_ctx* c, int sel, bool accumulate) {
   const InertialArgs ia = inertial_args<J>(c, sel);
   const int blocks = c->n_pix_blocks + c->n_imu_blocks;
   const size_t smem = J ? inertial_stash_bytes(K) : 0;
-  if (J && accumulate) HB_CUDA(launch_dependent(c, factor_eval_kernel<K, 4, J, J>, dim3(blocks), dim3(kEvalThreads), smem, pa, ia, c->basis, c->bias_basis, c->n_pix_blocks));
-  else HB_CUDA(launch_dependent(c, factor_eval_kernel<K, 4, J, false>, dim3(blocks), dim3(kEvalThreads), smem, pa, ia, c->basis, c->bias_basis, c->n_pix_blocks));
+  if (J && accumulate) factor_eval_kernel<K, 4, J, J><<<blocks, kEvalThreads, smem, c->stream>>>(pa, ia, c->basis, c->bias_basis, c->n_pix_blocks);
+  else factor_eval_kernel<K, 4, J, false><<<blocks, kEvalThreads, smem, c->stream>>>(pa, ia, c->basis, c->bias_basis, c->n_pix_blocks);
   HB_LAUNCH(c, "factor_eval_kernel");
   return 0;
 }
@@ -564,8 +533,7 @@ int enqueue_evaluate(hb200_ctx* c, bool want_J, int sel, bool accumulate = false
   const bool J_any = want_J || accumulate;
   // Small windows are latency-bound: one launch for both factor families.  Large windows are throughput-bound: the
   // merged kernel would run the pixel CTAs at the inertial body's 255 registers, so the families stay separate.
-  static const bool no_merge = getenv("HB200_NO_MERGE") != nullptr;   // profiling aid: one kernel per factor family
-  if (c->Nv && c->Ni && !no_merge && c->n_pix_blocks + c->n_imu_blocks <= 4 * c->num_sms) {   // (also while profiling: same kernels as the graph)
+  if (c->Nv && c->Ni && c->n_pix_blocks + c->n_imu_blocks <= 4 * c->num_sms) {   // (also while profiling: same kernels as the graph)
     // visual and inertial factors side by side in one launch; pose factors (if any) on the side stream
     if (c->Nm && (rc = fork_side(c))) return rc;
     if (c->k == 4) rc = J_any ? launch_factors_merged<4, true>(c, sel, accumulate) : launch_factors_merged<4, false>(c, sel, false);
@@ -591,30 +559,17 @@ int enqueue_evaluate(hb200_ctx* c, bool want_J, int sel, bool accumulate = false
   return rc;
 }
 
-int enqueue_clear_system(hb200_ctx* c) {
-  HB_CUDA(cudaMemsetAsync(c->assembly(), 0, static_cast<size_t>(c->lay.total) * sizeof(double), c->stream));
-  prof_mark(c, "memset(system)");
-  return 0;
-}
-
-// J^T J of the inertial / manifold factors and the cost sum on the side stream, the landmark Schur complement on
-// the main stream: both accumulate into S with atomics (commutative), diag(J^T J) is kept apart from S, so nothing
-// orders them.  after_eval_on_main: the factor Jacobians were produced by a launch on the MAIN stream (merged
-// factor kernel), so the side stream is forked here rather than before the evaluation.
-int enqueue_build(hb200_ctx* c, bool pixel_fused = false) {
-  if (!pixel_fused) { int rc0 = enqueue_clear_system(c); if (rc0) return rc0; }
-  if (c->Nv && !pixel_fused) {
-    if (c->k == 4) pixel_hessian_kernel<4><<<c->nseg * c->pix_splits, kHessThreads, 0, c->stream>>>(c->seg_off.p, c->v_r.p, c->v_Jp.p, c->v_w.p, c->assembly(), c->lay, c->pix_splits);
-    else pixel_hessian_kernel<6><<<c->nseg * c->pix_splits, kHessThreads, 0, c->stream>>>(c->seg_off.p, c->v_r.p, c->v_Jp.p, c->v_w.p, c->assembly(), c->lay, c->pix_splits);
-    HB_LAUNCH(c, "pixel_hessian_kernel");
-  }
+// The rest of the normal equations, after the factor kernels have cleared the packed system and accumulated the pixel
+// J^T J into it: J^T J of the inertial / manifold factors and the cost sum on the side stream, the landmark Schur
+// complement on the main stream.  Both accumulate into S with atomics (commutative), diag(J^T J) is kept apart from S,
+// so nothing orders them.  The side stream is forked here, not before the evaluation, when the factor Jacobians were
+// produced on the MAIN stream (merged factor kernel).
+int enqueue_build(hb200_ctx* c) {
   { const int rf = fork_side(c); if (rf) return rf; }   // (no-op when already forked or while profiling)
   if (c->Ni) {
     // large windows (>= 16 384 inertial factors): the augmented product on the FP64 tensor cores, ~6 CTAs per SM of 8-factor
-    // chunks; small windows: the scalar block-by-block kernel on short runs (cfg1, ~9 factors per CTA), which is faster
-    // there.  HB200_IMU_HESS=0 / 1 forces the scalar / tensor-core kernel (A/B switch)
-    static const int hess_env = getenv("HB200_IMU_HESS") != nullptr ? atoi(getenv("HB200_IMU_HESS")) : -1;
-    const bool scalar_hess = hess_env >= 0 ? hess_env == 0 : c->Ni < 16384;
+    // chunks; small windows: the scalar block-by-block kernel on short runs (cfg1, ~9 factors per CTA), which is faster there
+    const bool scalar_hess = c->Ni < 16384;
     // (order 6 keeps 12-factor chunks at ~2 CTAs per SM, which beat 8-factor chunks at ~6 CTAs per SM on the order-6 window)
     const int splits = (scalar_hess || c->k != 4) ? c->imu_splits : c->imu_splits_mma;
     const int grid = c->nruns * splits;
@@ -626,10 +581,9 @@ int enqueue_build(hb200_ctx* c, bool pixel_fused = false) {
         inertial_hessian_kernel<6, 4><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->i_idx.p, c->i_r.p, c->i_Jp.p, c->i_wg.p, c->i_wa.p,
                                                                           c->i_Jg.p, c->imu_scale, c->assembly(), c->lay, c->o_bg(), c->o_ba(), c->o_g(), c->imu_splits);
     } else {
-      static const bool small_chunks = !(getenv("HB200_IMU_CH") != nullptr && atoi(getenv("HB200_IMU_CH")) != 8);   // 8-factor chunks (HB200_IMU_CH=16: 16 / 12)
 #define HB_IMU_MMA(KK, CHH) inertial_hessian_mma_kernel<KK, 4, CHH><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->i_idx.p, c->i_r.p, c->i_Jp.p, c->i_wg.p, c->i_wa.p, \
                                                     c->i_Jg.p, c->imu_scale, c->assembly(), c->lay, c->o_bg(), c->o_ba(), c->o_g(), splits)
-      if (c->k == 4) { if (small_chunks) HB_IMU_MMA(4, 8); else HB_IMU_MMA(4, 16); }
+      if (c->k == 4) HB_IMU_MMA(4, 8);
       else HB_IMU_MMA(6, 12);
 #undef HB_IMU_MMA
     }
@@ -703,7 +657,7 @@ int enqueue_solve(hb200_ctx* c, bool fuse_retract = false, bool* fused = nullptr
       band_cluster_config(c, &cfg, at);
       HB_CUDA(cudaLaunchKernelEx(&cfg, band_solve_kernel<true>, static_cast<const double*>(c->sys.p), c->lay, c->band_ws.p, c->dp.p, c->spd.p, c->band_dbg.p, st, fx, Dout, 0));
     } else band_solve_kernel<false><<<1, kBandThreads, c->band_chunk_smem, c->stream>>>(c->sys.p, c->lay, c->band_ws.p, c->dp.p, c->spd.p, c->band_dbg.p, st, fx, Dout, c->band_chunk_cols);
-    HB_LAUNCH(c, "band_solve_kernel");
+    HB_LAUNCH(c, c->band_smem ? "band_solve_kernel" : "band_solve_kernel<false>");   // (the chunked path gets its own profile label)
   } else {
     { const int rd = enqueue_densify(c); if (rd) return rd; }
     int n = c->n;
@@ -728,11 +682,11 @@ int enqueue_solve(hb200_ctx* c, bool fuse_retract = false, bool* fused = nullptr
         if (fused) *fused = true;
       }
       if (c->k == 4)
-        HB_CUDA(launch_dependent(c, lm_backsub_kernel<4>, dim3(c->n_lm_blocks + extra), dim3(kLmWarps * 32), 0, c->L, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p,
-                                 c->Vinv.p, c->gl.p, c->Dl.p, c->dp.p, c->dl.p, c->lm_part.p, c->lms[0].p, c->lms[1].p, c->n_lm_blocks, ra));
+        lm_backsub_kernel<4><<<c->n_lm_blocks + extra, kLmWarps * 32, 0, c->stream>>>(c->L, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p,
+                                                                                 c->Vinv.p, c->gl.p, c->Dl.p, c->dp.p, c->dl.p, c->lm_part.p, c->lms[0].p, c->lms[1].p, c->n_lm_blocks, ra);
       else
-        HB_CUDA(launch_dependent(c, lm_backsub_kernel<6>, dim3(c->n_lm_blocks + extra), dim3(kLmWarps * 32), 0, c->L, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p,
-                                 c->Vinv.p, c->gl.p, c->Dl.p, c->dp.p, c->dl.p, c->lm_part.p, c->lms[0].p, c->lms[1].p, c->n_lm_blocks, ra));
+        lm_backsub_kernel<6><<<c->n_lm_blocks + extra, kLmWarps * 32, 0, c->stream>>>(c->L, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p,
+                                                                                 c->Vinv.p, c->gl.p, c->Dl.p, c->dp.p, c->dl.p, c->lm_part.p, c->lms[0].p, c->lms[1].p, c->n_lm_blocks, ra);
       HB_LAUNCH(c, "lm_backsub_kernel");
     } else {
       HB_CUDA(cudaMemsetAsync(c->dl.p, 0, 3 * static_cast<size_t>(c->L) * sizeof(double), c->stream));
@@ -788,8 +742,8 @@ int enqueue_accept(hb200_ctx* c) {
   const bool mailbox = c->nccl && c->peers_open;
   MailboxArgs mb{};
   mb.nranks = mailbox ? c->nranks : 1; mb.rank = c->rank; mb.peers = c->d_peers.p; mb.local = c->mbox.p; mb.seq = c->mbox_seq.p;
-  HB_CUDA(launch_dependent(c, accept_kernel, dim3(1), dim3(kAcceptThreads), 0, c->sys.p, c->lay, c->scal.p, c->dp.p, c->D.p, c->fixed.p, c->st.p, c->spd.p, c->records.p, c->max_records,
-                           (!c->multi() || mailbox) ? 1 : 0, sa, fuse_commit ? 1 : 0, a, mb, term_args(c)));
+  accept_kernel<<<1, kAcceptThreads, 0, c->stream>>>(c->sys.p, c->lay, c->scal.p, c->dp.p, c->D.p, c->fixed.p, c->st.p, c->spd.p, c->records.p, c->max_records,
+                                                    (!c->multi() || mailbox) ? 1 : 0, sa, fuse_commit ? 1 : 0, a, mb, term_args(c));
   HB_LAUNCH(c, "accept_kernel");
   if (!fuse_commit) {
     const int blocks = static_cast<int>(std::min<size_t>((mx + 255) / 256, static_cast<size_t>(c->num_sms) * 4));
@@ -847,12 +801,9 @@ int enqueue_reduce_scalars(hb200_ctx* c) {
 // One LM iteration enqueued on the stream (graph-capturable unless the callback hook is in use).
 int enqueue_iteration(hb200_ctx* c) {
   int rc = 0;
-  // pixel J^T J: fused into the factor kernel (small windows: one launch less on the latency chain) or a separate
-  // segment-wise pass over the Jacobians (large windows); HB200_FUSE=0/1 overrides the choice
-  static const int fuse_env = getenv("HB200_FUSE") ? atoi(getenv("HB200_FUSE")) : -1;
-  const bool fuse = fuse_env >= 0 ? fuse_env != 0 : true;
-  if ((rc = enqueue_evaluate(c, true, 0, fuse, /*keep_fork=*/true, /*clear_system=*/fuse))) return rc;
-  if ((rc = enqueue_build(c, fuse))) return rc;
+  // the factor kernels clear the packed system and accumulate the pixel J^T J into it (enqueue_build does the rest)
+  if ((rc = enqueue_evaluate(c, true, 0, /*accumulate=*/true, /*keep_fork=*/true, /*clear_system=*/true))) return rc;
+  if ((rc = enqueue_build(c))) return rc;
   if ((rc = enqueue_reduce_system(c))) return rc;
   bool retracted = false;
   if ((rc = enqueue_solve(c, /*fuse_retract=*/true, &retracted))) return rc;
@@ -982,7 +933,7 @@ void hb200_destroy(hb200_ctx* c) {
   c->cams.release(); c->imu.release(); c->cam_tab.release(); c->imu_tab.release(); c->fixed.release();
   c->v_stamp.release(); c->v_pixel.release(); c->i_stamp.release(); c->i_meas.release(); c->v_cam.release(); c->v_lm.release(); c->v_idx.release(); c->i_idx.release();
   c->v_z.release(); c->v_w.release(); c->m_stamp.release(); c->m_meas.release(); c->sensors.release(); c->m_sensor.release(); c->m_idx.release(); c->m_r.release(); c->m_Jp.release();
-  c->seg_off.release(); c->run_off.release(); c->lm_off.release(); c->lm_obs.release(); c->d_invalid.release(); c->lm_order.release(); c->lm_group_off.release();
+  c->run_off.release(); c->lm_off.release(); c->lm_obs.release(); c->d_invalid.release(); c->lm_order.release(); c->lm_group_off.release();
   c->v_r.release(); c->v_Jp.release(); c->v_Jl.release(); c->i_r.release(); c->i_Jp.release(); c->i_wg.release(); c->i_wa.release(); c->i_Jg.release();
   c->sys.release(); c->D.release(); c->Lw.release(); c->Ldiag.release(); c->dp.release(); c->dl.release(); c->Vinv.release(); c->gl.release(); c->Dl.release();
   c->band_ws.release(); c->band_dbg.release(); c->bcr_ws.release(); c->bcr_bar.release(); c->lm_part.release(); c->scal.release(); c->spd.release(); c->st.release(); c->records.release();
@@ -1256,20 +1207,19 @@ int sync_host_mirrors(hb200_ctx* c) {
   return 0;
 }
 
-// Incidence lists of the device-resident factor lists (landmark CSR, inertial runs, segment offsets, longest
-// track) by counting + scan kernels, then everything hb200_bind derives from them.  One small read-back.
+// Incidence lists of the device-resident factor lists (landmark CSR, inertial runs, longest track) by counting + scan
+// kernels, then everything hb200_bind derives from them.  One small read-back.
 int rebuild_incidence_device(hb200_ctx* c) {
-  const int Nv = c->Nv, Ni = c->Ni, L = c->L, K = c->K;
-  c->nseg = K - c->k + 1;
+  const int Nv = c->Nv, Ni = c->Ni, L = c->L;
   HB_CUDA(c->w_scal.ensure(8));
   HB_CUDA(cudaMemsetAsync(c->w_scal.p, 0, 8 * sizeof(int), c->stream));
   HB_CUDA(c->lm_off.ensure(static_cast<size_t>(L) + 2)); HB_CUDA(c->lm_obs.ensure(std::max(Nv, 1)));
-  HB_CUDA(c->seg_off.ensure(static_cast<size_t>(c->nseg) + 2)); HB_CUDA(c->run_off.ensure(static_cast<size_t>(Ni) + 2));
-  HB_CUDA(c->w_cnt.ensure(static_cast<size_t>(std::max(std::max(L, c->nseg), 1)) + 1));
+  HB_CUDA(c->run_off.ensure(static_cast<size_t>(Ni) + 2));
+  HB_CUDA(c->w_cnt.ensure(static_cast<size_t>(std::max(L, 1)) + 1));
   HB_CUDA(c->w_keep.ensure(std::max(std::max(Nv, Ni), 1))); HB_CUDA(c->w_pos.ensure(std::max(std::max(Nv, Ni), 1)));
   // landmark CSR
   HB_CUDA(cudaMemsetAsync(c->w_cnt.p, 0, sizeof(int) * (static_cast<size_t>(L) + 1), c->stream));
-  if (Nv) { count_kernel<<<(Nv + 255) / 256, 256, 0, c->stream>>>(Nv, c->v_idx.p, 1, c->w_cnt.p); HB_LAUNCH(c, "count_kernel"); }
+  if (Nv) { count_kernel<<<(Nv + 255) / 256, 256, 0, c->stream>>>(Nv, c->v_idx.p, c->w_cnt.p); HB_LAUNCH(c, "count_kernel"); }
   scan_kernel<<<1, 1024, 0, c->stream>>>(c->w_cnt.p, L + 1, c->lm_off.p, c->w_scal.p + 0);
   HB_LAUNCH(c, "scan_kernel");
   HB_CUDA(cudaMemsetAsync(c->w_cnt.p, 0, sizeof(int) * (static_cast<size_t>(L) + 1), c->stream));
@@ -1279,11 +1229,6 @@ int rebuild_incidence_device(hb200_ctx* c) {
     csr_sort_kernel<<<(L + 127) / 128, 128, 0, c->stream>>>(L, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->k, c->w_scal.p + 1);
     HB_LAUNCH(c, "csr_sort_kernel");
   }
-  // segment offsets of the visual list
-  HB_CUDA(cudaMemsetAsync(c->w_cnt.p, 0, sizeof(int) * (static_cast<size_t>(c->nseg) + 1), c->stream));
-  if (Nv) { count_kernel<<<(Nv + 255) / 256, 256, 0, c->stream>>>(Nv, c->v_idx.p, 0, c->w_cnt.p); HB_LAUNCH(c, "count_kernel"); }
-  scan_kernel<<<1, 1024, 0, c->stream>>>(c->w_cnt.p, c->nseg + 1, c->seg_off.p, c->w_scal.p + 2);
-  HB_LAUNCH(c, "scan_kernel");
   // inertial runs
   if (Ni) {
     run_flag_kernel<<<(Ni + 255) / 256, 256, 0, c->stream>>>(Ni, c->i_idx.p, c->w_keep.p);
@@ -1412,11 +1357,7 @@ int hb200_bind(hb200_ctx* c, int* num_invalid) {
     }
     HB_CUDA(cudaStreamSynchronize(c->stream));
   }
-  // segment offsets (pixel), runs (inertial), landmark incidence (CSR)
-  c->nseg = c->K - c->k + 1;
-  std::vector<int> seg(c->nseg + 1, 0);
-  for (int p = 0; p < Nv; ++p) seg[c->h_v_idx[p].x + 1] += 1;
-  for (int s = 0; s < c->nseg; ++s) seg[s + 1] += seg[s];
+  // runs (inertial), landmark incidence (CSR)
   std::vector<int> runs;
   for (int p = 0; p < Ni; ++p) {
     const int4& a = c->h_i_idx[p];
@@ -1435,18 +1376,17 @@ int hb200_bind(hb200_ctx* c, int* num_invalid) {
   for (int l = 0; l < c->L; ++l)
     if (off[l + 1] > off[l]) c->max_rows = std::max(c->max_rows, 6 * (c->h_v_idx[obs[off[l + 1] - 1]].x + c->k - c->h_v_idx[obs[off[l]]].x));
   if (2 * 3 * static_cast<size_t>(c->max_rows) * sizeof(double) > 200 * 1024) return fail(-6, "landmark track spans %d control-point dofs; exceeds the Schur kernel's shared-memory tile", c->max_rows);
-  HB_CUDA(c->seg_off.ensure(seg.size())); HB_CUDA(c->run_off.ensure(runs.size())); HB_CUDA(c->lm_off.ensure(off.size())); HB_CUDA(c->lm_obs.ensure(obs.size()));
-  HB_CUDA(cudaMemcpyAsync(c->seg_off.p, seg.data(), sizeof(int) * seg.size(), cudaMemcpyHostToDevice, c->stream));
+  HB_CUDA(c->run_off.ensure(runs.size())); HB_CUDA(c->lm_off.ensure(off.size())); HB_CUDA(c->lm_obs.ensure(obs.size()));
   HB_CUDA(cudaMemcpyAsync(c->run_off.p, runs.data(), sizeof(int) * runs.size(), cudaMemcpyHostToDevice, c->stream));
   HB_CUDA(cudaMemcpyAsync(c->lm_off.p, off.data(), sizeof(int) * off.size(), cudaMemcpyHostToDevice, c->stream));
   HB_CUDA(cudaMemcpyAsync(c->lm_obs.p, obs.data(), sizeof(int) * obs.size(), cudaMemcpyHostToDevice, c->stream));
   {
     // landmark groups for the large-window Schur kernel: observed landmarks ordered by their first knot base, cut so that
     // a group has at most kSchurGroup members and its control-point rows fit one window of RT rows
-    static const int min_lm = getenv("HB200_SCHUR_GROUP_MIN") ? atoi(getenv("HB200_SCHUR_GROUP_MIN")) : 8192;
+    constexpr int kSchurGroupMin = 8192;   // landmarks from which schur_group_kernel replaces schur_kernel
     c->schur_groups = false;
     c->schur_rt = ((c->max_rows + 12 + 7) / 8) * 8;
-    if (c->L >= min_lm && Nv) {
+    if (c->L >= kSchurGroupMin && Nv) {
       std::vector<int> order;
       order.reserve(c->L);
       for (int l = 0; l < c->L; ++l) if (off[l + 1] > off[l]) order.push_back(l);
@@ -1785,6 +1725,9 @@ int hb200_build_system(hb200_ctx* c) {
   if (rc) return rc;
   if (!c->evaluated_J) return fail(-2, "call hb200_evaluate(HB200_EVAL_JACOBIANS) first");
   HB_CUDA(cudaSetDevice(c->device));
+  // assembled as enqueue_iteration does: the Jacobian sweep at the current state runs again with the pixel J^T J
+  // accumulated by the factor kernels (it rewrites the same residuals and Jacobians), then the rest of the system
+  if ((rc = enqueue_evaluate(c, true, 0, /*accumulate=*/true, /*keep_fork=*/true, /*clear_system=*/true))) return rc;
   if ((rc = enqueue_build(c))) return rc;
   if ((rc = enqueue_reduce_system(c))) return rc;
   c->system_built = true;
@@ -2282,12 +2225,6 @@ int hb200_append_knots(hb200_ctx* c, int count) {
   for (int i = 0; i < count; ++i) { c->h_knot_stamp.push_back(tail[8 * i + 7]); c->h_knot_const.push_back(0); }
   c->K = K + count;
   if ((rc = update_fixed(c))) return rc;
-  c->nseg = c->K - c->k + 1;
-  HB_CUDA(c->seg_off.grow(static_cast<size_t>(c->nseg) + 2, static_cast<size_t>(c->nseg - count) + 1, c->stream));
-  {   // the new segments hold no visual factor yet: their offsets equal the list length
-    std::vector<int> fill(count, c->Nv);
-    HB_CUDA(cudaMemcpyAsync(c->seg_off.p + (c->nseg - count) + 1, fill.data(), sizeof(int) * count, cudaMemcpyHostToDevice, c->stream));
-  }
   if ((rc = ensure_system(c))) return rc;
   HB_CUDA(cudaStreamSynchronize(c->stream));
   c->invalidate(); c->have_snapshot = false;

@@ -351,7 +351,6 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
                                                                   const SolverState* __restrict__ st, const unsigned char* __restrict__ fixed,
                                                                   double* __restrict__ Dout, int chunk_cols) {
   extern __shared__ double s_band[];
-  pdl_launch_dependents();   // the back-substitution grid behind the solve may become resident (it waits for this grid's completion)
   const long long t_entry = clock64();
   // SMEM: the workspace is resident in shared memory and the kernel runs as a 2-CTA cluster, chain r in CTA r, each
   // chain on its own SM (its own shared-memory crossbar and four schedulers).  Both CTAs lay out the whole workspace

@@ -185,7 +185,7 @@ __device__ __noinline__ void bcr_forward_warp(const double* L, int ldl, int n, c
 // on the FP64 tensor cores (mma.sync m8n8k4 -> DMMA.8x8x4): one 8 x 8 output tile per warp pass, contraction over
 // the n rows in steps of 4.  Deliberately a small out-of-line loop: this code runs once per node, and one-shot
 // code is bound by instruction fetch, not issue (tools/microbench).
-__device__ __noinline__ void bcr_gram(const double* Y, int ldy, int n, int nc, double* G, int variant = 0) {
+__device__ __noinline__ void bcr_gram(const double* Y, int ldy, int n, int nc, double* G) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, lr = lane >> 2, lk = lane & 3;
   const int T = (nc + 7) / 8, ntiles = T * (T + 1) / 2;
   for (int tile = warp; tile < ntiles; tile += kBcrThreads / 32) {
@@ -197,7 +197,6 @@ __device__ __noinline__ void bcr_gram(const double* Y, int ldy, int n, int nc, d
     double c0 = 0.0, c1 = 0.0;
     const double* pa = Y + lk * ldy + (va ? ca : 0);
     const double* pb = Y + lk * ldy + (vb ? cb : 0);
-    if (variant != 2)
     for (int k0 = 0; k0 < n; k0 += 16) {   // four k-steps per round: eight loads in flight, then the dependent DMMA chain
       double av[4], bv[4];
 #pragma unroll
@@ -211,7 +210,7 @@ __device__ __noinline__ void bcr_gram(const double* Y, int ldy, int n, int nc, d
         asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};" : "+d"(c0), "+d"(c1) : "d"(av[u]), "d"(bv[u]));
     }
     const int row = 8 * ti + lr, col = 8 * tj + 2 * lk;
-    if (row < nc && variant != 1) {
+    if (row < nc) {
       if (col <= row) G[row * nc + col] = c0;
       if (col + 1 <= row) G[row * nc + col + 1] = c1;
     }
@@ -340,7 +339,7 @@ __global__ void __launch_bounds__(kBcrThreads) bcr_solve_kernel(const double* __
       }
       for (int u = tid; u < nb; u += kBcrThreads) N[pl.oy + u] = sR[u * ldr + 2 * nb + m];
       if (lv == 0) stamp();
-      bcr_gram(sR, ldr, nb, ncols, N + pl.oG, dbg ? static_cast<int>(dbg[71]) : 0);
+      bcr_gram(sR, ldr, nb, ncols, N + pl.oG);
       if (lv == 0) stamp();
       __syncthreads();
       if (lv == 0) stamp();

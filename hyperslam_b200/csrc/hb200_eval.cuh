@@ -143,7 +143,6 @@ HB_DI void knot_table_row(const double* q, const double* p, double stamp, const 
 // clear / nclear: optional buffer zeroed by the same launch (the packed reduced system at the start of an
 // iteration -- saves the separate memset node).
 __global__ void prep_kernel(int K, const double* __restrict__ knots, double* __restrict__ tab, double* __restrict__ clear, size_t nclear) {
-  pdl_launch_dependents();   // the factor kernel behind it may become resident now (it waits for this grid's completion)
   const size_t gid = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
   for (size_t e = gid; e < nclear; e += static_cast<size_t>(gridDim.x) * blockDim.x) clear[e] = 0.0;
   const int j = static_cast<int>(gid);
@@ -397,8 +396,7 @@ struct PixelArgs {
   int K_knots;
   double* sys;            // packed band-only reduced system (SysLayout) to accumulate J^T J / J^T r into, or null
   SysLayout lay;
-  int tiles_per_cta;      // consecutive 64-factor tiles one CTA of pixel_eval_kernel walks (large windows: its J^T J accumulators
-                          // stay in registers across tiles of the same knot base, one flush per base instead of one per tile)
+  int tiles_per_cta;      // 64-factor tiles per CTA of the order-6 fused pass: always 1, read at run time (pixel_eval_body)
 };
 
 // J^T J / J^T r of up to 32 consecutive pixel factors [f0, f0 + cnt) of this CTA, accumulated into the
@@ -553,7 +551,10 @@ HB_DI void pixel_eval_body(const PixelArgs& a, const Basis& B, int bid0) {
   __shared__ double s_J[FUSE ? 128 * PixelHessAcc<K>::LD : 1];
   __shared__ double s_r[FUSE ? 128 : 1];
   __shared__ int s_b[FUSE ? 66 : 1];
-  const int T = (FUSE && a.tiles_per_cta > 1) ? a.tiles_per_cta : 1;
+  // One 64-factor tile per CTA.  The order-6 fused pass keeps the tile count a run-time value (the host passes 1): with
+  // the loop compiled away it is allocated 224 instead of 254 registers and measured 5 % slower on cfg2 (DESIGN.md §5).
+  // Order 4 compiles the loop away, which removes spills there.
+  const int T = (K == 6 && FUSE && a.tiles_per_cta > 1) ? a.tiles_per_cta : 1;
   PixelHessAcc<K> acc;
   if (FUSE) pixel_hess_reset<K>(acc, -1);
   for (int tt = 0; tt < T; ++tt) {
@@ -982,8 +983,6 @@ __global__ void __launch_bounds__(kEvalThreads) inertial_eval_kernel(InertialArg
 // side they cost the longer of the two.
 template <int K, int KB, bool WANT_J, bool FUSE>
 __global__ void __launch_bounds__(kEvalThreads) factor_eval_kernel(PixelArgs pa, InertialArgs ia, Basis B, Basis BB, int n_pix_blocks) {
-  pdl_launch_dependents();
-  pdl_wait();   // (launched as a programmatic dependent of the knot-table / retraction kernel on the iteration path)
   if (static_cast<int>(blockIdx.x) < n_pix_blocks) pixel_eval_body<K, WANT_J, FUSE>(pa, B, blockIdx.x);
   else inertial_eval_body<K, KB, WANT_J>(ia, B, BB, blockIdx.x - n_pix_blocks);
 }

@@ -15,70 +15,8 @@ namespace cg = cooperative_groups;
 
 // The packed reduced system is band-only: see SysLayout / sys_index (hb200_types.cuh).
 
-// ---------------------------------------------------------------------------------------------
-// J^T J / J^T r of the pixel factors, one CTA per spline segment (factors are sorted by knot base
-// index, so a segment's factors are contiguous and share the same 6K x 6K block of H).
-// ---------------------------------------------------------------------------------------------
+// The pixel factors' J^T J / J^T r is accumulated by the factor kernel itself (cta_pixel_hessian, hb200_eval.cuh).
 constexpr int kHessThreads = 128;
-
-template <int K>
-__global__ void __launch_bounds__(kHessThreads) pixel_hessian_kernel(const int* __restrict__ seg_off, const double* __restrict__ r,
-                                                                     const double* __restrict__ Jp, const double* __restrict__ wv, double* sys, SysLayout lay, int splits) {
-  constexpr int NB = 6 * K;
-  constexpr int CH = 16;
-  constexpr int EPT = (NB * NB + kHessThreads - 1) / kHessThreads;
-  __shared__ double sJ[CH][2][NB];
-  __shared__ double sr[CH][2];
-  const int seg = blockIdx.x / splits, part = blockIdx.x - seg * splits;
-  const int slo = seg_off[seg], shi = seg_off[seg + 1];
-  const int len = (shi - slo + splits - 1) / splits;
-  const int lo = slo + part * len, hi = min(shi, lo + len);
-  if (lo >= hi) return;
-  double acc[EPT], gacc = 0.0;
-#pragma unroll
-  for (int e = 0; e < EPT; ++e) acc[e] = 0.0;
-  for (int f0 = lo; f0 < hi; f0 += CH) {
-    const int cnt = min(CH, hi - f0);
-    __syncthreads();
-    for (int e = threadIdx.x; e < cnt * 2 * NB; e += kHessThreads) {
-      const int ff = e / (2 * NB), rem = e - ff * 2 * NB;
-      const int f = f0 + ff;
-      const double r0 = r[2 * f], r1 = r[2 * f + 1];
-      const double sw = sqrt(wv[f]);
-      sJ[ff][rem / NB][rem % NB] = sw * Jp[static_cast<size_t>(f) * 2 * NB + rem];
-      if (rem < 2) sr[ff][rem] = sw * (rem == 0 ? r0 : r1);
-    }
-    __syncthreads();
-#pragma unroll
-    for (int e = 0; e < EPT; ++e) {
-      const int id = threadIdx.x + e * kHessThreads;
-      if (id < NB * NB) {
-        const int a = id / NB, b = id - a * NB;
-        if (b <= a) {   // lower triangle only: the solvers read S[row >= col]
-          double s = 0;
-          for (int ff = 0; ff < cnt; ++ff) s += sJ[ff][0][a] * sJ[ff][0][b] + sJ[ff][1][a] * sJ[ff][1][b];
-          acc[e] += s;
-        }
-      }
-    }
-    if (threadIdx.x < NB) {
-      double s = 0;
-      for (int ff = 0; ff < cnt; ++ff) s += sJ[ff][0][threadIdx.x] * sr[ff][0] + sJ[ff][1][threadIdx.x] * sr[ff][1];
-      gacc += s;
-    }
-  }
-  const int c0 = 6 * seg;  // segment index == knot base index
-#pragma unroll
-  for (int e = 0; e < EPT; ++e) {
-    const int id = threadIdx.x + e * kHessThreads;
-    if (id < NB * NB) {
-      const int a = id / NB, b = id - a * NB;
-      if (b <= a) atomicAdd(&sys[sys_index(lay, c0 + a, c0 + b)], acc[e]);
-      if (b == a) atomicAdd(&sys[lay.oD + c0 + a], acc[e]);
-    }
-  }
-  if (threadIdx.x < NB) atomicAdd(&sys[lay.og + c0 + threadIdx.x], gacc);
-}
 
 // Inertial factors: one CTA per (run of identical (pose base, gyro-bias base, accel-bias base), split).
 // The factor Jacobian is structured -- pose block 6 x 6K dense, bias blocks wg[m] I3 (gyro rows) /
@@ -1056,8 +994,6 @@ __global__ void __launch_bounds__(kLmWarps * 32) lm_backsub_kernel(int L, const 
                                                                   double* __restrict__ dl, double* __restrict__ part /*[n_lm_blocks][5]*/,
                                                                   const double* __restrict__ lms, double* __restrict__ lms_t,
                                                                   int n_lm_blocks, RetractArgs ra) {
-  pdl_launch_dependents();
-  pdl_wait();   // (programmatic dependent of the solver kernel on the iteration path: resident early, starts when the solve is complete)
   // blocks past the landmark range retract the knots / biases / gravity in the same launch (they only need dp)
   if (static_cast<int>(blockIdx.x) >= n_lm_blocks) { retract_body(ra, (blockIdx.x - n_lm_blocks) * blockDim.x + threadIdx.x); return; }
   constexpr int NB = 6 * K;
@@ -1303,7 +1239,6 @@ __global__ void __launch_bounds__(kAcceptThreads) accept_kernel(const double* __
   __shared__ double s[NV][kAcceptThreads / 32];
   __shared__ int s_done;
   const int wl = threadIdx.x & 31, ww = threadIdx.x >> 5;
-  pdl_wait();   // (programmatic dependent of the trial-cost factor kernel)
   if (st->terminated) {   // the solve has ended: later iterations of the same call leave everything alone
     if (threadIdx.x == 0 && mb.nranks > 1 && fuse_scalars) *mb.seq += 1;   // (the peers skip their exchange too: keep the counters aligned)
     return;

@@ -56,12 +56,6 @@ __host__ __device__ inline long long sys_index(const SysLayout& L, int row, int 
   return L.oC + static_cast<long long>(row - L.np) * L.m + (col - L.np);
 }
 
-// Programmatic dependent launch (sm_90+): a kernel launched with the programmatic-serialization attribute may become
-// resident while its predecessor still runs; pdl_wait() returns once the predecessor grid has completed and its writes
-// are visible (a no-op for a normal launch), pdl_launch_dependents() lets the dependent's launch start early.
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-
 struct SolverState {  // lives on the device; updated by accept_kernel
   double radius;
   double decrease_factor;

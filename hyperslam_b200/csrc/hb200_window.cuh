@@ -130,9 +130,10 @@ __global__ void append_knots_kernel(int K, int count, double* __restrict__ knots
 }
 
 // ---- incidence lists -------------------------------------------------------------------------------------------
-__global__ void count_kernel(int n, const int4* __restrict__ idx, int which /*0: base (x), 1: landmark (y)*/, int* __restrict__ cnt) {
+// observations per landmark (y)
+__global__ void count_kernel(int n, const int4* __restrict__ idx, int* __restrict__ cnt) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
-  if (f < n) atomicAdd(&cnt[which ? idx[f].y : idx[f].x], 1);
+  if (f < n) atomicAdd(&cnt[idx[f].y], 1);
 }
 // fill the landmark CSR; within a landmark the observations must come in bound order (ascending factor index): the
 // factor list is sorted by base, so a landmark's first / last observation give its control-point span

@@ -3,8 +3,8 @@
   cfg3  4-camera rig, 500 knots, 500 k pixel factors       (n = 3 026)
   cfg4  1 M factors (833 k pixel + 167 k IMU), 500 knots    (n = 3 026)
 Every factor's index map, residual and Jacobian, the full reduced system, the LM step and three LM iterations
-are compared with the CPU oracle on the same seeded window -- the chunked (out-of-shared-memory) band solver is the
-default path at these sizes; cfg2 is repeated with the dense cooperative Cholesky.
+are compared with the CPU oracle on the same seeded window -- block cyclic reduction across CTAs (bcr_solve_kernel)
+is the band solver at these sizes; cfg2 is repeated with the dense cooperative Cholesky.
 """
 import numpy as np
 import pytest

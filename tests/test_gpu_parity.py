@@ -380,13 +380,21 @@ def test_bearing_and_manifold_factor_evaluate_ceres_shape(built):
     ctx.close()
 
 
-@pytest.mark.parametrize("order,knots", [(4, 140), (6, 96), (4, 64)])
-def test_long_windows_band_solver_out_of_shared_memory(built, order, knots):
-    """Windows whose band + arrow workspace exceeds shared memory: the two-sided factorisation then runs chunk
-    by chunk on shared-memory views of a global workspace.  Compared with the dense cooperative Cholesky on
-    the same system and with the oracle's step; also through full LM iterations."""
+@pytest.mark.parametrize("order,knots,bias_dt,solver", [
+    pytest.param(4, 140, 10.0, "bcr_solve_kernel", id="4-140"),
+    pytest.param(6, 96, 10.0, "bcr_solve_kernel", id="6-96"),
+    pytest.param(4, 64, 10.0, "bcr_solve_kernel", id="4-64"),
+    # bias knots every 1 s: 17 per spline, an arrow of m = 104 rows, wider than block cyclic reduction takes
+    pytest.param(4, 140, 1.0, "band_solve_kernel<false>", id="4-140-wide_arrow"),
+])
+def test_long_windows_band_solver_out_of_shared_memory(built, order, knots, bias_dt, solver):
+    """Windows whose band + arrow workspace exceeds shared memory.  Block cyclic reduction across CTAs
+    (bcr_solve_kernel) solves them when 6 beta <= 48 and the arrow has at most 54 rows; otherwise the single-CTA
+    two-sided factorisation runs chunk by chunk on shared-memory views of a global workspace (band_solve_kernel<false>,
+    not the resident 2-CTA cluster kernel).  Each case asserts which solver ran.  Compared with the dense cooperative Cholesky on the same system and
+    with the oracle's step; also through full LM iterations."""
     win = synthetic.make_window(order=order, num_knots=knots, num_landmarks=300, num_imu=600, seed=synthetic.SEED_BASE + 600 + knots,
-                                constant_knots=2)
+                                constant_knots=2, bias_dt=bias_dt)
     ow = ol.OracleWindow(win)
     o = ow.iterate(apply=False)
     deltas = []
@@ -408,4 +416,6 @@ def test_long_windows_band_solver_out_of_shared_memory(built, order, knots):
     for rec in recs:
         oo = ow.iterate(apply=True)
         assert rec["spd"] == 1 and abs(rec["cost"] - oo["cost"]) <= 1e-7 * oo["cost"] and rec["accepted"] == oo["accepted"]
+    ran = {name for name, _ in ctx.profile_iteration(reps=1)} & {"band_solve_kernel", "band_solve_kernel<false>", "bcr_solve_kernel"}
+    assert ran == {solver}, ran
     ctx.close()
