@@ -189,7 +189,6 @@ struct hb200_ctx {
   DevBuf<int2> m_idx;
   std::vector<int2> h_m_idx;
   double huber_bearing = 1.6e-3;   // reference optimizer.cpp:204
-  DevBuf<int> v_cam, v_lm;
   DevBuf<int4> v_idx, i_idx;
   std::vector<int4> h_v_idx, h_i_idx;       // bound order
   std::vector<int> v_perm, i_perm;          // bound position -> user index
@@ -931,7 +930,7 @@ void hb200_destroy(hb200_ctx* c) {
   for (cudaEvent_t e : c->prof_events) cudaEventDestroy(e);
   for (int s = 0; s < 2; ++s) { c->knots[s].release(); c->bg[s].release(); c->ba[s].release(); c->grav[s].release(); c->lms[s].release(); c->tab[s].release(); c->cp_pix[s].release(); c->cp_imu[s].release(); }
   c->cams.release(); c->imu.release(); c->cam_tab.release(); c->imu_tab.release(); c->fixed.release();
-  c->v_stamp.release(); c->v_pixel.release(); c->i_stamp.release(); c->i_meas.release(); c->v_cam.release(); c->v_lm.release(); c->v_idx.release(); c->i_idx.release();
+  c->v_stamp.release(); c->v_pixel.release(); c->i_stamp.release(); c->i_meas.release(); c->v_idx.release(); c->i_idx.release();
   c->v_z.release(); c->v_w.release(); c->m_stamp.release(); c->m_meas.release(); c->sensors.release(); c->m_sensor.release(); c->m_idx.release(); c->m_r.release(); c->m_Jp.release();
   c->run_off.release(); c->lm_off.release(); c->lm_obs.release(); c->d_invalid.release(); c->lm_order.release(); c->lm_group_off.release();
   c->v_r.release(); c->v_Jp.release(); c->v_Jl.release(); c->i_r.release(); c->i_Jp.release(); c->i_wg.release(); c->i_wa.release(); c->i_Jg.release();
@@ -1207,10 +1206,13 @@ int sync_host_mirrors(hb200_ctx* c) {
   return 0;
 }
 
-// Incidence lists of the device-resident factor lists (landmark CSR, inertial runs, longest track) by counting + scan
-// kernels, then everything hb200_bind derives from them.  One small read-back.
-int rebuild_incidence_device(hb200_ctx* c) {
-  const int Nv = c->Nv, Ni = c->Ni, L = c->L;
+// Everything the iteration runs on that follows from the bound factor lists on the device: the incidence lists
+// (landmark CSR, inertial runs, longest track) by counting + scan kernels with one small read-back, then the output
+// buffers and launch shapes of every factor family and the reduced system.  hb200_bind, hb200_append_* and
+// hb200_slide all end here; the ones that change the lists on the device mark the host mirrors stale
+// (device_managed) and drop the snapshot themselves.
+int derive_window(hb200_ctx* c) {
+  const int Nv = c->Nv, Ni = c->Ni, Nm = c->Nm, L = c->L;
   HB_CUDA(c->w_scal.ensure(8));
   HB_CUDA(cudaMemsetAsync(c->w_scal.p, 0, 8 * sizeof(int), c->stream));
   HB_CUDA(c->lm_off.ensure(static_cast<size_t>(L) + 2)); HB_CUDA(c->lm_obs.ensure(std::max(Nv, 1)));
@@ -1240,21 +1242,22 @@ int rebuild_incidence_device(hb200_ctx* c) {
   HB_CUDA(cudaMemcpyAsync(h, c->w_scal.p, sizeof(h), cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
   c->max_rows = std::max(6 * c->k, h[1]);
-  c->schur_groups = false;   // (the groups are cut on the host at hb200_bind; after device-side bookkeeping the per-landmark kernel runs)
+  c->schur_groups = false;   // the landmark groups are cut by hb200_bind, after this
   c->nruns = Ni ? h[3] : 0;
   if (Ni) { run_fill_kernel<<<(Ni + 255) / 256, 256, 0, c->stream>>>(Ni, c->w_keep.p, c->w_pos.p, c->nruns, c->run_off.p); HB_LAUNCH(c, "run_fill_kernel"); }
   else { const int z = 0; HB_CUDA(cudaMemcpyAsync(c->run_off.p, &z, sizeof(int), cudaMemcpyHostToDevice, c->stream)); }
   if (2 * 3 * static_cast<size_t>(c->max_rows) * sizeof(double) > 200 * 1024) return fail(-6, "landmark track spans %d control-point dofs; exceeds the Schur kernel's shared-memory tile", c->max_rows);
-  // outputs and launch shapes (as hb200_bind)
+  // outputs and launch shapes
   const size_t k = c->k;
   HB_CUDA(c->v_z.ensure(std::max(Nv, 1))); HB_CUDA(c->v_w.ensure(std::max(Nv, 1)));
   HB_CUDA(c->v_r.ensure(2 * static_cast<size_t>(std::max(Nv, 1)))); HB_CUDA(c->v_Jp.ensure(12 * k * std::max(Nv, 1))); HB_CUDA(c->v_Jl.ensure(6 * static_cast<size_t>(std::max(Nv, 1))));
   HB_CUDA(c->i_r.ensure(6 * static_cast<size_t>(std::max(Ni, 1)))); HB_CUDA(c->i_Jp.ensure(36 * k * std::max(Ni, 1)));
   HB_CUDA(c->i_wg.ensure(4 * static_cast<size_t>(std::max(Ni, 1)))); HB_CUDA(c->i_wa.ensure(4 * static_cast<size_t>(std::max(Ni, 1)))); HB_CUDA(c->i_Jg.ensure(12 * static_cast<size_t>(std::max(Ni, 1))));
+  HB_CUDA(c->m_r.ensure(6 * static_cast<size_t>(std::max(Nm, 1)))); HB_CUDA(c->m_Jp.ensure(36 * k * std::max(Nm, 1)));
   c->n_pix_blocks = (Nv + kEvalThreads - 1) / kEvalThreads;
   c->n_imu_blocks = (Ni + kEvalThreads - 1) / kEvalThreads;
-  c->n_man_blocks = 0;
-  for (int s2 = 0; s2 < 2; ++s2) { HB_CUDA(c->cp_pix[s2].ensure(std::max(c->n_pix_blocks, 1))); HB_CUDA(c->cp_imu[s2].ensure(std::max(c->n_imu_blocks, 1))); }
+  c->n_man_blocks = (Nm + kEvalThreads - 1) / kEvalThreads;
+  for (int s = 0; s < 2; ++s) { HB_CUDA(c->cp_pix[s].ensure(std::max(c->n_pix_blocks, 1))); HB_CUDA(c->cp_imu[s].ensure(std::max(c->n_imu_blocks + c->n_man_blocks, 1))); }
   if (c->max_rows * 6 * sizeof(double) > 48 * 1024) {
     const int smem = static_cast<int>(2 * 3 * static_cast<size_t>(c->max_rows) * sizeof(double));
     HB_CUDA(cudaFuncSetAttribute(schur_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
@@ -1265,10 +1268,31 @@ int rebuild_incidence_device(hb200_ctx* c) {
   if ((rc = ensure_system(c))) return rc;
   HB_CUDA(cudaStreamSynchronize(c->stream));
   c->bound = true;
-  c->device_managed = true;
   c->invalidate();
-  c->have_snapshot = false;
-  return sync_layout(c);
+  return sync_layout(c);   // multi-GPU: all ranks adopt the widest band (collective when a communicator is attached)
+}
+
+// Uploads the stamps, camera and landmark ids of n pixel factors to list positions [at, at + n) and binds them there;
+// factors that fail to bind are counted in d_invalid[0].  The ids only feed bind_pixel_kernel, so they go through
+// window scratch.
+int bind_pixel_range(hb200_ctx* c, int at, int n, const double* stamp, const int* camera, const int* landmark) {
+  HB_CUDA(c->w_keep.ensure(n)); HB_CUDA(c->w_pos.ensure(n));
+  HB_CUDA(cudaMemcpyAsync(c->v_stamp.p + at, stamp, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
+  HB_CUDA(cudaMemcpyAsync(c->w_keep.p, camera, sizeof(int) * n, cudaMemcpyHostToDevice, c->stream));
+  HB_CUDA(cudaMemcpyAsync(c->w_pos.p, landmark, sizeof(int) * n, cudaMemcpyHostToDevice, c->stream));
+  bind_pixel_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(n, c->v_stamp.p + at, c->w_keep.p, c->w_pos.p, c->knots[0].p, c->K, c->k, c->C, c->L, c->v_idx.p + at, c->d_invalid.p);
+  HB_LAUNCH(c, "bind_pixel_kernel");
+  return 0;
+}
+
+// Uploads the stamps of n inertial factors to list positions [at, at + n) and binds them there; factors that fail to
+// bind are counted in d_invalid[0].
+int bind_inertial_range(hb200_ctx* c, int at, int n, const double* stamp) {
+  HB_CUDA(cudaMemcpyAsync(c->i_stamp.p + at, stamp, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
+  bind_inertial_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(n, c->i_stamp.p + at, c->knots[0].p, c->K, c->k, c->bg[0].p, c->Kbg, c->ba[0].p, c->Kba, c->kb,
+                                                             c->i_idx.p + at, c->d_invalid.p);
+  HB_LAUNCH(c, "bind_inertial_kernel");
+  return 0;
 }
 }  // namespace
 
@@ -1286,27 +1310,20 @@ int hb200_bind(hb200_ctx* c, int* num_invalid) {
   HB_CUDA(c->d_invalid.ensure(1));
   HB_CUDA(cudaMemsetAsync(c->d_invalid.p, 0, sizeof(int), c->stream));
   HB_CUDA(c->v_stamp.ensure(std::max(Nv, 1))); HB_CUDA(c->v_pixel.ensure(2 * static_cast<size_t>(std::max(Nv, 1))));
-  HB_CUDA(c->v_cam.ensure(std::max(Nv, 1))); HB_CUDA(c->v_lm.ensure(std::max(Nv, 1))); HB_CUDA(c->v_idx.ensure(std::max(Nv, 1)));
-  HB_CUDA(c->v_z.ensure(std::max(Nv, 1))); HB_CUDA(c->v_w.ensure(std::max(Nv, 1)));
+  HB_CUDA(c->v_idx.ensure(std::max(Nv, 1))); HB_CUDA(c->v_z.ensure(std::max(Nv, 1)));
   HB_CUDA(c->m_stamp.ensure(std::max(Nm, 1))); HB_CUDA(c->m_meas.ensure(7 * static_cast<size_t>(std::max(Nm, 1)))); HB_CUDA(c->m_sensor.ensure(std::max(Nm, 1)));
   HB_CUDA(c->m_idx.ensure(std::max(Nm, 1)));
   c->h_m_idx.assign(Nm, make_int2(0, 0));
   HB_CUDA(c->i_stamp.ensure(std::max(Ni, 1))); HB_CUDA(c->i_meas.ensure(6 * static_cast<size_t>(std::max(Ni, 1)))); HB_CUDA(c->i_idx.ensure(std::max(Ni, 1)));
   c->h_v_idx.assign(Nv, make_int4(0, 0, 0, 0)); c->h_i_idx.assign(Ni, make_int4(0, 0, 0, 0));
   // pass 1: index maps in user order (device), a2/a4
+  int rc = 0;
   if (Nv) {
-    HB_CUDA(cudaMemcpyAsync(c->v_stamp.p, c->h_v_stamp.data(), sizeof(double) * Nv, cudaMemcpyHostToDevice, c->stream));
-    HB_CUDA(cudaMemcpyAsync(c->v_cam.p, c->h_v_cam.data(), sizeof(int) * Nv, cudaMemcpyHostToDevice, c->stream));
-    HB_CUDA(cudaMemcpyAsync(c->v_lm.p, c->h_v_lm.data(), sizeof(int) * Nv, cudaMemcpyHostToDevice, c->stream));
-    bind_pixel_kernel<<<(Nv + 127) / 128, 128, 0, c->stream>>>(Nv, c->v_stamp.p, c->v_cam.p, c->v_lm.p, c->knots[0].p, c->K, c->k, c->C, c->L, c->v_idx.p, c->d_invalid.p);
-    HB_LAUNCH(c, "bind_pixel_kernel");
+    if ((rc = bind_pixel_range(c, 0, Nv, c->h_v_stamp.data(), c->h_v_cam.data(), c->h_v_lm.data()))) return rc;
     HB_CUDA(cudaMemcpyAsync(c->h_v_idx.data(), c->v_idx.p, sizeof(int4) * Nv, cudaMemcpyDeviceToHost, c->stream));
   }
   if (Ni) {
-    HB_CUDA(cudaMemcpyAsync(c->i_stamp.p, c->h_i_stamp.data(), sizeof(double) * Ni, cudaMemcpyHostToDevice, c->stream));
-    bind_inertial_kernel<<<(Ni + 127) / 128, 128, 0, c->stream>>>(Ni, c->i_stamp.p, c->knots[0].p, c->K, c->k, c->bg[0].p, c->Kbg, c->ba[0].p, c->Kba, c->kb,
-                                                               c->i_idx.p, c->d_invalid.p);
-    HB_LAUNCH(c, "bind_inertial_kernel");
+    if ((rc = bind_inertial_range(c, 0, Ni, c->h_i_stamp.data()))) return rc;
     HB_CUDA(cudaMemcpyAsync(c->h_i_idx.data(), c->i_idx.p, sizeof(int4) * Ni, cudaMemcpyDeviceToHost, c->stream));
   }
   if (Nm) {
@@ -1357,47 +1374,26 @@ int hb200_bind(hb200_ctx* c, int* num_invalid) {
     }
     HB_CUDA(cudaStreamSynchronize(c->stream));
   }
-  // runs (inertial), landmark incidence (CSR)
-  std::vector<int> runs;
-  for (int p = 0; p < Ni; ++p) {
-    const int4& a = c->h_i_idx[p];
-    if (p == 0 || a.x != c->h_i_idx[p - 1].x || a.y != c->h_i_idx[p - 1].y || a.z != c->h_i_idx[p - 1].z) runs.push_back(p);
-  }
-  c->nruns = static_cast<int>(runs.size());
-  runs.push_back(Ni);
-  std::vector<int> off(c->L + 1, 0), obs(std::max(Nv, 1));
-  for (int p = 0; p < Nv; ++p) off[c->h_v_idx[p].y + 1] += 1;
-  for (int l = 0; l < c->L; ++l) off[l + 1] += off[l];
-  {
-    std::vector<int> cur(off.begin(), off.end() - 1);
-    for (int p = 0; p < Nv; ++p) obs[cur[c->h_v_idx[p].y]++] = p;
-  }
-  c->max_rows = 6 * c->k;
-  for (int l = 0; l < c->L; ++l)
-    if (off[l + 1] > off[l]) c->max_rows = std::max(c->max_rows, 6 * (c->h_v_idx[obs[off[l + 1] - 1]].x + c->k - c->h_v_idx[obs[off[l]]].x));
-  if (2 * 3 * static_cast<size_t>(c->max_rows) * sizeof(double) > 200 * 1024) return fail(-6, "landmark track spans %d control-point dofs; exceeds the Schur kernel's shared-memory tile", c->max_rows);
-  HB_CUDA(c->run_off.ensure(runs.size())); HB_CUDA(c->lm_off.ensure(off.size())); HB_CUDA(c->lm_obs.ensure(obs.size()));
-  HB_CUDA(cudaMemcpyAsync(c->run_off.p, runs.data(), sizeof(int) * runs.size(), cudaMemcpyHostToDevice, c->stream));
-  HB_CUDA(cudaMemcpyAsync(c->lm_off.p, off.data(), sizeof(int) * off.size(), cudaMemcpyHostToDevice, c->stream));
-  HB_CUDA(cudaMemcpyAsync(c->lm_obs.p, obs.data(), sizeof(int) * obs.size(), cudaMemcpyHostToDevice, c->stream));
+  if ((rc = derive_window(c))) return rc;
   {
     // landmark groups for the large-window Schur kernel: observed landmarks ordered by their first knot base, cut so that
     // a group has at most kSchurGroup members and its control-point rows fit one window of RT rows
     constexpr int kSchurGroupMin = 8192;   // landmarks from which schur_group_kernel replaces schur_kernel
-    c->schur_groups = false;
     c->schur_rt = ((c->max_rows + 12 + 7) / 8) * 8;
     if (c->L >= kSchurGroupMin && Nv) {
+      // first / last knot base of every observed landmark (-1: unobserved); bound order is ascending knot base
+      std::vector<int> first(c->L, -1), last(c->L, -1);
+      for (const int4& id : c->h_v_idx) { if (first[id.y] < 0) first[id.y] = id.x; last[id.y] = id.x; }
       std::vector<int> order;
       order.reserve(c->L);
-      for (int l = 0; l < c->L; ++l) if (off[l + 1] > off[l]) order.push_back(l);
-      auto first_base = [&](int l) { return c->h_v_idx[obs[off[l]]].x; };
-      std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return first_base(a) < first_base(b); });
+      for (int l = 0; l < c->L; ++l) if (first[l] >= 0) order.push_back(l);
+      std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return first[a] < first[b]; });
       std::vector<int> goff;
       const int win = c->schur_rt / 6;   // control points per window
       int glo = 0;
       for (size_t i = 0; i < order.size(); ++i) {
         const int l = order[i];
-        const int lo = first_base(l), hi = c->h_v_idx[obs[off[l + 1] - 1]].x + c->k;
+        const int lo = first[l], hi = last[l] + c->k;
         if (goff.empty() || static_cast<int>(i) - goff.back() >= kSchurGroup || hi - glo > win) { goff.push_back(static_cast<int>(i)); glo = lo; }
       }
       c->n_lm_groups = static_cast<int>(goff.size());
@@ -1405,7 +1401,6 @@ int hb200_bind(hb200_ctx* c, int* num_invalid) {
       HB_CUDA(c->lm_order.ensure(std::max<size_t>(order.size(), 1))); HB_CUDA(c->lm_group_off.ensure(goff.size()));
       HB_CUDA(cudaMemcpyAsync(c->lm_order.p, order.data(), sizeof(int) * order.size(), cudaMemcpyHostToDevice, c->stream));
       HB_CUDA(cudaMemcpyAsync(c->lm_group_off.p, goff.data(), sizeof(int) * goff.size(), cudaMemcpyHostToDevice, c->stream));
-      HB_CUDA(cudaStreamSynchronize(c->stream));
       c->schur_groups = c->n_lm_groups > 0;
       const size_t smem = (3 * static_cast<size_t>(kSchurGroup) * (c->schur_rt + 1) + 3 * kSchurGroup + 4 * 3 * static_cast<size_t>(c->schur_rt)) * sizeof(double);
       if (smem > 200 * 1024) c->schur_groups = false;
@@ -1415,34 +1410,13 @@ int hb200_bind(hb200_ctx* c, int* num_invalid) {
       }
     }
   }
-  // outputs
-  const size_t k = c->k;
-  HB_CUDA(c->v_r.ensure(2 * static_cast<size_t>(std::max(Nv, 1)))); HB_CUDA(c->v_Jp.ensure(12 * k * std::max(Nv, 1))); HB_CUDA(c->v_Jl.ensure(6 * static_cast<size_t>(std::max(Nv, 1))));
-  HB_CUDA(c->i_r.ensure(6 * static_cast<size_t>(std::max(Ni, 1)))); HB_CUDA(c->i_Jp.ensure(36 * k * std::max(Ni, 1)));
-  HB_CUDA(c->i_wg.ensure(4 * static_cast<size_t>(std::max(Ni, 1)))); HB_CUDA(c->i_wa.ensure(4 * static_cast<size_t>(std::max(Ni, 1)))); HB_CUDA(c->i_Jg.ensure(12 * static_cast<size_t>(std::max(Ni, 1))));
-  c->n_pix_blocks = (Nv + kEvalThreads - 1) / kEvalThreads;
-  c->n_imu_blocks = (Ni + kEvalThreads - 1) / kEvalThreads;
-  c->n_man_blocks = (Nm + kEvalThreads - 1) / kEvalThreads;
-  HB_CUDA(c->m_r.ensure(6 * static_cast<size_t>(std::max(Nm, 1)))); HB_CUDA(c->m_Jp.ensure(36 * k * std::max(Nm, 1)));
-  for (int s = 0; s < 2; ++s) { HB_CUDA(c->cp_pix[s].ensure(std::max(c->n_pix_blocks, 1))); HB_CUDA(c->cp_imu[s].ensure(std::max(c->n_imu_blocks + c->n_man_blocks, 1))); }
-  if (c->max_rows * 6 * sizeof(double) > 48 * 1024) {
-    const int smem = static_cast<int>(2 * 3 * static_cast<size_t>(c->max_rows) * sizeof(double));
-    HB_CUDA(cudaFuncSetAttribute(schur_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    HB_CUDA(cudaFuncSetAttribute(schur_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  }
-  int rc = update_fixed(c);
-  if (rc) return rc;
-  rc = ensure_system(c);
-  if (rc) return rc;
   if (c->schur_groups) {   // unobserved landmarks are not in any group: their blocks stay zero (no step)
     HB_CUDA(cudaMemsetAsync(c->Vinv.p, 0, sizeof(double) * 9 * static_cast<size_t>(std::max(c->L, 1)), c->stream));
     HB_CUDA(cudaMemsetAsync(c->gl.p, 0, sizeof(double) * 3 * static_cast<size_t>(std::max(c->L, 1)), c->stream));
     HB_CUDA(cudaMemsetAsync(c->Dl.p, 0, sizeof(double) * 3 * static_cast<size_t>(std::max(c->L, 1)), c->stream));
   }
   HB_CUDA(cudaStreamSynchronize(c->stream));
-  c->bound = true;
-  c->invalidate();
-  return sync_layout(c);   // multi-GPU: all ranks adopt the widest band (collective when a communicator is attached)
+  return 0;
 }
 
 int hb200_get_index_maps(hb200_ctx* c, int* pixel_base, int* inertial_base, int* gyro_bias_base, int* accel_bias_base) {
@@ -2241,7 +2215,8 @@ int hb200_append_landmarks(hb200_ctx* c, int n, const double* xyz) {
   HB_CUDA(cudaMemcpyAsync(c->lms[0].p + 3 * L, xyz, sizeof(double) * 3 * n, cudaMemcpyHostToDevice, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
   c->L = static_cast<int>(L) + n;
-  return rebuild_incidence_device(c);
+  c->device_managed = true; c->have_snapshot = false;
+  return derive_window(c);
 }
 
 int hb200_append_pixel_factors(hb200_ctx* c, int n, const double* stamp, const int* camera, const int* landmark, const double* pixel) {
@@ -2251,16 +2226,10 @@ int hb200_append_pixel_factors(hb200_ctx* c, int n, const double* stamp, const i
   HB_CUDA(cudaSetDevice(c->device));
   const size_t Nv = c->Nv;
   HB_CUDA(c->v_stamp.grow(Nv + n, Nv, c->stream)); HB_CUDA(c->v_pixel.grow(2 * (Nv + n), 2 * Nv, c->stream)); HB_CUDA(c->v_idx.grow(Nv + n, Nv, c->stream));
-  DevBuf<int> d_cam, d_lm;
-  HB_CUDA(d_cam.ensure(n)); HB_CUDA(d_lm.ensure(n));
   HB_CUDA(c->d_invalid.ensure(2));
   HB_CUDA(cudaMemsetAsync(c->d_invalid.p, 0, 2 * sizeof(int), c->stream));
-  HB_CUDA(cudaMemcpyAsync(c->v_stamp.p + Nv, stamp, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
   HB_CUDA(cudaMemcpyAsync(c->v_pixel.p + 2 * Nv, pixel, sizeof(double) * 2 * n, cudaMemcpyHostToDevice, c->stream));
-  HB_CUDA(cudaMemcpyAsync(d_cam.p, camera, sizeof(int) * n, cudaMemcpyHostToDevice, c->stream));
-  HB_CUDA(cudaMemcpyAsync(d_lm.p, landmark, sizeof(int) * n, cudaMemcpyHostToDevice, c->stream));
-  bind_pixel_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(n, c->v_stamp.p + Nv, d_cam.p, d_lm.p, c->knots[0].p, c->K, c->k, c->C, c->L, c->v_idx.p + Nv, c->d_invalid.p);
-  HB_LAUNCH(c, "bind_pixel_kernel");
+  if ((rc = bind_pixel_range(c, static_cast<int>(Nv), n, stamp, camera, landmark))) return rc;
   tail_sorted_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(static_cast<int>(Nv), n, c->v_idx.p, c->d_invalid.p + 1);
   HB_LAUNCH(c, "tail_sorted_kernel");
   int bad[2] = {0, 0};
@@ -2269,7 +2238,8 @@ int hb200_append_pixel_factors(hb200_ctx* c, int n, const double* stamp, const i
   if (bad[0]) return fail(2, "%d appended factor(s) reference a stamp outside the spline's valid range or an invalid camera / landmark", bad[0]);
   if (bad[1]) return fail(3, "appended factors must arrive in stamp order (%d fall before the end of the list): use hb200_set_pixel_factors + hb200_bind", bad[1]);
   c->Nv = static_cast<int>(Nv) + n; c->Np = c->Nv;
-  return rebuild_incidence_device(c);
+  c->device_managed = true; c->have_snapshot = false;
+  return derive_window(c);
 }
 
 int hb200_append_inertial_factors(hb200_ctx* c, int n, const double* stamp, const double* meas) {
@@ -2282,11 +2252,8 @@ int hb200_append_inertial_factors(hb200_ctx* c, int n, const double* stamp, cons
   HB_CUDA(c->i_stamp.grow(Ni + n, Ni, c->stream)); HB_CUDA(c->i_meas.grow(6 * (Ni + n), 6 * Ni, c->stream)); HB_CUDA(c->i_idx.grow(Ni + n, Ni, c->stream));
   HB_CUDA(c->d_invalid.ensure(2));
   HB_CUDA(cudaMemsetAsync(c->d_invalid.p, 0, 2 * sizeof(int), c->stream));
-  HB_CUDA(cudaMemcpyAsync(c->i_stamp.p + Ni, stamp, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
   HB_CUDA(cudaMemcpyAsync(c->i_meas.p + 6 * Ni, meas, sizeof(double) * 6 * n, cudaMemcpyHostToDevice, c->stream));
-  bind_inertial_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(n, c->i_stamp.p + Ni, c->knots[0].p, c->K, c->k, c->bg[0].p, c->Kbg, c->ba[0].p, c->Kba, c->kb,
-                                                             c->i_idx.p + Ni, c->d_invalid.p);
-  HB_LAUNCH(c, "bind_inertial_kernel");
+  if ((rc = bind_inertial_range(c, static_cast<int>(Ni), n, stamp))) return rc;
   tail_sorted_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(static_cast<int>(Ni), n, c->i_idx.p, c->d_invalid.p + 1);
   HB_LAUNCH(c, "tail_sorted_kernel");
   int bad[2] = {0, 0};
@@ -2295,7 +2262,8 @@ int hb200_append_inertial_factors(hb200_ctx* c, int n, const double* stamp, cons
   if (bad[0]) return fail(2, "%d appended factor(s) reference a stamp outside the state or bias splines' valid range", bad[0]);
   if (bad[1]) return fail(3, "appended factors must arrive in stamp order (%d fall before the end of the list): use hb200_set_inertial_factors + hb200_bind", bad[1]);
   c->Ni = static_cast<int>(Ni) + n;
-  return rebuild_incidence_device(c);
+  c->device_managed = true; c->have_snapshot = false;
+  return derive_window(c);
 }
 
 int hb200_slide(hb200_ctx* c, double lower_bound, int flags, hb200_slide_stats* stats) {
@@ -2388,7 +2356,8 @@ int hb200_slide(hb200_ctx* c, double lower_bound, int flags, hb200_slide_stats* 
     stats->visual_factors_dropped = Nv - Nv_new; stats->inertial_factors_dropped = Ni - Ni_new;
     stats->knots = K_new; stats->landmarks = L_new; stats->visual_factors = Nv_new; stats->inertial_factors = Ni_new;
   }
-  return rebuild_incidence_device(c);
+  c->device_managed = true; c->have_snapshot = false;
+  return derive_window(c);
 }
 
 int hb200_window_sizes(hb200_ctx* c, int* knots, int* landmarks, int* visual_factors, int* inertial_factors) {

@@ -5,8 +5,8 @@
 // at or before the window's lower bound constant and removing the ones no residual touches any more
 // (optimizer.cpp:286-345) -- here on the flattened window that already lives in HBM: no host re-sort, no re-upload
 // of the factor lists.  New factors arrive in stamp order, so appending keeps the bound order (sorted by knot base);
-// removal is an order-preserving stream compaction; the incidence lists (landmark CSR, inertial runs, segment
-// offsets) are rebuilt by counting + scan kernels.  Integer work: bit-exact against the host path by construction.
+// removal is an order-preserving stream compaction.  The incidence lists (landmark CSR, inertial runs, longest track)
+// are built by the counting + scan kernels below, after hb200_bind as after every append or slide.
 #pragma once
 #include "hb200_eval.cuh"
 
