@@ -792,9 +792,10 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
     // A[row l/4][k l%4] and B[k l%4][col l/4] -- both are AR[row][col0 + l%4] -- and C[row l/4][col 2(l%4)+{0,1}].
     const int nrb = (m + 1 + 7) / 8, ncb = (m + 7) / 8;
     const int lr = lane >> 2, lk = lane & 3;
-    const int nks = SMEM ? 1 : 4;   // split the contraction when the panels stream from global memory (more warps, more loads in flight)
-    for (int e = warp; e < nrb * ncb * nks; e += kBandThreads / 32) {
-      const int part = e % nks, tile = e / nks;
+    // One warp owns each output tile and contracts every column of both chains into it, in a fixed order, so the
+    // corner, and with it the step, is bit-identical from solve to solve (splitting a tile's contraction across
+    // warps and merging the parts with shared-memory atomics made the chunked solver's step vary in the last bits).
+    for (int tile = warp; tile < nrb * ncb; tile += kBandThreads / 32) {
       const int ub = tile / ncb, vb = tile - ub * ncb;
       if (vb > ub) continue;
       double c0 = 0.0, c1 = 0.0;
@@ -802,9 +803,7 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
       for (int ci = 0; ci < 2; ++ci) {
         if (CL && ci != rank) continue;
         const BandChain& Q = ci ? C1 : C0;
-        const int nused = ci ? 6 * C1.Ke : C0.npc;
-        const int per = ((nused + 4 * nks - 1) / (4 * nks)) * 4;          // columns of this part (multiple of 4)
-        const int lo = part * per, hi = min(nused, lo + per);
+        const int lo = 0, hi = ci ? 6 * C1.Ke : C0.npc;                    // the chain's eliminated columns
         const double* pa = Q.AR + static_cast<size_t>(min(8 * ub + lr, m)) * Q.npc + lk;
         const double* pb = Q.AR + static_cast<size_t>(min(8 * vb + lr, m)) * Q.npc + lk;
         for (int col = lo; col < hi; col += 16) {
@@ -824,8 +823,8 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
       double* cu = CC + static_cast<size_t>(u) * LDc + v;
       const bool in0 = u <= m && v < m && v <= u, in1 = u <= m && v + 1 < m && v + 1 <= u;
       if (!CL) {
-        if (in0) atomicAdd(cu, -c0);
-        if (in1) atomicAdd(cu + 1, -c1);
+        if (in0) cu[0] -= c0;
+        if (in1) cu[1] -= c1;
       } else if (rank == 1) {   // every corner entry belongs to one lane of one tile
         if (in0) cu[0] = c0;
         if (in1) cu[1] = c1;

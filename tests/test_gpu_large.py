@@ -10,6 +10,7 @@ import numpy as np
 import pytest
 
 import oracle_lib as ol
+import sysref as sr
 from hyperslam_b200 import runtime, synthetic
 
 pytestmark = pytest.mark.gpu
@@ -29,7 +30,7 @@ def chunked_rel_err(a, b, rows=65536):
 
 
 @pytest.mark.parametrize("config,force_dense", [(2, False), (2, True), (3, False), (4, False)])
-def test_full_size_config_parity(built, config, force_dense):
+def test_full_size_config_parity(built, record_property, config, force_dense):
     win = synthetic.make_config(config, constant_knots=2)
     ow = ol.OracleWindow(win)
     assert ow.bad == 0
@@ -62,6 +63,9 @@ def test_full_size_config_parity(built, config, force_dense):
     assert res < 1e-7, res
     assert rel_err(dp, o["delta_p"]) < 1e-5
     assert rel_err(dl, o["delta_l"]) < 1e-5
+    # block by block in equilibrated units (inertial, Schur-group and manifold Hessian blocks each carry their own scale)
+    for key, v in sr.check_system_and_step(S, b, dp, o["S"], o["b"], win.knots.shape[0], win.gyro_bias.shape[0], win.accel_bias.shape[0]).items():
+        record_property(key, v)
     del S, o
 
     # three LM iterations: costs, acceptance, trust region, final state
@@ -77,5 +81,7 @@ def test_full_size_config_parity(built, config, force_dense):
     st, so = ctx.state(), ow.state()
     for key in so:
         assert rel_err(st[key], so[key]) < 1e-6, key
+    for key, v in sr.bias_values(so).items():
+        assert rel_err(sr.bias_values(st)[key], v) < 1e-6, key
     assert recs[-1]["cost"] < recs[0]["cost"]
     ctx.close()

@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 
 import oracle_lib as ol
+import sysref as sr
 from hyperslam_b200 import runtime, synthetic
 
 pytestmark = pytest.mark.gpu
@@ -17,6 +18,15 @@ J_TOL = 1e-8   # Jacobians, relative to the largest entry of the list
 
 def rel_err(a, b):
     return float(np.abs(a - b).max() / (np.abs(b).max() + 1e-300))
+
+
+def sizes(win):
+    return win.knots.shape[0], win.gyro_bias.shape[0], win.accel_bias.shape[0]
+
+
+def report(record_property, measured):
+    for key, v in measured.items():
+        record_property(key, v)
 
 
 def make_ctx(win, **kw):
@@ -116,7 +126,7 @@ def test_edge_cases(built):
 
 @pytest.mark.parametrize("force_dense", [False, True])
 @pytest.mark.parametrize("name", ["k4", "k6", "k4_generic_calib", "cfg0_plumbing", "pixel_only"])
-def test_system_and_step_parity(built, name, force_dense):
+def test_system_and_step_parity(built, record_property, name, force_dense):
     kw = dict(CASES[name])
     win = synthetic.make_window(seed=synthetic.SEED_BASE + 200, constant_knots=2, **kw)
     ow = ol.OracleWindow(win)
@@ -129,6 +139,8 @@ def test_system_and_step_parity(built, name, force_dense):
     assert rel_err(b, o["b"]) < 1e-9
     ctx.solve()
     dp, dl = ctx.delta()
+    # block by block in equilibrated units; the step by its backward error on the GPU's own system
+    report(record_property, sr.check_system_and_step(S, b, dp, o["S"], o["b"], *sizes(win)))
     # the reduced system is ill-conditioned along gauge directions: compare through the residual
     # of the linear system and directly with a condition-aware tolerance
     res = np.abs(o["S"] @ dp - o["b"]).max() / (np.abs(o["b"]).max() + 1e-300)
@@ -155,6 +167,8 @@ def test_iterate_parity(built, use_graph, force_dense):
     st, so = ctx.state(), ow.state()
     for key in so:
         assert rel_err(st[key], so[key]) < 1e-6, key
+    for key, v in sr.bias_values(so).items():
+        assert rel_err(sr.bias_values(st)[key], v) < 1e-6, key
     assert recs[-1]["cost"] < recs[0]["cost"]
     ctx.close()
 
@@ -285,7 +299,7 @@ def test_bearing_and_manifold_evaluate_parity(built, order):
 
 @pytest.mark.parametrize("force_dense", [False, True])
 @pytest.mark.parametrize("order", [4, 6])
-def test_bearing_and_manifold_system_parity(built, order, force_dense):
+def test_bearing_and_manifold_system_parity(built, record_property, order, force_dense):
     win = widened_window(order, seed_off=1)
     ow = ol.OracleWindow(win)
     o = ow.iterate(apply=False)
@@ -297,6 +311,7 @@ def test_bearing_and_manifold_system_parity(built, order, force_dense):
     assert rel_err(b, o["b"]) < 1e-9
     ctx.solve()
     dp, dl = ctx.delta()
+    report(record_property, sr.check_system_and_step(S, b, dp, o["S"], o["b"], *sizes(win)))
     res = np.abs(o["S"] @ dp - o["b"]).max() / (np.abs(o["b"]).max() + 1e-300)
     assert res < 1e-7, res
     assert rel_err(dp, o["delta_p"]) < 1e-5
@@ -319,6 +334,8 @@ def test_bearing_and_manifold_iterate_parity(built, use_graph):
     st, so = ctx.state(), ow.state()
     for key in so:
         assert rel_err(st[key], so[key]) < 1e-6, key
+    for key, v in sr.bias_values(so).items():
+        assert rel_err(sr.bias_values(st)[key], v) < 1e-6, key
     assert recs[-1]["cost"] < recs[0]["cost"]
     ctx.close()
 
@@ -387,7 +404,7 @@ def test_bearing_and_manifold_factor_evaluate_ceres_shape(built):
     # bias knots every 1 s: 17 per spline, an arrow of m = 104 rows, wider than block cyclic reduction takes
     pytest.param(4, 140, 1.0, "band_solve_kernel<false>", id="4-140-wide_arrow"),
 ])
-def test_long_windows_band_solver_out_of_shared_memory(built, order, knots, bias_dt, solver):
+def test_long_windows_band_solver_out_of_shared_memory(built, record_property, order, knots, bias_dt, solver):
     """Windows whose band + arrow workspace exceeds shared memory.  Block cyclic reduction across CTAs
     (bcr_solve_kernel) solves them when 6 beta <= 48 and the arrow has at most 54 rows; otherwise the single-CTA
     two-sided factorisation runs chunk by chunk on shared-memory views of a global workspace (band_solve_kernel<false>,
@@ -404,6 +421,10 @@ def test_long_windows_band_solver_out_of_shared_memory(built, order, knots, bias
         ctx.build_system()
         ctx.solve()
         dp, dl = ctx.delta()
+        S, b = ctx.system()
+        measured = sr.check_system_and_step(S, b, dp, o["S"], o["b"], *sizes(win))
+        report(record_property, {f"{'dense' if force_dense else 'band'}_{k}": v for k, v in measured.items()})
+        del S
         res = np.abs(o["S"] @ dp - o["b"]).max() / (np.abs(o["b"]).max() + 1e-300)
         assert res < 1e-7, (force_dense, res)
         assert rel_err(dp, o["delta_p"]) < 1e-5
