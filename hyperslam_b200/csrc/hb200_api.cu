@@ -18,6 +18,7 @@
 #include "../../include/hyperb200.h"
 #include "hb200_bcr.cuh"
 #include "hb200_calib.cuh"
+#include "hb200_cov.cuh"
 #include "hb200_window.cuh"
 
 using namespace hb;
@@ -253,6 +254,24 @@ struct hb200_ctx {
   int n_lm_blocks = 0;
   bool system_built = false;
 
+  // marginal covariances (hb200_build_covariance / hb200_compute_covariance).  cov_st: the build's own solver state
+  // (radius +inf: no damping inside the landmark elimination; st is never touched).  cov_at: launch count after the last
+  // covariance call -- any other launch since (an evaluation, an iteration, a slide) rewrote what the compute reads.
+  // *_next: what the next compute writes / the knots the build saw; committed to the unsuffixed buffers on success only.
+  DevBuf<SolverState> cov_st;
+  DevBuf<double> cov_ws, cov_packed, cov_packed_next, cov_lm, cov_lm_next, cov_knots, cov_knots_next, cov_tab, cov_tab_next;
+  DevBuf<int> cov_counts;
+  DevBuf<CovStatus> cov_status;
+  bool cov_built = false, cov_valid = false;
+  long long cov_at = -1;
+  int cov_degenerate = 0, cov_unobserved = 0;
+  SysLayout cov_lay{}, cov_lay_next{};
+  Basis cov_basis{}, cov_basis_next{};
+  int cov_L = 0, cov_L_next = 0;
+  int cov_k_next = 0, cov_Nv_next = 0, cov_max_rows_next = 0;   // shapes the build's landmark outputs were written with
+  DevBuf<double> cov_t, cov_o;   // hb200_interpolate_covariance staging
+  DevBuf<int> cov_bad;
+
   hb200_allreduce_fn allreduce = nullptr;
   void* allreduce_user = nullptr;
   // multi-GPU: one NCCL all-reduce of the packed system per iteration, enqueued from C on the context's stream
@@ -296,7 +315,7 @@ struct hb200_ctx {
   int o_bg() const { return 6 * K; }
   int o_ba() const { return 6 * K + 3 * Kbg; }
   int o_g() const { return 6 * K + 3 * Kbg + 3 * Kba; }
-  void invalidate() { graph_valid = false; system_built = false; evaluated_J = false; mirror_valid = false; calib_valid = false; }
+  void invalidate() { graph_valid = false; system_built = false; cov_built = false; evaluated_J = false; mirror_valid = false; calib_valid = false; }
 };
 
 namespace {
@@ -571,7 +590,8 @@ int enqueue_evaluate(hb200_ctx* c, bool want_J, int sel, bool accumulate = false
 // complement on the main stream.  Both accumulate into S with atomics (commutative), diag(J^T J) is kept apart from S,
 // so nothing orders them.  The side stream is forked here, not before the evaluation, when the factor Jacobians were
 // produced on the MAIN stream (merged factor kernel).
-int enqueue_build(hb200_ctx* c) {
+// st: the solver state whose radius damps the landmark blocks (the LM's c->st, or the covariance build's radius +inf).
+int enqueue_build(hb200_ctx* c, const SolverState* st) {
   { const int rf = fork_side(c); if (rf) return rf; }   // (no-op when already forked or while profiling)
   if (c->Ni) {
     // large windows (>= 16 384 inertial factors): the augmented product on the FP64 tensor cores, ~6 CTAs per SM of 8-factor
@@ -612,18 +632,18 @@ int enqueue_build(hb200_ctx* c) {
     const size_t smem = (3 * static_cast<size_t>(kSchurGroup) * (c->schur_rt + 1) + 3 * kSchurGroup + 4 * 3 * static_cast<size_t>(c->schur_rt)) * sizeof(double);
     if (c->k == 4)
       schur_group_kernel<4><<<c->n_lm_groups, kSchurGThreads, smem, c->stream>>>(c->lm_group_off.p, c->lm_order.p, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p, c->v_Jp.p,
-                                                                                 c->v_Jl.p, c->v_w.p, c->st.p, c->assembly(), c->lay, c->Vchol.p, c->gl.p, c->Dl.p, c->schur_rt);
+                                                                                 c->v_Jl.p, c->v_w.p, st, c->assembly(), c->lay, c->Vchol.p, c->gl.p, c->Dl.p, c->schur_rt);
     else
       schur_group_kernel<6><<<c->n_lm_groups, kSchurGThreads, smem, c->stream>>>(c->lm_group_off.p, c->lm_order.p, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p, c->v_Jp.p,
-                                                                                 c->v_Jl.p, c->v_w.p, c->st.p, c->assembly(), c->lay, c->Vchol.p, c->gl.p, c->Dl.p, c->schur_rt);
+                                                                                 c->v_Jl.p, c->v_w.p, st, c->assembly(), c->lay, c->Vchol.p, c->gl.p, c->Dl.p, c->schur_rt);
     HB_LAUNCH(c, "schur_group_kernel");
   } else if (c->Nv && c->L) {
     const size_t smem = 2 * 3 * static_cast<size_t>(c->max_rows) * sizeof(double);
     if (c->k == 4)
-      schur_kernel<4><<<c->L, kSchurThreads, smem, c->stream>>>(c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p, c->st.p,
+      schur_kernel<4><<<c->L, kSchurThreads, smem, c->stream>>>(c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p, st,
                                                                 c->assembly(), c->lay, c->Vchol.p, c->gl.p, c->Dl.p, c->max_rows);
     else
-      schur_kernel<6><<<c->L, kSchurThreads, smem, c->stream>>>(c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p, c->st.p,
+      schur_kernel<6><<<c->L, kSchurThreads, smem, c->stream>>>(c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p, st,
                                                                 c->assembly(), c->lay, c->Vchol.p, c->gl.p, c->Dl.p, c->max_rows);
     HB_LAUNCH(c, "schur_kernel");
   }
@@ -810,7 +830,7 @@ int enqueue_iteration(hb200_ctx* c) {
   int rc = 0;
   // the factor kernels clear the packed system and accumulate the pixel J^T J into it (enqueue_build does the rest)
   if ((rc = enqueue_evaluate(c, true, 0, /*accumulate=*/true, /*keep_fork=*/true, /*clear_system=*/true))) return rc;
-  if ((rc = enqueue_build(c))) return rc;
+  if ((rc = enqueue_build(c, c->st.p))) return rc;
   if ((rc = enqueue_reduce_system(c))) return rc;
   bool retracted = false;
   if ((rc = enqueue_solve(c, /*fuse_retract=*/true, &retracted))) return rc;
@@ -987,7 +1007,7 @@ int hb200_set_spline(hb200_ctx* c, int order, int K, const double* knots) {
   HB_CUDA(cudaMemcpyAsync(c->knots[0].p, knots, 8 * sizeof(double) * K, cudaMemcpyHostToDevice, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
   if (reshape) { c->h_knot_const.assign(K, 0); c->bound = false; c->invalidate(); c->have_snapshot = false; int rc = update_fixed(c); if (rc) return rc; }
-  c->evaluated_J = false; c->system_built = false; c->mirror_valid = false; c->calib_valid = false;
+  c->evaluated_J = false; c->system_built = false; c->cov_built = false; c->mirror_valid = false; c->calib_valid = false;
   return 0;
 }
 
@@ -1019,7 +1039,7 @@ int hb200_set_bias_splines(hb200_ctx* c, int order, int Kg, const double* gyro, 
   HB_CUDA(cudaMemcpyAsync(c->ba[0].p, accel, 4 * sizeof(double) * Ka, cudaMemcpyHostToDevice, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
   if (reshape) { c->bound = false; c->invalidate(); c->have_snapshot = false; int rc = update_fixed(c); if (rc) return rc; }
-  c->evaluated_J = false; c->system_built = false; c->mirror_valid = false; c->calib_valid = false;
+  c->evaluated_J = false; c->system_built = false; c->cov_built = false; c->mirror_valid = false; c->calib_valid = false;
   return 0;
 }
 
@@ -1029,7 +1049,7 @@ int hb200_set_gravity(hb200_ctx* c, const double* g) {
   HB_CUDA(cudaMemcpyAsync(c->grav[0].p, g, 3 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
   c->have_gravity = true;
-  c->evaluated_J = false; c->system_built = false; c->mirror_valid = false; c->calib_valid = false;
+  c->evaluated_J = false; c->system_built = false; c->cov_built = false; c->mirror_valid = false; c->calib_valid = false;
   return 0;
 }
 
@@ -1044,7 +1064,7 @@ int hb200_set_cameras(hb200_ctx* c, int C, const double* cams) {
   calib_kernel<<<(C + 63) / 64, 64, 0, c->stream>>>(C, c->cams.p, c->cam_tab.p, nullptr, nullptr, 0);
   HB_LAUNCH(c, "calib_kernel");
   HB_CUDA(cudaStreamSynchronize(c->stream));
-  c->evaluated_J = false; c->system_built = false; c->mirror_valid = false; c->calib_valid = false;
+  c->evaluated_J = false; c->system_built = false; c->cov_built = false; c->mirror_valid = false; c->calib_valid = false;
   return 0;
 }
 
@@ -1057,7 +1077,7 @@ int hb200_set_imu(hb200_ctx* c, const double* imu) {
   HB_LAUNCH(c, "calib_kernel");
   HB_CUDA(cudaStreamSynchronize(c->stream));
   c->have_imu = true;
-  c->evaluated_J = false; c->system_built = false; c->mirror_valid = false; c->calib_valid = false;
+  c->evaluated_J = false; c->system_built = false; c->cov_built = false; c->mirror_valid = false; c->calib_valid = false;
   return 0;
 }
 
@@ -1069,7 +1089,7 @@ int hb200_set_landmarks(hb200_ctx* c, int L, const double* xyz) {
   for (int s = 0; s < 2; ++s) HB_CUDA(c->lms[s].ensure(3 * static_cast<size_t>(std::max(L, 1))));
   if (L) HB_CUDA(cudaMemcpyAsync(c->lms[0].p, xyz, 3 * sizeof(double) * L, cudaMemcpyHostToDevice, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
-  c->evaluated_J = false; c->system_built = false; c->mirror_valid = false; c->calib_valid = false;
+  c->evaluated_J = false; c->system_built = false; c->cov_built = false; c->mirror_valid = false; c->calib_valid = false;
   return 0;
 }
 
@@ -1080,7 +1100,7 @@ int hb200_set_constant(hb200_ctx* c, const unsigned char* knot_constant, int gra
   if (knot_constant) c->h_knot_const.assign(knot_constant, knot_constant + c->K);
   else c->h_knot_const.assign(c->K, 0);
   c->gravity_const = gravity_constant; c->bias_const = bias_constant;
-  c->system_built = false;
+  c->system_built = false; c->cov_built = false;
   return update_fixed(c);
 }
 
@@ -1094,7 +1114,7 @@ int hb200_set_reference_quirks(hb200_ctx* c, int quirks) {
     HB_LAUNCH(c, "calib_kernel");
     HB_CUDA(cudaStreamSynchronize(c->stream));
   }
-  c->evaluated_J = false; c->system_built = false; c->mirror_valid = false; c->calib_valid = false;
+  c->evaluated_J = false; c->system_built = false; c->cov_built = false; c->mirror_valid = false; c->calib_valid = false;
   return 0;
 }
 
@@ -1104,7 +1124,7 @@ int hb200_set_options(hb200_ctx* c, double huber_pixel, double imu_loss_scale, d
   HB_CUDA(cudaSetDevice(c->device));
   if (huber_pixel != c->huber || imu_loss_scale != c->imu_scale) c->graph_valid = false;  // baked into kernel arguments
   c->huber = huber_pixel; c->imu_scale = imu_loss_scale; c->radius0 = radius;
-  c->system_built = false; c->evaluated_J = false;
+  c->system_built = false; c->cov_built = false; c->evaluated_J = false;
   return reset_solver_state(c);
 }
 
@@ -1153,7 +1173,7 @@ int hb200_set_bearing_loss(hb200_ctx* c, double huber_bearing) {
   if (!(huber_bearing > 0)) return fail(-1, "options must be positive");
   if (huber_bearing != c->huber_bearing) c->graph_valid = false;
   c->huber_bearing = huber_bearing;
-  c->system_built = false; c->evaluated_J = false;
+  c->system_built = false; c->cov_built = false; c->evaluated_J = false;
   return 0;
 }
 
@@ -1477,7 +1497,7 @@ int hb200_evaluate(hb200_ctx* c, int flags) {
   rc = enqueue_evaluate(c, J, sel);
   if (rc) return rc;
   c->evaluated_J = J && sel == 0;   // a trial-state sweep overwrites the residual / Jacobian buffers
-  c->mirror_valid = false; c->calib_valid = false; c->system_built = false;
+  c->mirror_valid = false; c->calib_valid = false; c->system_built = false; c->cov_built = false;
   return 0;
 }
 
@@ -1741,7 +1761,7 @@ int hb200_build_system(hb200_ctx* c) {
   // assembled as enqueue_iteration does: the Jacobian sweep at the current state runs again with the pixel J^T J
   // accumulated by the factor kernels (it rewrites the same residuals and Jacobians), then the rest of the system
   if ((rc = enqueue_evaluate(c, true, 0, /*accumulate=*/true, /*keep_fork=*/true, /*clear_system=*/true))) return rc;
-  if ((rc = enqueue_build(c))) return rc;
+  if ((rc = enqueue_build(c, c->st.p))) return rc;
   if ((rc = enqueue_reduce_system(c))) return rc;
   c->system_built = true;
   return 0;
@@ -1770,6 +1790,164 @@ int hb200_get_delta(hb200_ctx* c, double* dp, double* dl) {
   if (dp) HB_CUDA(cudaMemcpyAsync(dp, c->dp.p, sizeof(double) * c->n, cudaMemcpyDeviceToHost, c->stream));
   if (dl && c->L) HB_CUDA(cudaMemcpyAsync(dl, c->dl.p, sizeof(double) * 3 * c->L, cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
+  return 0;
+}
+
+// ---- marginal covariances (hb200_cov.cuh) ------------------------------------------------------------------------
+namespace {
+int cov_check(hb200_ctx* c) {
+  if (!c) return fail(-1, "null context");
+  if (c->multi()) return fail(-3, "covariance: not supported with a communicator or all-reduce callback attached (single GPU only)");
+  return 0;
+}
+void cov_info(hb200_ctx* c, hb200_covariance_info* info) {
+  info->degenerate_landmarks = c->cov_degenerate; info->unobserved_landmarks = c->cov_unobserved;
+  info->K = c->cov_valid ? c->cov_lay.K : 0; info->beta = c->cov_valid ? c->cov_lay.beta : 0;
+  info->m = c->cov_valid ? c->cov_lay.m : 0; info->L = c->cov_valid ? c->cov_L : 0;
+}
+}  // namespace
+
+int hb200_build_covariance(hb200_ctx* c) {
+  int rc = cov_check(c);
+  if (rc) return rc;
+  if ((rc = check_ready(c))) return rc;
+  HB_CUDA(cudaSetDevice(c->device));
+  const size_t smem = cov_smem_doubles(c->beta, c->lay.m) * sizeof(double);
+  if (smem > 220 * 1024)
+    return fail(-6, "covariance: a window of %d block columns and %d arrow rows needs %zu B of shared memory", c->beta + 1, c->lay.m, smem);
+  c->cov_built = false;
+  SolverState s{};
+  s.radius = INFINITY;   // mu = 1 / radius = 0 in the Schur kernels
+  HB_CUDA(c->cov_st.ensure(1));
+  HB_CUDA(cudaMemcpyAsync(c->cov_st.p, &s, sizeof(s), cudaMemcpyHostToDevice, c->stream));
+  // the Jacobian sweep at the current state with the pixel J^T J accumulated, then the rest of the system (undamped)
+  if ((rc = enqueue_evaluate(c, true, 0, /*accumulate=*/true, /*keep_fork=*/true, /*clear_system=*/true))) return rc;
+  if ((rc = enqueue_build(c, c->cov_st.p))) return rc;
+  // the linearisation point of this build, for the interpolated covariance
+  HB_CUDA(c->cov_knots_next.ensure(8 * static_cast<size_t>(c->K)));
+  HB_CUDA(c->cov_tab_next.ensure(static_cast<size_t>(kTabStride) * c->K));
+  HB_CUDA(cudaMemcpyAsync(c->cov_knots_next.p, c->knots[0].p, sizeof(double) * 8 * c->K, cudaMemcpyDeviceToDevice, c->stream));
+  HB_CUDA(cudaMemcpyAsync(c->cov_tab_next.p, c->tab[0].p, sizeof(double) * kTabStride * c->K, cudaMemcpyDeviceToDevice, c->stream));
+  int counts[2] = {0, c->L};
+  if (c->Nv && c->L) {
+    HB_CUDA(c->cov_counts.ensure(2));
+    cov_landmark_flags_kernel<<<1, kCovFlagThreads, 0, c->stream>>>(c->L, c->lm_off.p, c->Vchol.p, c->Dl.p, c->cov_counts.p);
+    HB_LAUNCH(c, "cov_landmark_flags_kernel");
+    HB_CUDA(cudaMemcpyAsync(counts, c->cov_counts.p, sizeof(counts), cudaMemcpyDeviceToHost, c->stream));
+  }
+  HB_CUDA(cudaStreamSynchronize(c->stream));
+  c->cov_degenerate = counts[0]; c->cov_unobserved = counts[1];
+  c->cov_lay_next = c->lay; c->cov_basis_next = c->basis; c->cov_L_next = c->L;
+  c->cov_k_next = c->k; c->cov_Nv_next = c->Nv; c->cov_max_rows_next = c->max_rows;
+  // the factor outputs are those of an evaluation at the current state; the packed buffer is not what hb200_solve expects
+  c->evaluated_J = true; c->system_built = false; c->cov_built = false; c->mirror_valid = false; c->calib_valid = false;
+  c->cov_built = true;
+  c->cov_at = c->launches;
+  return 0;
+}
+
+int hb200_compute_covariance(hb200_ctx* c, hb200_covariance_info* info) {
+  int rc = cov_check(c);
+  if (rc) return rc;
+  if (!info) return fail(-1, "null info");
+  // every setter that changes shapes, constants or the state clears cov_built; any other launch since the build (an
+  // evaluation, an iteration, a slide) rewrote the factor outputs or the packed buffer the compute reads
+  if (!c->cov_built || c->cov_at != c->launches || c->L != c->cov_L_next || c->k != c->cov_k_next || c->Nv != c->cov_Nv_next ||
+      c->max_rows != c->cov_max_rows_next || c->lay.total != c->cov_lay_next.total || c->lay.beta != c->cov_lay_next.beta)
+    return fail(-2, "call hb200_build_covariance first (the window was evaluated, iterated or changed since)");
+  HB_CUDA(cudaSetDevice(c->device));
+  info->status = 0; info->bad_dof = -1; info->min_pivot_ratio = 0.0;
+  if (c->cov_degenerate) {
+    cov_info(c, info);
+    info->status = 2;
+    return fail(HB200_COV_DEGENERATE_LANDMARKS, "covariance: %d landmark(s) with a rank-deficient V_l (observed by too few factors)", c->cov_degenerate);
+  }
+  const SysLayout lay = c->cov_lay_next;
+  const size_t smem = cov_smem_doubles(lay.beta, lay.m) * sizeof(double);
+  HB_CUDA(c->cov_ws.ensure(static_cast<size_t>(cov_workspace_doubles(lay))));
+  HB_CUDA(c->cov_packed_next.ensure(static_cast<size_t>(cov_packed_doubles(lay))));
+  const int L = c->cov_L_next, k = c->cov_k_next, max_rows = c->cov_max_rows_next;   // (the build's shapes)
+  HB_CUDA(c->cov_lm_next.ensure(9 * static_cast<size_t>(std::max(L, 1))));
+  HB_CUDA(c->cov_status.ensure(1));
+  HB_CUDA(cudaFuncSetAttribute(cov_selinv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+  cov_selinv_kernel<<<1, kCovThreads, smem, c->stream>>>(c->sys.p, lay, c->fixed.p, c->cov_ws.p, c->cov_packed_next.p, c->cov_status.p);
+  HB_LAUNCH(c, "cov_selinv_kernel");
+  if (L && c->cov_Nv_next) {
+    const int blocks = (L + kLmWarps - 1) / kLmWarps;
+    const size_t lsmem = static_cast<size_t>(kLmWarps) * 3 * max_rows * sizeof(double);
+    if (k == 4)
+      cov_landmark_kernel<4><<<blocks, kLmWarps * 32, lsmem, c->stream>>>(L, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p, c->Vchol.p,
+                                                                         c->cov_packed_next.p, lay, c->cov_status.p, c->cov_lm_next.p, max_rows);
+    else
+      cov_landmark_kernel<6><<<blocks, kLmWarps * 32, lsmem, c->stream>>>(L, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p, c->Vchol.p,
+                                                                         c->cov_packed_next.p, lay, c->cov_status.p, c->cov_lm_next.p, max_rows);
+    HB_LAUNCH(c, "cov_landmark_kernel");
+  } else if (L) {
+    HB_CUDA(cudaMemsetAsync(c->cov_lm_next.p, 0, sizeof(double) * 9 * L, c->stream));
+  }
+  CovStatus st{};
+  HB_CUDA(cudaMemcpyAsync(&st, c->cov_status.p, sizeof(st), cudaMemcpyDeviceToHost, c->stream));
+  HB_CUDA(cudaStreamSynchronize(c->stream));
+  c->cov_at = c->launches;
+  info->bad_dof = st.bad_dof;
+  info->min_pivot_ratio = std::isfinite(st.min_pivot) ? st.min_pivot : 0.0;
+  if (st.status) {
+    cov_info(c, info);
+    info->status = 1;
+    return fail(HB200_COV_NOT_POSITIVE_DEFINITE, "covariance: the reduced system is not positive definite (pivot %.3e of dof %d, threshold %.0e)",
+                st.min_pivot, st.bad_dof, kCovMinPivot);
+  }
+  // commit: results, and the linearisation point they belong to
+  c->cov_packed.swap(c->cov_packed_next);
+  c->cov_lm.swap(c->cov_lm_next);
+  HB_CUDA(c->cov_knots.ensure(8 * static_cast<size_t>(lay.K)));
+  HB_CUDA(c->cov_tab.ensure(static_cast<size_t>(kTabStride) * lay.K));
+  HB_CUDA(cudaMemcpyAsync(c->cov_knots.p, c->cov_knots_next.p, sizeof(double) * 8 * lay.K, cudaMemcpyDeviceToDevice, c->stream));
+  HB_CUDA(cudaMemcpyAsync(c->cov_tab.p, c->cov_tab_next.p, sizeof(double) * kTabStride * lay.K, cudaMemcpyDeviceToDevice, c->stream));
+  HB_CUDA(cudaStreamSynchronize(c->stream));
+  c->cov_lay = lay; c->cov_basis = c->cov_basis_next; c->cov_L = c->cov_L_next;
+  c->cov_valid = true;
+  cov_info(c, info);
+  return 0;
+}
+
+int hb200_get_covariance(hb200_ctx* c, double* packed, double* landmark) {
+  int rc = cov_check(c);
+  if (rc) return rc;
+  if (!c->cov_valid) return fail(-2, "no covariance computed (hb200_compute_covariance has not succeeded)");
+  HB_CUDA(cudaSetDevice(c->device));
+  if (packed) HB_CUDA(cudaMemcpyAsync(packed, c->cov_packed.p, sizeof(double) * cov_packed_doubles(c->cov_lay), cudaMemcpyDeviceToHost, c->stream));
+  if (landmark && c->cov_L) HB_CUDA(cudaMemcpyAsync(landmark, c->cov_lm.p, sizeof(double) * 9 * c->cov_L, cudaMemcpyDeviceToHost, c->stream));
+  HB_CUDA(cudaStreamSynchronize(c->stream));
+  return 0;
+}
+
+int hb200_interpolate_covariance(hb200_ctx* c, int n, const double* stamps, double* cov, int* num_invalid) {
+  int rc = cov_check(c);
+  if (rc) return rc;
+  if (n < 0 || (n > 0 && (!stamps || !cov))) return fail(-1, "invalid argument");
+  if (!c->cov_valid) return fail(-2, "no covariance computed (hb200_compute_covariance has not succeeded)");
+  HB_CUDA(cudaSetDevice(c->device));
+  if (num_invalid) *num_invalid = 0;
+  if (n == 0) return 0;
+  const bool stamp = c->cov_built && c->cov_at == c->launches;   // (reads nothing a compute needs)
+  DevBuf<double>& d_t = c->cov_t;
+  DevBuf<double>& d_o = c->cov_o;
+  DevBuf<int>& d_bad = c->cov_bad;
+  HB_CUDA(d_t.ensure(n)); HB_CUDA(d_o.ensure(36 * static_cast<size_t>(n))); HB_CUDA(d_bad.ensure(n));
+  HB_CUDA(cudaMemcpyAsync(d_t.p, stamps, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
+  const SysLayout& lay = c->cov_lay;
+  if (c->cov_basis.k == 4)
+    cov_interpolate_kernel<4><<<(n + 127) / 128, 128, 0, c->stream>>>(n, d_t.p, c->cov_knots.p, c->cov_tab.p, lay.K, c->cov_basis, c->cov_packed.p, lay, d_o.p, d_bad.p);
+  else
+    cov_interpolate_kernel<6><<<(n + 127) / 128, 128, 0, c->stream>>>(n, d_t.p, c->cov_knots.p, c->cov_tab.p, lay.K, c->cov_basis, c->cov_packed.p, lay, d_o.p, d_bad.p);
+  HB_LAUNCH(c, "cov_interpolate_kernel");
+  std::vector<int> bad(n);
+  HB_CUDA(cudaMemcpyAsync(cov, d_o.p, sizeof(double) * 36 * n, cudaMemcpyDeviceToHost, c->stream));
+  HB_CUDA(cudaMemcpyAsync(bad.data(), d_bad.p, sizeof(int) * n, cudaMemcpyDeviceToHost, c->stream));
+  HB_CUDA(cudaStreamSynchronize(c->stream));
+  if (num_invalid) *num_invalid = std::accumulate(bad.begin(), bad.end(), 0);
+  if (stamp) c->cov_at = c->launches;
   return 0;
 }
 
@@ -1837,7 +2015,7 @@ int iterate_enqueue(hb200_ctx* c, int iterations) {
       if (c->nccl) c->comm_warm = true;
     }
   }
-  c->evaluated_J = false; c->system_built = false; c->mirror_valid = false; c->calib_valid = false;
+  c->evaluated_J = false; c->system_built = false; c->cov_built = false; c->mirror_valid = false; c->calib_valid = false;
   if (!c->term_enabled) c->iter_total += iterations;   // (with the termination tests on, the device counter is authoritative: pick_records)
   return 0;
 }
@@ -2090,7 +2268,7 @@ int hb200_profile_iteration(hb200_ctx* c, int reps, int max_entries, char* names
     ms[n_out] = acc[i] / reps;
   }
   *count = n_out;
-  c->evaluated_J = false; c->system_built = false; c->mirror_valid = false; c->calib_valid = false;
+  c->evaluated_J = false; c->system_built = false; c->cov_built = false; c->mirror_valid = false; c->calib_valid = false;
   return 0;
 }
 
@@ -2157,7 +2335,7 @@ int hb200_restore(hb200_ctx* c) {
   if (c->L) HB_CUDA(cudaMemcpyAsync(c->lms[0].p, c->snap_lms.p, sizeof(double) * 3 * c->L, cudaMemcpyDeviceToDevice, c->stream));
   HB_CUDA(cudaMemcpyAsync(c->st.p, c->snap_st.p, sizeof(SolverState), cudaMemcpyDeviceToDevice, c->stream));
   c->iter_total = c->snap_iter_total;
-  c->evaluated_J = false; c->system_built = false; c->mirror_valid = false; c->calib_valid = false;
+  c->evaluated_J = false; c->system_built = false; c->cov_built = false; c->mirror_valid = false; c->calib_valid = false;
   return 0;
 }
 

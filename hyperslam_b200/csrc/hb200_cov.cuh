@@ -1,0 +1,499 @@
+// Marginal covariances of the window's estimates (hb200_build_covariance / hb200_compute_covariance), sm_90a, FP64.
+//
+// Sigma = (J^T W J)^-1 over the non-constant dofs at the current state, the model of ceres::Covariance with its defaults.
+// The build assembles the undamped reduced system S (landmark Schur complement with mu = 0) into the packed band-only
+// buffer; the kernels here then produce, from S and the landmark factors of that build:
+//   cov_selinv_kernel     the entries of S^-1 on the block band, the arrow and the corner (selected inversion);
+//   cov_landmark_kernel   the 3 x 3 marginal of every landmark, Sigma_ll = L^-T (I + Y^T Sigma_pp Y) L^-1;
+//   cov_interpolate_kernel the 6 x 6 covariance of the interpolated pose at arbitrary stamps, J(t) Sigma J(t)^T.
+// All three are deterministic: no atomics, every sum in a fixed order.
+#pragma once
+#include "hb200_solve.cuh"
+
+namespace hb {
+
+// Pivot threshold of the covariance factorisations.  The reduced system is factored after the symmetric diagonal
+// equilibration D S D, D = diag(S)^-1/2, so a pivot is its own ratio to the diagonal; a landmark pivot is compared with
+// d_j = clamp(diag V_l).  Ceres' Covariance::Options::min_reciprocal_condition_number (1e-14) is too close to rounding
+// here: a system that is singular in exact arithmetic but assembled in FP64 keeps an equilibrated pivot of order n eps
+// (4e-15 at n = 86 in tests/test_covref.py, ~7e-13 = n eps at K = 500), so the threshold sits at 1e-10, 150 x above
+// that at K = 500 and far below the smallest pivot of the positive definite windows the tests run.
+constexpr double kCovMinPivot = 1e-10;
+constexpr int kCovThreads = 512;
+constexpr int kCovFlagThreads = 256;
+
+struct CovStatus {
+  int status;        // 0 ok, 1 a pivot of the reduced system failed
+  int bad_dof;       // first reduced-system dof whose pivot failed, else -1
+  double min_pivot;  // smallest pivot of the equilibrated factor (the failing one when status = 1)
+};
+
+// Sliding window of the selected inversion: beta + 1 block slots of 6 rows (block b in slot b mod (beta + 1)) and the
+// m arrow rows, stored as a full symmetric square with an odd leading dimension.
+__host__ __device__ inline int cov_window(int beta, int m) { return 6 * (beta + 1) + m; }
+__host__ __device__ inline int cov_ld(int w) { return w | 1; }
+__host__ __device__ inline size_t cov_smem_doubles(int beta, int m) {
+  const size_t w = cov_window(beta, m);
+  return w * cov_ld(static_cast<int>(w)) + 3 * 6 * w + 3 * 36;
+}
+// global workspace: factor L in the packed P | A | C layout, D (n), L_C^-1 (m x m)
+__host__ __device__ inline long long cov_packed_doubles(const SysLayout& L) { return L.oC + static_cast<long long>(L.m) * L.m; }
+__host__ __device__ inline long long cov_workspace_doubles(const SysLayout& L) {
+  return cov_packed_doubles(L) + L.n + static_cast<long long>(L.m) * L.m;
+}
+
+// Landmarks whose undamped V_l is not numerically positive definite (a pivot of the Schur kernels' factor at or below
+// kCovMinPivot d_j; NaN-safe) and landmarks without observations.  One CTA, counts in counts[0] / counts[1].
+__global__ void __launch_bounds__(kCovFlagThreads) cov_landmark_flags_kernel(int L, const int* __restrict__ lm_off, const double* __restrict__ Vchol,
+                                                                             const double* __restrict__ Dl, int* __restrict__ counts) {
+  int degenerate = 0, unobserved = 0;
+  for (int l = threadIdx.x; l < L; l += kCovFlagThreads) {
+    if (lm_off[l + 1] <= lm_off[l]) { ++unobserved; continue; }
+    const double* F = Vchol + 9 * static_cast<size_t>(l);   // packed (1/L00, L10, 1/L11, L20, L21, 1/L22)
+    const double* d = Dl + 3 * static_cast<size_t>(l);
+    const double f[3] = {F[0], F[2], F[5]};
+    bool bad = false;
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+      const double pivot = 1.0 / (f[j] * f[j]);
+      if (!(pivot > kCovMinPivot * d[j])) bad = true;
+    }
+    degenerate += bad ? 1 : 0;
+  }
+  degenerate = __reduce_add_sync(0xffffffffu, degenerate);
+  unobserved = __reduce_add_sync(0xffffffffu, unobserved);
+  __shared__ int s[2][kCovFlagThreads / 32];
+  if ((threadIdx.x & 31) == 0) { s[0][threadIdx.x >> 5] = degenerate; s[1][threadIdx.x >> 5] = unobserved; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int a = 0, b = 0;
+    for (int w = 0; w < kCovFlagThreads / 32; ++w) { a += s[0][w]; b += s[1][w]; }
+    counts[0] = a; counts[1] = b;
+  }
+}
+
+// Entry (i, j) of A_hat = D S D with the constant-dof mask (identity rows / columns), read from the lower triangle.
+HB_DI double cov_ahat(const double* __restrict__ sys, const SysLayout& lay, const unsigned char* __restrict__ fixed, const double* __restrict__ d,
+                      int i, int j) {
+  if (fixed[i] || fixed[j]) return i == j ? 1.0 : 0.0;
+  const int hi = max(i, j), lo = min(i, j);
+  if (hi < lay.np && hi - 6 * (lo / 6) >= lay.h) return 0.0;
+  return d[i] * sys[sys_index(lay, hi, lo)] * d[j];
+}
+
+// Global dof of window row p while the window holds blocks lo .. lo + beta; -1 for a slot whose block is past the window.
+HB_DI int cov_gdof(int p, int lo, int nb, int wp, int K, int np) {
+  if (p >= wp) return np + (p - wp);
+  const int s = p / 6;
+  const int b = lo + ((s - lo % nb) % nb + nb) % nb;
+  return b < K ? 6 * b + (p - 6 * s) : -1;
+}
+
+// 6 x 6 lower-triangular inverse (row-major)
+HB_DI void cov_tri_inv6(const double* L, double* Li) {
+  for (int c = 0; c < 6; ++c) {
+    for (int i = 0; i < c; ++i) Li[i * 6 + c] = 0.0;
+    Li[c * 6 + c] = 1.0 / L[c * 6 + c];
+    for (int i = c + 1; i < 6; ++i) {
+      double s = 0.0;
+      for (int l = c; l < i; ++l) s += L[i * 6 + l] * Li[l * 6 + c];
+      Li[i * 6 + c] = -s / L[i * 6 + i];
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Band + arrow Cholesky of A_hat and its selected inverse, one CTA.
+//   Forward: right-looking blocked Cholesky in natural order over 6-wide block columns; the window holds the trailing
+//   blocks j .. j+beta and the arrow.  Per column: factor the diagonal block (pivots checked against kCovMinPivot),
+//   L_Sj = A_Sj L_jj^-T, trailing update of the window, write column j of L to Lf (packed layout), then block j+beta+1
+//   enters the freed slot (it has no fill from columns <= j: it is more than beta blocks from them).  Finally the corner.
+//   Backward (Takahashi): Z_CC = L_C^-T L_C^-1; for j = K-1 .. 0, with S = {j+1 .. j+beta} u arrow,
+//   X = L_Sj L_jj^-1, Z_Sj = -Z_SS X, Z_jj = L_jj^-T L_jj^-1 - X^T Z_Sj.  The window now holds Z over blocks j .. j+beta
+//   and the arrow; every Z entry it needs is within the band.
+//   Output: Sigma = D Z D in the packed P | A | C layout (diagonal blocks and corner full, padding rows 0), constant dofs 0.
+// Dynamic shared memory: cov_smem_doubles(beta, m) doubles.
+// ---------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kCovThreads) cov_selinv_kernel(const double* __restrict__ sys, SysLayout lay, const unsigned char* __restrict__ fixed,
+                                                                 double* __restrict__ ws, double* __restrict__ out, CovStatus* __restrict__ status) {
+  extern __shared__ double s_cov[];
+  const int K = lay.K, m = lay.m, np = lay.np, n = lay.n, h = lay.h;
+  const int nb = lay.beta + 1, wp = 6 * nb, w = wp + m, ld = cov_ld(w);
+  double* Wm = s_cov;                               // [w][ld]
+  double* Lc = Wm + static_cast<size_t>(w) * ld;    // [w][6]  column j of L (rows of the window)
+  double* Xc = Lc + 6 * w;                          // [w][6]
+  double* Zc = Xc + 6 * w;                          // [w][6]
+  double* Ljj = Zc + 6 * w;                         // [36]
+  double* Li = Ljj + 36;                            // [36]
+  double* Zjj = Li + 36;                            // [36]
+  double* Lf = ws;                                  // factor, packed layout
+  double* dv = ws + cov_packed_doubles(lay);        // D
+  double* Yc = dv + n;                              // L_C^-1 [m][m]
+  __shared__ int s_fail;
+  __shared__ double s_minpiv, s_failpiv;
+  const int tid = threadIdx.x;
+
+  for (int i = tid; i < n; i += kCovThreads) {
+    const double s = sys[sys_index(lay, i, i)];
+    dv[i] = (fixed[i] || !(s > 0.0) || !isfinite(s)) ? 1.0 : 1.0 / sqrt(s);   // a non-positive diagonal fails at its pivot
+  }
+  if (tid == 0) { s_fail = -1; s_minpiv = INFINITY; s_failpiv = 0.0; }
+  __syncthreads();
+  for (int e = tid; e < w * w; e += kCovThreads) {
+    const int p = e / w, q = e - p * w;
+    const int gi = cov_gdof(p, 0, nb, wp, K, np), gj = cov_gdof(q, 0, nb, wp, K, np);
+    Wm[p * ld + q] = (gi < 0 || gj < 0) ? 0.0 : cov_ahat(sys, lay, fixed, dv, gi, gj);
+  }
+
+  // ---- forward sweep ----
+  for (int j = 0; j < K; ++j) {
+    const int c0 = 6 * (j % nb);
+    __syncthreads();
+    if (tid == 0) {
+      double L[36];
+      for (int i = 0; i < 36; ++i) L[i] = 0.0;
+      for (int k = 0; k < 6 && s_fail < 0; ++k) {
+        double piv = Wm[(c0 + k) * ld + c0 + k];
+        for (int l = 0; l < k; ++l) piv -= L[k * 6 + l] * L[k * 6 + l];
+        if (!(piv > kCovMinPivot)) { s_fail = 6 * j + k; s_failpiv = piv; break; }
+        s_minpiv = fmin(s_minpiv, piv);
+        const double lkk = sqrt(piv);
+        L[k * 6 + k] = lkk;
+        for (int i = k + 1; i < 6; ++i) {
+          double s = Wm[(c0 + i) * ld + c0 + k];
+          for (int l = 0; l < k; ++l) s -= L[i * 6 + l] * L[k * 6 + l];
+          L[i * 6 + k] = s / lkk;
+        }
+      }
+      if (s_fail < 0) {
+        for (int i = 0; i < 36; ++i) Ljj[i] = L[i];
+        cov_tri_inv6(L, Li);
+      }
+    }
+    __syncthreads();
+    if (s_fail >= 0) break;
+    // L_pj = A_pj L_jj^-T (rows of the diagonal block: L_jj itself)
+    for (int e = tid; e < 6 * w; e += kCovThreads) {
+      const int p = e / 6, a = e - 6 * p;
+      double v = 0.0;
+      if (p >= c0 && p < c0 + 6) v = Ljj[(p - c0) * 6 + a];
+      else for (int b = 0; b <= a; ++b) v += Li[a * 6 + b] * Wm[p * ld + c0 + b];
+      Lc[e] = v;
+    }
+    __syncthreads();
+    for (int e = tid; e < 6 * w; e += kCovThreads) {
+      const int p = e / 6, a = e - 6 * p;
+      const int gi = cov_gdof(p, j, nb, wp, K, np);
+      if (gi < 0) continue;
+      if (gi < np) Lf[(static_cast<size_t>(j) * h + (gi - 6 * j)) * 6 + a] = Lc[e];
+      else Lf[lay.oA + static_cast<size_t>(gi - np) * np + 6 * j + a] = Lc[e];
+    }
+    for (int e = tid; e < w * w; e += kCovThreads) {
+      const int p = e / w, q = e - p * w;
+      if ((p >= c0 && p < c0 + 6) || (q >= c0 && q < c0 + 6)) continue;
+      const double* lp = Lc + 6 * p;
+      const double* lq = Lc + 6 * q;
+      double s = lp[0] * lq[0];
+#pragma unroll
+      for (int a = 1; a < 6; ++a) s += lp[a] * lq[a];
+      Wm[p * ld + q] -= s;
+    }
+    __syncthreads();
+    // block j + beta + 1 enters slot j % nb (zero past the window)
+    const int nbk = j + nb;
+    for (int e = tid; e < 6 * w; e += kCovThreads) {
+      const int a = e / w, q = e - a * w;
+      const bool in_slot = q >= c0 && q < c0 + 6;
+      double v = 0.0;
+      if (nbk < K) {
+        const int gj = in_slot ? 6 * nbk + (q - c0) : cov_gdof(q, j + 1, nb, wp, K, np);
+        if (gj >= 0) v = cov_ahat(sys, lay, fixed, dv, 6 * nbk + a, gj);
+      }
+      Wm[(c0 + a) * ld + q] = v;
+      if (!in_slot) Wm[q * ld + c0 + a] = v;
+    }
+  }
+  __syncthreads();
+
+  // ---- corner: right-looking Cholesky in place (lower triangle) ----
+  for (int k = 0; k < m && s_fail < 0; ++k) {
+    const int kk = wp + k;
+    if (tid == 0) {
+      const double piv = Wm[kk * ld + kk];
+      if (!(piv > kCovMinPivot)) { s_fail = np + k; s_failpiv = piv; }
+      else { s_minpiv = fmin(s_minpiv, piv); Wm[kk * ld + kk] = sqrt(piv); }
+    }
+    __syncthreads();
+    if (s_fail >= 0) break;
+    const double lkk = Wm[kk * ld + kk];
+    for (int i = kk + 1 + tid; i < w; i += kCovThreads) Wm[i * ld + kk] /= lkk;
+    __syncthreads();
+    const int r = m - k - 1;
+    for (int e = tid; e < r * r; e += kCovThreads) {
+      const int i = kk + 1 + e / r, l = kk + 1 + e % r;
+      if (l <= i) Wm[i * ld + l] -= Wm[i * ld + kk] * Wm[l * ld + kk];
+    }
+    __syncthreads();
+  }
+  if (s_fail >= 0) {
+    if (tid == 0) { status->status = 1; status->bad_dof = s_fail; status->min_pivot = s_failpiv; }
+    return;
+  }
+  // L_C^-1, one column per thread
+  for (int t = tid; t < m; t += kCovThreads) {
+    for (int i = 0; i < t; ++i) Yc[i * m + t] = 0.0;
+    for (int i = t; i < m; ++i) {
+      double s = (i == t) ? 1.0 : 0.0;
+      for (int l = t; l < i; ++l) s -= Wm[(wp + i) * ld + wp + l] * Yc[l * m + t];
+      Yc[i * m + t] = s / Wm[(wp + i) * ld + wp + i];
+    }
+  }
+  __syncthreads();
+  // the window becomes Z: corner Z_CC = L_C^-T L_C^-1, pose slots 0 (blocks past the window)
+  for (int e = tid; e < w * w; e += kCovThreads) {
+    const int p = e / w, q = e - p * w;
+    double v = 0.0;
+    if (p >= wp && q >= wp) {
+      const int a = p - wp, b = q - wp;
+      for (int k = max(a, b); k < m; ++k) v += Yc[k * m + a] * Yc[k * m + b];
+      const int gi = np + a, gj = np + b;
+      out[lay.oC + static_cast<size_t>(a) * m + b] = (fixed[gi] || fixed[gj]) ? 0.0 : dv[gi] * v * dv[gj];
+    }
+    Wm[p * ld + q] = v;
+  }
+
+  // ---- backward sweep (Takahashi) ----
+  for (int j = K - 1; j >= 0; --j) {
+    const int c0 = 6 * (j % nb);
+    __syncthreads();
+    for (int e = tid; e < 6 * w; e += kCovThreads) {
+      const int p = e / 6, a = e - 6 * p;
+      const int gi = cov_gdof(p, j, nb, wp, K, np);
+      double v = 0.0;
+      if (gi >= 0) v = gi < np ? Lf[(static_cast<size_t>(j) * h + (gi - 6 * j)) * 6 + a] : Lf[lay.oA + static_cast<size_t>(gi - np) * np + 6 * j + a];
+      if (p >= c0 && p < c0 + 6) { Ljj[(p - c0) * 6 + a] = v; v = 0.0; }
+      Lc[e] = v;
+    }
+    __syncthreads();
+    if (tid == 0) cov_tri_inv6(Ljj, Li);
+    __syncthreads();
+    // X = L_Sj L_jj^-1
+    for (int e = tid; e < 6 * w; e += kCovThreads) {
+      const int p = e / 6, a = e - 6 * p;
+      double v = 0.0;
+      for (int b = a; b < 6; ++b) v += Lc[6 * p + b] * Li[b * 6 + a];
+      Xc[e] = v;
+    }
+    __syncthreads();
+    // Z_Sj = -Z_SS X (the slot of j holds stale entries; its rows of X are 0)
+    for (int e = tid; e < 6 * w; e += kCovThreads) {
+      const int p = e / 6, a = e - 6 * p;
+      double v = 0.0;
+      if (!(p >= c0 && p < c0 + 6)) {
+        const double* zr = Wm + static_cast<size_t>(p) * ld;
+        for (int q = 0; q < w; ++q) v += zr[q] * Xc[6 * q + a];
+        v = -v;
+      }
+      Zc[e] = v;
+    }
+    __syncthreads();
+    // Z_jj = L_jj^-T L_jj^-1 - X^T Z_Sj (lower triangle computed, mirrored)
+    if (tid < 36) {
+      const int a = tid / 6, b = tid - 6 * a;
+      if (b <= a) {
+        double s = 0.0, t = 0.0;
+        for (int k = a; k < 6; ++k) s += Li[k * 6 + a] * Li[k * 6 + b];
+        for (int p = 0; p < w; ++p) t += Xc[6 * p + a] * Zc[6 * p + b];
+        Zjj[a * 6 + b] = s - t;
+        Zjj[b * 6 + a] = s - t;
+      }
+    }
+    __syncthreads();
+    // slot of j <- column j of Z; column j of Sigma to the output
+    for (int e = tid; e < 6 * w; e += kCovThreads) {
+      const int p = e / 6, a = e - 6 * p;
+      const bool in_slot = p >= c0 && p < c0 + 6;
+      const double v = in_slot ? Zjj[(p - c0) * 6 + a] : Zc[e];
+      Wm[p * ld + c0 + a] = v;
+      if (!in_slot) Wm[(c0 + a) * ld + p] = v;
+      const int gj = 6 * j + a;
+      const int gi = cov_gdof(p, j, nb, wp, K, np);
+      const double sv = (gi < 0 || fixed[gi] || fixed[gj]) ? 0.0 : dv[gi] * v * dv[gj];
+      if (p >= wp) out[lay.oA + static_cast<size_t>(p - wp) * np + gj] = sv;
+      else {
+        const int off = ((p / 6 - j % nb) % nb + nb) % nb;   // block offset from j (rows past the last pose dof: padding)
+        out[(static_cast<size_t>(j) * h + 6 * off + p % 6) * 6 + a] = sv;
+      }
+    }
+  }
+  __syncthreads();
+  if (tid == 0) { status->status = 0; status->bad_dof = -1; status->min_pivot = s_minpiv; }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Landmark marginals, one warp per landmark (the observation loop of lm_backsub_kernel / schur_group_kernel):
+//   W = sum w Jp^T Jl over the landmark's control-point span, Y = W L^-T with the build's undamped factor V_l = L L^T,
+//   M = Y^T Sigma_pp Y (Sigma_pp from the selected inverse: the span lies inside the band),
+//   Sigma_ll = L^-T (I + M) L^-1 = V^-1 + V^-1 W^T Sigma_pp W V^-1.
+// Unobserved landmarks get a zero block.  Nothing runs when the selected inversion failed.
+// Dynamic shared memory: kLmWarps * 3 * max_rows doubles.
+// ---------------------------------------------------------------------------------------------
+template <int K>
+__global__ void __launch_bounds__(kLmWarps * 32) cov_landmark_kernel(int L, const int* __restrict__ lm_off, const int* __restrict__ lm_obs,
+                                                                     const int4* __restrict__ idx, const double* __restrict__ Jp,
+                                                                     const double* __restrict__ Jl, const double* __restrict__ wv,
+                                                                     const double* __restrict__ Vchol, const double* __restrict__ cov, SysLayout lay,
+                                                                     const CovStatus* __restrict__ status, double* __restrict__ out, int max_rows) {
+  constexpr int NB = 6 * K;
+  extern __shared__ double s_lw[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int l = blockIdx.x * kLmWarps + warp;
+  if (status->status != 0 || l >= L) return;
+  double* Y = s_lw + static_cast<size_t>(warp) * 3 * max_rows;
+  double* o = out + 9 * static_cast<size_t>(l);
+  const int o_lo = lm_off[l], o_hi = lm_off[l + 1];
+  if (o_lo >= o_hi) {
+    if (lane < 9) o[lane] = 0.0;
+    return;
+  }
+  const int cp_lo = idx[lm_obs[o_lo]].x, cp_hi = idx[lm_obs[o_hi - 1]].x + K;
+  const int rows = 6 * (cp_hi - cp_lo);
+  for (int e = lane; e < 3 * rows; e += 32) Y[e] = 0.0;
+  __syncwarp();
+  for (int ob = o_lo; ob < o_hi; ++ob) {
+    const int f = lm_obs[ob];
+    const double wgt = wv[f];
+    const int b0 = 6 * (idx[f].x - cp_lo);
+    const double* jp = Jp + static_cast<size_t>(f) * 2 * NB;
+    const double* jl = Jl + 6 * static_cast<size_t>(f);
+    for (int a = lane; a < NB; a += 32) {
+      const double j0 = wgt * jp[a], j1 = wgt * jp[NB + a];
+      double* wr = Y + 3 * (b0 + a);
+      wr[0] += j0 * jl[0] + j1 * jl[3];
+      wr[1] += j0 * jl[1] + j1 * jl[4];
+      wr[2] += j0 * jl[2] + j1 * jl[5];
+    }
+    __syncwarp();
+  }
+  double F[6];
+#pragma unroll
+  for (int i = 0; i < 6; ++i) F[i] = Vchol[9 * static_cast<size_t>(l) + i];
+  for (int r = lane; r < rows; r += 32) {
+    double y[3];
+    lm_lsolve(F, Y[3 * r], Y[3 * r + 1], Y[3 * r + 2], y);
+    Y[3 * r] = y[0]; Y[3 * r + 1] = y[1]; Y[3 * r + 2] = y[2];
+  }
+  __syncwarp();
+  double M[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+  const int g0 = 6 * cp_lo;
+  for (int r = lane; r < rows; r += 32) {
+    double t[3] = {0, 0, 0};
+    const int gr = g0 + r;
+    for (int s = 0; s < rows; ++s) {
+      const int gs = g0 + s;
+      const double z = cov[sys_index(lay, max(gr, gs), min(gr, gs))];
+      t[0] += z * Y[3 * s]; t[1] += z * Y[3 * s + 1]; t[2] += z * Y[3 * s + 2];
+    }
+#pragma unroll
+    for (int a = 0; a < 3; ++a)
+#pragma unroll
+      for (int b = 0; b < 3; ++b) M[3 * a + b] += Y[3 * r + a] * t[b];
+  }
+#pragma unroll
+  for (int i = 0; i < 9; ++i)
+#pragma unroll
+    for (int x = 16; x > 0; x >>= 1) M[i] += __shfl_xor_sync(0xffffffffu, M[i], x);
+  if (lane == 0) {
+    // L^-1 (lower), columns L^-1 e_c
+    double Li[9], y[3];
+    lm_lsolve(F, 1.0, 0.0, 0.0, y); Li[0] = y[0]; Li[3] = y[1]; Li[6] = y[2];
+    lm_lsolve(F, 0.0, 1.0, 0.0, y); Li[1] = y[0]; Li[4] = y[1]; Li[7] = y[2];
+    lm_lsolve(F, 0.0, 0.0, 1.0, y); Li[2] = y[0]; Li[5] = y[1]; Li[8] = y[2];
+    double A[9], T[9];
+#pragma unroll
+    for (int i = 0; i < 9; ++i) A[i] = 0.5 * (M[i] + M[3 * (i % 3) + i / 3]) + ((i % 4 == 0) ? 1.0 : 0.0);
+    m3_mul(A, Li, T);        // (I + M) L^-1
+    double S[9];
+    m3_tmul(Li, T, S);       // L^-T (I + M) L^-1
+#pragma unroll
+    for (int i = 0; i < 9; ++i) o[i] = 0.5 * (S[i] + S[3 * (i % 3) + i / 3]);
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Covariance of the interpolated pose at arbitrary stamps, one thread per stamp: J(t) (6 x 6k) is the Jacobian of the
+// pose [theta | p] at t (global rotation tangent, R <- Exp(theta) R, p <- p + rho) with respect to the tangents of its k
+// control points -- the pose-factor Jacobian of manifold_eval_kernel with an identity sensor at zero residual -- and
+// Sigma(t) = sum_ab J_a Z_ab J_b^T over the k x k control-point blocks (within the band).  knots / tab are the snapshot of
+// the last successful compute.  A stamp outside the valid span gives a zero block and invalid[f] = 1.
+// ---------------------------------------------------------------------------------------------
+template <int K>
+__global__ void cov_interpolate_kernel(int n, const double* __restrict__ stamps, const double* __restrict__ knots, const double* __restrict__ tab,
+                                       int Kn, Basis B, const double* __restrict__ cov, SysLayout lay, double* __restrict__ out,
+                                       int* __restrict__ invalid) {
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= n) return;
+  double* o = out + 36 * static_cast<size_t>(f);
+  const int base = segment_base(knots, 8, 7, Kn, K, stamps[f]);
+  invalid[f] = base < 0 ? 1 : 0;
+  if (base < 0) {
+    for (int i = 0; i < 36; ++i) o[i] = 0.0;
+    return;
+  }
+  constexpr int left = (K - 1) / 2;
+  const double* row0 = tab + static_cast<size_t>(base) * kTabStride;
+  const double t0 = row0[left * kTabStride + 24], t1 = row0[(left + 1) * kTabStride + 24];
+  const double inv_dt = 1.0 / (t1 - t0);
+  double lam[K + 1];
+  basis_eval<K, false>(B, (stamps[f] - t0) * inv_dt, inv_dt, lam, nullptr, nullptr);
+  double P[9], M[(K - 1) * 9];
+#pragma unroll
+  for (int i = 0; i < 9; ++i) P[i] = row0[i];
+#pragma unroll
+  for (int j = 1; j < K; ++j) {
+    const double* rj = row0 + j * kTabStride;
+    const double wj[3] = {lam[j] * rj[12], lam[j] * rj[13], lam[j] * rj[14]};
+    double A[9], Jr[9], Pn[9], G[9], JG[9], PJG[9];
+    so3_exp_and_Jr(wj, A, Jr);
+    m3_mul(P, A, Pn);
+#pragma unroll
+    for (int i = 0; i < 9; ++i) G[i] = rj[15 + i];
+    m3_mul(Jr, G, JG);
+    m3_mul(Pn, JG, PJG);
+#pragma unroll
+    for (int i = 0; i < 9; ++i) { M[(j - 1) * 9 + i] = lam[j] * PJG[i]; P[i] = Pn[i]; }
+  }
+  // J_m = [D_m 0 ; 0 w_m I], D_m = d theta / d phi_m, w_m = lambda_m - lambda_{m+1}
+  auto Dm = [&](int mm, int i) { return ((mm == 0) ? ((i % 4 == 0) ? 1.0 : 0.0) : M[(mm - 1) * 9 + i]) - ((mm + 1 < K) ? M[mm * 9 + i] : 0.0); };
+  double S[36];
+#pragma unroll
+  for (int i = 0; i < 36; ++i) S[i] = 0.0;
+  for (int a = 0; a < K; ++a) {
+    double Da[9];
+    for (int i = 0; i < 9; ++i) Da[i] = Dm(a, i);
+    const double wa = lam[a] - lam[a + 1];
+    for (int b = 0; b < K; ++b) {
+      double Db[9];
+      for (int i = 0; i < 9; ++i) Db[i] = Dm(b, i);
+      const double wb = lam[b] - lam[b + 1];
+      double Z[36], T[36];
+      for (int r = 0; r < 6; ++r)
+        for (int s = 0; s < 6; ++s) {
+          const int gi = 6 * (base + a) + r, gj = 6 * (base + b) + s;
+          Z[r * 6 + s] = cov[sys_index(lay, max(gi, gj), min(gi, gj))];
+        }
+      for (int r = 0; r < 6; ++r) {   // T = Z_ab J_b^T
+        for (int c = 0; c < 3; ++c) T[r * 6 + c] = Z[r * 6] * Db[c * 3] + Z[r * 6 + 1] * Db[c * 3 + 1] + Z[r * 6 + 2] * Db[c * 3 + 2];
+        for (int c = 3; c < 6; ++c) T[r * 6 + c] = wb * Z[r * 6 + c];
+      }
+      for (int c = 0; c < 6; ++c) {   // S += J_a T
+        for (int i = 0; i < 3; ++i) S[i * 6 + c] += Da[i * 3] * T[c] + Da[i * 3 + 1] * T[6 + c] + Da[i * 3 + 2] * T[12 + c];
+        for (int i = 3; i < 6; ++i) S[i * 6 + c] += wa * T[i * 6 + c];
+      }
+    }
+  }
+  for (int i = 0; i < 6; ++i)
+    for (int c = 0; c < 6; ++c) o[i * 6 + c] = 0.5 * (S[i * 6 + c] + S[c * 6 + i]);
+}
+
+}  // namespace hb

@@ -101,6 +101,7 @@ class Optimizer {   // OptimizerSuite::H100
 
  private:
   friend class ExteroceptiveCost;
+  friend class Covariance;
   void upload(bool factors);
   void download();
   Index cameraIndex(const Camera* camera) const;

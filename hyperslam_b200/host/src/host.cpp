@@ -7,6 +7,7 @@
 #include <stdexcept>
 #include <string>
 
+#include "hyper/covariance.hpp"
 #include "hyper/optimizer.hpp"
 #include "../../../include/hyperb200.h"
 
@@ -401,6 +402,125 @@ Pointers<Scalar> ExteroceptiveCost::update() {
 
 bool ExteroceptiveCost::Evaluate(const double* const* parameters, double* residuals, double** jacobians) const {
   return hb200_factor_evaluate(optimizer_->ctx_, static_cast<int>(kind_), index_, parameters, residuals, jacobians) == 0;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Covariance
+// ---------------------------------------------------------------------------------------------
+bool Covariance::locate(const double* p, Block* b) const {
+  const Optimizer& o = optimizer_;
+  const int K = static_cast<int>(o.state_->elements().size());
+  const int Kbg = o.imu_ ? static_cast<int>(o.imu_->gyroscopeBias().size()) : 0;
+  const int Kba = o.imu_ ? static_cast<int>(o.imu_->accelerometerBias().size()) : 0;
+  for (int j = 0; j < K; ++j)
+    if (o.state_->elements()[j].data() == p) { *b = {kState, j, 6 * j, 6, 8}; return true; }
+  for (int j = 0; j < Kbg; ++j)
+    if (o.imu_->gyroscopeBias()[j].data() == p) { *b = {kGyroBias, j, 6 * K + 3 * j, 3, 4}; return true; }
+  for (int j = 0; j < Kba; ++j)
+    if (o.imu_->accelerometerBias()[j].data() == p) { *b = {kAccelBias, j, 6 * K + 3 * Kbg + 3 * j, 3, 4}; return true; }
+  if (o.gravity_ && o.gravity_->data() == p) { *b = {kGravity, 0, 6 * K + 3 * (Kbg + Kba), 2, 3}; return true; }
+  for (size_t l = 0; l < o.landmarks_.size(); ++l)
+    if (o.landmarks_[l]->variable.data() == p) { *b = {kLandmark, static_cast<int>(l), -1, 3, 3}; return true; }
+  return false;
+}
+
+bool Covariance::inPattern(const Block& a, const Block& b, int beta) const {
+  if (a.kind == kLandmark || b.kind == kLandmark) return a.kind == b.kind && a.index == b.index;
+  if (a.kind == kState && b.kind == kState) return std::abs(a.index - b.index) <= beta;
+  return true;   // arrow and corner
+}
+
+Manifold Covariance::manifold(const Block& b) const {
+  switch (b.kind) {
+    case kState: return Manifold::StampedSE3(true, false, false);
+    case kGyroBias:
+    case kAccelBias: return Manifold::StampedEuclidean(3, true, false);
+    case kGravity: return Manifold::Sphere(3);
+    default: return Manifold::Euclidean(3);
+  }
+}
+
+bool Covariance::Compute(const std::vector<std::pair<const double*, const double*>>& blocks) {
+  Optimizer& o = optimizer_;
+  if (!o.state_) return false;
+  o.upload(o.dirty_);   // the device window == the host variables (as Ceres evaluates at the values it aliases)
+  int beta = 0;
+  check(hb200_get_bandwidth(o.ctx_, &beta), "hb200_get_bandwidth");
+  for (const auto& [pa, pb] : blocks) {
+    Block a, b;
+    if (!locate(pa, &a) || !locate(pb, &b) || !inPattern(a, b, beta)) return false;
+  }
+  check(hb200_build_covariance(o.ctx_), "hb200_build_covariance");
+  hb200_covariance_info info{};
+  const int rc = hb200_compute_covariance(o.ctx_, &info);
+  info_ = info;
+  if (rc == HB200_COV_NOT_POSITIVE_DEFINITE || rc == HB200_COV_DEGENERATE_LANDMARKS) return false;
+  check(rc, "hb200_compute_covariance");
+  packed_.assign(static_cast<size_t>(info.K) * (6 + 6 * info.beta) * 6 + static_cast<size_t>(info.m) * 6 * info.K + static_cast<size_t>(info.m) * info.m, 0.0);
+  landmarks_.assign(9 * static_cast<size_t>(info.L), 0.0);
+  check(hb200_get_covariance(o.ctx_, packed_.data(), landmarks_.empty() ? nullptr : landmarks_.data()), "hb200_get_covariance");
+  beta_ = info.beta; K_ = info.K; n_ = 6 * info.K + info.m;
+  computed_ = blocks;
+  values_.clear();
+  for (const auto& [pa, pb] : blocks)
+    for (const double* p : {pa, pb}) {
+      Block b;
+      locate(p, &b);
+      values_[p] = std::vector<double>(p, p + b.ambient);
+    }
+  return true;
+}
+
+bool Covariance::tangentBlock(const double* pa, const double* pb, std::vector<double>* out, Block* a, Block* b) const {
+  bool found = false;
+  for (const auto& [x, y] : computed_) found = found || (x == pa && y == pb) || (x == pb && y == pa);
+  if (!found || !locate(pa, a) || !locate(pb, b)) return false;
+  out->assign(static_cast<size_t>(a->tangent) * b->tangent, 0.0);
+  if (a->kind == kLandmark) {   // (same landmark: the only landmark pair in the pattern)
+    for (int i = 0; i < 9; ++i) (*out)[i] = landmarks_[9 * static_cast<size_t>(a->index) + i];
+    return true;
+  }
+  // entry (r, c), r >= c, of the packed P | A | C layout (diagonal blocks and corner stored in full)
+  const int np = 6 * K_, h = 6 + 6 * beta_, m = n_ - np;
+  auto at = [&](int r, int c) {
+    if (r < c) std::swap(r, c);
+    if (r < np) { const int cb = c / 6; return packed_[(static_cast<size_t>(cb) * h + (r - 6 * cb)) * 6 + (c - 6 * cb)]; }
+    if (c < np) return packed_[static_cast<size_t>(K_) * h * 6 + static_cast<size_t>(r - np) * np + c];
+    return packed_[static_cast<size_t>(K_) * h * 6 + static_cast<size_t>(m) * np + static_cast<size_t>(r - np) * m + (c - np)];
+  };
+  // Ceres' quaternion tangent: delta = theta / 2
+  auto scale = [](const Block& bl, int i) { return (bl.kind == kState && i < 3) ? 0.5 : 1.0; };
+  for (int i = 0; i < a->tangent; ++i)
+    for (int j = 0; j < b->tangent; ++j) (*out)[static_cast<size_t>(i) * b->tangent + j] = scale(*a, i) * at(a->dof + i, b->dof + j) * scale(*b, j);
+  return true;
+}
+
+bool Covariance::GetCovarianceBlockInTangentSpace(const double* pa, const double* pb, double* cov) const {
+  std::vector<double> T;
+  Block a, b;
+  if (!tangentBlock(pa, pb, &T, &a, &b)) return false;
+  std::copy(T.begin(), T.end(), cov);
+  return true;
+}
+
+bool Covariance::GetCovarianceBlock(const double* pa, const double* pb, double* cov) const {
+  std::vector<double> T;
+  Block a, b;
+  if (!tangentBlock(pa, pb, &T, &a, &b)) return false;
+  const Manifold ma = manifold(a), mb = manifold(b);
+  const int ta = ma.TangentSize(), tb = mb.TangentSize();
+  std::vector<double> Pa(static_cast<size_t>(a.ambient) * ta), Pb(static_cast<size_t>(b.ambient) * tb);
+  ma.PlusJacobian(values_.at(pa).data(), Pa.data());
+  mb.PlusJacobian(values_.at(pb).data(), Pb.data());
+  // P_a T P_b^T
+  for (int r = 0; r < a.ambient; ++r)
+    for (int c = 0; c < b.ambient; ++c) {
+      double s = 0.0;
+      for (int i = 0; i < ta; ++i)
+        for (int j = 0; j < tb; ++j) s += Pa[static_cast<size_t>(r) * ta + i] * T[static_cast<size_t>(i) * tb + j] * Pb[static_cast<size_t>(c) * tb + j];
+      cov[static_cast<size_t>(r) * b.ambient + c] = s;
+    }
+  return true;
 }
 
 }  // namespace hyper

@@ -38,6 +38,14 @@ class Iteration(C.Structure):
                 ("radius", C.c_double), ("accepted", C.c_int), ("spd", C.c_int)]
 
 
+class CovarianceInfo(C.Structure):
+    _fields_ = [("status", C.c_int), ("bad_dof", C.c_int), ("degenerate_landmarks", C.c_int), ("unobserved_landmarks", C.c_int),
+                ("min_pivot_ratio", C.c_double), ("K", C.c_int), ("beta", C.c_int), ("m", C.c_int), ("L", C.c_int)]
+
+
+COV_NOT_POSITIVE_DEFINITE, COV_DEGENERATE_LANDMARKS = 40, 41
+
+
 ALLREDUCE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p)
 
 EXPORTS = [
@@ -56,7 +64,7 @@ EXPORTS = [
     "hb200_append_knots", "hb200_append_landmarks", "hb200_append_pixel_factors", "hb200_append_inertial_factors", "hb200_slide",
     "hb200_window_sizes", "hb200_set_termination", "hb200_get_termination",
     "hb200_append_bearing_factors", "hb200_append_manifold_factors", "hb200_append_stereo_tracks", "hb200_slide_landmark_map",
-    "hb200_factor_counts",
+    "hb200_factor_counts", "hb200_build_covariance", "hb200_compute_covariance", "hb200_get_covariance", "hb200_interpolate_covariance",
 ]
 
 _lib = None
@@ -107,6 +115,7 @@ class Context:
         self._cb = None
         self.order = self.K = self.Kbg = self.Kba = self.L = self.Nv = self.Ni = self.Nb = self.Nm = 0
         self._slide_L = 0   # landmarks before the last slide (landmark_map)
+        self._cov_shape = (0, 0, 0, 0)
         self.bias_order = 4
 
     def _check(self, rc: int):
@@ -359,6 +368,52 @@ class Context:
         dp, dl = np.zeros(self.reduced_size()), np.zeros((self.L, 3))
         self._check(self.lib.hb200_get_delta(self.h, _d(dp), _d(dl)))
         return dp, dl
+
+    # ---- marginal covariances (ceres::Covariance) --------------------------------------------------------------
+    def build_covariance(self):
+        """Undamped reduced system at the current state into the packed buffer (hb200_build_covariance)."""
+        self._check(self.lib.hb200_build_covariance(self.h))
+
+    def compute_covariance(self):
+        """Selected inverse + landmark marginals.  Returns the info dict; a status != 0 (not positive definite, degenerate
+        landmarks) is reported there, not raised, and the previous results stay in place."""
+        info = CovarianceInfo()
+        rc = self.lib.hb200_compute_covariance(self.h, C.byref(info))
+        if rc not in (0, COV_NOT_POSITIVE_DEFINITE, COV_DEGENERATE_LANDMARKS):
+            self._check(rc)
+        out = {n: getattr(info, n) for n, _ in CovarianceInfo._fields_}
+        out["rc"] = rc
+        if rc:
+            out["message"] = self.lib.hb200_last_error_string().decode()
+        self._cov_shape = (info.K, info.beta, info.m, info.L)
+        return out
+
+    def covariance_packed(self):
+        """(packed P | A | C of Sigma, landmark blocks (L, 3, 3), (K, beta, m, L)) of the last successful compute."""
+        K, beta, m, L = self._cov_shape
+        h = 6 + 6 * beta
+        packed = np.zeros(K * h * 6 + m * 6 * K + m * m)
+        lm = np.zeros((L, 3, 3))
+        self._check(self.lib.hb200_get_covariance(self.h, _d(packed), _d(lm)))
+        return packed, lm, (K, beta, m, L)
+
+    def covariance(self):
+        """The last successful compute as blocks: band (K, beta+1, 6, 6) with band[j, o] = Sigma(block j+o, block j) (zero past
+        the window), arrow (m, 6K), corner (m, m) and landmarks (L, 3, 3)."""
+        packed, lm, (K, beta, m, L) = self.covariance_packed()
+        h = 6 + 6 * beta
+        P = packed[:K * h * 6].reshape(K, beta + 1, 6, 6)
+        A = packed[K * h * 6:K * h * 6 + m * 6 * K].reshape(m, 6 * K)
+        Cc = packed[K * h * 6 + m * 6 * K:].reshape(m, m)
+        return dict(band=P, arrow=A, corner=Cc, landmarks=lm)
+
+    def interpolate_covariance(self, stamps):
+        """6 x 6 covariances of the interpolated pose [theta | p] at the stamps; returns (cov (n, 6, 6), num_invalid)."""
+        stamps = _f64(stamps).ravel()
+        out = np.zeros((stamps.size, 6, 6))
+        bad = C.c_int(0)
+        self._check(self.lib.hb200_interpolate_covariance(self.h, stamps.size, _d(stamps), _d(out), C.byref(bad)))
+        return out, bad.value
 
     def iterate(self, iterations=1, records=True):
         rec = (Iteration * max(iterations, 1))()

@@ -180,6 +180,44 @@ int hb200_get_system(hb200_ctx* ctx, double* S /* n x n */, double* b /* n */);
 /* dense Cholesky of the reduced system, back-substitution, landmark back-substitution. */
 int hb200_solve(hb200_ctx* ctx);
 int hb200_get_delta(hb200_ctx* ctx, double* delta_pose /* n */, double* delta_landmark /* 3L */);
+/* ---- marginal covariances: the replacement of ceres::Covariance (default options: apply_loss_function, constant
+ * blocks get zero covariance) -----------------------------------------------------------------------------------------
+ * Sigma = (J^T W J)^-1 over the non-constant dofs at the current state, W the loss weights of the LM build (Huber rho' of
+ * pixel / bearing factors, the inertial ScaledLoss, none for pose factors), no damping anywhere (mu = 0, also inside the
+ * landmark elimination).  Constant knots, bias_const and gravity_const dofs get exact zeros.  Tangent convention of the
+ * device: rotation global (R <- Exp(theta) R), SE3 split [theta | rho] with p <- p + rho, gravity the 2-dof sphere tangent.
+ *   hb200_build_covariance:   evaluates at the current state and assembles the UNDAMPED reduced system into the packed
+ *                             buffer (hb200_system_device_ptr) with the factor, J^T J and Schur kernels of hb200_build_system;
+ *                             flags degenerate / unobserved landmarks; one read-back.  The LM's trust-region state is not
+ *                             touched, but the packed buffer is no longer a damped-solve input: hb200_get_system / hb200_solve
+ *                             return -2 until the next hb200_build_system.  Copies the knots it linearised at.
+ *   hb200_compute_covariance: band + arrow Cholesky of the (equilibrated, masked) packed buffer and its selected inverse --
+ *                             every entry of Sigma on the block band of half-width beta, the arrow and the corner -- then the
+ *                             3 x 3 marginal of every landmark.  Only valid right after hb200_build_covariance (-2 when a
+ *                             setter changed the window or any other call launched work since).  status 1 (returns HB200_COV_NOT_POSITIVE_DEFINITE): a pivot
+ *                             of the equilibrated reduced factor is <= 1e-10 (gauge not fixed, a bias / gravity dof without a
+ *                             factor); bad_dof = the first such dof.  status 2 (returns HB200_COV_DEGENERATE_LANDMARKS): a
+ *                             landmark's undamped V_l is rank-deficient (seen by one pixel factor only).  An unobserved
+ *                             landmark is no failure: zero block, counted.  On failure the previous results stay in place.
+ *   hb200_get_covariance:     packed = Sigma in the P | A | C part of the packed layout (doubles [0, oC + m*m): diagonal blocks
+ *                             and corner full, padding rows 0), landmark = [L][3][3] (may be NULL).  Shape: info K, beta, m, L.
+ *   hb200_interpolate_covariance: the 6 x 6 covariance of the pose [theta | p] interpolated at each stamp, at the knots of
+ *                             the last successful compute; stamps outside the valid span give zero blocks, counted.
+ * Single GPU: a context with a communicator or all-reduce callback gets -3.  A window whose band + arrow (6 (beta+1) + m
+ * rows, square) does not fit one CTA's shared memory gets -6.  Ceres-tangent and ambient blocks: hyper::Covariance (host). */
+typedef struct hb200_covariance_info {
+  int status;                 /* 0 ok, 1 reduced system not positive definite, 2 degenerate landmarks */
+  int bad_dof;                /* status 1: first reduced-system dof whose pivot failed, else -1 */
+  int degenerate_landmarks, unobserved_landmarks;
+  double min_pivot_ratio;     /* smallest pivot of the equilibrated reduced factor (status 1: the failing one) */
+  int K, beta, m, L;          /* shape of what hb200_get_covariance returns */
+} hb200_covariance_info;
+enum { HB200_COV_NOT_POSITIVE_DEFINITE = 40, HB200_COV_DEGENERATE_LANDMARKS = 41 };
+int hb200_build_covariance(hb200_ctx* ctx);
+int hb200_compute_covariance(hb200_ctx* ctx, hb200_covariance_info* info);
+int hb200_get_covariance(hb200_ctx* ctx, double* packed /* P | A | C of SysLayout */, double* landmark /* [L][3][3], may be NULL */);
+int hb200_interpolate_covariance(hb200_ctx* ctx, int n, const double* stamps, double* cov /* [n][6][6] */, int* num_invalid);
+
 /* full LM iterations: evaluate -> build -> [allreduce] -> solve -> retract -> cost at trial ->
  * accept/reject, all on the device.  records may be NULL. */
 int hb200_iterate(hb200_ctx* ctx, int iterations, hb200_iteration* records);
