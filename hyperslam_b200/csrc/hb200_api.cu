@@ -227,6 +227,7 @@ struct hb200_ctx {
   // none yet), kept until the next slide for hb200_slide_landmark_map
   DevBuf<int> w_keep, w_pos, w_lkeep, w_lpos, w_cnt, w_scal;
   int slide_L = -1;
+  int bg_dropped = 0, ba_dropped = 0;   // leading gyro / accel bias knots the last hb200_slide removed (HB200_SLIDE_DROP_BIAS)
   // hb200_append_stereo_tracks inputs: [stamp | pixel0 | pixel1] and [camera0 | camera1 | landmark | new flag | rank]
   DevBuf<double> trk_d;
   DevBuf<int> trk_i;
@@ -453,8 +454,13 @@ int ensure_system(hb200_ctx* c) {
       const size_t colbytes = (static_cast<size_t>(6 + 6 * c->beta) * 6 + 6 * static_cast<size_t>(c->n - 6 * c->K + 1) + 48) * sizeof(double);
       const int fit = static_cast<int>((200 * 1024) / (2 * colbytes));
       c->band_chunk_cols = std::max(c->beta + 2, std::min(fit, c->K + c->beta));
-      c->band_chunk_smem = 2 * colbytes * c->band_chunk_cols;
-      if (c->band_chunk_smem > 220 * 1024) return fail(-6, "band solver: a chunk of %d block columns does not fit shared memory (arrow too wide)", c->band_chunk_cols);
+      // after the factorisation the corner system [m + 1][m | 1], its solution and factor diagonal (2m) and the
+      // 6-double block scratch behind them move into the same shared memory (band_solve_kernel<false>): a wide
+      // arrowhead needs more than the two chunk views
+      const int m = c->n - 6 * c->K;
+      const size_t corner = (static_cast<size_t>(m + 1) * (m | 1) + 2 * static_cast<size_t>(m) + 6) * sizeof(double);
+      c->band_chunk_smem = std::max(2 * colbytes * c->band_chunk_cols, corner);
+      if (c->band_chunk_smem > 220 * 1024) return fail(-6, "band solver: a chunk of %d block columns or the %d x %d corner does not fit shared memory (arrow too wide)", c->band_chunk_cols, m, m);
       HB_CUDA(cudaFuncSetAttribute(band_solve_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(c->band_chunk_smem)));
     }
   }
@@ -2442,7 +2448,7 @@ int hb200_append_knots(hb200_ctx* c, int count) {
     HB_CUDA(c->knots[s2].grow(8 * static_cast<size_t>(K + count), s2 == 0 ? 8 * static_cast<size_t>(K) : 0, c->stream));
     HB_CUDA(c->tab[s2].ensure(static_cast<size_t>(K + count) * kTabStride));
   }
-  append_knots_kernel<<<1, 32, 0, c->stream>>>(K, count, c->knots[0].p);
+  append_knots_kernel<<<1, 32, 0, c->stream>>>(K, count, 8, 7, c->knots[0].p);
   HB_LAUNCH(c, "append_knots_kernel");
   std::vector<double> tail(8 * static_cast<size_t>(count));
   HB_CUDA(cudaMemcpyAsync(tail.data(), c->knots[0].p + 8 * static_cast<size_t>(K), sizeof(double) * tail.size(), cudaMemcpyDeviceToHost, c->stream));
@@ -2454,6 +2460,88 @@ int hb200_append_knots(hb200_ctx* c, int count) {
   HB_CUDA(cudaStreamSynchronize(c->stream));
   c->invalidate(); c->have_snapshot = false;
   return sync_layout(c);
+}
+
+}  // extern "C"
+
+namespace {
+// Fewest knots append_knots_kernel must append to a bias spline (stamps s, order kb) so that segment_base accepts t:
+// s[left] <= t < s'[K' - right] (left = (kb-1)/2, right = kb-1-left) over the K' extended stamps s', where new stamp
+// K - 1 + i is fma(i, dt, s[K-1]) with dt = s[K-1] - s[K-2].  0 on success, 2 for t before the span, -1 past HB200_BIAS_APPEND_MAX.
+int bias_append_count(const std::vector<double>& s, int kb, double t, int* count) {
+  const int K = static_cast<int>(s.size()), left = (kb - 1) / 2, right = kb - 1 - left;
+  const double dt = s[K - 1] - s[K - 2];
+  auto end_of = [&](int added) {   // the valid span's end with `added` knots appended: stamp of knot K + added - right
+    const int j = K + added - right;
+    return j < K ? s[j] : std::fma(static_cast<double>(j - (K - 1)), dt, s[K - 1]);
+  };
+  *count = 0;
+  if (t < s[left]) return 2;
+  if (t < end_of(0)) return 0;
+  const double est = std::floor((t - s[K - 1]) / dt) + right;   // first guess; the loops below decide
+  if (!(est <= HB200_BIAS_APPEND_MAX + 1.0)) return -1;
+  int n = std::max(1, static_cast<int>(est));
+  while (n > 1 && t < end_of(n - 1)) --n;
+  while (!(t < end_of(n)) && n <= HB200_BIAS_APPEND_MAX) ++n;
+  if (n > HB200_BIAS_APPEND_MAX) return -1;
+  *count = n;
+  return 0;
+}
+}  // namespace
+
+extern "C" {
+
+int hb200_append_bias_knots(hb200_ctx* c, double stamp, int* gyro_added, int* accel_added) {
+  if (gyro_added) *gyro_added = 0;
+  if (accel_added) *accel_added = 0;
+  if (!c) return fail(-1, "null context");
+  if (c->Kbg == 0 || c->Kba == 0) return fail(-2, "bias splines not set");
+  int rc = check_device_window(c);
+  if (rc) return rc;
+  if (!std::isfinite(stamp)) return fail(-1, "stamp is not finite");
+  int add[2] = {0, 0};
+  for (int w = 0; w < 2; ++w) {
+    rc = bias_append_count(w ? c->h_ba_stamp : c->h_bg_stamp, c->kb, stamp, &add[w]);
+    if (rc == 2) return fail(2, "stamp %.17g lies before the %s bias spline's valid span (bias knots are never prepended)", stamp, w ? "accelerometer" : "gyroscope");
+    if (rc) return fail(-1, "stamp %.17g needs more than %d new %s bias knots", stamp, HB200_BIAS_APPEND_MAX, w ? "accelerometer" : "gyroscope");
+  }
+  if (add[0] == 0 && add[1] == 0) return 0;
+  HB_CUDA(cudaSetDevice(c->device));
+  DevBuf<double>* bias[2] = {c->bg, c->ba};
+  const int Kb[2] = {c->Kbg, c->Kba};
+  for (int w = 0; w < 2; ++w)   // both state copies, contents kept, before anything changes
+    for (int s2 = 0; s2 < 2 && add[w]; ++s2) HB_CUDA(bias[w][s2].grow(4 * static_cast<size_t>(Kb[w] + add[w]), 4 * static_cast<size_t>(Kb[w]), c->stream));
+  for (int w = 0; w < 2; ++w) {
+    if (!add[w]) continue;
+    append_knots_kernel<<<1, 32, 0, c->stream>>>(Kb[w], add[w], 4, 3, bias[w][0].p);
+    HB_LAUNCH(c, "append_knots_kernel");
+  }
+  // the host stamp mirrors (hb200_optimize checks bias stamps against them) from the device's own results
+  for (int w = 0; w < 2; ++w) {
+    if (!add[w]) continue;
+    std::vector<double> tail(4 * static_cast<size_t>(add[w]));
+    HB_CUDA(cudaMemcpyAsync(tail.data(), bias[w][0].p + 4 * static_cast<size_t>(Kb[w]), sizeof(double) * tail.size(), cudaMemcpyDeviceToHost, c->stream));
+    HB_CUDA(cudaStreamSynchronize(c->stream));
+    std::vector<double>& hs = w ? c->h_ba_stamp : c->h_bg_stamp;
+    for (int i = 0; i < add[w]; ++i) hs.push_back(tail[4 * i + 3]);
+  }
+  c->Kbg = static_cast<int>(c->h_bg_stamp.size()); c->Kba = static_cast<int>(c->h_ba_stamp.size());
+  if (gyro_added) *gyro_added = add[0];
+  if (accel_added) *accel_added = add[1];
+  if ((rc = update_fixed(c))) return rc;
+  if ((rc = ensure_system(c))) return rc;
+  HB_CUDA(cudaStreamSynchronize(c->stream));
+  c->invalidate(); c->have_snapshot = false;
+  return sync_layout(c);
+}
+
+int hb200_bias_knots(hb200_ctx* c, int* num_gyro, int* num_accel, int* gyro_dropped, int* accel_dropped) {
+  if (!c) return fail(-1, "null context");
+  if (num_gyro) *num_gyro = c->Kbg;
+  if (num_accel) *num_accel = c->Kba;
+  if (gyro_dropped) *gyro_dropped = c->bg_dropped;
+  if (accel_dropped) *accel_dropped = c->ba_dropped;
+  return 0;
 }
 
 int hb200_append_landmarks(hb200_ctx* c, int n, const double* xyz) {
@@ -2605,9 +2693,12 @@ int hb200_slide(hb200_ctx* c, double lower_bound, int flags, hb200_slide_stats* 
   int ub = static_cast<int>(std::upper_bound(c->h_knot_stamp.begin(), c->h_knot_stamp.end(), lower_bound) - c->h_knot_stamp.begin());
   const int begin = std::max(0, ub - 1 - (c->k - 1) / 2);
   const int last_const = ub - 1;   // knots 0 .. last_const have stamp <= lower bound
-  HB_CUDA(c->w_scal.ensure(8));
-  // [L_new, Nv_new, Ni_new, min base visual, min base inertial, Nm_new, min base manifold, kept bearing factors]
-  int init[8] = {0, 0, 0, 0x7fffffff, 0x7fffffff, 0, 0x7fffffff, 0};
+  // leading bias knots go only with the inertial factors that reached them: without DROP_INERTIAL nothing is dropped
+  const bool drop_bias = (flags & HB200_SLIDE_DROP_BIAS) && (flags & HB200_SLIDE_DROP_INERTIAL) && c->Kbg && c->Kba;
+  HB_CUDA(c->w_scal.ensure(10));
+  // [L_new, Nv_new, Ni_new, min base visual, min base inertial, Nm_new, min base manifold, kept bearing factors,
+  //  min gyro bias base, min accel bias base (kept inertial factors)]
+  int init[10] = {0, 0, 0, 0x7fffffff, 0x7fffffff, 0, 0x7fffffff, 0, 0x7fffffff, 0x7fffffff};
   HB_CUDA(cudaMemcpyAsync(c->w_scal.p, init, sizeof(init), cudaMemcpyHostToDevice, c->stream));
   HB_CUDA(c->w_last.ensure(std::max(L, 1))); HB_CUDA(c->w_lkeep.ensure(std::max(L, 1) + 1)); HB_CUDA(c->w_lpos.ensure(std::max(L, 1) + 1));
   HB_CUDA(c->w_keep.ensure(std::max(std::max(Nv, Ni), 1))); HB_CUDA(c->w_pos.ensure(std::max(std::max(Nv, Ni), 1)));
@@ -2629,7 +2720,8 @@ int hb200_slide(hb200_ctx* c, double lower_bound, int flags, hb200_slide_stats* 
     HB_LAUNCH(c, "scan_kernel");
   }
   if (Ni) {
-    inertial_keep_kernel<<<(Ni + 255) / 256, 256, 0, c->stream>>>(Ni, c->i_idx.p, c->k, (flags & HB200_SLIDE_DROP_INERTIAL) ? last_const : -1, i_keep, c->w_scal.p + 4);
+    inertial_keep_kernel<<<(Ni + 255) / 256, 256, 0, c->stream>>>(Ni, c->i_idx.p, c->k, (flags & HB200_SLIDE_DROP_INERTIAL) ? last_const : -1, i_keep, c->w_scal.p + 4,
+                                                                  drop_bias ? c->w_scal.p + 8 : nullptr);
     HB_LAUNCH(c, "inertial_keep_kernel");
     scan_kernel<<<1, 1024, 0, c->stream>>>(i_keep, Ni, i_pos, c->w_scal.p + 2);
     HB_LAUNCH(c, "scan_kernel");
@@ -2640,7 +2732,7 @@ int hb200_slide(hb200_ctx* c, double lower_bound, int flags, hb200_slide_stats* 
     scan_kernel<<<1, 1024, 0, c->stream>>>(m_keep, Nm, m_pos, c->w_scal.p + 5);
     HB_LAUNCH(c, "scan_kernel");
   }
-  int h[8];
+  int h[10];
   HB_CUDA(cudaMemcpyAsync(h, c->w_scal.p, sizeof(h), cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
   const int L_new = L ? h[0] : 0, Nv_new = Nv ? h[1] : 0, Ni_new = Ni ? h[2] : 0, Nm_new = Nm ? h[5] : 0, Nb_new = Nv ? h[7] : 0;
@@ -2648,6 +2740,14 @@ int hb200_slide(hb200_ctx* c, double lower_bound, int flags, hb200_slide_stats* 
   int shift = std::min(std::min(begin, h[6]), std::min(h[3], h[4]));
   shift = std::max(0, std::min(shift, K - c->k));
   const int K_new = K - shift;
+  // the same rule on each bias spline, with the smallest bias base of the kept inertial factors
+  auto bias_shift = [&](const std::vector<double>& s, int min_base) {
+    const int ubb = static_cast<int>(std::upper_bound(s.begin(), s.end(), lower_bound) - s.begin());
+    const int sh = std::min(std::max(0, ubb - 1 - (c->kb - 1) / 2), min_base);
+    return std::max(0, std::min(sh, static_cast<int>(s.size()) - c->kb));
+  };
+  const int g_shift = drop_bias ? bias_shift(c->h_bg_stamp, h[8]) : 0, a_shift = drop_bias ? bias_shift(c->h_ba_stamp, h[9]) : 0;
+  const int Kbg_new = c->Kbg - g_shift, Kba_new = c->Kba - a_shift;
   // compaction into the alternate buffers, then swap
   const int n_alt = std::max(std::max(std::max(Nv_new, Ni_new), Nm_new), 1);
   HB_CUDA(c->alt_stamp.ensure(n_alt)); HB_CUDA(c->alt_idx.ensure(n_alt));
@@ -2664,7 +2764,8 @@ int hb200_slide(hb200_ctx* c, double lower_bound, int flags, hb200_slide_stats* 
   }
   HB_CUDA(c->alt_meas.ensure(std::max(6 * static_cast<size_t>(Ni_new), 7 * static_cast<size_t>(Nm_new)) + 1));
   if (Ni) {
-    compact_inertial_kernel<<<(Ni + 255) / 256, 256, 0, c->stream>>>(Ni, i_keep, i_pos, shift, c->i_stamp.p, c->i_meas.p, c->i_idx.p, c->alt_stamp.p, c->alt_meas.p, c->alt_idx.p);
+    compact_inertial_kernel<<<(Ni + 255) / 256, 256, 0, c->stream>>>(Ni, i_keep, i_pos, shift, g_shift, a_shift, c->i_stamp.p, c->i_meas.p, c->i_idx.p, c->alt_stamp.p,
+                                                                     c->alt_meas.p, c->alt_idx.p);
     HB_LAUNCH(c, "compact_inertial_kernel");
     HB_CUDA(cudaMemcpyAsync(c->i_stamp.p, c->alt_stamp.p, sizeof(double) * Ni_new, cudaMemcpyDeviceToDevice, c->stream));
     HB_CUDA(cudaMemcpyAsync(c->i_meas.p, c->alt_meas.p, sizeof(double) * 6 * Ni_new, cudaMemcpyDeviceToDevice, c->stream));
@@ -2686,16 +2787,32 @@ int hb200_slide(hb200_ctx* c, double lower_bound, int flags, hb200_slide_stats* 
     HB_LAUNCH(c, "compact_landmarks_kernel");
     HB_CUDA(cudaMemcpyAsync(c->lms[0].p, c->alt_lms.p, sizeof(double) * 3 * L_new, cudaMemcpyDeviceToDevice, c->stream));
   }
+  // (one scratch buffer for the three splines: the copies back are ordered on the stream)
+  const size_t alt_need = std::max(shift ? 8 * static_cast<size_t>(K_new) : 0,
+                                   std::max(g_shift ? 4 * static_cast<size_t>(Kbg_new) : 0, a_shift ? 4 * static_cast<size_t>(Kba_new) : 0));
+  if (alt_need) HB_CUDA(c->alt_knots.ensure(alt_need));
   if (shift) {
-    HB_CUDA(c->alt_knots.ensure(8 * static_cast<size_t>(K_new)));
-    shift_knots_kernel<<<(8 * K_new + 255) / 256, 256, 0, c->stream>>>(K_new, shift, c->knots[0].p, c->alt_knots.p);
+    shift_knots_kernel<<<(8 * K_new + 255) / 256, 256, 0, c->stream>>>(K_new, shift, 8, c->knots[0].p, c->alt_knots.p);
     HB_LAUNCH(c, "shift_knots_kernel");
     HB_CUDA(cudaMemcpyAsync(c->knots[0].p, c->alt_knots.p, sizeof(double) * 8 * K_new, cudaMemcpyDeviceToDevice, c->stream));
+  }
+  if (g_shift) {
+    shift_knots_kernel<<<(4 * Kbg_new + 255) / 256, 256, 0, c->stream>>>(Kbg_new, g_shift, 4, c->bg[0].p, c->alt_knots.p);
+    HB_LAUNCH(c, "shift_knots_kernel");
+    HB_CUDA(cudaMemcpyAsync(c->bg[0].p, c->alt_knots.p, sizeof(double) * 4 * Kbg_new, cudaMemcpyDeviceToDevice, c->stream));
+  }
+  if (a_shift) {
+    shift_knots_kernel<<<(4 * Kba_new + 255) / 256, 256, 0, c->stream>>>(Kba_new, a_shift, 4, c->ba[0].p, c->alt_knots.p);
+    HB_LAUNCH(c, "shift_knots_kernel");
+    HB_CUDA(cudaMemcpyAsync(c->ba[0].p, c->alt_knots.p, sizeof(double) * 4 * Kba_new, cudaMemcpyDeviceToDevice, c->stream));
   }
   HB_CUDA(cudaStreamSynchronize(c->stream));
   // host bookkeeping: sizes, stamps, constancy (elements at or before the lower bound: reference optimizer.cpp:322-328;
   // gravity once the window no longer covers the whole state range: reference abstract.cpp:57-61)
   c->h_knot_stamp.erase(c->h_knot_stamp.begin(), c->h_knot_stamp.begin() + shift);
+  c->h_bg_stamp.erase(c->h_bg_stamp.begin(), c->h_bg_stamp.begin() + g_shift);
+  c->h_ba_stamp.erase(c->h_ba_stamp.begin(), c->h_ba_stamp.begin() + a_shift);
+  c->Kbg = Kbg_new; c->Kba = Kba_new; c->bg_dropped = g_shift; c->ba_dropped = a_shift;
   c->h_knot_const.assign(K_new, 0);
   for (int j = 0; j < K_new; ++j) c->h_knot_const[j] = c->h_knot_stamp[j] <= lower_bound ? 1 : 0;
   if (ub > 0) c->gravity_const = 1;

@@ -7,7 +7,9 @@
 // of the factor lists.  New factors arrive in stamp order, so appending keeps the bound order (sorted by knot base);
 // removal is an order-preserving stream compaction.  All four families: pixel and bearing factors share the visual
 // list (kind in idx.w), inertial and manifold factors have their own; stereo tracks (the reference's live frame loop,
-// abstract.cpp:243-260) become bearing factors and new landmarks in stereo_track_kernel.  The incidence lists (landmark
+// abstract.cpp:243-260) become bearing factors and new landmarks in stereo_track_kernel.  The bias splines grow by the
+// same extrapolation (updateSensor, abstract.cpp:272-292) and lose their leading knots by the same removal rule when
+// HB200_SLIDE_DROP_BIAS is set.  The incidence lists (landmark
 // CSR, inertial runs, longest track) are built by the counting + scan kernels below, after hb200_bind as after every
 // append or slide.
 #pragma once
@@ -84,14 +86,19 @@ __global__ void visual_keep_kernel(int n, const int4* __restrict__ idx, const in
 }
 // inertial (int4 index) and manifold (int2 index) factors: kept (the reference never removes them); with drop_base >= 0
 // those whose control points ALL lie at or before the lower bound (base + order - 1 <= drop_base: every block the
-// residual moves with is constant) go
+// residual moves with is constant) go.  min_bias (inertial only, may be null): smallest kept gyro / accel bias base.
 template <typename Idx>
-__global__ void inertial_keep_kernel(int n, const Idx* __restrict__ idx, int order, int drop_base, int* __restrict__ keep, int* __restrict__ min_base) {
+__global__ void inertial_keep_kernel(int n, const Idx* __restrict__ idx, int order, int drop_base, int* __restrict__ keep, int* __restrict__ min_base,
+                                     int* __restrict__ min_bias = nullptr) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= n) return;
-  const int k = (drop_base >= 0 && idx[f].x + order - 1 <= drop_base) ? 0 : 1;
+  const Idx id = idx[f];
+  const int k = (drop_base >= 0 && id.x + order - 1 <= drop_base) ? 0 : 1;
   keep[f] = k;
-  if (k) atomicMin(min_base, idx[f].x);
+  if (k) atomicMin(min_base, id.x);
+  if constexpr (sizeof(Idx) == sizeof(int4)) {
+    if (k && min_bias) { atomicMin(&min_bias[0], id.y); atomicMin(&min_bias[1], id.z); }
+  }
 }
 
 // z: third bearing component of bearing factors (idx.w = 1), moved with the pixel pair
@@ -118,14 +125,14 @@ __global__ void compact_manifold_kernel(int n, const int* __restrict__ keep, con
 #pragma unroll
   for (int q = 0; q < 7; ++q) meas_o[7 * static_cast<size_t>(p) + q] = meas[7 * static_cast<size_t>(f) + q];
 }
-__global__ void compact_inertial_kernel(int n, const int* __restrict__ keep, const int* __restrict__ pos, int knot_shift, const double* __restrict__ stamp,
-                                        const double* __restrict__ meas, const int4* __restrict__ idx, double* __restrict__ stamp_o,
-                                        double* __restrict__ meas_o, int4* __restrict__ idx_o) {
+__global__ void compact_inertial_kernel(int n, const int* __restrict__ keep, const int* __restrict__ pos, int knot_shift, int gyro_shift, int accel_shift,
+                                        const double* __restrict__ stamp, const double* __restrict__ meas, const int4* __restrict__ idx,
+                                        double* __restrict__ stamp_o, double* __restrict__ meas_o, int4* __restrict__ idx_o) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= n || !keep[f]) return;
   const int p = pos[f];
   int4 id = idx[f];
-  id.x -= knot_shift;
+  id.x -= knot_shift; id.y -= gyro_shift; id.z -= accel_shift;
   stamp_o[p] = stamp[f]; idx_o[p] = id;
 #pragma unroll
   for (int q = 0; q < 6; ++q) meas_o[6 * static_cast<size_t>(p) + q] = meas[6 * static_cast<size_t>(f) + q];
@@ -137,9 +144,10 @@ __global__ void compact_landmarks_kernel(int L, const int* __restrict__ keep, co
 #pragma unroll
   for (int c = 0; c < 3; ++c) xyz_o[3 * static_cast<size_t>(p) + c] = xyz[3 * static_cast<size_t>(l) + c];
 }
-__global__ void shift_knots_kernel(int K_new, int shift, const double* __restrict__ knots, double* __restrict__ knots_o) {
+// knots of `stride` doubles (8: state elements, 4: bias knots): drop the first `shift`
+__global__ void shift_knots_kernel(int K_new, int shift, int stride, const double* __restrict__ knots, double* __restrict__ knots_o) {
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
-  if (e < 8 * K_new) knots_o[e] = knots[8 * shift + e];
+  if (e < stride * K_new) knots_o[e] = knots[stride * shift + e];
 }
 
 // process(VisualTracks) on the device (reference abstract.cpp:243-260): track f becomes the bearing factors at visual
@@ -173,14 +181,16 @@ __global__ void stereo_track_kernel(int n, const double* __restrict__ stamps, co
 }
 
 // reference abstract.cpp:126-136: the new element and the current last one take the variable of the second to last;
-// stamps continue at the knot separation
-__global__ void append_knots_kernel(int K, int count, double* __restrict__ knots) {
+// stamps continue at the knot separation.  Knots of `stride` doubles, the variable in the first `comps`, the stamp at
+// `comps` (8 / 7: state elements, 4 / 3: bias knots).  New stamp i is fma(i + 1, dt, last stamp), one rounding: the
+// host mirrors of the stamps (hb200_append_bias_knots) compute it the same way.
+__global__ void append_knots_kernel(int K, int count, int stride, int comps, double* __restrict__ knots) {
   if (blockIdx.x != 0 || threadIdx.x != 0) return;
-  const double dt = knots[8 * (K - 1) + 7] - knots[8 * (K - 2) + 7];
-  for (int q = 0; q < 7; ++q) knots[8 * (K - 1) + q] = knots[8 * (K - 2) + q];
+  const double dt = knots[stride * (K - 1) + comps] - knots[stride * (K - 2) + comps];
+  for (int q = 0; q < comps; ++q) knots[stride * (K - 1) + q] = knots[stride * (K - 2) + q];
   for (int i = 0; i < count; ++i) {
-    for (int q = 0; q < 7; ++q) knots[8 * (K + i) + q] = knots[8 * (K - 2) + q];
-    knots[8 * (K + i) + 7] = knots[8 * (K - 1) + 7] + (i + 1) * dt;
+    for (int q = 0; q < comps; ++q) knots[stride * (K + i) + q] = knots[stride * (K - 2) + q];
+    knots[stride * (K + i) + comps] = fma(static_cast<double>(i + 1), dt, knots[stride * (K - 1) + comps]);
   }
 }
 

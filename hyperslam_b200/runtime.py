@@ -30,7 +30,8 @@ class SlideStats(C.Structure):
                                        "knots", "landmarks", "visual_factors", "inertial_factors")]
 
 
-SLIDE_DROP_INERTIAL, SLIDE_DROP_MANIFOLD = 1, 2
+SLIDE_DROP_INERTIAL, SLIDE_DROP_MANIFOLD, SLIDE_DROP_BIAS = 1, 2, 4
+BIAS_APPEND_MAX = 1024   # knots one append_bias_knots call may add to one bias spline
 
 
 class Iteration(C.Structure):
@@ -65,6 +66,7 @@ EXPORTS = [
     "hb200_window_sizes", "hb200_set_termination", "hb200_get_termination",
     "hb200_append_bearing_factors", "hb200_append_manifold_factors", "hb200_append_stereo_tracks", "hb200_slide_landmark_map",
     "hb200_factor_counts", "hb200_build_covariance", "hb200_compute_covariance", "hb200_get_covariance", "hb200_interpolate_covariance",
+    "hb200_append_bias_knots", "hb200_bias_knots",
 ]
 
 _lib = None
@@ -229,6 +231,21 @@ class Context:
         self._check(self.lib.hb200_window_sizes(self.h, *[C.byref(x) for x in v]))
         self.K, self.L = v[0].value, v[1].value
         self.Nv, self.Ni, self.Nb, self.Nm = (int(n) for n in self.factor_counts())
+        b = self.bias_knots()
+        self.Kbg, self.Kba = b["gyro"], b["accel"]
+
+    def bias_knots(self):
+        """Current gyro / accel bias knot counts and the leading knots the last slide removed from each."""
+        v = [C.c_int(0) for _ in range(4)]
+        self._check(self.lib.hb200_bias_knots(self.h, *[C.byref(x) for x in v]))
+        return dict(gyro=v[0].value, accel=v[1].value, gyro_dropped=v[2].value, accel_dropped=v[3].value)
+
+    def append_bias_knots(self, stamp):
+        """updateSensor: extend each bias spline by the fewest knots that make `stamp` valid.  Returns (gyro_added, accel_added)."""
+        g, a = C.c_int(0), C.c_int(0)
+        self._check(self.lib.hb200_append_bias_knots(self.h, C.c_double(stamp), C.byref(g), C.byref(a)))
+        self._refresh_sizes()
+        return g.value, a.value
 
     def factor_counts(self):
         """Factor counts per family, indexed by PIXEL / INERTIAL / BEARING / MANIFOLD."""
@@ -288,10 +305,10 @@ class Context:
         self._refresh_sizes()
         return out, new.value
 
-    def slide(self, lower_bound, drop_inertial=True, drop_manifold=False):
+    def slide(self, lower_bound, drop_inertial=True, drop_manifold=False, drop_bias=False):
         st = SlideStats()
         self._slide_L = self.L
-        flags = (SLIDE_DROP_INERTIAL if drop_inertial else 0) | (SLIDE_DROP_MANIFOLD if drop_manifold else 0)
+        flags = (SLIDE_DROP_INERTIAL if drop_inertial else 0) | (SLIDE_DROP_MANIFOLD if drop_manifold else 0) | (SLIDE_DROP_BIAS if drop_bias else 0)
         self._check(self.lib.hb200_slide(self.h, C.c_double(lower_bound), flags, C.byref(st)))
         self._refresh_sizes()
         return {n: getattr(st, n) for n, _ in SlideStats._fields_}

@@ -131,6 +131,23 @@ int hb200_get_index_maps(hb200_ctx* ctx, int* pixel_base, int* inertial_base, in
  *                          never removes inertial or pose residuals; HB200_SLIDE_DROP_INERTIAL / _MANIFOLD additionally
  *                          drop the inertial / manifold factors whose control points are all at or before the bound, so
  *                          that the window stays bounded.  visual_factors in the stats counts pixel + bearing factors.
+ *                          HB200_SLIDE_DROP_BIAS applies the removal rule (:331-341) to each bias spline as well: with
+ *                          ub = number of bias stamps <= lower_bound, the leading min(max(0, ub - 1 - (kb-1)/2), smallest
+ *                          gyro (accel) bias base of the inertial factors this slide keeps) knots go, at least kb stay,
+ *                          and the kept factors' bias bases are remapped.  It only acts together with
+ *                          HB200_SLIDE_DROP_INERTIAL (the inertial factors are what holds the leading bias knots).
+ *   hb200_append_bias_knots: the reference's updateSensor (abstract.cpp:272-292) for a stamp past the bias splines:
+ *                          each spline independently gets the fewest knots that put `stamp` inside its valid span (the
+ *                          span hb200_bind and hb200_append_inertial_factors accept), by the hb200_append_knots rule --
+ *                          the new knots AND the current last one take the value of the second to last, stamps continue
+ *                          at the spline's own separation (new stamp i = fma(i + 1, dt, last stamp)).  A convention of
+ *                          this library: the reference leaves updateSensor unimplemented.  A stamp already inside
+ *                          appends nothing.  gyro_added / accel_added (may be NULL): knots appended.  Returns -1 for a
+ *                          non-finite stamp or one that needs more than HB200_BIAS_APPEND_MAX knots on a spline, -2
+ *                          without bias splines or a bound window, 2 for a stamp before a spline's valid span (knots
+ *                          are never prepended); a failed call changes nothing.
+ *   hb200_bias_knots:      current gyro / accel bias knot counts and the leading knots the last hb200_slide removed
+ *                          from each (a caller drops as many leading elements from its own copy); any may be NULL.
  *   hb200_slide_landmark_map: old -> new landmark index across the last hb200_slide (-1: dropped); n = number of
  *                          landmarks before that slide.  With landmark_out it keeps a caller's id -> slot map.
  *   hb200_factor_counts:   factor counts per family, indexed by HB200_PIXEL / _INERTIAL / _BEARING / _MANIFOLD. */
@@ -138,8 +155,11 @@ typedef struct hb200_slide_stats {
   int knots_dropped, knots_constant, landmarks_dropped, visual_factors_dropped, inertial_factors_dropped;
   int knots, landmarks, visual_factors, inertial_factors;   /* sizes after the call */
 } hb200_slide_stats;
-enum { HB200_SLIDE_DROP_INERTIAL = 1, HB200_SLIDE_DROP_MANIFOLD = 2 };
+enum { HB200_SLIDE_DROP_INERTIAL = 1, HB200_SLIDE_DROP_MANIFOLD = 2, HB200_SLIDE_DROP_BIAS = 4 };
+enum { HB200_BIAS_APPEND_MAX = 1024 };   /* knots one hb200_append_bias_knots call may add to one spline */
 int hb200_append_knots(hb200_ctx* ctx, int count);
+int hb200_append_bias_knots(hb200_ctx* ctx, double stamp, int* gyro_added, int* accel_added);
+int hb200_bias_knots(hb200_ctx* ctx, int* num_gyro, int* num_accel, int* gyro_dropped, int* accel_dropped);
 int hb200_append_landmarks(hb200_ctx* ctx, int n, const double* xyz);
 int hb200_append_pixel_factors(hb200_ctx* ctx, int n, const double* stamp, const int* camera, const int* landmark, const double* pixel);
 int hb200_append_inertial_factors(hb200_ctx* ctx, int n, const double* stamp, const double* measurement);
