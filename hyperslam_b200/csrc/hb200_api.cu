@@ -3,6 +3,7 @@
 // (reference internal/hyper/optimizers/ceres/optimizer.cpp:189-382) but flattened: one set of
 // device arrays per variable family and two factor lists.
 #include <algorithm>
+#include <array>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -10,6 +11,7 @@
 #include <cstring>
 #include <numeric>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include <cuda_runtime.h>
@@ -304,8 +306,8 @@ struct hb200_ctx {
   std::vector<cudaEvent_t> prof_events;
   std::vector<std::string> prof_names;
   size_t prof_used = 0;
-  // snapshot
-  DevBuf<double> snap_knots, snap_bg, snap_ba, snap_grav, snap_lms;
+  // snapshot (the variable blocks in the order of state_blocks)
+  DevBuf<double> snap[5];
   DevBuf<SolverState> snap_st;
   bool have_snapshot = false;
 
@@ -316,7 +318,28 @@ struct hb200_ctx {
   int o_bg() const { return 6 * K; }
   int o_ba() const { return 6 * K + 3 * Kbg; }
   int o_g() const { return 6 * K + 3 * Kbg + 3 * Kba; }
-  void invalidate() { graph_valid = false; system_built = false; cov_built = false; evaluated_J = false; mirror_valid = false; calib_valid = false; }
+
+  // What a change makes stale, from the narrowest to the widest.  The calibration and output mirrors are only read
+  // while evaluated_J holds, so dropping them with it never refuses a valid call.  `bound` and `have_snapshot` are
+  // cleared by the callers that need it: appends keep the window bound but drop the snapshot, a new camera count
+  // unbinds the window but keeps the snapshot.
+  // constants or the state changed: the built system and the covariance build no longer match them
+  void system_changed() { system_built = false; cov_built = false; }
+  // the factor outputs changed or no longer match the state
+  void outputs_changed() { system_changed(); evaluated_J = false; mirror_valid = false; calib_valid = false; }
+  // shapes or buffers the captured iteration was recorded with changed
+  void kernel_args_changed() { outputs_changed(); graph_valid = false; }
+
+  // The variable blocks in their canonical order (knots, gyroscope bias, accelerometer bias, gravity, landmarks): the
+  // current state, the trial state, the snapshot and the block's length in doubles.
+  struct StateBlock { DevBuf<double>* cur; DevBuf<double>* trial; DevBuf<double>* snap; size_t count; };
+  std::array<StateBlock, 5> state_blocks() {
+    return {{{&knots[0], &knots[1], &snap[0], 8 * static_cast<size_t>(K)},
+             {&bg[0], &bg[1], &snap[1], 4 * static_cast<size_t>(Kbg)},
+             {&ba[0], &ba[1], &snap[2], 4 * static_cast<size_t>(Kba)},
+             {&grav[0], &grav[1], &snap[3], 3},
+             {&lms[0], &lms[1], &snap[4], 3 * static_cast<size_t>(L)}}};
+  }
 };
 
 namespace {
@@ -342,6 +365,19 @@ int check_launch(hb200_ctx* c, const char* what) {
     int rc__ = check_launch(ctx, what);            \
     if (rc__) return rc__;                         \
   } while (0)
+
+// The kernels are instantiated per spline order: f(std::integral_constant<int, K>) for K = k.
+template <typename F>
+int with_order(int k, F&& f) {
+  if (k == 4) return f(std::integral_constant<int, 4>{});
+  if (k == 6) return f(std::integral_constant<int, 6>{});
+  return fail(-4, "spline order %d not supported (4 or 6)", k);
+}
+// f(std::true_type) or f(std::false_type), for the kernels' bool template flags
+template <typename F>
+int with_flag(bool b, F&& f) {
+  return b ? f(std::true_type{}) : f(std::false_type{});
+}
 
 // Launch configuration of the resident band solver: a grid of one 2-CTA cluster (chain r in CTA r) on the context's
 // stream, the whole workspace in each CTA's shared memory.  at: storage for the cluster-dimension attribute.
@@ -544,17 +580,12 @@ int launch_manifold(hb200_ctx* c, int sel) {
   HB_LAUNCH(c, "manifold_eval_kernel");
   return 0;
 }
-int enqueue_manifold(hb200_ctx* c, bool want_J, int sel) {
-  if (c->k == 4) return want_J ? launch_manifold<4, true>(c, sel) : launch_manifold<4, false>(c, sel);
-  return want_J ? launch_manifold<6, true>(c, sel) : launch_manifold<6, false>(c, sel);
-}
 
 // keep_fork: leave the side stream forked on return (the caller enqueues more side-stream work and joins).
 // clear_system: zero the packed reduced system in the knot-table launch; skip_prep: the table of state `sel` is
 // already up to date (retract_kernel built the trial table).
 int enqueue_evaluate(hb200_ctx* c, bool want_J, int sel, bool accumulate = false, bool keep_fork = false, bool clear_system = false,
                      bool skip_prep = false) {
-  if (c->k != 4 && c->k != 6) return fail(-4, "spline order %d not supported (4 or 6)", c->k);
   if (!skip_prep) {
     const size_t nclear = clear_system ? static_cast<size_t>(c->lay.total) : 0;
     const int blocks = clear_system ? static_cast<int>(std::min<size_t>((nclear / 4 + 255) / 256, static_cast<size_t>(c->num_sms) * 4)) : (c->K + 255) / 256;
@@ -568,9 +599,12 @@ int enqueue_evaluate(hb200_ctx* c, bool want_J, int sel, bool accumulate = false
   if (c->Nv && c->Ni && c->n_pix_blocks + c->n_imu_blocks <= 4 * c->num_sms) {   // (also while profiling: same kernels as the graph)
     // visual and inertial factors side by side in one launch; pose factors (if any) on the side stream
     if (c->Nm && (rc = fork_side(c))) return rc;
-    if (c->k == 4) rc = J_any ? launch_factors_merged<4, true>(c, sel, accumulate) : launch_factors_merged<4, false>(c, sel, false);
-    else rc = J_any ? launch_factors_merged<6, true>(c, sel, accumulate) : launch_factors_merged<6, false>(c, sel, false);
-    if (!rc) rc = enqueue_manifold(c, J_any, sel);
+    rc = with_order(c->k, [&](auto K) {
+      return with_flag(J_any, [&](auto J) {
+        const int r = launch_factors_merged<K, J>(c, sel, accumulate);
+        return r ? r : launch_manifold<K, J>(c, sel);
+      });
+    });
     // always join here: the inertial Jacobians were produced on the MAIN stream, so the J^T J kernels that follow
     // (enqueue_build) must not run on a still-forked side stream
     { const int rj = join_side(c); if (!rc) rc = rj; }
@@ -578,15 +612,14 @@ int enqueue_evaluate(hb200_ctx* c, bool want_J, int sel, bool accumulate = false
   }
   // visual factors on the main stream, inertial + manifold factors concurrently on the side stream
   if (c->Nv && (c->Ni || c->Nm) && (rc = fork_side(c))) return rc;
-  if (accumulate) {   // fused path: pixel J^T J is accumulated by the factor kernel itself
-    rc = (c->k == 4) ? launch_pixel<4, true>(c, sel, true) : launch_pixel<6, true>(c, sel, true);
-    if (!rc) rc = (c->k == 4) ? launch_inertial<4, true>(c, sel) : launch_inertial<6, true>(c, sel);
-    if (!rc) rc = enqueue_manifold(c, true, sel);
-  } else {
-    if (c->k == 4) { rc = want_J ? launch_pixel<4, true>(c, sel) : launch_pixel<4, false>(c, sel); if (!rc) rc = want_J ? launch_inertial<4, true>(c, sel) : launch_inertial<4, false>(c, sel); }
-    else { rc = want_J ? launch_pixel<6, true>(c, sel) : launch_pixel<6, false>(c, sel); if (!rc) rc = want_J ? launch_inertial<6, true>(c, sel) : launch_inertial<6, false>(c, sel); }
-    if (!rc) rc = enqueue_manifold(c, want_J, sel);
-  }
+  // accumulate (fused path): the pixel J^T J is accumulated by the factor kernel itself
+  rc = with_order(c->k, [&](auto K) {
+    return with_flag(J_any, [&](auto J) {
+      int r = launch_pixel<K, J>(c, sel, accumulate);
+      if (!r) r = launch_inertial<K, J>(c, sel);
+      return r ? r : launch_manifold<K, J>(c, sel);
+    });
+  });
   if (rc || !keep_fork) { const int rj = join_side(c); if (!rc) rc = rj; }
   return rc;
 }
@@ -606,27 +639,24 @@ int enqueue_build(hb200_ctx* c, const SolverState* st) {
     // (order 6 keeps 12-factor chunks at ~2 CTAs per SM, which beat 8-factor chunks at ~6 CTAs per SM on the order-6 window)
     const int splits = (scalar_hess || c->k != 4) ? c->imu_splits : c->imu_splits_mma;
     const int grid = c->nruns * splits;
-    if (scalar_hess) {
-      if (c->k == 4)
-        inertial_hessian_kernel<4, 4><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->i_idx.p, c->i_r.p, c->i_Jp.p, c->i_wg.p, c->i_wa.p,
+    const int rc = with_order(c->k, [&](auto K) {
+      if (scalar_hess)
+        inertial_hessian_kernel<K, 4><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->i_idx.p, c->i_r.p, c->i_Jp.p, c->i_wg.p, c->i_wa.p,
                                                                           c->i_Jg.p, c->imu_scale, c->assembly(), c->lay, c->o_bg(), c->o_ba(), c->o_g(), c->imu_splits);
       else
-        inertial_hessian_kernel<6, 4><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->i_idx.p, c->i_r.p, c->i_Jp.p, c->i_wg.p, c->i_wa.p,
-                                                                          c->i_Jg.p, c->imu_scale, c->assembly(), c->lay, c->o_bg(), c->o_ba(), c->o_g(), c->imu_splits);
-    } else {
-#define HB_IMU_MMA(KK, CHH) inertial_hessian_mma_kernel<KK, 4, CHH><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->i_idx.p, c->i_r.p, c->i_Jp.p, c->i_wg.p, c->i_wa.p, \
-                                                    c->i_Jg.p, c->imu_scale, c->assembly(), c->lay, c->o_bg(), c->o_ba(), c->o_g(), splits)
-      if (c->k == 4) HB_IMU_MMA(4, 8);
-      else HB_IMU_MMA(6, 12);
-#undef HB_IMU_MMA
-    }
-    HB_LAUNCH(c, scalar_hess ? "inertial_hessian_kernel" : "inertial_hessian_mma_kernel");
+        inertial_hessian_mma_kernel<K, 4, K == 4 ? 8 : 12><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->i_idx.p, c->i_r.p, c->i_Jp.p, c->i_wg.p, c->i_wa.p,
+                                                                                              c->i_Jg.p, c->imu_scale, c->assembly(), c->lay, c->o_bg(), c->o_ba(), c->o_g(), splits);
+      return check_launch(c, scalar_hess ? "inertial_hessian_kernel" : "inertial_hessian_mma_kernel");
+    });
+    if (rc) return rc;
   }
   if (c->Nm) {
     const int blocks = (c->Nm + kManWarps - 1) / kManWarps;
-    if (c->k == 4) manifold_hessian_kernel<4><<<blocks, kManWarps * 32, 0, side(c)>>>(c->Nm, c->m_idx.p, c->m_r.p, c->m_Jp.p, c->assembly(), c->lay);
-    else manifold_hessian_kernel<6><<<blocks, kManWarps * 32, 0, side(c)>>>(c->Nm, c->m_idx.p, c->m_r.p, c->m_Jp.p, c->assembly(), c->lay);
-    HB_LAUNCH(c, "manifold_hessian_kernel");
+    const int rc = with_order(c->k, [&](auto K) {
+      manifold_hessian_kernel<K><<<blocks, kManWarps * 32, 0, side(c)>>>(c->Nm, c->m_idx.p, c->m_r.p, c->m_Jp.p, c->assembly(), c->lay);
+      return check_launch(c, "manifold_hessian_kernel");
+    });
+    if (rc) return rc;
   }
   if (c->forked) {   // the cost partials of the visual factors come from the main stream
     HB_CUDA(cudaEventRecord(c->ev_mid, c->stream));
@@ -636,22 +666,20 @@ int enqueue_build(hb200_ctx* c, const SolverState* st) {
   HB_LAUNCH(c, "cost_kernel");
   if (c->Nv && c->L && c->schur_groups) {
     const size_t smem = (3 * static_cast<size_t>(kSchurGroup) * (c->schur_rt + 1) + 3 * kSchurGroup + 4 * 3 * static_cast<size_t>(c->schur_rt)) * sizeof(double);
-    if (c->k == 4)
-      schur_group_kernel<4><<<c->n_lm_groups, kSchurGThreads, smem, c->stream>>>(c->lm_group_off.p, c->lm_order.p, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p, c->v_Jp.p,
+    const int rc = with_order(c->k, [&](auto K) {
+      schur_group_kernel<K><<<c->n_lm_groups, kSchurGThreads, smem, c->stream>>>(c->lm_group_off.p, c->lm_order.p, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p, c->v_Jp.p,
                                                                                  c->v_Jl.p, c->v_w.p, st, c->assembly(), c->lay, c->Vchol.p, c->gl.p, c->Dl.p, c->schur_rt);
-    else
-      schur_group_kernel<6><<<c->n_lm_groups, kSchurGThreads, smem, c->stream>>>(c->lm_group_off.p, c->lm_order.p, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p, c->v_Jp.p,
-                                                                                 c->v_Jl.p, c->v_w.p, st, c->assembly(), c->lay, c->Vchol.p, c->gl.p, c->Dl.p, c->schur_rt);
-    HB_LAUNCH(c, "schur_group_kernel");
+      return check_launch(c, "schur_group_kernel");
+    });
+    if (rc) return rc;
   } else if (c->Nv && c->L) {
     const size_t smem = 2 * 3 * static_cast<size_t>(c->max_rows) * sizeof(double);
-    if (c->k == 4)
-      schur_kernel<4><<<c->L, kSchurThreads, smem, c->stream>>>(c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p, st,
+    const int rc = with_order(c->k, [&](auto K) {
+      schur_kernel<K><<<c->L, kSchurThreads, smem, c->stream>>>(c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p, st,
                                                                 c->assembly(), c->lay, c->Vchol.p, c->gl.p, c->Dl.p, c->max_rows);
-    else
-      schur_kernel<6><<<c->L, kSchurThreads, smem, c->stream>>>(c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p, st,
-                                                                c->assembly(), c->lay, c->Vchol.p, c->gl.p, c->Dl.p, c->max_rows);
-    HB_LAUNCH(c, "schur_kernel");
+      return check_launch(c, "schur_kernel");
+    });
+    if (rc) return rc;
   }
   return join_side(c);
 }
@@ -714,13 +742,12 @@ int enqueue_solve(hb200_ctx* c, bool fuse_retract = false, bool* fused = nullptr
         extra = (std::max(std::max(c->K, 1), std::max(c->Kbg, c->Kba)) + kLmWarps * 32 - 1) / (kLmWarps * 32);
         if (fused) *fused = true;
       }
-      if (c->k == 4)
-        lm_backsub_kernel<4><<<c->n_lm_blocks + extra, kLmWarps * 32, 0, c->stream>>>(c->L, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p,
+      const int rc = with_order(c->k, [&](auto K) {
+        lm_backsub_kernel<K><<<c->n_lm_blocks + extra, kLmWarps * 32, 0, c->stream>>>(c->L, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p,
                                                                                  c->Vchol.p, c->gl.p, c->Dl.p, c->dp.p, c->dl.p, c->lm_part.p, c->lms[0].p, c->lms[1].p, c->n_lm_blocks, ra);
-      else
-        lm_backsub_kernel<6><<<c->n_lm_blocks + extra, kLmWarps * 32, 0, c->stream>>>(c->L, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p,
-                                                                                 c->Vchol.p, c->gl.p, c->Dl.p, c->dp.p, c->dl.p, c->lm_part.p, c->lms[0].p, c->lms[1].p, c->n_lm_blocks, ra);
-      HB_LAUNCH(c, "lm_backsub_kernel");
+        return check_launch(c, "lm_backsub_kernel");
+      });
+      if (rc) return rc;
     } else {
       HB_CUDA(cudaMemsetAsync(c->dl.p, 0, 3 * static_cast<size_t>(c->L) * sizeof(double), c->stream));
       HB_CUDA(cudaMemsetAsync(c->lm_part.p, 0, 5 * static_cast<size_t>(c->n_lm_blocks) * sizeof(double), c->stream));
@@ -764,11 +791,12 @@ TermArgs term_args(hb200_ctx* c) {
 int enqueue_accept(hb200_ctx* c) {
   ScalarArgs sa{c->cp_pix[1].p, c->Nv ? c->n_pix_blocks : 0, c->cp_imu[1].p, c->n_imu_blocks + c->n_man_blocks, c->lm_part.p, (c->L && c->Nv) ? c->n_lm_blocks : 0};
   CommitArgs a{};
-  const size_t counts[5] = {8 * static_cast<size_t>(c->K), 4 * static_cast<size_t>(c->Kbg), 4 * static_cast<size_t>(c->Kba), 3, 3 * static_cast<size_t>(c->L)};
-  const double* srcs[5] = {c->knots[1].p, c->bg[1].p, c->ba[1].p, c->grav[1].p, c->lms[1].p};
-  double* dsts[5] = {c->knots[0].p, c->bg[0].p, c->ba[0].p, c->grav[0].p, c->lms[0].p};
+  const auto blocks = c->state_blocks();
   size_t mx = 1, total = 0;
-  for (int i = 0; i < 5; ++i) { a.count[i] = counts[i]; a.src[i] = srcs[i]; a.dst[i] = dsts[i]; mx = std::max(mx, counts[i]); total += counts[i]; }
+  for (int i = 0; i < 5; ++i) {
+    a.count[i] = blocks[i].count; a.src[i] = blocks[i].trial->p; a.dst[i] = blocks[i].cur->p;
+    mx = std::max(mx, blocks[i].count); total += blocks[i].count;
+  }
   const bool fuse_commit = total <= 65536;   // small windows: one CTA commits the accepted state right away
   // scalars: summed inside this kernel on one GPU and, across GPUs, exchanged by it through peer memory; only the
   // fallbacks (callback hook, no peer mapping) run scalars_kernel + a second reduction before it
@@ -862,7 +890,7 @@ int sync_layout(hb200_ctx* c) {
     c->min_beta = v;
     const int rc = ensure_system(c);
     if (rc) return rc;
-    c->invalidate();
+    c->kernel_args_changed();
   }
   return 0;
 }
@@ -962,15 +990,6 @@ void hb200_destroy(hb200_ctx* c) {
   if (c->nccl && c->own_nccl && g_nccl.CommDestroy) g_nccl.CommDestroy(c->nccl);
   c->nccl = nullptr;
   for (cudaEvent_t e : c->prof_events) cudaEventDestroy(e);
-  for (int s = 0; s < 2; ++s) { c->knots[s].release(); c->bg[s].release(); c->ba[s].release(); c->grav[s].release(); c->lms[s].release(); c->tab[s].release(); c->cp_pix[s].release(); c->cp_imu[s].release(); }
-  c->cams.release(); c->imu.release(); c->cam_tab.release(); c->imu_tab.release(); c->fixed.release();
-  c->v_stamp.release(); c->v_pixel.release(); c->i_stamp.release(); c->i_meas.release(); c->v_idx.release(); c->i_idx.release();
-  c->v_z.release(); c->v_w.release(); c->m_stamp.release(); c->m_meas.release(); c->sensors.release(); c->m_sensor.release(); c->m_idx.release(); c->m_r.release(); c->m_Jp.release();
-  c->run_off.release(); c->lm_off.release(); c->lm_obs.release(); c->d_invalid.release(); c->lm_order.release(); c->lm_group_off.release();
-  c->v_r.release(); c->v_Jp.release(); c->v_Jl.release(); c->i_r.release(); c->i_Jp.release(); c->i_wg.release(); c->i_wa.release(); c->i_Jg.release();
-  c->sys.release(); c->D.release(); c->Lw.release(); c->Ldiag.release(); c->dp.release(); c->dl.release(); c->Vchol.release(); c->gl.release(); c->Dl.release();
-  c->band_ws.release(); c->band_dbg.release(); c->bcr_ws.release(); c->bcr_bar.release(); c->lm_part.release(); c->scal.release(); c->spd.release(); c->st.release(); c->records.release();
-  c->snap_knots.release(); c->snap_bg.release(); c->snap_ba.release(); c->snap_grav.release(); c->snap_lms.release(); c->snap_st.release();
   if (c->h_stage) cudaFreeHost(c->h_stage);
   c->d_stage.release();
   if (c->ev_fork) cudaEventDestroy(c->ev_fork);
@@ -1012,8 +1031,8 @@ int hb200_set_spline(hb200_ctx* c, int order, int K, const double* knots) {
   for (int s = 0; s < 2; ++s) { HB_CUDA(c->knots[s].ensure(8 * static_cast<size_t>(K))); HB_CUDA(c->tab[s].ensure(static_cast<size_t>(K) * kTabStride)); }
   HB_CUDA(cudaMemcpyAsync(c->knots[0].p, knots, 8 * sizeof(double) * K, cudaMemcpyHostToDevice, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
-  if (reshape) { c->h_knot_const.assign(K, 0); c->bound = false; c->invalidate(); c->have_snapshot = false; int rc = update_fixed(c); if (rc) return rc; }
-  c->evaluated_J = false; c->system_built = false; c->cov_built = false; c->mirror_valid = false; c->calib_valid = false;
+  if (reshape) { c->h_knot_const.assign(K, 0); c->bound = false; c->kernel_args_changed(); c->have_snapshot = false; int rc = update_fixed(c); if (rc) return rc; }
+  c->outputs_changed();
   return 0;
 }
 
@@ -1044,8 +1063,8 @@ int hb200_set_bias_splines(hb200_ctx* c, int order, int Kg, const double* gyro, 
   HB_CUDA(cudaMemcpyAsync(c->bg[0].p, gyro, 4 * sizeof(double) * Kg, cudaMemcpyHostToDevice, c->stream));
   HB_CUDA(cudaMemcpyAsync(c->ba[0].p, accel, 4 * sizeof(double) * Ka, cudaMemcpyHostToDevice, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
-  if (reshape) { c->bound = false; c->invalidate(); c->have_snapshot = false; int rc = update_fixed(c); if (rc) return rc; }
-  c->evaluated_J = false; c->system_built = false; c->cov_built = false; c->mirror_valid = false; c->calib_valid = false;
+  if (reshape) { c->bound = false; c->kernel_args_changed(); c->have_snapshot = false; int rc = update_fixed(c); if (rc) return rc; }
+  c->outputs_changed();
   return 0;
 }
 
@@ -1055,14 +1074,14 @@ int hb200_set_gravity(hb200_ctx* c, const double* g) {
   HB_CUDA(cudaMemcpyAsync(c->grav[0].p, g, 3 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
   c->have_gravity = true;
-  c->evaluated_J = false; c->system_built = false; c->cov_built = false; c->mirror_valid = false; c->calib_valid = false;
+  c->outputs_changed();
   return 0;
 }
 
 int hb200_set_cameras(hb200_ctx* c, int C, const double* cams) {
   if (!c || !cams || C <= 0) return fail(-1, "invalid cameras");
   HB_CUDA(cudaSetDevice(c->device));
-  if (C != c->C) { c->bound = false; c->invalidate(); }
+  if (C != c->C) { c->bound = false; c->kernel_args_changed(); }
   c->C = C;
   HB_CUDA(c->cams.ensure(15 * static_cast<size_t>(C)));
   HB_CUDA(c->cam_tab.ensure(kCamStride * static_cast<size_t>(C)));
@@ -1070,7 +1089,7 @@ int hb200_set_cameras(hb200_ctx* c, int C, const double* cams) {
   calib_kernel<<<(C + 63) / 64, 64, 0, c->stream>>>(C, c->cams.p, c->cam_tab.p, nullptr, nullptr, 0);
   HB_LAUNCH(c, "calib_kernel");
   HB_CUDA(cudaStreamSynchronize(c->stream));
-  c->evaluated_J = false; c->system_built = false; c->cov_built = false; c->mirror_valid = false; c->calib_valid = false;
+  c->outputs_changed();
   return 0;
 }
 
@@ -1083,19 +1102,19 @@ int hb200_set_imu(hb200_ctx* c, const double* imu) {
   HB_LAUNCH(c, "calib_kernel");
   HB_CUDA(cudaStreamSynchronize(c->stream));
   c->have_imu = true;
-  c->evaluated_J = false; c->system_built = false; c->cov_built = false; c->mirror_valid = false; c->calib_valid = false;
+  c->outputs_changed();
   return 0;
 }
 
 int hb200_set_landmarks(hb200_ctx* c, int L, const double* xyz) {
   if (!c || (L > 0 && !xyz) || L < 0) return fail(-1, "invalid landmarks");
   HB_CUDA(cudaSetDevice(c->device));
-  if (L != c->L) { c->bound = false; c->invalidate(); c->have_snapshot = false; }
+  if (L != c->L) { c->bound = false; c->kernel_args_changed(); c->have_snapshot = false; }
   c->L = L;
   for (int s = 0; s < 2; ++s) HB_CUDA(c->lms[s].ensure(3 * static_cast<size_t>(std::max(L, 1))));
   if (L) HB_CUDA(cudaMemcpyAsync(c->lms[0].p, xyz, 3 * sizeof(double) * L, cudaMemcpyHostToDevice, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
-  c->evaluated_J = false; c->system_built = false; c->cov_built = false; c->mirror_valid = false; c->calib_valid = false;
+  c->outputs_changed();
   return 0;
 }
 
@@ -1106,7 +1125,7 @@ int hb200_set_constant(hb200_ctx* c, const unsigned char* knot_constant, int gra
   if (knot_constant) c->h_knot_const.assign(knot_constant, knot_constant + c->K);
   else c->h_knot_const.assign(c->K, 0);
   c->gravity_const = gravity_constant; c->bias_const = bias_constant;
-  c->system_built = false; c->cov_built = false;
+  c->system_changed();
   return update_fixed(c);
 }
 
@@ -1120,7 +1139,7 @@ int hb200_set_reference_quirks(hb200_ctx* c, int quirks) {
     HB_LAUNCH(c, "calib_kernel");
     HB_CUDA(cudaStreamSynchronize(c->stream));
   }
-  c->evaluated_J = false; c->system_built = false; c->cov_built = false; c->mirror_valid = false; c->calib_valid = false;
+  c->outputs_changed();
   return 0;
 }
 
@@ -1130,7 +1149,7 @@ int hb200_set_options(hb200_ctx* c, double huber_pixel, double imu_loss_scale, d
   HB_CUDA(cudaSetDevice(c->device));
   if (huber_pixel != c->huber || imu_loss_scale != c->imu_scale) c->graph_valid = false;  // baked into kernel arguments
   c->huber = huber_pixel; c->imu_scale = imu_loss_scale; c->radius0 = radius;
-  c->system_built = false; c->cov_built = false; c->evaluated_J = false;
+  c->outputs_changed();
   return reset_solver_state(c);
 }
 
@@ -1152,7 +1171,7 @@ void visual_user_order(hb200_ctx* c) {
 }
 void rebuild_visual(hb200_ctx* c) {
   visual_user_order(c);
-  c->bound = false; c->invalidate();
+  c->bound = false; c->kernel_args_changed();
 }
 }  // namespace
 
@@ -1179,7 +1198,7 @@ int hb200_set_bearing_loss(hb200_ctx* c, double huber_bearing) {
   if (!(huber_bearing > 0)) return fail(-1, "options must be positive");
   if (huber_bearing != c->huber_bearing) c->graph_valid = false;
   c->huber_bearing = huber_bearing;
-  c->system_built = false; c->cov_built = false; c->evaluated_J = false;
+  c->outputs_changed();
   return 0;
 }
 
@@ -1192,7 +1211,7 @@ int hb200_set_pose_sensors(hb200_ctx* c, int n, const double* T_bs) {
   HB_CUDA(c->sensors.ensure(7 * static_cast<size_t>(std::max(n, 1))));
   if (n) HB_CUDA(cudaMemcpyAsync(c->sensors.p, c->h_sensors.data(), sizeof(double) * 7 * n, cudaMemcpyHostToDevice, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
-  c->invalidate();
+  c->kernel_args_changed();
   return 0;
 }
 
@@ -1200,7 +1219,7 @@ int hb200_set_manifold_factors(hb200_ctx* c, int n, const double* stamp, const i
   if (!c || n < 0 || (n > 0 && (!stamp || !sensor || !pose))) return fail(-1, "invalid manifold factors");
   c->Nm = n;
   c->h_m_stamp.assign(stamp, stamp + n); c->h_m_sensor.assign(sensor, sensor + n); c->h_m_meas.assign(pose, pose + 7 * static_cast<size_t>(n));
-  c->bound = false; c->invalidate();
+  c->bound = false; c->kernel_args_changed();
   return 0;
 }
 
@@ -1208,7 +1227,7 @@ int hb200_set_inertial_factors(hb200_ctx* c, int n, const double* stamp, const d
   if (!c || n < 0 || (n > 0 && (!stamp || !meas))) return fail(-1, "invalid inertial factors");
   c->Ni = n;
   c->h_i_stamp.assign(stamp, stamp + n); c->h_i_meas.assign(meas, meas + 6 * static_cast<size_t>(n));
-  c->bound = false; c->invalidate();
+  c->bound = false; c->kernel_args_changed();
   return 0;
 }
 
@@ -1330,7 +1349,7 @@ int derive_window(hb200_ctx* c) {
   if ((rc = ensure_system(c))) return rc;
   HB_CUDA(cudaStreamSynchronize(c->stream));
   c->bound = true;
-  c->invalidate();
+  c->kernel_args_changed();
   return sync_layout(c);   // multi-GPU: all ranks adopt the widest band (collective when a communicator is attached)
 }
 
@@ -1502,8 +1521,8 @@ int hb200_evaluate(hb200_ctx* c, int flags) {
   const int sel = (flags & HB200_EVAL_TRIAL) ? 1 : 0;
   rc = enqueue_evaluate(c, J, sel);
   if (rc) return rc;
+  c->outputs_changed();
   c->evaluated_J = J && sel == 0;   // a trial-state sweep overwrites the residual / Jacobian buffers
-  c->mirror_valid = false; c->calib_valid = false; c->system_built = false; c->cov_built = false;
   return 0;
 }
 
@@ -1613,25 +1632,31 @@ int ensure_calib_mirror(hb200_ctx* c) {
   if (Nv) {
     HB_CUDA(dv.ensure(28 * Nv));
     const int blocks = static_cast<int>((Nv + kEvalThreads - 1) / kEvalThreads);
-    if (c->k == 4) pixel_calib_kernel<4><<<blocks, kEvalThreads, 0, c->stream>>>(c->Nv, c->v_stamp.p, reinterpret_cast<const double2*>(c->v_pixel.p), c->v_z.p, c->v_idx.p, c->tab[0].p, c->cam_tab.p, c->lms[0].p, c->basis, dv.p);
-    else pixel_calib_kernel<6><<<blocks, kEvalThreads, 0, c->stream>>>(c->Nv, c->v_stamp.p, reinterpret_cast<const double2*>(c->v_pixel.p), c->v_z.p, c->v_idx.p, c->tab[0].p, c->cam_tab.p, c->lms[0].p, c->basis, dv.p);
-    HB_LAUNCH(c, "pixel_calib_kernel");
+    const int rc = with_order(c->k, [&](auto K) {
+      pixel_calib_kernel<K><<<blocks, kEvalThreads, 0, c->stream>>>(c->Nv, c->v_stamp.p, reinterpret_cast<const double2*>(c->v_pixel.p), c->v_z.p, c->v_idx.p, c->tab[0].p, c->cam_tab.p, c->lms[0].p, c->basis, dv.p);
+      return check_launch(c, "pixel_calib_kernel");
+    });
+    if (rc) return rc;
     HB_CUDA(cudaMemcpyAsync(tv.data(), dv.p, sizeof(double) * 28 * Nv, cudaMemcpyDeviceToHost, c->stream));
   }
   if (Ni) {
     HB_CUDA(di.ensure(216 * Ni));
     const int blocks = static_cast<int>((Ni + kEvalThreads - 1) / kEvalThreads);
-    if (c->k == 4) inertial_calib_kernel<4><<<blocks, kEvalThreads, 0, c->stream>>>(c->Ni, c->i_stamp.p, c->i_idx.p, c->tab[0].p, c->imu.p, c->grav[0].p, c->basis, c->quirks, di.p);
-    else inertial_calib_kernel<6><<<blocks, kEvalThreads, 0, c->stream>>>(c->Ni, c->i_stamp.p, c->i_idx.p, c->tab[0].p, c->imu.p, c->grav[0].p, c->basis, c->quirks, di.p);
-    HB_LAUNCH(c, "inertial_calib_kernel");
+    const int rc = with_order(c->k, [&](auto K) {
+      inertial_calib_kernel<K><<<blocks, kEvalThreads, 0, c->stream>>>(c->Ni, c->i_stamp.p, c->i_idx.p, c->tab[0].p, c->imu.p, c->grav[0].p, c->basis, c->quirks, di.p);
+      return check_launch(c, "inertial_calib_kernel");
+    });
+    if (rc) return rc;
     HB_CUDA(cudaMemcpyAsync(ti.data(), di.p, sizeof(double) * 216 * Ni, cudaMemcpyDeviceToHost, c->stream));
   }
   if (Nm) {
     HB_CUDA(dm.ensure(36 * Nm));
     const int blocks = static_cast<int>((Nm + kEvalThreads - 1) / kEvalThreads);
-    if (c->k == 4) manifold_calib_kernel<4><<<blocks, kEvalThreads, 0, c->stream>>>(c->Nm, c->m_stamp.p, c->m_meas.p, c->m_idx.p, c->tab[0].p, c->sensors.p, c->basis, dm.p);
-    else manifold_calib_kernel<6><<<blocks, kEvalThreads, 0, c->stream>>>(c->Nm, c->m_stamp.p, c->m_meas.p, c->m_idx.p, c->tab[0].p, c->sensors.p, c->basis, dm.p);
-    HB_LAUNCH(c, "manifold_calib_kernel");
+    const int rc = with_order(c->k, [&](auto K) {
+      manifold_calib_kernel<K><<<blocks, kEvalThreads, 0, c->stream>>>(c->Nm, c->m_stamp.p, c->m_meas.p, c->m_idx.p, c->tab[0].p, c->sensors.p, c->basis, dm.p);
+      return check_launch(c, "manifold_calib_kernel");
+    });
+    if (rc) return rc;
     HB_CUDA(cudaMemcpyAsync(c->m_m_Jc.data(), dm.p, sizeof(double) * 36 * Nm, cudaMemcpyDeviceToHost, c->stream));
   }
   HB_CUDA(cudaStreamSynchronize(c->stream));
@@ -1846,8 +1871,8 @@ int hb200_build_covariance(hb200_ctx* c) {
   c->cov_lay_next = c->lay; c->cov_basis_next = c->basis; c->cov_L_next = c->L;
   c->cov_k_next = c->k; c->cov_Nv_next = c->Nv; c->cov_max_rows_next = c->max_rows;
   // the factor outputs are those of an evaluation at the current state; the packed buffer is not what hb200_solve expects
-  c->evaluated_J = true; c->system_built = false; c->cov_built = false; c->mirror_valid = false; c->calib_valid = false;
-  c->cov_built = true;
+  c->outputs_changed();
+  c->evaluated_J = true; c->cov_built = true;
   c->cov_at = c->launches;
   return 0;
 }
@@ -1881,13 +1906,12 @@ int hb200_compute_covariance(hb200_ctx* c, hb200_covariance_info* info) {
   if (L && c->cov_Nv_next) {
     const int blocks = (L + kLmWarps - 1) / kLmWarps;
     const size_t lsmem = static_cast<size_t>(kLmWarps) * 3 * max_rows * sizeof(double);
-    if (k == 4)
-      cov_landmark_kernel<4><<<blocks, kLmWarps * 32, lsmem, c->stream>>>(L, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p, c->Vchol.p,
+    rc = with_order(k, [&](auto K) {
+      cov_landmark_kernel<K><<<blocks, kLmWarps * 32, lsmem, c->stream>>>(L, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p, c->Vchol.p,
                                                                          c->cov_packed_next.p, lay, c->cov_status.p, c->cov_lm_next.p, max_rows);
-    else
-      cov_landmark_kernel<6><<<blocks, kLmWarps * 32, lsmem, c->stream>>>(L, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p, c->Vchol.p,
-                                                                         c->cov_packed_next.p, lay, c->cov_status.p, c->cov_lm_next.p, max_rows);
-    HB_LAUNCH(c, "cov_landmark_kernel");
+      return check_launch(c, "cov_landmark_kernel");
+    });
+    if (rc) return rc;
   } else if (L) {
     HB_CUDA(cudaMemsetAsync(c->cov_lm_next.p, 0, sizeof(double) * 9 * L, c->stream));
   }
@@ -1943,11 +1967,11 @@ int hb200_interpolate_covariance(hb200_ctx* c, int n, const double* stamps, doub
   HB_CUDA(d_t.ensure(n)); HB_CUDA(d_o.ensure(36 * static_cast<size_t>(n))); HB_CUDA(d_bad.ensure(n));
   HB_CUDA(cudaMemcpyAsync(d_t.p, stamps, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
   const SysLayout& lay = c->cov_lay;
-  if (c->cov_basis.k == 4)
-    cov_interpolate_kernel<4><<<(n + 127) / 128, 128, 0, c->stream>>>(n, d_t.p, c->cov_knots.p, c->cov_tab.p, lay.K, c->cov_basis, c->cov_packed.p, lay, d_o.p, d_bad.p);
-  else
-    cov_interpolate_kernel<6><<<(n + 127) / 128, 128, 0, c->stream>>>(n, d_t.p, c->cov_knots.p, c->cov_tab.p, lay.K, c->cov_basis, c->cov_packed.p, lay, d_o.p, d_bad.p);
-  HB_LAUNCH(c, "cov_interpolate_kernel");
+  rc = with_order(c->cov_basis.k, [&](auto K) {
+    cov_interpolate_kernel<K><<<(n + 127) / 128, 128, 0, c->stream>>>(n, d_t.p, c->cov_knots.p, c->cov_tab.p, lay.K, c->cov_basis, c->cov_packed.p, lay, d_o.p, d_bad.p);
+    return check_launch(c, "cov_interpolate_kernel");
+  });
+  if (rc) return rc;
   std::vector<int> bad(n);
   HB_CUDA(cudaMemcpyAsync(cov, d_o.p, sizeof(double) * 36 * n, cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaMemcpyAsync(bad.data(), d_bad.p, sizeof(int) * n, cudaMemcpyDeviceToHost, c->stream));
@@ -1973,7 +1997,7 @@ int iterate_enqueue(hb200_ctx* c, int iterations) {
       cudaGraph_t& graph = slot_b ? c->graph_b : c->graph;
       cudaGraphExec_t& exec = slot_b ? c->graph_exec_b : c->graph_exec;
       bool& valid = slot_b ? c->graph_b_valid : c->graph_valid;
-      if (!c->graph_valid) c->graph_b_valid = false;   // (invalidate() only knows the first slot)
+      if (!c->graph_valid) c->graph_b_valid = false;   // (kernel_args_changed() only knows the first slot)
       if (!valid) {
         if (exec) { cudaGraphExecDestroy(exec); exec = nullptr; }
         if (graph) { cudaGraphDestroy(graph); graph = nullptr; }
@@ -2021,7 +2045,7 @@ int iterate_enqueue(hb200_ctx* c, int iterations) {
       if (c->nccl) c->comm_warm = true;
     }
   }
-  c->evaluated_J = false; c->system_built = false; c->cov_built = false; c->mirror_valid = false; c->calib_valid = false;
+  c->outputs_changed();
   if (!c->term_enabled) c->iter_total += iterations;   // (with the termination tests on, the device counter is authoritative: pick_records)
   return 0;
 }
@@ -2099,11 +2123,15 @@ int hb200_optimize(hb200_ctx* c, int iterations, double* knots, double* gyro, do
   if (knots) for (int j = 0; j < c->K; ++j) if (knots[8 * j + 7] != c->h_knot_stamp[j]) return fail(-2, "knot %d: stamp differs from the bound window (re-bind after changing stamps)", j);
   if (gyro) for (int j = 0; j < c->Kbg; ++j) if (gyro[4 * j + 3] != c->h_bg_stamp[j]) return fail(-2, "gyroscope bias knot %d: stamp differs from the bound window", j);
   if (accel) for (int j = 0; j < c->Kba; ++j) if (accel[4 * j + 3] != c->h_ba_stamp[j]) return fail(-2, "accelerometer bias knot %d: stamp differs from the bound window", j);
-  double* host[5] = {knots, (gyro && c->Kbg) ? gyro : nullptr, (accel && c->Kba) ? accel : nullptr, gravity, (landmarks && c->L) ? landmarks : nullptr};
-  double* dev[5] = {c->knots[0].p, c->bg[0].p, c->ba[0].p, c->grav[0].p, c->lms[0].p};
-  const size_t cnt[5] = {8 * static_cast<size_t>(c->K), 4 * static_cast<size_t>(c->Kbg), 4 * static_cast<size_t>(c->Kba), 3, 3 * static_cast<size_t>(c->L)};
-  size_t off[5], total = 0;
-  for (int i = 0; i < 5; ++i) { off[i] = total; if (host[i]) total += cnt[i]; }
+  const auto blocks = c->state_blocks();
+  double* host[5] = {knots, gyro, accel, gravity, landmarks};
+  double* dev[5];
+  size_t cnt[5], off[5], total = 0;
+  for (int i = 0; i < 5; ++i) {
+    dev[i] = blocks[i].cur->p; cnt[i] = blocks[i].count;
+    if (!cnt[i]) host[i] = nullptr;   // (an empty block is never copied)
+    off[i] = total; if (host[i]) total += cnt[i];
+  }
   if (gravity) c->have_gravity = true;
   // Small windows: 11 small copies cost more than the iteration's kernels save; pack the blocks into one pinned
   // staging buffer (host memcpy, a few KB), one H2D, one segmented device copy -- and the mirror image back.
@@ -2274,7 +2302,7 @@ int hb200_profile_iteration(hb200_ctx* c, int reps, int max_entries, char* names
     ms[n_out] = acc[i] / reps;
   }
   *count = n_out;
-  c->evaluated_J = false; c->system_built = false; c->cov_built = false; c->mirror_valid = false; c->calib_valid = false;
+  c->outputs_changed();
   return 0;
 }
 
@@ -2293,9 +2321,11 @@ int hb200_interpolate(hb200_ctx* c, int n, const double* stamps, double* pose, d
   HB_CUDA(cudaMemcpyAsync(d_t.p, stamps, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
   prep_kernel<<<(c->K + 63) / 64, 64, 0, c->stream>>>(c->K, c->knots[0].p, c->tab[0].p, nullptr, 0);
   HB_LAUNCH(c, "prep_kernel");
-  if (c->k == 4) interpolate_kernel<4><<<(n + 127) / 128, 128, 0, c->stream>>>(n, d_t.p, c->knots[0].p, c->tab[0].p, c->K, c->basis, d_p.p, d_v.p, d_a.p, c->d_invalid.p);
-  else interpolate_kernel<6><<<(n + 127) / 128, 128, 0, c->stream>>>(n, d_t.p, c->knots[0].p, c->tab[0].p, c->K, c->basis, d_p.p, d_v.p, d_a.p, c->d_invalid.p);
-  HB_LAUNCH(c, "interpolate_kernel");
+  const int rc = with_order(c->k, [&](auto K) {
+    interpolate_kernel<K><<<(n + 127) / 128, 128, 0, c->stream>>>(n, d_t.p, c->knots[0].p, c->tab[0].p, c->K, c->basis, d_p.p, d_v.p, d_a.p, c->d_invalid.p);
+    return check_launch(c, "interpolate_kernel");
+  });
+  if (rc) return rc;
   int bad = 0;
   HB_CUDA(cudaMemcpyAsync(pose, d_p.p, sizeof(double) * 7 * n, cudaMemcpyDeviceToHost, c->stream));
   if (velocity) HB_CUDA(cudaMemcpyAsync(velocity, d_v.p, sizeof(double) * 6 * n, cudaMemcpyDeviceToHost, c->stream));
@@ -2317,14 +2347,11 @@ int hb200_debug_band_timing(hb200_ctx* c, long long* cycles /*[144]: per CTA, 8 
 int hb200_snapshot(hb200_ctx* c) {
   if (!c || c->K == 0) return fail(-2, "spline not set");
   HB_CUDA(cudaSetDevice(c->device));
-  HB_CUDA(c->snap_knots.ensure(8 * static_cast<size_t>(c->K))); HB_CUDA(c->snap_bg.ensure(4 * static_cast<size_t>(std::max(c->Kbg, 1))));
-  HB_CUDA(c->snap_ba.ensure(4 * static_cast<size_t>(std::max(c->Kba, 1)))); HB_CUDA(c->snap_grav.ensure(4)); HB_CUDA(c->snap_lms.ensure(3 * static_cast<size_t>(std::max(c->L, 1))));
+  const auto blocks = c->state_blocks();
+  for (const auto& b : blocks) HB_CUDA(b.snap->ensure(std::max<size_t>(b.count, 1)));
   HB_CUDA(c->snap_st.ensure(1));
-  HB_CUDA(cudaMemcpyAsync(c->snap_knots.p, c->knots[0].p, sizeof(double) * 8 * c->K, cudaMemcpyDeviceToDevice, c->stream));
-  if (c->Kbg) HB_CUDA(cudaMemcpyAsync(c->snap_bg.p, c->bg[0].p, sizeof(double) * 4 * c->Kbg, cudaMemcpyDeviceToDevice, c->stream));
-  if (c->Kba) HB_CUDA(cudaMemcpyAsync(c->snap_ba.p, c->ba[0].p, sizeof(double) * 4 * c->Kba, cudaMemcpyDeviceToDevice, c->stream));
-  HB_CUDA(cudaMemcpyAsync(c->snap_grav.p, c->grav[0].p, sizeof(double) * 3, cudaMemcpyDeviceToDevice, c->stream));
-  if (c->L) HB_CUDA(cudaMemcpyAsync(c->snap_lms.p, c->lms[0].p, sizeof(double) * 3 * c->L, cudaMemcpyDeviceToDevice, c->stream));
+  for (const auto& b : blocks)
+    if (b.count) HB_CUDA(cudaMemcpyAsync(b.snap->p, b.cur->p, sizeof(double) * b.count, cudaMemcpyDeviceToDevice, c->stream));
   HB_CUDA(cudaMemcpyAsync(c->snap_st.p, c->st.p, sizeof(SolverState), cudaMemcpyDeviceToDevice, c->stream));
   c->have_snapshot = true;
   c->snap_iter_total = c->iter_total;
@@ -2334,14 +2361,11 @@ int hb200_snapshot(hb200_ctx* c) {
 int hb200_restore(hb200_ctx* c) {
   if (!c || !c->have_snapshot) return fail(-2, "no snapshot");
   HB_CUDA(cudaSetDevice(c->device));
-  HB_CUDA(cudaMemcpyAsync(c->knots[0].p, c->snap_knots.p, sizeof(double) * 8 * c->K, cudaMemcpyDeviceToDevice, c->stream));
-  if (c->Kbg) HB_CUDA(cudaMemcpyAsync(c->bg[0].p, c->snap_bg.p, sizeof(double) * 4 * c->Kbg, cudaMemcpyDeviceToDevice, c->stream));
-  if (c->Kba) HB_CUDA(cudaMemcpyAsync(c->ba[0].p, c->snap_ba.p, sizeof(double) * 4 * c->Kba, cudaMemcpyDeviceToDevice, c->stream));
-  HB_CUDA(cudaMemcpyAsync(c->grav[0].p, c->snap_grav.p, sizeof(double) * 3, cudaMemcpyDeviceToDevice, c->stream));
-  if (c->L) HB_CUDA(cudaMemcpyAsync(c->lms[0].p, c->snap_lms.p, sizeof(double) * 3 * c->L, cudaMemcpyDeviceToDevice, c->stream));
+  for (const auto& b : c->state_blocks())
+    if (b.count) HB_CUDA(cudaMemcpyAsync(b.cur->p, b.snap->p, sizeof(double) * b.count, cudaMemcpyDeviceToDevice, c->stream));
   HB_CUDA(cudaMemcpyAsync(c->st.p, c->snap_st.p, sizeof(SolverState), cudaMemcpyDeviceToDevice, c->stream));
   c->iter_total = c->snap_iter_total;
-  c->evaluated_J = false; c->system_built = false; c->cov_built = false; c->mirror_valid = false; c->calib_valid = false;
+  c->outputs_changed();
   return 0;
 }
 
@@ -2349,7 +2373,6 @@ int hb200_ingest_stereo(hb200_ctx* c, int n, const double* stamp, const int* cam
                         const double* pixel1, double* bearing0, double* bearing1, double* landmark, int* num_invalid) {
   if (!c || n < 0) return fail(-1, "invalid arguments");
   if (c->K == 0 || c->C == 0) return fail(-2, "spline / cameras not set");
-  if (c->k != 4 && c->k != 6) return fail(-4, "spline order %d not supported (4 or 6)", c->k);
   if (n > 0 && (!stamp || !camera0 || !camera1 || !pixel0 || !pixel1 || !bearing0 || !bearing1 || !landmark)) return fail(-1, "null argument");
   if (num_invalid) *num_invalid = 0;
   if (n == 0) return 0;
@@ -2368,9 +2391,11 @@ int hb200_ingest_stereo(hb200_ctx* c, int n, const double* stamp, const int* cam
   HB_CUDA(cudaMemcpyAsync(d_p1.p, pixel1, sizeof(double) * 2 * N, cudaMemcpyHostToDevice, c->stream));
   prep_kernel<<<(c->K + 63) / 64, 64, 0, c->stream>>>(c->K, c->knots[0].p, c->tab[0].p, nullptr, 0);
   HB_LAUNCH(c, "prep_kernel");
-  if (c->k == 4) ingest_stereo_kernel<4><<<(n + 127) / 128, 128, 0, c->stream>>>(n, d_t.p, d_c0.p, d_c1.p, d_p0.p, d_p1.p, c->knots[0].p, c->tab[0].p, c->K, c->basis, c->cams.p, c->C, d_b0.p, d_b1.p, d_lm.p, c->d_invalid.p);
-  else ingest_stereo_kernel<6><<<(n + 127) / 128, 128, 0, c->stream>>>(n, d_t.p, d_c0.p, d_c1.p, d_p0.p, d_p1.p, c->knots[0].p, c->tab[0].p, c->K, c->basis, c->cams.p, c->C, d_b0.p, d_b1.p, d_lm.p, c->d_invalid.p);
-  HB_LAUNCH(c, "ingest_stereo_kernel");
+  const int rc = with_order(c->k, [&](auto K) {
+    ingest_stereo_kernel<K><<<(n + 127) / 128, 128, 0, c->stream>>>(n, d_t.p, d_c0.p, d_c1.p, d_p0.p, d_p1.p, c->knots[0].p, c->tab[0].p, c->K, c->basis, c->cams.p, c->C, d_b0.p, d_b1.p, d_lm.p, c->d_invalid.p);
+    return check_launch(c, "ingest_stereo_kernel");
+  });
+  if (rc) return rc;
   int bad = 0;
   HB_CUDA(cudaMemcpyAsync(bearing0, d_b0.p, sizeof(double) * 3 * N, cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaMemcpyAsync(bearing1, d_b1.p, sizeof(double) * 3 * N, cudaMemcpyDeviceToHost, c->stream));
@@ -2385,11 +2410,10 @@ int hb200_ingest_stereo(hb200_ctx* c, int n, const double* stamp, const int* cam
 int hb200_get_state(hb200_ctx* c, double* knots, double* gyro, double* accel, double* gravity, double* landmarks) {
   if (!c) return fail(-1, "null context");
   HB_CUDA(cudaSetDevice(c->device));
-  if (knots && c->K) HB_CUDA(cudaMemcpyAsync(knots, c->knots[0].p, sizeof(double) * 8 * c->K, cudaMemcpyDeviceToHost, c->stream));
-  if (gyro && c->Kbg) HB_CUDA(cudaMemcpyAsync(gyro, c->bg[0].p, sizeof(double) * 4 * c->Kbg, cudaMemcpyDeviceToHost, c->stream));
-  if (accel && c->Kba) HB_CUDA(cudaMemcpyAsync(accel, c->ba[0].p, sizeof(double) * 4 * c->Kba, cudaMemcpyDeviceToHost, c->stream));
-  if (gravity) HB_CUDA(cudaMemcpyAsync(gravity, c->grav[0].p, sizeof(double) * 3, cudaMemcpyDeviceToHost, c->stream));
-  if (landmarks && c->L) HB_CUDA(cudaMemcpyAsync(landmarks, c->lms[0].p, sizeof(double) * 3 * c->L, cudaMemcpyDeviceToHost, c->stream));
+  double* host[5] = {knots, gyro, accel, gravity, landmarks};
+  const auto blocks = c->state_blocks();
+  for (int i = 0; i < 5; ++i)
+    if (host[i] && blocks[i].count) HB_CUDA(cudaMemcpyAsync(host[i], blocks[i].cur->p, sizeof(double) * blocks[i].count, cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
   return 0;
 }
@@ -2458,7 +2482,7 @@ int hb200_append_knots(hb200_ctx* c, int count) {
   if ((rc = update_fixed(c))) return rc;
   if ((rc = ensure_system(c))) return rc;
   HB_CUDA(cudaStreamSynchronize(c->stream));
-  c->invalidate(); c->have_snapshot = false;
+  c->kernel_args_changed(); c->have_snapshot = false;
   return sync_layout(c);
 }
 
@@ -2531,7 +2555,7 @@ int hb200_append_bias_knots(hb200_ctx* c, double stamp, int* gyro_added, int* ac
   if ((rc = update_fixed(c))) return rc;
   if ((rc = ensure_system(c))) return rc;
   HB_CUDA(cudaStreamSynchronize(c->stream));
-  c->invalidate(); c->have_snapshot = false;
+  c->kernel_args_changed(); c->have_snapshot = false;
   return sync_layout(c);
 }
 
@@ -2605,7 +2629,6 @@ int hb200_append_stereo_tracks(hb200_ctx* c, int n, const double* stamp, const i
   int rc = check_device_window(c);
   if (rc) return rc;
   if (n <= 0 || !stamp || !camera0 || !camera1 || !pixel0 || !pixel1 || !landmark) return fail(-1, "invalid stereo tracks");
-  if (c->k != 4 && c->k != 6) return fail(-4, "spline order %d not supported (4 or 6)", c->k);
   if (c->C == 0) return fail(-2, "cameras not set");
   HB_CUDA(cudaSetDevice(c->device));
   const size_t N = n, Nv = c->Nv, L = c->L;
@@ -2635,15 +2658,13 @@ int hb200_append_stereo_tracks(hb200_ctx* c, int n, const double* stamp, const i
   prep_kernel<<<(c->K + 63) / 64, 64, 0, c->stream>>>(c->K, c->knots[0].p, c->tab[0].p, nullptr, 0);   // knot table of the current state
   HB_LAUNCH(c, "prep_kernel");
   double2* v_pixel = reinterpret_cast<double2*>(c->v_pixel.p);
-  if (c->k == 4)
-    stereo_track_kernel<4><<<(n + 127) / 128, 128, 0, c->stream>>>(n, d_t, c->trk_i.p, c->trk_i.p + N, d_t + N, d_t + 3 * N, d_lm, d_rank, c->knots[0].p, c->tab[0].p, c->K,
+  rc = with_order(c->k, [&](auto K) {
+    stereo_track_kernel<K><<<(n + 127) / 128, 128, 0, c->stream>>>(n, d_t, c->trk_i.p, c->trk_i.p + N, d_t + N, d_t + 3 * N, d_lm, d_rank, c->knots[0].p, c->tab[0].p, c->K,
                                                                   c->basis, c->cams.p, c->C, static_cast<int>(L), static_cast<int>(Nv), c->v_stamp.p, v_pixel, c->v_z.p,
                                                                   c->v_idx.p, c->lms[0].p, c->d_invalid.p);
-  else
-    stereo_track_kernel<6><<<(n + 127) / 128, 128, 0, c->stream>>>(n, d_t, c->trk_i.p, c->trk_i.p + N, d_t + N, d_t + 3 * N, d_lm, d_rank, c->knots[0].p, c->tab[0].p, c->K,
-                                                                  c->basis, c->cams.p, c->C, static_cast<int>(L), static_cast<int>(Nv), c->v_stamp.p, v_pixel, c->v_z.p,
-                                                                  c->v_idx.p, c->lms[0].p, c->d_invalid.p);
-  HB_LAUNCH(c, "stereo_track_kernel");
+    return check_launch(c, "stereo_track_kernel");
+  });
+  if (rc) return rc;
   tail_sorted_kernel<<<(2 * n + 127) / 128, 128, 0, c->stream>>>(static_cast<int>(Nv), 2 * n, c->v_idx.p, c->d_invalid.p + 1);
   HB_LAUNCH(c, "tail_sorted_kernel");
   int h[3] = {0, 0, 0};   // bad tracks, order violations, new landmarks
@@ -2980,7 +3001,7 @@ int hb200_set_min_bandwidth(hb200_ctx* c, int beta) {
     HB_CUDA(cudaStreamSynchronize(c->stream));
     const int rc = ensure_system(c);
     if (rc) return rc;
-    c->invalidate();
+    c->kernel_args_changed();
   }
   return 0;
 }
