@@ -2077,6 +2077,17 @@ int pick_records(hb200_ctx* c, RecordFetch* f, long long it_before, int requeste
   return performed;
 }
 
+// The reductions that can only sum (callback hook, NCCL without a peer mapping) cannot form the maximum of the landmark
+// gradient over the ranks (scalars_kernel), so the gradient-tolerance test would see only the replicated blocks.  Checked
+// when the iterations run, so that the order of hb200_set_termination and attaching the reduction does not matter.
+int check_gradient_test(hb200_ctx* c) {
+  const bool sum_only = c->multi() && !(c->nccl && c->peers_open);
+  if (sum_only && c->term_enabled && c->term_gtol > 0.0)
+    return fail(-2, "the gradient tolerance needs the peer mailbox across ranks (NCCL + hb200_peer_connect); set it to 0 with the "
+                    "all-reduce callback or NCCL without a peer mapping");
+  return 0;
+}
+
 void convert_records(const std::vector<SolverState>& rec, hb200_iteration* records) {
   for (size_t i = 0; i < rec.size(); ++i) {
     records[i].cost = rec[i].cost; records[i].cost_new = rec[i].cost_new; records[i].model_change = rec[i].model_change; records[i].rho = rec[i].rho;
@@ -2091,6 +2102,7 @@ int hb200_iterate(hb200_ctx* c, int iterations, hb200_iteration* records) {
   int rc = check_ready(c);
   if (rc) return rc;
   if (iterations < 0 || iterations > c->max_records) return fail(-1, "iterations must be in [0, %d]", c->max_records);
+  if ((rc = check_gradient_test(c))) return rc;
   HB_CUDA(cudaSetDevice(c->device));
   if (c->term_enabled) {   // a new call continues the trust region but starts with a clean termination state
     new_solve_kernel<<<1, 1, 0, c->stream>>>(c->st.p, c->radius0, 0);
@@ -2117,6 +2129,7 @@ int hb200_optimize(hb200_ctx* c, int iterations, double* knots, double* gyro, do
   int rc = check_ready(c);
   if (rc) return rc;
   if (iterations < 0 || iterations > c->max_records) return fail(-1, "iterations must be in [0, %d]", c->max_records);
+  if ((rc = check_gradient_test(c))) return rc;
   HB_CUDA(cudaSetDevice(c->device));
   // the blocks alias the caller's variables, stamps included: the bound index maps are only valid for the stamps
   // they were computed from (a slid window needs hb200_set_spline / hb200_slide + hb200_bind first)

@@ -1077,33 +1077,34 @@ __global__ void __launch_bounds__(kLmWarps * 32) lm_backsub_kernel(int L, const 
 }
 
 
-// scal = [cost_new, dl.g_l, dl.D_l.dl, |dl|^2, |x_l|^2, |g_l|_inf, 0, 0] (rank-local partials, fixed order).
-// Fallback paths only (callback hook / no peer mapping): the sums are reduced across ranks, the maximum is then only
-// rank-local -- the gradient-tolerance test of hb200_set_termination needs the peer mailbox at N > 1.
+// scal = [cost_new, dl.g_l, dl.D_l.dl, |dl|^2, |x_l|^2, 0, 0, 0] (rank-local partials, fixed order).
+// The paths that can only SUM across ranks (callback hook, NCCL without a peer mapping) run this before their reduction of
+// scal.  A sum of per-rank maxima is not the maximum, so the landmark gradient maximum |g_l|_inf is left at 0: after the
+// reduction gradient_max_norm covers the replicated blocks only, and hb200_iterate / hb200_optimize refuse a gradient
+// tolerance on these paths (the peer mailbox in accept_kernel takes the true maximum).
 __global__ void scalars_kernel(const double* __restrict__ cp_pix, int n_pix_blocks, const double* __restrict__ cp_imu, int n_imu_blocks,
                                const double* __restrict__ lm_part, int n_lm_blocks, double* __restrict__ scal) {
-  __shared__ double s[6][256];
-  double v[6] = {0, 0, 0, 0, 0, 0};
+  __shared__ double s[5][256];
+  double v[5] = {0, 0, 0, 0, 0};
   for (int i = threadIdx.x; i < n_pix_blocks; i += blockDim.x) v[0] += cp_pix[i];
   for (int i = threadIdx.x; i < n_imu_blocks; i += blockDim.x) v[0] += cp_imu[i];
   for (int i = threadIdx.x; i < n_lm_blocks; i += blockDim.x) {
-    v[1] += lm_part[5 * i]; v[2] += lm_part[5 * i + 1]; v[3] += lm_part[5 * i + 2]; v[4] += lm_part[5 * i + 3]; v[5] = fmax(v[5], lm_part[5 * i + 4]);
+    v[1] += lm_part[5 * i]; v[2] += lm_part[5 * i + 1]; v[3] += lm_part[5 * i + 2]; v[4] += lm_part[5 * i + 3];
   }
 #pragma unroll
-  for (int q = 0; q < 6; ++q) s[q][threadIdx.x] = v[q];
+  for (int q = 0; q < 5; ++q) s[q][threadIdx.x] = v[q];
   __syncthreads();
   for (int o = blockDim.x / 2; o > 0; o >>= 1) {
     if (threadIdx.x < o) {
 #pragma unroll
       for (int q = 0; q < 5; ++q) s[q][threadIdx.x] += s[q][threadIdx.x + o];
-      s[5][threadIdx.x] = fmax(s[5][threadIdx.x], s[5][threadIdx.x + o]);
     }
     __syncthreads();
   }
   if (threadIdx.x == 0) {
 #pragma unroll
-    for (int q = 0; q < 6; ++q) scal[q] = s[q][0];
-    scal[6] = 0.0; scal[7] = 0.0;
+    for (int q = 0; q < 5; ++q) scal[q] = s[q][0];
+    scal[5] = 0.0; scal[6] = 0.0; scal[7] = 0.0;
   }
 }
 

@@ -251,7 +251,9 @@ int hb200_cost(hb200_ctx* ctx, double* cost);
  * trust-region radius, 5 five consecutive invalid steps; plus the number of iterations performed by the last call
  * that fetched records and the last |x - Plus(x, -g)|_inf, |step|, |x| the tests saw.
  * hb200_optimize starts every call at the initial radius of hb200_set_options (as ceres::Solve does); hb200_iterate
- * continues the trust region of the previous call.  At N > 1 the gradient test needs the peer mailbox. */
+ * continues the trust region of the previous call.  At N > 1 the gradient test needs the peer mailbox: with the
+ * all-reduce callback or NCCL without a peer mapping the ranks can only sum, gradient_max_norm then covers the replicated
+ * blocks (knots, biases, gravity) and not the landmarks, and hb200_iterate / hb200_optimize refuse a gradient tolerance > 0. */
 int hb200_set_termination(hb200_ctx* ctx, double function_tolerance, double gradient_tolerance, double parameter_tolerance, double min_trust_region_radius);
 int hb200_get_termination(hb200_ctx* ctx, int* type, int* iterations_performed, double* gradient_max_norm, double* step_norm, double* x_norm);
 /* The drop-in for CeresOptimizer::optimize() (reference optimizer.cpp:276-280) with the parameter
@@ -325,7 +327,7 @@ int hb200_comm_info(hb200_ctx* ctx, int* nranks, int* rank, int* nccl, int* peer
 int hb200_get_bandwidth(hb200_ctx* ctx, int* beta);
 int hb200_set_min_bandwidth(hb200_ctx* ctx, int beta);
 /* Escape hatch for hosts without NCCL: the caller sums `count_doubles` doubles at `device_buffer` across ranks
- * on `stream` (called twice per iteration: packed system, then 4 scalars).  Disables CUDA-graph capture. */
+ * on `stream` (called twice per iteration: packed system, then 8 scalars).  Disables CUDA-graph capture. */
 typedef int (*hb200_allreduce_fn)(void* user, void* device_buffer, long long count_doubles, void* stream);
 int hb200_set_allreduce(hb200_ctx* ctx, hb200_allreduce_fn fn, void* user);
 void* hb200_system_device_ptr(hb200_ctx* ctx, long long* count_doubles);

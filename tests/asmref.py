@@ -22,6 +22,8 @@ that sensitivity are the only legitimate differences left.
 """
 from __future__ import annotations
 
+import dataclasses
+
 import numpy as np
 
 import sysref as sr
@@ -275,11 +277,12 @@ def compare(buf, ref, beta):
     """Worst |buf - ref| / bound per part of the packed buffer (S band, arrow, corner, b, g, diagH, cost), and the number of
     slots that must be exactly zero and are not.  A part passes when its ratio is <= 1."""
     val, bnd, Lay = packed(ref, beta)
-    buf = np.asarray(buf, dtype=np.float64)
+    return _ratios(np.asarray(buf, dtype=np.float64), val, bnd, bnd == 0, Lay, ref["n"])
+
+
+def _ratios(buf, val, bnd, zero, Lay, n):
     assert buf.size == val.size
     err = np.abs(buf.astype(LD) - val).astype(np.float64)
-    zero = bnd == 0
-    n = ref["n"]
     parts = dict(band=slice(0, Lay["oA"]), arrow=slice(Lay["oA"], Lay["oC"]), corner=slice(Lay["oC"], Lay["ob"]),
                  b=slice(Lay["ob"], Lay["ob"] + n), diagH=slice(Lay["oD"], Lay["oD"] + n), g=slice(Lay["og"], Lay["og"] + n),
                  cost=slice(Lay["os"], Lay["os"] + 1))
@@ -297,3 +300,55 @@ def check(buf, ref, beta):
     bad = {k: v for k, v in res.items() if k not in ("nonzero_outside", "finite") and not v <= 1.0}
     assert res["finite"] and res["nonzero_outside"] == 0 and not bad, res
     return res
+
+
+# ---- sharded systems ----------------------------------------------------------------------------------------
+SHARD_FIELDS = dict(pixel=("v_stamp", "v_cam", "v_lm", "v_pixel"), bearing=("b_stamp", "b_cam", "b_lm", "b_bearing"),
+                    inertial=("i_stamp", "i_meas"), pose=("m_stamp", "m_sensor", "m_pose"))
+
+
+def partition(win, ranks, world):
+    """The factor shards of `win` for `world` ranks: ranks[family][f] = rank of factor f, for every family of SHARD_FIELDS.
+    State (knots, biases, gravity, landmarks, calibration) is replicated in every shard."""
+    out = []
+    for r in range(world):
+        kw = {}
+        for fam, keys in SHARD_FIELDS.items():
+            sel = np.asarray(ranks[fam]) == r
+            assert sel.size == getattr(win, keys[0]).shape[0], fam
+            kw.update({key: np.ascontiguousarray(getattr(win, key)[sel]) for key in keys})
+        out.append(dataclasses.replace(win, **kw))
+    return out
+
+
+def compare_shard_sum(refs, full):
+    """Long-double sum of the shard references against the reference of the whole window: worst |sum - full| / bound per
+    part (S, b, g, diagH, cost) with bound = the sum of the shard bounds + the full window's bound, and the number of entries
+    that differ where every bound is 0.  A partition that keeps each landmark's observations on one rank passes (<= 1)."""
+    out = dict(nonzero_outside=0)
+    for key in ("S", "b", "g", "diagH", "cost"):
+        err = np.abs(sum(r[key] for r in refs) - full[key]).astype(np.float64)
+        bnd = sum(r[key + "_bound"] for r in refs) + full[key + "_bound"]
+        err, bnd = np.atleast_1d(err), np.atleast_1d(bnd)
+        z = bnd == 0
+        out[key] = float((err[~z] / bnd[~z]).max()) if (~z).any() else 0.0
+        out["nonzero_outside"] += int(np.count_nonzero(err[z]))
+    return out
+
+
+def compare_summed_buffers(bufs, refs, beta):
+    """Partial packed buffers (one per rank, all at half-width beta) summed in rank order in float64, as the reduction does,
+    against the long-double sum of their references.  Bound per slot: the sum of the shard bounds + (N - 1) u sum_r |buf_r|
+    (the float64 sum of N terms).  Slots where every shard's bound is 0 must be exactly 0.  Same keys as compare()."""
+    vals, bnds = [], []
+    for r in refs:
+        v, b, Lay = packed(r, beta)
+        vals.append(v)
+        bnds.append(b)
+    bufs = [np.asarray(b, dtype=np.float64) for b in bufs]
+    tot = bufs[0].copy()
+    for b in bufs[1:]:
+        tot = tot + b
+    own = sum(bnds)
+    bnd = own + (len(bufs) - 1) * U * sum(np.abs(b) for b in bufs)
+    return _ratios(tot, sum(vals), bnd, own == 0, Lay, refs[0]["n"])
