@@ -257,6 +257,15 @@ struct hb200_ctx {
   int n_lm_blocks = 0;
   bool system_built = false;
 
+  // deterministic assembly (hb200_set_deterministic; DetOut, hb200_eval.cuh): the J^T J kernels' record regions, the
+  // records, the entry -> records index and its ready flag.  det_ready: the regions fit the current window
+  // (prepare_det, dropped by kernel_args_changed()).
+  bool deterministic = false, det_ready = false;
+  DetOut det_pix{}, det_imu{}, det_man{}, det_schur{};
+  long long det_records = 0;
+  DevBuf<double> det_val;
+  DevBuf<int> det_key, det_cnt, det_off, det_perm, det_flag, det_seg_off;
+
   // marginal covariances (hb200_build_covariance / hb200_compute_covariance).  cov_st: the build's own solver state
   // (radius +inf: no damping inside the landmark elimination; st is never touched).  cov_at: launch count after the last
   // covariance call -- any other launch since (an evaluation, an iteration, a slide) rewrote what the compute reads.
@@ -328,7 +337,7 @@ struct hb200_ctx {
   // the factor outputs changed or no longer match the state
   void outputs_changed() { system_changed(); evaluated_J = false; mirror_valid = false; calib_valid = false; }
   // shapes or buffers the captured iteration was recorded with changed
-  void kernel_args_changed() { outputs_changed(); graph_valid = false; }
+  void kernel_args_changed() { outputs_changed(); graph_valid = false; det_ready = false; }
 
   // The variable blocks in their canonical order (knots, gyroscope bias, accelerometer bias, gravity, landmarks): the
   // current state, the trial state, the snapshot and the block's length in doubles.
@@ -545,6 +554,11 @@ template <int K, bool J>
 int launch_pixel(hb200_ctx* c, int sel, bool accumulate = false) {
   if (c->Nv == 0) return 0;
   PixelArgs a = pixel_args<J>(c, sel, accumulate);
+  if (J && accumulate && c->deterministic) {
+    pixel_eval_det_kernel<K><<<c->n_pix_blocks, kEvalThreads, 0, c->stream>>>(a, c->basis, c->det_pix, c->det_seg_off.p);
+    HB_LAUNCH(c, "pixel_eval_det_kernel");
+    return 0;
+  }
   if (J && accumulate) pixel_eval_kernel<K, J, J><<<c->n_pix_blocks, kEvalThreads, 0, c->stream>>>(a, c->basis);
   else pixel_eval_kernel<K, J, false><<<c->n_pix_blocks, kEvalThreads, 0, c->stream>>>(a, c->basis);
   HB_LAUNCH(c, "pixel_eval_kernel");
@@ -565,6 +579,11 @@ int launch_factors_merged(hb200_ctx* c, int sel, bool accumulate) {
   const InertialArgs ia = inertial_args<J>(c, sel);
   const int blocks = c->n_pix_blocks + c->n_imu_blocks;
   const size_t smem = J ? inertial_stash_bytes(K) : 0;
+  if (J && accumulate && c->deterministic) {
+    factor_eval_det_kernel<K, 4><<<blocks, kEvalThreads, smem, c->stream>>>(pa, ia, c->basis, c->bias_basis, c->n_pix_blocks, c->det_pix, c->det_seg_off.p);
+    HB_LAUNCH(c, "factor_eval_det_kernel");
+    return 0;
+  }
   if (J && accumulate) factor_eval_kernel<K, 4, J, J><<<blocks, kEvalThreads, smem, c->stream>>>(pa, ia, c->basis, c->bias_basis, c->n_pix_blocks);
   else factor_eval_kernel<K, 4, J, false><<<blocks, kEvalThreads, smem, c->stream>>>(pa, ia, c->basis, c->bias_basis, c->n_pix_blocks);
   HB_LAUNCH(c, "factor_eval_kernel");
@@ -630,31 +649,48 @@ int enqueue_evaluate(hb200_ctx* c, bool want_J, int sel, bool accumulate = false
 // so nothing orders them.  The side stream is forked here, not before the evaluation, when the factor Jacobians were
 // produced on the MAIN stream (merged factor kernel).
 // st: the solver state whose radius damps the landmark blocks (the LM's c->st, or the covariance build's radius +inf).
+// Inertial J^T J: large windows (>= 16 384 inertial factors) take the augmented product on the FP64 tensor cores, ~6 CTAs
+// per SM of 8-factor chunks; small windows the scalar block-by-block kernel on short runs (cfg1, ~9 factors per CTA), which
+// is faster there.  (Order 6 keeps 12-factor chunks at ~2 CTAs per SM, which beat 8-factor chunks at ~6 CTAs per SM on the
+// order-6 window.)  Returns the CTAs per run.
+int inertial_splits(const hb200_ctx* c, bool* scalar_hess) {
+  *scalar_hess = c->Ni < 16384;
+  return (*scalar_hess || c->k != 4) ? c->imu_splits : c->imu_splits_mma;
+}
+
 int enqueue_build(hb200_ctx* c, const SolverState* st) {
+  const bool det = c->deterministic;
+  if (det && !c->det_ready) return fail(-2, "deterministic assembly: record slots not laid out for this window");
   { const int rf = fork_side(c); if (rf) return rf; }   // (no-op when already forked or while profiling)
   if (c->Ni) {
-    // large windows (>= 16 384 inertial factors): the augmented product on the FP64 tensor cores, ~6 CTAs per SM of 8-factor
-    // chunks; small windows: the scalar block-by-block kernel on short runs (cfg1, ~9 factors per CTA), which is faster there
-    const bool scalar_hess = c->Ni < 16384;
-    // (order 6 keeps 12-factor chunks at ~2 CTAs per SM, which beat 8-factor chunks at ~6 CTAs per SM on the order-6 window)
-    const int splits = (scalar_hess || c->k != 4) ? c->imu_splits : c->imu_splits_mma;
+    bool scalar_hess = false;
+    const int splits = inertial_splits(c, &scalar_hess);
     const int grid = c->nruns * splits;
     const int rc = with_order(c->k, [&](auto K) {
-      if (scalar_hess)
+      if (det && scalar_hess)
+        inertial_hessian_det_kernel<K, 4><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->i_idx.p, c->i_r.p, c->i_Jp.p, c->i_wg.p, c->i_wa.p,
+                                                                              c->i_Jg.p, c->imu_scale, c->lay, c->o_bg(), c->o_ba(), c->o_g(), splits, c->det_imu);
+      else if (det)
+        inertial_hessian_mma_det_kernel<K, 4, K == 4 ? 8 : 12><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->i_idx.p, c->i_r.p, c->i_Jp.p, c->i_wg.p, c->i_wa.p,
+                                                                                                  c->i_Jg.p, c->imu_scale, c->lay, c->o_bg(), c->o_ba(), c->o_g(), splits,
+                                                                                                  c->det_imu);
+      else if (scalar_hess)
         inertial_hessian_kernel<K, 4><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->i_idx.p, c->i_r.p, c->i_Jp.p, c->i_wg.p, c->i_wa.p,
                                                                           c->i_Jg.p, c->imu_scale, c->assembly(), c->lay, c->o_bg(), c->o_ba(), c->o_g(), c->imu_splits);
       else
         inertial_hessian_mma_kernel<K, 4, K == 4 ? 8 : 12><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->i_idx.p, c->i_r.p, c->i_Jp.p, c->i_wg.p, c->i_wa.p,
                                                                                               c->i_Jg.p, c->imu_scale, c->assembly(), c->lay, c->o_bg(), c->o_ba(), c->o_g(), splits);
-      return check_launch(c, scalar_hess ? "inertial_hessian_kernel" : "inertial_hessian_mma_kernel");
+      return check_launch(c, scalar_hess ? (det ? "inertial_hessian_det_kernel" : "inertial_hessian_kernel")
+                                         : (det ? "inertial_hessian_mma_det_kernel" : "inertial_hessian_mma_kernel"));
     });
     if (rc) return rc;
   }
   if (c->Nm) {
     const int blocks = (c->Nm + kManWarps - 1) / kManWarps;
     const int rc = with_order(c->k, [&](auto K) {
-      manifold_hessian_kernel<K><<<blocks, kManWarps * 32, 0, side(c)>>>(c->Nm, c->m_idx.p, c->m_r.p, c->m_Jp.p, c->assembly(), c->lay);
-      return check_launch(c, "manifold_hessian_kernel");
+      if (det) manifold_hessian_det_kernel<K><<<blocks, kManWarps * 32, 0, side(c)>>>(c->Nm, c->m_idx.p, c->m_r.p, c->m_Jp.p, c->lay, c->det_man);
+      else manifold_hessian_kernel<K><<<blocks, kManWarps * 32, 0, side(c)>>>(c->Nm, c->m_idx.p, c->m_r.p, c->m_Jp.p, c->assembly(), c->lay);
+      return check_launch(c, det ? "manifold_hessian_det_kernel" : "manifold_hessian_kernel");
     });
     if (rc) return rc;
   }
@@ -667,21 +703,95 @@ int enqueue_build(hb200_ctx* c, const SolverState* st) {
   if (c->Nv && c->L && c->schur_groups) {
     const size_t smem = (3 * static_cast<size_t>(kSchurGroup) * (c->schur_rt + 1) + 3 * kSchurGroup + 4 * 3 * static_cast<size_t>(c->schur_rt)) * sizeof(double);
     const int rc = with_order(c->k, [&](auto K) {
-      schur_group_kernel<K><<<c->n_lm_groups, kSchurGThreads, smem, c->stream>>>(c->lm_group_off.p, c->lm_order.p, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p, c->v_Jp.p,
-                                                                                 c->v_Jl.p, c->v_w.p, st, c->assembly(), c->lay, c->Vchol.p, c->gl.p, c->Dl.p, c->schur_rt);
-      return check_launch(c, "schur_group_kernel");
+      if (det)
+        schur_group_det_kernel<K><<<c->n_lm_groups, kSchurGThreads, smem, c->stream>>>(c->lm_group_off.p, c->lm_order.p, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p,
+                                                                                       c->v_Jp.p, c->v_Jl.p, c->v_w.p, st, c->lay, c->Vchol.p, c->gl.p, c->Dl.p, c->schur_rt,
+                                                                                       c->det_schur);
+      else
+        schur_group_kernel<K><<<c->n_lm_groups, kSchurGThreads, smem, c->stream>>>(c->lm_group_off.p, c->lm_order.p, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p, c->v_Jp.p,
+                                                                                   c->v_Jl.p, c->v_w.p, st, c->assembly(), c->lay, c->Vchol.p, c->gl.p, c->Dl.p, c->schur_rt);
+      return check_launch(c, det ? "schur_group_det_kernel" : "schur_group_kernel");
     });
     if (rc) return rc;
   } else if (c->Nv && c->L) {
     const size_t smem = 2 * 3 * static_cast<size_t>(c->max_rows) * sizeof(double);
     const int rc = with_order(c->k, [&](auto K) {
-      schur_kernel<K><<<c->L, kSchurThreads, smem, c->stream>>>(c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p, st,
-                                                                c->assembly(), c->lay, c->Vchol.p, c->gl.p, c->Dl.p, c->max_rows);
-      return check_launch(c, "schur_kernel");
+      if (det)
+        schur_det_kernel<K><<<c->L, kSchurThreads, smem, c->stream>>>(c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p, st,
+                                                                      c->lay, c->Vchol.p, c->gl.p, c->Dl.p, c->max_rows, c->det_schur);
+      else
+        schur_kernel<K><<<c->L, kSchurThreads, smem, c->stream>>>(c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p, st,
+                                                                  c->assembly(), c->lay, c->Vchol.p, c->gl.p, c->Dl.p, c->max_rows);
+      return check_launch(c, det ? "schur_det_kernel" : "schur_kernel");
     });
     if (rc) return rc;
   }
-  return join_side(c);
+  { const int rj = join_side(c); if (rj) return rj; }
+  if (!det) return 0;
+  // the fixed-order sums: the entry index (built by the first build after the slots were laid out), then every entry
+  long long nrec = c->det_records;
+  const int* key = c->det_key.p;
+  int nent = static_cast<int>(c->lay.total);
+  int *cnt = c->det_cnt.p, *off = c->det_off.p, *perm = c->det_perm.p, *flag = c->det_flag.p;
+  void* args[] = {&nrec, &key, &nent, &cnt, &off, &perm, &flag};
+  HB_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(det_index_kernel), dim3(c->num_sms), dim3(kDetThreads), args, 0, c->stream));
+  HB_LAUNCH(c, "det_index_kernel");
+  const int blocks = static_cast<int>(std::min<long long>((nent + kDetThreads - 1) / kDetThreads, 8LL * c->num_sms));
+  det_reduce_kernel<<<std::max(blocks, 1), kDetThreads, 0, c->stream>>>(nent, c->det_off.p, c->det_perm.p, c->det_val.p, c->assembly());
+  HB_LAUNCH(c, "det_reduce_kernel");
+  return 0;
+}
+
+// Lays out the deterministic assembly's record regions for the bound window and clears the keys and the entry index,
+// which the next build rebuilds.  Eager (it reads the pixel segment count back), so it runs before a build is enqueued or
+// captured; once per window shape (kernel_args_changed() drops det_ready).
+int prepare_det(hb200_ctx* c) {
+  if (!c->deterministic || c->det_ready) return 0;
+  long long off = 0;
+  auto region = [&](DetOut& d, long long slots, long long per_slot) { d.off = off; d.per_slot = per_slot; off += slots * per_slot; };
+  c->det_pix = c->det_imu = c->det_man = c->det_schur = DetOut{};
+  const int rc = with_order(c->k, [&](auto K) {
+    if (c->Nv) {   // pixel: one slot per (64-factor tile, knot-base segment)
+      const int tiles = c->n_pix_blocks;
+      HB_CUDA(c->det_seg_off.ensure(2 * (static_cast<size_t>(tiles) + 1)));   // offsets | counts
+      int* counts = c->det_seg_off.p + tiles + 1;
+      HB_CUDA(cudaMemsetAsync(counts, 0, sizeof(int) * (static_cast<size_t>(tiles) + 1), c->stream));
+      det_pixel_segments_kernel<<<(tiles + 127) / 128, 128, 0, c->stream>>>(c->Nv, c->v_idx.p, counts);
+      HB_LAUNCH(c, "det_pixel_segments_kernel");
+      HB_CUDA(c->w_scal.ensure(8));
+      scan_kernel<<<1, 1024, 0, c->stream>>>(counts, tiles + 1, c->det_seg_off.p, c->w_scal.p);
+      HB_LAUNCH(c, "scan_kernel");
+      int segs = 0;
+      HB_CUDA(cudaMemcpyAsync(&segs, c->w_scal.p, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+      HB_CUDA(cudaStreamSynchronize(c->stream));
+      region(c->det_pix, segs, kEvalThreads * pixel_det_writes<K>());
+    }
+    if (c->Ni) {   // inertial: one slot per CTA
+      bool scalar_hess = false;
+      const int splits = inertial_splits(c, &scalar_hess);
+      region(c->det_imu, static_cast<long long>(c->nruns) * splits, kHessThreads * (scalar_hess ? ImuHessScalar<K, 4>::DET_WRITES : imu_hess_mma_det_writes<K, 4>()));
+    }
+    if (c->Nm) region(c->det_man, c->Nm, 32 * manifold_det_writes<K>());   // one slot per factor
+    if (c->Nv && c->L) {   // one slot per landmark group / landmark
+      if (c->schur_groups) region(c->det_schur, c->n_lm_groups, kSchurGThreads * schur_group_det_writes(c->schur_rt));
+      else region(c->det_schur, c->L, kSchurThreads * schur_det_writes(c->max_rows));
+    }
+    return 0;
+  });
+  if (rc) return rc;
+  if (off >= (1LL << 31) - 1 || c->lay.total >= (1LL << 31) - 1)
+    return fail(-6, "deterministic assembly: %lld records for a system of %lld entries exceed 32-bit indexing", off, c->lay.total);
+  c->det_records = off;
+  HB_CUDA(c->det_val.ensure(std::max<long long>(off, 1))); HB_CUDA(c->det_key.ensure(std::max<long long>(off, 1)));
+  HB_CUDA(c->det_perm.ensure(std::max<long long>(off, 1)));
+  HB_CUDA(c->det_cnt.ensure(static_cast<size_t>(c->lay.total))); HB_CUDA(c->det_off.ensure(static_cast<size_t>(c->lay.total) + 1));
+  HB_CUDA(c->det_flag.ensure(1));
+  HB_CUDA(cudaMemsetAsync(c->det_key.p, 0xff, sizeof(int) * std::max<long long>(off, 1), c->stream));
+  HB_CUDA(cudaMemsetAsync(c->det_flag.p, 0, sizeof(int), c->stream));
+  for (DetOut* d : {&c->det_pix, &c->det_imu, &c->det_man, &c->det_schur}) { d->val = c->det_val.p; d->key = c->det_key.p; }
+  HB_CUDA(cudaStreamSynchronize(c->stream));
+  c->det_ready = true;
+  return 0;
 }
 
 // band-only raw system -> dense damped work copy Lw (dense fallback solver, hb200_get_system)
@@ -954,6 +1064,8 @@ int create_impl(const hb200_options* options, hb200_ctx* c) {
   HB_CUDA(cudaFuncSetAttribute(factor_eval_kernel<4, 4, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(inertial_stash_bytes(4))));
   HB_CUDA(cudaFuncSetAttribute(factor_eval_kernel<6, 4, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(inertial_stash_bytes(6))));
   HB_CUDA(cudaFuncSetAttribute(factor_eval_kernel<6, 4, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(inertial_stash_bytes(6))));
+  HB_CUDA(cudaFuncSetAttribute(factor_eval_det_kernel<4, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(inertial_stash_bytes(4))));
+  HB_CUDA(cudaFuncSetAttribute(factor_eval_det_kernel<6, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(inertial_stash_bytes(6))));
   return reset_solver_state(c);
 }
 }  // namespace
@@ -1343,6 +1455,8 @@ int derive_window(hb200_ctx* c) {
     const int smem = static_cast<int>(2 * 3 * static_cast<size_t>(c->max_rows) * sizeof(double));
     HB_CUDA(cudaFuncSetAttribute(schur_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     HB_CUDA(cudaFuncSetAttribute(schur_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    HB_CUDA(cudaFuncSetAttribute(schur_det_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    HB_CUDA(cudaFuncSetAttribute(schur_det_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   }
   int rc = update_fixed(c);
   if (rc) return rc;
@@ -1488,6 +1602,8 @@ int hb200_bind(hb200_ctx* c, int* num_invalid) {
       else {
         HB_CUDA(cudaFuncSetAttribute(schur_group_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
         HB_CUDA(cudaFuncSetAttribute(schur_group_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+        HB_CUDA(cudaFuncSetAttribute(schur_group_det_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+        HB_CUDA(cudaFuncSetAttribute(schur_group_det_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
       }
     }
   }
@@ -1789,6 +1905,7 @@ int hb200_build_system(hb200_ctx* c) {
   if (rc) return rc;
   if (!c->evaluated_J) return fail(-2, "call hb200_evaluate(HB200_EVAL_JACOBIANS) first");
   HB_CUDA(cudaSetDevice(c->device));
+  if ((rc = prepare_det(c))) return rc;
   // assembled as enqueue_iteration does: the Jacobian sweep at the current state runs again with the pixel J^T J
   // accumulated by the factor kernels (it rewrites the same residuals and Jacobians), then the rest of the system
   if ((rc = enqueue_evaluate(c, true, 0, /*accumulate=*/true, /*keep_fork=*/true, /*clear_system=*/true))) return rc;
@@ -1847,6 +1964,7 @@ int hb200_build_covariance(hb200_ctx* c) {
   if (smem > 220 * 1024)
     return fail(-6, "covariance: a window of %d block columns and %d arrow rows needs %zu B of shared memory", c->beta + 1, c->lay.m, smem);
   c->cov_built = false;
+  if ((rc = prepare_det(c))) return rc;
   SolverState s{};
   s.radius = INFINITY;   // mu = 1 / radius = 0 in the Schur kernels
   HB_CUDA(c->cov_st.ensure(1));
@@ -1986,7 +2104,8 @@ int hb200_interpolate_covariance(hb200_ctx* c, int n, const double* stamps, doub
 namespace {
 
 int iterate_enqueue(hb200_ctx* c, int iterations) {
-  int rc = 0;
+  int rc = prepare_det(c);
+  if (rc) return rc;
   for (int it = 0; it < iterations; ++it) {
     // the callback hook cannot be captured; with NCCL the first iteration runs eagerly (NCCL finishes its lazy
     // channel / buffer setup outside of a capture), every later one is a graph launch.  With the peer-memory
@@ -2288,6 +2407,7 @@ int hb200_profile_iteration(hb200_ctx* c, int reps, int max_entries, char* names
   const bool reps_mode_evaluate = reps < 0;   // negative reps: profile the Evaluate sweep only
   if (reps < 0) reps = -reps;
   HB_CUDA(cudaSetDevice(c->device));
+  if ((rc = prepare_det(c))) return rc;
   std::vector<double> acc;
   std::vector<std::string> nm;
   for (int rep = 0; rep < reps; ++rep) {
@@ -3016,6 +3136,21 @@ int hb200_set_min_bandwidth(hb200_ctx* c, int beta) {
     if (rc) return rc;
     c->kernel_args_changed();
   }
+  return 0;
+}
+
+int hb200_set_deterministic(hb200_ctx* c, int enable) {
+  if (!c) return fail(-1, "null context");
+  const bool on = enable != 0;
+  if (on == c->deterministic) return 0;
+  c->deterministic = on;
+  c->kernel_args_changed();
+  return 0;
+}
+
+int hb200_get_deterministic(hb200_ctx* c, int* enable) {
+  if (!c || !enable) return fail(-1, "invalid argument");
+  *enable = c->deterministic ? 1 : 0;
   return 0;
 }
 

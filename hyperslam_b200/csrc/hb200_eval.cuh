@@ -14,6 +14,30 @@
 namespace hb {
 
 // ---------------------------------------------------------------------------------------------
+// Deterministic assembly (hb200_set_deterministic).  The J^T J kernels' variants for it add nothing into the packed
+// system: each contribution is stored with a plain store into a record of its own, next to the index of the packed
+// entry it belongs to, and det_reduce_kernel (hb200_solve.cuh) sums every entry's records in ascending record order.
+// A kernel owns one region of records, cut into equal slots (a pixel segment, an inertial CTA, a manifold factor, a
+// landmark or a landmark group); the k-th write of thread t of a slot goes to record  off + slot per_slot + k T + t
+// (T threads per slot).  Which records a slot writes, and to which entries, follows from the bound window alone, so
+// the order of every sum does too.
+// ---------------------------------------------------------------------------------------------
+struct DetOut {
+  double* val;       // [records] contribution
+  int* key;          // [records] packed-system index (-1: never written)
+  long long off;     // first record of the kernel's region
+  long long per_slot;
+};
+struct DetCursor {
+  double* val;
+  int* key;
+  long long p;
+  int step;
+  HB_DI void put(long long e, double v) { val[p] = v; key[p] = static_cast<int>(e); p += step; }
+};
+HB_DI DetCursor det_cursor(const DetOut& d, long long slot, int threads, int t) { return DetCursor{d.val, d.key, d.off + slot * d.per_slot + t, threads}; }
+
+// ---------------------------------------------------------------------------------------------
 // TMA (1-D bulk copy) + mbarrier helpers
 // ---------------------------------------------------------------------------------------------
 HB_DI uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
@@ -426,12 +450,19 @@ HB_DI void pixel_hess_reset(PixelHessAcc<K>& acc, int base) {
   for (int q = 0; q < PixelHessAcc<K>::PER_WARP; ++q) { acc.c0[q] = 0.0; acc.c1[q] = 0.0; }
   acc.g = 0.0; acc.base = base;
 }
+// writes per thread of one flush in deterministic mode (3 per tile: two entries of S and one of diag(J^T J); the gradient)
 template <int K>
-HB_DI void pixel_hess_flush(const PixelArgs& a, const PixelHessAcc<K>& acc) {
+__host__ __device__ constexpr int pixel_det_writes() { return 3 * PixelHessAcc<K>::PER_WARP + 1; }
+
+// DET: the slot's records instead of atomics (slot = the flushed segment's index in the window, see DetOut)
+template <int K, bool DET = false>
+HB_DI void pixel_hess_flush(const PixelArgs& a, const PixelHessAcc<K>& acc, const DetOut& det = DetOut{}, int slot = 0) {
   constexpr int NB = 6 * K, NTILES = PixelHessAcc<K>::NTILES;
   if (acc.base < 0) return;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, lm = lane >> 2, lk = lane & 3;
   double* S = a.sys;
+  DetCursor dc = det_cursor(det, slot, kEvalThreads, tid);
+  auto add = [&](long long e, double v) { if constexpr (DET) dc.put(e, v); else atomicAdd(&S[e], v); };
   const int c0 = 6 * acc.base;
 #pragma unroll
   for (int q = 0; q < PixelHessAcc<K>::PER_WARP; ++q) {
@@ -442,14 +473,14 @@ HB_DI void pixel_hess_flush(const PixelArgs& a, const PixelHessAcc<K>& acc) {
     const int tj = tile - ti * (ti + 1) / 2;
     const int rr = 8 * ti + lm, cc = 8 * tj + 2 * lk;
     if (rr < NB) {
-      if (cc < NB && cc <= rr) atomicAdd(&S[sys_index(a.lay, c0 + rr, c0 + cc)], acc.c0[q]);
-      if (cc + 1 < NB && cc + 1 <= rr) atomicAdd(&S[sys_index(a.lay, c0 + rr, c0 + cc + 1)], acc.c1[q]);
+      if (cc < NB && cc <= rr) add(sys_index(a.lay, c0 + rr, c0 + cc), acc.c0[q]);
+      if (cc + 1 < NB && cc + 1 <= rr) add(sys_index(a.lay, c0 + rr, c0 + cc + 1), acc.c1[q]);
       // diag(J^T J) is accumulated on its own (the LM damping needs it BEFORE the Schur complement touches S)
-      if (cc == rr) atomicAdd(&S[a.lay.oD + c0 + rr], acc.c0[q]);
-      if (cc + 1 == rr) atomicAdd(&S[a.lay.oD + c0 + rr], acc.c1[q]);
+      if (cc == rr) add(a.lay.oD + c0 + rr, acc.c0[q]);
+      if (cc + 1 == rr) add(a.lay.oD + c0 + rr, acc.c1[q]);
     }
   }
-  if (tid >= kEvalThreads - NB) atomicAdd(&S[a.lay.og + c0 + tid - (kEvalThreads - NB)], acc.g);
+  if (tid >= kEvalThreads - NB) add(a.lay.og + c0 + tid - (kEvalThreads - NB), acc.g);
 }
 
 // lower-triangle tile number -> (tile row, tile column), compile time
@@ -479,8 +510,10 @@ HB_DI void pixel_hess_steps(PixelHessAcc<K>& acc, const double* sJ, int r_lo, in
   }
 }
 
-template <int K>
-HB_DI void cta_pixel_hessian(const PixelArgs& a, int f0, int cnt, double* sJ /*[128][LD]*/, double* sr /*[128]*/, int* sseg /*[66]*/, PixelHessAcc<K>& acc) {
+// seg0 (DET): window index of the tile's first segment
+template <int K, bool DET = false>
+HB_DI void cta_pixel_hessian(const PixelArgs& a, int f0, int cnt, double* sJ /*[128][LD]*/, double* sr /*[128]*/, int* sseg /*[66]*/, PixelHessAcc<K>& acc,
+                             const DetOut& det = DetOut{}, int seg0 = 0) {
   constexpr int NB = 6 * K, LD = PixelHessAcc<K>::LD;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   __shared__ double s_sw[kEvalThreads];
@@ -529,7 +562,7 @@ HB_DI void cta_pixel_hessian(const PixelArgs& a, int f0, int cnt, double* sJ /*[
   for (int j = 0; j < nseg; ++j) {
     const int r_lo = 2 * sseg[j], r_hi = 2 * sseg[j + 1];
     const int base = a.idx[f0 + sseg[j]].x;
-    if (base != acc.base) { pixel_hess_flush<K>(a, acc); pixel_hess_reset<K>(acc, base); }   // (uniform across the CTA)
+    if (base != acc.base) { pixel_hess_flush<K, DET>(a, acc, det, seg0 + j - 1); pixel_hess_reset<K>(acc, base); }   // (uniform across the CTA)
     if (warp == 0) pixel_hess_steps<K, 0>(acc, sJ, r_lo, r_hi, lm, lk);
     else pixel_hess_steps<K, 1>(acc, sJ, r_lo, r_hi, lm, lk);
     if (tid >= kEvalThreads - NB) {   // gradient: the last NB threads
@@ -541,9 +574,10 @@ HB_DI void cta_pixel_hessian(const PixelArgs& a, int f0, int cnt, double* sJ /*[
   }
 }
 
-// bid: the CTA's index within the pixel grid (the merged factor kernel offsets it)
-template <int K, bool WANT_J, bool FUSE>
-HB_DI void pixel_eval_body(const PixelArgs& a, const Basis& B, int bid0) {
+// bid: the CTA's index within the pixel grid (the merged factor kernel offsets it).  DET (fused pass, one tile per CTA):
+// the J^T J goes to the slots of the tile's segments, seg_off[bid] .. seg_off[bid + 1] - 1
+template <int K, bool WANT_J, bool FUSE, bool DET = false>
+HB_DI void pixel_eval_body(const PixelArgs& a, const Basis& B, int bid0, const DetOut& det = DetOut{}, const int* seg_off = nullptr) {
   __shared__ __align__(16) double s_tab[kTileRows * kTabStride];
   __shared__ __align__(8) uint64_t s_bar;
   __shared__ int s_red[2];
@@ -602,14 +636,29 @@ HB_DI void pixel_eval_body(const PixelArgs& a, const Basis& B, int bid0) {
     // fused normal equations of this CTA's factors (residuals / Jacobians were written above; the barrier in the
     // cost reduction ordered them for the whole CTA)
     const int f_lo = bid * kEvalThreads;
-    cta_pixel_hessian<K>(a, f_lo, min(kEvalThreads, a.n - f_lo), s_J, s_r, s_b, acc);
+    cta_pixel_hessian<K, DET>(a, f_lo, min(kEvalThreads, a.n - f_lo), s_J, s_r, s_b, acc, det, DET ? seg_off[bid] : 0);
   }
   }   // tiles
-  if (FUSE && a.sys != nullptr) pixel_hess_flush<K>(a, acc);
+  if (FUSE && a.sys != nullptr) pixel_hess_flush<K, DET>(a, acc, det, DET ? seg_off[bid0 + 1] - 1 : 0);
 }
 
 template <int K, bool WANT_J, bool FUSE = false>
 __global__ void __launch_bounds__(kEvalThreads, (K == 4 && FUSE) ? 6 : 1) pixel_eval_kernel(PixelArgs a, Basis B) { pixel_eval_body<K, WANT_J, FUSE>(a, B, blockIdx.x); }
+// the fused pass of the deterministic assembly
+template <int K>
+__global__ void __launch_bounds__(kEvalThreads, K == 4 ? 6 : 1) pixel_eval_det_kernel(PixelArgs a, Basis B, DetOut det, const int* __restrict__ seg_off) {
+  pixel_eval_body<K, true, true, true>(a, B, blockIdx.x, det, seg_off);
+}
+
+// segments (runs of equal knot base) of every 64-factor tile of the visual list: the slots of the deterministic fused pass
+__global__ void det_pixel_segments_kernel(int n, const int4* __restrict__ idx, int* __restrict__ cnt) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t * kEvalThreads >= n) return;
+  const int lo = t * kEvalThreads, hi = min(n, lo + kEvalThreads);
+  int s = 1;
+  for (int f = lo + 1; f < hi; ++f) s += idx[f].x != idx[f - 1].x;
+  cnt[t] = s;
+}
 
 // ---------------------------------------------------------------------------------------------
 // Inertial factor (a6 + a3 with value/velocity/acceleration Jacobian stacks fused).
@@ -986,6 +1035,12 @@ template <int K, int KB, bool WANT_J, bool FUSE>
 __global__ void __launch_bounds__(kEvalThreads) factor_eval_kernel(PixelArgs pa, InertialArgs ia, Basis B, Basis BB, int n_pix_blocks) {
   if (static_cast<int>(blockIdx.x) < n_pix_blocks) pixel_eval_body<K, WANT_J, FUSE>(pa, B, blockIdx.x);
   else inertial_eval_body<K, KB, WANT_J>(ia, B, BB, blockIdx.x - n_pix_blocks);
+}
+template <int K, int KB>
+__global__ void __launch_bounds__(kEvalThreads) factor_eval_det_kernel(PixelArgs pa, InertialArgs ia, Basis B, Basis BB, int n_pix_blocks, DetOut det,
+                                                                       const int* __restrict__ seg_off) {
+  if (static_cast<int>(blockIdx.x) < n_pix_blocks) pixel_eval_body<K, true, true, true>(pa, B, blockIdx.x, det, seg_off);
+  else inertial_eval_body<K, KB, true>(ia, B, BB, blockIdx.x - n_pix_blocks);
 }
 
 

@@ -25,23 +25,32 @@ constexpr int kHessThreads = 128;
 // blocks, gyro-accel coupling is identically zero), gravity-bias, gravity-gravity.  Lower triangle of
 // S only (dof order pose < gyro bias < accel bias < gravity).
 template <int K, int KB>
-__global__ void __launch_bounds__(kHessThreads) inertial_hessian_kernel(const int* __restrict__ run_off, const int4* __restrict__ idx,
-                                                                        const double* __restrict__ r, const double* __restrict__ Jp,
-                                                                        const double* __restrict__ wg, const double* __restrict__ wa,
-                                                                        const double* __restrict__ Jg, double loss_scale, double* sys,
-                                                                        SysLayout lay, int o_bg, int o_ba, int o_g, int splits) {
-  constexpr int NP = 6 * K;
+struct ImuHessScalar {
+  static constexpr int NP = 6 * K;
+  static constexpr int NBP = 3 * KB * NP;                // bias-pose entries (per bias spline)
+  static constexpr int NGP = 2 * NP;                     // gravity-pose
+  static constexpr int NBB = KB * (KB + 1) / 2;          // bias-bias scalar weights (lower), each lands on 3 diagonal entries
+  static constexpr int NGB = 2 * 3 * KB;                 // gravity-bias (per bias spline)
+  static constexpr int NMISC = 2 * NBB + 2 * NGB + 3 + NP + 2 * 3 * KB + 2;   // + gravity-gravity (3) + gradients
+  static constexpr int NT = (NP + 7) / 8, NTL = NT * (NT + 1) / 2;     // pose-pose 8 x 8 tiles (lower) for the FP64 tensor cores
+  static constexpr int TPW = (NTL + kHessThreads / 32 - 1) / (kHessThreads / 32);   // tiles per warp
+  static constexpr int E2 = (NBP + kHessThreads - 1) / kHessThreads;
+  static constexpr int E4 = (NGP + kHessThreads - 1) / kHessThreads;
+  static constexpr int E5 = (NMISC + kHessThreads - 1) / kHessThreads;
+  // writes per thread of the deterministic flush: 3 per pose tile, 2 per bias-pose entry, 1 per gravity-pose entry, at
+  // most 6 per small-block entry (3 bias components, each with its diag(J^T J) entry)
+  static constexpr int DET_WRITES = 3 * TPW + 2 * E2 + E4 + 6 * E5;
+};
+
+template <int K, int KB, bool DET>
+HB_DI void inertial_hessian_body(const int* __restrict__ run_off, const int4* __restrict__ idx, const double* __restrict__ r, const double* __restrict__ Jp,
+                                 const double* __restrict__ wg, const double* __restrict__ wa, const double* __restrict__ Jg, double loss_scale, double* sys,
+                                 SysLayout lay, int o_bg, int o_ba, int o_g, int splits, const DetOut& det) {
+  using H = ImuHessScalar<K, KB>;
+  constexpr int NP = H::NP;
   constexpr int CH = 16;
-  constexpr int NBP = 3 * KB * NP;                // bias-pose entries (per bias spline)
-  constexpr int NGP = 2 * NP;                     // gravity-pose
-  constexpr int NBB = KB * (KB + 1) / 2;          // bias-bias scalar weights (lower), each lands on 3 diagonal entries
-  constexpr int NGB = 2 * 3 * KB;                 // gravity-bias (per bias spline)
-  constexpr int NMISC = 2 * NBB + 2 * NGB + 3 + NP + 2 * 3 * KB + 2;   // + gravity-gravity (3) + gradients
-  constexpr int NT = (NP + 7) / 8, NTL = NT * (NT + 1) / 2;     // pose-pose 8 x 8 tiles (lower) for the FP64 tensor cores
-  constexpr int TPW = (NTL + kHessThreads / 32 - 1) / (kHessThreads / 32);   // tiles per warp
-  constexpr int E2 = (NBP + kHessThreads - 1) / kHessThreads;
-  constexpr int E4 = (NGP + kHessThreads - 1) / kHessThreads;
-  constexpr int E5 = (NMISC + kHessThreads - 1) / kHessThreads;
+  constexpr int NBP = H::NBP, NGP = H::NGP, NBB = H::NBB, NGB = H::NGB, NMISC = H::NMISC, NTL = H::NTL, TPW = H::TPW;
+  constexpr int E2 = H::E2, E4 = H::E4, E5 = H::E5;
   __shared__ double sJ[CH][6][NP + 1];
   __shared__ double sWg[CH][KB], sWa[CH][KB], sG[CH][12], sR[CH][6];
   const int run = blockIdx.x / splits, part = blockIdx.x - run * splits;
@@ -163,7 +172,11 @@ __global__ void __launch_bounds__(kHessThreads) inertial_hessian_kernel(const in
     }
   }
   // ---- flush (loss scaling applied once here: J^T J and J^T r both carry loss_scale) ----
-  double* gv = sys + lay.og;
+  DetCursor dc = det_cursor(det, blockIdx.x, kHessThreads, tid);
+  auto add = [&](long long e, double v) { if constexpr (DET) dc.put(e, v); else atomicAdd(&sys[e], v); };
+  double* gv = nullptr;   // (the deterministic variant has no system pointer)
+  if constexpr (!DET) gv = sys + lay.og;
+  auto addg = [&](int i, double v) { if constexpr (DET) dc.put(lay.og + i, v); else atomicAdd(&gv[i], v); };
   const int cp = 6 * id0.x, cg = o_bg + 3 * id0.y, ca = o_ba + 3 * id0.z;
   const double ls = loss_scale;
 #pragma unroll
@@ -175,10 +188,10 @@ __global__ void __launch_bounds__(kHessThreads) inertial_hessian_kernel(const in
       const int tj = tile - ti * (ti + 1) / 2;
       const int a = 8 * ti + lm, b = 8 * tj + 2 * lk;
       if (a < NP) {
-        if (b < NP && b <= a) atomicAdd(&sys[sys_index(lay, cp + a, cp + b)], ls * a1[2 * q]);
-        if (b + 1 < NP && b + 1 <= a) atomicAdd(&sys[sys_index(lay, cp + a, cp + b + 1)], ls * a1[2 * q + 1]);
-        if (b == a) atomicAdd(&sys[lay.oD + cp + a], ls * a1[2 * q]);               // diag(J^T J), kept apart from S
-        if (b + 1 == a) atomicAdd(&sys[lay.oD + cp + a], ls * a1[2 * q + 1]);
+        if (b < NP && b <= a) add(sys_index(lay, cp + a, cp + b), ls * a1[2 * q]);
+        if (b + 1 < NP && b + 1 <= a) add(sys_index(lay, cp + a, cp + b + 1), ls * a1[2 * q + 1]);
+        if (b == a) add(lay.oD + cp + a, ls * a1[2 * q]);               // diag(J^T J), kept apart from S
+        if (b + 1 == a) add(lay.oD + cp + a, ls * a1[2 * q + 1]);
       }
     }
   }
@@ -187,14 +200,14 @@ __global__ void __launch_bounds__(kHessThreads) inertial_hessian_kernel(const in
     const int id = tid + e * kHessThreads;
     if (id < NBP) {
       const int a = id % NP, mc = id / NP;
-      atomicAdd(&sys[sys_index(lay, cg + mc, cp + a)], ls * a2[e]);
-      atomicAdd(&sys[sys_index(lay, ca + mc, cp + a)], ls * a3[e]);
+      add(sys_index(lay, cg + mc, cp + a), ls * a2[e]);
+      add(sys_index(lay, ca + mc, cp + a), ls * a3[e]);
     }
   }
 #pragma unroll
   for (int e = 0; e < E4; ++e) {
     const int id = tid + e * kHessThreads;
-    if (id < NGP) atomicAdd(&sys[sys_index(lay, o_g + id / NP, cp + id % NP)], ls * a4[e]);
+    if (id < NGP) add(sys_index(lay, o_g + id / NP, cp + id % NP), ls * a4[e]);
   }
 #pragma unroll
   for (int e = 0; e < E5; ++e) {
@@ -211,28 +224,45 @@ __global__ void __launch_bounds__(kHessThreads) inertial_hessian_kernel(const in
         const int c0 = acc_b ? ca : cg;
 #pragma unroll
         for (int c = 0; c < 3; ++c) {
-          atomicAdd(&sys[sys_index(lay, c0 + 3 * m + c, c0 + 3 * m2 + c)], val);
-          if (m == m2) atomicAdd(&sys[lay.oD + c0 + 3 * m + c], val);
+          add(sys_index(lay, c0 + 3 * m + c, c0 + 3 * m2 + c), val);
+          if (m == m2) add(lay.oD + c0 + 3 * m + c, val);
         }
       } else if ((id -= 2 * NBB) < 2 * NGB) {
         const bool acc_b = id >= NGB;
         const int q = acc_b ? id - NGB : id;
         const int gm = q / (3 * KB), mc = q - gm * 3 * KB;
-        atomicAdd(&sys[sys_index(lay, o_g + gm, (acc_b ? ca : cg) + mc)], val);
+        add(sys_index(lay, o_g + gm, (acc_b ? ca : cg) + mc), val);
       } else if ((id -= 2 * NGB) < 3) {
         const int ga = (id == 0) ? 0 : 1, gb = (id == 2) ? 1 : 0;
-        atomicAdd(&sys[sys_index(lay, o_g + ga, o_g + gb)], val);
-        if (ga == gb) atomicAdd(&sys[lay.oD + o_g + ga], val);
+        add(sys_index(lay, o_g + ga, o_g + gb), val);
+        if (ga == gb) add(lay.oD + o_g + ga, val);
       } else if ((id -= 3) < NP) {
-        atomicAdd(&gv[cp + id], val);
+        addg(cp + id, val);
       } else if ((id -= NP) < 2 * 3 * KB) {
         const bool acc_b = id >= 3 * KB;
-        atomicAdd(&gv[(acc_b ? ca : cg) + (acc_b ? id - 3 * KB : id)], val);
+        addg((acc_b ? ca : cg) + (acc_b ? id - 3 * KB : id), val);
       } else {
-        atomicAdd(&gv[o_g + id - 2 * 3 * KB], val);
+        addg(o_g + id - 2 * 3 * KB, val);
       }
     }
   }
+}
+template <int K, int KB>
+__global__ void __launch_bounds__(kHessThreads) inertial_hessian_kernel(const int* __restrict__ run_off, const int4* __restrict__ idx,
+                                                                        const double* __restrict__ r, const double* __restrict__ Jp,
+                                                                        const double* __restrict__ wg, const double* __restrict__ wa,
+                                                                        const double* __restrict__ Jg, double loss_scale, double* sys,
+                                                                        SysLayout lay, int o_bg, int o_ba, int o_g, int splits) {
+  inertial_hessian_body<K, KB, false>(run_off, idx, r, Jp, wg, wa, Jg, loss_scale, sys, lay, o_bg, o_ba, o_g, splits, DetOut{});
+}
+// deterministic assembly: slot = CTA
+template <int K, int KB>
+__global__ void __launch_bounds__(kHessThreads) inertial_hessian_det_kernel(const int* __restrict__ run_off, const int4* __restrict__ idx,
+                                                                            const double* __restrict__ r, const double* __restrict__ Jp,
+                                                                            const double* __restrict__ wg, const double* __restrict__ wa,
+                                                                            const double* __restrict__ Jg, double loss_scale, SysLayout lay,
+                                                                            int o_bg, int o_ba, int o_g, int splits, DetOut det) {
+  inertial_hessian_body<K, KB, true>(run_off, idx, r, Jp, wg, wa, Jg, loss_scale, nullptr, lay, o_bg, o_ba, o_g, splits, det);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -274,13 +304,15 @@ HB_DI void imu_hess_steps(double (&c0)[ImuHess<K, KB>::PER_WARP], double (&c1)[I
   }
 }
 
+// writes per thread of the deterministic flush: two accumulators per tile, each an entry of S and one of diag(J^T J)
+template <int K, int KB>
+__host__ __device__ constexpr int imu_hess_mma_det_writes() { return 4 * ImuHess<K, KB>::PER_WARP; }
+
 // CH: factors per chunk (static shared memory: 6 CH rows of pitch 60 / 68 doubles, <= 48 KB -> 16 / 12 at most)
-template <int K, int KB, int CH>
-__global__ void __launch_bounds__(kHessThreads) inertial_hessian_mma_kernel(const int* __restrict__ run_off, const int4* __restrict__ idx,
-                                                                            const double* __restrict__ r, const double* __restrict__ Jp,
-                                                                            const double* __restrict__ wg, const double* __restrict__ wa,
-                                                                            const double* __restrict__ Jg, double loss_scale, double* sys,
-                                                                            SysLayout lay, int o_bg, int o_ba, int o_g, int splits) {
+template <int K, int KB, int CH, bool DET>
+HB_DI void inertial_hessian_mma_body(const int* __restrict__ run_off, const int4* __restrict__ idx, const double* __restrict__ r, const double* __restrict__ Jp,
+                                     const double* __restrict__ wg, const double* __restrict__ wa, const double* __restrict__ Jg, double loss_scale, double* sys,
+                                     SysLayout lay, int o_bg, int o_ba, int o_g, int splits, const DetOut& det) {
   using H = ImuHess<K, KB>;
   constexpr int NP = H::NP, NBG = H::NBG, NA = H::NA, NT = H::NT, NTL = H::NTL, LD = ImuHessLD<K, KB>::value;
   static_assert(LD >= 8 * NT && (LD % 16 == 4 || LD % 16 == 12), "row pitch: conflict-free fragment loads");
@@ -328,7 +360,9 @@ __global__ void __launch_bounds__(kHessThreads) inertial_hessian_mma_kernel(cons
     else imu_hess_steps<K, KB, 3>(c0, c1, sJ, krows, lm, lk);
   }
   // ---- flush: entry (a, b), a >= b, of the augmented product (loss scaling applied once here) ----
-  double* gv = sys + lay.og;
+  DetCursor dc = det_cursor(det, blockIdx.x, kHessThreads, tid);
+  auto add = [&](long long e, double v) { if constexpr (DET) dc.put(e, v); else atomicAdd(&sys[e], v); };
+  const long long gv = lay.og;
   const int cp = 6 * id0.x, cg = o_bg + 3 * id0.y, ca = o_ba + 3 * id0.z;
   const double ls = loss_scale;
   auto dof = [&](int a) -> int {   // augmented column -> reduced-system dof
@@ -340,7 +374,7 @@ __global__ void __launch_bounds__(kHessThreads) inertial_hessian_mma_kernel(cons
   auto flush = [&](int a, int b, double v) {
     if (a >= NA || b > a) return;
     if (a == NA - 1) {                         // last row: J^T r
-      if (b < NA - 1) atomicAdd(&gv[dof(b)], ls * v);
+      if (b < NA - 1) add(gv + dof(b), ls * v);
       return;
     }
     if (a >= NP && a < NP + 2 * NBG && b >= NP) {   // bias x bias: only equal components of the same sensor
@@ -348,8 +382,8 @@ __global__ void __launch_bounds__(kHessThreads) inertial_hessian_mma_kernel(cons
       if ((a - NP) % 3 != (b - NP) % 3) return;
     }
     const int da = dof(a), db = dof(b);
-    atomicAdd(&sys[sys_index(lay, da, db)], ls * v);
-    if (a == b) atomicAdd(&sys[lay.oD + da], ls * v);   // diag(J^T J), kept apart from S
+    add(sys_index(lay, da, db), ls * v);
+    if (a == b) add(lay.oD + da, ls * v);   // diag(J^T J), kept apart from S
   };
 #pragma unroll
   for (int q = 0; q < H::PER_WARP; ++q) {
@@ -362,12 +396,33 @@ __global__ void __launch_bounds__(kHessThreads) inertial_hessian_mma_kernel(cons
     }
   }
 }
+template <int K, int KB, int CH>
+__global__ void __launch_bounds__(kHessThreads) inertial_hessian_mma_kernel(const int* __restrict__ run_off, const int4* __restrict__ idx,
+                                                                            const double* __restrict__ r, const double* __restrict__ Jp,
+                                                                            const double* __restrict__ wg, const double* __restrict__ wa,
+                                                                            const double* __restrict__ Jg, double loss_scale, double* sys,
+                                                                            SysLayout lay, int o_bg, int o_ba, int o_g, int splits) {
+  inertial_hessian_mma_body<K, KB, CH, false>(run_off, idx, r, Jp, wg, wa, Jg, loss_scale, sys, lay, o_bg, o_ba, o_g, splits, DetOut{});
+}
+// deterministic assembly: slot = CTA
+template <int K, int KB, int CH>
+__global__ void __launch_bounds__(kHessThreads) inertial_hessian_mma_det_kernel(const int* __restrict__ run_off, const int4* __restrict__ idx,
+                                                                                const double* __restrict__ r, const double* __restrict__ Jp,
+                                                                                const double* __restrict__ wg, const double* __restrict__ wa,
+                                                                                const double* __restrict__ Jg, double loss_scale, SysLayout lay,
+                                                                                int o_bg, int o_ba, int o_g, int splits, DetOut det) {
+  inertial_hessian_mma_body<K, KB, CH, true>(run_off, idx, r, Jp, wg, wa, Jg, loss_scale, nullptr, lay, o_bg, o_ba, o_g, splits, det);
+}
 
 // J^T J / J^T r of the manifold (pose) factors: one warp per factor, lower triangle of its 6K x 6K block.
 constexpr int kManWarps = 4;
+// writes per lane of the deterministic variant: an entry of S and one of diag(J^T J) per pass over the block, the gradient
 template <int K>
-__global__ void __launch_bounds__(kManWarps * 32) manifold_hessian_kernel(int nf, const int2* __restrict__ idx, const double* __restrict__ r,
-                                                                         const double* __restrict__ Jp, double* sys, SysLayout lay) {
+__host__ __device__ constexpr int manifold_det_writes() { return 2 * ((36 * K * K + 31) / 32) + (6 * K + 31) / 32; }
+
+template <int K, bool DET>
+HB_DI void manifold_hessian_body(int nf, const int2* __restrict__ idx, const double* __restrict__ r, const double* __restrict__ Jp, double* sys, SysLayout lay,
+                                 const DetOut& det) {
   constexpr int NB = 6 * K;
   __shared__ double sJ[kManWarps][6][NB];
   __shared__ double sr[kManWarps][6];
@@ -377,23 +432,37 @@ __global__ void __launch_bounds__(kManWarps * 32) manifold_hessian_kernel(int nf
   for (int e = lane; e < 6 * NB; e += 32) sJ[warp][e / NB][e % NB] = Jp[static_cast<size_t>(f) * 6 * NB + e];
   if (lane < 6) sr[warp][lane] = r[6 * static_cast<size_t>(f) + lane];
   __syncwarp();
+  DetCursor dc = det_cursor(det, f, 32, lane);   // slot = factor
+  auto add = [&](long long e, double v) { if constexpr (DET) dc.put(e, v); else atomicAdd(&sys[e], v); };
   const int c0 = 6 * idx[f].x;
-  double* g = sys + lay.og;
+  double* g = nullptr;   // (the deterministic variant has no system pointer)
+  if constexpr (!DET) g = sys + lay.og;
   for (int e = lane; e < NB * NB; e += 32) {
     const int a = e / NB, b = e - a * NB;
     if (b > a) continue;
     double s = 0;
 #pragma unroll
     for (int q = 0; q < 6; ++q) s += sJ[warp][q][a] * sJ[warp][q][b];
-    atomicAdd(&sys[sys_index(lay, c0 + a, c0 + b)], s);
-    if (a == b) atomicAdd(&sys[lay.oD + c0 + a], s);
+    add(sys_index(lay, c0 + a, c0 + b), s);
+    if (a == b) add(lay.oD + c0 + a, s);
   }
   for (int a = lane; a < NB; a += 32) {
     double s = 0;
 #pragma unroll
     for (int q = 0; q < 6; ++q) s += sJ[warp][q][a] * sr[warp][q];
-    atomicAdd(&g[c0 + a], s);
+    if constexpr (DET) dc.put(lay.og + c0 + a, s);
+    else atomicAdd(&g[c0 + a], s);
   }
+}
+template <int K>
+__global__ void __launch_bounds__(kManWarps * 32) manifold_hessian_kernel(int nf, const int2* __restrict__ idx, const double* __restrict__ r,
+                                                                         const double* __restrict__ Jp, double* sys, SysLayout lay) {
+  manifold_hessian_body<K, false>(nf, idx, r, Jp, sys, lay, DetOut{});
+}
+template <int K>
+__global__ void __launch_bounds__(kManWarps * 32) manifold_hessian_det_kernel(int nf, const int2* __restrict__ idx, const double* __restrict__ r,
+                                                                             const double* __restrict__ Jp, SysLayout lay, DetOut det) {
+  manifold_hessian_body<K, true>(nf, idx, r, Jp, nullptr, lay, det);
 }
 
 // cost at the linearisation point = sum of the evaluation kernels' per-block partials (fixed order) -> scal[0] of
@@ -445,13 +514,17 @@ HB_DI void lm_lsolve(const double* f, double x0, double x1, double x2, double* y
   y[2] = (x2 - f[3] * y[0] - f[4] * y[1]) * f[5];
 }
 
-template <int K>
-__global__ void __launch_bounds__(kSchurThreads) schur_kernel(const int* __restrict__ lm_off, const int* __restrict__ lm_obs,
-                                                              const int4* __restrict__ idx, const double* __restrict__ r,
-                                                              const double* __restrict__ Jp, const double* __restrict__ Jl, const double* __restrict__ wv,
-                                                              const SolverState* __restrict__ st, double* sys, SysLayout lay,
-                                                              double* __restrict__ Vchol, double* __restrict__ gl, double* __restrict__ Dl,
-                                                              int max_rows) {
+// writes per thread of the deterministic variant: b over the rows, then the lower triangle of Y Y^T
+__host__ __device__ inline long long schur_det_writes(int max_rows) {
+  return (max_rows + kSchurThreads - 1) / kSchurThreads + (static_cast<long long>(max_rows) * max_rows + kSchurThreads - 1) / kSchurThreads;
+}
+
+// DET: every entry the landmark's rows cover is written (zeros included), into the landmark's slot
+template <int K, bool DET>
+HB_DI void schur_body(const int* __restrict__ lm_off, const int* __restrict__ lm_obs, const int4* __restrict__ idx, const double* __restrict__ r,
+                      const double* __restrict__ Jp, const double* __restrict__ Jl, const double* __restrict__ wv, const SolverState* __restrict__ st,
+                      double* sys, SysLayout lay, double* __restrict__ Vchol, double* __restrict__ gl, double* __restrict__ Dl, int max_rows,
+                      const DetOut& det) {
   constexpr int NB = 6 * K;
   extern __shared__ double s_dyn[];
   double* W = s_dyn;                  // [rows][3]
@@ -518,20 +591,40 @@ __global__ void __launch_bounds__(kSchurThreads) schur_kernel(const int* __restr
   }
   __syncthreads();
   const int r0g = 6 * cp_lo;
+  DetCursor dc = det_cursor(det, l, kSchurThreads, threadIdx.x);
+  auto add = [&](long long e, double v) { if constexpr (DET) dc.put(e, v); else atomicAdd(&sys[e], v); };
   for (int row = threadIdx.x; row < rows; row += kSchurThreads) {
     double y[3];
     lm_lsolve(sF, W[3 * row], W[3 * row + 1], W[3 * row + 2], y);
     Y[3 * row] = y[0]; Y[3 * row + 1] = y[1]; Y[3 * row + 2] = y[2];
     const double val = y[0] * sF[6] + y[1] * sF[7] + y[2] * sF[8];
-    if (val != 0.0) atomicAdd(&sys[lay.ob + r0g + row], val);
+    if (DET || val != 0.0) add(lay.ob + r0g + row, val);
   }
   __syncthreads();
   for (int e = threadIdx.x; e < rows * rows; e += kSchurThreads) {
     const int a = e / rows, b = e - a * rows;
     if (b > a) continue;
     const double val = Y[3 * a] * Y[3 * b] + Y[3 * a + 1] * Y[3 * b + 1] + Y[3 * a + 2] * Y[3 * b + 2];
-    if (val != 0.0) atomicAdd(&sys[sys_index(lay, r0g + a, r0g + b)], -val);
+    if (DET || val != 0.0) add(sys_index(lay, r0g + a, r0g + b), -val);
   }
+}
+template <int K>
+__global__ void __launch_bounds__(kSchurThreads) schur_kernel(const int* __restrict__ lm_off, const int* __restrict__ lm_obs,
+                                                              const int4* __restrict__ idx, const double* __restrict__ r,
+                                                              const double* __restrict__ Jp, const double* __restrict__ Jl, const double* __restrict__ wv,
+                                                              const SolverState* __restrict__ st, double* sys, SysLayout lay,
+                                                              double* __restrict__ Vchol, double* __restrict__ gl, double* __restrict__ Dl,
+                                                              int max_rows) {
+  schur_body<K, false>(lm_off, lm_obs, idx, r, Jp, Jl, wv, st, sys, lay, Vchol, gl, Dl, max_rows, DetOut{});
+}
+template <int K>
+__global__ void __launch_bounds__(kSchurThreads) schur_det_kernel(const int* __restrict__ lm_off, const int* __restrict__ lm_obs,
+                                                                  const int4* __restrict__ idx, const double* __restrict__ r,
+                                                                  const double* __restrict__ Jp, const double* __restrict__ Jl, const double* __restrict__ wv,
+                                                                  const SolverState* __restrict__ st, SysLayout lay,
+                                                                  double* __restrict__ Vchol, double* __restrict__ gl, double* __restrict__ Dl,
+                                                                  int max_rows, DetOut det) {
+  schur_body<K, true>(lm_off, lm_obs, idx, r, Jp, Jl, wv, st, nullptr, lay, Vchol, gl, Dl, max_rows, det);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -547,13 +640,17 @@ __global__ void __launch_bounds__(kSchurThreads) schur_kernel(const int* __restr
 // ---------------------------------------------------------------------------------------------
 constexpr int kSchurGroup = 32;       // landmarks per group (3 * 32 = 96 contraction rows)
 constexpr int kSchurGThreads = 128;
-template <int K>
-__global__ void __launch_bounds__(kSchurGThreads) schur_group_kernel(const int* __restrict__ group_off, const int* __restrict__ lm_order,
-                                                                    const int* __restrict__ lm_off, const int* __restrict__ lm_obs,
-                                                                    const int4* __restrict__ idx, const double* __restrict__ r,
-                                                                    const double* __restrict__ Jp, const double* __restrict__ Jl, const double* __restrict__ wv,
-                                                                    const SolverState* __restrict__ st, double* sys, SysLayout lay,
-                                                                    double* __restrict__ Vchol, double* __restrict__ gl, double* __restrict__ Dl, int RT) {
+// writes per thread of the deterministic variant: two per tile a warp owns, then b over the window's rows
+__host__ __device__ inline long long schur_group_det_writes(int RT) {
+  const int NT = RT / 8, ntiles = NT * (NT + 1) / 2;
+  return 2 * ((ntiles + kSchurGThreads / 32 - 1) / (kSchurGThreads / 32)) + (RT + kSchurGThreads - 1) / kSchurGThreads;
+}
+
+template <int K, bool DET>
+HB_DI void schur_group_body(const int* __restrict__ group_off, const int* __restrict__ lm_order, const int* __restrict__ lm_off, const int* __restrict__ lm_obs,
+                            const int4* __restrict__ idx, const double* __restrict__ r, const double* __restrict__ Jp, const double* __restrict__ Jl,
+                            const double* __restrict__ wv, const SolverState* __restrict__ st, double* sys, SysLayout lay, double* __restrict__ Vchol,
+                            double* __restrict__ gl, double* __restrict__ Dl, int RT, const DetOut& det) {
   constexpr int NB = 6 * K;
   extern __shared__ double s_grp[];
   const int LD = RT + 1;
@@ -681,6 +778,8 @@ __global__ void __launch_bounds__(kSchurGThreads) schur_group_kernel(const int* 
   const int NT = RT / 8, ntiles = NT * (NT + 1) / 2, kk = 3 * cnt;
   const int lm = lane >> 2, lk = lane & 3;
   const int r0g = 6 * tile_lo;
+  DetCursor dc = det_cursor(det, blockIdx.x, kSchurGThreads, tid);   // slot = group
+  auto add = [&](long long e, double v) { if constexpr (DET) dc.put(e, v); else atomicAdd(&sys[e], v); };
   for (int tile = warp; tile < ntiles; tile += kSchurGThreads / 32) {
     int ti = 0;
     while ((ti + 1) * (ti + 2) / 2 <= tile) ++ti;
@@ -696,14 +795,121 @@ __global__ void __launch_bounds__(kSchurGThreads) schur_group_kernel(const int* 
     const int m = 8 * ti + lm, n = 8 * tj + 2 * lk;
     const int row = r0g + m;
     if (row < lay.np) {
-      if (n <= m && c0 != 0.0 && row - 6 * ((r0g + n) / 6) < lay.h) atomicAdd(&sys[sys_index(lay, row, r0g + n)], -c0);
-      if (n + 1 <= m && c1 != 0.0 && row - 6 * ((r0g + n + 1) / 6) < lay.h) atomicAdd(&sys[sys_index(lay, row, r0g + n + 1)], -c1);
+      if (n <= m && (DET || c0 != 0.0) && row - 6 * ((r0g + n) / 6) < lay.h) add(sys_index(lay, row, r0g + n), -c0);
+      if (n + 1 <= m && (DET || c1 != 0.0) && row - 6 * ((r0g + n + 1) / 6) < lay.h) add(sys_index(lay, row, r0g + n + 1), -c1);
     }
   }
   for (int m = tid; m < RT; m += kSchurGThreads) {
     double acc = 0.0;
     for (int k = 0; k < kk; ++k) acc += Ys[k * LD + m] * zs[k];
-    if (acc != 0.0 && r0g + m < lay.np) atomicAdd(&sys[lay.ob + r0g + m], acc);
+    if ((DET || acc != 0.0) && r0g + m < lay.np) add(lay.ob + r0g + m, acc);
+  }
+}
+template <int K>
+__global__ void __launch_bounds__(kSchurGThreads) schur_group_kernel(const int* __restrict__ group_off, const int* __restrict__ lm_order,
+                                                                    const int* __restrict__ lm_off, const int* __restrict__ lm_obs,
+                                                                    const int4* __restrict__ idx, const double* __restrict__ r,
+                                                                    const double* __restrict__ Jp, const double* __restrict__ Jl, const double* __restrict__ wv,
+                                                                    const SolverState* __restrict__ st, double* sys, SysLayout lay,
+                                                                    double* __restrict__ Vchol, double* __restrict__ gl, double* __restrict__ Dl, int RT) {
+  schur_group_body<K, false>(group_off, lm_order, lm_off, lm_obs, idx, r, Jp, Jl, wv, st, sys, lay, Vchol, gl, Dl, RT, DetOut{});
+}
+template <int K>
+__global__ void __launch_bounds__(kSchurGThreads) schur_group_det_kernel(const int* __restrict__ group_off, const int* __restrict__ lm_order,
+                                                                        const int* __restrict__ lm_off, const int* __restrict__ lm_obs,
+                                                                        const int4* __restrict__ idx, const double* __restrict__ r,
+                                                                        const double* __restrict__ Jp, const double* __restrict__ Jl, const double* __restrict__ wv,
+                                                                        const SolverState* __restrict__ st, SysLayout lay,
+                                                                        double* __restrict__ Vchol, double* __restrict__ gl, double* __restrict__ Dl, int RT,
+                                                                        DetOut det) {
+  schur_group_body<K, true>(group_off, lm_order, lm_off, lm_obs, idx, r, Jp, Jl, wv, st, nullptr, lay, Vchol, gl, Dl, RT, det);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Deterministic assembly, second half: the entry -> records index and the fixed-order sums (see DetOut, hb200_eval.cuh).
+// det_index_kernel runs in every deterministic build but works only on the first after the slots were laid out
+// (*ready == 0): it counts the records of every entry, scans the counts, fills each entry's list and sorts it by record
+// position (the one-time cost is measured in DESIGN.md §5.4).  The keys it reads are those the J^T J kernels of the same build wrote just before -- the same every build,
+// since they follow from the window alone.  Cooperative launch (grid syncs between the phases).
+// ---------------------------------------------------------------------------------------------
+constexpr int kDetThreads = 256;
+__global__ void __launch_bounds__(kDetThreads) det_index_kernel(long long nrec, const int* __restrict__ key, int nent, int* __restrict__ cnt,
+                                                                int* __restrict__ off, int* __restrict__ perm, int* __restrict__ ready) {
+  if (*ready) return;   // (uniform across the grid: nothing writes it before the last phase)
+  cg::grid_group grid = cg::this_grid();
+  const long long t0 = static_cast<long long>(blockIdx.x) * kDetThreads + threadIdx.x, nt = static_cast<long long>(gridDim.x) * kDetThreads;
+  for (long long e = t0; e < nent; e += nt) cnt[e] = 0;
+  grid.sync();
+  for (long long p = t0; p < nrec; p += nt) { const int k = key[p]; if (k >= 0) atomicAdd(&cnt[k], 1); }
+  grid.sync();
+  if (blockIdx.x == 0) {   // exclusive scan of the counts -> off[0 .. nent]
+    __shared__ int s_warp[kDetThreads / 32];
+    __shared__ int s_carry;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if (tid == 0) s_carry = 0;
+    __syncthreads();
+    for (int base = 0; base < nent; base += kDetThreads) {
+      const int i = base + tid;
+      const int v = i < nent ? cnt[i] : 0;
+      int x = v;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
+      if (lane == 31) s_warp[warp] = x;
+      __syncthreads();
+      int wsum = 0;
+      for (int w = 0; w < warp; ++w) wsum += s_warp[w];
+      const int incl = x + wsum + s_carry;
+      if (i < nent) off[i] = incl - v;
+      __syncthreads();
+      if (tid == kDetThreads - 1) s_carry = incl;
+      __syncthreads();
+    }
+    if (tid == 0) off[nent] = s_carry;
+  }
+  grid.sync();
+  for (long long e = t0; e < nent; e += nt) cnt[e] = 0;
+  grid.sync();
+  for (long long p = t0; p < nrec; p += nt) {
+    const int k = key[p];
+    if (k >= 0) perm[off[k] + atomicAdd(&cnt[k], 1)] = static_cast<int>(p);
+  }
+  grid.sync();
+  // each entry's list into ascending record position (the fill above is in atomic order).  Heap sort, O(n log n) per
+  // list: a list holds one record per slot covering the entry -- a handful for most entries, but one per inertial CTA for
+  // the gravity entries and one per landmark for the pose entries under the per-landmark Schur kernel (thousands)
+  for (long long e = t0; e < nent; e += nt) {
+    int* a = perm + off[e];
+    const int n = off[e + 1] - off[e];
+    auto sift = [&](int root, int end) {   // max-heap on a[0 .. end)
+      const int v = a[root];
+      int i = root;
+      for (int c = 2 * i + 1; c < end; c = 2 * i + 1) {
+        if (c + 1 < end && a[c + 1] > a[c]) ++c;
+        if (a[c] <= v) break;
+        a[i] = a[c];
+        i = c;
+      }
+      a[i] = v;
+    };
+    for (int i = n / 2 - 1; i >= 0; --i) sift(i, n);
+    for (int end = n - 1; end > 0; --end) {
+      const int t = a[0]; a[0] = a[end]; a[end] = t;
+      sift(0, end);
+    }
+  }
+  if (t0 == 0) *ready = 1;
+}
+
+// every packed entry with records = their sum in ascending record order (the system was cleared by prep_kernel; the
+// entries no slot covers stay zero)
+__global__ void __launch_bounds__(kDetThreads) det_reduce_kernel(int nent, const int* __restrict__ off, const int* __restrict__ perm,
+                                                                 const double* __restrict__ val, double* __restrict__ sys) {
+  for (int e = blockIdx.x * kDetThreads + threadIdx.x; e < nent; e += gridDim.x * kDetThreads) {
+    const int lo = off[e], hi = off[e + 1];
+    if (lo == hi) continue;
+    double s = 0.0;
+    for (int i = lo; i < hi; ++i) s += val[perm[i]];
+    sys[e] = s;
   }
 }
 

@@ -93,6 +93,10 @@ class Optimizer {   // OptimizerSuite::H100
   // defaults (reference optimizer.cpp:38-54): setSolverTolerances() with no arguments switches exactly those on.
   void setSolverTolerances(double function_tolerance = 1e-6, double gradient_tolerance = 1e-10, double parameter_tolerance = 1e-8,
                            double min_trust_region_radius = 1e-32);
+  // Deterministic assembly (hb200_set_deterministic): optimize() and Covariance give bit-identical results when the same
+  // problem is solved again on the same GPU model with the same build, as the reference's single-threaded solve does
+  // (reference optimizer.cpp:38-54).  Off by default.
+  void setDeterministic(bool deterministic);
   // summary.termination_type of the last optimize(): 0 iteration limit, 1 function, 2 parameter, 3 gradient tolerance, 4 radius, 5 invalid steps
   int terminationType() const;
 

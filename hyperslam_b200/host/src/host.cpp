@@ -208,6 +208,7 @@ Optimizer::~Optimizer() { hb200_destroy(ctx_); }
 void Optimizer::setSolverTolerances(double function_tolerance, double gradient_tolerance, double parameter_tolerance, double min_trust_region_radius) {
   check(hb200_set_termination(ctx_, function_tolerance, gradient_tolerance, parameter_tolerance, min_trust_region_radius), "hb200_set_termination");
 }
+void Optimizer::setDeterministic(bool deterministic) { check(hb200_set_deterministic(ctx_, deterministic ? 1 : 0), "hb200_set_deterministic"); }
 int Optimizer::terminationType() const {
   int type = 0;
   hb200_get_termination(ctx_, &type, nullptr, nullptr, nullptr, nullptr);

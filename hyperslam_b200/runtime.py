@@ -66,7 +66,7 @@ EXPORTS = [
     "hb200_window_sizes", "hb200_set_termination", "hb200_get_termination",
     "hb200_append_bearing_factors", "hb200_append_manifold_factors", "hb200_append_stereo_tracks", "hb200_slide_landmark_map",
     "hb200_factor_counts", "hb200_build_covariance", "hb200_compute_covariance", "hb200_get_covariance", "hb200_interpolate_covariance",
-    "hb200_append_bias_knots", "hb200_bias_knots",
+    "hb200_append_bias_knots", "hb200_bias_knots", "hb200_set_deterministic", "hb200_get_deterministic",
 ]
 
 _lib = None
@@ -544,6 +544,17 @@ class Context:
         v = C.c_double(0)
         self._check(self.lib.hb200_measure_fp64_peak(self.h, C.byref(v)))
         return v.value
+
+    def set_deterministic(self, on=True):
+        """Deterministic assembly: the normal equations are summed in an order fixed by the bound window instead of with
+        FP64 atomics, so reruns of the same window and call sequence on the same GPU model and build are bit-identical
+        (hb200_set_deterministic).  Off by default."""
+        self._check(self.lib.hb200_set_deterministic(self.h, 1 if on else 0))
+
+    def deterministic(self) -> bool:
+        v = C.c_int(0)
+        self._check(self.lib.hb200_get_deterministic(self.h, C.byref(v)))
+        return bool(v.value)
 
     def bandwidth(self) -> int:
         b = C.c_int(0)

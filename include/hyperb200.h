@@ -256,6 +256,23 @@ int hb200_cost(hb200_ctx* ctx, double* cost);
  * blocks (knots, biases, gravity) and not the landmarks, and hb200_iterate / hb200_optimize refuse a gradient tolerance > 0. */
 int hb200_set_termination(hb200_ctx* ctx, double function_tolerance, double gradient_tolerance, double parameter_tolerance, double min_trust_region_radius);
 int hb200_get_termination(hb200_ctx* ctx, int* type, int* iterations_performed, double* gradient_max_norm, double* step_norm, double* x_norm);
+/* Deterministic assembly (off by default).  By default the normal-equation kernels add into the packed system with FP64
+ * atomics, so the order of the additions -- and the last bits of S, b and g -- depends on how the GPU schedules them,
+ * and two runs of the same window can take different LM steps.  With it on, every kernel stores its contributions
+ * with plain stores into slots of its own and one reduction kernel sums each packed entry over its slots in an order
+ * fixed by the bound window.  Same build of this library, same GPU model, same window and the same call sequence then
+ * give bit-identical results for:
+ *   - the packed buffer hb200_build_system leaves (hb200_system_device_ptr), hb200_get_system, hb200_solve / hb200_get_delta
+ *   - hb200_iterate / hb200_optimize: records, termination and state
+ *   - hb200_build_covariance + hb200_compute_covariance (hb200_get_covariance) and hb200_interpolate_covariance
+ *   - sharded contexts: each rank's partial system; the peer-memory reduction sums the ranks in rank order.
+ * Not covered: other GPU models or builds, the dense fallback solver (hb200_options.reserved bit 0) and the NCCL
+ * all-reduce (as deterministic as NCCL's reduction).  It costs extra device memory for the slots and time for the
+ * reduction (DESIGN.md §5.4).  May be set before or after hb200_bind; a change drops a built system and a pending
+ * covariance build (as any change of the kernels' arguments does) and takes effect at the next build or iteration,
+ * which then lays out the slots for the window.  Setting the current value changes nothing. */
+int hb200_set_deterministic(hb200_ctx* ctx, int enable);
+int hb200_get_deterministic(hb200_ctx* ctx, int* enable);
 /* The drop-in for CeresOptimizer::optimize() (reference optimizer.cpp:276-280) with the parameter
  * blocks in HOST memory, as Ceres aliases them: uploads the five variable families, runs
  * `iterations` LM iterations on the device, downloads the updated blocks into the same buffers and

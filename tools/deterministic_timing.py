@@ -1,0 +1,102 @@
+#!/usr/bin/env python
+"""LM step time with the default (atomic) assembly and the deterministic assembly (hb200_set_deterministic).
+
+For cfg1, cfg2 and the 1M-factor window (cfg4): one context per mode on the same window, the two modes timed
+alternately in rounds, each step as bench.py times it (device snapshot restored before every step, 256 MiB L2 flush,
+CUDA events around one graph-launched iteration).  Also prints the per-kernel split of one iteration in each mode
+(hb200_profile_iteration), the entry index's one-time cost on the first build after a window change, the extra device
+memory of the deterministic mode (cudaMemGetInfo around its first step) and the card's name and power limit read in the
+same run.  Needs an H100.
+
+  python tools/deterministic_timing.py [--steps 50] [--rounds 4] [--configs 1,2,4]
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+from hyperslam_b200 import runtime, synthetic  # noqa: E402
+
+
+def card():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
+    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else "unknown (nvidia-smi unavailable)"
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=50)
+    ap.add_argument("--rounds", type=int, default=4)
+    ap.add_argument("--configs", default="1,2,4")
+    args = ap.parse_args()
+    import torch
+    if not torch.cuda.is_available():
+        raise SystemExit("no CUDA device")
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device="cuda")
+    out = dict(card=card())
+    for cfg in (int(c) for c in args.configs.split(",")):
+        win = synthetic.make_config(cfg, constant_knots=2)
+        ctxs, mem = {}, {}
+        for mode in ("default", "deterministic"):
+            torch.cuda.synchronize()
+            free0 = torch.cuda.mem_get_info()[0]
+            ctx = runtime.Context(0, use_graph=True)
+            ctx.set_deterministic(mode == "deterministic")
+            ctx.load_window(win)
+            ctx.snapshot()
+            ctx.iterate(1, records=False)
+            ctx.restore()
+            ctx.synchronize()
+            mem[mode] = free0 - torch.cuda.mem_get_info()[0]
+            ctxs[mode] = ctx
+        ext = {m: torch.cuda.ExternalStream(c.stream) for m, c in ctxs.items()}
+        ms = {m: [] for m in ctxs}
+        for _ in range(args.rounds):
+            for mode, ctx in ctxs.items():
+                for _ in range(3):   # warm-up
+                    ctx.restore(); ctx.iterate(1, records=False)
+                ctx.synchronize()
+                ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(args.steps)]
+                for a, b in ev:
+                    ctx.restore()
+                    with torch.cuda.stream(ext[mode]):
+                        flush.fill_(1.0)
+                    a.record(ext[mode])
+                    ctx.iterate(1, records=False)
+                    b.record(ext[mode])
+                ctx.synchronize(); torch.cuda.synchronize()
+                ms[mode].append(sum(a.elapsed_time(b) for a, b in ev) / args.steps)
+        # one-time cost after a window change (append, slide, rebind): the slot layout (host, with two synchronisations)
+        # and the first build's entry index.  Switching the mode off and on drops the layout as a window change does.
+        ctx = ctxs["deterministic"]
+        ctx.restore(); ctx.set_deterministic(False); ctx.set_deterministic(True)
+        torch.cuda.synchronize()
+        first = dict(ctx.profile_iteration(reps=1))
+        ctx.restore()
+        steady = dict(ctx.profile_iteration(reps=1))
+        index_ms = dict(first_build=round(first["det_index_kernel"], 4), later_builds=round(steady["det_index_kernel"], 4))
+        prof = {}
+        for mode, ctx in ctxs.items():
+            ctx.restore()
+            agg = {}
+            for name, t in ctx.profile_iteration(reps=3):
+                agg[name] = round(agg.get(name, 0.0) + t, 4)
+            prof[mode] = agg
+        entry = dict(workload=synthetic.CONFIG_NAMES[cfg], factors=win.num_factors,
+                     ms_per_step={m: dict(per_round=[round(x, 4) for x in v], median=round(sorted(v)[len(v) // 2], 4)) for m, v in ms.items()},
+                     det_index_kernel_ms=index_ms,
+                     extra_device_mb_deterministic=round((mem["deterministic"] - mem["default"]) / 2 ** 20, 1),
+                     iteration_kernel_ms=prof)
+        print(json.dumps(entry), flush=True)
+        out[synthetic.CONFIG_NAMES[cfg].split(":")[0]] = entry
+        for ctx in ctxs.values():
+            ctx.close()
+    print(json.dumps(dict(card=out["card"])))
+
+
+if __name__ == "__main__":
+    main()

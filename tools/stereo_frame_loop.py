@@ -6,7 +6,8 @@ Two variants of the stereo-track step run on two contexts, frame by frame altern
   composed: hb200_ingest_stereo (bearings + landmarks to the host), hb200_append_landmarks, hb200_append_bearing_factors
   device:   hb200_append_stereo_tracks
 Prints one JSON line: median / minimum wall clock per frame of each (host bookkeeping and every copy included), the
-window sizes, and the card's name and power limit read in the same run."""
+window sizes, and the card's name and power limit read in the same run.  --deterministic: both contexts assemble
+deterministically, so every frame also pays the slot layout and the entry index of its new window (DESIGN.md §5.4)."""
 import argparse
 import json
 import os
@@ -30,6 +31,7 @@ def main():
     p = argparse.ArgumentParser()
     p.add_argument("--warm", type=int, default=50, help="frames before timing (the window starts without landmarks and fills up)")
     p.add_argument("--frames", type=int, default=30, help="timed frames per variant")
+    p.add_argument("--deterministic", action="store_true", help="both contexts with the deterministic assembly (hb200_set_deterministic)")
     a = p.parse_args()
     import torch
     if not torch.cuda.is_available():
@@ -51,6 +53,7 @@ def main():
     ctxs = dict(composed=runtime.Context(0), device=runtime.Context(0))
     slots = {name: {} for name in ctxs}   # caller's landmark id -> window slot, per context
     for ctx in ctxs.values():
+        ctx.set_deterministic(a.deterministic)
         ctx.load_window(win)
     times = {name: [] for name in ctxs}
     sizes = {}
@@ -102,7 +105,7 @@ def main():
             sizes[name] = dict(knots=stats["knots"], landmarks=stats["landmarks"], bearing_factors=int(counts[runtime.BEARING]),
                                inertial_factors=int(counts[runtime.INERTIAL]), manifold_factors=int(counts[runtime.MANIFOLD]))
     assert sizes["device"] == sizes["composed"], sizes
-    out = dict(tool="stereo_frame_loop", card=card(), order=k, K0=K0, warm_frames=a.warm, timed_frames=a.frames,
+    out = dict(tool="stereo_frame_loop", card=card(), deterministic=a.deterministic, order=k, K0=K0, warm_frames=a.warm, timed_frames=a.frames,
                window=sizes["device"], per_frame="append 1 state element + the frame's stereo tracks (2 camera frames) + IMU factors (+ 1 pose factor "
                "every 3rd frame), hb200_slide (both drop flags), 5 LM iterations, state read-back; wall clock")
     for name in ctxs:
