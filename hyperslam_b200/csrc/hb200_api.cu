@@ -389,10 +389,10 @@ int with_flag(bool b, F&& f) {
 }
 
 // Launch configuration of the resident band solver: a grid of one 2-CTA cluster (chain r in CTA r) on the context's
-// stream, the whole workspace in each CTA's shared memory.  at: storage for the cluster-dimension attribute.
+// stream, each chain's workspace in its CTA's shared memory.  at: storage for the cluster-dimension attribute.
 void band_cluster_config(hb200_ctx* c, cudaLaunchConfig_t* cfg, cudaLaunchAttribute* at) {
   cfg->gridDim = dim3(2); cfg->blockDim = dim3(kBandThreads); cfg->stream = c->stream;
-  cfg->dynamicSmemBytes = band_workspace_doubles(c->K, c->beta, c->n - 6 * c->K) * sizeof(double);
+  cfg->dynamicSmemBytes = band_cluster_doubles(c->K, c->beta, c->n - 6 * c->K) * sizeof(double);
   at[0].id = cudaLaunchAttributeClusterDimension;
   at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
   cfg->attrs = at; cfg->numAttrs = 1;
@@ -457,7 +457,7 @@ int ensure_system(hb200_ctx* c) {
   // solver selection: block-banded + arrowhead unless the band is wide on a large system
   const size_t ws = band_workspace_doubles(c->K, c->beta, c->n - 6 * c->K) * sizeof(double);
   c->band_solver = !c->force_dense && ((c->n <= 512) || (12 * (c->beta + 1) <= 6 * c->K));
-  c->band_smem = ws <= 220 * 1024;
+  c->band_smem = ws <= kBandSmemBytes;
   c->use_bcr = false;
   if (c->band_solver && !c->band_smem && 6 * c->beta <= kBcrMaxNb && c->n - 6 * c->K <= 54) {
     // the band does not fit one CTA's shared memory: cyclic reduction over super-blocks of beta control points
@@ -485,14 +485,14 @@ int ensure_system(hb200_ctx* c) {
   }
   if (c->band_solver && !c->use_bcr) {
     if (c->band_smem) {
-      // resident workspace: one chain per CTA of a 2-CTA cluster, ws bytes of shared memory in each
-      HB_CUDA(cudaFuncSetAttribute(band_solve_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(ws)));
+      // resident workspace: one chain per CTA of a 2-CTA cluster, each CTA with its own chain's workspace
       cudaLaunchConfig_t cfg{};
       cudaLaunchAttribute at[1];
       band_cluster_config(c, &cfg, at);
+      HB_CUDA(cudaFuncSetAttribute(band_solve_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(cfg.dynamicSmemBytes)));
       int nclusters = 0;
       HB_CUDA(cudaOccupancyMaxActiveClusters(&nclusters, band_solve_kernel<true>, &cfg));
-      if (nclusters < 1) return fail(-6, "band solver: a cluster of 2 CTAs x %d threads with %zu B of shared memory each cannot be resident", kBandThreads, ws);
+      if (nclusters < 1) return fail(-6, "band solver: a cluster of 2 CTAs x %d threads with %zu B of shared memory each cannot be resident", kBandThreads, cfg.dynamicSmemBytes);
     } else {
       HB_CUDA(c->band_ws.ensure(ws / sizeof(double)));
       // chunked factorisation: two shared-memory views of band_chunk_cols block columns (band + arrow + LI)
@@ -2471,7 +2471,7 @@ int hb200_interpolate(hb200_ctx* c, int n, const double* stamps, double* pose, d
   return 0;
 }
 
-int hb200_debug_band_timing(hb200_ctx* c, long long* cycles /*[144]: per CTA, 8 phase totals + 8 steps x 8 raw stamps*/) {
+int hb200_debug_band_timing(hb200_ctx* c, long long* cycles /*[144]: per CTA, 8 phase totals + 8 steps x 8 raw stamps; [70]: SPD flag of the solve*/) {
   if (!c || !c->band_dbg.p) return fail(-2, "set HB200_BAND_TIMING=1 before hb200_bind");
   HB_CUDA(cudaMemcpy(cycles, c->band_dbg.p, 144 * sizeof(long long), cudaMemcpyDeviceToHost));
   return 0;

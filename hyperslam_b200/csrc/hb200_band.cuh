@@ -55,6 +55,53 @@ __host__ __device__ inline size_t band_workspace_doubles(int K, int beta, int m)
   return d + 8;
 }
 
+// Shared-memory budget of one CTA of the band solvers.
+constexpr size_t kBandSmemBytes = 220 * 1024;
+
+// Chain of CTA `rank` of the resident solver (band_plan): Ke block columns it eliminates, then the bs separator columns
+// it stores (ncol in all); forward from block column 0 (rank 0) or reversed from K (rank 1).  Chain 0 eliminates the
+// separator (elim).
+struct SegChain { int Ke, ncol, anchor; bool rev, elim; };
+__host__ __device__ inline SegChain seg_chain(const BandPlan& pl, int K, int rank) {
+  SegChain c;
+  c.Ke = rank ? pl.Kb : pl.Kt;
+  c.ncol = c.Ke ? c.Ke + pl.bs : 0;
+  c.rev = rank == 1;
+  c.elim = pl.bs > 0 && rank == 0;
+  c.anchor = rank ? K : 0;
+  return c;
+}
+
+// Per-CTA workspace of the resident solver, offsets in doubles: the CTA's own chain only (W, AR, LI, X as in
+// band_workspace_doubles), the receive buffer of the separator copy the other chain stores (elim: RBW band block columns,
+// RBA arrow columns + rhs), the corner CC (CTA 0: the corner system; CTA 1: its partial sum of the corner update), XA + DG
+// and the staging.
+struct CtaLayout { size_t W, AR, LI, X, RBW, RBA, CC, XA, total; };
+__host__ __device__ inline CtaLayout cta_layout(const BandPlan& pl, int K, int beta, int m, int rank) {
+  const SegChain g = seg_chain(pl, K, rank);
+  const size_t h6 = 36 + 36 * static_cast<size_t>(beta), npc = 6 * static_cast<size_t>(g.ncol);
+  CtaLayout L;
+  size_t p = 0;
+  L.W = p; p += g.ncol * h6;
+  L.AR = p; p += static_cast<size_t>(m + 1) * npc;
+  L.LI = p; p += g.ncol * 48;
+  L.X = p; p += npc;
+  L.RBW = p; if (g.elim) p += pl.bs * h6;
+  L.RBA = p; if (g.elim) p += static_cast<size_t>(m + 1) * 6 * pl.bs;
+  L.CC = p; p += static_cast<size_t>(m + 1) * (m | 1);
+  L.XA = p; p += 2 * static_cast<size_t>(m);
+  p += 6 * static_cast<size_t>(K) + m + (6 * static_cast<size_t>(K) + m) / 8 + 1;
+  L.total = p + 8;
+  return L;
+}
+
+// Dynamic shared memory of each CTA of the resident solver's cluster (the larger CTA workspace).
+__host__ __device__ inline size_t band_cluster_doubles(int K, int beta, int m) {
+  const BandPlan pl = band_plan(K, beta);
+  const size_t d0 = cta_layout(pl, K, beta, m, 0).total, d1 = cta_layout(pl, K, beta, m, 1).total;
+  return d0 > d1 ? d0 : d1;
+}
+
 // Right-looking Cholesky of a 6x6 SPD block (lower, row-major with stride ld), division-free:
 // inv[j] = 1 / L[j][j] comes straight out of rsqrt.  If X != nullptr the block first receives its
 // pending trailing update A -= X X^T (X = the 6 panel rows of this block, row-major 6x6), so the
@@ -147,6 +194,7 @@ struct BandChain {
   int ncol;   // block columns it stores (Ke + separator)
   int npc;    // 6 * ncol
   int ars;    // row stride of AR in doubles (= npc for a whole chain; the chunk capacity for a shared-memory view)
+  int ne;     // block columns whose factor the chain holds (Ke, + the separator if it eliminates it)
 };
 
 // Panel of block column s: solve x L^T = a for every row below the diagonal block (band rows, arrow rows,
@@ -353,17 +401,20 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
   extern __shared__ double s_band[];
   const long long t_entry = clock64();
   // SMEM: the workspace is resident in shared memory and the kernel runs as a 2-CTA cluster, chain r in CTA r, each
-  // chain on its own SM (its own shared-memory crossbar and four schedulers).  Both CTAs lay out the whole workspace
-  // identically, so a peer's copy of anything sits at the local address mapped to the peer's rank.  CTA 0 also owns
-  // the corner.  !SMEM: one CTA runs both chains on chunked shared-memory views of a global workspace.
+  // chain on its own SM (its own shared-memory crossbar and four schedulers).  Each CTA lays out only its own chain
+  // (cta_layout); either CTA can compute the other's layout and the dynamic shared memory starts at the same address in
+  // both, so a peer's array sits at the local address mapped to the peer's rank.  CTA 0 (the hub) also owns the corner.
+  // !SMEM: one CTA runs both chains on chunked shared-memory views of a global workspace.
   constexpr bool CL = SMEM;
   const int rank = CL ? cluster_rank() : 0;
-  const bool has0 = !CL || rank == 0, has1 = !CL || rank == 1;
-  if (CL && dbg) dbg += 72 * rank;
-  double* ws = SMEM ? s_band : ws_global;
   const int n = lay.n, K = lay.K, beta = lay.beta;
   const int np = 6 * K, m = n - np, h = 6 + 6 * beta, h6 = h * 6;
   const BandPlan pl = band_plan(K, beta);
+  const SegChain g = seg_chain(pl, K, rank);
+  const bool hub = !CL || rank == 0;
+  const bool has0 = !CL || !g.rev, has1 = !CL || g.rev;   // CL: the CTA's chain is forward (C0) or reversed (C1)
+  if (CL && dbg) dbg += 72 * rank;
+  double* ws = SMEM ? s_band : ws_global;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   // Roles (!CL).  Each chain owns one scheduler for its latency-critical work (the arbiter favours the highest
   // warp id of a scheduler): scheduler 0 = chain 0 (warp 12 look-ahead, warp 8 lane 0 block inverses),
@@ -372,9 +423,24 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
   // Roles (CL).  Warp 15 is the look-ahead warp, alone on scheduler 3 (warps 3, 7, 11 idle in the step loop); the
   // first kBandUpdWarps warps of schedulers 0..2, in the order 0, 1, 2, 4, 5, 6, 8, ..., do panel rows and updates.
   const int sched = warp & 3;
-  const int my_chain = CL ? rank : ((sched < 2) ? sched : (warp >> 3));
+  const int my_chain = CL ? (g.rev ? 1 : 0) : ((sched < 2) ? sched : (warp >> 3));
   BandChain C0, C1;
-  {
+  int o0 = 0, e1 = K;   // natural block column of C0's column 0; one past the natural block column of C1's column 0
+  double* CC;
+  int LDc;
+  if (CL) {
+    const CtaLayout L = cta_layout(pl, K, beta, m, rank);
+    BandChain own;
+    own.W = ws + L.W; own.AR = ws + L.AR; own.LI = ws + L.LI; own.X = ws + L.X;
+    own.Ke = g.Ke; own.ncol = g.ncol; own.npc = own.ars = 6 * g.ncol;
+    own.ne = g.elim ? g.ncol : g.Ke;
+    BandChain none = own;
+    none.Ke = none.ncol = none.npc = none.ars = none.ne = 0;
+    C0 = g.rev ? none : own; C1 = g.rev ? own : none;
+    (g.rev ? e1 : o0) = g.anchor;
+    CC = ws + L.CC;
+    LDc = m | 1;
+  } else {
     double* p = ws;
     BandChain* cc[2] = {&C0, &C1};
     for (int i = 0; i < 2; ++i) {
@@ -383,18 +449,17 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
       C.ncol = (i && pl.Kb == 0) ? 0 : C.Ke + pl.bs;
       C.npc = 6 * C.ncol;
       C.ars = C.npc;
+      C.ne = i ? C.Ke : C.ncol;
       C.W = p; p += static_cast<size_t>(C.ncol) * h6;
       C.AR = p; p += static_cast<size_t>(m + 1) * C.npc;
       C.LI = p; p += static_cast<size_t>(C.ncol) * 48;
       C.X = p; p += C.npc;
     }
-    ws = p;
+    CC = p;
+    LDc = m | 1;
   }
-  double* CC = ws;
-  const int LDc = m | 1;
   double* XA = CC + static_cast<size_t>(m + 1) * LDc;   // (both move to shared memory after the factorisation when !SMEM)
   const BandChain C = my_chain ? C1 : C0;           // this thread's chain in the update phase (registers)
-  const BandChain CP = (tid >> 8) ? C1 : C0;        // ... and in the panel phase (threads 0..255 / 256..511)
   const double* S = sys;                 // band-only storage: P at offset 0 in the chain-0 column layout
   const double* b = sys + lay.ob;
   // Dout != null: the system is the raw accumulation (lower triangle of H with the Schur complement applied,
@@ -411,7 +476,7 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
       const double dcl = damp ? fmin(fmax(diagH[a], 1e-6), 1e32) : 0.0;
       s_dmp[a] = mu * dcl;
       s_fix[a] = damp ? fixed[a] : 0;
-      if (damp && has0) Dout[a] = dcl;
+      if (damp && hub) Dout[a] = dcl;
     }
   }
   __syncthreads();
@@ -477,15 +542,15 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
           const int u = u0 + w * kBandThreads;
           const int c = u / h, i = u - c * h;
           rowv[w] = 6 * c + i; cv[w] = c;
-          if (u < nu0 && rowv[w] < C0.npc) load6(rowv[w], 6 * c, v[w]);
+          if (u < nu0 && rowv[w] < C0.npc) load6(6 * o0 + rowv[w], 6 * (o0 + c), v[w]);
           else { for (int t = 0; t < 6; ++t) v[w][t] = 0.0; rowv[w] = -1; }
         }
 #pragma unroll
         for (int w = 0; w < 2; ++w) {
           const int u = u0 + w * kBandThreads;
           const int c = u / (hq * 6), rem = u - c * hq * 6, q = rem / 6, j = rem - 6 * q;
-          av[w] = np - 1 - (6 * c + j);
-          b0v[w] = np - 6 * (c + q) - 6;
+          av[w] = 6 * e1 - 1 - (6 * c + j);
+          b0v[w] = 6 * e1 - 6 * (c + q) - 6;
           if (u < nu1 && b0v[w] >= 0) load6(av[w], b0v[w], v1[w]);
           else { for (int t = 0; t < 6; ++t) v1[w][t] = 0.0; av[w] = -1; }
         }
@@ -493,7 +558,7 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
         for (int w = 0; w < 2; ++w) {
           const int u = u0 + w * kBandThreads;
           if (u >= nu0) continue;
-          if (rowv[w] >= 0) fix6(rowv[w], 6 * cv[w], v[w]);
+          if (rowv[w] >= 0) fix6(6 * o0 + rowv[w], 6 * (o0 + cv[w]), v[w]);
           double* dst = C0.W + static_cast<size_t>(u) * 6;
 #pragma unroll
           for (int t = 0; t < 6; ++t) dst[t] = v[w][t];
@@ -528,9 +593,9 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
             const double* src = Arows + static_cast<size_t>((on && !rhs) ? r : 0) * np;
 #pragma unroll
             for (int u = 0; u < 6; ++u) {
-              const int col = c0 + lane + 32 * u;
-              v0[w][u] = (on && col < N0) ? (rhs ? b[col] - gvec[col] : src[col]) : 0.0;
-              const int col1 = np - 1 - col;
+              const int col = c0 + lane + 32 * u, col0 = 6 * o0 + col;
+              v0[w][u] = (on && col < N0) ? (rhs ? b[col0] - gvec[col0] : src[col0]) : 0.0;
+              const int col1 = 6 * e1 - 1 - col;
               v1[w][u] = (on && col < n1v) ? (rhs ? b[col1] - gvec[col1] : src[col1]) : 0.0;
             }
           }
@@ -541,8 +606,8 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
             const bool rfix = (r < m) && s_fix[np + r];
 #pragma unroll
             for (int u = 0; u < 6; ++u) {
-              const int col = c0 + lane + 32 * u, col1 = np - 1 - col;
-              if (col < N0) C0.AR[static_cast<size_t>(r) * N0 + col] = (rfix || s_fix[col]) ? 0.0 : v0[w][u];
+              const int col = c0 + lane + 32 * u, col1 = 6 * e1 - 1 - col;
+              if (col < N0) C0.AR[static_cast<size_t>(r) * N0 + col] = (rfix || s_fix[6 * o0 + col]) ? 0.0 : v0[w][u];
               if (col < N1) C1.AR[static_cast<size_t>(r) * N1 + col] = (col < n1v && !(rfix || s_fix[col1])) ? v1[w][u] : 0.0;
             }
           }
@@ -551,7 +616,7 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
     }
     t_g[2] = clock64();
     t_g[3] = clock64();
-    for (int e = tid; has0 && e < (m + 1) * m; e += kBandThreads) {
+    for (int e = tid; hub && e < (m + 1) * m; e += kBandThreads) {
       const int r = e / m, q = e - r * m;
       CC[static_cast<size_t>(r) * LDc + q] = (r < m) ? ((q <= r) ? Sval(np + r, np + q) : 0.0) : bval(np + q);
     }
@@ -724,89 +789,28 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
   __syncthreads();
   if (dbg && tid < 64) dbg[8 + tid] = s_ts[tid >> 3][tid & 7];
   HB_TICKD(1, C.W);
-  // CL: CTA 1 stores chain 1's separator copy and its separator arrow columns into CTA 0's (unused) chain-1 storage at
-  // the same addresses: remote stores do not stall the way remote loads in the merge would.  Both chains are then
-  // eliminated (cluster barrier 1).  CTA 0 arrives on barrier 2 at once: it waits there for CTA 1's part of the corner
-  // update, and CTA 1 has nothing to wait for from CTA 0 until the corner is solved (barrier 3).
-  if (CL) {
-    if (rank == 1 && pl.Kb) {
-      const int nsep = 6 * pl.bs;
-      double* w = C1.W + static_cast<size_t>(C1.Ke) * h6;
-      for (int e = tid; e < pl.bs * h6; e += kBandThreads) st_peer(w + e, 0, w[e]);
-      for (int e = tid; e < (m + 1) * nsep; e += kBandThreads) {
-        const int r = e / nsep, v = e - r * nsep;
-        double* a = C1.AR + static_cast<size_t>(r) * C1.npc + 6 * C1.Ke + v;
-        st_peer(a, 0, *a);
-      }
-    }
-    cluster_arrive(); cluster_wait();
-    if (rank == 0) {
-      if (tid == 0 && !ld_peer(&s_ok, 1)) s_ok = 0;   // chain 1's SPD flag
-      cluster_arrive();
-    }
-  }
-  // ---- merge chain 1's copy of the separator (index-reversed) and of its arrow columns into chain 0,
-  // then chain 0's pipeline eliminates the separator columns ----
-  if (pl.Kb && has0) {
-    const int nsep = 6 * pl.bs, N1 = C1.npc;
-    for (int e = tid; e < nsep * nsep; e += kBandThreads) {
-      const int u = e / nsep, v = e - u * nsep;
-      if (v > u) continue;
-      const int ru = N1 - 1 - u, rv = N1 - 1 - v;   // ru <= rv: stored in block column ru / 6
-      C0.W[(static_cast<size_t>(C0.Ke + v / 6) * h + (u - 6 * (v / 6))) * 6 + v % 6] +=
-          C1.W[(static_cast<size_t>(ru / 6) * h + (rv - 6 * (ru / 6))) * 6 + ru % 6];
-    }
-    for (int e = tid; e < (m + 1) * nsep; e += kBandThreads) {
-      const int r = e / nsep, v = e - r * nsep;
-      C0.AR[static_cast<size_t>(r) * C0.npc + 6 * C0.Ke + v] += C1.AR[static_cast<size_t>(r) * N1 + (N1 - 1 - v)];
-    }
-    __syncthreads();
-    if (tid == 0 && !chol6(C0.W + static_cast<size_t>(C0.Ke) * h6, 6, C0.LI + static_cast<size_t>(C0.Ke) * 48)) s_ok = 0;
-    __syncthreads();
-    if (SMEM) { if ((is_la || is_worker) && my_chain == 0) run_steps(C0, C0.Ke, C0.ncol, false, false); }
-    else run_chunked(C0.Ke, C0.ncol, 0, false);
-    __syncthreads();
-  }
-  HB_TICKD(2, C0.W);
-  if (!SMEM) {
-    // the chunk views are dead: the corner system, its solution and (if they fit) both chains' solution vectors
-    // move into that shared memory for the latency-bound tail phases
-    __syncthreads();
-    double* p = s_band;
-    const size_t ncc = static_cast<size_t>(m + 1) * LDc + 2 * static_cast<size_t>(m);
-    for (size_t e = tid; e < ncc; e += kBandThreads) p[e] = CC[e];
-    CC = p; XA = CC + static_cast<size_t>(m + 1) * LDc;
-    p += ncc;
-    const size_t avail = 2 * static_cast<size_t>(chunk_cols) * (h6 + 6 * static_cast<size_t>(m + 1) + 48);
-    if (ncc + C0.npc + C1.npc <= avail) { C0.X = p; C1.X = p + C0.npc; }
-    __syncthreads();
-  }
-  // ---- the deferred corner update C -= sum over all eliminated columns of (arrow panel)(arrow panel)^T, rhs row
-  // included (row m).  CL: each CTA contracts its own chain's columns; CTA 1 stores its partial sum in its (otherwise
-  // unused) corner storage, CTA 0 waits for it (cluster barrier 2) and subtracts its own partial, then CTA 1's, in
-  // this fixed order (no atomics across the cluster: replicas of the solve stay bit-identical) ----
-  if (CL && rank == 0) cluster_wait();
-  if (!CL || rank == 0 || pl.Kb) {
-    // FP64 tensor-core tiles (mma.sync m8n8k4 -> SASS DMMA.8x8x4): output tile (ub, vb) of 8 x 8 corner entries,
-    // K = the eliminated columns in steps of 4.  Operand fragments: lane l holds
-    // A[row l/4][k l%4] and B[k l%4][col l/4] -- both are AR[row][col0 + l%4] -- and C[row l/4][col 2(l%4)+{0,1}].
+  // ---- the deferred corner update CC -= sum over the eliminated columns of (arrow panel)(arrow panel)^T, rhs row
+  // included (row m): FP64 tensor-core tiles (mma.sync m8n8k4 -> SASS DMMA.8x8x4), output tile (ub, vb) of 8 x 8
+  // corner entries, K = the eliminated columns in steps of 4.  Operand fragments: lane l holds
+  // A[row l/4][k l%4] and B[k l%4][col l/4] -- both are AR[row][col0 + l%4] -- and C[row l/4][col 2(l%4)+{0,1}].
+  // One warp owns each output tile and contracts every column of Qa, then of Qb, into it, in a fixed order, so the
+  // corner, and with it the step, is bit-identical from solve to solve (splitting a tile's contraction across
+  // warps and merging the parts with shared-memory atomics made the chunked solver's step vary in the last bits).
+  // store: CC = the sum (a partial that CTA 0 subtracts later) instead of CC -= the sum. ----
+  auto corner_update = [&](const BandChain& Qa, const BandChain& Qb, bool store) {
     const int nrb = (m + 1 + 7) / 8, ncb = (m + 7) / 8;
     const int lr = lane >> 2, lk = lane & 3;
-    // One warp owns each output tile and contracts every column of both chains into it, in a fixed order, so the
-    // corner, and with it the step, is bit-identical from solve to solve (splitting a tile's contraction across
-    // warps and merging the parts with shared-memory atomics made the chunked solver's step vary in the last bits).
     for (int tile = warp; tile < nrb * ncb; tile += kBandThreads / 32) {
       const int ub = tile / ncb, vb = tile - ub * ncb;
       if (vb > ub) continue;
       double c0 = 0.0, c1 = 0.0;
 #pragma unroll
       for (int ci = 0; ci < 2; ++ci) {
-        if (CL && ci != rank) continue;
-        const BandChain& Q = ci ? C1 : C0;
-        const int lo = 0, hi = ci ? 6 * C1.Ke : C0.npc;                    // the chain's eliminated columns
+        const BandChain& Q = ci ? Qb : Qa;
+        const int hi = 6 * Q.ne;                    // the chain's eliminated columns
         const double* pa = Q.AR + static_cast<size_t>(min(8 * ub + lr, m)) * Q.npc + lk;
         const double* pb = Q.AR + static_cast<size_t>(min(8 * vb + lr, m)) * Q.npc + lk;
-        for (int col = lo; col < hi; col += 16) {
+        for (int col = 0; col < hi; col += 16) {
           double av[4], bv[4];
 #pragma unroll
           for (int u = 0; u < 4; ++u) {
@@ -822,26 +826,35 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
       const int u = 8 * ub + lr, v = 8 * vb + 2 * lk;
       double* cu = CC + static_cast<size_t>(u) * LDc + v;
       const bool in0 = u <= m && v < m && v <= u, in1 = u <= m && v + 1 < m && v + 1 <= u;
-      if (!CL) {
-        if (in0) cu[0] -= c0;
-        if (in1) cu[1] -= c1;
-      } else if (rank == 1) {   // every corner entry belongs to one lane of one tile
-        if (in0) cu[0] = c0;
-        if (in1) cu[1] = c1;
-      } else {
-        if (in0) cu[0] = (cu[0] - c0) - (pl.Kb ? ld_peer(cu, 1) : 0.0);
-        if (in1) cu[1] = (cu[1] - c1) - (pl.Kb ? ld_peer(cu + 1, 1) : 0.0);
-      }
+      if (in0) cu[0] = store ? c0 : cu[0] - c0;
+      if (in1) cu[1] = store ? c1 : cu[1] - c1;
     }
-  }
-  __syncthreads();
-  HB_TICKD(3, CC);
-  if (CL && rank == 1) cluster_arrive();
+  };
+  // row transform of the first ncols columns of a chain (one row per thread): panel rows B <- B L^-1 and/or the rhs y <- y L^-1
+  auto row_transform = [&](const BandChain& Q, int ncols, bool panel, bool rhs) {
+    const int rows_per_col = (h - 6) + 1;
+    for (int e = tid; e < ncols * rows_per_col; e += kBandThreads) {
+      const int c = e / rows_per_col, t = e - c * rows_per_col;
+      const int nb = min(h - 6, Q.npc - 6 * (c + 1));
+      const double* L = Q.W + static_cast<size_t>(c) * h6;
+      const double* rd = Q.LI + static_cast<size_t>(c) * 48;
+      if (t < nb) { if (panel) band_transform_row(Q.W + (static_cast<size_t>(c) * h + 6 + t) * 6, L, rd); }
+      else if (t == h - 6 && rhs) band_transform_row(Q.AR + static_cast<size_t>(m) * Q.npc + 6 * c, L, rd);
+    }
+  };
+  // arrow contribution to every eliminated block's right-hand side, all at once: y_p -= AR^T x_a (row m of AR = y)
+  auto arrow_prepass = [&](const BandChain& Q, const double* xa) {
+    for (int col = tid; col < 6 * Q.ne; col += kBandThreads) {
+      double sacc = 0.0;
+      for (int r = 0; r < m; ++r) sacc += Q.AR[static_cast<size_t>(r) * Q.npc + col] * xa[r];
+      Q.AR[static_cast<size_t>(m) * Q.npc + col] -= sacc;
+    }
+  };
   // ---- corner (m x m, rhs carried as row m): right-looking Cholesky by the whole CTA with FIXED element
   // ownership (element (u, v), v <= min(u, m-1), decoded once), two barriers per column and no
   // division / modulo in the column loop.  The pivot's square root goes to XA's neighbour array DG so
   // that nobody overwrites CC[q][q] while others still read it. ----
-  if (has0) {
+  auto corner_solve = [&]() {
     double* DG = XA + m;   // diagonal of the corner factor
     const int ntri = m * (m + 1) / 2, nel = ntri + m;
     auto decode = [&](int e, int* pu, int* pv) {
@@ -934,80 +947,166 @@ __global__ void __launch_bounds__(kBandThreads) band_solve_kernel(const double* 
         __syncwarp();
       }
     }
-  }
-  __syncthreads();
-  // row transform of the eliminated columns (one row per thread): panel rows B <- B L^-1 and/or the rhs y <- y L^-1
-  auto row_transform = [&](bool panel, bool rhs) {
-    const int rows_per_col = (h - 6) + 1;
-    const int nc0 = has0 ? C0.ncol : 0, ncols = nc0 + (has1 ? C1.Ke : 0);
-    for (int e = tid; e < ncols * rows_per_col; e += kBandThreads) {
-      const int cc = e / rows_per_col, t = e - cc * rows_per_col;
-      const BandChain& Q = cc < nc0 ? C0 : C1;
-      const int c = cc < nc0 ? cc : cc - nc0;
-      const int nb = min(h - 6, Q.npc - 6 * (c + 1));
-      const double* L = Q.W + static_cast<size_t>(c) * h6;
-      const double* rd = Q.LI + static_cast<size_t>(c) * 48;
-      if (t < nb) { if (panel) band_transform_row(Q.W + (static_cast<size_t>(c) * h + 6 + t) * 6, L, rd); }
-      else if (t == h - 6 && rhs) band_transform_row(Q.AR + static_cast<size_t>(m) * Q.npc + 6 * c, L, rd);
-    }
   };
-  if (CL && rank == 1) {
-    // chain 1's panel rows do not depend on the corner solution: transform them while CTA 0 solves the corner; CTA 0
-    // then stores the corner solution and the separator part of chain 0's solution here (cluster barrier 3)
-    row_transform(true, false);
-    __syncthreads();
-    HB_TICK(4);
-    cluster_wait();
-    cluster_arrive(); cluster_wait();
-  }
-  HB_TICKD(5, XA);
-  // arrow contribution to every eliminated block's right-hand side, all at once: y_p -= AR^T x_a (row m of AR = y)
-  {
-    const int n0 = has0 ? C0.npc : 0, n1 = has1 ? 6 * C1.Ke : 0;
-    for (int e = tid; e < n0 + n1; e += kBandThreads) {
-      const BandChain& Q = e < n0 ? C0 : C1;
-      const int col = e < n0 ? e : e - n0;
-      double sacc = 0.0;
-      for (int r = 0; r < m; ++r) sacc += Q.AR[static_cast<size_t>(r) * Q.npc + col] * XA[r];
-      Q.AR[static_cast<size_t>(m) * Q.npc + col] -= sacc;
-    }
-  }
-  __syncthreads();
-  row_transform(!CL || rank == 0, true);
-  __syncthreads();
-  HB_TICKD(7, C.AR);
-  // separator columns first (chain 0, warp 0), then outwards: chain 0 in warp 0, chain 1 in warp 1 (CL: warp 0 of CTA 1)
-  if (has0 && warp == 0 && C0.ncol > C0.Ke) band_backsub_chain(C0, C0.ncol - 1, C0.Ke, h, m, lane);
-  __syncthreads();
-  if (CL && rank == 0) {   // barrier 3: the corner solution and the separator solution, in CTA 1's XA and X
+  if (!CL) {
+    // ---- merge chain 1's copy of the separator (index-reversed) and of its arrow columns into chain 0,
+    // then chain 0's pipeline eliminates the separator columns ----
     if (pl.Kb) {
-      for (int e = tid; e < m; e += kBandThreads) st_peer(XA + e, 1, XA[e]);
-      for (int v = tid; v < 6 * pl.bs; v += kBandThreads) st_peer(C1.X + C1.npc - 1 - v, 1, C0.X[6 * C0.Ke + v]);
+      const int nsep = 6 * pl.bs, N1 = C1.npc;
+      for (int e = tid; e < nsep * nsep; e += kBandThreads) {
+        const int u = e / nsep, v = e - u * nsep;
+        if (v > u) continue;
+        const int ru = N1 - 1 - u, rv = N1 - 1 - v;   // ru <= rv: stored in block column ru / 6
+        C0.W[(static_cast<size_t>(C0.Ke + v / 6) * h + (u - 6 * (v / 6))) * 6 + v % 6] +=
+            C1.W[(static_cast<size_t>(ru / 6) * h + (rv - 6 * (ru / 6))) * 6 + ru % 6];
+      }
+      for (int e = tid; e < (m + 1) * nsep; e += kBandThreads) {
+        const int r = e / nsep, v = e - r * nsep;
+        C0.AR[static_cast<size_t>(r) * C0.npc + 6 * C0.Ke + v] += C1.AR[static_cast<size_t>(r) * N1 + (N1 - 1 - v)];
+      }
+      __syncthreads();
+      if (tid == 0 && !chol6(C0.W + static_cast<size_t>(C0.Ke) * h6, 6, C0.LI + static_cast<size_t>(C0.Ke) * 48)) s_ok = 0;
+      __syncthreads();
+      run_chunked(C0.Ke, C0.ncol, 0, false);
+      __syncthreads();
     }
-    cluster_arrive();
-  }
-  if (!CL && pl.Kb) {
-    for (int v = tid; v < 6 * pl.bs; v += kBandThreads) C1.X[C1.npc - 1 - v] = C0.X[6 * C0.Ke + v];
+    HB_TICKD(2, C0.W);
+    // the chunk views are dead: the corner system, its solution and (if they fit) both chains' solution vectors
+    // move into that shared memory for the latency-bound tail phases
     __syncthreads();
-  }
-  if (CL ? warp == 0 : warp < 2) {
-    const BandChain& Q = (CL ? rank : warp) ? C1 : C0;
-    band_backsub_chain(Q, Q.Ke - 1, 0, h, m, lane);
-  }
-  __syncthreads();
-  HB_TICKD(6, C.X);
-  if (has0) {
+    double* p = s_band;
+    const size_t ncc = static_cast<size_t>(m + 1) * LDc + 2 * static_cast<size_t>(m);
+    for (size_t e = tid; e < ncc; e += kBandThreads) p[e] = CC[e];
+    CC = p; XA = CC + static_cast<size_t>(m + 1) * LDc;
+    p += ncc;
+    const size_t avail = 2 * static_cast<size_t>(chunk_cols) * (h6 + 6 * static_cast<size_t>(m + 1) + 48);
+    if (ncc + C0.npc + C1.npc <= avail) { C0.X = p; C1.X = p + C0.npc; }
+    __syncthreads();
+    corner_update(C0, C1, false);
+    __syncthreads();
+    HB_TICKD(3, CC);
+    corner_solve();
+    __syncthreads();
+    HB_TICKD(5, XA);
+    arrow_prepass(C0, XA);
+    arrow_prepass(C1, XA);
+    __syncthreads();
+    row_transform(C0, C0.ne, true, true);
+    row_transform(C1, C1.ne, true, true);
+    __syncthreads();
+    HB_TICKD(7, C.AR);
+    // separator columns first (chain 0, warp 0), then outwards: chain 0 in warp 0, chain 1 in warp 1
+    if (warp == 0 && C0.ncol > C0.Ke) band_backsub_chain(C0, C0.ncol - 1, C0.Ke, h, m, lane);
+    __syncthreads();
+    if (pl.Kb) {
+      for (int v = tid; v < 6 * pl.bs; v += kBandThreads) C1.X[C1.npc - 1 - v] = C0.X[6 * C0.Ke + v];
+      __syncthreads();
+    }
+    if (warp < 2) {
+      const BandChain& Q = warp ? C1 : C0;
+      band_backsub_chain(Q, Q.Ke - 1, 0, h, m, lane);
+    }
+    __syncthreads();
+    HB_TICKD(6, C.X);
     for (int e = tid; e < C0.npc; e += kBandThreads) x_out[e] = C0.X[e];
     for (int e = tid; e < m; e += kBandThreads) x_out[np + e] = XA[e];
+    for (int e = tid; e < 6 * C1.Ke; e += kBandThreads) x_out[np - 1 - e] = C1.X[e];
+  } else {
+    // ---- cluster: after its chain, each CTA meets the other at cluster barriers (release on arrive, acquire on wait);
+    // data crosses by remote shared-memory stores ahead of a barrier, or by CTA 0's remote loads behind one.
+    //   1. CTA 1's separator copy -> CTA 0, which merges it and eliminates the separator;
+    //   2. CTA 1's partial corner update and SPD flag -> CTA 0, which factors and solves the corner;
+    //   3. the corner's and the separator's solutions -> CTA 1.  Then both CTAs solve their chains outwards. ----
+    const int nsep = 6 * pl.bs, peer = 1 - rank;
+    const SegChain gp = seg_chain(pl, K, peer);
+    const CtaLayout Lo = cta_layout(pl, K, beta, m, rank), Lp = cta_layout(pl, K, beta, m, peer);
+    BandChain E = C;   // no columns: corner_update's second operand
+    E.ne = 0;
+    if (!g.elim && g.Ke && nsep) {   // remote stores do not stall the way remote loads in the merge would
+      const double* w = C.W + static_cast<size_t>(C.Ke) * h6;
+      for (int e = tid; e < pl.bs * h6; e += kBandThreads) st_peer(ws + Lp.RBW + e, peer, w[e]);
+      for (int e = tid; e < (m + 1) * nsep; e += kBandThreads) {
+        const int r = e / nsep, v = e - r * nsep;
+        st_peer(ws + Lp.RBA + e, peer, C.AR[static_cast<size_t>(r) * C.npc + 6 * C.Ke + v]);
+      }
+    }
+    cluster_arrive(); cluster_wait();   // barrier 1
+    if (g.elim) {
+      // chain 1's copy is index-reversed: separator-local index u <-> nsep - 1 - u
+      const double* rbw = ws + Lo.RBW;
+      const double* rba = ws + Lo.RBA;
+      for (int e = tid; e < nsep * nsep; e += kBandThreads) {
+        const int u = e / nsep, v = e - u * nsep;
+        if (v > u) continue;
+        const int ru = nsep - 1 - u, rv = nsep - 1 - v;   // ru <= rv: stored in block column ru / 6
+        C.W[(static_cast<size_t>(C.Ke + v / 6) * h + (u - 6 * (v / 6))) * 6 + v % 6] +=
+            rbw[(static_cast<size_t>(ru / 6) * h + (rv - 6 * (ru / 6))) * 6 + ru % 6];
+      }
+      for (int e = tid; e < (m + 1) * nsep; e += kBandThreads) {
+        const int r = e / nsep, v = e - r * nsep;
+        C.AR[static_cast<size_t>(r) * C.npc + 6 * C.Ke + v] += rba[static_cast<size_t>(r) * nsep + (nsep - 1 - v)];
+      }
+      __syncthreads();
+      if (tid == 0 && !chol6(C.W + static_cast<size_t>(C.Ke) * h6, 6, C.LI + static_cast<size_t>(C.Ke) * 48)) s_ok = 0;
+      __syncthreads();
+      if (is_la || is_worker) run_steps(C, C.Ke, C.ncol, false, false);
+      __syncthreads();
+    }
+    HB_TICKD(2, C.W);
+    // the CTA's own part of the corner update (CTA 1: stored as a partial for CTA 0), and its panel rows, which do not
+    // depend on the solution
+    corner_update(C, E, !hub);
+    row_transform(C, C.ne, true, false);
+    __syncthreads();
+    HB_TICKD(3, CC);
+    cluster_arrive(); cluster_wait();   // barrier 2
+    if (!hub) HB_TICK(4);
+    // the CTA's rhs: arrow pre-pass and transform, then (CTA 0) the separator's back substitution, handed to CTA 1
+    auto solve_own = [&]() {
+      arrow_prepass(C, XA);
+      __syncthreads();
+      row_transform(C, C.ne, false, true);
+      __syncthreads();
+      if (g.elim) {
+        if (warp == 0) band_backsub_chain(C, C.ncol - 1, C.Ke, h, m, lane);
+        __syncthreads();
+        for (int i = tid; i < nsep; i += kBandThreads) st_peer(ws + Lp.X + 6 * gp.Ke + (nsep - 1 - i), peer, C.X[6 * C.Ke + i]);
+      }
+    };
+    if (hub) {
+      if (tid == 0 && !ld_peer(&s_ok, 1)) s_ok = 0;   // chain 1's SPD flag
+      // CTA 1's partial corner update, subtracted after CTA 0's own (no atomics across the cluster: replicas of the
+      // solve stay bit-identical); a window too short for two chains leaves CTA 1 without columns
+      const double* pc = ws + Lp.CC;
+      for (int e = tid; pl.Kb && e < (m + 1) * m; e += kBandThreads) {
+        const int r = e / m, q = e - r * m;
+        if (r < m && q > r) continue;
+        CC[static_cast<size_t>(r) * LDc + q] -= ld_peer(pc + static_cast<size_t>(r) * LDc + q, 1);
+      }
+      __syncthreads();
+      corner_solve();
+      __syncthreads();
+      solve_own();
+      for (int e = tid; e < m; e += kBandThreads) st_peer(ws + Lp.XA + e, 1, XA[e]);
+    }
+    cluster_arrive(); cluster_wait();   // barrier 3
+    HB_TICK(5);
+    if (!hub) solve_own();
+    HB_TICKD(7, C.AR);
+    if (warp == 0) band_backsub_chain(C, C.Ke - 1, 0, h, m, lane);
+    __syncthreads();
+    HB_TICKD(6, C.X);
+    for (int e = tid; e < 6 * C.ne; e += kBandThreads) x_out[g.rev ? 6 * g.anchor - 1 - e : 6 * g.anchor + e] = C.X[e];
+    if (hub)
+      for (int e = tid; e < m; e += kBandThreads) x_out[np + e] = XA[e];
   }
-  if (has1) for (int e = tid; e < 6 * C1.Ke; e += kBandThreads) x_out[np - 1 - e] = C1.X[e];
   if (dbg && tid == 0) { for (int i = 0; i < 8; ++i) dbg[i] = t_acc[i]; dbg[8 + 6] = t_staged - t_entry; dbg[8 + 7] = t_gathered - t_staged; dbg[8 + 14] = clock64() - t_entry; dbg[8 + 15] = t_g[0] - t_staged; dbg[8 + 22] = t_g[1] - t_g[0]; dbg[8 + 23] = t_g[2] - t_g[1]; dbg[8 + 30] = t_g[3] - t_g[2]; dbg[8 + 31] = t_gathered - t_g[3]; }
-  if (tid == 0 && has0) *spd_flag = s_ok;
-  // neither CTA may exit while the other can still read its shared memory (barrier 4)
-  if (CL) {
-    if (rank == 0) cluster_wait();
-    cluster_arrive(); cluster_wait();
+  if (tid == 0 && hub) {
+    *spd_flag = s_ok;
+    if (dbg) dbg[70] = s_ok;   // (a word the step stamps leave free)
   }
+  // neither CTA may exit while the other can still read or write its shared memory (last cluster barrier)
+  if (CL) { cluster_arrive(); cluster_wait(); }
 }
 
 }  // namespace hb

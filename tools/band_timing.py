@@ -13,15 +13,19 @@ us = lambda c: c / (hz / 1e6)
 buf = (C.c_longlong*144)()
 ctx.lib.hb200_debug_band_timing(ctx.h, buf)
 # the resident solver runs chain r on CTA r of a 2-CTA cluster; each CTA records its own phases (72 values each)
-names = {0: ["potf2 prologue","two-sided factorisation (chain 0)","merge + separator columns","deferred corner update (chain 0 + CTA 1's part)","corner Cholesky","corner back substitution","outward back substitution","arrow pre-pass + row transform"],
-         1: ["potf2 prologue","two-sided factorisation (chain 1)","-","deferred corner update (chain 1 part)","panel-row transform","wait for CTA 0 (corner, separator)","outward back substitution","arrow pre-pass + rhs transform"]}
+names = {0: ["potf2 prologue", "two-sided factorisation (chain 0)", "wait for CTA 1 (barrier 1), merge + separator columns",
+             "own corner update + panel-row transform", "wait for CTA 1 (barrier 2), its corner partial, corner Cholesky",
+             "corner back subst., arrow pre-pass, rhs transform, separator back subst., stores to CTA 1", "outward back substitution", "-"],
+         1: ["potf2 prologue", "two-sided factorisation (chain 1)", "separator copy to CTA 0 (barrier 1)",
+             "own corner partial + panel-row transform", "wait for CTA 0 (barrier 2)", "wait for CTA 0 (corner and separator solutions)",
+             "outward back substitution", "arrow pre-pass + rhs transform"]}
 for r in (0, 1):
     cyc = buf[72 * r:72 * (r + 1)]
-    if r == 1 and cyc[22] == 0:
+    if r > 0 and cyc[22] == 0:
         break   # single-CTA kernel (chunked workspace)
-    print(f"==== CTA {r}")
+    print(f"==== CTA {r}" + (f" (SPD flag of the solve: {cyc[70]})" if r == 0 else ""))
     tot=sum(cyc[0:8])
-    for n,c in zip(names[r],cyc): print(f"{n:48s} {c:9d} cycles {us(c):8.1f} us {100*c/max(tot,1):5.1f}%")
+    for n,c in zip(names[r],cyc): print(f"{n:72s} {c:9d} cycles {us(c):8.1f} us {100*c/max(tot,1):5.1f}%")
     print(f"chain {r}, steps 4..11: cycles relative to the update warp's release (B of the previous step)")
     print("step  panel_end  A_release  upd_end | la_release  la_end | next_release")
     for i in range(8):
