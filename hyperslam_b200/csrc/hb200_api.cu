@@ -925,13 +925,14 @@ int enqueue_accept(hb200_ctx* c) {
 }
 
 // Sum of the packed partial systems over the ranks: ONE ncclAllReduce on the context's stream (capturable).
-int enqueue_reduce_system(hb200_ctx* c) {
+// err_st: the solver state whose comm_error a peer-memory timeout sets (the LM's c->st unless given).
+int enqueue_reduce_system(hb200_ctx* c, SolverState* err_st = nullptr) {
   if (c->peer_reduce()) {
     // fused barrier + reduction over peer memory (peer_reduce_kernel); the next iteration assembles into the other half
     PeerReduceArgs a{};
     a.nranks = c->nranks; a.rank = c->rank; a.peers = c->d_peers.p; a.local = c->mbox.p;
     a.part_offset = kArenaParts + static_cast<long long>(c->peer_par) * c->arena_cap; a.total = c->lay.total;
-    a.out = c->sys.p; a.round = c->red_round.p; a.arrive = c->red_arrive.p; a.st = c->st.p;
+    a.out = c->sys.p; a.round = c->red_round.p; a.arrive = c->red_arrive.p; a.st = err_st ? err_st : c->st.p;
     const long long pairs = c->lay.total / 2;
     const int grid = static_cast<int>(std::max<long long>(1, std::min<long long>(4LL * c->num_sms, (pairs + kReduceThreads - 1) / kReduceThreads)));
     peer_reduce_kernel<<<grid, kReduceThreads, 0, c->stream>>>(a);
@@ -1945,7 +1946,6 @@ int hb200_get_delta(hb200_ctx* c, double* dp, double* dl) {
 namespace {
 int cov_check(hb200_ctx* c) {
   if (!c) return fail(-1, "null context");
-  if (c->multi()) return fail(-3, "covariance: not supported with a communicator or all-reduce callback attached (single GPU only)");
   return 0;
 }
 void cov_info(hb200_ctx* c, hb200_covariance_info* info) {
@@ -1955,11 +1955,16 @@ void cov_info(hb200_ctx* c, hb200_covariance_info* info) {
 }
 }  // namespace
 
+// Sharded contexts (a communicator or the all-reduce callback): collective.  Each rank assembles its undamped partial
+// system and writes its degenerate-landmark count into the tail slot kCovDegenerateSlot; ONE system reduction (as
+// hb200_build_system) then leaves the same reduced system and the window-wide count on every rank.  The -6 refusal
+// depends only on the agreed layout, so every rank refuses before the reduction.
 int hb200_build_covariance(hb200_ctx* c) {
   int rc = cov_check(c);
   if (rc) return rc;
   if ((rc = check_ready(c))) return rc;
   HB_CUDA(cudaSetDevice(c->device));
+  const bool sharded = c->multi();
   const size_t smem = cov_smem_doubles(c->beta, c->lay.m) * sizeof(double);
   if (smem > 220 * 1024)
     return fail(-6, "covariance: a window of %d block columns and %d arrow rows needs %zu B of shared memory", c->beta + 1, c->lay.m, smem);
@@ -1982,10 +1987,28 @@ int hb200_build_covariance(hb200_ctx* c) {
     HB_CUDA(c->cov_counts.ensure(2));
     cov_landmark_flags_kernel<<<1, kCovFlagThreads, 0, c->stream>>>(c->L, c->lm_off.p, c->Vchol.p, c->Dl.p, c->cov_counts.p);
     HB_LAUNCH(c, "cov_landmark_flags_kernel");
+    if (sharded) {
+      cov_degenerate_slot_kernel<<<1, 1, 0, c->stream>>>(c->cov_counts.p, c->assembly(), c->lay);
+      HB_LAUNCH(c, "cov_degenerate_slot_kernel");
+    }
     HB_CUDA(cudaMemcpyAsync(counts, c->cov_counts.p, sizeof(counts), cudaMemcpyDeviceToHost, c->stream));
   }
+  double window_degenerate = 0.0;
+  SolverState red_st{};
+  if (sharded) {
+    // the peer reduction reports a timed-out peer in cov_st, not in the LM's state; it flips peer_par like any eager
+    // reduction, so the next hb200_iterate assembles into (and launches the graph of) the other arena half
+    if ((rc = enqueue_reduce_system(c, c->cov_st.p))) { c->outputs_changed(); return rc; }
+    HB_CUDA(cudaMemcpyAsync(&window_degenerate, c->sys.p + c->lay.os + kCovDegenerateSlot, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    HB_CUDA(cudaMemcpyAsync(&red_st, c->cov_st.p, sizeof(red_st), cudaMemcpyDeviceToHost, c->stream));
+  }
   HB_CUDA(cudaStreamSynchronize(c->stream));
-  c->cov_degenerate = counts[0]; c->cov_unobserved = counts[1];
+  if (red_st.comm_error) {
+    c->outputs_changed();
+    return fail(-7, "covariance: a peer did not reach the system reduction in time (every rank must call hb200_build_covariance)");
+  }
+  c->cov_degenerate = sharded ? static_cast<int>(window_degenerate) : counts[0];
+  c->cov_unobserved = counts[1];
   c->cov_lay_next = c->lay; c->cov_basis_next = c->basis; c->cov_L_next = c->L;
   c->cov_k_next = c->k; c->cov_Nv_next = c->Nv; c->cov_max_rows_next = c->max_rows;
   // the factor outputs are those of an evaluation at the current state; the packed buffer is not what hb200_solve expects
@@ -1995,6 +2018,9 @@ int hb200_build_covariance(hb200_ctx* c) {
   return 0;
 }
 
+// No collective step: on a sharded context every rank inverts the same reduced system with the same atomic-free kernel
+// (Sigma, the status, bad_dof and the pivot are bit-identical across ranks; the degenerate count is the window's), and
+// the landmark kernel runs over the rank's own landmarks and their factors.
 int hb200_compute_covariance(hb200_ctx* c, hb200_covariance_info* info) {
   int rc = cov_check(c);
   if (rc) return rc;

@@ -72,6 +72,15 @@ __global__ void __launch_bounds__(kCovFlagThreads) cov_landmark_flags_kernel(int
   }
 }
 
+// Sharded contexts: the rank's degenerate-landmark count goes into a tail slot of its partial packed system, which the
+// system reduction then sums with everything else (one collective per build).  scal[kCovDegenerateSlot] is written by no
+// other kernel of a build (cost_kernel writes scal[0] and scal[1]) and is cleared with the rest of the buffer; the sum of
+// small integers is exact in any order.
+constexpr int kCovDegenerateSlot = 7;
+__global__ void cov_degenerate_slot_kernel(const int* __restrict__ counts, double* sys, SysLayout lay) {
+  sys[lay.os + kCovDegenerateSlot] = static_cast<double>(counts[0]);
+}
+
 // Entry (i, j) of A_hat = D S D with the constant-dof mask (identity rows / columns), read from the lower triangle.
 HB_DI double cov_ahat(const double* __restrict__ sys, const SysLayout& lay, const unsigned char* __restrict__ fixed, const double* __restrict__ d,
                       int i, int j) {

@@ -388,12 +388,15 @@ class Context:
 
     # ---- marginal covariances (ceres::Covariance) --------------------------------------------------------------
     def build_covariance(self):
-        """Undamped reduced system at the current state into the packed buffer (hb200_build_covariance)."""
+        """Undamped reduced system at the current state into the packed buffer (hb200_build_covariance).  Sharded
+        contexts: collective, every rank calls it (one reduction of the partial systems)."""
         self._check(self.lib.hb200_build_covariance(self.h))
 
     def compute_covariance(self):
         """Selected inverse + landmark marginals.  Returns the info dict; a status != 0 (not positive definite, degenerate
-        landmarks) is reported there, not raised, and the previous results stay in place."""
+        landmarks) is reported there, not raised, and the previous results stay in place.  Sharded contexts: every rank
+        calls it and gets the same Sigma and status; landmark blocks are valid on their owner (zero elsewhere), and
+        `L` / `unobserved_landmarks` count the landmarks this context holds."""
         info = CovarianceInfo()
         rc = self.lib.hb200_compute_covariance(self.h, C.byref(info))
         if rc not in (0, COV_NOT_POSITIVE_DEFINITE, COV_DEGENERATE_LANDMARKS):

@@ -223,11 +223,23 @@ int hb200_get_delta(hb200_ctx* ctx, double* delta_pose /* n */, double* delta_la
  *                             and corner full, padding rows 0), landmark = [L][3][3] (may be NULL).  Shape: info K, beta, m, L.
  *   hb200_interpolate_covariance: the 6 x 6 covariance of the pose [theta | p] interpolated at each stamp, at the knots of
  *                             the last successful compute; stamps outside the valid span give zero blocks, counted.
- * Single GPU: a context with a communicator or all-reduce callback gets -3.  A window whose band + arrow (6 (beta+1) + m
- * rows, square) does not fit one CTA's shared memory gets -6.  Ceres-tangent and ambient blocks: hyper::Covariance (host). */
+ * Sharded contexts (a communicator or the all-reduce callback): hb200_build_covariance and hb200_compute_covariance are
+ * collective, see the SHARDING CONTRACT below.  The build assembles each rank's undamped partial system (its factors, the
+ * Schur complement of the landmarks it owns) and sums it over the ranks with ONE system reduction, as hb200_build_system
+ * does; the compute then inverts the same reduced system on every rank (band, arrow, corner, status, bad_dof and
+ * min_pivot_ratio bit-identical across ranks) and the marginals of the rank's own landmarks: read a landmark's block from
+ * its owner (a landmark a rank holds but does not observe gets a zero block there).  hb200_get_covariance and
+ * hb200_interpolate_covariance are local calls; the interpolated covariances are identical on every rank.  A peer that
+ * does not reach the reduction makes the build fail (-7 after the peer-memory reduction's timeout, the callback's error
+ * + 200) instead of hanging the others.
+ * A window whose band + arrow (6 (beta+1) + m rows, square) does not fit one CTA's shared memory gets -6 (on a sharded
+ * context from every rank, before the reduction: it depends only on the agreed layout).  Ceres-tangent and ambient
+ * blocks: hyper::Covariance (host, one GPU). */
 typedef struct hb200_covariance_info {
   int status;                 /* 0 ok, 1 reduced system not positive definite, 2 degenerate landmarks */
   int bad_dof;                /* status 1: first reduced-system dof whose pivot failed, else -1 */
+  /* degenerate_landmarks (and so status 2) counts the whole window on a sharded context and is the same on every rank;
+   * unobserved_landmarks and L are rank-local: the landmarks this context holds, and those of them it does not observe. */
   int degenerate_landmarks, unobserved_landmarks;
   double min_pivot_ratio;     /* smallest pivot of the equilibrated reduced factor (status 1: the failing one) */
   int K, beta, m, L;          /* shape of what hb200_get_covariance returns */
@@ -317,7 +329,12 @@ int hb200_ingest_stereo(hb200_ctx* ctx, int n, const double* stamp, const int* c
  *     read each landmark back from its owner.
  *   - inertial and manifold factors may be split arbitrarily; every factor lives on exactly one rank.
  *   - knots, bias splines, gravity, calibration, constancy flags and options must be identical on all ranks,
- *     and every rank must make the same sequence of hb200_iterate / hb200_optimize / hb200_build_system calls.
+ *     and every rank must make the same sequence of hb200_iterate / hb200_optimize / hb200_build_system /
+ *     hb200_build_covariance / hb200_compute_covariance calls.  The covariance build takes one system reduction
+ *     (like hb200_build_system) and leaves the LM's trust-region state alone; the compute has no collective step.
+ *     A rank that fails a call for a reason of its own (an invalid argument, a stale build) breaks the contract as
+ *     in hb200_iterate; the peer reduction's timeout and the callback's error return keep the others from waiting
+ *     forever.
  *
  * Reduced buffer (what is summed): the band-only packed system, hb200_system_device_ptr(), in doubles
  *   [ P K*h*6 | A m*6K | C m*m | b n | diagH n | g n | scal 8 ],  h = 6 + 6*beta, m = n - 6K
@@ -344,7 +361,8 @@ int hb200_comm_info(hb200_ctx* ctx, int* nranks, int* rank, int* nccl, int* peer
 int hb200_get_bandwidth(hb200_ctx* ctx, int* beta);
 int hb200_set_min_bandwidth(hb200_ctx* ctx, int beta);
 /* Escape hatch for hosts without NCCL: the caller sums `count_doubles` doubles at `device_buffer` across ranks
- * on `stream` (called twice per iteration: packed system, then 8 scalars).  Disables CUDA-graph capture. */
+ * on `stream` (called twice per iteration: packed system, then 8 scalars; once per hb200_build_system and
+ * hb200_build_covariance: packed system).  Disables CUDA-graph capture. */
 typedef int (*hb200_allreduce_fn)(void* user, void* device_buffer, long long count_doubles, void* stream);
 int hb200_set_allreduce(hb200_ctx* ctx, hb200_allreduce_fn fn, void* user);
 void* hb200_system_device_ptr(hb200_ctx* ctx, long long* count_doubles);
