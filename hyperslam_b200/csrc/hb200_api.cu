@@ -179,22 +179,19 @@ struct hb200_ctx {
   bool term_enabled = false;
   double term_ftol = 1e-6, term_gtol = 1e-10, term_ptol = 1e-8, term_min_radius = 1e-32;
 
-  // factors (host copies in user order; device copies in bound order)
-  // visual list = pixel factors [0, Np) followed by bearing factors [Np, Np + Nb): both travel through the
-  // same kernels and the same compact layout (kind flag in idx.w); manifold (pose) factors have their own.
+  // factor lists, on the device only (the setters write them in user order, hb200_bind sorts them into bound order):
+  // the visual list holds pixel and bearing factors (kind flag in idx.w), which travel through the same kernels and the
+  // same compact layout; inertial and manifold (pose) factors have their own lists.
   int Nv = 0, Ni = 0, Np = 0, Nb = 0, Nm = 0, P = 0;
-  std::vector<double> h_p_stamp, h_p_pixel, h_b_stamp, h_b_bearing, h_m_stamp, h_m_meas, h_sensors;
-  std::vector<int> h_p_cam, h_p_lm, h_b_cam, h_b_lm, h_m_sensor;
-  std::vector<double> h_v_stamp, h_v_pixel, h_v_z, h_i_stamp, h_i_meas;
-  std::vector<int> h_v_cam, h_v_lm;
+  std::vector<double> h_sensors;
   DevBuf<double> v_stamp, v_pixel, v_z, v_w, i_stamp, i_meas, m_stamp, m_meas, sensors;
   DevBuf<int> m_sensor;
   DevBuf<int2> m_idx;
-  std::vector<int2> h_m_idx;
   double huber_bearing = 1.6e-3;   // reference optimizer.cpp:204
   DevBuf<int4> v_idx, i_idx;
-  std::vector<int4> h_v_idx, h_i_idx;       // bound order
-  std::vector<int> v_perm, i_perm;          // bound position -> user index
+  // list position -> user index (visual: pixel factors 0 .. Np-1, bearing factors Np .. Nv-1); appends and slides clear
+  // them, ensure_perms rebuilds them
+  std::vector<int> v_perm, i_perm;
   DevBuf<int> run_off, lm_off, lm_obs, d_invalid;
   // large windows: landmarks ordered by first knot base and cut into groups for schur_group_kernel
   DevBuf<int> lm_order, lm_group_off;
@@ -217,9 +214,7 @@ struct hb200_ctx {
   DevBuf<long long> band_dbg;   // optional phase timings of band_solve_kernel (HB200_BAND_TIMING=1)
   bool bound = false;
 
-  // device-side window bookkeeping (hb200_append_* / hb200_slide): the factor lists live on the device only, the host
-  // mirrors above are refreshed on demand (sync_host_mirrors)
-  bool device_managed = false;
+  // device-side window bookkeeping (hb200_append_* / hb200_slide) and the compactions / permutations of the factor lists
   DevBuf<double> alt_stamp, alt_meas, alt_z, alt_lms, alt_knots;
   DevBuf<double2> alt_pixel;
   DevBuf<int4> alt_idx;
@@ -1024,6 +1019,9 @@ int ensure_placeholders(hb200_ctx* c) {
   }
   HB_CUDA(c->imu_tab.ensure(kImuStride)); HB_CUDA(c->cam_tab.ensure(kCamStride));
   HB_CUDA(c->v_z.ensure(1)); HB_CUDA(c->v_w.ensure(1)); HB_CUDA(c->sensors.ensure(7)); HB_CUDA(c->m_idx.ensure(1));
+  HB_CUDA(c->v_stamp.ensure(1)); HB_CUDA(c->v_pixel.ensure(2)); HB_CUDA(c->v_idx.ensure(1));
+  HB_CUDA(c->i_stamp.ensure(1)); HB_CUDA(c->i_meas.ensure(6)); HB_CUDA(c->i_idx.ensure(1));
+  HB_CUDA(c->m_stamp.ensure(1)); HB_CUDA(c->m_meas.ensure(7)); HB_CUDA(c->m_sensor.ensure(1));
   return 0;
 }
 
@@ -1267,43 +1265,109 @@ int hb200_set_options(hb200_ctx* c, double huber_pixel, double imu_loss_scale, d
 }
 
 namespace {
-// visual list = pixel factors followed by bearing factors
-void visual_user_order(hb200_ctx* c) {
-  const size_t Np = c->Np, Nb = c->Nb, N = Np + Nb;
-  c->Nv = static_cast<int>(N);
-  c->h_v_stamp.resize(N); c->h_v_cam.resize(N); c->h_v_lm.resize(N); c->h_v_pixel.resize(2 * N); c->h_v_z.assign(N, 0.0);
-  std::copy(c->h_p_stamp.begin(), c->h_p_stamp.end(), c->h_v_stamp.begin());
-  std::copy(c->h_p_cam.begin(), c->h_p_cam.end(), c->h_v_cam.begin());
-  std::copy(c->h_p_lm.begin(), c->h_p_lm.end(), c->h_v_lm.begin());
-  std::copy(c->h_p_pixel.begin(), c->h_p_pixel.end(), c->h_v_pixel.begin());
-  for (size_t f = 0; f < Nb; ++f) {
-    c->h_v_stamp[Np + f] = c->h_b_stamp[f]; c->h_v_cam[Np + f] = c->h_b_cam[f]; c->h_v_lm[Np + f] = c->h_b_lm[f];
-    c->h_v_pixel[2 * (Np + f)] = c->h_b_bearing[3 * f]; c->h_v_pixel[2 * (Np + f) + 1] = c->h_b_bearing[3 * f + 1];
-    c->h_v_z[Np + f] = c->h_b_bearing[3 * f + 2];
+// The user index of every list position, when appends or slides cleared it: each family of the visual list in list
+// order (pixel factors 0 .. Np-1, bearing factors Np .. Nv-1), the inertial list as it stands.
+int ensure_perms(hb200_ctx* c) {
+  const size_t Nv = c->Nv, Ni = c->Ni;
+  if (c->v_perm.size() != Nv) {
+    std::vector<int4> id(Nv);
+    HB_CUDA(cudaSetDevice(c->device));
+    HB_CUDA(cudaMemcpyAsync(id.data(), c->v_idx.p, sizeof(int4) * Nv, cudaMemcpyDeviceToHost, c->stream));
+    HB_CUDA(cudaStreamSynchronize(c->stream));
+    c->v_perm.resize(Nv);
+    for (size_t f = 0, p = 0, b = c->Np; f < Nv; ++f) c->v_perm[f] = static_cast<int>(id[f].w == 0 ? p++ : b++);
   }
+  if (c->i_perm.size() != Ni) { c->i_perm.resize(Ni); std::iota(c->i_perm.begin(), c->i_perm.end(), 0); }
+  return 0;
 }
-void rebuild_visual(hb200_ctx* c) {
-  visual_user_order(c);
+
+// capacity for N visual factors, the current ones preserved
+int grow_visual(hb200_ctx* c, size_t N) {
+  const size_t Nv = c->Nv;
+  HB_CUDA(c->v_stamp.grow(N, Nv, c->stream)); HB_CUDA(c->v_pixel.grow(2 * N, 2 * Nv, c->stream));
+  HB_CUDA(c->v_z.grow(N, Nv, c->stream)); HB_CUDA(c->v_idx.grow(N, Nv, c->stream));
+  return 0;
+}
+
+// Writes n visual factors of one kind to list positions [at, at + n): meas = pixel [n][2] (kind 0) or bearing [n][3]
+// (kind 1: x, y in the pixel pair, z apart), and landmark, camera and kind into the index map, whose knot base
+// bind_pixel_kernel fills in.
+int upload_visual(hb200_ctx* c, int at, int n, const double* stamp, const int* camera, const int* landmark, const double* meas, int kind) {
+  std::vector<double> xy(kind ? 2 * static_cast<size_t>(n) : 0), z(kind ? n : 0);
+  for (int f = 0; f < static_cast<int>(z.size()); ++f) { xy[2 * f] = meas[3 * f]; xy[2 * f + 1] = meas[3 * f + 1]; z[f] = meas[3 * f + 2]; }
+  std::vector<int4> id(n);
+  for (int f = 0; f < n; ++f) id[f] = make_int4(0, landmark[f], camera[f], kind);
+  HB_CUDA(cudaMemcpyAsync(c->v_stamp.p + at, stamp, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
+  HB_CUDA(cudaMemcpyAsync(c->v_pixel.p + 2 * static_cast<size_t>(at), kind ? xy.data() : meas, sizeof(double) * 2 * n, cudaMemcpyHostToDevice, c->stream));
+  if (kind) HB_CUDA(cudaMemcpyAsync(c->v_z.p + at, z.data(), sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
+  HB_CUDA(cudaMemcpyAsync(c->v_idx.p + at, id.data(), sizeof(int4) * n, cudaMemcpyHostToDevice, c->stream));
+  HB_CUDA(cudaStreamSynchronize(c->stream));
+  return 0;
+}
+
+// Moves the visual factors with keep[f] (nullptr: all n) to positions pos[f] of the alternate buffers -- knot base less
+// knot_shift, landmark through lm_pos (nullptr: unchanged) -- and copies positions [at, at + count) back.
+int compact_visual(hb200_ctx* c, int n, const int* keep, const int* pos, const int* lm_pos, int knot_shift, int at, int count) {
+  const size_t end = std::max(at + count, 1);
+  HB_CUDA(c->alt_stamp.ensure(end)); HB_CUDA(c->alt_pixel.ensure(end)); HB_CUDA(c->alt_z.ensure(end)); HB_CUDA(c->alt_idx.ensure(end));
+  compact_visual_kernel<<<(n + 255) / 256, 256, 0, c->stream>>>(n, keep, pos, lm_pos, knot_shift, c->v_stamp.p, reinterpret_cast<const double2*>(c->v_pixel.p),
+                                                                c->v_z.p, c->v_idx.p, c->alt_stamp.p, c->alt_pixel.p, c->alt_z.p, c->alt_idx.p);
+  HB_LAUNCH(c, "compact_visual_kernel");
+  // (v_pixel is a DevBuf<double>: copy the compacted pairs back instead of swapping differently typed buffers)
+  HB_CUDA(cudaMemcpyAsync(c->v_pixel.p + 2 * static_cast<size_t>(at), c->alt_pixel.p + at, sizeof(double2) * count, cudaMemcpyDeviceToDevice, c->stream));
+  HB_CUDA(cudaMemcpyAsync(c->v_stamp.p + at, c->alt_stamp.p + at, sizeof(double) * count, cudaMemcpyDeviceToDevice, c->stream));
+  HB_CUDA(cudaMemcpyAsync(c->v_z.p + at, c->alt_z.p + at, sizeof(double) * count, cudaMemcpyDeviceToDevice, c->stream));
+  HB_CUDA(cudaMemcpyAsync(c->v_idx.p + at, c->alt_idx.p + at, sizeof(int4) * count, cudaMemcpyDeviceToDevice, c->stream));
+  return 0;
+}
+
+// The inertial counterpart of compact_visual: positions [0, count) come back, bases less the three shifts.
+int compact_inertial(hb200_ctx* c, int n, const int* keep, const int* pos, int knot_shift, int gyro_shift, int accel_shift, int count) {
+  const size_t end = std::max(count, 1);
+  HB_CUDA(c->alt_stamp.ensure(end)); HB_CUDA(c->alt_meas.ensure(6 * end)); HB_CUDA(c->alt_idx.ensure(end));
+  compact_inertial_kernel<<<(n + 255) / 256, 256, 0, c->stream>>>(n, keep, pos, knot_shift, gyro_shift, accel_shift, c->i_stamp.p, c->i_meas.p, c->i_idx.p, c->alt_stamp.p,
+                                                                  c->alt_meas.p, c->alt_idx.p);
+  HB_LAUNCH(c, "compact_inertial_kernel");
+  HB_CUDA(cudaMemcpyAsync(c->i_stamp.p, c->alt_stamp.p, sizeof(double) * count, cudaMemcpyDeviceToDevice, c->stream));
+  HB_CUDA(cudaMemcpyAsync(c->i_meas.p, c->alt_meas.p, sizeof(double) * 6 * count, cudaMemcpyDeviceToDevice, c->stream));
+  HB_CUDA(cudaMemcpyAsync(c->i_idx.p, c->alt_idx.p, sizeof(int4) * count, cudaMemcpyDeviceToDevice, c->stream));
+  return 0;
+}
+
+// Replaces the visual family of one kind (0 pixel, 1 bearing) by n factors in user order.  The list becomes [pixel
+// family | bearing family], each in user order: the other family is moved there by one compaction.
+int set_visual_family(hb200_ctx* c, int kind, int n, const double* stamp, const int* camera, const int* landmark, const double* meas) {
+  HB_CUDA(cudaSetDevice(c->device));
+  int rc = ensure_perms(c);
+  if (rc) return rc;
+  const int Nv = c->Nv, Np = kind ? c->Np : n, Nb = kind ? n : c->Nb;
+  const int kept = kind ? Np : Nb, kept_at = kind ? 0 : n, kept_from = kind ? 0 : c->Np;   // the other family: count, new position, old user index
+  if ((rc = grow_visual(c, Np + Nb))) return rc;
+  if (kept) {
+    std::vector<int> keep(Nv), pos(Nv);
+    for (int f = 0; f < Nv; ++f) { const int u = c->v_perm[f]; keep[f] = (u < c->Np) == (kind == 1); pos[f] = kept_at + u - kept_from; }
+    HB_CUDA(c->w_keep.ensure(Nv)); HB_CUDA(c->w_pos.ensure(Nv));
+    HB_CUDA(cudaMemcpyAsync(c->w_keep.p, keep.data(), sizeof(int) * Nv, cudaMemcpyHostToDevice, c->stream));
+    HB_CUDA(cudaMemcpyAsync(c->w_pos.p, pos.data(), sizeof(int) * Nv, cudaMemcpyHostToDevice, c->stream));
+    if ((rc = compact_visual(c, Nv, c->w_keep.p, c->w_pos.p, nullptr, 0, kept_at, kept))) return rc;
+  }
+  if (n && (rc = upload_visual(c, kind ? Np : 0, n, stamp, camera, landmark, meas, kind))) return rc;
+  HB_CUDA(cudaStreamSynchronize(c->stream));
+  c->Np = Np; c->Nb = Nb; c->Nv = Np + Nb;
+  c->v_perm.resize(c->Nv); std::iota(c->v_perm.begin(), c->v_perm.end(), 0);
   c->bound = false; c->kernel_args_changed();
+  return 0;
 }
 }  // namespace
 
 int hb200_set_pixel_factors(hb200_ctx* c, int n, const double* stamp, const int* camera, const int* landmark, const double* pixel) {
   if (!c || n < 0 || (n > 0 && (!stamp || !camera || !landmark || !pixel))) return fail(-1, "invalid pixel factors");
-  c->Np = n;
-  c->h_p_stamp.assign(stamp, stamp + n); c->h_p_cam.assign(camera, camera + n); c->h_p_lm.assign(landmark, landmark + n);
-  c->h_p_pixel.assign(pixel, pixel + 2 * static_cast<size_t>(n));
-  rebuild_visual(c);
-  return 0;
+  return set_visual_family(c, 0, n, stamp, camera, landmark, pixel);
 }
 
 int hb200_set_bearing_factors(hb200_ctx* c, int n, const double* stamp, const int* camera, const int* landmark, const double* bearing) {
   if (!c || n < 0 || (n > 0 && (!stamp || !camera || !landmark || !bearing))) return fail(-1, "invalid bearing factors");
-  c->Nb = n;
-  c->h_b_stamp.assign(stamp, stamp + n); c->h_b_cam.assign(camera, camera + n); c->h_b_lm.assign(landmark, landmark + n);
-  c->h_b_bearing.assign(bearing, bearing + 3 * static_cast<size_t>(n));
-  rebuild_visual(c);
-  return 0;
+  return set_visual_family(c, 1, n, stamp, camera, landmark, bearing);
 }
 
 int hb200_set_bearing_loss(hb200_ctx* c, double huber_bearing) {
@@ -1330,16 +1394,32 @@ int hb200_set_pose_sensors(hb200_ctx* c, int n, const double* T_bs) {
 
 int hb200_set_manifold_factors(hb200_ctx* c, int n, const double* stamp, const int* sensor, const double* pose) {
   if (!c || n < 0 || (n > 0 && (!stamp || !sensor || !pose))) return fail(-1, "invalid manifold factors");
+  HB_CUDA(cudaSetDevice(c->device));
+  const size_t N = n;
+  HB_CUDA(c->m_stamp.ensure(N)); HB_CUDA(c->m_meas.ensure(7 * N)); HB_CUDA(c->m_sensor.ensure(N)); HB_CUDA(c->m_idx.ensure(N));
+  if (N) {
+    HB_CUDA(cudaMemcpyAsync(c->m_stamp.p, stamp, sizeof(double) * N, cudaMemcpyHostToDevice, c->stream));
+    HB_CUDA(cudaMemcpyAsync(c->m_meas.p, pose, sizeof(double) * 7 * N, cudaMemcpyHostToDevice, c->stream));
+    HB_CUDA(cudaMemcpyAsync(c->m_sensor.p, sensor, sizeof(int) * N, cudaMemcpyHostToDevice, c->stream));
+  }
+  HB_CUDA(cudaStreamSynchronize(c->stream));
   c->Nm = n;
-  c->h_m_stamp.assign(stamp, stamp + n); c->h_m_sensor.assign(sensor, sensor + n); c->h_m_meas.assign(pose, pose + 7 * static_cast<size_t>(n));
   c->bound = false; c->kernel_args_changed();
   return 0;
 }
 
 int hb200_set_inertial_factors(hb200_ctx* c, int n, const double* stamp, const double* meas) {
   if (!c || n < 0 || (n > 0 && (!stamp || !meas))) return fail(-1, "invalid inertial factors");
+  HB_CUDA(cudaSetDevice(c->device));
+  const size_t N = n;
+  HB_CUDA(c->i_stamp.ensure(N)); HB_CUDA(c->i_meas.ensure(6 * N)); HB_CUDA(c->i_idx.ensure(N));
+  if (N) {
+    HB_CUDA(cudaMemcpyAsync(c->i_stamp.p, stamp, sizeof(double) * N, cudaMemcpyHostToDevice, c->stream));
+    HB_CUDA(cudaMemcpyAsync(c->i_meas.p, meas, sizeof(double) * 6 * N, cudaMemcpyHostToDevice, c->stream));
+  }
+  HB_CUDA(cudaStreamSynchronize(c->stream));
   c->Ni = n;
-  c->h_i_stamp.assign(stamp, stamp + n); c->h_i_meas.assign(meas, meas + 6 * static_cast<size_t>(n));
+  c->i_perm.resize(N); std::iota(c->i_perm.begin(), c->i_perm.end(), 0);
   c->bound = false; c->kernel_args_changed();
   return 0;
 }
@@ -1347,64 +1427,11 @@ int hb200_set_inertial_factors(hb200_ctx* c, int n, const double* stamp, const d
 }  // extern "C"
 
 namespace {
-// After hb200_append_* / hb200_slide the factor lists exist on the device only.  The host mirrors the copy-out calls
-// and a later full hb200_bind need are refreshed here, on demand: the visual list splits by kind (idx.w) into the pixel
-// factors (user indices 0 .. Np-1) and the bearing factors (Np .. Nv-1), each family in bound order; the inertial and
-// manifold lists keep their device order.
-int sync_host_mirrors(hb200_ctx* c) {
-  if (!c->device_managed) return 0;
-  HB_CUDA(cudaSetDevice(c->device));
-  const size_t Nv = c->Nv, Ni = c->Ni, Nm = c->Nm;
-  std::vector<double> st(Nv), px(2 * Nv), vz(Nv);
-  c->h_v_idx.resize(Nv); c->h_i_idx.resize(Ni); c->h_i_stamp.resize(Ni); c->h_i_meas.resize(6 * Ni);
-  c->h_m_stamp.resize(Nm); c->h_m_meas.resize(7 * Nm); c->h_m_sensor.resize(Nm); c->h_m_idx.resize(Nm);
-  if (Nv) {
-    HB_CUDA(cudaMemcpyAsync(st.data(), c->v_stamp.p, sizeof(double) * Nv, cudaMemcpyDeviceToHost, c->stream));
-    HB_CUDA(cudaMemcpyAsync(px.data(), c->v_pixel.p, sizeof(double) * 2 * Nv, cudaMemcpyDeviceToHost, c->stream));
-    HB_CUDA(cudaMemcpyAsync(vz.data(), c->v_z.p, sizeof(double) * Nv, cudaMemcpyDeviceToHost, c->stream));
-    HB_CUDA(cudaMemcpyAsync(c->h_v_idx.data(), c->v_idx.p, sizeof(int4) * Nv, cudaMemcpyDeviceToHost, c->stream));
-  }
-  if (Ni) {
-    HB_CUDA(cudaMemcpyAsync(c->h_i_stamp.data(), c->i_stamp.p, sizeof(double) * Ni, cudaMemcpyDeviceToHost, c->stream));
-    HB_CUDA(cudaMemcpyAsync(c->h_i_meas.data(), c->i_meas.p, sizeof(double) * 6 * Ni, cudaMemcpyDeviceToHost, c->stream));
-    HB_CUDA(cudaMemcpyAsync(c->h_i_idx.data(), c->i_idx.p, sizeof(int4) * Ni, cudaMemcpyDeviceToHost, c->stream));
-  }
-  if (Nm) {
-    HB_CUDA(cudaMemcpyAsync(c->h_m_stamp.data(), c->m_stamp.p, sizeof(double) * Nm, cudaMemcpyDeviceToHost, c->stream));
-    HB_CUDA(cudaMemcpyAsync(c->h_m_meas.data(), c->m_meas.p, sizeof(double) * 7 * Nm, cudaMemcpyDeviceToHost, c->stream));
-    HB_CUDA(cudaMemcpyAsync(c->h_m_sensor.data(), c->m_sensor.p, sizeof(int) * Nm, cudaMemcpyDeviceToHost, c->stream));
-    HB_CUDA(cudaMemcpyAsync(c->h_m_idx.data(), c->m_idx.p, sizeof(int2) * Nm, cudaMemcpyDeviceToHost, c->stream));
-  }
-  HB_CUDA(cudaStreamSynchronize(c->stream));
-  size_t Np = 0;
-  for (size_t f = 0; f < Nv; ++f) Np += c->h_v_idx[f].w == 0;
-  const size_t Nb = Nv - Np;
-  c->h_p_stamp.resize(Np); c->h_p_pixel.resize(2 * Np); c->h_p_cam.resize(Np); c->h_p_lm.resize(Np);
-  c->h_b_stamp.resize(Nb); c->h_b_bearing.resize(3 * Nb); c->h_b_cam.resize(Nb); c->h_b_lm.resize(Nb);
-  c->v_perm.resize(Nv);
-  for (size_t f = 0, p = 0, b = 0; f < Nv; ++f) {
-    const int4 id = c->h_v_idx[f];
-    if (id.w == 0) {
-      c->h_p_stamp[p] = st[f]; c->h_p_pixel[2 * p] = px[2 * f]; c->h_p_pixel[2 * p + 1] = px[2 * f + 1]; c->h_p_cam[p] = id.z; c->h_p_lm[p] = id.y;
-      c->v_perm[f] = static_cast<int>(p++);
-    } else {
-      c->h_b_stamp[b] = st[f]; c->h_b_bearing[3 * b] = px[2 * f]; c->h_b_bearing[3 * b + 1] = px[2 * f + 1]; c->h_b_bearing[3 * b + 2] = vz[f];
-      c->h_b_cam[b] = id.z; c->h_b_lm[b] = id.y;
-      c->v_perm[f] = static_cast<int>(Np + b++);
-    }
-  }
-  c->Np = static_cast<int>(Np); c->Nb = static_cast<int>(Nb);
-  visual_user_order(c);   // what hb200_set_pixel_factors / hb200_set_bearing_factors leave for hb200_bind
-  c->i_perm.resize(Ni); std::iota(c->i_perm.begin(), c->i_perm.end(), 0);
-  c->device_managed = false;
-  return 0;
-}
-
 // Everything the iteration runs on that follows from the bound factor lists on the device: the incidence lists
 // (landmark CSR, inertial runs, longest track) by counting + scan kernels with one small read-back, then the output
 // buffers and launch shapes of every factor family and the reduced system.  hb200_bind, hb200_append_* and
-// hb200_slide all end here; the ones that change the lists on the device mark the host mirrors stale
-// (device_managed) and drop the snapshot themselves.
+// hb200_slide all end here; the ones that change the lists on the device clear the user-index maps and drop the
+// snapshot themselves.
 int derive_window(hb200_ctx* c) {
   const int Nv = c->Nv, Ni = c->Ni, Nm = c->Nm, L = c->L;
   HB_CUDA(c->w_scal.ensure(8));
@@ -1468,27 +1495,33 @@ int derive_window(hb200_ctx* c) {
   return sync_layout(c);   // multi-GPU: all ranks adopt the widest band (collective when a communicator is attached)
 }
 
-// Uploads the stamps, camera and landmark ids of n visual factors of one kind (0 pixel, 1 bearing) to list positions
-// [at, at + n) and binds them there; factors that fail to bind are counted in d_invalid[0].  The ids only feed
-// bind_pixel_kernel, so they go through window scratch.
-int bind_pixel_range(hb200_ctx* c, int at, int n, const double* stamp, const int* camera, const int* landmark, int kind) {
-  HB_CUDA(c->w_keep.ensure(n)); HB_CUDA(c->w_pos.ensure(n));
-  HB_CUDA(cudaMemcpyAsync(c->v_stamp.p + at, stamp, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
-  HB_CUDA(cudaMemcpyAsync(c->w_keep.p, camera, sizeof(int) * n, cudaMemcpyHostToDevice, c->stream));
-  HB_CUDA(cudaMemcpyAsync(c->w_pos.p, landmark, sizeof(int) * n, cudaMemcpyHostToDevice, c->stream));
-  bind_pixel_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(n, c->v_stamp.p + at, c->w_keep.p, c->w_pos.p, c->knots[0].p, c->K, c->k, c->C, c->L, kind, c->v_idx.p + at, c->d_invalid.p);
+// Binds the visual factors at list positions [at, at + n) in place; factors that fail to bind are counted in d_invalid[0].
+int bind_pixel_range(hb200_ctx* c, int at, int n) {
+  bind_pixel_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(n, c->v_stamp.p + at, c->knots[0].p, c->K, c->k, c->C, c->L, c->v_idx.p + at, c->d_invalid.p);
   HB_LAUNCH(c, "bind_pixel_kernel");
   return 0;
 }
 
-// Uploads the stamps of n inertial factors to list positions [at, at + n) and binds them there; factors that fail to
-// bind are counted in d_invalid[0].
-int bind_inertial_range(hb200_ctx* c, int at, int n, const double* stamp) {
-  HB_CUDA(cudaMemcpyAsync(c->i_stamp.p + at, stamp, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
+// Binds the inertial factors at list positions [at, at + n) in place; factors that fail to bind are counted in d_invalid[0].
+int bind_inertial_range(hb200_ctx* c, int at, int n) {
   bind_inertial_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(n, c->i_stamp.p + at, c->knots[0].p, c->K, c->k, c->bg[0].p, c->Kbg, c->ba[0].p, c->Kba, c->kb,
                                                              c->i_idx.p + at, c->d_invalid.p);
   HB_LAUNCH(c, "bind_inertial_kernel");
   return 0;
+}
+
+// Bound order of a list whose index maps id (host read-back) are not yet sorted by `less`: the stable sort's inverse
+// permutation (old position -> new), with id and the user-index map perm permuted alongside.
+template <typename Less>
+std::vector<int> bound_order(std::vector<int4>& id, std::vector<int>& perm, Less less) {
+  const size_t n = id.size();
+  std::vector<int> s(n), inv(n), perm_s(n);
+  std::vector<int4> id_s(n);
+  std::iota(s.begin(), s.end(), 0);
+  std::stable_sort(s.begin(), s.end(), [&](int a, int b) { return less(id[a], id[b]); });
+  for (size_t p = 0; p < n; ++p) { inv[s[p]] = static_cast<int>(p); id_s[p] = id[s[p]]; perm_s[p] = perm[s[p]]; }
+  id.swap(id_s); perm.swap(perm_s);
+  return inv;
 }
 }  // namespace
 
@@ -1496,80 +1529,49 @@ extern "C" {
 
 int hb200_bind(hb200_ctx* c, int* num_invalid) {
   if (!c) return fail(-1, "null context");
-  { const int rs = sync_host_mirrors(c); if (rs) return rs; }
   if (c->K == 0) return fail(-2, "spline not set");
   if (c->Ni && (c->Kbg == 0 || c->Kba == 0)) return fail(-2, "bias splines not set");
   if (c->Nv && (c->C == 0 || c->L == 0)) return fail(-2, "cameras / landmarks not set");
   if (c->Nm && c->P == 0) return fail(-2, "pose sensors not set");
   HB_CUDA(cudaSetDevice(c->device));
+  int rc = ensure_perms(c);
+  if (rc) return rc;
   const int Nv = c->Nv, Ni = c->Ni, Nm = c->Nm;
   HB_CUDA(c->d_invalid.ensure(1));
   HB_CUDA(cudaMemsetAsync(c->d_invalid.p, 0, sizeof(int), c->stream));
-  HB_CUDA(c->v_stamp.ensure(std::max(Nv, 1))); HB_CUDA(c->v_pixel.ensure(2 * static_cast<size_t>(std::max(Nv, 1))));
-  HB_CUDA(c->v_idx.ensure(std::max(Nv, 1))); HB_CUDA(c->v_z.ensure(std::max(Nv, 1)));
-  HB_CUDA(c->m_stamp.ensure(std::max(Nm, 1))); HB_CUDA(c->m_meas.ensure(7 * static_cast<size_t>(std::max(Nm, 1)))); HB_CUDA(c->m_sensor.ensure(std::max(Nm, 1)));
-  HB_CUDA(c->m_idx.ensure(std::max(Nm, 1)));
-  c->h_m_idx.assign(Nm, make_int2(0, 0));
-  HB_CUDA(c->i_stamp.ensure(std::max(Ni, 1))); HB_CUDA(c->i_meas.ensure(6 * static_cast<size_t>(std::max(Ni, 1)))); HB_CUDA(c->i_idx.ensure(std::max(Ni, 1)));
-  c->h_v_idx.assign(Nv, make_int4(0, 0, 0, 0)); c->h_i_idx.assign(Ni, make_int4(0, 0, 0, 0));
-  // pass 1: index maps in user order (device), a2/a4
-  int rc = 0;
-  if (Nv) {
-    if ((rc = bind_pixel_range(c, 0, Nv, c->h_v_stamp.data(), c->h_v_cam.data(), c->h_v_lm.data(), 0))) return rc;
-    HB_CUDA(cudaMemcpyAsync(c->h_v_idx.data(), c->v_idx.p, sizeof(int4) * Nv, cudaMemcpyDeviceToHost, c->stream));
-  }
-  if (Ni) {
-    if ((rc = bind_inertial_range(c, 0, Ni, c->h_i_stamp.data()))) return rc;
-    HB_CUDA(cudaMemcpyAsync(c->h_i_idx.data(), c->i_idx.p, sizeof(int4) * Ni, cudaMemcpyDeviceToHost, c->stream));
-  }
+  // pass 1: index maps of the lists where they stand (a2/a4), one read-back of the invalid count and the keys
+  if (Nv && (rc = bind_pixel_range(c, 0, Nv))) return rc;
+  if (Ni && (rc = bind_inertial_range(c, 0, Ni))) return rc;
   if (Nm) {
-    HB_CUDA(cudaMemcpyAsync(c->m_stamp.p, c->h_m_stamp.data(), sizeof(double) * Nm, cudaMemcpyHostToDevice, c->stream));
-    HB_CUDA(cudaMemcpyAsync(c->m_meas.p, c->h_m_meas.data(), sizeof(double) * 7 * Nm, cudaMemcpyHostToDevice, c->stream));
-    HB_CUDA(cudaMemcpyAsync(c->m_sensor.p, c->h_m_sensor.data(), sizeof(int) * Nm, cudaMemcpyHostToDevice, c->stream));
     bind_manifold_kernel<<<(Nm + 127) / 128, 128, 0, c->stream>>>(Nm, c->m_stamp.p, c->m_sensor.p, c->knots[0].p, c->K, c->k, c->P, c->m_idx.p, c->d_invalid.p);
     HB_LAUNCH(c, "bind_manifold_kernel");
-    HB_CUDA(cudaMemcpyAsync(c->h_m_idx.data(), c->m_idx.p, sizeof(int2) * Nm, cudaMemcpyDeviceToHost, c->stream));
   }
+  std::vector<int4> vi(Nv), ii(Ni);
   int invalid = 0;
+  if (Nv) HB_CUDA(cudaMemcpyAsync(vi.data(), c->v_idx.p, sizeof(int4) * Nv, cudaMemcpyDeviceToHost, c->stream));
+  if (Ni) HB_CUDA(cudaMemcpyAsync(ii.data(), c->i_idx.p, sizeof(int4) * Ni, cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaMemcpyAsync(&invalid, c->d_invalid.p, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
   if (num_invalid) *num_invalid = invalid;
   if (invalid) return fail(2, "%d factor(s) reference a stamp outside the spline's valid range or an invalid camera / landmark / sensor", invalid);
-  for (int u = c->Np; u < Nv; ++u) c->h_v_idx[u].w = 1;   // bearing factors
 
-  // pass 2: bound order = stable sort by knot base index (pixel) / (base, gyro base, accel base)
-  c->v_perm.resize(Nv); std::iota(c->v_perm.begin(), c->v_perm.end(), 0);
-  c->i_perm.resize(Ni); std::iota(c->i_perm.begin(), c->i_perm.end(), 0);
-  {
-    const std::vector<int4>& id = c->h_v_idx;
-    if (!std::is_sorted(id.begin(), id.end(), [](const int4& a, const int4& b) { return a.x < b.x; }))
-      std::stable_sort(c->v_perm.begin(), c->v_perm.end(), [&](int a, int b) { return id[a].x < id[b].x; });
-    auto key = [](const int4& a, const int4& b) { return a.x != b.x ? a.x < b.x : (a.y != b.y ? a.y < b.y : a.z < b.z); };
-    const std::vector<int4>& ii = c->h_i_idx;
-    if (!std::is_sorted(ii.begin(), ii.end(), key)) std::stable_sort(c->i_perm.begin(), c->i_perm.end(), [&](int a, int b) { return key(ii[a], ii[b]); });
+  // pass 2: bound order = stable sort by knot base index (visual) / (base, gyro base, accel base) (inertial), applied on
+  // the device by the compaction kernels with pos = the inverse permutation; the manifold list stays as it is
+  auto by_base = [](const int4& a, const int4& b) { return a.x < b.x; };
+  auto by_bases = [](const int4& a, const int4& b) { return a.x != b.x ? a.x < b.x : (a.y != b.y ? a.y < b.y : a.z < b.z); };
+  std::vector<int> v_inv, i_inv;   // (host sources of the uploads below, alive until the synchronize)
+  HB_CUDA(c->w_pos.ensure(std::max(std::max(Nv, Ni), 1)));
+  if (!std::is_sorted(vi.begin(), vi.end(), by_base)) {
+    v_inv = bound_order(vi, c->v_perm, by_base);
+    HB_CUDA(cudaMemcpyAsync(c->w_pos.p, v_inv.data(), sizeof(int) * Nv, cudaMemcpyHostToDevice, c->stream));
+    if ((rc = compact_visual(c, Nv, nullptr, c->w_pos.p, nullptr, 0, 0, Nv))) return rc;
   }
-  {
-    std::vector<double> st(Nv), px(2 * static_cast<size_t>(Nv)), vz(Nv);
-    std::vector<int4> id(Nv);
-    for (int p = 0; p < Nv; ++p) { const int u = c->v_perm[p]; st[p] = c->h_v_stamp[u]; px[2 * p] = c->h_v_pixel[2 * u]; px[2 * p + 1] = c->h_v_pixel[2 * u + 1]; vz[p] = c->h_v_z[u]; id[p] = c->h_v_idx[u]; }
-    c->h_v_idx = id;
-    if (Nv) {
-      HB_CUDA(cudaMemcpyAsync(c->v_stamp.p, st.data(), sizeof(double) * Nv, cudaMemcpyHostToDevice, c->stream));
-      HB_CUDA(cudaMemcpyAsync(c->v_pixel.p, px.data(), sizeof(double) * 2 * Nv, cudaMemcpyHostToDevice, c->stream));
-      HB_CUDA(cudaMemcpyAsync(c->v_z.p, vz.data(), sizeof(double) * Nv, cudaMemcpyHostToDevice, c->stream));
-      HB_CUDA(cudaMemcpyAsync(c->v_idx.p, id.data(), sizeof(int4) * Nv, cudaMemcpyHostToDevice, c->stream));
-    }
-    std::vector<double> is(Ni), im(6 * static_cast<size_t>(Ni));
-    std::vector<int4> iid(Ni);
-    for (int p = 0; p < Ni; ++p) { const int u = c->i_perm[p]; is[p] = c->h_i_stamp[u]; for (int q = 0; q < 6; ++q) im[6 * p + q] = c->h_i_meas[6 * u + q]; iid[p] = c->h_i_idx[u]; }
-    c->h_i_idx = iid;
-    if (Ni) {
-      HB_CUDA(cudaMemcpyAsync(c->i_stamp.p, is.data(), sizeof(double) * Ni, cudaMemcpyHostToDevice, c->stream));
-      HB_CUDA(cudaMemcpyAsync(c->i_meas.p, im.data(), sizeof(double) * 6 * Ni, cudaMemcpyHostToDevice, c->stream));
-      HB_CUDA(cudaMemcpyAsync(c->i_idx.p, iid.data(), sizeof(int4) * Ni, cudaMemcpyHostToDevice, c->stream));
-    }
-    HB_CUDA(cudaStreamSynchronize(c->stream));
+  if (!std::is_sorted(ii.begin(), ii.end(), by_bases)) {
+    i_inv = bound_order(ii, c->i_perm, by_bases);
+    HB_CUDA(cudaMemcpyAsync(c->w_pos.p, i_inv.data(), sizeof(int) * Ni, cudaMemcpyHostToDevice, c->stream));
+    if ((rc = compact_inertial(c, Ni, nullptr, c->w_pos.p, 0, 0, 0, Ni))) return rc;
   }
+  HB_CUDA(cudaStreamSynchronize(c->stream));
   if ((rc = derive_window(c))) return rc;
   {
     // landmark groups for the large-window Schur kernel: observed landmarks ordered by their first knot base, cut so that
@@ -1579,7 +1581,7 @@ int hb200_bind(hb200_ctx* c, int* num_invalid) {
     if (c->L >= kSchurGroupMin && Nv) {
       // first / last knot base of every observed landmark (-1: unobserved); bound order is ascending knot base
       std::vector<int> first(c->L, -1), last(c->L, -1);
-      for (const int4& id : c->h_v_idx) { if (first[id.y] < 0) first[id.y] = id.x; last[id.y] = id.x; }
+      for (const int4& id : vi) { if (first[id.y] < 0) first[id.y] = id.x; last[id.y] = id.x; }
       std::vector<int> order;
       order.reserve(c->L);
       for (int l = 0; l < c->L; ++l) if (first[l] >= 0) order.push_back(l);
@@ -1619,13 +1621,19 @@ int hb200_bind(hb200_ctx* c, int* num_invalid) {
 
 int hb200_get_index_maps(hb200_ctx* c, int* pixel_base, int* inertial_base, int* gyro_bias_base, int* accel_bias_base) {
   if (!c || !c->bound) return fail(-2, "not bound");
-  { const int rs = sync_host_mirrors(c); if (rs) return rs; }
-  for (int p = 0; p < c->Nv; ++p) if (pixel_base && c->v_perm[p] < c->Np) pixel_base[c->v_perm[p]] = c->h_v_idx[p].x;
-  for (int p = 0; p < c->Ni; ++p) {
+  int rc = ensure_perms(c);
+  if (rc) return rc;
+  const int Nv = pixel_base ? c->Nv : 0, Ni = (inertial_base || gyro_bias_base || accel_bias_base) ? c->Ni : 0;
+  std::vector<int4> vi(Nv), ii(Ni);
+  if (Nv) HB_CUDA(cudaMemcpyAsync(vi.data(), c->v_idx.p, sizeof(int4) * Nv, cudaMemcpyDeviceToHost, c->stream));
+  if (Ni) HB_CUDA(cudaMemcpyAsync(ii.data(), c->i_idx.p, sizeof(int4) * Ni, cudaMemcpyDeviceToHost, c->stream));
+  HB_CUDA(cudaStreamSynchronize(c->stream));
+  for (int p = 0; p < Nv; ++p) if (c->v_perm[p] < c->Np) pixel_base[c->v_perm[p]] = vi[p].x;
+  for (int p = 0; p < Ni; ++p) {
     const int u = c->i_perm[p];
-    if (inertial_base) inertial_base[u] = c->h_i_idx[p].x;
-    if (gyro_bias_base) gyro_bias_base[u] = c->h_i_idx[p].y;
-    if (accel_bias_base) accel_bias_base[u] = c->h_i_idx[p].z;
+    if (inertial_base) inertial_base[u] = ii[p].x;
+    if (gyro_bias_base) gyro_bias_base[u] = ii[p].y;
+    if (accel_bias_base) accel_bias_base[u] = ii[p].z;
   }
   return 0;
 }
@@ -1645,7 +1653,7 @@ int hb200_evaluate(hb200_ctx* c, int flags) {
 
 int hb200_get_pixel_outputs(hb200_ctx* c, double* r, double* Jp, double* Jl) {
   if (!c || !c->bound) return fail(-2, "not bound");
-  { const int rs = sync_host_mirrors(c); if (rs) return rs; }
+  { const int rs = ensure_perms(c); if (rs) return rs; }
   HB_CUDA(cudaSetDevice(c->device));
   const size_t N = c->Nv, w = 12 * static_cast<size_t>(c->k);
   std::vector<double> tr(2 * N), tJ(Jp ? w * N : 0), tl(Jl ? 6 * N : 0);
@@ -1667,7 +1675,7 @@ int hb200_get_pixel_outputs(hb200_ctx* c, double* r, double* Jp, double* Jl) {
 
 int hb200_get_bearing_outputs(hb200_ctx* c, double* r, double* Jp, double* Jl) {
   if (!c || !c->bound) return fail(-2, "not bound");
-  { const int rs = sync_host_mirrors(c); if (rs) return rs; }
+  { const int rs = ensure_perms(c); if (rs) return rs; }
   HB_CUDA(cudaSetDevice(c->device));
   const size_t N = c->Nv, w = 12 * static_cast<size_t>(c->k);
   if (c->Nb == 0) return 0;
@@ -1688,7 +1696,6 @@ int hb200_get_bearing_outputs(hb200_ctx* c, double* r, double* Jp, double* Jl) {
 
 int hb200_get_manifold_outputs(hb200_ctx* c, double* r, double* Jp) {
   if (!c || !c->bound) return fail(-2, "not bound");
-  { const int rs = sync_host_mirrors(c); if (rs) return rs; }
   HB_CUDA(cudaSetDevice(c->device));
   const size_t N = c->Nm, w = 36 * static_cast<size_t>(c->k);
   if (N == 0) return 0;
@@ -1700,7 +1707,7 @@ int hb200_get_manifold_outputs(hb200_ctx* c, double* r, double* Jp) {
 
 int hb200_get_inertial_outputs(hb200_ctx* c, double* r, double* Jp, double* wg, double* wa, double* Jg) {
   if (!c || !c->bound) return fail(-2, "not bound");
-  { const int rs = sync_host_mirrors(c); if (rs) return rs; }
+  { const int rs = ensure_perms(c); if (rs) return rs; }
   HB_CUDA(cudaSetDevice(c->device));
   const size_t N = c->Ni, w = 36 * static_cast<size_t>(c->k);
   std::vector<double> tr(6 * N), tJ(Jp ? w * N : 0), tg(wg ? 4 * N : 0), ta(wa ? 4 * N : 0), tG(Jg ? 12 * N : 0);
@@ -1790,7 +1797,7 @@ int hb200_factor_evaluate(hb200_ctx* c, int kind, int index, const double* const
   if (!c || !c->bound) return fail(-2, "not bound");
   if (!c->evaluated_J) return fail(-2, "call hb200_evaluate(HB200_EVAL_JACOBIANS) first");
   if (!parameters || !residuals) return fail(-1, "null argument");
-  { const int rs = sync_host_mirrors(c); if (rs) return rs; }
+  { const int rs = ensure_perms(c); if (rs) return rs; }
   if (!c->mirror_valid) {
     const size_t k = c->k;
     c->m_v_r.resize(2 * static_cast<size_t>(c->Np)); c->m_v_Jp.resize(12 * k * c->Np); c->m_v_Jl.resize(6 * static_cast<size_t>(c->Np));
@@ -2585,27 +2592,17 @@ int check_device_window(hb200_ctx* c) {
   return 0;
 }
 
-// capacity for N visual factors, the bound ones preserved
-int grow_visual(hb200_ctx* c, size_t N) {
-  const size_t Nv = c->Nv;
-  HB_CUDA(c->v_stamp.grow(N, Nv, c->stream)); HB_CUDA(c->v_pixel.grow(2 * N, 2 * Nv, c->stream));
-  HB_CUDA(c->v_z.grow(N, Nv, c->stream)); HB_CUDA(c->v_idx.grow(N, Nv, c->stream));
-  return 0;
-}
-
-// Appends n visual factors of one kind to the tail of the visual list and binds them there: xy = pixel [n][2] (kind 0)
-// or the first two bearing components (kind 1), z = the third bearing component (kind 1 only).  The counts advance
-// only when every new factor binds and the tail keeps the bound order.
-int append_visual(hb200_ctx* c, int n, const double* stamp, const int* camera, const int* landmark, const double* xy, const double* z, int kind) {
+// Appends n visual factors of one kind to the tail of the visual list and binds them there: meas = pixel [n][2] (kind 0)
+// or bearing [n][3] (kind 1).  The counts advance only when every new factor binds and the tail keeps the bound order.
+int append_visual(hb200_ctx* c, int n, const double* stamp, const int* camera, const int* landmark, const double* meas, int kind) {
   HB_CUDA(cudaSetDevice(c->device));
   const size_t Nv = c->Nv;
   int rc = grow_visual(c, Nv + n);
   if (rc) return rc;
   HB_CUDA(c->d_invalid.ensure(2));
   HB_CUDA(cudaMemsetAsync(c->d_invalid.p, 0, 2 * sizeof(int), c->stream));
-  HB_CUDA(cudaMemcpyAsync(c->v_pixel.p + 2 * Nv, xy, sizeof(double) * 2 * n, cudaMemcpyHostToDevice, c->stream));
-  if (z) HB_CUDA(cudaMemcpyAsync(c->v_z.p + Nv, z, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
-  if ((rc = bind_pixel_range(c, static_cast<int>(Nv), n, stamp, camera, landmark, kind))) return rc;
+  if ((rc = upload_visual(c, static_cast<int>(Nv), n, stamp, camera, landmark, meas, kind))) return rc;
+  if ((rc = bind_pixel_range(c, static_cast<int>(Nv), n))) return rc;
   tail_sorted_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(static_cast<int>(Nv), n, c->v_idx.p, c->d_invalid.p + 1);
   HB_LAUNCH(c, "tail_sorted_kernel");
   int bad[2] = {0, 0};
@@ -2616,7 +2613,7 @@ int append_visual(hb200_ctx* c, int n, const double* stamp, const int* camera, c
                           kind ? "bearing" : "pixel");
   c->Nv = static_cast<int>(Nv) + n;
   (kind ? c->Nb : c->Np) += n;
-  c->device_managed = true; c->have_snapshot = false;
+  c->v_perm.clear(); c->i_perm.clear(); c->have_snapshot = false;
   return derive_window(c);
 }
 }  // namespace
@@ -2737,7 +2734,7 @@ int hb200_append_landmarks(hb200_ctx* c, int n, const double* xyz) {
   HB_CUDA(cudaMemcpyAsync(c->lms[0].p + 3 * L, xyz, sizeof(double) * 3 * n, cudaMemcpyHostToDevice, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
   c->L = static_cast<int>(L) + n;
-  c->device_managed = true; c->have_snapshot = false;
+  c->v_perm.clear(); c->i_perm.clear(); c->have_snapshot = false;
   return derive_window(c);
 }
 
@@ -2745,17 +2742,14 @@ int hb200_append_pixel_factors(hb200_ctx* c, int n, const double* stamp, const i
   int rc = check_device_window(c);
   if (rc) return rc;
   if (n <= 0 || !stamp || !camera || !landmark || !pixel) return fail(-1, "invalid pixel factors");
-  return append_visual(c, n, stamp, camera, landmark, pixel, nullptr, 0);
+  return append_visual(c, n, stamp, camera, landmark, pixel, 0);
 }
 
 int hb200_append_bearing_factors(hb200_ctx* c, int n, const double* stamp, const int* camera, const int* landmark, const double* bearing) {
   int rc = check_device_window(c);
   if (rc) return rc;
   if (n <= 0 || !stamp || !camera || !landmark || !bearing) return fail(-1, "invalid bearing factors");
-  // the visual list's compact layout: x, y in the pixel pair, z apart
-  std::vector<double> xy(2 * static_cast<size_t>(n)), z(n);
-  for (int f = 0; f < n; ++f) { xy[2 * f] = bearing[3 * f]; xy[2 * f + 1] = bearing[3 * f + 1]; z[f] = bearing[3 * f + 2]; }
-  return append_visual(c, n, stamp, camera, landmark, xy.data(), z.data(), 1);
+  return append_visual(c, n, stamp, camera, landmark, bearing, 1);
 }
 
 int hb200_append_manifold_factors(hb200_ctx* c, int n, const double* stamp, const int* sensor, const double* pose) {
@@ -2779,7 +2773,7 @@ int hb200_append_manifold_factors(hb200_ctx* c, int n, const double* stamp, cons
   HB_CUDA(cudaStreamSynchronize(c->stream));
   if (bad) return fail(2, "%d appended factor(s) reference a stamp outside the spline's valid range or an invalid pose sensor", bad);
   c->Nm = static_cast<int>(Nm) + n;
-  c->device_managed = true; c->have_snapshot = false;
+  c->v_perm.clear(); c->i_perm.clear(); c->have_snapshot = false;
   return derive_window(c);
 }
 
@@ -2835,7 +2829,7 @@ int hb200_append_stereo_tracks(hb200_ctx* c, int n, const double* stamp, const i
     for (size_t f = 0, r = 0; f < N; ++f) landmark_out[f] = landmark[f] < 0 ? static_cast<int>(L + r++) : landmark[f];
   if (num_new) *num_new = h[2];
   c->Nv = static_cast<int>(Nv + 2 * N); c->Nb += 2 * n; c->L = static_cast<int>(L) + h[2];
-  c->device_managed = true; c->have_snapshot = false;
+  c->v_perm.clear(); c->i_perm.clear(); c->have_snapshot = false;
   return derive_window(c);
 }
 
@@ -2849,8 +2843,9 @@ int hb200_append_inertial_factors(hb200_ctx* c, int n, const double* stamp, cons
   HB_CUDA(c->i_stamp.grow(Ni + n, Ni, c->stream)); HB_CUDA(c->i_meas.grow(6 * (Ni + n), 6 * Ni, c->stream)); HB_CUDA(c->i_idx.grow(Ni + n, Ni, c->stream));
   HB_CUDA(c->d_invalid.ensure(2));
   HB_CUDA(cudaMemsetAsync(c->d_invalid.p, 0, 2 * sizeof(int), c->stream));
+  HB_CUDA(cudaMemcpyAsync(c->i_stamp.p + Ni, stamp, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
   HB_CUDA(cudaMemcpyAsync(c->i_meas.p + 6 * Ni, meas, sizeof(double) * 6 * n, cudaMemcpyHostToDevice, c->stream));
-  if ((rc = bind_inertial_range(c, static_cast<int>(Ni), n, stamp))) return rc;
+  if ((rc = bind_inertial_range(c, static_cast<int>(Ni), n))) return rc;
   tail_sorted_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(static_cast<int>(Ni), n, c->i_idx.p, c->d_invalid.p + 1);
   HB_LAUNCH(c, "tail_sorted_kernel");
   int bad[2] = {0, 0};
@@ -2859,7 +2854,7 @@ int hb200_append_inertial_factors(hb200_ctx* c, int n, const double* stamp, cons
   if (bad[0]) return fail(2, "%d appended factor(s) reference a stamp outside the state or bias splines' valid range", bad[0]);
   if (bad[1]) return fail(3, "appended factors must arrive in stamp order (%d fall before the end of the list): use hb200_set_inertial_factors + hb200_bind", bad[1]);
   c->Ni = static_cast<int>(Ni) + n;
-  c->device_managed = true; c->have_snapshot = false;
+  c->v_perm.clear(); c->i_perm.clear(); c->have_snapshot = false;
   return derive_window(c);
 }
 
@@ -2931,26 +2926,9 @@ int hb200_slide(hb200_ctx* c, double lower_bound, int flags, hb200_slide_stats* 
   // compaction into the alternate buffers, then swap
   const int n_alt = std::max(std::max(std::max(Nv_new, Ni_new), Nm_new), 1);
   HB_CUDA(c->alt_stamp.ensure(n_alt)); HB_CUDA(c->alt_idx.ensure(n_alt));
-  HB_CUDA(c->alt_pixel.ensure(std::max(Nv_new, 1))); HB_CUDA(c->alt_z.ensure(std::max(Nv_new, 1)));
-  if (Nv) {
-    compact_visual_kernel<<<(Nv + 255) / 256, 256, 0, c->stream>>>(Nv, c->w_keep.p, c->w_pos.p, c->w_lpos.p, shift, c->v_stamp.p, reinterpret_cast<const double2*>(c->v_pixel.p),
-                                                                  c->v_z.p, c->v_idx.p, c->alt_stamp.p, c->alt_pixel.p, c->alt_z.p, c->alt_idx.p);
-    HB_LAUNCH(c, "compact_visual_kernel");
-    // (v_pixel is a DevBuf<double>: copy the compacted pairs back instead of swapping differently typed buffers)
-    HB_CUDA(cudaMemcpyAsync(c->v_pixel.p, c->alt_pixel.p, sizeof(double2) * Nv_new, cudaMemcpyDeviceToDevice, c->stream));
-    HB_CUDA(cudaMemcpyAsync(c->v_stamp.p, c->alt_stamp.p, sizeof(double) * Nv_new, cudaMemcpyDeviceToDevice, c->stream));
-    HB_CUDA(cudaMemcpyAsync(c->v_z.p, c->alt_z.p, sizeof(double) * Nv_new, cudaMemcpyDeviceToDevice, c->stream));
-    HB_CUDA(cudaMemcpyAsync(c->v_idx.p, c->alt_idx.p, sizeof(int4) * Nv_new, cudaMemcpyDeviceToDevice, c->stream));
-  }
+  if (Nv && (rc = compact_visual(c, Nv, c->w_keep.p, c->w_pos.p, c->w_lpos.p, shift, 0, Nv_new))) return rc;
   HB_CUDA(c->alt_meas.ensure(std::max(6 * static_cast<size_t>(Ni_new), 7 * static_cast<size_t>(Nm_new)) + 1));
-  if (Ni) {
-    compact_inertial_kernel<<<(Ni + 255) / 256, 256, 0, c->stream>>>(Ni, i_keep, i_pos, shift, g_shift, a_shift, c->i_stamp.p, c->i_meas.p, c->i_idx.p, c->alt_stamp.p,
-                                                                     c->alt_meas.p, c->alt_idx.p);
-    HB_LAUNCH(c, "compact_inertial_kernel");
-    HB_CUDA(cudaMemcpyAsync(c->i_stamp.p, c->alt_stamp.p, sizeof(double) * Ni_new, cudaMemcpyDeviceToDevice, c->stream));
-    HB_CUDA(cudaMemcpyAsync(c->i_meas.p, c->alt_meas.p, sizeof(double) * 6 * Ni_new, cudaMemcpyDeviceToDevice, c->stream));
-    HB_CUDA(cudaMemcpyAsync(c->i_idx.p, c->alt_idx.p, sizeof(int4) * Ni_new, cudaMemcpyDeviceToDevice, c->stream));
-  }
+  if (Ni && (rc = compact_inertial(c, Ni, i_keep, i_pos, shift, g_shift, a_shift, Ni_new))) return rc;
   if (Nm) {
     HB_CUDA(c->alt_midx.ensure(std::max(Nm_new, 1))); HB_CUDA(c->alt_sensor.ensure(std::max(Nm_new, 1)));
     compact_manifold_kernel<<<(Nm + 255) / 256, 256, 0, c->stream>>>(Nm, m_keep, m_pos, shift, c->m_stamp.p, c->m_meas.p, c->m_sensor.p, c->m_idx.p, c->alt_stamp.p, c->alt_meas.p,
@@ -3003,7 +2981,7 @@ int hb200_slide(hb200_ctx* c, double lower_bound, int flags, hb200_slide_stats* 
     stats->visual_factors_dropped = Nv - Nv_new; stats->inertial_factors_dropped = Ni - Ni_new;
     stats->knots = K_new; stats->landmarks = L_new; stats->visual_factors = Nv_new; stats->inertial_factors = Ni_new;
   }
-  c->device_managed = true; c->have_snapshot = false;
+  c->v_perm.clear(); c->i_perm.clear(); c->have_snapshot = false;
   return derive_window(c);
 }
 

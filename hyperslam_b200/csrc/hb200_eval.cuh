@@ -114,16 +114,16 @@ HB_DI int segment_base(const double* knots, int stride, int stamp_off, int K, in
   return base;
 }
 
-// kind: 0 pixel, 1 bearing factor (idx.w of the visual list)
-__global__ void bind_pixel_kernel(int n, const double* __restrict__ stamp, const int* __restrict__ cam, const int* __restrict__ lm,
-                                  const double* __restrict__ knots, int K, int k, int C, int L, int kind, int4* __restrict__ idx,
-                                  int* __restrict__ num_invalid) {
+// visual list index map in place: landmark (y), camera (z) and kind (w: 0 pixel, 1 bearing factor) are read, the knot
+// base is written to x
+__global__ void bind_pixel_kernel(int n, const double* __restrict__ stamp, const double* __restrict__ knots, int K, int k, int C, int L,
+                                  int4* __restrict__ idx, int* __restrict__ num_invalid) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= n) return;
-  const int base = segment_base(knots, 8, 7, K, k, stamp[f]);
-  const int c = cam[f], l = lm[f];
-  idx[f] = make_int4(base, l, c, kind);
-  if (base < 0 || c < 0 || c >= C || l < 0 || l >= L) atomicAdd(num_invalid, 1);
+  int4 id = idx[f];
+  id.x = segment_base(knots, 8, 7, K, k, stamp[f]);
+  idx[f] = id;
+  if (id.x < 0 || id.z < 0 || id.z >= C || id.y < 0 || id.y >= L) atomicAdd(num_invalid, 1);
 }
 
 __global__ void bind_inertial_kernel(int n, const double* __restrict__ stamp, const double* __restrict__ knots, int K, int k,

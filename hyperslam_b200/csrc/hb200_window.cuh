@@ -101,16 +101,18 @@ __global__ void inertial_keep_kernel(int n, const Idx* __restrict__ idx, int ord
   }
 }
 
-// z: third bearing component of bearing factors (idx.w = 1), moved with the pixel pair
+// z: third bearing component of bearing factors (idx.w = 1), moved with the pixel pair.  keep == nullptr keeps every
+// factor (pos is then a permutation), lm_pos == nullptr keeps the landmark indices.
 __global__ void compact_visual_kernel(int n, const int* __restrict__ keep, const int* __restrict__ pos, const int* __restrict__ lm_pos, int knot_shift,
                                       const double* __restrict__ stamp, const double2* __restrict__ pixel, const double* __restrict__ z,
                                       const int4* __restrict__ idx, double* __restrict__ stamp_o, double2* __restrict__ pixel_o,
                                       double* __restrict__ z_o, int4* __restrict__ idx_o) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
-  if (f >= n || !keep[f]) return;
+  if (f >= n || (keep && !keep[f])) return;
   const int p = pos[f];
   int4 id = idx[f];
-  id.x -= knot_shift; id.y = lm_pos[id.y];
+  id.x -= knot_shift;
+  if (lm_pos) id.y = lm_pos[id.y];
   stamp_o[p] = stamp[f]; pixel_o[p] = pixel[f]; z_o[p] = z[f]; idx_o[p] = id;
 }
 __global__ void compact_manifold_kernel(int n, const int* __restrict__ keep, const int* __restrict__ pos, int knot_shift, const double* __restrict__ stamp,
@@ -125,11 +127,12 @@ __global__ void compact_manifold_kernel(int n, const int* __restrict__ keep, con
 #pragma unroll
   for (int q = 0; q < 7; ++q) meas_o[7 * static_cast<size_t>(p) + q] = meas[7 * static_cast<size_t>(f) + q];
 }
+// keep == nullptr: every factor stays
 __global__ void compact_inertial_kernel(int n, const int* __restrict__ keep, const int* __restrict__ pos, int knot_shift, int gyro_shift, int accel_shift,
                                         const double* __restrict__ stamp, const double* __restrict__ meas, const int4* __restrict__ idx,
                                         double* __restrict__ stamp_o, double* __restrict__ meas_o, int4* __restrict__ idx_o) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
-  if (f >= n || !keep[f]) return;
+  if (f >= n || (keep && !keep[f])) return;
   const int p = pos[f];
   int4 id = idx[f];
   id.x -= knot_shift; id.y -= gyro_shift; id.z -= accel_shift;

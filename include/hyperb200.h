@@ -83,7 +83,10 @@ int hb200_set_options(hb200_ctx* ctx, double huber_pixel, double imu_loss_scale,
  * All variants coincide on the calibration every reference fixture uses (I_g = I_a = I, S_g = X_a = 0, R_bs = I). */
 int hb200_set_reference_quirks(hb200_ctx* ctx, int quirks);
 
-/* ---- factor lists: replace problem_.AddResidualBlock (reference optimizer.cpp:212-232,253-274) */
+/* ---- factor lists: replace problem_.AddResidualBlock (reference optimizer.cpp:212-232,253-274).  The lists live on
+ * the device only.  Each setter writes its family there in the given (user) order, replacing that family whatever
+ * appends or slides did to it, keeps the other families as they stand and unbinds the window; the copy-out calls and
+ * hb200_get_index_maps number each family's factors in user order. */
 int hb200_set_pixel_factors(hb200_ctx* ctx, int n, const double* stamp, const int* camera, const int* landmark, const double* pixel);
 int hb200_set_inertial_factors(hb200_ctx* ctx, int n, const double* stamp, const double* measurement /* [n][6] gyro|accel */);
 /* VisualBearingObservation -> AngularMetric residual behind HuberLoss(1.6e-3) (reference
@@ -98,7 +101,9 @@ int hb200_set_pose_sensors(hb200_ctx* ctx, int num_sensors, const double* T_bs /
 int hb200_set_manifold_factors(hb200_ctx* ctx, int n, const double* stamp, const int* sensor, const double* pose /* [n][7] */);
 /* ExteroceptiveCost::update() for every factor (reference exteroceptive.cpp:25-99): resolves the
  * knot base index of each stamp and the segment / landmark incidence lists.  num_invalid receives
- * the number of factors whose stamp or indices fall outside the window (they are an error). */
+ * the number of factors whose stamp or indices fall outside the window (they are an error).  The lists are
+ * bound where they stand and put into bound order on the device by a stable sort: visual factors by knot base, inertial
+ * factors by knot, gyro and accel bias base; manifold factors keep their order. */
 int hb200_bind(hb200_ctx* ctx, int* num_invalid);
 int hb200_get_index_maps(hb200_ctx* ctx, int* pixel_base, int* inertial_base, int* gyro_bias_base, int* accel_bias_base);
 
@@ -107,6 +112,7 @@ int hb200_get_index_maps(hb200_ctx* ctx, int* pixel_base, int* inertial_base, in
  * HBM -- no host re-sort, no re-upload of the factor lists (all four families).  After any of these calls the user
  * order of each family is its bound order on the device: the visual list holds pixel and bearing factors together in
  * bound order, and the copy-out calls number the pixel factors 0 .. Np-1 and the bearing factors 0 .. Nb-1 in that order.
+ * A later hb200_bind without a setter in between keeps that numbering and the list order of factors with equal keys.
  *   hb200_append_knots:    `count` state elements appended by the reference's extrapolation -- the new elements AND
  *                          the current last one take the variable of the second to last, stamps continue at the knot
  *                          separation (reference internal/hyper/optimizers/abstract.cpp:126-136).

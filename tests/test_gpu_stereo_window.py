@@ -276,7 +276,7 @@ def test_mixed_visual_list_outputs_and_full_rebind(built):
         assert rel_err(got[key], want[key]) < 1e-8, key
     ctx.build_system()
     S0, b0 = ctx.system()
-    ctx.bind()   # full re-upload of the host mirrors, host sort, derive
+    ctx.bind()   # full re-bind of the device lists where they stand, host sort of the keys, derive
     ctx.evaluate(jacobians=True)
     again = ctx.outputs()
     for key in got:
