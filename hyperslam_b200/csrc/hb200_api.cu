@@ -199,7 +199,10 @@ struct hb200_ctx {
   bool schur_groups = false;
   int nruns = 0, max_rows = 6;
   int imu_splits = 1, imu_splits_mma = 1;
-  int beta = 3, min_beta = 0;   // min_beta: lower bound agreed across ranks (the packed layout must be identical everywhere)
+  // beta = max(own, min_beta, agreed_beta): min_beta is the caller's floor (hb200_set_min_bandwidth), agreed_beta the
+  // largest own value over the ranks at the latest agreement (hb200_bind with NCCL, or the last collective sliding-window
+  // call) -- the packed layout must be identical on every rank, and it shrinks again when the longest track leaves
+  int beta = 3, min_beta = 0, agreed_beta = 0;
   bool band_solver = true, band_smem = true, force_dense = false;
   DevBuf<double> band_ws;
   int band_chunk_cols = 0;       // !band_smem: block columns per shared-memory chunk view (per chain)
@@ -223,6 +226,7 @@ struct hb200_ctx {
   // w_lkeep / w_lpos: landmark keep flags and new positions of the last hb200_slide (slide_L landmarks before it; -1:
   // none yet), kept until the next slide for hb200_slide_landmark_map
   DevBuf<int> w_keep, w_pos, w_lkeep, w_lpos, w_cnt, w_scal;
+  DevBuf<double> w_vote;   // sharded contexts: the agreement payload of a collective sliding-window call (agree_round)
   int slide_L = -1;
   int bg_dropped = 0, ba_dropped = 0;   // leading gyro / accel bias knots the last hb200_slide removed (HB200_SLIDE_DROP_BIAS)
   // hb200_append_stereo_tracks inputs: [stamp | pixel0 | pixel1] and [camera0 | camera1 | landmark | new flag | rank]
@@ -434,7 +438,7 @@ int ensure_dense(hb200_ctx* c) {
 int ensure_system(hb200_ctx* c) {
   const size_t n = c->n;
   // block half-bandwidth of the reduced pose system = longest landmark track in control points (>= k - 1)
-  c->beta = std::max(std::max(c->k - 1, c->max_rows / 6 - 1), c->min_beta);
+  c->beta = std::max(std::max(c->k - 1, c->max_rows / 6 - 1), std::max(c->min_beta, c->agreed_beta));
   c->beta = std::min(c->beta, std::max(c->K - 1, 0));
   c->lay = sys_layout(c->K, c->beta, c->n - 6 * c->K);
   HB_CUDA(c->sys.ensure(static_cast<size_t>(c->lay.total)));
@@ -981,7 +985,8 @@ int enqueue_iteration(hb200_ctx* c) {
 }
 
 // The band layout depends on the longest landmark track of the LOCAL shard; the ranks agree on the maximum
-// (one 4-byte ncclAllReduce(max) at bind / attach time, never on the iteration path).
+// (one 4-byte ncclAllReduce(max) at bind / attach time, never on the iteration path).  The collective sliding-window
+// calls agree on it again through agree_round.
 int sync_layout(hb200_ctx* c) {
   if (!c->nccl || !c->bound) return 0;
   DevBuf<int> d;
@@ -992,13 +997,70 @@ int sync_layout(hb200_ctx* c) {
   HB_CUDA(cudaMemcpyAsync(&v, d.p, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
   c->comm_warm = true;
+  c->agreed_beta = v;
   if (v != c->beta) {
-    c->min_beta = v;
     const int rc = ensure_system(c);
     if (rc) return rc;
     c->kernel_args_changed();
   }
   return 0;
+}
+
+// ---- agreement of the collective sliding-window calls on a sharded context (hb200_window.cuh) ----
+enum { kCallPixel = 1, kCallBearing = 2, kCallStereo = 3, kCallSlide = 4 };
+
+VoteHeader vote_header(const hb200_ctx* c, int kind, int flags = 0, int ub = 0, int ubg = 0, int uba = 0) {
+  return VoteHeader{{1.0, double(c->K), double(c->Kbg), double(c->Kba), double(kind), double(flags), double(ub), double(ubg), double(uba)}};
+}
+
+// One agreement round: this rank's payload (window_vote_kernel), its sum over the ranks through the channel the context
+// already has (NCCL -- peer-memory contexts have the communicator too -- or the callback hook), and the agreed values
+// written to out[kAgreeOut] on the device (window_agree_kernel).  Enqueued on the context's stream: the caller's
+// existing read-back brings the result home, so a round adds no host synchronisation.
+int agree_round(hb200_ctx* c, const VoteHeader& h, const VoteSrc& src, int* out) {
+  const int len = vote_payload_len(c->K, c->Kbg, c->Kba);
+  if (static_cast<size_t>(len) > c->w_vote.cap) HB_CUDA(c->w_vote.ensure(2 * static_cast<size_t>(len)));   // (the window grows by a knot a frame)
+  window_vote_kernel<<<1, 256, 0, c->stream>>>(c->w_vote.p, c->K, c->Kbg, c->Kba, c->k, h, src);
+  HB_LAUNCH(c, "window_vote_kernel");
+  if (c->nccl) {
+    HB_NCCL(g_nccl.AllReduce(c->w_vote.p, c->w_vote.p, static_cast<size_t>(len), /*ncclDouble*/ 8, /*ncclSum*/ 0, c->nccl, c->stream));
+    c->nccl_calls += 1;
+    c->comm_warm = true;
+    prof_mark(c, "ncclAllReduce(window)");
+  } else {
+    const int rc = c->allreduce(c->allreduce_user, c->w_vote.p, len, c->stream);
+    if (rc) return fail(200 + rc, "all-reduce callback failed (%d)", rc);
+    prof_mark(c, "allreduce_callback(window)");
+  }
+  window_agree_kernel<<<1, 256, 0, c->stream>>>(c->w_vote.p, c->K, c->Kbg, c->Kba, h, out);
+  HB_LAUNCH(c, "window_agree_kernel");
+  return 0;
+}
+
+// A context that leaves (or changes) its communicator or hook: the band no longer follows the other ranks' tracks.
+int forget_agreement(hb200_ctx* c) {
+  if (!c->agreed_beta) return 0;
+  c->agreed_beta = 0;
+  if (!c->bound) return 0;
+  HB_CUDA(cudaSetDevice(c->device));
+  HB_CUDA(cudaStreamSynchronize(c->stream));
+  const int rc = ensure_system(c);
+  if (rc) return rc;
+  c->kernel_args_changed();
+  return 0;
+}
+
+// What every rank returns after round A.  own: this rank's status code, its message already in the error string (0:
+// its own checks passed); agreed: the read-back of agree_round's out (ignored on one context).  -2 when the ranks' calls
+// differ, else the window-wide code: 0 lets the call go on, on every rank or on none.
+int window_outcome(hb200_ctx* c, const int* agreed, int own) {
+  if (!c->multi()) return own;
+  if (agreed[kAgreeMismatch])
+    return fail(-2, "sharded window calls out of step: the ranks made different calls or hold different knot / bias knot counts; no rank changed its window");
+  const int code = agreed[kAgreeStatus];
+  if (!code) return 0;
+  if (own) return fail(code, "this rank failed its checks, so no rank changed its window: %s", std::string(g_error).c_str());
+  return fail(code, "another rank failed its checks (code %d), so no rank changed its window", code);
 }
 
 int check_ready(hb200_ctx* c) {
@@ -1431,11 +1493,13 @@ namespace {
 // (landmark CSR, inertial runs, longest track) by counting + scan kernels with one small read-back, then the output
 // buffers and launch shapes of every factor family and the reduced system.  hb200_bind, hb200_append_* and
 // hb200_slide all end here; the ones that change the lists on the device clear the user-index maps and drop the
-// snapshot themselves.
-int derive_window(hb200_ctx* c) {
+// snapshot themselves.  kind > 0: a collective sliding-window call (kCall*), which on a sharded context ends with
+// round B of the agreement -- the ranks' largest band half-width becomes agreed_beta.
+int derive_window(hb200_ctx* c, int kind = 0) {
   const int Nv = c->Nv, Ni = c->Ni, Nm = c->Nm, L = c->L;
-  HB_CUDA(c->w_scal.ensure(8));
-  HB_CUDA(cudaMemsetAsync(c->w_scal.p, 0, 8 * sizeof(int), c->stream));
+  // [L total, longest track rows, -, inertial runs, -, -, -, - | agreement (kAgreeOut)]
+  HB_CUDA(c->w_scal.ensure(8 + kAgreeOut));
+  HB_CUDA(cudaMemsetAsync(c->w_scal.p, 0, (8 + kAgreeOut) * sizeof(int), c->stream));
   HB_CUDA(c->lm_off.ensure(static_cast<size_t>(L) + 2)); HB_CUDA(c->lm_obs.ensure(std::max(Nv, 1)));
   HB_CUDA(c->run_off.ensure(static_cast<size_t>(Ni) + 2));
   HB_CUDA(c->w_cnt.ensure(static_cast<size_t>(std::max(L, 1)) + 1));
@@ -1459,15 +1523,26 @@ int derive_window(hb200_ctx* c) {
     scan_kernel<<<1, 1024, 0, c->stream>>>(c->w_keep.p, Ni, c->w_pos.p, c->w_scal.p + 3);
     HB_LAUNCH(c, "scan_kernel");
   }
-  int h[8];
+  const bool agree = kind && c->multi();
+  if (agree) {
+    int rc = agree_round(c, vote_header(c, kind), VoteSrc{nullptr, {nullptr, nullptr, nullptr}, nullptr, c->w_scal.p + 1}, c->w_scal.p + 8);
+    if (rc) return rc;
+  }
+  int h[8 + kAgreeOut];
   HB_CUDA(cudaMemcpyAsync(h, c->w_scal.p, sizeof(h), cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
+  if (agree) {
+    if (h[8 + kAgreeMismatch]) return fail(-2, "sharded window calls out of step at the band agreement: the ranks made different calls or hold different knot / bias knot counts");
+    c->agreed_beta = h[8 + kAgreeBeta];
+  }
   c->max_rows = std::max(6 * c->k, h[1]);
   c->schur_groups = false;   // the landmark groups are cut by hb200_bind, after this
   c->nruns = Ni ? h[3] : 0;
   if (Ni) { run_fill_kernel<<<(Ni + 255) / 256, 256, 0, c->stream>>>(Ni, c->w_keep.p, c->w_pos.p, c->nruns, c->run_off.p); HB_LAUNCH(c, "run_fill_kernel"); }
   else { const int z = 0; HB_CUDA(cudaMemcpyAsync(c->run_off.p, &z, sizeof(int), cudaMemcpyHostToDevice, c->stream)); }
-  if (2 * 3 * static_cast<size_t>(c->max_rows) * sizeof(double) > 200 * 1024) return fail(-6, "landmark track spans %d control-point dofs; exceeds the Schur kernel's shared-memory tile", c->max_rows);
+  // sharded: the longest track over the ranks (6 (agreed beta + 1) rows), so that every rank refuses the window together
+  const int rows = agree ? std::max(c->max_rows, 6 * (c->agreed_beta + 1)) : c->max_rows;
+  if (2 * 3 * static_cast<size_t>(rows) * sizeof(double) > 200 * 1024) return fail(-6, "landmark track spans %d control-point dofs; exceeds the Schur kernel's shared-memory tile", rows);
   // outputs and launch shapes
   const size_t k = c->k;
   HB_CUDA(c->v_z.ensure(std::max(Nv, 1))); HB_CUDA(c->v_w.ensure(std::max(Nv, 1)));
@@ -1492,7 +1567,7 @@ int derive_window(hb200_ctx* c) {
   HB_CUDA(cudaStreamSynchronize(c->stream));
   c->bound = true;
   c->kernel_args_changed();
-  return sync_layout(c);   // multi-GPU: all ranks adopt the widest band (collective when a communicator is attached)
+  return 0;
 }
 
 // Binds the visual factors at list positions [at, at + n) in place; factors that fail to bind are counted in d_invalid[0].
@@ -1572,7 +1647,11 @@ int hb200_bind(hb200_ctx* c, int* num_invalid) {
     if ((rc = compact_inertial(c, Ni, nullptr, c->w_pos.p, 0, 0, 0, Ni))) return rc;
   }
   HB_CUDA(cudaStreamSynchronize(c->stream));
+  // a new window: the band starts from this rank's own tracks and the caller's floor; with a communicator attached the
+  // ranks agree on the widest one here (collective), through the callback hook the host sets the floor
+  c->agreed_beta = 0;
   if ((rc = derive_window(c))) return rc;
+  if ((rc = sync_layout(c))) return rc;
   {
     // landmark groups for the large-window Schur kernel: observed landmarks ordered by their first knot base, cut so that
     // a group has at most kSchurGroup members and its control-point rows fit one window of RT rows
@@ -2593,29 +2672,39 @@ int check_device_window(hb200_ctx* c) {
 }
 
 // Appends n visual factors of one kind to the tail of the visual list and binds them there: meas = pixel [n][2] (kind 0)
-// or bearing [n][3] (kind 1).  The counts advance only when every new factor binds and the tail keeps the bound order.
+// or bearing [n][3] (kind 1).  The counts advance only when every new factor binds and the tail keeps the bound order --
+// on a sharded context on every rank or on none (round A of the agreement; n = 0 takes part).
 int append_visual(hb200_ctx* c, int n, const double* stamp, const int* camera, const int* landmark, const double* meas, int kind) {
   HB_CUDA(cudaSetDevice(c->device));
   const size_t Nv = c->Nv;
   int rc = grow_visual(c, Nv + n);
   if (rc) return rc;
-  HB_CUDA(c->d_invalid.ensure(2));
-  HB_CUDA(cudaMemsetAsync(c->d_invalid.p, 0, 2 * sizeof(int), c->stream));
-  if ((rc = upload_visual(c, static_cast<int>(Nv), n, stamp, camera, landmark, meas, kind))) return rc;
-  if ((rc = bind_pixel_range(c, static_cast<int>(Nv), n))) return rc;
-  tail_sorted_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(static_cast<int>(Nv), n, c->v_idx.p, c->d_invalid.p + 1);
-  HB_LAUNCH(c, "tail_sorted_kernel");
-  int bad[2] = {0, 0};
-  HB_CUDA(cudaMemcpyAsync(bad, c->d_invalid.p, 2 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+  HB_CUDA(c->d_invalid.ensure(2 + kAgreeOut));   // [bad index, arrival order | agreement]
+  HB_CUDA(cudaMemsetAsync(c->d_invalid.p, 0, (2 + kAgreeOut) * sizeof(int), c->stream));
+  if (n) {
+    if ((rc = upload_visual(c, static_cast<int>(Nv), n, stamp, camera, landmark, meas, kind))) return rc;
+    if ((rc = bind_pixel_range(c, static_cast<int>(Nv), n))) return rc;
+    tail_sorted_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(static_cast<int>(Nv), n, c->v_idx.p, c->d_invalid.p + 1);
+    HB_LAUNCH(c, "tail_sorted_kernel");
+  }
+  const int call = kind ? kCallBearing : kCallPixel;
+  if (c->multi() && (rc = agree_round(c, vote_header(c, call), VoteSrc{c->d_invalid.p, {nullptr, nullptr, nullptr}, nullptr, nullptr}, c->d_invalid.p + 2))) return rc;
+  int bad[2 + kAgreeOut] = {};
+  HB_CUDA(cudaMemcpyAsync(bad, c->d_invalid.p, sizeof(bad), cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
-  if (bad[0]) return fail(2, "%d appended factor(s) reference a stamp outside the spline's valid range or an invalid camera / landmark", bad[0]);
-  if (bad[1]) return fail(3, "appended factors must arrive in stamp order (%d fall before the end of the visual list): use hb200_set_%s_factors + hb200_bind", bad[1],
-                          kind ? "bearing" : "pixel");
+  int own = 0;
+  if (bad[0]) own = fail(2, "%d appended factor(s) reference a stamp outside the spline's valid range or an invalid camera / landmark", bad[0]);
+  else if (bad[1]) own = fail(3, "appended factors must arrive in stamp order (%d fall before the end of the visual list): use hb200_set_%s_factors + hb200_bind", bad[1],
+                              kind ? "bearing" : "pixel");
+  if ((rc = window_outcome(c, bad + 2, own))) return rc;
   c->Nv = static_cast<int>(Nv) + n;
   (kind ? c->Nb : c->Np) += n;
   c->v_perm.clear(); c->i_perm.clear(); c->have_snapshot = false;
-  return derive_window(c);
+  return derive_window(c, call);
 }
+
+// n = 0 (with any pointers) is a valid collective call on a sharded context: the rank has nothing of its own this time
+bool empty_collective(const hb200_ctx* c, int n) { return n == 0 && c->multi(); }
 }  // namespace
 
 int hb200_append_knots(hb200_ctx* c, int count) {
@@ -2639,7 +2728,7 @@ int hb200_append_knots(hb200_ctx* c, int count) {
   if ((rc = ensure_system(c))) return rc;
   HB_CUDA(cudaStreamSynchronize(c->stream));
   c->kernel_args_changed(); c->have_snapshot = false;
-  return sync_layout(c);
+  return 0;   // replicated: every rank appends the same knots, the agreed band half-width stays what it was
 }
 
 }  // extern "C"
@@ -2712,7 +2801,7 @@ int hb200_append_bias_knots(hb200_ctx* c, double stamp, int* gyro_added, int* ac
   if ((rc = ensure_system(c))) return rc;
   HB_CUDA(cudaStreamSynchronize(c->stream));
   c->kernel_args_changed(); c->have_snapshot = false;
-  return sync_layout(c);
+  return 0;   // replicated, as hb200_append_knots
 }
 
 int hb200_bias_knots(hb200_ctx* c, int* num_gyro, int* num_accel, int* gyro_dropped, int* accel_dropped) {
@@ -2741,14 +2830,14 @@ int hb200_append_landmarks(hb200_ctx* c, int n, const double* xyz) {
 int hb200_append_pixel_factors(hb200_ctx* c, int n, const double* stamp, const int* camera, const int* landmark, const double* pixel) {
   int rc = check_device_window(c);
   if (rc) return rc;
-  if (n <= 0 || !stamp || !camera || !landmark || !pixel) return fail(-1, "invalid pixel factors");
+  if (!empty_collective(c, n) && (n <= 0 || !stamp || !camera || !landmark || !pixel)) return fail(-1, "invalid pixel factors");
   return append_visual(c, n, stamp, camera, landmark, pixel, 0);
 }
 
 int hb200_append_bearing_factors(hb200_ctx* c, int n, const double* stamp, const int* camera, const int* landmark, const double* bearing) {
   int rc = check_device_window(c);
   if (rc) return rc;
-  if (n <= 0 || !stamp || !camera || !landmark || !bearing) return fail(-1, "invalid bearing factors");
+  if (!empty_collective(c, n) && (n <= 0 || !stamp || !camera || !landmark || !bearing)) return fail(-1, "invalid bearing factors");
   return append_visual(c, n, stamp, camera, landmark, bearing, 1);
 }
 
@@ -2781,7 +2870,7 @@ int hb200_append_stereo_tracks(hb200_ctx* c, int n, const double* stamp, const i
                                const double* pixel1, const int* landmark, int* landmark_out, int* num_new) {
   int rc = check_device_window(c);
   if (rc) return rc;
-  if (n <= 0 || !stamp || !camera0 || !camera1 || !pixel0 || !pixel1 || !landmark) return fail(-1, "invalid stereo tracks");
+  if (!empty_collective(c, n) && (n <= 0 || !stamp || !camera0 || !camera1 || !pixel0 || !pixel1 || !landmark)) return fail(-1, "invalid stereo tracks");
   if (c->C == 0) return fail(-2, "cameras not set");
   HB_CUDA(cudaSetDevice(c->device));
   const size_t N = n, Nv = c->Nv, L = c->L;
@@ -2798,39 +2887,44 @@ int hb200_append_stereo_tracks(hb200_ctx* c, int n, const double* stamp, const i
   }
   if ((rc = grow_visual(c, Nv + 2 * N))) return rc;
   for (int s2 = 0; s2 < 2; ++s2) HB_CUDA(c->lms[s2].grow(3 * (L + fresh), s2 == 0 ? 3 * L : 0, c->stream));
-  HB_CUDA(c->trk_d.ensure(5 * N)); HB_CUDA(c->trk_i.ensure(5 * N));
-  HB_CUDA(c->d_invalid.ensure(3));
-  HB_CUDA(cudaMemsetAsync(c->d_invalid.p, 0, 3 * sizeof(int), c->stream));
-  HB_CUDA(cudaMemcpyAsync(c->trk_d.p, hd.data(), sizeof(double) * 5 * N, cudaMemcpyHostToDevice, c->stream));
-  HB_CUDA(cudaMemcpyAsync(c->trk_i.p, hi.data(), sizeof(int) * 4 * N, cudaMemcpyHostToDevice, c->stream));
-  const double* d_t = c->trk_d.p;
-  const int* d_lm = c->trk_i.p + 2 * N;
-  int* d_rank = c->trk_i.p + 4 * N;
-  scan_kernel<<<1, 1024, 0, c->stream>>>(c->trk_i.p + 3 * N, n, d_rank, c->d_invalid.p + 2);
-  HB_LAUNCH(c, "scan_kernel");
-  prep_kernel<<<(c->K + 63) / 64, 64, 0, c->stream>>>(c->K, c->knots[0].p, c->tab[0].p, nullptr, 0);   // knot table of the current state
-  HB_LAUNCH(c, "prep_kernel");
-  double2* v_pixel = reinterpret_cast<double2*>(c->v_pixel.p);
-  rc = with_order(c->k, [&](auto K) {
-    stereo_track_kernel<K><<<(n + 127) / 128, 128, 0, c->stream>>>(n, d_t, c->trk_i.p, c->trk_i.p + N, d_t + N, d_t + 3 * N, d_lm, d_rank, c->knots[0].p, c->tab[0].p, c->K,
-                                                                  c->basis, c->cams.p, c->C, static_cast<int>(L), static_cast<int>(Nv), c->v_stamp.p, v_pixel, c->v_z.p,
-                                                                  c->v_idx.p, c->lms[0].p, c->d_invalid.p);
-    return check_launch(c, "stereo_track_kernel");
-  });
-  if (rc) return rc;
-  tail_sorted_kernel<<<(2 * n + 127) / 128, 128, 0, c->stream>>>(static_cast<int>(Nv), 2 * n, c->v_idx.p, c->d_invalid.p + 1);
-  HB_LAUNCH(c, "tail_sorted_kernel");
-  int h[3] = {0, 0, 0};   // bad tracks, order violations, new landmarks
+  HB_CUDA(c->d_invalid.ensure(3 + kAgreeOut));   // [bad tracks, order violations, new landmarks | agreement]
+  HB_CUDA(cudaMemsetAsync(c->d_invalid.p, 0, (3 + kAgreeOut) * sizeof(int), c->stream));
+  if (n) {
+    HB_CUDA(c->trk_d.ensure(5 * N)); HB_CUDA(c->trk_i.ensure(5 * N));
+    HB_CUDA(cudaMemcpyAsync(c->trk_d.p, hd.data(), sizeof(double) * 5 * N, cudaMemcpyHostToDevice, c->stream));
+    HB_CUDA(cudaMemcpyAsync(c->trk_i.p, hi.data(), sizeof(int) * 4 * N, cudaMemcpyHostToDevice, c->stream));
+    const double* d_t = c->trk_d.p;
+    const int* d_lm = c->trk_i.p + 2 * N;
+    int* d_rank = c->trk_i.p + 4 * N;
+    scan_kernel<<<1, 1024, 0, c->stream>>>(c->trk_i.p + 3 * N, n, d_rank, c->d_invalid.p + 2);
+    HB_LAUNCH(c, "scan_kernel");
+    prep_kernel<<<(c->K + 63) / 64, 64, 0, c->stream>>>(c->K, c->knots[0].p, c->tab[0].p, nullptr, 0);   // knot table of the current state
+    HB_LAUNCH(c, "prep_kernel");
+    double2* v_pixel = reinterpret_cast<double2*>(c->v_pixel.p);
+    rc = with_order(c->k, [&](auto K) {
+      stereo_track_kernel<K><<<(n + 127) / 128, 128, 0, c->stream>>>(n, d_t, c->trk_i.p, c->trk_i.p + N, d_t + N, d_t + 3 * N, d_lm, d_rank, c->knots[0].p, c->tab[0].p, c->K,
+                                                                    c->basis, c->cams.p, c->C, static_cast<int>(L), static_cast<int>(Nv), c->v_stamp.p, v_pixel, c->v_z.p,
+                                                                    c->v_idx.p, c->lms[0].p, c->d_invalid.p);
+      return check_launch(c, "stereo_track_kernel");
+    });
+    if (rc) return rc;
+    tail_sorted_kernel<<<(2 * n + 127) / 128, 128, 0, c->stream>>>(static_cast<int>(Nv), 2 * n, c->v_idx.p, c->d_invalid.p + 1);
+    HB_LAUNCH(c, "tail_sorted_kernel");
+  }
+  if (c->multi() && (rc = agree_round(c, vote_header(c, kCallStereo), VoteSrc{c->d_invalid.p, {nullptr, nullptr, nullptr}, nullptr, nullptr}, c->d_invalid.p + 3))) return rc;
+  int h[3 + kAgreeOut] = {};   // bad tracks, order violations, new landmarks | agreement
   HB_CUDA(cudaMemcpyAsync(h, c->d_invalid.p, sizeof(h), cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
-  if (h[0]) return fail(2, "%d stereo track(s) have a stamp outside the spline's valid range, an invalid camera / landmark or a non-finite triangulation", h[0]);
-  if (h[1]) return fail(3, "stereo tracks must arrive in stamp order (%d fall before the end of the visual list)", h[1]);
+  int own = 0;
+  if (h[0]) own = fail(2, "%d stereo track(s) have a stamp outside the spline's valid range, an invalid camera / landmark or a non-finite triangulation", h[0]);
+  else if (h[1]) own = fail(3, "stereo tracks must arrive in stamp order (%d fall before the end of the visual list)", h[1]);
+  if ((rc = window_outcome(c, h + 3, own))) return rc;
   if (landmark_out)
     for (size_t f = 0, r = 0; f < N; ++f) landmark_out[f] = landmark[f] < 0 ? static_cast<int>(L + r++) : landmark[f];
   if (num_new) *num_new = h[2];
   c->Nv = static_cast<int>(Nv + 2 * N); c->Nb += 2 * n; c->L = static_cast<int>(L) + h[2];
   c->v_perm.clear(); c->i_perm.clear(); c->have_snapshot = false;
-  return derive_window(c);
+  return derive_window(c, kCallStereo);
 }
 
 int hb200_append_inertial_factors(hb200_ctx* c, int n, const double* stamp, const double* meas) {
@@ -2870,10 +2964,10 @@ int hb200_slide(hb200_ctx* c, double lower_bound, int flags, hb200_slide_stats* 
   const int last_const = ub - 1;   // knots 0 .. last_const have stamp <= lower bound
   // leading bias knots go only with the inertial factors that reached them: without DROP_INERTIAL nothing is dropped
   const bool drop_bias = (flags & HB200_SLIDE_DROP_BIAS) && (flags & HB200_SLIDE_DROP_INERTIAL) && c->Kbg && c->Kba;
-  HB_CUDA(c->w_scal.ensure(10));
+  HB_CUDA(c->w_scal.ensure(10 + kAgreeOut));
   // [L_new, Nv_new, Ni_new, min base visual, min base inertial, Nm_new, min base manifold, kept bearing factors,
-  //  min gyro bias base, min accel bias base (kept inertial factors)]
-  int init[10] = {0, 0, 0, 0x7fffffff, 0x7fffffff, 0, 0x7fffffff, 0, 0x7fffffff, 0x7fffffff};
+  //  min gyro bias base, min accel bias base (kept inertial factors) | agreement (sharded contexts)]
+  int init[10 + kAgreeOut] = {0, 0, 0, 0x7fffffff, 0x7fffffff, 0, 0x7fffffff, 0, 0x7fffffff, 0x7fffffff};
   HB_CUDA(cudaMemcpyAsync(c->w_scal.p, init, sizeof(init), cudaMemcpyHostToDevice, c->stream));
   HB_CUDA(c->w_last.ensure(std::max(L, 1))); HB_CUDA(c->w_lkeep.ensure(std::max(L, 1) + 1)); HB_CUDA(c->w_lpos.ensure(std::max(L, 1) + 1));
   HB_CUDA(c->w_keep.ensure(std::max(std::max(Nv, Ni), 1))); HB_CUDA(c->w_pos.ensure(std::max(std::max(Nv, Ni), 1)));
@@ -2907,21 +3001,34 @@ int hb200_slide(hb200_ctx* c, double lower_bound, int flags, hb200_slide_stats* 
     scan_kernel<<<1, 1024, 0, c->stream>>>(m_keep, Nm, m_pos, c->w_scal.p + 5);
     HB_LAUNCH(c, "scan_kernel");
   }
-  int h[10];
+  // sharded: round A of the agreement -- the smallest kept knot and bias bases over the ranks, before anything moves
+  auto ub_of = [&](const std::vector<double>& s) { return static_cast<int>(std::upper_bound(s.begin(), s.end(), lower_bound) - s.begin()); };
+  if (c->multi()) {
+    int* w = c->w_scal.p;
+    rc = agree_round(c, vote_header(c, kCallSlide, flags, ub, ub_of(c->h_bg_stamp), ub_of(c->h_ba_stamp)),
+                     VoteSrc{nullptr, {w + 3, w + 4, w + 6}, drop_bias ? w + 8 : nullptr, nullptr}, w + 10);
+    if (rc) return rc;
+  }
+  int h[10 + kAgreeOut];
   HB_CUDA(cudaMemcpyAsync(h, c->w_scal.p, sizeof(h), cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
+  if ((rc = window_outcome(c, h + 10, 0))) {
+    c->slide_L = -1;   // (the keep flags of this attempt replaced the last slide's landmark map)
+    return rc;
+  }
   const int L_new = L ? h[0] : 0, Nv_new = Nv ? h[1] : 0, Ni_new = Ni ? h[2] : 0, Nm_new = Nm ? h[5] : 0, Nb_new = Nv ? h[7] : 0;
+  const int knot_min = c->multi() ? h[10 + kAgreeKnotMin] : std::min(h[6], std::min(h[3], h[4]));
+  const int gyro_min = c->multi() ? h[10 + kAgreeGyroMin] : h[8], accel_min = c->multi() ? h[10 + kAgreeAccelMin] : h[9];
   // state elements in front of `begin` go once no residual touches them (reference optimizer.cpp:331-341)
-  int shift = std::min(std::min(begin, h[6]), std::min(h[3], h[4]));
+  int shift = std::min(begin, knot_min);
   shift = std::max(0, std::min(shift, K - c->k));
   const int K_new = K - shift;
   // the same rule on each bias spline, with the smallest bias base of the kept inertial factors
   auto bias_shift = [&](const std::vector<double>& s, int min_base) {
-    const int ubb = static_cast<int>(std::upper_bound(s.begin(), s.end(), lower_bound) - s.begin());
-    const int sh = std::min(std::max(0, ubb - 1 - (c->kb - 1) / 2), min_base);
+    const int sh = std::min(std::max(0, ub_of(s) - 1 - (c->kb - 1) / 2), min_base);
     return std::max(0, std::min(sh, static_cast<int>(s.size()) - c->kb));
   };
-  const int g_shift = drop_bias ? bias_shift(c->h_bg_stamp, h[8]) : 0, a_shift = drop_bias ? bias_shift(c->h_ba_stamp, h[9]) : 0;
+  const int g_shift = drop_bias ? bias_shift(c->h_bg_stamp, gyro_min) : 0, a_shift = drop_bias ? bias_shift(c->h_ba_stamp, accel_min) : 0;
   const int Kbg_new = c->Kbg - g_shift, Kba_new = c->Kba - a_shift;
   // compaction into the alternate buffers, then swap
   const int n_alt = std::max(std::max(std::max(Nv_new, Ni_new), Nm_new), 1);
@@ -2982,7 +3089,7 @@ int hb200_slide(hb200_ctx* c, double lower_bound, int flags, hb200_slide_stats* 
     stats->knots = K_new; stats->landmarks = L_new; stats->visual_factors = Nv_new; stats->inertial_factors = Ni_new;
   }
   c->v_perm.clear(); c->i_perm.clear(); c->have_snapshot = false;
-  return derive_window(c);
+  return derive_window(c, kCallSlide);
 }
 
 int hb200_window_sizes(hb200_ctx* c, int* knots, int* landmarks, int* visual_factors, int* inertial_factors) {
@@ -3017,9 +3124,10 @@ int hb200_slide_landmark_map(hb200_ctx* c, int n, int* new_index) {
 int hb200_set_allreduce(hb200_ctx* c, hb200_allreduce_fn fn, void* user) {
   if (!c) return fail(-1, "null context");
   if (fn && c->nccl) return fail(-2, "a NCCL communicator is attached; the callback hook is its replacement, not an addition");
+  const bool detach = !fn && c->allreduce;
   c->allreduce = fn; c->allreduce_user = user;
   c->graph_valid = false;
-  return 0;
+  return detach ? forget_agreement(c) : 0;
 }
 
 int hb200_comm_unique_id(char* id) {
@@ -3048,7 +3156,8 @@ int hb200_set_nccl_comm(hb200_ctx* c, void* comm, int nranks, int rank) {
   c->nccl = comm; c->own_nccl = false;
   c->nranks = comm ? nranks : 1; c->rank = comm ? rank : 0;
   c->comm_warm = false; c->graph_valid = false;
-  return sync_layout(c);
+  const int rc = forget_agreement(c);   // a new communicator agrees afresh; none leaves a single context
+  return rc ? rc : sync_layout(c);
 }
 
 int hb200_comm_init_rank(hb200_ctx* c, int nranks, int rank, const char* id) {

@@ -242,4 +242,74 @@ __global__ void tail_sorted_kernel(int n_old, int n_new, const int4* __restrict_
   if (f >= n_old + n_new || f == 0) return;
   if (idx[f].x < idx[f - 1].x) atomicAdd(bad, 1);
 }
+
+// ---- agreement of a sharded window's collective sliding-window calls --------------------------------------------
+// Every rank fills one payload of doubles, the ranks SUM it, and every rank reads the same answer from the sum:
+//   [ header kVoteHeader | its squares kVoteHeader | status 2 | smallest kept knot base K | gyro bias base Kbg |
+//     accel bias base Kba | beta K ]
+// The header holds exact small integers (1, K, Kbg, Kba, call kind, slide flags, ub, ubg, uba).  After the sum, entry x
+// must give sum(x) = n a and sum(x^2) = n a^2 for this rank's own a (n = nranks, the sum of the leading 1): together
+// they say sum((x - a)^2) = 0, so either every rank holds a or every rank sees the mismatch (the sum alone would let
+// 1, 3, 5 pass on the rank holding 3).  Status: one rank-count per window-wide
+// code (bad index: 2, arrival order: 3).  The votes are one-hot: a rank puts a 1 at its own value, so the sum is
+// nonzero exactly at the values some rank voted for -- the first nonzero entry is the minimum, the last the maximum.
+constexpr int kVoteHeader = 9, kVoteStatus = 2, kVoteHead = 2 * kVoteHeader + kVoteStatus;   // (status at 2 kVoteHeader, votes at kVoteHead)
+__host__ __device__ inline int vote_payload_len(int K, int Kbg, int Kba) { return kVoteHead + 2 * K + Kbg + Kba; }
+struct VoteHeader { double v[kVoteHeader]; };
+// What a rank votes with; a null pointer (or a minimum of INT_MAX, a family without factors) casts no vote.
+struct VoteSrc {
+  const int* status;       // [2]: bad-index count, arrival-order count of this rank's validation
+  const int* knot_min[3];  // smallest kept knot base of the visual, inertial and manifold factors
+  const int* bias_min;     // [2]: smallest kept gyro / accel bias base
+  const int* max_rows;     // longest landmark track in control-point rows (csr_sort_kernel); 0: no visual factor
+};
+// agreed values, as window_agree_kernel writes them
+enum { kAgreeStatus = 0, kAgreeMismatch = 1, kAgreeBeta = 2, kAgreeKnotMin = 3, kAgreeGyroMin = 4, kAgreeAccelMin = 5, kAgreeOut = 6 };
+
+// one CTA: zero the payload, then place the header, the status and the one-hot votes
+__global__ void __launch_bounds__(256) window_vote_kernel(double* __restrict__ pay, int K, int Kbg, int Kba, int order, VoteHeader h, VoteSrc src) {
+  const int len = vote_payload_len(K, Kbg, Kba);
+  for (int i = threadIdx.x; i < len; i += blockDim.x) pay[i] = 0.0;
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  for (int i = 0; i < kVoteHeader; ++i) { pay[i] = h.v[i]; pay[kVoteHeader + i] = h.v[i] * h.v[i]; }
+  if (src.status) {
+    pay[2 * kVoteHeader] = src.status[0] ? 1.0 : 0.0;
+    pay[2 * kVoteHeader + 1] = (!src.status[0] && src.status[1]) ? 1.0 : 0.0;
+  }
+  double* votes = pay + kVoteHead;
+  auto vote = [](double* region, int n, int v) { if (v != 0x7fffffff && n > 0) region[min(max(v, 0), n - 1)] = 1.0; };
+  int m = 0x7fffffff;
+  for (int f = 0; f < 3; ++f) if (src.knot_min[f]) m = min(m, *src.knot_min[f]);
+  vote(votes, K, m);
+  if (src.bias_min) { vote(votes + K, Kbg, src.bias_min[0]); vote(votes + K + Kbg, Kba, src.bias_min[1]); }
+  if (src.max_rows && *src.max_rows > 0) vote(votes + K + Kbg + Kba, K, max(order - 1, *src.max_rows / 6 - 1));
+}
+
+// one CTA, on the summed payload: out[kAgree*] (status code 0 / 2 / 3, header mismatch 0 / 1, the largest beta vote (0:
+// none), the smallest knot / gyro / accel base votes (INT_MAX: none))
+__global__ void __launch_bounds__(256) window_agree_kernel(const double* __restrict__ pay, int K, int Kbg, int Kba, VoteHeader h, int* __restrict__ out) {
+  __shared__ int s[kAgreeOut];
+  const int t = threadIdx.x;
+  if (t == 0) {
+    s[kAgreeStatus] = pay[2 * kVoteHeader] > 0.0 ? 2 : (pay[2 * kVoteHeader + 1] > 0.0 ? 3 : 0);
+    int bad = 0;
+    for (int i = 0; i < kVoteHeader; ++i) bad |= (pay[i] != pay[0] * h.v[i]) | (pay[kVoteHeader + i] != pay[0] * (h.v[i] * h.v[i]));
+    s[kAgreeMismatch] = bad;
+    s[kAgreeBeta] = 0;
+    s[kAgreeKnotMin] = s[kAgreeGyroMin] = s[kAgreeAccelMin] = 0x7fffffff;
+  }
+  __syncthreads();
+  const double* votes = pay + kVoteHead;
+  const int len = 2 * K + Kbg + Kba;
+  for (int i = t; i < len; i += blockDim.x) {
+    if (votes[i] == 0.0) continue;
+    if (i < K) atomicMin(&s[kAgreeKnotMin], i);
+    else if (i < K + Kbg) atomicMin(&s[kAgreeGyroMin], i - K);
+    else if (i < K + Kbg + Kba) atomicMin(&s[kAgreeAccelMin], i - K - Kbg);
+    else atomicMax(&s[kAgreeBeta], i - K - Kbg - Kba);
+  }
+  __syncthreads();
+  if (t < kAgreeOut) out[t] = s[t];
+}
 }  // namespace hb

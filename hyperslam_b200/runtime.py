@@ -266,7 +266,7 @@ class Context:
     def append_pixel_factors(self, stamp, cam, lm, pixel):
         stamp, pixel = _f64(stamp), _f64(pixel)
         cam, lm = np.ascontiguousarray(cam, dtype=np.int32), np.ascontiguousarray(lm, dtype=np.int32)
-        if stamp.size:
+        if stamp.size or self.sharded:
             self._check(self.lib.hb200_append_pixel_factors(self.h, stamp.size, _d(stamp), _i(cam), _i(lm), _d(pixel)))
             self._refresh_sizes()
 
@@ -279,7 +279,7 @@ class Context:
     def append_bearing_factors(self, stamp, cam, lm, bearing):
         stamp, bearing = _f64(stamp), _f64(bearing)
         cam, lm = np.ascontiguousarray(cam, dtype=np.int32), np.ascontiguousarray(lm, dtype=np.int32)
-        if stamp.size:
+        if stamp.size or self.sharded:
             self._check(self.lib.hb200_append_bearing_factors(self.h, stamp.size, _d(stamp), _i(cam), _i(lm), _d(bearing)))
             self._refresh_sizes()
 
@@ -297,7 +297,7 @@ class Context:
         cam0, cam1 = np.ascontiguousarray(cam0, dtype=np.int32), np.ascontiguousarray(cam1, dtype=np.int32)
         landmark = np.ascontiguousarray(landmark, dtype=np.int32)
         out = np.zeros(stamp.size, dtype=np.int32)
-        if not stamp.size:
+        if not stamp.size and not self.sharded:
             return out, 0
         new = C.c_int(0)
         self._check(self.lib.hb200_append_stereo_tracks(self.h, stamp.size, _d(stamp), _i(cam0), _i(cam1), _d(px0), _d(px1), _i(landmark), _i(out),
@@ -573,6 +573,12 @@ class Context:
         self._check(self.lib.hb200_comm_info(self.h, *[C.byref(x) for x in v], C.byref(pay)))
         return dict(nranks=v[0].value, rank=v[1].value, nccl=bool(v[2].value), peer_mailbox=bool(v[3].value), peer_reduce=(v[3].value == 2),
                     graph=bool(v[4].value), payload_doubles=pay.value)
+
+    @property
+    def sharded(self) -> bool:
+        """A communicator or the all-reduce hook is attached: the visual appends and slide are collective calls, which
+        every rank makes in the same sequence, with n = 0 when it has nothing of its own (include/hyperb200.h)."""
+        return self._cb is not None or self.comm_info()["nccl"]
 
     def connect_torch_distributed(self, dist, peer_mailbox=True, log=lambda m: None):
         """Plumbing only: ships the NCCL unique id and the mailbox handles over an initialised torch.distributed

@@ -156,7 +156,11 @@ int hb200_get_index_maps(hb200_ctx* ctx, int* pixel_base, int* inertial_base, in
  *                          from each (a caller drops as many leading elements from its own copy); any may be NULL.
  *   hb200_slide_landmark_map: old -> new landmark index across the last hb200_slide (-1: dropped); n = number of
  *                          landmarks before that slide.  With landmark_out it keeps a caller's id -> slot map.
- *   hb200_factor_counts:   factor counts per family, indexed by HB200_PIXEL / _INERTIAL / _BEARING / _MANIFOLD. */
+ *   hb200_factor_counts:   factor counts per family, indexed by HB200_PIXEL / _INERTIAL / _BEARING / _MANIFOLD.
+ * On a sharded context (a communicator or the all-reduce hook attached) these calls fall into three classes, see the
+ * SHARDING CONTRACT below: hb200_append_pixel_factors / _bearing_factors / _stereo_tracks and hb200_slide are
+ * collective (n = 0 accepted), hb200_append_knots / hb200_append_bias_knots replicated, hb200_append_landmarks /
+ * _inertial_factors / _manifold_factors rank-local. */
 typedef struct hb200_slide_stats {
   int knots_dropped, knots_constant, landmarks_dropped, visual_factors_dropped, inertial_factors_dropped;
   int knots, landmarks, visual_factors, inertial_factors;   /* sizes after the call */
@@ -341,6 +345,35 @@ int hb200_ingest_stereo(hb200_ctx* ctx, int n, const double* stamp, const int* c
  *     A rank that fails a call for a reason of its own (an invalid argument, a stale build) breaks the contract as
  *     in hb200_iterate; the peer reduction's timeout and the callback's error return keep the others from waiting
  *     forever.
+ *   - a sharded window slides.  The sliding-window calls come in three classes:
+ *       collective  hb200_append_pixel_factors, _bearing_factors, _stereo_tracks, hb200_slide: every rank makes the
+ *                   same sequence of these calls, each with its own shard's data (n = 0, with any pointers, when it
+ *                   has nothing of its own).  Each ends with agreement rounds on one small payload of doubles that a
+ *                   SUM over the ranks answers, through the context's channel (ncclAllReduce, or the hook): round A
+ *                   before anything moves (the header -- K, Kbg, Kba, call kind, slide flags, knots and bias knots at
+ *                   or before the lower bound --, every rank's validation status and, for hb200_slide, the smallest
+ *                   kept knot and bias bases), round B after the incidence lists (the band half-width).  Ranks whose
+ *                   calls differ all return -2 and change nothing (the header and its squares are summed, so a
+ *                   difference is seen on every rank); when any rank's own checks fail, every rank
+ *                   returns the same window-wide code (2 before 3) and changes nothing (the error string tells this
+ *                   rank's failure from another's).  The knot and bias shifts are the whole window's; slide stats
+ *                   knots* are identical on every rank, landmark and factor counts and hb200_slide_landmark_map are
+ *                   rank-local.  A slide refused with -2 leaves no landmark map (-2 from hb200_slide_landmark_map).
+ *                   The payload has 20 + 2K + Kbg + Kba doubles: ranks whose K, Kbg or Kba already differ (replicated
+ *                   calls out of step) reduce payloads of different lengths, which the hook can see but NCCL does not
+ *                   check -- the header catches differing calls, not replicated state that already diverged.  A track
+ *                   too long for the Schur tile (-6) is refused on every rank, after the call has taken effect, as
+ *                   on one context.  Detaching the hook or the communicator drops the agreed half-width.
+ *       replicated  hb200_append_knots, hb200_append_bias_knots: every rank calls with the same arguments; no
+ *                   communication, the result follows from replicated state.
+ *       rank-local  hb200_append_landmarks, _inertial_factors, _manifold_factors: no collective call -- they change
+ *                   neither the band nor replicated state.
+ *     Routing is the caller's: tracks of a known landmark go to its owner, a new landmark's owner is the caller's
+ *     choice, inertial and pose factors may go to any rank.  Owners never change (no landmark moves between ranks).
+ *     beta = max(own, the hb200_set_min_bandwidth floor, the agreed value of the latest agreement): hb200_bind with a
+ *     communicator takes the maximum over the ranks as the agreed value (collective); through the hook hb200_bind
+ *     agrees on nothing and the host sets the floor.  So a sharded band narrows again, as one context's does, when
+ *     the longest track leaves the window -- down to the floor.
  *
  * Reduced buffer (what is summed): the band-only packed system, hb200_system_device_ptr(), in doubles
  *   [ P K*h*6 | A m*6K | C m*m | b n | diagH n | g n | scal 8 ],  h = 6 + 6*beta, m = n - 6K
@@ -362,13 +395,15 @@ int hb200_peer_disconnect(hb200_ctx* ctx);
 int hb200_comm_info(hb200_ctx* ctx, int* nranks, int* rank, int* nccl, int* peer_mailbox, int* graph, long long* payload_doubles);
 /* Block half-bandwidth beta of the packed layout.  It follows from the longest landmark track of the local factor
  * shard; with a communicator attached hb200_bind / hb200_set_nccl_comm agree on the maximum over the ranks
- * themselves (collective).  Hosts using the callback hook below must do that: read it after hb200_bind, take the
- * maximum over ranks, set it as the lower bound everywhere. */
+ * themselves (collective), and the collective sliding-window calls agree on it again.  Hosts using the callback hook
+ * below must do that after hb200_bind: read it, take the maximum over ranks, set it as the lower bound everywhere
+ * (a floor the band then never goes below; hb200_set_min_bandwidth(0) after the first collective call lifts it). */
 int hb200_get_bandwidth(hb200_ctx* ctx, int* beta);
 int hb200_set_min_bandwidth(hb200_ctx* ctx, int beta);
 /* Escape hatch for hosts without NCCL: the caller sums `count_doubles` doubles at `device_buffer` across ranks
  * on `stream` (called twice per iteration: packed system, then 8 scalars; once per hb200_build_system and
- * hb200_build_covariance: packed system).  Disables CUDA-graph capture. */
+ * hb200_build_covariance: packed system; once per agreement round of a collective sliding-window call -- two per
+ * call, one when a rank's checks failed or the calls differ).  Disables CUDA-graph capture. */
 typedef int (*hb200_allreduce_fn)(void* user, void* device_buffer, long long count_doubles, void* stream);
 int hb200_set_allreduce(hb200_ctx* ctx, hb200_allreduce_fn fn, void* user);
 void* hb200_system_device_ptr(hb200_ctx* ctx, long long* count_doubles);
