@@ -121,19 +121,41 @@ inline void quat_exp(const double* d, double* q) {
   q[0] = s * d[0]; q[1] = s * d[1]; q[2] = s * d[2]; q[3] = c;
 }
 
-// Rodrigues coefficients: a = sin(t)/t, b = (1-cos t)/t^2, c = (t - sin t)/t^3.
+// (t - sin t)/t^3 = sum_n (-1)^n t^2n / (2n+3)!, n = 0..9: below t^2 = 2.5 the closed form cancels by more than
+// 6/t^2 ulps, and the truncated tail stays under 1e-17 relative.
+inline double so3_c_series(double t2) {
+  static const double k[10] = {1.0 / 6.0, -1.0 / 120.0, 1.0 / 5040.0, -1.0 / 362880.0, 1.0 / 39916800.0, -1.0 / 6227020800.0,
+                               1.0 / 1307674368000.0, -1.0 / 355687428096000.0, 1.0 / 121645100408832000.0,
+                               -1.0 / 51090942171709440000.0};
+  double c = k[9];
+  for (int n = 8; n >= 0; --n) c = c * t2 + k[n];
+  return c;
+}
+// 1/t^2 - (1 + cos t)/(2 t sin t) = sum_n |B_2n+2| t^2n / (2n+2)!, n = 0..16: below t^2 = 4 the closed form cancels by
+// more than 24/t^2 ulps, and the truncated tail stays under 1e-17 relative.
+inline double so3_e_series(double t2) {
+  static const double k[17] = {1.0 / 12.0, 1.0 / 720.0, 3.306878306878307e-05, 8.267195767195768e-07, 2.08767569878681e-08,
+                               5.284190138687493e-10, 1.3382536530684679e-11, 3.3896802963225827e-13, 8.586062056277845e-15,
+                               2.174868698558062e-16, 5.5090028283602295e-18, 1.3954464685812522e-19, 3.534707039629467e-21,
+                               8.953517427037546e-23, 2.267952452337683e-24, 5.744790668872202e-26, 1.455172475614865e-27};
+  double e = k[16];
+  for (int n = 15; n >= 0; --n) e = e * t2 + k[n];
+  return e;
+}
+// Rodrigues coefficients: a = sin(t)/t, b = (1-cos t)/t^2, c = (t - sin t)/t^3.  a and b come from the half angle
+// (1 - cos t = 2 sin^2(t/2) does not cancel); c takes its series wherever t - sin t would cancel.
 inline void so3_coeffs(double t2, double* a, double* b, double* c) {
   if (t2 < 1e-8) {
     *a = 1.0 - t2 / 6.0 + t2 * t2 / 120.0;
     *b = 0.5 - t2 / 24.0 + t2 * t2 / 720.0;
-    *c = 1.0 / 6.0 - t2 / 120.0 + t2 * t2 / 5040.0;
   } else {
     const double t = std::sqrt(t2);
-    const double s = std::sin(t), co = std::cos(t);
-    *a = s / t;
-    *b = (1.0 - co) / t2;
-    *c = (t - s) / (t2 * t);
+    const double sh = std::sin(0.5 * t), ch = std::cos(0.5 * t);
+    const double h = sh / t;
+    *a = 2.0 * h * ch;
+    *b = 2.0 * h * h;
   }
+  *c = (t2 < 2.5) ? so3_c_series(t2) : (1.0 - *a) / t2;
 }
 // R = Exp(w) = I + a w^ + b w^^2
 inline void so3_exp(const double* w, double* R) {
@@ -157,11 +179,11 @@ inline void so3_Jr(const double* w, double* J) {
 inline void so3_Jr_inv(const double* w, double* J) {
   const double t2 = v3_dot(w, w);
   double e;
-  if (t2 < 1e-6) {
-    e = 1.0 / 12.0 + t2 / 720.0 + t2 * t2 / 30240.0;
+  if (t2 < 4.0) {
+    e = so3_e_series(t2);
   } else {
     const double t = std::sqrt(t2);
-    e = 1.0 / t2 - (1.0 + std::cos(t)) / (2.0 * t * std::sin(t));
+    e = (1.0 - 0.5 * t * std::cos(0.5 * t) / std::sin(0.5 * t)) / t2;   // (1 + cos t)/sin t = cot(t/2)
   }
   double W[9], W2[9];
   hat(w, W); m3_mul(W, W, W2);

@@ -7,9 +7,12 @@ Independent of both the C oracle and the CUDA kernels:
   * body rates come from finite differences of R(t) in time (omega^ = R^T Rdot,
     alpha^ = R^T Rddot - omega^ omega^), NOT from the Sommer recursion the oracle/kernels use;
   * Jacobians come from central differences of the residual along the manifold retractions
-    (R <- Exp(theta) R, p <- p + rho, Ceres SphereManifold Plus for gravity), h = 1e-20.
-Run:  python tests/golden/make_golden.py      (takes ~1-2 minutes)
+    (R <- Exp(theta) R, p <- p + rho, Ceres SphereManifold Plus for gravity), h = 1e-20;
+  * the edge windows (k*_spline_edges) also carry hb200_interpolate answers: pose, body velocity and body
+    acceleration from the same time differences.
+Run:  python tests/golden/make_golden.py      (takes ~1 minute)
 """
+import dataclasses
 import json
 import os
 import sys
@@ -89,15 +92,17 @@ def basis(k, u):
     return lam
 
 
-def segment(stamps, k, t):
-    j = max(i for i in range(len(stamps)) if stamps[i] <= t)
+def segment(stamps, k, t, pin=None):
+    """Base knot and u of t in the segment holding `pin` (default t): time differences stay on the segment of the
+    stamp they differentiate at, as the kernels do, even where t +- h crosses a knot."""
+    j = max(i for i in range(len(stamps)) if stamps[i] <= (t if pin is None else pin))
     return j - (k - 1) // 2, (t - stamps[j]) / (stamps[j + 1] - stamps[j])
 
 
-def pose(knots, k, t):
-    """R(t), p(t) of the split cumulative spline; knots: list of [q(4) p(3) stamp]."""
+def pose_q(knots, k, t, pin=None):
+    """q(t) [x y z w], p(t) of the split cumulative spline; knots: list of [q(4) p(3) stamp]."""
     stamps = [kn[7] for kn in knots]
-    base, u = segment(stamps, k, t)
+    base, u = segment(stamps, k, t, pin)
     lam = basis(k, u)
     q = list(knots[base][:4])
     p = mp.matrix(knots[base][4:7])
@@ -106,6 +111,12 @@ def pose(knots, k, t):
         d = quat_log(quat_mul([-qa[0], -qa[1], -qa[2], qa[3]], qb))
         q = quat_mul(q, quat_exp([lam[j] * c for c in d]))
         p = p + lam[j] * (mp.matrix(knots[base + j][4:7]) - mp.matrix(knots[base + j - 1][4:7]))
+    return q, p
+
+
+def pose(knots, k, t, pin=None):
+    """R(t), p(t) of the split cumulative spline."""
+    q, p = pose_q(knots, k, t, pin)
     return quat_to_rot(q), p
 
 
@@ -171,8 +182,8 @@ def imu_matrix(c):
 def inertial_residual(st, f):
     t = f["stamp"]
     R0, p0 = pose(st["knots"], st["k"], t)
-    Rp, pp = pose(st["knots"], st["k"], t + H_T)
-    Rm, pm = pose(st["knots"], st["k"], t - H_T)
+    Rp, pp = pose(st["knots"], st["k"], t + H_T, pin=t)
+    Rm, pm = pose(st["knots"], st["k"], t - H_T, pin=t)
     Rd = (Rp - Rm) / (2 * H_T)
     Rdd = (Rp - 2 * R0 + Rm) / H_T ** 2
     pdd = (pp - 2 * p0 + pm) / H_T ** 2
@@ -252,84 +263,222 @@ def numdiff(fn, st, f, kind, index, comp):
 def to_mp_state(w):
     f = lambda a: [[mp.mpf(float(x)) for x in row] for row in np.asarray(a)]
     return dict(k=w.order, kb=w.bias_order, knots=f(w.knots), cams=f(w.cameras), imu=[mp.mpf(float(x)) for x in w.imu],
-                landmarks=f(w.landmarks), bg=f(w.gyro_bias), ba=f(w.accel_bias), gravity=[mp.mpf(float(x)) for x in w.gravity])
+                landmarks=f(w.landmarks), bg=f(w.gyro_bias), ba=f(w.accel_bias), gravity=[mp.mpf(float(x)) for x in w.gravity],
+                pose_sensors=f(w.pose_sensors))
 
 
 def make_case(name, n_pix=3, n_imu=3, **kw):
     w = synthetic.make_window(**kw)
     st = to_mp_state(w)
-    k, kb = w.order, w.bias_order
-    stamps = [kn[7] for kn in st["knots"]]
-    bst = [b[3] for b in st["bg"]]
     rng = np.random.default_rng(7)
     pix_idx = sorted(rng.choice(w.v_stamp.size, n_pix, replace=False).tolist()) if w.v_stamp.size else []
     imu_idx = sorted(rng.choice(w.i_stamp.size, n_imu, replace=False).tolist())
-    case = dict(name=name, window=dict(order=k, bias_order=kb, knots=w.knots.tolist(), gyro_bias=w.gyro_bias.tolist(), accel_bias=w.accel_bias.tolist(),
-                                       gravity=w.gravity.tolist(), cameras=w.cameras.tolist(), imu=w.imu.tolist(), landmarks=w.landmarks.tolist()),
-                pixel=[], inertial=[], digits=mp.mp.dps)
-    fl = lambda v: [float(x) for x in v]
+    case = dict(name=name, window=window_json(w), pixel=[], inertial=[], digits=mp.mp.dps)
     for f_ in pix_idx:
-        f = dict(stamp=mp.mpf(float(w.v_stamp[f_])), cam=int(w.v_cam[f_]), lm=int(w.v_lm[f_]), pixel=[mp.mpf(float(x)) for x in w.v_pixel[f_]])
-        base, _ = segment(stamps, k, f["stamp"])
-        r = pixel_residual(st, f)
-        Jp = [numdiff(pixel_residual, st, f, "knot", base + m, c) for m in range(k) for c in range(6)]   # columns
-        Jl = [numdiff(pixel_residual, st, f, "landmark", f["lm"], c) for c in range(3)]
-        case["pixel"].append(dict(stamp=float(w.v_stamp[f_]), cam=f["cam"], lm=f["lm"], pixel=w.v_pixel[f_].tolist(), base=base, r=fl(r),
-                                  Jp=[[float(Jp[c][row]) for c in range(6 * k)] for row in range(2)],
-                                  Jl=[[float(Jl[c][row]) for c in range(3)] for row in range(2)]))
-        print(name, "pixel", f_, fl(r))
+        case["pixel"].append(pixel_answer(st, w, f_))
+        print(name, "pixel", f_, case["pixel"][-1]["r"])
     for f_ in imu_idx:
-        f = dict(stamp=mp.mpf(float(w.i_stamp[f_])), meas=[mp.mpf(float(x)) for x in w.i_meas[f_]])
-        base, _ = segment(stamps, k, f["stamp"])
-        gb, _ = segment(bst, kb, f["stamp"])
-        r = inertial_residual(st, f)
-        Jp = [numdiff(inertial_residual, st, f, "knot", base + m, c) for m in range(k) for c in range(6)]
-        wg = [numdiff(inertial_residual, st, f, "bg", gb + m, 0)[0] for m in range(kb)]
-        wa = [numdiff(inertial_residual, st, f, "ba", gb + m, 0)[3] for m in range(kb)]
-        Jg = [numdiff(inertial_residual, st, f, "gravity", 0, c) for c in range(2)]
-        case["inertial"].append(dict(stamp=float(w.i_stamp[f_]), meas=w.i_meas[f_].tolist(), base=base, bias_base=gb, r=fl(r),
-                                     Jp=[[float(Jp[c][row]) for c in range(6 * k)] for row in range(6)], wg=fl(wg), wa=fl(wa),
-                                     Jg=[[float(Jg[c][row]) for c in range(2)] for row in range(6)]))
-        print(name, "inertial", f_, fl(r)[:3])
-    out = os.path.join(os.path.dirname(os.path.abspath(__file__)), f"{name}.json")
-    with open(out, "w") as fh:
-        json.dump(case, fh)
-    print("wrote", out)
+        case["inertial"].append(inertial_answer(st, w, f_))
+        print(name, "inertial", f_, case["inertial"][-1]["r"][:3])
+    write_case(name, case)
 
 
 def make_widened_case(name, n_bearing=3, n_pose=3, **kw):
     """Bearing + pose factors (the two other residual families of reference optimizer.cpp:189-251)."""
     w = synthetic.add_bearing_and_pose_factors(synthetic.make_window(**kw), num_bearing=8, num_pose=8, seed=kw["seed"] + 50)
     st = to_mp_state(w)
-    st["pose_sensors"] = [[mp.mpf(float(x)) for x in row] for row in w.pose_sensors]
-    k = w.order
-    stamps = [kn[7] for kn in st["knots"]]
-    case = dict(name=name, window=dict(order=k, bias_order=w.bias_order, knots=w.knots.tolist(), gyro_bias=w.gyro_bias.tolist(), accel_bias=w.accel_bias.tolist(),
-                                       gravity=w.gravity.tolist(), cameras=w.cameras.tolist(), imu=w.imu.tolist(), landmarks=w.landmarks.tolist(),
-                                       pose_sensors=w.pose_sensors.tolist()),
-                pixel=[], inertial=[], bearing=[], pose=[], digits=mp.mp.dps)
-    fl = lambda v: [float(x) for x in v]
+    case = dict(name=name, window=window_json(w), pixel=[], inertial=[], bearing=[], pose=[], digits=mp.mp.dps)
     for f_ in range(n_bearing):
-        f = dict(stamp=mp.mpf(float(w.b_stamp[f_])), cam=int(w.b_cam[f_]), lm=int(w.b_lm[f_]), bearing=[mp.mpf(float(x)) for x in w.b_bearing[f_]])
-        base, _ = segment(stamps, k, f["stamp"])
-        r = bearing_residual(st, f)
-        Jp = [numdiff(bearing_residual, st, f, "knot", base + m, c) for m in range(k) for c in range(6)]
-        Jl = [numdiff(bearing_residual, st, f, "landmark", f["lm"], c) for c in range(3)]
-        case["bearing"].append(dict(stamp=float(w.b_stamp[f_]), cam=f["cam"], lm=f["lm"], bearing=w.b_bearing[f_].tolist(), base=base, r=fl(r),
-                                    Jp=[float(Jp[c][0]) for c in range(6 * k)], Jl=[float(Jl[c][0]) for c in range(3)]))
-        print(name, "bearing", f_, fl(r))
+        case["bearing"].append(bearing_answer(st, w, f_))
+        print(name, "bearing", f_, case["bearing"][-1]["r"])
     for f_ in range(n_pose):
-        f = dict(stamp=mp.mpf(float(w.m_stamp[f_])), sensor=int(w.m_sensor[f_]), pose=[mp.mpf(float(x)) for x in w.m_pose[f_]])
-        base, _ = segment(stamps, k, f["stamp"])
-        r = pose_residual(st, f)
-        Jp = [numdiff(pose_residual, st, f, "knot", base + m, c) for m in range(k) for c in range(6)]
-        case["pose"].append(dict(stamp=float(w.m_stamp[f_]), sensor=f["sensor"], pose=w.m_pose[f_].tolist(), base=base, r=fl(r),
-                                 Jp=[[float(Jp[c][row]) for c in range(6 * k)] for row in range(6)]))
-        print(name, "pose", f_, fl(r)[:3])
+        case["pose"].append(pose_answer(st, w, f_))
+        print(name, "pose", f_, case["pose"][-1]["r"][:3])
+    write_case(name, case)
+
+
+fl = lambda v: [float(x) for x in v]
+
+
+def pixel_answer(st, w, i):
+    k = st["k"]
+    f = dict(stamp=mp.mpf(float(w.v_stamp[i])), cam=int(w.v_cam[i]), lm=int(w.v_lm[i]), pixel=[mp.mpf(float(x)) for x in w.v_pixel[i]])
+    base, _ = segment([kn[7] for kn in st["knots"]], k, f["stamp"])
+    r = pixel_residual(st, f)
+    Jp = [numdiff(pixel_residual, st, f, "knot", base + m, c) for m in range(k) for c in range(6)]   # columns
+    Jl = [numdiff(pixel_residual, st, f, "landmark", f["lm"], c) for c in range(3)]
+    return dict(stamp=float(w.v_stamp[i]), cam=f["cam"], lm=f["lm"], pixel=w.v_pixel[i].tolist(), base=base, r=fl(r),
+                Jp=[[float(Jp[c][row]) for c in range(6 * k)] for row in range(2)], Jl=[[float(Jl[c][row]) for c in range(3)] for row in range(2)])
+
+
+def inertial_answer(st, w, i):
+    k, kb = st["k"], st["kb"]
+    f = dict(stamp=mp.mpf(float(w.i_stamp[i])), meas=[mp.mpf(float(x)) for x in w.i_meas[i]])
+    base, _ = segment([kn[7] for kn in st["knots"]], k, f["stamp"])
+    gb, _ = segment([b[3] for b in st["bg"]], kb, f["stamp"])
+    r = inertial_residual(st, f)
+    Jp = [numdiff(inertial_residual, st, f, "knot", base + m, c) for m in range(k) for c in range(6)]
+    wg = [numdiff(inertial_residual, st, f, "bg", gb + m, 0)[0] for m in range(kb)]
+    wa = [numdiff(inertial_residual, st, f, "ba", gb + m, 0)[3] for m in range(kb)]
+    Jg = [numdiff(inertial_residual, st, f, "gravity", 0, c) for c in range(2)]
+    return dict(stamp=float(w.i_stamp[i]), meas=w.i_meas[i].tolist(), base=base, bias_base=gb, r=fl(r),
+                Jp=[[float(Jp[c][row]) for c in range(6 * k)] for row in range(6)], wg=fl(wg), wa=fl(wa),
+                Jg=[[float(Jg[c][row]) for c in range(2)] for row in range(6)])
+
+
+def bearing_answer(st, w, i):
+    k = st["k"]
+    f = dict(stamp=mp.mpf(float(w.b_stamp[i])), cam=int(w.b_cam[i]), lm=int(w.b_lm[i]), bearing=[mp.mpf(float(x)) for x in w.b_bearing[i]])
+    base, _ = segment([kn[7] for kn in st["knots"]], k, f["stamp"])
+    r = bearing_residual(st, f)
+    Jp = [numdiff(bearing_residual, st, f, "knot", base + m, c) for m in range(k) for c in range(6)]
+    Jl = [numdiff(bearing_residual, st, f, "landmark", f["lm"], c) for c in range(3)]
+    return dict(stamp=float(w.b_stamp[i]), cam=f["cam"], lm=f["lm"], bearing=w.b_bearing[i].tolist(), base=base, r=fl(r),
+                Jp=[float(Jp[c][0]) for c in range(6 * k)], Jl=[float(Jl[c][0]) for c in range(3)])
+
+
+def pose_answer(st, w, i):
+    k = st["k"]
+    f = dict(stamp=mp.mpf(float(w.m_stamp[i])), sensor=int(w.m_sensor[i]), pose=[mp.mpf(float(x)) for x in w.m_pose[i]])
+    base, _ = segment([kn[7] for kn in st["knots"]], k, f["stamp"])
+    r = pose_residual(st, f)
+    Jp = [numdiff(pose_residual, st, f, "knot", base + m, c) for m in range(k) for c in range(6)]
+    return dict(stamp=float(w.m_stamp[i]), sensor=f["sensor"], pose=w.m_pose[i].tolist(), base=base, r=fl(r),
+                Jp=[[float(Jp[c][row]) for c in range(6 * k)] for row in range(6)])
+
+
+def window_json(w):
+    out = dict(order=w.order, bias_order=w.bias_order, knots=w.knots.tolist(), gyro_bias=w.gyro_bias.tolist(), accel_bias=w.accel_bias.tolist(),
+               gravity=w.gravity.tolist(), cameras=w.cameras.tolist(), imu=w.imu.tolist(), landmarks=w.landmarks.tolist())
+    if w.pose_sensors.size:
+        out["pose_sensors"] = w.pose_sensors.tolist()
+    return out
+
+
+def write_case(name, case):
     out = os.path.join(os.path.dirname(os.path.abspath(__file__)), f"{name}.json")
     with open(out, "w") as fh:
         json.dump(case, fh)
     print("wrote", out)
+
+
+# ---- windows at the spline's numerical edges --------------------------------------------------------
+# The SO(3) coefficient functions take w = d_j (a knot increment) or lambda_j d_j (a blended one).  They switch to series
+# at |w| = 1e-7 (quaternion exp and log) and |w|^2 = 1e-8 (sin t / t, (1 - cos t)/t^2), and their closed forms cancel
+# for small |w| (1 - cos t, t - sin t, 1 - (t/2) cot(t/2)).  The edge window steps its knots by these increments (0 =
+# identical knots), so d_j and lambda_j d_j fall on both sides of 1e-7, 1e-4 and 1e-3; stores every other knot as -q;
+# and puts stamps where lambda_j |d_j| equals each target, at u = 0 and at the last double below a segment end.
+INCREMENTS = [1e-9, 0.0, 5e-8, 1.5e-7, 8e-5, 1.2e-4, 5e-4, 1.5e-3, 1e-2, 0.3, 1.05e-4, 2e-3]
+SWITCH_TARGETS = [1.05e-4, 1.2e-4, 9.5e-5, 1.05e-3, 9.5e-4, 1.05e-7, 9.5e-8]
+
+
+def edge_knots(seed):
+    """Knots 0.125 s apart (a binary fraction: every segment has the same dt, so the time differences see a spline that
+    is C^(k-2) across knots) whose rotations step by INCREMENTS about random axes while the positions drift slowly."""
+    rng = np.random.default_rng(seed)
+    q = synthetic.rot_to_quat(synthetic.so3_exp(rng.normal(0, 1.0, (1, 3))))[0]
+    quats = [q]
+    for inc in INCREMENTS:
+        axis = rng.normal(size=3)
+        if inc:
+            q = np.array(quat_mul(list(q), list(np.append(np.sin(inc / 2) * axis / np.linalg.norm(axis), np.cos(inc / 2)))))
+            q /= np.linalg.norm(q)
+        quats.append(q)
+    kt = np.arange(len(quats)) * 0.125
+    knots = np.zeros((len(quats), 8))
+    knots[:, :4] = quats
+    knots[1::2, :4] *= -1
+    knots[:, 4:7] = 0.2 * np.stack([np.sin(0.45 * kt), np.sin(0.3 * kt + 0.7), 0.5 * np.sin(0.6 * kt + 0.2)], -1)
+    knots[:, 7] = kt
+    return knots
+
+
+def edge_stamps(knots, k):
+    """For each target, the stamp where some lambda_j(u) |d_j| equals it with the largest lambda_j; then u = 0 and the
+    last double below the end of every other valid segment."""
+    Mc, left, K = synthetic.blending_matrix(k), (k - 1) // 2, knots.shape[0]
+    R = synthetic.quat_to_rot(knots[:, :4])
+    inc = [np.linalg.norm(synthetic.so3_log((R[i].T @ R[i + 1])[None])[0]) for i in range(K - 1)]
+    lam = lambda j, u: float(Mc[j] @ (u ** np.arange(k)))
+    segs = range(left, K - k + left + 1)
+    out = []
+    for target in SWITCH_TARGETS:
+        best = (0.0, None)
+        for s in segs:
+            for j in range(1, k):
+                d = inc[s - left + j - 1]
+                if d == 0 or not lam(j, 0.0) <= target / d < lam(j, 1.0):
+                    continue
+                lo, hi = 0.0, 1.0
+                for _ in range(80):
+                    lo, hi = (0.5 * (lo + hi), hi) if lam(j, 0.5 * (lo + hi)) * d < target else (lo, 0.5 * (lo + hi))
+                best = max(best, (lam(j, lo), knots[s, 7] + lo * (knots[s + 1, 7] - knots[s, 7])), key=lambda b: b[0])
+        if best[1] is not None:
+            out.append(best[1])
+    for s in list(segs)[::2]:
+        out += [knots[s, 7], float(np.nextafter(knots[s + 1, 7], -np.inf))]
+    return out
+
+
+def interpolate_answer(st, t):
+    """hb200_interpolate's outputs at t: pose [q | p], body velocity [omega | R^T p'] and acceleration [alpha | R^T p'']
+    from time differences of the value formula."""
+    q, p0 = pose_q(st["knots"], st["k"], t)
+    R0 = quat_to_rot(q)
+    Rp, pp = pose(st["knots"], st["k"], t + H_T, pin=t)
+    Rm, pm = pose(st["knots"], st["k"], t - H_T, pin=t)
+    w = vee(R0.T * (Rp - Rm) / (2 * H_T))
+    al = vee(R0.T * (Rp - 2 * R0 + Rm) / H_T ** 2 - hat(w) * hat(w))
+    v = R0.T * ((pp - pm) / (2 * H_T))
+    a = R0.T * ((pp - 2 * p0 + pm) / H_T ** 2)
+    return dict(stamp=float(t), pose=fl(q) + fl(p0), vel=fl(w) + fl(v), acc=fl(al) + fl(a))
+
+
+def make_edge_case(name, order, seed, n_pix=5, n_bearing=2, n_pose=2, n_imu=2):
+    """Pixel, bearing, pose and inertial factors (stamps taken from edge_stamps, switch stamps first) and interpolation
+    answers at every edge stamp.  Each visual factor observes its own landmark, placed in front of its camera;
+    measurements are the model's prediction plus noise."""
+    rng = np.random.default_rng(seed)
+    k = order
+    knots = edge_knots(seed)
+    base_win = synthetic.make_window(order=k, num_knots=knots.shape[0], num_landmarks=0, num_imu=0, seed=seed, generic_calibration=True)
+    cams = base_win.cameras
+    stamps = edge_stamps(knots, k)
+    v_stamp, b_stamp = np.array(stamps[:n_pix]), np.array(stamps[-n_bearing:])
+    m_stamp, i_stamp = np.array(stamps[:n_pose]), np.array([stamps[0], stamps[-2]][:n_imu])
+    vis_stamp = np.concatenate([v_stamp, b_stamp])
+    vis_cam = (np.arange(vis_stamp.size) % cams.shape[0]).astype(np.int32)
+    R, p, *_ = synthetic.spline_eval(knots, k, vis_stamp)
+    c = cams[vis_cam]
+    px = np.stack([rng.uniform(150, 600, vis_stamp.size), rng.uniform(120, 360, vis_stamp.size)], -1)
+    p_s = np.stack([(px[:, 0] - c[:, 7]) / c[:, 9], (px[:, 1] - c[:, 8]) / c[:, 10], np.ones(vis_stamp.size)], -1)
+    p_s *= rng.uniform(2.0, 8.0, (vis_stamp.size, 1))
+    p_b = (synthetic.quat_to_rot(c[:, :4]) @ p_s[..., None])[..., 0] + c[:, 4:7]
+    landmarks = (R @ p_b[..., None])[..., 0] + p
+    lm = np.arange(vis_stamp.size, dtype=np.int32)
+    v_pixel = synthetic.pixel_model(knots, k, cams, landmarks, v_stamp, vis_cam[:n_pix], lm[:n_pix])[0] + rng.normal(0, 2.0, (n_pix, 2))
+    b = p_s[n_pix:] / np.linalg.norm(p_s[n_pix:], axis=1, keepdims=True) + rng.normal(0, 3e-2, (n_bearing, 3))
+    sensors = np.zeros((2, 7))
+    sensors[:, :4] = synthetic.rot_to_quat(synthetic.so3_exp(rng.normal(0, 0.3, (2, 3))))
+    sensors[:, 4:] = rng.normal(0, 0.1, (2, 3))
+    m_sensor = (np.arange(n_pose) % 2).astype(np.int32)
+    Rm, pm, *_ = synthetic.spline_eval(knots, k, m_stamp)
+    ang = np.array([1.05e-4, 1.05e-3])[np.arange(n_pose) % 2]                # pose residual angles about 1e-4 and 1e-3
+    axis = rng.normal(size=(n_pose, 3))
+    R_ws = synthetic.so3_exp(ang[:, None] * axis / np.linalg.norm(axis, axis=1, keepdims=True)) @ Rm @ synthetic.quat_to_rot(sensors[m_sensor, :4])
+    p_ws = pm + (Rm @ sensors[m_sensor, 4:, None])[..., 0] + rng.normal(0, 5e-3, (n_pose, 3))
+    i_meas = synthetic.inertial_model(knots, k, base_win.imu, base_win.gyro_bias, base_win.accel_bias, base_win.bias_order, base_win.gravity, i_stamp)
+    i_meas += np.concatenate([rng.normal(0, 2e-3, (n_imu, 3)), rng.normal(0, 3e-2, (n_imu, 3))], axis=1)
+    w = dataclasses.replace(base_win, knots=knots, landmarks=landmarks, v_stamp=v_stamp, v_cam=vis_cam[:n_pix], v_lm=lm[:n_pix], v_pixel=v_pixel,
+                            i_stamp=i_stamp, i_meas=i_meas, knot_const=np.zeros(knots.shape[0], dtype=np.uint8),
+                            b_stamp=b_stamp, b_cam=vis_cam[n_pix:], b_lm=lm[n_pix:], b_bearing=b, pose_sensors=sensors, m_stamp=m_stamp,
+                            m_sensor=m_sensor, m_pose=np.concatenate([synthetic.rot_to_quat(R_ws), p_ws], axis=1))
+    st = to_mp_state(w)
+    case = dict(name=name, window=window_json(w), digits=mp.mp.dps,
+                pixel=[pixel_answer(st, w, i) for i in range(n_pix)], bearing=[bearing_answer(st, w, i) for i in range(n_bearing)],
+                pose=[pose_answer(st, w, i) for i in range(n_pose)], inertial=[inertial_answer(st, w, i) for i in range(n_imu)],
+                interpolate=[interpolate_answer(st, mp.mpf(float(t))) for t in stamps])
+    write_case(name, case)
 
 
 if __name__ == "__main__":
@@ -343,3 +492,5 @@ if __name__ == "__main__":
     make_case("k6_generic_calibration", order=6, num_knots=12, num_landmarks=12, num_imu=20, generic_calibration=True, seed=synthetic.SEED_BASE + 904, n_pix=2, n_imu=2)
     make_widened_case("k4_bearing_pose", order=4, num_knots=10, num_landmarks=12, num_imu=0, seed=synthetic.SEED_BASE + 905)
     make_widened_case("k6_bearing_pose", order=6, num_knots=12, num_landmarks=12, num_imu=0, seed=synthetic.SEED_BASE + 906, n_bearing=2, n_pose=2)
+    make_edge_case("k4_spline_edges", order=4, seed=synthetic.SEED_BASE + 914)
+    make_edge_case("k6_spline_edges", order=6, seed=synthetic.SEED_BASE + 916)

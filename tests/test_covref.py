@@ -139,6 +139,26 @@ def test_pose_jacobian_central_differences(order):
         assert np.abs(num - J).max() < 1e-7, (t, np.abs(num - J).max())
 
 
+def test_so3_jacobians_against_mpmath():
+    """Jr and Jr^-1 of the J(t) reference, entry by entry against 50 digits, for angles from 1e-9 to pi: a few ulps of
+    the matrix (whose largest entry is 1) everywhere, including where 1 - cos t and t - sin t cancel."""
+    mp = pytest.importorskip("mpmath")
+    mp.mp.dps = 50
+    rng = np.random.default_rng(3)
+    worst = 0.0
+    for t in np.concatenate([np.geomspace(1e-9, 3.1, 400), [1e-4, 1.0001e-4, 1e-3, 1.0001e-3, 1e-8, 1e-7, 1.5, 2.0, np.pi]]):
+        axis = rng.normal(size=3)
+        w = t * axis / np.linalg.norm(axis)
+        W = mp.matrix([[0, -w[2], w[1]], [w[2], 0, -w[0]], [-w[1], w[0], 0]])
+        th = mp.sqrt(mp.mpf(w[0]) ** 2 + mp.mpf(w[1]) ** 2 + mp.mpf(w[2]) ** 2)
+        b, c = (1 - mp.cos(th)) / th ** 2, (th - mp.sin(th)) / th ** 3
+        e = 1 / th ** 2 - (1 + mp.cos(th)) / (2 * th * mp.sin(th))
+        for got, ref in ((cr._so3_Jr(w), mp.eye(3) - b * W + c * W * W), (cr._so3_Jr_inv(w), mp.eye(3) + W / 2 + e * W * W)):
+            err = max(abs(mp.mpf(got[i, j]) - ref[i, j]) for i in range(3) for j in range(3))
+            worst = max(worst, float(err) / 2.0 ** -53)
+    assert worst < 4, worst
+
+
 def test_metric_rejects_mutations():
     K, beta, m = 12, 3, 26
     S, *_ = sr.make_system(K, beta, m, seed=11)

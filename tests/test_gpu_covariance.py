@@ -11,7 +11,8 @@ hb200_get_covariance / hb200_interpolate_covariance against tests/covref.py.
 * a build made stale by a change of the window (landmarks, an evaluation, constants) is refused with -2;
 * failures (gauge not fixed, biases without IMU factors, a single-observation landmark) are reported with finite outputs
   and leave the previous results in place; an unobserved landmark gets a zero block;
-* the interpolated pose covariance equals J(t) Sigma J(t)^T of covref within 1e-11 in the correlation metric;
+* the interpolated pose covariance equals J(t) Sigma J(t)^T of covref within 1e-11 in the correlation metric, also where
+  the knot increments straddle the small-angle switches of the SO(3) coefficients;
 * the LM path is untouched: iterate() with a covariance computed in between differs from a plain run by no more than
   twice the spread of three plain runs (the assembly's atomics), hb200_get_system refuses after the covariance build, the iteration's kernel list is
   unchanged.
@@ -261,6 +262,41 @@ def test_e2e_cfg1_shaped(built, record_property, order):
         worst = max(worst, cr.cov_error(cov[i], want))
     record_property("err_interpolated", worst)
     print(f"order {order}: interpolated covariance, correlation error {worst:.3e}")
+    assert worst < 1e-11, worst
+
+
+NEAR_STATIONARY = [1.05e-4, 1.2e-4, 0.0, 1e-9, 5e-8, 2e-7, 1.05e-3, 5e-5, 1.3e-4, 9e-4, 1.1e-4]
+
+
+@pytest.mark.parametrize("order", [4, 6])
+def test_interpolated_covariance_near_stationary(built, record_property, order):
+    """J(t) Sigma J(t)^T where the platform barely turns: knots 10..20 step by the increments above (0 = identical knots),
+    which put lambda_j d_j and d_j on both sides of the small-angle switches of the SO(3) coefficients."""
+    win = e2e_window(order, num_knots=30, num_landmarks=300, num_imu=600, bearing=100, pose=10, seed=40 + order)
+    rng = np.random.default_rng(order)
+    for i, inc in enumerate(NEAR_STATIONARY, start=10):
+        axis = rng.normal(size=3)
+        R = synthetic.quat_to_rot(win.knots[i - 1, None, :4])[0] @ synthetic.so3_exp(inc * axis[None] / np.linalg.norm(axis))[0]
+        q = win.knots[i - 1, :4] if inc == 0 else synthetic.rot_to_quat(R[None])[0]
+        win.knots[i, :4] = q if np.dot(q, win.knots[i - 1, :4]) >= 0 else -q
+    kt = win.knots[:, 7]
+    inside = np.concatenate([kt[10:21], kt[10:21] + 0.3 * (kt[11:22] - kt[10:21]), np.nextafter(kt[11:22], -np.inf)])
+    ctx = runtime.Context(0)
+    try:
+        ctx.load_window(win)
+        ctx.build_covariance()
+        info = ctx.compute_covariance()
+        assert info["status"] == 0, info
+        packed, _, _ = ctx.covariance_packed()
+        beta, knots = ctx.bandwidth(), ctx.state()["knots"]
+        cov, bad = ctx.interpolate_covariance(inside)
+    finally:
+        ctx.close()
+    assert bad == 0
+    K, m = win.knots.shape[0], 3 * (win.gyro_bias.shape[0] + win.accel_bias.shape[0]) + 2
+    got = cr.packed_to_dense(packed, K, beta, m)
+    worst = max(cr.cov_error(cov[i], cr.interpolated(knots, order, t, got)) for i, t in enumerate(inside))
+    record_property("err_interpolated", worst)
     assert worst < 1e-11, worst
 
 
