@@ -280,8 +280,12 @@ struct hb200_ctx {
   Basis cov_basis{}, cov_basis_next{};
   int cov_L = 0, cov_L_next = 0;
   int cov_k_next = 0, cov_Nv_next = 0, cov_max_rows_next = 0;   // shapes the build's landmark outputs were written with
-  DevBuf<double> cov_t, cov_o;   // hb200_interpolate_covariance staging
+  DevBuf<double> cov_t, cov_o;   // hb200_interpolate_covariance / hb200_interpolate_state_covariance staging
   DevBuf<int> cov_bad;
+  // the bias splines of the same linearisation point (knot values and stamps), for hb200_interpolate_state_covariance
+  DevBuf<double> cov_bg, cov_bg_next, cov_ba, cov_ba_next;
+  int cov_Kbg = 0, cov_Kbg_next = 0, cov_Kba = 0, cov_Kba_next = 0;
+  Basis cov_bias_basis{}, cov_bias_basis_next{};
 
   hb200_allreduce_fn allreduce = nullptr;
   void* allreduce_user = nullptr;
@@ -2068,6 +2072,10 @@ int hb200_build_covariance(hb200_ctx* c) {
   HB_CUDA(c->cov_tab_next.ensure(static_cast<size_t>(kTabStride) * c->K));
   HB_CUDA(cudaMemcpyAsync(c->cov_knots_next.p, c->knots[0].p, sizeof(double) * 8 * c->K, cudaMemcpyDeviceToDevice, c->stream));
   HB_CUDA(cudaMemcpyAsync(c->cov_tab_next.p, c->tab[0].p, sizeof(double) * kTabStride * c->K, cudaMemcpyDeviceToDevice, c->stream));
+  HB_CUDA(c->cov_bg_next.ensure(4 * static_cast<size_t>(c->Kbg)));
+  HB_CUDA(c->cov_ba_next.ensure(4 * static_cast<size_t>(c->Kba)));
+  if (c->Kbg) HB_CUDA(cudaMemcpyAsync(c->cov_bg_next.p, c->bg[0].p, sizeof(double) * 4 * c->Kbg, cudaMemcpyDeviceToDevice, c->stream));
+  if (c->Kba) HB_CUDA(cudaMemcpyAsync(c->cov_ba_next.p, c->ba[0].p, sizeof(double) * 4 * c->Kba, cudaMemcpyDeviceToDevice, c->stream));
   int counts[2] = {0, c->L};
   if (c->Nv && c->L) {
     HB_CUDA(c->cov_counts.ensure(2));
@@ -2097,6 +2105,7 @@ int hb200_build_covariance(hb200_ctx* c) {
   c->cov_unobserved = counts[1];
   c->cov_lay_next = c->lay; c->cov_basis_next = c->basis; c->cov_L_next = c->L;
   c->cov_k_next = c->k; c->cov_Nv_next = c->Nv; c->cov_max_rows_next = c->max_rows;
+  c->cov_Kbg_next = c->Kbg; c->cov_Kba_next = c->Kba; c->cov_bias_basis_next = c->bias_basis;
   // the factor outputs are those of an evaluation at the current state; the packed buffer is not what hb200_solve expects
   c->outputs_changed();
   c->evaluated_J = true; c->cov_built = true;
@@ -2164,8 +2173,14 @@ int hb200_compute_covariance(hb200_ctx* c, hb200_covariance_info* info) {
   HB_CUDA(c->cov_tab.ensure(static_cast<size_t>(kTabStride) * lay.K));
   HB_CUDA(cudaMemcpyAsync(c->cov_knots.p, c->cov_knots_next.p, sizeof(double) * 8 * lay.K, cudaMemcpyDeviceToDevice, c->stream));
   HB_CUDA(cudaMemcpyAsync(c->cov_tab.p, c->cov_tab_next.p, sizeof(double) * kTabStride * lay.K, cudaMemcpyDeviceToDevice, c->stream));
+  const int Kbg = c->cov_Kbg_next, Kba = c->cov_Kba_next;
+  HB_CUDA(c->cov_bg.ensure(4 * static_cast<size_t>(Kbg)));
+  HB_CUDA(c->cov_ba.ensure(4 * static_cast<size_t>(Kba)));
+  if (Kbg) HB_CUDA(cudaMemcpyAsync(c->cov_bg.p, c->cov_bg_next.p, sizeof(double) * 4 * Kbg, cudaMemcpyDeviceToDevice, c->stream));
+  if (Kba) HB_CUDA(cudaMemcpyAsync(c->cov_ba.p, c->cov_ba_next.p, sizeof(double) * 4 * Kba, cudaMemcpyDeviceToDevice, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
   c->cov_lay = lay; c->cov_basis = c->cov_basis_next; c->cov_L = c->cov_L_next;
+  c->cov_Kbg = Kbg; c->cov_Kba = Kba; c->cov_bias_basis = c->cov_bias_basis_next;
   c->cov_valid = true;
   cov_info(c, info);
   return 0;
@@ -2205,6 +2220,36 @@ int hb200_interpolate_covariance(hb200_ctx* c, int n, const double* stamps, doub
   std::vector<int> bad(n);
   HB_CUDA(cudaMemcpyAsync(cov, d_o.p, sizeof(double) * 36 * n, cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaMemcpyAsync(bad.data(), d_bad.p, sizeof(int) * n, cudaMemcpyDeviceToHost, c->stream));
+  HB_CUDA(cudaStreamSynchronize(c->stream));
+  if (num_invalid) *num_invalid = std::accumulate(bad.begin(), bad.end(), 0);
+  if (stamp) c->cov_at = c->launches;
+  return 0;
+}
+
+int hb200_interpolate_state_covariance(hb200_ctx* c, int n, const double* stamps, double* cov, int* num_invalid) {
+  int rc = cov_check(c);
+  if (rc) return rc;
+  if (n < 0 || (n > 0 && (!stamps || !cov))) return fail(-1, "invalid argument");
+  if (!c->cov_valid) return fail(-2, "no covariance computed (hb200_compute_covariance has not succeeded)");
+  HB_CUDA(cudaSetDevice(c->device));
+  if (num_invalid) *num_invalid = 0;
+  if (n == 0) return 0;
+  const bool stamp = c->cov_built && c->cov_at == c->launches;   // (reads nothing a compute needs)
+  constexpr size_t D2 = HB200_STATE_COV_DIM * HB200_STATE_COV_DIM;
+  static_assert(HB200_STATE_COV_DIM == kStateDim, "state covariance dimension");
+  HB_CUDA(c->cov_t.ensure(n)); HB_CUDA(c->cov_o.ensure(D2 * n)); HB_CUDA(c->cov_bad.ensure(n));
+  HB_CUDA(cudaMemcpyAsync(c->cov_t.p, stamps, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
+  const SysLayout& lay = c->cov_lay;
+  rc = with_order(c->cov_basis.k, [&](auto K) {
+    cov_state_interpolate_kernel<K><<<(n + kStateWarps - 1) / kStateWarps, kStateWarps * 32, 0, c->stream>>>(
+        n, c->cov_t.p, c->cov_knots.p, c->cov_tab.p, lay.K, c->cov_basis, c->cov_bg.p, c->cov_Kbg, c->cov_ba.p, c->cov_Kba, c->cov_bias_basis,
+        c->cov_packed.p, lay, c->cov_o.p, c->cov_bad.p);
+    return check_launch(c, "cov_state_interpolate_kernel");
+  });
+  if (rc) return rc;
+  std::vector<int> bad(n);
+  HB_CUDA(cudaMemcpyAsync(cov, c->cov_o.p, sizeof(double) * D2 * n, cudaMemcpyDeviceToHost, c->stream));
+  HB_CUDA(cudaMemcpyAsync(bad.data(), c->cov_bad.p, sizeof(int) * n, cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
   if (num_invalid) *num_invalid = std::accumulate(bad.begin(), bad.end(), 0);
   if (stamp) c->cov_at = c->launches;

@@ -5,8 +5,9 @@
 // buffer; the kernels here then produce, from S and the landmark factors of that build:
 //   cov_selinv_kernel     the entries of S^-1 on the block band, the arrow and the corner (selected inversion);
 //   cov_landmark_kernel   the 3 x 3 marginal of every landmark, Sigma_ll = L^-T (I + Y^T Sigma_pp Y) L^-1;
-//   cov_interpolate_kernel the 6 x 6 covariance of the interpolated pose at arbitrary stamps, J(t) Sigma J(t)^T.
-// All three are deterministic: no atomics, every sum in a fixed order.
+//   cov_interpolate_kernel the 6 x 6 covariance of the interpolated pose at arbitrary stamps, J(t) Sigma J(t)^T;
+//   cov_state_interpolate_kernel the 18 x 18 joint covariance of pose, body velocity and IMU biases at arbitrary stamps.
+// All are deterministic: no atomics, every sum in a fixed order.
 #pragma once
 #include "hb200_solve.cuh"
 
@@ -503,6 +504,190 @@ __global__ void cov_interpolate_kernel(int n, const double* __restrict__ stamps,
   }
   for (int i = 0; i < 6; ++i)
     for (int c = 0; c < 6; ++c) o[i * 6 + c] = 0.5 * (S[i * 6 + c] + S[c * 6 + i]);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Joint covariance of the interpolated state x(t) = [theta p | omega v | b_g b_a] (18 rows) at arbitrary stamps, one warp
+// per stamp.  J(t) (18 x NC, NC = 6k + 24) is taken with respect to the tangents [phi | rho] of the stamp's k control
+// points and the 4 knots of each bias spline (columns 6k + 3m + c gyro, 6k + 12 + 3m + c accel); Sigma(t) = J Z J^T with
+// Z the span of the packed Sigma (control-point pairs in the band, pose x bias in the arrow, bias x bias in the corner).
+// Jacobian blocks of control point m, with P_j = R_0 A_1 .. A_j, A_j = Exp(lambda_j d_j), G_j = Jr^-1(d_j) R_j^T:
+//   theta: D_m = M_m - M_{m+1},             M_j = lambda_j P_j Jr(lambda_j d_j) G_j   (cov_interpolate_kernel; M_0 = I)
+//   omega: R^T (Y_m - Y_{m+1}),             Y_j = P_j X_j G_j, X_j = hat(A_j^T w_{j-1}) lambda_j Jr(lambda_j d_j) + lamd_j I
+//          -- inertial_factor's rate rows X -> XG, whose left factor A_{k-1}^T .. A_{j+1}^T is R^T P_j;
+//   v = R^T pdot: hat(v) R^T D_m on phi_m and (lamd_m - lamd_{m+1}) R^T on rho_m;  p: (lambda_m - lambda_{m+1}) I on rho_m;
+//   b_g / b_a: (lb_m - lb_{m+1}) I on knot gb + m / ab + m (the bias basis, as inertial_factor evaluates it).
+// Lane 0 builds J in shared memory (one forward sweep); each lane then forms rows a of T = Z J^T from the packed Sigma
+// and entries of J T; the output is 0.5 (S + S^T).  Sums run in a fixed order, no atomics.  A stamp outside the pose
+// spline's valid span, or outside the span of a bias spline that has knots, gives a zero block and invalid[f] = 1; a
+// spline without knots (Kbg or Kba = 0) gives zero rows and columns.  All inputs are the snapshot of the last compute.
+// ---------------------------------------------------------------------------------------------
+constexpr int kStateDim = 18;
+constexpr int kStateWarps = 2;   // stamps per CTA (static shared memory: 2 x 17.5 KB at k = 6)
+
+template <int K>
+__global__ void __launch_bounds__(kStateWarps * 32) cov_state_interpolate_kernel(
+    int n, const double* __restrict__ stamps, const double* __restrict__ knots, const double* __restrict__ tab, int Kn, Basis B,
+    const double* __restrict__ bg, int Kbg, const double* __restrict__ ba, int Kba, Basis BB, const double* __restrict__ cov,
+    SysLayout lay, double* __restrict__ out, int* __restrict__ invalid) {
+  constexpr int NC = 6 * K + 24, D = kStateDim, KB = 4;
+  __shared__ double s_J[kStateWarps][D * NC];   // J (row-major), then S
+  __shared__ double s_T[kStateWarps][NC * D];   // T = Z J^T (row a of Z per row)
+  __shared__ int s_dof[kStateWarps][NC];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int f = blockIdx.x * kStateWarps + warp;
+  if (f >= n) return;
+  double* J = s_J[warp];
+  double* T = s_T[warp];
+  int* dof = s_dof[warp];
+  double* o = out + D * D * static_cast<size_t>(f);
+  const double t = stamps[f];
+  const int base = segment_base(knots, 8, 7, Kn, K, t);
+  const int gb = Kbg ? segment_base(bg, 4, 3, Kbg, KB, t) : 0;
+  const int ab = Kba ? segment_base(ba, 4, 3, Kba, KB, t) : 0;
+  if (base < 0 || gb < 0 || ab < 0) {
+    for (int e = lane; e < D * D; e += 32) o[e] = 0.0;
+    if (lane == 0) invalid[f] = 1;
+    return;
+  }
+  if (lane == 0) invalid[f] = 0;
+  for (int e = lane; e < D * NC; e += 32) J[e] = 0.0;
+  for (int c = lane; c < NC; c += 32) {
+    int g;
+    if (c < 6 * K) g = 6 * base + c;
+    else if (c < 6 * K + 12) g = Kbg ? lay.np + 3 * gb + (c - 6 * K) : -1;
+    else g = Kba ? lay.np + 3 * Kbg + 3 * ab + (c - 6 * K - 12) : -1;
+    dof[c] = g;
+  }
+  __syncwarp();
+  if (lane == 0) {
+    constexpr int left = (K - 1) / 2;
+    const double* row0 = tab + static_cast<size_t>(base) * kTabStride;
+    const double t0 = row0[left * kTabStride + 24], t1 = row0[(left + 1) * kTabStride + 24];
+    const double inv_dt = 1.0 / (t1 - t0);
+    double lam[K + 1], lamd[K + 1], lamdd[K + 1];
+    basis_eval<K, true>(B, (t - t0) * inv_dt, inv_dt, lam, lamd, lamdd);
+    auto blk = [&](int r, int c) { return J + r * NC + c; };   // 3 x 3 block at row r, column c
+    auto add3 = [&](double* b, const double* M, double s) {
+      for (int i = 0; i < 3; ++i)
+        for (int c = 0; c < 3; ++c) b[i * NC + c] += s * M[3 * i + c];
+    };
+    for (int i = 0; i < 3; ++i) J[i * NC + i] = 1.0;   // M_0 = I
+    double P[9], w[3] = {0, 0, 0}, pd[3] = {0, 0, 0};
+    for (int i = 0; i < 9; ++i) P[i] = row0[i];
+#pragma unroll 1
+    for (int j = 1; j < K; ++j) {
+      const double* rj = row0 + j * kTabStride;
+      const double d[3] = {rj[12], rj[13], rj[14]};
+      const double lw[3] = {lam[j] * d[0], lam[j] * d[1], lam[j] * d[2]};
+      double A[9], Jr[9], Pn[9], G[9], lj[9], X[9], XG[9], M[9];
+      so3_exp_and_Jr(lw, A, Jr);
+      m3_mul(P, A, Pn);
+      for (int i = 0; i < 9; ++i) { G[i] = rj[15 + i]; lj[i] = lam[j] * Jr[i]; }
+      double aw[3];
+      m3_tvec(A, w, aw);
+      hat_mul(aw, lj, X);
+      for (int i = 0; i < 3; ++i) X[4 * i] += lamd[j];
+      // theta rows: + M_j on phi_j, - M_j on phi_{j-1} (the same roundings as cov_interpolate_kernel's D_m)
+      m3_mul(Jr, G, XG);
+      m3_mul(Pn, XG, M);
+      for (int i = 0; i < 9; ++i) M[i] *= lam[j];
+      add3(blk(0, 6 * j), M, 1.0);
+      add3(blk(0, 6 * (j - 1)), M, -1.0);
+      // omega rows (R^T applied below): + Y_j on phi_j, - Y_j on phi_{j-1}
+      m3_mul(X, G, XG);
+      m3_mul(Pn, XG, M);
+      add3(blk(6, 6 * j), M, 1.0);
+      add3(blk(6, 6 * (j - 1)), M, -1.0);
+      for (int c = 0; c < 3; ++c) {
+        w[c] = aw[c] + lamd[j] * d[c];
+        pd[c] += lamd[j] * (rj[9 + c] - rj[9 + c - kTabStride]);
+      }
+      for (int i = 0; i < 9; ++i) P[i] = Pn[i];
+    }
+    // P = R: omega rows R^T (Y_m - Y_{m+1}); v rows hat(v) R^T D_m and (lamd_m - lamd_{m+1}) R^T; p rows w_m I
+    double v[3], H[9];
+    m3_tvec(P, pd, v);
+    {
+      double Rt[9];
+      for (int i = 0; i < 3; ++i)
+        for (int c = 0; c < 3; ++c) Rt[3 * i + c] = P[3 * c + i];
+      hat_mul(v, Rt, H);
+    }
+#pragma unroll 1
+    for (int m = 0; m < K; ++m) {
+      double Y[9], Dm[9], Z[9];
+      for (int i = 0; i < 3; ++i)
+        for (int c = 0; c < 3; ++c) { Y[3 * i + c] = blk(6, 6 * m)[i * NC + c]; Dm[3 * i + c] = blk(0, 6 * m)[i * NC + c]; }
+      m3_tmul(P, Y, Z);
+      for (int i = 0; i < 3; ++i)
+        for (int c = 0; c < 3; ++c) blk(6, 6 * m)[i * NC + c] = Z[3 * i + c];
+      m3_mul(H, Dm, Z);
+      add3(blk(9, 6 * m), Z, 1.0);
+      const double wd = lamd[m] - lamd[m + 1], wm = lam[m] - lam[m + 1];
+      for (int i = 0; i < 3; ++i) {
+        blk(3, 6 * m + 3)[i * NC + i] = wm;
+        for (int c = 0; c < 3; ++c) blk(9, 6 * m + 3)[i * NC + c] = wd * P[3 * c + i];
+      }
+    }
+    // bias rows
+    constexpr int lb = (KB - 1) / 2;
+    double lbw[KB + 1];
+    for (int s = 0; s < 2; ++s) {
+      const int Kb = s ? Kba : Kbg;
+      if (!Kb) continue;
+      const double* b0 = (s ? ba + 4 * static_cast<size_t>(ab) : bg + 4 * static_cast<size_t>(gb));
+      const double s0 = b0[4 * lb + 3], s1 = b0[4 * (lb + 1) + 3];
+      basis_eval<KB, false>(BB, (t - s0) / (s1 - s0), 0.0, lbw, nullptr, nullptr);
+      for (int m = 0; m < KB; ++m)
+        for (int i = 0; i < 3; ++i) J[(12 + 3 * s + i) * NC + 6 * K + 12 * s + 3 * m + i] = lbw[m] - lbw[m + 1];
+    }
+  }
+  __syncwarp();
+  // T = Z J^T, one row a of Z per lane at a time, its entries read once from the packed Sigma
+  for (int a = lane; a < NC; a += 32) {
+    double acc[D];
+#pragma unroll
+    for (int r = 0; r < D; ++r) acc[r] = 0.0;
+    const int ga = dof[a];
+    if (ga >= 0) {
+#pragma unroll 2
+      for (int b = 0; b < NC; ++b) {
+        const int gbb = dof[b];
+        if (gbb < 0) continue;
+        const double z = cov[sys_index(lay, max(ga, gbb), min(ga, gbb))];
+#pragma unroll
+        for (int r = 0; r < D; ++r) acc[r] += z * J[r * NC + b];
+      }
+    }
+#pragma unroll
+    for (int r = 0; r < D; ++r) T[a * D + r] = acc[r];
+  }
+  __syncwarp();
+  // S = J T, then 0.5 (S + S^T) (S overwrites J once every lane has read it)
+  constexpr int PER = (D * D + 31) / 32;
+  double s[PER];
+#pragma unroll
+  for (int q = 0; q < PER; ++q) {
+    const int e = lane + 32 * q;
+    double v = 0.0;
+    if (e < D * D) {
+      const int r = e / D, c = e - r * D;
+      for (int a = 0; a < NC; ++a) v += J[r * NC + a] * T[a * D + c];
+    }
+    s[q] = v;
+  }
+  __syncwarp();
+#pragma unroll
+  for (int q = 0; q < PER; ++q) {
+    const int e = lane + 32 * q;
+    if (e < D * D) J[e] = s[q];
+  }
+  __syncwarp();
+  for (int e = lane; e < D * D; e += 32) {
+    const int r = e / D, c = e - r * D;
+    o[e] = 0.5 * (J[r * D + c] + J[c * D + r]);
+  }
 }
 
 }  // namespace hb

@@ -45,6 +45,7 @@ class CovarianceInfo(C.Structure):
 
 
 COV_NOT_POSITIVE_DEFINITE, COV_DEGENERATE_LANDMARKS = 40, 41
+STATE_COV_DIM = 18   # HB200_STATE_COV_DIM: [theta p | omega v | b_g b_a]
 
 
 ALLREDUCE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p)
@@ -67,6 +68,7 @@ EXPORTS = [
     "hb200_append_bearing_factors", "hb200_append_manifold_factors", "hb200_append_stereo_tracks", "hb200_slide_landmark_map",
     "hb200_factor_counts", "hb200_build_covariance", "hb200_compute_covariance", "hb200_get_covariance", "hb200_interpolate_covariance",
     "hb200_append_bias_knots", "hb200_bias_knots", "hb200_set_deterministic", "hb200_get_deterministic",
+    "hb200_interpolate_state_covariance",
 ]
 
 _lib = None
@@ -433,6 +435,15 @@ class Context:
         out = np.zeros((stamps.size, 6, 6))
         bad = C.c_int(0)
         self._check(self.lib.hb200_interpolate_covariance(self.h, stamps.size, _d(stamps), _d(out), C.byref(bad)))
+        return out, bad.value
+
+    def interpolate_state_covariance(self, stamps):
+        """18 x 18 joint covariances of [theta p | omega v | b_g b_a] at the stamps (pose as interpolate_covariance, body
+        velocity as interpolate, both bias splines); returns (cov (n, 18, 18), num_invalid)."""
+        stamps = _f64(stamps).ravel()
+        out = np.zeros((stamps.size, STATE_COV_DIM, STATE_COV_DIM))
+        bad = C.c_int(0)
+        self._check(self.lib.hb200_interpolate_state_covariance(self.h, stamps.size, _d(stamps), _d(out), C.byref(bad)))
         return out, bad.value
 
     def iterate(self, iterations=1, records=True):

@@ -233,15 +233,25 @@ int hb200_get_delta(hb200_ctx* ctx, double* delta_pose /* n */, double* delta_la
  *                             and corner full, padding rows 0), landmark = [L][3][3] (may be NULL).  Shape: info K, beta, m, L.
  *   hb200_interpolate_covariance: the 6 x 6 covariance of the pose [theta | p] interpolated at each stamp, at the knots of
  *                             the last successful compute; stamps outside the valid span give zero blocks, counted.
+ *   hb200_interpolate_state_covariance: the 18 x 18 joint covariance of x(t) = [theta p | omega v | b_g b_a] at each stamp:
+ *                             the pose as above, the body velocity of hb200_interpolate (omega the body rate, v = R^T pdot)
+ *                             and both bias splines evaluated at t, J(t) Sigma J(t)^T over the stamp's k control points
+ *                             and the 4 knots of each bias spline (all within the band, the arrow and the corner), exactly
+ *                             symmetric.  Knots, knot table and bias splines are those of the last successful compute:
+ *                             later iterations, appends and slides change nothing until the next one.  A stamp outside the
+ *                             pose spline's valid span, or outside that of a bias spline with knots, gives a zero block,
+ *                             counted; a window without bias splines gives zero bias rows and columns.  Gravity cross terms
+ *                             are in the corner of hb200_get_covariance.  -2 before a compute succeeded, -1 for n < 0 or a
+ *                             NULL stamps / cov with n > 0.
  * Sharded contexts (a communicator or the all-reduce callback): hb200_build_covariance and hb200_compute_covariance are
  * collective, see the SHARDING CONTRACT below.  The build assembles each rank's undamped partial system (its factors, the
  * Schur complement of the landmarks it owns) and sums it over the ranks with ONE system reduction, as hb200_build_system
  * does; the compute then inverts the same reduced system on every rank (band, arrow, corner, status, bad_dof and
  * min_pivot_ratio bit-identical across ranks) and the marginals of the rank's own landmarks: read a landmark's block from
  * its owner (a landmark a rank holds but does not observe gets a zero block there).  hb200_get_covariance and
- * hb200_interpolate_covariance are local calls; the interpolated covariances are identical on every rank.  A peer that
- * does not reach the reduction makes the build fail (-7 after the peer-memory reduction's timeout, the callback's error
- * + 200) instead of hanging the others.
+ * hb200_interpolate_covariance / hb200_interpolate_state_covariance are local calls; the interpolated covariances are
+ * identical on every rank.  A peer that does not reach the reduction makes the build fail (-7 after the peer-memory
+ * reduction's timeout, the callback's error + 200) instead of hanging the others.
  * A window whose band + arrow (6 (beta+1) + m rows, square) does not fit one CTA's shared memory gets -6 (on a sharded
  * context from every rank, before the reduction: it depends only on the agreed layout).  Ceres-tangent and ambient
  * blocks: hyper::Covariance (host, one GPU). */
@@ -259,6 +269,8 @@ int hb200_build_covariance(hb200_ctx* ctx);
 int hb200_compute_covariance(hb200_ctx* ctx, hb200_covariance_info* info);
 int hb200_get_covariance(hb200_ctx* ctx, double* packed /* P | A | C of SysLayout */, double* landmark /* [L][3][3], may be NULL */);
 int hb200_interpolate_covariance(hb200_ctx* ctx, int n, const double* stamps, double* cov /* [n][6][6] */, int* num_invalid);
+enum { HB200_STATE_COV_DIM = 18 };
+int hb200_interpolate_state_covariance(hb200_ctx* ctx, int n, const double* stamps, double* cov /* [n][18][18] */, int* num_invalid);
 
 /* full LM iterations: evaluate -> build -> [allreduce] -> solve -> retract -> cost at trial ->
  * accept/reject, all on the device.  records may be NULL. */

@@ -1,8 +1,10 @@
 """Time the marginal covariances on the device: hb200_build_covariance, hb200_compute_covariance (selected inverse +
-landmark marginals) and hb200_interpolate_covariance at 1000 stamps, with CUDA events around each call, on cfg1, cfg2
-and a K = 500 window.  Prints the card and its power limit first; one JSON line per window.
+landmark marginals), hb200_interpolate_covariance and hb200_interpolate_state_covariance at 1000 stamps, with CUDA
+events around each call (host copies included), on cfg1, cfg2 and a K = 500 window.  Prints the card and its power
+limit first; one JSON line per window.  --baseline-lib PATH alternates, round by round, with contexts of another build
+of libhyperb200.so (the calls it lacks are skipped) and prints its line (lib = "baseline") after each window's.
 
-    python tools/covariance_timing.py [--reps 5]
+    python tools/covariance_timing.py [--reps 5] [--baseline-lib PATH]
 """
 import argparse
 import json
@@ -44,34 +46,55 @@ def window(name):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--baseline-lib", default=None)
     args = ap.parse_args()
+    import ctypes
     import torch
     from hyperslam_b200 import runtime
+    libs = dict(current=runtime.load_library())
+    if args.baseline_lib:
+        base = ctypes.CDLL(os.path.abspath(args.baseline_lib))   # RTLD_LOCAL: both builds' symbols stay apart
+        for fn, res in (("hb200_last_error_string", ctypes.c_char_p), ("hb200_stream", ctypes.c_void_p), ("hb200_launch_count", ctypes.c_longlong)):
+            getattr(base, fn).restype = res
+        base.hb200_launch_count.argtypes = [ctypes.c_void_p]
+        base.hb200_destroy.argtypes, base.hb200_destroy.restype = [ctypes.c_void_p], None
+        libs["baseline"] = base
     print(f"# {card()}")
     for name in ("cfg1", "cfg2", "K500"):
         win = window(name)
-        ctx = runtime.Context(0)
-        ctx.load_window(win)
-        stream = torch.cuda.ExternalStream(ctx.stream)
+        ctxs = {}
+        for lib_name, lib in libs.items():
+            runtime._lib = lib          # a Context keeps the library it was created with
+            ctxs[lib_name] = runtime.Context(0)
+            ctxs[lib_name].load_window(win)
+        runtime._lib = libs["current"]
         kt = win.knots[:, 7]
         stamps = np.linspace(kt[win.order], kt[-win.order], 1000)
-        t = dict(build=[], compute=[], interpolate=[])
-        info = None
+        t = {n: dict(build=[], compute=[], interpolate=[], interpolate_state=[]) for n in ctxs}
+        info = {}
         for r in range(args.reps + 1):
-            for key, fn in (("build", ctx.build_covariance), ("compute", ctx.compute_covariance), ("interpolate", lambda: ctx.interpolate_covariance(stamps))):
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record(stream)
-                out = fn()
-                e1.record(stream)
-                e1.synchronize()
-                if key == "compute":
-                    info = out
-                if r:   # first round: warm-up
-                    t[key].append(e0.elapsed_time(e1))
-        K, beta, m, L = info["K"], info["beta"], info["m"], info["L"]
-        print(json.dumps(dict(window=name, K=K, beta=beta, m=m, L=L, status=info["status"], min_pivot_ratio=info["min_pivot_ratio"],
-                              **{f"{k}_ms": float(np.median(v)) for k, v in t.items()}, reps=args.reps)))
-        ctx.close()
+            for lib_name, ctx in ctxs.items():
+                stream = torch.cuda.ExternalStream(ctx.stream)
+                calls = [("build", ctx.build_covariance), ("compute", ctx.compute_covariance),
+                         ("interpolate", lambda: ctx.interpolate_covariance(stamps))]
+                if hasattr(ctx.lib, "hb200_interpolate_state_covariance"):
+                    calls.append(("interpolate_state", lambda: ctx.interpolate_state_covariance(stamps)))
+                for key, fn in calls:
+                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                    e0.record(stream)
+                    out = fn()
+                    e1.record(stream)
+                    e1.synchronize()
+                    if key == "compute":
+                        info[lib_name] = out
+                    if r:   # first round: warm-up
+                        t[lib_name][key].append(e0.elapsed_time(e1))
+        for lib_name, ctx in ctxs.items():
+            inf = info[lib_name]
+            K, beta, m, L = inf["K"], inf["beta"], inf["m"], inf["L"]
+            print(json.dumps(dict(window=name, lib=lib_name, K=K, beta=beta, m=m, L=L, status=inf["status"], min_pivot_ratio=inf["min_pivot_ratio"],
+                                  **{f"{k}_ms": float(np.median(v)) for k, v in t[lib_name].items() if v}, reps=args.reps)))
+            ctx.close()
 
 
 if __name__ == "__main__":
