@@ -1317,11 +1317,15 @@ HB_DI int stereo_track(int f, const double* __restrict__ stamps, const int* __re
   const double dt[3] = {cb[4] - ca[4], cb[5] - ca[5], cb[6] - ca[6]};
   m3_tvec(Ra, dt, t01);
   m3_vec(R01, b1, d1);
-  const double aa = b0[0] * b0[0] + b0[1] * b0[1] + b0[2] * b0[2], bb = b0[0] * d1[0] + b0[1] * d1[1] + b0[2] * d1[2];
-  const double cc = d1[0] * d1[0] + d1[1] * d1[1] + d1[2] * d1[2];
-  const double ee = b0[0] * t01[0] + b0[1] * t01[1] + b0[2] * t01[2], ff = d1[0] * t01[0] + d1[1] * t01[1] + d1[2] * t01[2];
-  const double idet = 1.0 / (aa * cc - bb * bb);
-  const double sa = (ee * cc - bb * ff) * idet, ub = (bb * ee - aa * ff) * idet;
+  // Closest points s b0 and t01 + u d1 from n = b0 x d1: s = ((t01 x d1) . n) / |n|^2, u = ((t01 x b0) . n) / |n|^2.
+  // The error follows the problem's conditioning (depth / baseline); the Gram form a c - b^2 = sin^2(parallax) cancels
+  // and grows as (depth / baseline)^2.  Parallel rays give n = 0 and a non-finite point (0 / 0).
+  double n[3], td[3], tb[3];
+  cross(b0, d1, n);
+  cross(t01, d1, td);
+  cross(t01, b0, tb);
+  const double inn = 1.0 / (n[0] * n[0] + n[1] * n[1] + n[2] * n[2]);
+  const double sa = (td[0] * n[0] + td[1] * n[1] + td[2] * n[2]) * inn, ub = (tb[0] * n[0] + tb[1] * n[1] + tb[2] * n[2]) * inn;
   double p0[3], pb[3], pw[3];
 #pragma unroll
   for (int i = 0; i < 3; ++i) p0[i] = 0.5 * (sa * b0[i] + t01[i] + ub * d1[i]);

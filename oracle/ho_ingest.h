@@ -34,16 +34,19 @@ inline void pixel_to_bearing(const double* cam, const double* px, double* b) {
   b[0] = nrm[0] * inv; b[1] = nrm[1] * inv; b[2] = inv;
 }
 
-// midpoint triangulation in the frame of camera 0: rays s b0 and t_01 + t R_01 b1
+// midpoint triangulation in the frame of camera 0: rays s b0 and t_01 + u R_01 b1, closest points from n = b0 x d1
+// (s = ((t x d1) . n) / |n|^2, u = ((t x b0) . n) / |n|^2), so the error follows depth / baseline rather than its
+// square (the Gram determinant a c - b^2 = sin^2 of the parallax cancels).  Parallel rays: n = 0, non-finite point.
 inline void triangulate_midpoint(const double* T_01, const double* b0, const double* b1, double* p0) {
-  double R[9], d1[3];
+  double R[9], d1[3], n[3], td[3], tb[3];
   quat_to_rot(T_01, R);
   m3_vec(R, b1, d1);
   const double* t = T_01 + 4;
-  const double a = v3_dot(b0, b0), b = v3_dot(b0, d1), c = v3_dot(d1, d1);
-  const double e = v3_dot(b0, t), f = v3_dot(d1, t);
-  const double det = a * c - b * b;
-  const double s = (e * c - b * f) / det, u = (b * e - a * f) / det;
+  v3_cross(b0, d1, n);
+  v3_cross(t, d1, td);
+  v3_cross(t, b0, tb);
+  const double inn = 1.0 / v3_dot(n, n);
+  const double s = v3_dot(td, n) * inn, u = v3_dot(tb, n) * inn;
   for (int i = 0; i < 3; ++i) p0[i] = 0.5 * (s * b0[i] + t[i] + u * d1[i]);
 }
 

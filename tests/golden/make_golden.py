@@ -8,9 +8,14 @@ Independent of both the C oracle and the CUDA kernels:
     alpha^ = R^T Rddot - omega^ omega^), NOT from the Sommer recursion the oracle/kernels use;
   * Jacobians come from central differences of the residual along the manifold retractions
     (R <- Exp(theta) R, p <- p + rho, Ceres SphereManifold Plus for gravity), h = 1e-20;
+  * calib/<case>.json: calibration blocks (hb200_factor_evaluate) of the case's factors: camera / IMU / pose-sensor
+    extrinsics in the tangent R_bs <- Exp(theta) R_bs, t_bs <- t_bs + rho, and intrinsics, distortion, I_g, I_a, S_g,
+    X_a in their raw coordinates;
   * the edge windows (k*_spline_edges) also carry hb200_interpolate answers: pose, body velocity and body
-    acceleration from the same time differences.
-Run:  python tests/golden/make_golden.py      (takes ~1 minute)
+    acceleration from the same time differences;
+  * ingest/k*_stereo_ingest hold stereo tracks on the edge windows with their bearings (the distortion inverted by
+    mp.findroot), the midpoint p_0 in camera 0 and the world landmark.
+Run:  python tests/golden/make_golden.py      (takes ~2 minutes)
 """
 import dataclasses
 import json
@@ -251,7 +256,30 @@ def perturbed(st, kind, index, comp, h):
     elif kind == "gravity":
         d = [mp.mpf(0)] * 2; d[comp] = h
         out["gravity"] = sphere_plus(st["gravity"], d)
+    elif kind in ("cam_ext", "sensor_ext", "imu_ext"):
+        # extrinsics T_bs in the tangent of hb200_calib.cuh: R_bs <- Exp(theta) R_bs, t_bs <- t_bs + rho
+        key = {"cam_ext": "cams", "sensor_ext": "pose_sensors", "imu_ext": "imu"}[kind]
+        rows = [list(st["imu"])] if key == "imu" else [list(v) for v in st[key]]
+        T = rows[0 if key == "imu" else index]
+        if comp < 3:
+            d = [mp.mpf(0)] * 3; d[comp] = h
+            T[:4] = quat_mul(quat_exp(d), T[:4])
+        else:
+            T[4 + comp - 3] += h
+        out[key] = rows[0] if key == "imu" else rows
+    elif kind in ("cam_intr", "cam_dist"):
+        cams = [list(v) for v in st["cams"]]
+        cams[index][(7 if kind == "cam_intr" else 11) + comp] += h
+        out["cams"] = cams
+    elif kind in IMU_BLOCKS:
+        # I_g, I_a (6 raw entries, imu_matrix's order), S_g, X_a (9, column-major): raw coordinates
+        imu = list(st["imu"])
+        imu[IMU_BLOCKS[kind][0] + comp] += h
+        out["imu"] = imu
     return out
+
+
+IMU_BLOCKS = {"I_g": (7, 6), "I_a": (13, 6), "S_g": (19, 9), "X_a": (28, 9)}   # offset in the imu row, size
 
 
 def numdiff(fn, st, f, kind, index, comp):
@@ -281,6 +309,7 @@ def make_case(name, n_pix=3, n_imu=3, **kw):
         case["inertial"].append(inertial_answer(st, w, f_))
         print(name, "inertial", f_, case["inertial"][-1]["r"][:3])
     write_case(name, case)
+    write_calibration(name, st, case)
 
 
 def make_widened_case(name, n_bearing=3, n_pose=3, **kw):
@@ -295,9 +324,38 @@ def make_widened_case(name, n_bearing=3, n_pose=3, **kw):
         case["pose"].append(pose_answer(st, w, f_))
         print(name, "pose", f_, case["pose"][-1]["r"][:3])
     write_case(name, case)
+    write_calibration(name, st, case)
 
 
 fl = lambda v: [float(x) for x in v]
+
+
+def calib_block(fn, st, f, kind, index, n):
+    """Rows x n Jacobian of fn along the n coordinates of one calibration block (perturbed())."""
+    cols = [numdiff(fn, st, f, kind, index, c) for c in range(n)]
+    return [[float(col[row]) for col in cols] for row in range(len(cols[0]))]
+
+
+def write_calibration(name, st, case):
+    """calib/<name>.json: the calibration blocks (hb200_factor_evaluate's sensor blocks) of every pixel, bearing and pose
+    factor of a case and of its first inertial factor (216 entries each), in perturbed()'s coordinates."""
+    mpl = lambda v: [mp.mpf(x) for x in v]
+    out = dict(pixel=[], bearing=[], pose=[], inertial=[])
+    for a in case["pixel"]:
+        f = dict(stamp=mp.mpf(a["stamp"]), cam=a["cam"], lm=a["lm"], pixel=mpl(a["pixel"]))
+        out["pixel"].append(dict(Jext=calib_block(pixel_residual, st, f, "cam_ext", a["cam"], 6), Jintr=calib_block(pixel_residual, st, f, "cam_intr", a["cam"], 4),
+                                 Jdist=calib_block(pixel_residual, st, f, "cam_dist", a["cam"], 4)))
+    for a in case.get("bearing", []):
+        f = dict(stamp=mp.mpf(a["stamp"]), cam=a["cam"], lm=a["lm"], bearing=mpl(a["bearing"]))
+        out["bearing"].append(dict(Jext=calib_block(bearing_residual, st, f, "cam_ext", a["cam"], 6)[0]))
+    for a in case.get("pose", []):
+        f = dict(stamp=mp.mpf(a["stamp"]), sensor=a["sensor"], pose=mpl(a["pose"]))
+        out["pose"].append(dict(Jext=calib_block(pose_residual, st, f, "sensor_ext", a["sensor"], 6)))
+    for a in case["inertial"][:1]:
+        f = dict(stamp=mp.mpf(a["stamp"]), meas=mpl(a["meas"]))
+        out["inertial"].append(dict(Jext=calib_block(inertial_residual, st, f, "imu_ext", 0, 6),
+                                    **{"J" + b.replace("_", ""): calib_block(inertial_residual, st, f, b, 0, n) for b, (_, n) in IMU_BLOCKS.items()}))
+    write_case(os.path.join("calib", name), out)
 
 
 def pixel_answer(st, w, i):
@@ -479,9 +537,104 @@ def make_edge_case(name, order, seed, n_pix=5, n_bearing=2, n_pose=2, n_imu=2):
                 pose=[pose_answer(st, w, i) for i in range(n_pose)], inertial=[inertial_answer(st, w, i) for i in range(n_imu)],
                 interpolate=[interpolate_answer(st, mp.mpf(float(t))) for t in stamps])
     write_case(name, case)
+    write_calibration(name, st, case)
+
+
+# ---- stereo ingest (hb200_ingest_stereo, hb200_append_stereo_tracks) ---------------------------------------------
+INGEST_DEPTHS = [0.5, 2.0, 10.0, 100.0, 1000.0]
+
+
+def distort(cam, x, y):
+    k1, k2, p1, p2 = cam[11:15]
+    r2 = x * x + y * y
+    rad = 1 + k1 * r2 + k2 * r2 * r2
+    return [x * rad + 2 * p1 * x * y + p2 * (r2 + 2 * x * x), y * rad + p1 * (r2 + 2 * y * y) + 2 * p2 * x * y]
+
+
+def pixel_bearing(cam, px):
+    """Unit bearing of a pixel: the distortion inverted by mp.findroot, started at the distorted point.  Asserts that
+    the forward model is monotone (positive Jacobian determinant) on the ray from the centre to the root."""
+    cx, cy, fx, fy = cam[7:11]
+    d = [(px[0] - cx) / fx, (px[1] - cy) / fy]
+    x, y = mp.findroot(lambda x, y: [a - b for a, b in zip(distort(cam, x, y), d)], d)
+    for s in mp.linspace(0, 1, 41)[1:]:
+        J = mp.jacobian(lambda a, b: distort(cam, a, b), [s * x, s * y])
+        assert J[0, 0] * J[1, 1] - J[0, 1] * J[1, 0] > 0, (px, s)
+    assert max(abs(a - b) for a, b in zip(distort(cam, x, y), d)) < mp.mpf(10) ** -70
+    n = mp.sqrt(x * x + y * y + 1)
+    return mp.matrix([x / n, y / n, 1 / n])
+
+
+def stereo_answer(st, stamp, c0, c1, px0, px1):
+    """Bearings of both views, the midpoint p_0 of the common perpendicular in camera 0 (None for parallel rays) and
+    the world landmark R (R_b0 p_0 + t_b0) + p at the stamp, from the stored double inputs."""
+    ca, cb = st["cams"][c0], st["cams"][c1]
+    b0, b1 = pixel_bearing(ca, px0), pixel_bearing(cb, px1)
+    Ra, Rb = quat_to_rot(ca[:4]), quat_to_rot(cb[:4])
+    t = Ra.T * (mp.matrix(cb[4:7]) - mp.matrix(ca[4:7]))
+    d1 = Ra.T * Rb * b1
+    dot = lambda u, v: sum(u[i] * v[i] for i in range(3))
+    det = dot(b0, b0) * dot(d1, d1) - dot(b0, d1) ** 2
+    out = dict(stamp=float(stamp), cam0=c0, cam1=c1, px0=fl(px0), px1=fl(px1), b0=fl(b0), b1=fl(b1), p0=None, lm=None)
+    if det != 0:
+        s = (dot(b0, t) * dot(d1, d1) - dot(b0, d1) * dot(d1, t)) / det
+        u = (dot(b0, d1) * dot(b0, t) - dot(b0, b0) * dot(d1, t)) / det
+        p0 = (s * b0 + t + u * d1) / 2
+        R, p = pose(st["knots"], st["k"], stamp)
+        out.update(p0=fl(p0), lm=fl(R * (Ra * p0 + mp.matrix(ca[4:7])) + p))
+    return out
+
+
+def make_ingest_case(name, edges, seed):
+    """Stereo tracks on the window of the edges fixture, at its edge stamps: the EuRoC pair (cameras 0, 1), a generic
+    pair (2, 3: rotated rig, other intrinsics, barrel-free distortion with large tangential terms, 0.2 m baseline) and a
+    parallel pair (4, 5: identity rotations, no distortion, principal points).  Camera-0 pixels at the image centre,
+    the four corners and four points beyond the image, each with two of INGEST_DEPTHS along its ray (every depth three
+    or four times per pair); camera-1 pixels from the forward model in doubles."""
+    with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), f"{edges}.json")) as fh:
+        w = json.load(fh)["window"]
+    k, knots = w["order"], np.array(w["knots"])
+    rng = np.random.default_rng(seed)
+    gen0 = synthetic.EUROC_CAM0.copy()
+    gen0[:4] = synthetic.rot_to_quat(synthetic.so3_exp(rng.normal(0, 0.2, (1, 3))) @ synthetic.quat_to_rot(gen0[None, :4]))[0]
+    gen0[7:11] = [330.0, 260.0, 420.0, 425.0]
+    gen0[11:15] = [0.05, -0.01, 1.5e-3, -1.2e-3]
+    gen1 = gen0.copy()
+    gen1[:4] = synthetic.rot_to_quat(synthetic.so3_exp(rng.normal(0, 0.05, (1, 3))) @ synthetic.quat_to_rot(gen0[None, :4]))[0]
+    gen1[4:7] += synthetic.quat_to_rot(gen0[None, :4])[0] @ np.array([0.2, 0.01, -0.005])
+    gen1[7:11] = [345.0, 250.0, 430.0, 428.0]
+    gen1[11:15] = [0.04, -0.008, -1.1e-3, 9e-4]
+    par0 = np.concatenate([[0, 0, 0, 1, 0, 0, 0], gen0[7:11], [0, 0, 0, 0]])
+    par1 = par0.copy()
+    par1[4] = 0.11
+    cams = np.stack([synthetic.EUROC_CAM0, synthetic.EUROC_CAM1, gen0, gen1, par0, par1])
+    stamps = edge_stamps(knots, k)
+    pixels = [(376.0, 240.0), (0.0, 0.0), (751.0, 0.0), (0.0, 479.0), (751.0, 479.0), (-150.0, -100.0), (950.0, -80.0), (-120.0, 620.0),
+              (900.0, 640.0)]
+    mpm = lambda a: [[mp.mpf(float(x)) for x in row] for row in a]
+    st = dict(k=k, knots=mpm(knots), cams=mpm(cams))
+    inputs = []
+    for c0, c1 in ((0, 1), (2, 3)):
+        for i, px0 in enumerate(pixels):
+            b0 = np.array(fl(pixel_bearing(st["cams"][c0], [mp.mpf(v) for v in px0])))
+            for depth in (INGEST_DEPTHS[(i + c0) % 5], INGEST_DEPTHS[(i + c0 + 2) % 5]):
+                ca, cb = cams[c0], cams[c1]
+                p_s1 = synthetic.quat_to_rot(cb[None, :4])[0].T @ (synthetic.quat_to_rot(ca[None, :4])[0] @ (depth * b0) + ca[4:7] - cb[4:7])
+                assert p_s1[2] > 0
+                inputs.append((stamps[len(inputs) % len(stamps)], c0, c1, px0, synthetic.project(cams, np.array([c1]), p_s1[None])[0]))
+    inputs.append((stamps[0], 4, 5, par0[7:9], par1[7:9]))
+    inputs.sort(key=lambda a: a[0])                     # arrival order, as hb200_append_stereo_tracks requires
+    case = dict(name=name, edges=edges, digits=mp.mp.dps, cameras=cams.tolist(),
+                tracks=[stereo_answer(st, mp.mpf(float(t)), c0, c1, [mp.mpf(float(v)) for v in p0], [mp.mpf(float(v)) for v in p1])
+                        for t, c0, c1, p0, p1 in inputs])
+    write_case(os.path.join("ingest", name), case)
 
 
 if __name__ == "__main__":
+    if "--ingest-only" in sys.argv:
+        make_ingest_case("k4_stereo_ingest", "k4_spline_edges", seed=synthetic.SEED_BASE + 924)
+        make_ingest_case("k6_stereo_ingest", "k6_spline_edges", seed=synthetic.SEED_BASE + 926)
+        sys.exit(0)
     if "--widened-only" in sys.argv:
         make_widened_case("k4_bearing_pose", order=4, num_knots=10, num_landmarks=12, num_imu=0, seed=synthetic.SEED_BASE + 905)
         make_widened_case("k6_bearing_pose", order=6, num_knots=12, num_landmarks=12, num_imu=0, seed=synthetic.SEED_BASE + 906, n_bearing=2, n_pose=2)
@@ -494,3 +647,5 @@ if __name__ == "__main__":
     make_widened_case("k6_bearing_pose", order=6, num_knots=12, num_landmarks=12, num_imu=0, seed=synthetic.SEED_BASE + 906, n_bearing=2, n_pose=2)
     make_edge_case("k4_spline_edges", order=4, seed=synthetic.SEED_BASE + 914)
     make_edge_case("k6_spline_edges", order=6, seed=synthetic.SEED_BASE + 916)
+    make_ingest_case("k4_stereo_ingest", "k4_spline_edges", seed=synthetic.SEED_BASE + 924)
+    make_ingest_case("k6_stereo_ingest", "k6_spline_edges", seed=synthetic.SEED_BASE + 926)

@@ -1,5 +1,22 @@
 """Ingest (pixels -> bearings, stereo triangulation) and trajectory output around the hot path
-(SURVEY.md section 8f rank 4; reference abstract.cpp:186-264, main.cpp:56-83, evaluation/conversions.py)."""
+(SURVEY.md section 8f rank 4; reference abstract.cpp:186-264, main.cpp:56-83, evaluation/conversions.py).
+
+The k*_stereo_ingest known answers (tests/golden/ingest/, 80 digits: bearings from mp.findroot on the distortion, the
+midpoint p_0 and the world landmark from the stored double inputs) hold every output to |got - ref| <= C u scale,
+u = 2^-53, C = 150 (the bound of test_gpu_spline_edges.py):
+  * bearing: scale 1.  Ten Newton steps on the 2 x 2 distortion system, then a normalisation: a few ulps of a unit vector;
+  * landmark: scale max(|lm|, |p_0|^2 / |t_01|).  The rays s b_0 and t_01 + u d_1 meet at a parallax angle of about
+    |t_01| / |p_0|, so tilting either bearing by u (its rounding) slides the midpoint along the ray by about
+    |p_0| u / (|t_01| / |p_0|) = |p_0|^2 / |t_01| u; moving p_0 into the world frame rounds at the size of |lm|.
+    The Gram form of the midpoint (det = a c - b^2 = sin^2 of the parallax, and its numerators) loses another factor
+    of about |p_0| / |t_01| to cancellation: worst ratios of 250 - 500 at 2 m, 1600 - 2200 at 10 m and 9e3 - 2.5e4 at
+    100 m on these fixtures (device and oracle), against below 5 at every depth for the cross-product form.
+Parallel rays (cameras 4 and 5: identity rotations, no distortion, principal points) have no midpoint: ingest returns a
+non-finite landmark without counting it invalid, and append_stereo_tracks rejects the track (status 2).
+"""
+import dataclasses
+import glob
+import json
 import os
 
 import numpy as np
@@ -7,6 +24,11 @@ import pytest
 
 import oracle_lib as ol
 from hyperslam_b200 import synthetic, trajectory
+from test_oracle import window_from_golden
+
+U = 2.0 ** -53
+C = 150.0
+INGEST = sorted(glob.glob(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ingest", "*.json")))
 
 
 def stereo_frame(win, stamp, n, rng, noise=0.0):
@@ -43,6 +65,59 @@ def test_oracle_ingest_is_exact_on_noise_free_tracks(order):
     # re-projecting the bearing through the forward camera model gives the pixel back
     back = synthetic.project(win.cameras, np.zeros(lm.size, dtype=int), B0)
     assert np.abs(back - px0).max() < 1e-9
+
+
+def load_tracks(path):
+    """The fixture, its tracks as arrays, and the window it runs on: its spline-edge fixture's knots, biases, gravity and
+    IMU / pose factors with the fixture's cameras, and no landmarks or visual factors (tracks arrive in stamp order)."""
+    with open(path) as f:
+        case = json.load(f)
+    with open(os.path.join(os.path.dirname(os.path.dirname(path)), case["edges"] + ".json")) as f:
+        edges = json.load(f)
+    win = dataclasses.replace(window_from_golden(dict(edges, pixel=[], bearing=[])), cameras=np.array(case["cameras"]), landmarks=np.zeros((0, 3)))
+    tr = case["tracks"]
+    cols = dict(stamp=np.array([t["stamp"] for t in tr]), cam0=np.array([t["cam0"] for t in tr], np.int32),
+                cam1=np.array([t["cam1"] for t in tr], np.int32), px0=np.array([t["px0"] for t in tr]), px1=np.array([t["px1"] for t in tr]),
+                parallel=np.array([t["lm"] is None for t in tr]))
+    return case, cols, win
+
+
+def ingest_ratios(case, b0, b1, lm):
+    """Worst |got - ref| / (u scale) of the bearings and, per depth decade of |p_0|, of the landmarks."""
+    cams = np.array(case["cameras"])
+    worst = {}
+    for n, t in enumerate(case["tracks"]):
+        worst["bearing"] = max(worst.get("bearing", 0.0), np.abs(b0[n] - t["b0"]).max() / U, np.abs(b1[n] - t["b1"]).max() / U)
+        if t["lm"] is None:
+            continue
+        p0, ref = np.array(t["p0"]), np.array(t["lm"])
+        baseline = np.linalg.norm(cams[t["cam1"], 4:7] - cams[t["cam0"], 4:7])
+        scale = max(np.linalg.norm(ref), p0 @ p0 / baseline)
+        key = "landmark_%gm" % 10.0 ** np.floor(np.log10(np.linalg.norm(p0)))
+        worst[key] = max(worst.get(key, 0.0), np.abs(lm[n] - ref).max() / (U * scale))
+    return worst
+
+
+def check_ingest(worst, record_property, name):
+    for key, v in worst.items():
+        record_property(f"{name}:{key}", round(v, 3))
+    bad = {key: v for key, v in worst.items() if not v <= C}
+    assert not bad, f"{name}: worst |got - ref| / (u scale) above C = {C:g}: {bad}"
+
+
+@pytest.mark.parametrize("path", INGEST, ids=[os.path.basename(p) for p in INGEST])
+def test_oracle_ingest_against_golden(path, record_property):
+    """CPU twin of the GPU test: oracle/ho_ingest.h under the same bound."""
+    case, t, win = load_tracks(path)
+    k, cams = win.order, win.cameras
+    out = [np.zeros((t["stamp"].size, 3)) for _ in range(3)]
+    for n, stamp in enumerate(t["stamp"]):
+        j = int(np.searchsorted(win.knots[:, 7], stamp, side="right") - 1) - (k - 1) // 2
+        res = ol.ingest_stereo_frame(win.knots[j:j + k], stamp, cams[t["cam0"][n]], cams[t["cam1"][n]], t["px0"][n:n + 1], t["px1"][n:n + 1])
+        for o, r in zip(out, res):
+            o[n] = r[0]
+    assert not np.isfinite(out[2][t["parallel"]]).any() and np.isfinite(out[2][~t["parallel"]]).all()
+    check_ingest(ingest_ratios(case, *out), record_property, os.path.basename(path))
 
 
 def test_trajectory_format_and_tum_conversion(tmp_path):
@@ -90,6 +165,47 @@ def test_gpu_ingest_matches_oracle(built, order):
     _, _, _, bad = ctx.ingest_stereo(np.array([99.0, 0.5]), np.array([0, 7]), np.array([1, 1]), np.zeros((2, 2)), np.zeros((2, 2)))
     assert bad == 2
     ctx.close()
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("path", INGEST, ids=[os.path.basename(p) for p in INGEST])
+def test_gpu_ingest_against_golden(built, path, record_property):
+    """hb200_ingest_stereo against the known answers; hb200_append_stereo_tracks writes the same landmarks and
+    bearing factors bit for bit, and rejects the parallel track."""
+    from hyperslam_b200 import runtime
+    from test_gpu_stereo_window import error_code
+    case, t, win = load_tracks(path)
+    ctx, ref = runtime.Context(0), runtime.Context(0)
+    ctx.load_window(win)
+    ref.load_window(win)
+    args = [t[key] for key in ("stamp", "cam0", "cam1", "px0", "px1")]
+    b0, b1, lm, bad = ctx.ingest_stereo(*args)
+    par = t["parallel"]
+    assert bad == 0 and not np.isfinite(lm[par]).any() and np.isfinite(lm[~par]).all()
+    worst = ingest_ratios(case, b0, b1, lm)
+
+    counts = ctx.factor_counts().tolist()
+    assert error_code(ctx.append_stereo_tracks, *[a[par] for a in args], -np.ones(int(par.sum()), np.int32)) == 2
+    assert ctx.L == 0 and ctx.factor_counts().tolist() == counts
+    ok = ~par
+    n = int(ok.sum())
+    out, n_new = ctx.append_stereo_tracks(*[a[ok] for a in args], -np.ones(n, np.int32))
+    assert n_new == n and np.array_equal(out, np.arange(n))
+    assert np.array_equal(ctx.state()["landmarks"], lm[ok])
+    # the bearing factors it wrote: the same as appending ingest's bearings at positions 2i, 2i + 1
+    ref.append_landmarks(lm[ok])
+    ref.append_bearing_factors(np.repeat(t["stamp"][ok], 2), np.stack([t["cam0"][ok], t["cam1"][ok]], 1).ravel(), np.repeat(np.arange(n, dtype=np.int32), 2),
+                               np.stack([b0[ok], b1[ok]], 1).reshape(-1, 3))
+    assert ctx.factor_counts().tolist() == ref.factor_counts().tolist()
+    outs = []
+    for c in (ctx, ref):
+        c.evaluate(jacobians=True)
+        outs.append(c.outputs())
+    for key in ("b_r", "b_Jp", "b_Jl"):
+        assert np.array_equal(outs[0][key], outs[1][key]), key
+    ctx.close()
+    ref.close()
+    check_ingest(worst, record_property, os.path.basename(path))
 
 
 @pytest.mark.gpu
