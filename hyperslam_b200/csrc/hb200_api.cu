@@ -390,6 +390,14 @@ template <typename F>
 int with_flag(bool b, F&& f) {
   return b ? f(std::true_type{}) : f(std::false_type{});
 }
+// f(K, DET) for both spline orders and both assembly modes: kernel attributes are set for every instantiation at once
+template <typename F>
+int for_each_order_mode(F&& f) {
+  for (const int k : {4, 6})
+    for (const bool det : {false, true})
+      if (const int rc = with_order(k, [&](auto K) { return with_flag(det, [&](auto D) { return f(K, D); }); })) return rc;
+  return 0;
+}
 
 // Launch configuration of the resident band solver: a grid of one 2-CTA cluster (chain r in CTA r) on the context's
 // stream, each chain's workspace in its CTA's shared memory.  at: storage for the cluster-dimension attribute.
@@ -536,9 +544,9 @@ int reset_solver_state(hb200_ctx* c) {
 
 // ---- kernel dispatch on (order, bias order) -------------------------------------------------
 template <bool J>
-PixelArgs pixel_args(hb200_ctx* c, int sel, bool accumulate) {
+PixelArgs pixel_args(hb200_ctx* c, int sel, double* sys) {
   PixelArgs a{};
-  a.sys = accumulate ? c->assembly() : nullptr; a.lay = c->lay; a.tiles_per_cta = 1;
+  a.sys = sys; a.lay = c->lay; a.tiles_per_cta = 1;
   a.n = c->Nv; a.stamp = c->v_stamp.p; a.pixel = reinterpret_cast<const double2*>(c->v_pixel.p); a.meas_z = c->v_z.p; a.idx = c->v_idx.p;
   a.tab = c->tab[sel].p; a.cam_tab = c->cam_tab.p; a.landmarks = c->lms[sel].p;
   a.r = J ? c->v_r.p : nullptr; a.Jp = c->v_Jp.p; a.Jl = c->v_Jl.p; a.w = c->v_w.p; a.cost_partial = c->cp_pix[J ? 0 : 1].p; a.huber = c->huber; a.huber_bearing = c->huber_bearing; a.K_knots = c->K;
@@ -553,19 +561,23 @@ InertialArgs inertial_args(hb200_ctx* c, int sel) {
   a.cost_partial = c->cp_imu[J ? 0 : 1].p; a.loss_scale = c->imu_scale;
   return a;
 }
-template <int K, bool J>
-int launch_pixel(hb200_ctx* c, int sel, bool accumulate = false) {
-  if (c->Nv == 0) return 0;
-  PixelArgs a = pixel_args<J>(c, sel, accumulate);
-  if (J && accumulate && c->deterministic) {
-    pixel_eval_det_kernel<K><<<c->n_pix_blocks, kEvalThreads, 0, c->stream>>>(a, c->basis, c->det_pix, c->det_seg_off.p);
-    HB_LAUNCH(c, "pixel_eval_det_kernel");
-    return 0;
+// f(FUSE, DET) with the pixel body's flags: a Jacobian sweep with a system to accumulate into fuses the pixel J^T J,
+// into the records of the deterministic assembly when the context asks for it
+template <bool J, typename F>
+int with_pixel_pass(const hb200_ctx* c, const PixelArgs& a, F&& f) {
+  if constexpr (J) {
+    if (a.sys) return with_flag(c->deterministic, [&](auto D) { return f(std::true_type{}, D); });
   }
-  if (J && accumulate) pixel_eval_kernel<K, J, J><<<c->n_pix_blocks, kEvalThreads, 0, c->stream>>>(a, c->basis);
-  else pixel_eval_kernel<K, J, false><<<c->n_pix_blocks, kEvalThreads, 0, c->stream>>>(a, c->basis);
-  HB_LAUNCH(c, "pixel_eval_kernel");
-  return 0;
+  return f(std::false_type{}, std::false_type{});
+}
+template <int K, bool J>
+int launch_pixel(hb200_ctx* c, int sel, double* sys) {
+  if (c->Nv == 0) return 0;
+  const PixelArgs a = pixel_args<J>(c, sel, sys);
+  return with_pixel_pass<J>(c, a, [&](auto FUSE, auto DET) {
+    pixel_eval_kernel<K, J, FUSE, DET><<<c->n_pix_blocks, kEvalThreads, 0, c->stream>>>(a, c->basis, DET ? c->det_pix : DetOut{}, DET ? c->det_seg_off.p : nullptr);
+    return check_launch(c, DET ? "pixel_eval_det_kernel" : "pixel_eval_kernel");
+  });
 }
 template <int K, bool J>
 int launch_inertial(hb200_ctx* c, int sel) {
@@ -577,20 +589,16 @@ int launch_inertial(hb200_ctx* c, int sel) {
 }
 // visual + inertial factors in one launch (both lists non-empty)
 template <int K, bool J>
-int launch_factors_merged(hb200_ctx* c, int sel, bool accumulate) {
-  const PixelArgs pa = pixel_args<J>(c, sel, accumulate);
+int launch_factors_merged(hb200_ctx* c, int sel, double* sys) {
+  const PixelArgs pa = pixel_args<J>(c, sel, sys);
   const InertialArgs ia = inertial_args<J>(c, sel);
   const int blocks = c->n_pix_blocks + c->n_imu_blocks;
   const size_t smem = J ? inertial_stash_bytes(K) : 0;
-  if (J && accumulate && c->deterministic) {
-    factor_eval_det_kernel<K, 4><<<blocks, kEvalThreads, smem, c->stream>>>(pa, ia, c->basis, c->bias_basis, c->n_pix_blocks, c->det_pix, c->det_seg_off.p);
-    HB_LAUNCH(c, "factor_eval_det_kernel");
-    return 0;
-  }
-  if (J && accumulate) factor_eval_kernel<K, 4, J, J><<<blocks, kEvalThreads, smem, c->stream>>>(pa, ia, c->basis, c->bias_basis, c->n_pix_blocks);
-  else factor_eval_kernel<K, 4, J, false><<<blocks, kEvalThreads, smem, c->stream>>>(pa, ia, c->basis, c->bias_basis, c->n_pix_blocks);
-  HB_LAUNCH(c, "factor_eval_kernel");
-  return 0;
+  return with_pixel_pass<J>(c, pa, [&](auto FUSE, auto DET) {
+    factor_eval_kernel<K, 4, J, FUSE, DET><<<blocks, kEvalThreads, smem, c->stream>>>(pa, ia, c->basis, c->bias_basis, c->n_pix_blocks, DET ? c->det_pix : DetOut{},
+                                                                                     DET ? c->det_seg_off.p : nullptr);
+    return check_launch(c, DET ? "factor_eval_det_kernel" : "factor_eval_kernel");
+  });
 }
 template <int K, bool J>
 int launch_manifold(hb200_ctx* c, int sel) {
@@ -603,19 +611,12 @@ int launch_manifold(hb200_ctx* c, int sel) {
   return 0;
 }
 
-// keep_fork: leave the side stream forked on return (the caller enqueues more side-stream work and joins).
-// clear_system: zero the packed reduced system in the knot-table launch; skip_prep: the table of state `sel` is
-// already up to date (retract_kernel built the trial table).
-int enqueue_evaluate(hb200_ctx* c, bool want_J, int sel, bool accumulate = false, bool keep_fork = false, bool clear_system = false,
-                     bool skip_prep = false) {
-  if (!skip_prep) {
-    const size_t nclear = clear_system ? static_cast<size_t>(c->lay.total) : 0;
-    const int blocks = clear_system ? static_cast<int>(std::min<size_t>((nclear / 4 + 255) / 256, static_cast<size_t>(c->num_sms) * 4)) : (c->K + 255) / 256;
-    prep_kernel<<<std::max(blocks, (c->K + 255) / 256), 256, 0, c->stream>>>(c->K, c->knots[sel].p, c->tab[sel].p, clear_system ? c->assembly() : nullptr, nclear);
-    HB_LAUNCH(c, "prep_kernel");
-  }
+// The factor kernels of state `sel` (0: current, 1: trial) on its up-to-date knot table: residuals and cost partials,
+// Jacobians with want_J.  sys (enqueue_assembly): Jacobians, the pixel J^T J fused into this packed system, and the
+// side stream left forked for enqueue_build.
+int enqueue_factors(hb200_ctx* c, bool want_J, int sel, double* sys = nullptr) {
   int rc = 0;
-  const bool J_any = want_J || accumulate;
+  const bool J_any = want_J || sys;
   // Small windows are latency-bound: one launch for both factor families.  Large windows are throughput-bound: the
   // merged kernel would run the pixel CTAs at the inertial body's 255 registers, so the families stay separate.
   if (c->Nv && c->Ni && c->n_pix_blocks + c->n_imu_blocks <= 4 * c->num_sms) {   // (also while profiling: same kernels as the graph)
@@ -623,7 +624,7 @@ int enqueue_evaluate(hb200_ctx* c, bool want_J, int sel, bool accumulate = false
     if (c->Nm && (rc = fork_side(c))) return rc;
     rc = with_order(c->k, [&](auto K) {
       return with_flag(J_any, [&](auto J) {
-        const int r = launch_factors_merged<K, J>(c, sel, accumulate);
+        const int r = launch_factors_merged<K, J>(c, sel, sys);
         return r ? r : launch_manifold<K, J>(c, sel);
       });
     });
@@ -634,16 +635,23 @@ int enqueue_evaluate(hb200_ctx* c, bool want_J, int sel, bool accumulate = false
   }
   // visual factors on the main stream, inertial + manifold factors concurrently on the side stream
   if (c->Nv && (c->Ni || c->Nm) && (rc = fork_side(c))) return rc;
-  // accumulate (fused path): the pixel J^T J is accumulated by the factor kernel itself
+  // sys (fused path): the pixel J^T J is accumulated by the factor kernel itself
   rc = with_order(c->k, [&](auto K) {
     return with_flag(J_any, [&](auto J) {
-      int r = launch_pixel<K, J>(c, sel, accumulate);
+      int r = launch_pixel<K, J>(c, sel, sys);
       if (!r) r = launch_inertial<K, J>(c, sel);
       return r ? r : launch_manifold<K, J>(c, sel);
     });
   });
-  if (rc || !keep_fork) { const int rj = join_side(c); if (!rc) rc = rj; }
+  if (rc || !sys) { const int rj = join_side(c); if (!rc) rc = rj; }
   return rc;
+}
+
+// Knot table of state `sel`, then its factor sweep
+int enqueue_evaluate(hb200_ctx* c, bool want_J, int sel) {
+  prep_kernel<<<(c->K + 255) / 256, 256, 0, c->stream>>>(c->K, c->knots[sel].p, c->tab[sel].p, nullptr, 0);
+  HB_LAUNCH(c, "prep_kernel");
+  return enqueue_factors(c, want_J, sel);
 }
 
 // The rest of the normal equations, after the factor kernels have cleared the packed system and accumulated the pixel
@@ -661,6 +669,8 @@ int inertial_splits(const hb200_ctx* c, bool* scalar_hess) {
   return (*scalar_hess || c->k != 4) ? c->imu_splits : c->imu_splits_mma;
 }
 
+// DET instantiations (deterministic assembly) write the records of their region of the context's DetOut instead of
+// adding into the packed system; their profile labels keep the _det_kernel names.
 int enqueue_build(hb200_ctx* c, const SolverState* st) {
   const bool det = c->deterministic;
   if (det && !c->det_ready) return fail(-2, "deterministic assembly: record slots not laid out for this window");
@@ -670,30 +680,29 @@ int enqueue_build(hb200_ctx* c, const SolverState* st) {
     const int splits = inertial_splits(c, &scalar_hess);
     const int grid = c->nruns * splits;
     const int rc = with_order(c->k, [&](auto K) {
-      if (det && scalar_hess)
-        inertial_hessian_det_kernel<K, 4><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->i_idx.p, c->i_r.p, c->i_Jp.p, c->i_wg.p, c->i_wa.p,
-                                                                              c->i_Jg.p, c->imu_scale, c->lay, c->o_bg(), c->o_ba(), c->o_g(), splits, c->det_imu);
-      else if (det)
-        inertial_hessian_mma_det_kernel<K, 4, K == 4 ? 8 : 12><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->i_idx.p, c->i_r.p, c->i_Jp.p, c->i_wg.p, c->i_wa.p,
-                                                                                                  c->i_Jg.p, c->imu_scale, c->lay, c->o_bg(), c->o_ba(), c->o_g(), splits,
-                                                                                                  c->det_imu);
-      else if (scalar_hess)
-        inertial_hessian_kernel<K, 4><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->i_idx.p, c->i_r.p, c->i_Jp.p, c->i_wg.p, c->i_wa.p,
-                                                                          c->i_Jg.p, c->imu_scale, c->assembly(), c->lay, c->o_bg(), c->o_ba(), c->o_g(), c->imu_splits);
-      else
-        inertial_hessian_mma_kernel<K, 4, K == 4 ? 8 : 12><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->i_idx.p, c->i_r.p, c->i_Jp.p, c->i_wg.p, c->i_wa.p,
-                                                                                              c->i_Jg.p, c->imu_scale, c->assembly(), c->lay, c->o_bg(), c->o_ba(), c->o_g(), splits);
-      return check_launch(c, scalar_hess ? (det ? "inertial_hessian_det_kernel" : "inertial_hessian_kernel")
-                                         : (det ? "inertial_hessian_mma_det_kernel" : "inertial_hessian_mma_kernel"));
+      return with_flag(det, [&](auto DET) {
+        const DetOut d = DET ? c->det_imu : DetOut{};
+        if (scalar_hess)
+          inertial_hessian_kernel<K, 4, DET><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->i_idx.p, c->i_r.p, c->i_Jp.p, c->i_wg.p, c->i_wa.p, c->i_Jg.p,
+                                                                                 c->imu_scale, c->assembly(), c->lay, c->o_bg(), c->o_ba(), c->o_g(), splits, d);
+        else
+          inertial_hessian_mma_kernel<K, 4, K == 4 ? 8 : 12, DET><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->i_idx.p, c->i_r.p, c->i_Jp.p, c->i_wg.p, c->i_wa.p,
+                                                                                                     c->i_Jg.p, c->imu_scale, c->assembly(), c->lay, c->o_bg(), c->o_ba(),
+                                                                                                     c->o_g(), splits, d);
+        return check_launch(c, scalar_hess ? (DET ? "inertial_hessian_det_kernel" : "inertial_hessian_kernel")
+                                           : (DET ? "inertial_hessian_mma_det_kernel" : "inertial_hessian_mma_kernel"));
+      });
     });
     if (rc) return rc;
   }
   if (c->Nm) {
     const int blocks = (c->Nm + kManWarps - 1) / kManWarps;
     const int rc = with_order(c->k, [&](auto K) {
-      if (det) manifold_hessian_det_kernel<K><<<blocks, kManWarps * 32, 0, side(c)>>>(c->Nm, c->m_idx.p, c->m_r.p, c->m_Jp.p, c->lay, c->det_man);
-      else manifold_hessian_kernel<K><<<blocks, kManWarps * 32, 0, side(c)>>>(c->Nm, c->m_idx.p, c->m_r.p, c->m_Jp.p, c->assembly(), c->lay);
-      return check_launch(c, det ? "manifold_hessian_det_kernel" : "manifold_hessian_kernel");
+      return with_flag(det, [&](auto DET) {
+        manifold_hessian_kernel<K, DET><<<blocks, kManWarps * 32, 0, side(c)>>>(c->Nm, c->m_idx.p, c->m_r.p, c->m_Jp.p, c->assembly(), c->lay,
+                                                                               DET ? c->det_man : DetOut{});
+        return check_launch(c, DET ? "manifold_hessian_det_kernel" : "manifold_hessian_kernel");
+      });
     });
     if (rc) return rc;
   }
@@ -706,26 +715,22 @@ int enqueue_build(hb200_ctx* c, const SolverState* st) {
   if (c->Nv && c->L && c->schur_groups) {
     const size_t smem = (3 * static_cast<size_t>(kSchurGroup) * (c->schur_rt + 1) + 3 * kSchurGroup + 4 * 3 * static_cast<size_t>(c->schur_rt)) * sizeof(double);
     const int rc = with_order(c->k, [&](auto K) {
-      if (det)
-        schur_group_det_kernel<K><<<c->n_lm_groups, kSchurGThreads, smem, c->stream>>>(c->lm_group_off.p, c->lm_order.p, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p,
-                                                                                       c->v_Jp.p, c->v_Jl.p, c->v_w.p, st, c->lay, c->Vchol.p, c->gl.p, c->Dl.p, c->schur_rt,
-                                                                                       c->det_schur);
-      else
-        schur_group_kernel<K><<<c->n_lm_groups, kSchurGThreads, smem, c->stream>>>(c->lm_group_off.p, c->lm_order.p, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p, c->v_Jp.p,
-                                                                                   c->v_Jl.p, c->v_w.p, st, c->assembly(), c->lay, c->Vchol.p, c->gl.p, c->Dl.p, c->schur_rt);
-      return check_launch(c, det ? "schur_group_det_kernel" : "schur_group_kernel");
+      return with_flag(det, [&](auto DET) {
+        schur_group_kernel<K, DET><<<c->n_lm_groups, kSchurGThreads, smem, c->stream>>>(c->lm_group_off.p, c->lm_order.p, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p,
+                                                                                        c->v_Jp.p, c->v_Jl.p, c->v_w.p, st, c->assembly(), c->lay, c->Vchol.p, c->gl.p,
+                                                                                        c->Dl.p, c->schur_rt, DET ? c->det_schur : DetOut{});
+        return check_launch(c, DET ? "schur_group_det_kernel" : "schur_group_kernel");
+      });
     });
     if (rc) return rc;
   } else if (c->Nv && c->L) {
     const size_t smem = 2 * 3 * static_cast<size_t>(c->max_rows) * sizeof(double);
     const int rc = with_order(c->k, [&](auto K) {
-      if (det)
-        schur_det_kernel<K><<<c->L, kSchurThreads, smem, c->stream>>>(c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p, st,
-                                                                      c->lay, c->Vchol.p, c->gl.p, c->Dl.p, c->max_rows, c->det_schur);
-      else
-        schur_kernel<K><<<c->L, kSchurThreads, smem, c->stream>>>(c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p, st,
-                                                                  c->assembly(), c->lay, c->Vchol.p, c->gl.p, c->Dl.p, c->max_rows);
-      return check_launch(c, det ? "schur_det_kernel" : "schur_kernel");
+      return with_flag(det, [&](auto DET) {
+        schur_kernel<K, DET><<<c->L, kSchurThreads, smem, c->stream>>>(c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p, st,
+                                                                       c->assembly(), c->lay, c->Vchol.p, c->gl.p, c->Dl.p, c->max_rows, DET ? c->det_schur : DetOut{});
+        return check_launch(c, DET ? "schur_det_kernel" : "schur_kernel");
+      });
     });
     if (rc) return rc;
   }
@@ -743,6 +748,18 @@ int enqueue_build(hb200_ctx* c, const SolverState* st) {
   det_reduce_kernel<<<std::max(blocks, 1), kDetThreads, 0, c->stream>>>(nent, c->det_off.p, c->det_perm.p, c->det_val.p, c->assembly());
   HB_LAUNCH(c, "det_reduce_kernel");
   return 0;
+}
+
+// The normal equations at the current state: the knot-table launch also zeroes the packed system, the Jacobian sweep
+// accumulates the pixel J^T J into it (rewriting the same residuals and Jacobians), enqueue_build does the rest.
+// st: as for enqueue_build.  The deterministic record slots must be laid out (prepare_det) before this is enqueued.
+int enqueue_assembly(hb200_ctx* c, const SolverState* st) {
+  const size_t nclear = static_cast<size_t>(c->lay.total);
+  const int blocks = static_cast<int>(std::min<size_t>((nclear / 4 + 255) / 256, static_cast<size_t>(c->num_sms) * 4));
+  prep_kernel<<<std::max(blocks, (c->K + 255) / 256), 256, 0, c->stream>>>(c->K, c->knots[0].p, c->tab[0].p, c->assembly(), nclear);
+  HB_LAUNCH(c, "prep_kernel");
+  const int rc = enqueue_factors(c, true, 0, c->assembly());
+  return rc ? rc : enqueue_build(c, st);
 }
 
 // Lays out the deterministic assembly's record regions for the bound window and clears the keys and the entry index,
@@ -976,14 +993,12 @@ int enqueue_reduce_scalars(hb200_ctx* c) {
 // One LM iteration enqueued on the stream (graph-capturable unless the callback hook is in use).
 int enqueue_iteration(hb200_ctx* c) {
   int rc = 0;
-  // the factor kernels clear the packed system and accumulate the pixel J^T J into it (enqueue_build does the rest)
-  if ((rc = enqueue_evaluate(c, true, 0, /*accumulate=*/true, /*keep_fork=*/true, /*clear_system=*/true))) return rc;
-  if ((rc = enqueue_build(c, c->st.p))) return rc;
+  if ((rc = enqueue_assembly(c, c->st.p))) return rc;
   if ((rc = enqueue_reduce_system(c))) return rc;
   bool retracted = false;
   if ((rc = enqueue_solve(c, /*fuse_retract=*/true, &retracted))) return rc;
   if (!retracted && (rc = enqueue_retract(c))) return rc;   // (also builds the trial knot table)
-  if ((rc = enqueue_evaluate(c, false, 1, false, false, false, /*skip_prep=*/true))) return rc;
+  if ((rc = enqueue_factors(c, false, 1))) return rc;   // the trial state's cost (its knot table is built)
   if ((rc = enqueue_reduce_scalars(c))) return rc;
   return enqueue_accept(c);
 }
@@ -1123,15 +1138,16 @@ int create_impl(const hb200_options* options, hb200_ctx* c) {
   HB_CUDA(cudaFuncSetAttribute(cholesky_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kCholSmem)));
   // the Jacobian passes of the inertial factors park their forward-sweep state in dynamic shared memory (41.5 KB at
   // order 4, 69 KB at order 6); together with the static scratch of the merged kernel that is above the 48 KB default
-  HB_CUDA(cudaFuncSetAttribute(inertial_eval_kernel<4, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(inertial_stash_bytes(4))));
-  HB_CUDA(cudaFuncSetAttribute(inertial_eval_kernel<6, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(inertial_stash_bytes(6))));
-  HB_CUDA(cudaFuncSetAttribute(factor_eval_kernel<4, 4, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(inertial_stash_bytes(4))));
-  HB_CUDA(cudaFuncSetAttribute(factor_eval_kernel<4, 4, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(inertial_stash_bytes(4))));
-  HB_CUDA(cudaFuncSetAttribute(factor_eval_kernel<6, 4, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(inertial_stash_bytes(6))));
-  HB_CUDA(cudaFuncSetAttribute(factor_eval_kernel<6, 4, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(inertial_stash_bytes(6))));
-  HB_CUDA(cudaFuncSetAttribute(factor_eval_det_kernel<4, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(inertial_stash_bytes(4))));
-  HB_CUDA(cudaFuncSetAttribute(factor_eval_det_kernel<6, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(inertial_stash_bytes(6))));
-  return reset_solver_state(c);
+  rc = for_each_order_mode([&](auto K, auto DET) {
+    const int stash = static_cast<int>(inertial_stash_bytes(K));
+    HB_CUDA(cudaFuncSetAttribute(factor_eval_kernel<K, 4, true, true, DET>, cudaFuncAttributeMaxDynamicSharedMemorySize, stash));
+    if constexpr (!DET) {   // the Jacobian passes without a fused J^T J have no deterministic instantiation
+      HB_CUDA(cudaFuncSetAttribute(factor_eval_kernel<K, 4, true, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, stash));
+      HB_CUDA(cudaFuncSetAttribute(inertial_eval_kernel<K, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, stash));
+    }
+    return 0;
+  });
+  return rc ? rc : reset_solver_state(c);
 }
 }  // namespace
 
@@ -1560,10 +1576,11 @@ int derive_window(hb200_ctx* c, int kind = 0) {
   for (int s = 0; s < 2; ++s) { HB_CUDA(c->cp_pix[s].ensure(std::max(c->n_pix_blocks, 1))); HB_CUDA(c->cp_imu[s].ensure(std::max(c->n_imu_blocks + c->n_man_blocks, 1))); }
   if (c->max_rows * 6 * sizeof(double) > 48 * 1024) {
     const int smem = static_cast<int>(2 * 3 * static_cast<size_t>(c->max_rows) * sizeof(double));
-    HB_CUDA(cudaFuncSetAttribute(schur_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    HB_CUDA(cudaFuncSetAttribute(schur_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    HB_CUDA(cudaFuncSetAttribute(schur_det_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    HB_CUDA(cudaFuncSetAttribute(schur_det_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    const int rs = for_each_order_mode([&](auto K, auto DET) {
+      HB_CUDA(cudaFuncSetAttribute(schur_kernel<K, DET>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+      return 0;
+    });
+    if (rs) return rs;
   }
   int rc = update_fixed(c);
   if (rc) return rc;
@@ -1686,10 +1703,11 @@ int hb200_bind(hb200_ctx* c, int* num_invalid) {
       const size_t smem = (3 * static_cast<size_t>(kSchurGroup) * (c->schur_rt + 1) + 3 * kSchurGroup + 4 * 3 * static_cast<size_t>(c->schur_rt)) * sizeof(double);
       if (smem > 200 * 1024) c->schur_groups = false;
       else {
-        HB_CUDA(cudaFuncSetAttribute(schur_group_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-        HB_CUDA(cudaFuncSetAttribute(schur_group_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-        HB_CUDA(cudaFuncSetAttribute(schur_group_det_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-        HB_CUDA(cudaFuncSetAttribute(schur_group_det_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+        rc = for_each_order_mode([&](auto K, auto DET) {
+          HB_CUDA(cudaFuncSetAttribute(schur_group_kernel<K, DET>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+          return 0;
+        });
+        if (rc) return rc;
       }
     }
   }
@@ -1997,10 +2015,7 @@ int hb200_build_system(hb200_ctx* c) {
   if (!c->evaluated_J) return fail(-2, "call hb200_evaluate(HB200_EVAL_JACOBIANS) first");
   HB_CUDA(cudaSetDevice(c->device));
   if ((rc = prepare_det(c))) return rc;
-  // assembled as enqueue_iteration does: the Jacobian sweep at the current state runs again with the pixel J^T J
-  // accumulated by the factor kernels (it rewrites the same residuals and Jacobians), then the rest of the system
-  if ((rc = enqueue_evaluate(c, true, 0, /*accumulate=*/true, /*keep_fork=*/true, /*clear_system=*/true))) return rc;
-  if ((rc = enqueue_build(c, c->st.p))) return rc;
+  if ((rc = enqueue_assembly(c, c->st.p))) return rc;   // as enqueue_iteration assembles
   if ((rc = enqueue_reduce_system(c))) return rc;
   c->system_built = true;
   return 0;
@@ -2064,9 +2079,7 @@ int hb200_build_covariance(hb200_ctx* c) {
   s.radius = INFINITY;   // mu = 1 / radius = 0 in the Schur kernels
   HB_CUDA(c->cov_st.ensure(1));
   HB_CUDA(cudaMemcpyAsync(c->cov_st.p, &s, sizeof(s), cudaMemcpyHostToDevice, c->stream));
-  // the Jacobian sweep at the current state with the pixel J^T J accumulated, then the rest of the system (undamped)
-  if ((rc = enqueue_evaluate(c, true, 0, /*accumulate=*/true, /*keep_fork=*/true, /*clear_system=*/true))) return rc;
-  if ((rc = enqueue_build(c, c->cov_st.p))) return rc;
+  if ((rc = enqueue_assembly(c, c->cov_st.p))) return rc;   // undamped
   // the linearisation point of this build, for the interpolated covariance
   HB_CUDA(c->cov_knots_next.ensure(8 * static_cast<size_t>(c->K)));
   HB_CUDA(c->cov_tab_next.ensure(static_cast<size_t>(kTabStride) * c->K));

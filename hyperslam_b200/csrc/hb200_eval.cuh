@@ -14,7 +14,7 @@
 namespace hb {
 
 // ---------------------------------------------------------------------------------------------
-// Deterministic assembly (hb200_set_deterministic).  The J^T J kernels' variants for it add nothing into the packed
+// Deterministic assembly (hb200_set_deterministic).  The J^T J kernels' DET instantiations add nothing into the packed
 // system: each contribution is stored with a plain store into a record of its own, next to the index of the packed
 // entry it belongs to, and det_reduce_kernel (hb200_solve.cuh) sums every entry's records in ascending record order.
 // A kernel owns one region of records, cut into equal slots (a pixel segment, an inertial CTA, a manifold factor, a
@@ -576,8 +576,8 @@ HB_DI void cta_pixel_hessian(const PixelArgs& a, int f0, int cnt, double* sJ /*[
 
 // bid: the CTA's index within the pixel grid (the merged factor kernel offsets it).  DET (fused pass, one tile per CTA):
 // the J^T J goes to the slots of the tile's segments, seg_off[bid] .. seg_off[bid + 1] - 1
-template <int K, bool WANT_J, bool FUSE, bool DET = false>
-HB_DI void pixel_eval_body(const PixelArgs& a, const Basis& B, int bid0, const DetOut& det = DetOut{}, const int* seg_off = nullptr) {
+template <int K, bool WANT_J, bool FUSE, bool DET>
+HB_DI void pixel_eval_body(const PixelArgs& a, const Basis& B, int bid0, const DetOut& det, const int* seg_off) {
   __shared__ __align__(16) double s_tab[kTileRows * kTabStride];
   __shared__ __align__(8) uint64_t s_bar;
   __shared__ int s_red[2];
@@ -642,12 +642,11 @@ HB_DI void pixel_eval_body(const PixelArgs& a, const Basis& B, int bid0, const D
   if (FUSE && a.sys != nullptr) pixel_hess_flush<K, DET>(a, acc, det, DET ? seg_off[bid0 + 1] - 1 : 0);
 }
 
-template <int K, bool WANT_J, bool FUSE = false>
-__global__ void __launch_bounds__(kEvalThreads, (K == 4 && FUSE) ? 6 : 1) pixel_eval_kernel(PixelArgs a, Basis B) { pixel_eval_body<K, WANT_J, FUSE>(a, B, blockIdx.x); }
-// the fused pass of the deterministic assembly
-template <int K>
-__global__ void __launch_bounds__(kEvalThreads, K == 4 ? 6 : 1) pixel_eval_det_kernel(PixelArgs a, Basis B, DetOut det, const int* __restrict__ seg_off) {
-  pixel_eval_body<K, true, true, true>(a, B, blockIdx.x, det, seg_off);
+// DET: the fused pass of the deterministic assembly
+template <int K, bool WANT_J, bool FUSE, bool DET>
+__global__ void __launch_bounds__(kEvalThreads, (K == 4 && FUSE) ? 6 : 1) pixel_eval_kernel(PixelArgs a, Basis B, DetOut det, const int* __restrict__ seg_off) {
+  static_assert(!DET || (WANT_J && FUSE), "the deterministic assembly is a fused Jacobian pass");
+  pixel_eval_body<K, WANT_J, FUSE, DET>(a, B, blockIdx.x, det, seg_off);
 }
 
 // segments (runs of equal knot base) of every 64-factor tile of the visual list: the slots of the deterministic fused pass
@@ -1031,16 +1030,12 @@ __global__ void __launch_bounds__(kEvalThreads) inertial_eval_kernel(InertialArg
 // Visual and inertial factors in ONE launch (they are independent): CTAs [0, n_pix_blocks) run the pixel / bearing
 // body, the rest the inertial body.  At 12 k factors each of these kernels is a ~20 us latency-bound launch; side by
 // side they cost the longer of the two.
-template <int K, int KB, bool WANT_J, bool FUSE>
-__global__ void __launch_bounds__(kEvalThreads) factor_eval_kernel(PixelArgs pa, InertialArgs ia, Basis B, Basis BB, int n_pix_blocks) {
-  if (static_cast<int>(blockIdx.x) < n_pix_blocks) pixel_eval_body<K, WANT_J, FUSE>(pa, B, blockIdx.x);
+template <int K, int KB, bool WANT_J, bool FUSE, bool DET>
+__global__ void __launch_bounds__(kEvalThreads) factor_eval_kernel(PixelArgs pa, InertialArgs ia, Basis B, Basis BB, int n_pix_blocks, DetOut det,
+                                                                   const int* __restrict__ seg_off) {
+  static_assert(!DET || (WANT_J && FUSE), "the deterministic assembly is a fused Jacobian pass");
+  if (static_cast<int>(blockIdx.x) < n_pix_blocks) pixel_eval_body<K, WANT_J, FUSE, DET>(pa, B, blockIdx.x, det, seg_off);
   else inertial_eval_body<K, KB, WANT_J>(ia, B, BB, blockIdx.x - n_pix_blocks);
-}
-template <int K, int KB>
-__global__ void __launch_bounds__(kEvalThreads) factor_eval_det_kernel(PixelArgs pa, InertialArgs ia, Basis B, Basis BB, int n_pix_blocks, DetOut det,
-                                                                       const int* __restrict__ seg_off) {
-  if (static_cast<int>(blockIdx.x) < n_pix_blocks) pixel_eval_body<K, true, true, true>(pa, B, blockIdx.x, det, seg_off);
-  else inertial_eval_body<K, KB, true>(ia, B, BB, blockIdx.x - n_pix_blocks);
 }
 
 

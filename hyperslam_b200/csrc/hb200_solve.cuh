@@ -247,22 +247,14 @@ HB_DI void inertial_hessian_body(const int* __restrict__ run_off, const int4* __
     }
   }
 }
-template <int K, int KB>
+// DET (deterministic assembly): the records of det, slot = CTA, instead of atomics into sys
+template <int K, int KB, bool DET>
 __global__ void __launch_bounds__(kHessThreads) inertial_hessian_kernel(const int* __restrict__ run_off, const int4* __restrict__ idx,
                                                                         const double* __restrict__ r, const double* __restrict__ Jp,
                                                                         const double* __restrict__ wg, const double* __restrict__ wa,
                                                                         const double* __restrict__ Jg, double loss_scale, double* sys,
-                                                                        SysLayout lay, int o_bg, int o_ba, int o_g, int splits) {
-  inertial_hessian_body<K, KB, false>(run_off, idx, r, Jp, wg, wa, Jg, loss_scale, sys, lay, o_bg, o_ba, o_g, splits, DetOut{});
-}
-// deterministic assembly: slot = CTA
-template <int K, int KB>
-__global__ void __launch_bounds__(kHessThreads) inertial_hessian_det_kernel(const int* __restrict__ run_off, const int4* __restrict__ idx,
-                                                                            const double* __restrict__ r, const double* __restrict__ Jp,
-                                                                            const double* __restrict__ wg, const double* __restrict__ wa,
-                                                                            const double* __restrict__ Jg, double loss_scale, SysLayout lay,
-                                                                            int o_bg, int o_ba, int o_g, int splits, DetOut det) {
-  inertial_hessian_body<K, KB, true>(run_off, idx, r, Jp, wg, wa, Jg, loss_scale, nullptr, lay, o_bg, o_ba, o_g, splits, det);
+                                                                        SysLayout lay, int o_bg, int o_ba, int o_g, int splits, DetOut det) {
+  inertial_hessian_body<K, KB, DET>(run_off, idx, r, Jp, wg, wa, Jg, loss_scale, sys, lay, o_bg, o_ba, o_g, splits, det);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -396,22 +388,14 @@ HB_DI void inertial_hessian_mma_body(const int* __restrict__ run_off, const int4
     }
   }
 }
-template <int K, int KB, int CH>
+// DET: slot = CTA
+template <int K, int KB, int CH, bool DET>
 __global__ void __launch_bounds__(kHessThreads) inertial_hessian_mma_kernel(const int* __restrict__ run_off, const int4* __restrict__ idx,
                                                                             const double* __restrict__ r, const double* __restrict__ Jp,
                                                                             const double* __restrict__ wg, const double* __restrict__ wa,
                                                                             const double* __restrict__ Jg, double loss_scale, double* sys,
-                                                                            SysLayout lay, int o_bg, int o_ba, int o_g, int splits) {
-  inertial_hessian_mma_body<K, KB, CH, false>(run_off, idx, r, Jp, wg, wa, Jg, loss_scale, sys, lay, o_bg, o_ba, o_g, splits, DetOut{});
-}
-// deterministic assembly: slot = CTA
-template <int K, int KB, int CH>
-__global__ void __launch_bounds__(kHessThreads) inertial_hessian_mma_det_kernel(const int* __restrict__ run_off, const int4* __restrict__ idx,
-                                                                                const double* __restrict__ r, const double* __restrict__ Jp,
-                                                                                const double* __restrict__ wg, const double* __restrict__ wa,
-                                                                                const double* __restrict__ Jg, double loss_scale, SysLayout lay,
-                                                                                int o_bg, int o_ba, int o_g, int splits, DetOut det) {
-  inertial_hessian_mma_body<K, KB, CH, true>(run_off, idx, r, Jp, wg, wa, Jg, loss_scale, nullptr, lay, o_bg, o_ba, o_g, splits, det);
+                                                                            SysLayout lay, int o_bg, int o_ba, int o_g, int splits, DetOut det) {
+  inertial_hessian_mma_body<K, KB, CH, DET>(run_off, idx, r, Jp, wg, wa, Jg, loss_scale, sys, lay, o_bg, o_ba, o_g, splits, det);
 }
 
 // J^T J / J^T r of the manifold (pose) factors: one warp per factor, lower triangle of its 6K x 6K block.
@@ -454,15 +438,10 @@ HB_DI void manifold_hessian_body(int nf, const int2* __restrict__ idx, const dou
     else atomicAdd(&g[c0 + a], s);
   }
 }
-template <int K>
+template <int K, bool DET>
 __global__ void __launch_bounds__(kManWarps * 32) manifold_hessian_kernel(int nf, const int2* __restrict__ idx, const double* __restrict__ r,
-                                                                         const double* __restrict__ Jp, double* sys, SysLayout lay) {
-  manifold_hessian_body<K, false>(nf, idx, r, Jp, sys, lay, DetOut{});
-}
-template <int K>
-__global__ void __launch_bounds__(kManWarps * 32) manifold_hessian_det_kernel(int nf, const int2* __restrict__ idx, const double* __restrict__ r,
-                                                                             const double* __restrict__ Jp, SysLayout lay, DetOut det) {
-  manifold_hessian_body<K, true>(nf, idx, r, Jp, nullptr, lay, det);
+                                                                         const double* __restrict__ Jp, double* sys, SysLayout lay, DetOut det) {
+  manifold_hessian_body<K, DET>(nf, idx, r, Jp, sys, lay, det);
 }
 
 // cost at the linearisation point = sum of the evaluation kernels' per-block partials (fixed order) -> scal[0] of
@@ -608,23 +587,14 @@ HB_DI void schur_body(const int* __restrict__ lm_off, const int* __restrict__ lm
     if (DET || val != 0.0) add(sys_index(lay, r0g + a, r0g + b), -val);
   }
 }
-template <int K>
+template <int K, bool DET>
 __global__ void __launch_bounds__(kSchurThreads) schur_kernel(const int* __restrict__ lm_off, const int* __restrict__ lm_obs,
                                                               const int4* __restrict__ idx, const double* __restrict__ r,
                                                               const double* __restrict__ Jp, const double* __restrict__ Jl, const double* __restrict__ wv,
                                                               const SolverState* __restrict__ st, double* sys, SysLayout lay,
                                                               double* __restrict__ Vchol, double* __restrict__ gl, double* __restrict__ Dl,
-                                                              int max_rows) {
-  schur_body<K, false>(lm_off, lm_obs, idx, r, Jp, Jl, wv, st, sys, lay, Vchol, gl, Dl, max_rows, DetOut{});
-}
-template <int K>
-__global__ void __launch_bounds__(kSchurThreads) schur_det_kernel(const int* __restrict__ lm_off, const int* __restrict__ lm_obs,
-                                                                  const int4* __restrict__ idx, const double* __restrict__ r,
-                                                                  const double* __restrict__ Jp, const double* __restrict__ Jl, const double* __restrict__ wv,
-                                                                  const SolverState* __restrict__ st, SysLayout lay,
-                                                                  double* __restrict__ Vchol, double* __restrict__ gl, double* __restrict__ Dl,
-                                                                  int max_rows, DetOut det) {
-  schur_body<K, true>(lm_off, lm_obs, idx, r, Jp, Jl, wv, st, nullptr, lay, Vchol, gl, Dl, max_rows, det);
+                                                              int max_rows, DetOut det) {
+  schur_body<K, DET>(lm_off, lm_obs, idx, r, Jp, Jl, wv, st, sys, lay, Vchol, gl, Dl, max_rows, det);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -805,24 +775,15 @@ HB_DI void schur_group_body(const int* __restrict__ group_off, const int* __rest
     if ((DET || acc != 0.0) && r0g + m < lay.np) add(lay.ob + r0g + m, acc);
   }
 }
-template <int K>
+template <int K, bool DET>
 __global__ void __launch_bounds__(kSchurGThreads) schur_group_kernel(const int* __restrict__ group_off, const int* __restrict__ lm_order,
                                                                     const int* __restrict__ lm_off, const int* __restrict__ lm_obs,
                                                                     const int4* __restrict__ idx, const double* __restrict__ r,
                                                                     const double* __restrict__ Jp, const double* __restrict__ Jl, const double* __restrict__ wv,
                                                                     const SolverState* __restrict__ st, double* sys, SysLayout lay,
-                                                                    double* __restrict__ Vchol, double* __restrict__ gl, double* __restrict__ Dl, int RT) {
-  schur_group_body<K, false>(group_off, lm_order, lm_off, lm_obs, idx, r, Jp, Jl, wv, st, sys, lay, Vchol, gl, Dl, RT, DetOut{});
-}
-template <int K>
-__global__ void __launch_bounds__(kSchurGThreads) schur_group_det_kernel(const int* __restrict__ group_off, const int* __restrict__ lm_order,
-                                                                        const int* __restrict__ lm_off, const int* __restrict__ lm_obs,
-                                                                        const int4* __restrict__ idx, const double* __restrict__ r,
-                                                                        const double* __restrict__ Jp, const double* __restrict__ Jl, const double* __restrict__ wv,
-                                                                        const SolverState* __restrict__ st, SysLayout lay,
-                                                                        double* __restrict__ Vchol, double* __restrict__ gl, double* __restrict__ Dl, int RT,
-                                                                        DetOut det) {
-  schur_group_body<K, true>(group_off, lm_order, lm_off, lm_obs, idx, r, Jp, Jl, wv, st, nullptr, lay, Vchol, gl, Dl, RT, det);
+                                                                    double* __restrict__ Vchol, double* __restrict__ gl, double* __restrict__ Dl, int RT,
+                                                                    DetOut det) {
+  schur_group_body<K, DET>(group_off, lm_order, lm_off, lm_obs, idx, r, Jp, Jl, wv, st, sys, lay, Vchol, gl, Dl, RT, det);
 }
 
 // ---------------------------------------------------------------------------------------------
