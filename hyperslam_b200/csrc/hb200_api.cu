@@ -141,6 +141,15 @@ int load_nccl() {
     if (r__ != 0) return fail(300 + r__, "%s: %s", #expr, g_nccl.GetErrorString ? g_nccl.GetErrorString(r__) : "nccl error"); \
   } while (0)
 
+// The linearisation point hb200_build_covariance froze: the shapes its outputs were written with, and copies of the
+// knots, the knot table and both bias splines (knot values and stamps) for the interpolated covariances.
+struct CovPoint {
+  SysLayout lay{};
+  Basis basis{}, bias_basis{};
+  int L = 0, k = 0, Nv = 0, max_rows = 0, Kbg = 0, Kba = 0;
+  DevBuf<double> knots, tab, bg, ba;
+};
+
 }  // namespace
 
 struct hb200_ctx {
@@ -268,24 +277,21 @@ struct hb200_ctx {
   // marginal covariances (hb200_build_covariance / hb200_compute_covariance).  cov_st: the build's own solver state
   // (radius +inf: no damping inside the landmark elimination; st is never touched).  cov_at: launch count after the last
   // covariance call -- any other launch since (an evaluation, an iteration, a slide) rewrote what the compute reads.
-  // *_next: what the next compute writes / the knots the build saw; committed to the unsuffixed buffers on success only.
+  // cov_pt: two linearisation points.  The build freezes one into the slot that is not committed (cov_slot_built); a
+  // successful compute commits it by index (cov_slot_committed, meaningful while cov_valid), so a failed compute or a
+  // build not yet computed leaves every reader on the committed point.  *_next: what the next compute writes, swapped
+  // with the unsuffixed results on success only.
   DevBuf<SolverState> cov_st;
-  DevBuf<double> cov_ws, cov_packed, cov_packed_next, cov_lm, cov_lm_next, cov_knots, cov_knots_next, cov_tab, cov_tab_next;
+  DevBuf<double> cov_ws, cov_packed, cov_packed_next, cov_lm, cov_lm_next;
   DevBuf<int> cov_counts;
   DevBuf<CovStatus> cov_status;
   bool cov_built = false, cov_valid = false;
   long long cov_at = -1;
   int cov_degenerate = 0, cov_unobserved = 0;
-  SysLayout cov_lay{}, cov_lay_next{};
-  Basis cov_basis{}, cov_basis_next{};
-  int cov_L = 0, cov_L_next = 0;
-  int cov_k_next = 0, cov_Nv_next = 0, cov_max_rows_next = 0;   // shapes the build's landmark outputs were written with
+  CovPoint cov_pt[2];
+  int cov_slot_built = 0, cov_slot_committed = 0;
   DevBuf<double> cov_t, cov_o;   // hb200_interpolate_covariance / hb200_interpolate_state_covariance staging
   DevBuf<int> cov_bad;
-  // the bias splines of the same linearisation point (knot values and stamps), for hb200_interpolate_state_covariance
-  DevBuf<double> cov_bg, cov_bg_next, cov_ba, cov_ba_next;
-  int cov_Kbg = 0, cov_Kbg_next = 0, cov_Kba = 0, cov_Kba_next = 0;
-  Basis cov_bias_basis{}, cov_bias_basis_next{};
 
   hb200_allreduce_fn allreduce = nullptr;
   void* allreduce_user = nullptr;
@@ -2047,27 +2053,68 @@ int hb200_get_delta(hb200_ctx* c, double* dp, double* dl) {
   return 0;
 }
 
+}  // extern "C"
+
 // ---- marginal covariances (hb200_cov.cuh) ------------------------------------------------------------------------
 namespace {
-int cov_check(hb200_ctx* c) {
-  if (!c) return fail(-1, "null context");
+void cov_info(hb200_ctx* c, hb200_covariance_info* info) {
+  const CovPoint& pt = c->cov_pt[c->cov_slot_committed];
+  info->degenerate_landmarks = c->cov_degenerate; info->unobserved_landmarks = c->cov_unobserved;
+  info->K = c->cov_valid ? pt.lay.K : 0; info->beta = c->cov_valid ? pt.lay.beta : 0;
+  info->m = c->cov_valid ? pt.lay.m : 0; info->L = c->cov_valid ? pt.L : 0;
+}
+
+// the current state as the linearisation point of a build
+int freeze_point(hb200_ctx* c, CovPoint& pt) {
+  pt.lay = c->lay; pt.basis = c->basis; pt.bias_basis = c->bias_basis;
+  pt.L = c->L; pt.k = c->k; pt.Nv = c->Nv; pt.max_rows = c->max_rows; pt.Kbg = c->Kbg; pt.Kba = c->Kba;
+  HB_CUDA(pt.knots.ensure(8 * static_cast<size_t>(c->K)));
+  HB_CUDA(pt.tab.ensure(static_cast<size_t>(kTabStride) * c->K));
+  HB_CUDA(cudaMemcpyAsync(pt.knots.p, c->knots[0].p, sizeof(double) * 8 * c->K, cudaMemcpyDeviceToDevice, c->stream));
+  HB_CUDA(cudaMemcpyAsync(pt.tab.p, c->tab[0].p, sizeof(double) * kTabStride * c->K, cudaMemcpyDeviceToDevice, c->stream));
+  HB_CUDA(pt.bg.ensure(4 * static_cast<size_t>(c->Kbg)));
+  HB_CUDA(pt.ba.ensure(4 * static_cast<size_t>(c->Kba)));
+  if (c->Kbg) HB_CUDA(cudaMemcpyAsync(pt.bg.p, c->bg[0].p, sizeof(double) * 4 * c->Kbg, cudaMemcpyDeviceToDevice, c->stream));
+  if (c->Kba) HB_CUDA(cudaMemcpyAsync(pt.ba.p, c->ba[0].p, sizeof(double) * 4 * c->Kba, cudaMemcpyDeviceToDevice, c->stream));
   return 0;
 }
-void cov_info(hb200_ctx* c, hb200_covariance_info* info) {
-  info->degenerate_landmarks = c->cov_degenerate; info->unobserved_landmarks = c->cov_unobserved;
-  info->K = c->cov_valid ? c->cov_lay.K : 0; info->beta = c->cov_valid ? c->cov_lay.beta : 0;
-  info->m = c->cov_valid ? c->cov_lay.m : 0; info->L = c->cov_valid ? c->cov_L : 0;
+
+// Both interpolation entry points: `launch(K, pt)` enqueues one kernel over the committed point that reads the stamps
+// in cov_t and writes `block` doubles per stamp to cov_o and an invalid flag to cov_bad.
+template <typename F>
+int cov_interpolate(hb200_ctx* c, int n, const double* stamps, double* cov, int* num_invalid, size_t block, F&& launch) {
+  if (!c) return fail(-1, "null context");
+  if (n < 0 || (n > 0 && (!stamps || !cov))) return fail(-1, "invalid argument");
+  if (!c->cov_valid) return fail(-2, "no covariance computed (hb200_compute_covariance has not succeeded)");
+  HB_CUDA(cudaSetDevice(c->device));
+  if (num_invalid) *num_invalid = 0;
+  if (n == 0) return 0;
+  const bool stamp = c->cov_built && c->cov_at == c->launches;   // (reads nothing a compute needs)
+  HB_CUDA(c->cov_t.ensure(n)); HB_CUDA(c->cov_o.ensure(block * n)); HB_CUDA(c->cov_bad.ensure(n));
+  HB_CUDA(cudaMemcpyAsync(c->cov_t.p, stamps, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
+  const CovPoint& pt = c->cov_pt[c->cov_slot_committed];
+  const int rc = with_order(pt.basis.k, [&](auto K) { return launch(K, pt); });
+  if (rc) return rc;
+  std::vector<int> bad(n);
+  HB_CUDA(cudaMemcpyAsync(cov, c->cov_o.p, sizeof(double) * block * n, cudaMemcpyDeviceToHost, c->stream));
+  HB_CUDA(cudaMemcpyAsync(bad.data(), c->cov_bad.p, sizeof(int) * n, cudaMemcpyDeviceToHost, c->stream));
+  HB_CUDA(cudaStreamSynchronize(c->stream));
+  if (num_invalid) *num_invalid = std::accumulate(bad.begin(), bad.end(), 0);
+  if (stamp) c->cov_at = c->launches;
+  return 0;
 }
 }  // namespace
+
+extern "C" {
 
 // Sharded contexts (a communicator or the all-reduce callback): collective.  Each rank assembles its undamped partial
 // system and writes its degenerate-landmark count into the tail slot kCovDegenerateSlot; ONE system reduction (as
 // hb200_build_system) then leaves the same reduced system and the window-wide count on every rank.  The -6 refusal
 // depends only on the agreed layout, so every rank refuses before the reduction.
 int hb200_build_covariance(hb200_ctx* c) {
-  int rc = cov_check(c);
+  if (!c) return fail(-1, "null context");
+  int rc = check_ready(c);
   if (rc) return rc;
-  if ((rc = check_ready(c))) return rc;
   HB_CUDA(cudaSetDevice(c->device));
   const bool sharded = c->multi();
   const size_t smem = cov_smem_doubles(c->beta, c->lay.m) * sizeof(double);
@@ -2080,15 +2127,8 @@ int hb200_build_covariance(hb200_ctx* c) {
   HB_CUDA(c->cov_st.ensure(1));
   HB_CUDA(cudaMemcpyAsync(c->cov_st.p, &s, sizeof(s), cudaMemcpyHostToDevice, c->stream));
   if ((rc = enqueue_assembly(c, c->cov_st.p))) return rc;   // undamped
-  // the linearisation point of this build, for the interpolated covariance
-  HB_CUDA(c->cov_knots_next.ensure(8 * static_cast<size_t>(c->K)));
-  HB_CUDA(c->cov_tab_next.ensure(static_cast<size_t>(kTabStride) * c->K));
-  HB_CUDA(cudaMemcpyAsync(c->cov_knots_next.p, c->knots[0].p, sizeof(double) * 8 * c->K, cudaMemcpyDeviceToDevice, c->stream));
-  HB_CUDA(cudaMemcpyAsync(c->cov_tab_next.p, c->tab[0].p, sizeof(double) * kTabStride * c->K, cudaMemcpyDeviceToDevice, c->stream));
-  HB_CUDA(c->cov_bg_next.ensure(4 * static_cast<size_t>(c->Kbg)));
-  HB_CUDA(c->cov_ba_next.ensure(4 * static_cast<size_t>(c->Kba)));
-  if (c->Kbg) HB_CUDA(cudaMemcpyAsync(c->cov_bg_next.p, c->bg[0].p, sizeof(double) * 4 * c->Kbg, cudaMemcpyDeviceToDevice, c->stream));
-  if (c->Kba) HB_CUDA(cudaMemcpyAsync(c->cov_ba_next.p, c->ba[0].p, sizeof(double) * 4 * c->Kba, cudaMemcpyDeviceToDevice, c->stream));
+  c->cov_slot_built = 1 - c->cov_slot_committed;
+  if ((rc = freeze_point(c, c->cov_pt[c->cov_slot_built]))) return rc;
   int counts[2] = {0, c->L};
   if (c->Nv && c->L) {
     HB_CUDA(c->cov_counts.ensure(2));
@@ -2116,9 +2156,6 @@ int hb200_build_covariance(hb200_ctx* c) {
   }
   c->cov_degenerate = sharded ? static_cast<int>(window_degenerate) : counts[0];
   c->cov_unobserved = counts[1];
-  c->cov_lay_next = c->lay; c->cov_basis_next = c->basis; c->cov_L_next = c->L;
-  c->cov_k_next = c->k; c->cov_Nv_next = c->Nv; c->cov_max_rows_next = c->max_rows;
-  c->cov_Kbg_next = c->Kbg; c->cov_Kba_next = c->Kba; c->cov_bias_basis_next = c->bias_basis;
   // the factor outputs are those of an evaluation at the current state; the packed buffer is not what hb200_solve expects
   c->outputs_changed();
   c->evaluated_J = true; c->cov_built = true;
@@ -2130,13 +2167,13 @@ int hb200_build_covariance(hb200_ctx* c) {
 // (Sigma, the status, bad_dof and the pivot are bit-identical across ranks; the degenerate count is the window's), and
 // the landmark kernel runs over the rank's own landmarks and their factors.
 int hb200_compute_covariance(hb200_ctx* c, hb200_covariance_info* info) {
-  int rc = cov_check(c);
-  if (rc) return rc;
+  if (!c) return fail(-1, "null context");
   if (!info) return fail(-1, "null info");
   // every setter that changes shapes, constants or the state clears cov_built; any other launch since the build (an
   // evaluation, an iteration, a slide) rewrote the factor outputs or the packed buffer the compute reads
-  if (!c->cov_built || c->cov_at != c->launches || c->L != c->cov_L_next || c->k != c->cov_k_next || c->Nv != c->cov_Nv_next ||
-      c->max_rows != c->cov_max_rows_next || c->lay.total != c->cov_lay_next.total || c->lay.beta != c->cov_lay_next.beta)
+  const CovPoint& pt = c->cov_pt[c->cov_slot_built];
+  if (!c->cov_built || c->cov_at != c->launches || c->L != pt.L || c->k != pt.k || c->Nv != pt.Nv ||
+      c->max_rows != pt.max_rows || c->lay.total != pt.lay.total || c->lay.beta != pt.lay.beta)
     return fail(-2, "call hb200_build_covariance first (the window was evaluated, iterated or changed since)");
   HB_CUDA(cudaSetDevice(c->device));
   info->status = 0; info->bad_dof = -1; info->min_pivot_ratio = 0.0;
@@ -2145,20 +2182,20 @@ int hb200_compute_covariance(hb200_ctx* c, hb200_covariance_info* info) {
     info->status = 2;
     return fail(HB200_COV_DEGENERATE_LANDMARKS, "covariance: %d landmark(s) with a rank-deficient V_l (observed by too few factors)", c->cov_degenerate);
   }
-  const SysLayout lay = c->cov_lay_next;
+  const SysLayout& lay = pt.lay;
   const size_t smem = cov_smem_doubles(lay.beta, lay.m) * sizeof(double);
   HB_CUDA(c->cov_ws.ensure(static_cast<size_t>(cov_workspace_doubles(lay))));
   HB_CUDA(c->cov_packed_next.ensure(static_cast<size_t>(cov_packed_doubles(lay))));
-  const int L = c->cov_L_next, k = c->cov_k_next, max_rows = c->cov_max_rows_next;   // (the build's shapes)
+  const int L = pt.L, k = pt.k, max_rows = pt.max_rows;   // (the build's shapes)
   HB_CUDA(c->cov_lm_next.ensure(9 * static_cast<size_t>(std::max(L, 1))));
   HB_CUDA(c->cov_status.ensure(1));
   HB_CUDA(cudaFuncSetAttribute(cov_selinv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
   cov_selinv_kernel<<<1, kCovThreads, smem, c->stream>>>(c->sys.p, lay, c->fixed.p, c->cov_ws.p, c->cov_packed_next.p, c->cov_status.p);
   HB_LAUNCH(c, "cov_selinv_kernel");
-  if (L && c->cov_Nv_next) {
+  if (L && pt.Nv) {
     const int blocks = (L + kLmWarps - 1) / kLmWarps;
     const size_t lsmem = static_cast<size_t>(kLmWarps) * 3 * max_rows * sizeof(double);
-    rc = with_order(k, [&](auto K) {
+    const int rc = with_order(k, [&](auto K) {
       cov_landmark_kernel<K><<<blocks, kLmWarps * 32, lsmem, c->stream>>>(L, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p, c->Vchol.p,
                                                                          c->cov_packed_next.p, lay, c->cov_status.p, c->cov_lm_next.p, max_rows);
       return check_launch(c, "cov_landmark_kernel");
@@ -2182,91 +2219,38 @@ int hb200_compute_covariance(hb200_ctx* c, hb200_covariance_info* info) {
   // commit: results, and the linearisation point they belong to
   c->cov_packed.swap(c->cov_packed_next);
   c->cov_lm.swap(c->cov_lm_next);
-  HB_CUDA(c->cov_knots.ensure(8 * static_cast<size_t>(lay.K)));
-  HB_CUDA(c->cov_tab.ensure(static_cast<size_t>(kTabStride) * lay.K));
-  HB_CUDA(cudaMemcpyAsync(c->cov_knots.p, c->cov_knots_next.p, sizeof(double) * 8 * lay.K, cudaMemcpyDeviceToDevice, c->stream));
-  HB_CUDA(cudaMemcpyAsync(c->cov_tab.p, c->cov_tab_next.p, sizeof(double) * kTabStride * lay.K, cudaMemcpyDeviceToDevice, c->stream));
-  const int Kbg = c->cov_Kbg_next, Kba = c->cov_Kba_next;
-  HB_CUDA(c->cov_bg.ensure(4 * static_cast<size_t>(Kbg)));
-  HB_CUDA(c->cov_ba.ensure(4 * static_cast<size_t>(Kba)));
-  if (Kbg) HB_CUDA(cudaMemcpyAsync(c->cov_bg.p, c->cov_bg_next.p, sizeof(double) * 4 * Kbg, cudaMemcpyDeviceToDevice, c->stream));
-  if (Kba) HB_CUDA(cudaMemcpyAsync(c->cov_ba.p, c->cov_ba_next.p, sizeof(double) * 4 * Kba, cudaMemcpyDeviceToDevice, c->stream));
-  HB_CUDA(cudaStreamSynchronize(c->stream));
-  c->cov_lay = lay; c->cov_basis = c->cov_basis_next; c->cov_L = c->cov_L_next;
-  c->cov_Kbg = Kbg; c->cov_Kba = Kba; c->cov_bias_basis = c->cov_bias_basis_next;
+  c->cov_slot_committed = c->cov_slot_built;
   c->cov_valid = true;
   cov_info(c, info);
   return 0;
 }
 
 int hb200_get_covariance(hb200_ctx* c, double* packed, double* landmark) {
-  int rc = cov_check(c);
-  if (rc) return rc;
+  if (!c) return fail(-1, "null context");
   if (!c->cov_valid) return fail(-2, "no covariance computed (hb200_compute_covariance has not succeeded)");
   HB_CUDA(cudaSetDevice(c->device));
-  if (packed) HB_CUDA(cudaMemcpyAsync(packed, c->cov_packed.p, sizeof(double) * cov_packed_doubles(c->cov_lay), cudaMemcpyDeviceToHost, c->stream));
-  if (landmark && c->cov_L) HB_CUDA(cudaMemcpyAsync(landmark, c->cov_lm.p, sizeof(double) * 9 * c->cov_L, cudaMemcpyDeviceToHost, c->stream));
+  const CovPoint& pt = c->cov_pt[c->cov_slot_committed];
+  if (packed) HB_CUDA(cudaMemcpyAsync(packed, c->cov_packed.p, sizeof(double) * cov_packed_doubles(pt.lay), cudaMemcpyDeviceToHost, c->stream));
+  if (landmark && pt.L) HB_CUDA(cudaMemcpyAsync(landmark, c->cov_lm.p, sizeof(double) * 9 * pt.L, cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
   return 0;
 }
 
 int hb200_interpolate_covariance(hb200_ctx* c, int n, const double* stamps, double* cov, int* num_invalid) {
-  int rc = cov_check(c);
-  if (rc) return rc;
-  if (n < 0 || (n > 0 && (!stamps || !cov))) return fail(-1, "invalid argument");
-  if (!c->cov_valid) return fail(-2, "no covariance computed (hb200_compute_covariance has not succeeded)");
-  HB_CUDA(cudaSetDevice(c->device));
-  if (num_invalid) *num_invalid = 0;
-  if (n == 0) return 0;
-  const bool stamp = c->cov_built && c->cov_at == c->launches;   // (reads nothing a compute needs)
-  DevBuf<double>& d_t = c->cov_t;
-  DevBuf<double>& d_o = c->cov_o;
-  DevBuf<int>& d_bad = c->cov_bad;
-  HB_CUDA(d_t.ensure(n)); HB_CUDA(d_o.ensure(36 * static_cast<size_t>(n))); HB_CUDA(d_bad.ensure(n));
-  HB_CUDA(cudaMemcpyAsync(d_t.p, stamps, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
-  const SysLayout& lay = c->cov_lay;
-  rc = with_order(c->cov_basis.k, [&](auto K) {
-    cov_interpolate_kernel<K><<<(n + 127) / 128, 128, 0, c->stream>>>(n, d_t.p, c->cov_knots.p, c->cov_tab.p, lay.K, c->cov_basis, c->cov_packed.p, lay, d_o.p, d_bad.p);
+  return cov_interpolate(c, n, stamps, cov, num_invalid, 36, [&](auto K, const CovPoint& pt) {
+    cov_interpolate_kernel<K><<<(n + 127) / 128, 128, 0, c->stream>>>(n, c->cov_t.p, pt.knots.p, pt.tab.p, pt.lay.K, pt.basis, c->cov_packed.p, pt.lay,
+                                                                     c->cov_o.p, c->cov_bad.p);
     return check_launch(c, "cov_interpolate_kernel");
   });
-  if (rc) return rc;
-  std::vector<int> bad(n);
-  HB_CUDA(cudaMemcpyAsync(cov, d_o.p, sizeof(double) * 36 * n, cudaMemcpyDeviceToHost, c->stream));
-  HB_CUDA(cudaMemcpyAsync(bad.data(), d_bad.p, sizeof(int) * n, cudaMemcpyDeviceToHost, c->stream));
-  HB_CUDA(cudaStreamSynchronize(c->stream));
-  if (num_invalid) *num_invalid = std::accumulate(bad.begin(), bad.end(), 0);
-  if (stamp) c->cov_at = c->launches;
-  return 0;
 }
 
 int hb200_interpolate_state_covariance(hb200_ctx* c, int n, const double* stamps, double* cov, int* num_invalid) {
-  int rc = cov_check(c);
-  if (rc) return rc;
-  if (n < 0 || (n > 0 && (!stamps || !cov))) return fail(-1, "invalid argument");
-  if (!c->cov_valid) return fail(-2, "no covariance computed (hb200_compute_covariance has not succeeded)");
-  HB_CUDA(cudaSetDevice(c->device));
-  if (num_invalid) *num_invalid = 0;
-  if (n == 0) return 0;
-  const bool stamp = c->cov_built && c->cov_at == c->launches;   // (reads nothing a compute needs)
-  constexpr size_t D2 = HB200_STATE_COV_DIM * HB200_STATE_COV_DIM;
   static_assert(HB200_STATE_COV_DIM == kStateDim, "state covariance dimension");
-  HB_CUDA(c->cov_t.ensure(n)); HB_CUDA(c->cov_o.ensure(D2 * n)); HB_CUDA(c->cov_bad.ensure(n));
-  HB_CUDA(cudaMemcpyAsync(c->cov_t.p, stamps, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
-  const SysLayout& lay = c->cov_lay;
-  rc = with_order(c->cov_basis.k, [&](auto K) {
+  return cov_interpolate(c, n, stamps, cov, num_invalid, HB200_STATE_COV_DIM * HB200_STATE_COV_DIM, [&](auto K, const CovPoint& pt) {
     cov_state_interpolate_kernel<K><<<(n + kStateWarps - 1) / kStateWarps, kStateWarps * 32, 0, c->stream>>>(
-        n, c->cov_t.p, c->cov_knots.p, c->cov_tab.p, lay.K, c->cov_basis, c->cov_bg.p, c->cov_Kbg, c->cov_ba.p, c->cov_Kba, c->cov_bias_basis,
-        c->cov_packed.p, lay, c->cov_o.p, c->cov_bad.p);
+        n, c->cov_t.p, pt.knots.p, pt.tab.p, pt.lay.K, pt.basis, pt.bg.p, pt.Kbg, pt.ba.p, pt.Kba, pt.bias_basis, c->cov_packed.p, pt.lay, c->cov_o.p, c->cov_bad.p);
     return check_launch(c, "cov_state_interpolate_kernel");
   });
-  if (rc) return rc;
-  std::vector<int> bad(n);
-  HB_CUDA(cudaMemcpyAsync(cov, c->cov_o.p, sizeof(double) * D2 * n, cudaMemcpyDeviceToHost, c->stream));
-  HB_CUDA(cudaMemcpyAsync(bad.data(), c->cov_bad.p, sizeof(int) * n, cudaMemcpyDeviceToHost, c->stream));
-  HB_CUDA(cudaStreamSynchronize(c->stream));
-  if (num_invalid) *num_invalid = std::accumulate(bad.begin(), bad.end(), 0);
-  if (stamp) c->cov_at = c->launches;
-  return 0;
 }
 
 }  // extern "C"

@@ -10,7 +10,10 @@ hb200_get_covariance / hb200_interpolate_covariance against tests/covref.py.
   the kernels that ran (schur_group_kernel on the K = 500 window with 8192 landmarks);
 * a build made stale by a change of the window (landmarks, an evaluation, constants) is refused with -2;
 * failures (gauge not fixed, biases without IMU factors, a single-observation landmark) are reported with finite outputs
-  and leave the previous results in place; an unobserved landmark gets a zero block;
+  and leave the previous results in place (packed, landmark blocks and both interpolations, bit for bit); an unobserved
+  landmark gets a zero block;
+* the linearisation point of a build is committed only by a successful compute: a repeated compute, failed computes and
+  a return to an earlier window give every reader what it should see (deterministic assembly, bit for bit);
 * the interpolated pose covariance equals J(t) Sigma J(t)^T of covref within 1e-11 in the correlation metric, also where
   the knot increments straddle the small-angle switches of the SO(3) coefficients;
 * the LM path is untouched: iterate() with a covariance computed in between differs from a plain run by no more than
@@ -341,26 +344,48 @@ def test_stale_build_is_refused(built, record_property):
 
 
 # ---- failures ---------------------------------------------------------------------------------------------------------
+def failure_window(pose=10):
+    return e2e_window(4, num_knots=30, num_landmarks=200, num_imu=800, bearing=100, pose=pose, seed=31)
+
+
+def gauge_free_window():
+    """No constant knots, no pose factors (yaw and translation free): the compute fails with status 1."""
+    win = failure_window(pose=0)
+    win.knot_const = cr.untouched_knots(win).astype(np.uint8)
+    return win
+
+
+def readers(ctx, stamps):
+    """Everything a reader sees of the committed covariance: packed Sigma, landmark blocks, both interpolations."""
+    packed, lm, _ = ctx.covariance_packed()
+    pose, bad_pose = ctx.interpolate_covariance(stamps)
+    state, bad_state = ctx.interpolate_state_covariance(stamps)
+    return packed, lm, pose, state, bad_pose, bad_state
+
+
+def assert_same_readers(a, b):
+    """Bit for bit."""
+    for x, y in zip(a[:4], b[:4]):
+        assert x.shape == y.shape and np.array_equal(x.view(np.int64), y.view(np.int64))
+    assert a[4:] == b[4:]
+
+
 def test_failures_keep_previous_results(built, record_property):
-    good = e2e_window(4, num_knots=30, num_landmarks=200, num_imu=800, bearing=100, pose=10, seed=31)
+    good = failure_window()
+    stamps = good.knots[6:20, 7] + 0.013
     ctx = runtime.Context(0)
     try:
         ctx.load_window(good)
         ctx.build_covariance()
         info0 = ctx.compute_covariance()
         assert info0["status"] == 0
-        keep = ctx.covariance_packed()
+        keep = readers(ctx, stamps)
         record_property("accepted_min_pivot", info0["min_pivot_ratio"])
 
         def same_as_before():
-            now = ctx.covariance_packed()
-            assert np.array_equal(now[0], keep[0]) and np.array_equal(now[1], keep[1])
+            assert_same_readers(readers(ctx, stamps), keep)
 
-        # gauge not fixed: no constant knots, no pose factors (yaw and translation free)
-        nogauge = e2e_window(4, num_knots=30, num_landmarks=200, num_imu=800, bearing=100, pose=0, seed=31)
-        kc = cr.untouched_knots(nogauge).astype(np.uint8)
-        nogauge.knot_const = kc
-        ctx.load_window(nogauge)
+        ctx.load_window(gauge_free_window())
         ctx.build_covariance()
         info = ctx.compute_covariance()
         record_property("gauge_free_pivot", info["min_pivot_ratio"])
@@ -404,6 +429,53 @@ def test_failures_keep_previous_results(built, record_property):
         assert np.all(lm[5] == 0) and np.isfinite(lm).all() and (np.abs(lm[[4, 6]]) > 0).all()
     finally:
         ctx.close()
+
+
+def test_linearisation_point_slots(built):
+    """A build freezes its linearisation point beside the committed one and only a successful compute commits it:
+    window A, then B (A after two iterations) computed twice, two failed build + compute rounds, and A again, which must
+    equal a fresh context's A.  Deterministic assembly, so every comparison is bit for bit."""
+    win_a = failure_window()
+    stamps = win_a.knots[6:20, 7] + 0.013
+
+    def computed(ctx):
+        ctx.build_covariance()
+        info = ctx.compute_covariance()
+        assert info["status"] == 0, info
+        return info
+
+    ctx = runtime.Context(0)
+    try:
+        ctx.set_deterministic(True)
+        ctx.load_window(win_a)
+        computed(ctx)
+        at_a = readers(ctx, stamps)
+        ctx.iterate(2)
+        info_b = computed(ctx)
+        at_b = readers(ctx, stamps)
+        assert not np.array_equal(at_b[0], at_a[0]) and not np.array_equal(at_b[3], at_a[3])
+        assert ctx.compute_covariance() == info_b            # no build in between: the same point again
+        assert_same_readers(readers(ctx, stamps), at_b)
+        ctx.load_window(gauge_free_window())
+        for _ in range(2):
+            ctx.build_covariance()
+            info = ctx.compute_covariance()
+            assert info["status"] == 1, info
+            assert [info[k] for k in ("K", "beta", "m", "L")] == [info_b[k] for k in ("K", "beta", "m", "L")]
+            assert_same_readers(readers(ctx, stamps), at_b)
+        ctx.load_window(win_a)
+        info_a = computed(ctx)
+        again = readers(ctx, stamps)
+    finally:
+        ctx.close()
+    fresh = runtime.Context(0)
+    try:
+        fresh.set_deterministic(True)
+        fresh.load_window(win_a)
+        assert computed(fresh) == info_a
+        assert_same_readers(again, readers(fresh, stamps))
+    finally:
+        fresh.close()
 
 
 # ---- the LM path is untouched -----------------------------------------------------------------------------------------
