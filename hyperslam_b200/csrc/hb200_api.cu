@@ -292,6 +292,14 @@ struct hb200_ctx {
   int cov_slot_built = 0, cov_slot_committed = 0;
   DevBuf<double> cov_t, cov_o;   // hb200_interpolate_covariance / hb200_interpolate_state_covariance staging
   DevBuf<int> cov_bad;
+  // requested blocks (hb200_set_covariance_blocks): the registered list, its device copy, the landmark spans and the
+  // far-column plan and scratch of a compute; cov_blk / cov_blk_st (cov_blk_n of them) are the committed blocks
+  std::vector<int4> cov_req;
+  DevBuf<int4> cov_req_d;
+  DevBuf<int2> cov_span;
+  DevBuf<int> cov_plan, cov_blk_st, cov_blk_st_next;
+  DevBuf<double> cov_far, cov_blk, cov_blk_next;
+  int cov_blk_n = 0;
 
   hb200_allreduce_fn allreduce = nullptr;
   void* allreduce_user = nullptr;
@@ -2103,6 +2111,88 @@ int cov_interpolate(hb200_ctx* c, int n, const double* stamps, double* cov, int*
   if (stamp) c->cov_at = c->launches;
   return 0;
 }
+
+// A registered request against the build's shapes.
+bool cov_request_ok(const int4& r, const CovPoint& pt) {
+  auto ok = [&](int kind, int i) {
+    switch (kind) {
+      case kCovKnot: return i >= 0 && i < pt.lay.K;
+      case kCovGyroBias: return i >= 0 && i < pt.Kbg;
+      case kCovAccelBias: return i >= 0 && i < pt.Kba;
+      case kCovGravity: return i == 0;
+      case kCovLandmark: return i >= 0 && i < pt.L;
+      default: return false;
+    }
+  };
+  return ok(r.x, r.y) && ok(r.z, r.w);
+}
+
+// The requested blocks of a compute, after cov_landmark_kernel: the landmarks' control-point spans (one read-back, only
+// when a request has a landmark), the far-column plan -- for every knot pair more than beta blocks apart that a request
+// reads, directly or through a landmark's span, its column (the larger block) and the lowest row the march must reach --
+// then cov_far_column_kernel over the planned columns and cov_cross_landmark_kernel over the requests, into *_next.
+int cov_blocks_enqueue(hb200_ctx* c, const CovPoint& pt) {
+  const SysLayout& lay = pt.lay;
+  const int n = static_cast<int>(c->cov_req.size()), K = lay.K, beta = lay.beta;
+  HB_CUDA(c->cov_req_d.ensure(n));
+  HB_CUDA(cudaMemcpyAsync(c->cov_req_d.p, c->cov_req.data(), sizeof(int4) * n, cudaMemcpyHostToDevice, c->stream));
+  std::vector<int2> span(2 * static_cast<size_t>(n), make_int2(-1, -1));
+  const bool landmarks = pt.Nv && std::any_of(c->cov_req.begin(), c->cov_req.end(), [](const int4& r) { return r.x == kCovLandmark || r.z == kCovLandmark; });
+  if (landmarks) {
+    HB_CUDA(c->cov_span.ensure(2 * static_cast<size_t>(n)));
+    cov_landmark_span_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(n, c->cov_req_d.p, c->lm_off.p, c->lm_obs.p, c->v_idx.p, pt.k, c->cov_span.p);
+    HB_LAUNCH(c, "cov_landmark_span_kernel");
+    HB_CUDA(cudaMemcpyAsync(span.data(), c->cov_span.p, sizeof(int2) * 2 * n, cudaMemcpyDeviceToHost, c->stream));
+    HB_CUDA(cudaStreamSynchronize(c->stream));
+  }
+  std::vector<int> need(K, K);   // lowest row block per column block (K: none)
+  auto far = [&](int r, int s) {
+    if (std::abs(r - s) > beta) need[std::max(r, s)] = std::min(need[std::max(r, s)], std::min(r, s));
+  };
+  for (int q = 0; q < n; ++q) {
+    const int4& r = c->cov_req[q];
+    // each side as a knot range [first, end): a knot, a landmark's span; nothing for bias / gravity / unobserved
+    int lo[2] = {0, 0}, hi[2] = {0, 0};
+    const int kind[2] = {r.x, r.z}, index[2] = {r.y, r.w};
+    for (int s = 0; s < 2; ++s) {
+      if (kind[s] == kCovKnot) { lo[s] = index[s]; hi[s] = index[s] + 1; }
+      else if (kind[s] == kCovLandmark && span[2 * q + s].x >= 0) { lo[s] = span[2 * q + s].x; hi[s] = span[2 * q + s].y; }
+    }
+    if (kind[0] == kCovLandmark && kind[1] == kCovLandmark && index[0] == index[1]) continue;   // the marginal
+    for (int a = lo[0]; a < hi[0]; ++a)
+      for (int b = lo[1]; b < hi[1]; ++b) far(a, b);
+  }
+  std::vector<int> plan(K, -1);
+  int nc = 0, blocks = 0;
+  for (int j = 0; j < K; ++j)
+    if (need[j] < K) { plan[j] = nc++; }
+  plan.resize(K + 3 * static_cast<size_t>(nc));
+  for (int j = 0; j < K; ++j)
+    if (need[j] < K) {
+      const int s = plan[j];
+      plan[K + s] = j; plan[K + nc + s] = need[j]; plan[K + 2 * nc + s] = blocks;
+      blocks += j - beta - need[j];
+    }
+  HB_CUDA(c->cov_plan.ensure(plan.size()));
+  HB_CUDA(cudaMemcpyAsync(c->cov_plan.p, plan.data(), sizeof(int) * plan.size(), cudaMemcpyHostToDevice, c->stream));
+  HB_CUDA(c->cov_far.ensure(36 * static_cast<size_t>(blocks)));
+  HB_CUDA(c->cov_blk_next.ensure(36 * static_cast<size_t>(n)));
+  HB_CUDA(c->cov_blk_st_next.ensure(n));
+  const CovFarPlan fp{c->cov_plan.p, nc};
+  if (nc) {
+    const size_t smem = (36 * static_cast<size_t>(beta) + 6 * lay.m + 36) * sizeof(double);
+    cov_far_column_kernel<<<nc, kFarThreads, smem, c->stream>>>(c->cov_ws.p, c->cov_packed_next.p, lay, c->fixed.p, fp, c->cov_status.p, c->cov_far.p);
+    HB_LAUNCH(c, "cov_far_column_kernel");
+  }
+  const size_t smem = static_cast<size_t>(kLmWarps) * 6 * pt.max_rows * sizeof(double);
+  return with_order(pt.k, [&](auto Kc) {
+    HB_CUDA(cudaFuncSetAttribute(cov_cross_landmark_kernel<Kc>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+    cov_cross_landmark_kernel<Kc><<<(n + kLmWarps - 1) / kLmWarps, kLmWarps * 32, smem, c->stream>>>(
+        n, c->cov_req_d.p, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p, c->Vchol.p, c->cov_packed_next.p, c->cov_lm_next.p,
+        c->cov_far.p, fp, lay, pt.Kbg, c->multi() ? 1 : 0, c->cov_status.p, pt.max_rows, c->cov_blk_next.p, c->cov_blk_st_next.p);
+    return check_launch(c, "cov_cross_landmark_kernel");
+  });
+}
 }  // namespace
 
 extern "C" {
@@ -2182,6 +2272,10 @@ int hb200_compute_covariance(hb200_ctx* c, hb200_covariance_info* info) {
     info->status = 2;
     return fail(HB200_COV_DEGENERATE_LANDMARKS, "covariance: %d landmark(s) with a rank-deficient V_l (observed by too few factors)", c->cov_degenerate);
   }
+  for (size_t q = 0; q < c->cov_req.size(); ++q)
+    if (!cov_request_ok(c->cov_req[q], pt))
+      return fail(-1, "covariance block %zu: (kind %d, index %d) x (kind %d, index %d) is not a block of the built window", q, c->cov_req[q].x,
+                  c->cov_req[q].y, c->cov_req[q].z, c->cov_req[q].w);
   const SysLayout& lay = pt.lay;
   const size_t smem = cov_smem_doubles(lay.beta, lay.m) * sizeof(double);
   HB_CUDA(c->cov_ws.ensure(static_cast<size_t>(cov_workspace_doubles(lay))));
@@ -2204,6 +2298,10 @@ int hb200_compute_covariance(hb200_ctx* c, hb200_covariance_info* info) {
   } else if (L) {
     HB_CUDA(cudaMemsetAsync(c->cov_lm_next.p, 0, sizeof(double) * 9 * L, c->stream));
   }
+  // requested blocks: the landmark blocks need the build's factor outputs and the far columns the factor in cov_ws,
+  // both valid only until the next launch, so they are computed here (nothing runs without a request)
+  if (!c->cov_req.empty())
+    if (const int rc = cov_blocks_enqueue(c, pt)) return rc;
   CovStatus st{};
   HB_CUDA(cudaMemcpyAsync(&st, c->cov_status.p, sizeof(st), cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
@@ -2219,9 +2317,36 @@ int hb200_compute_covariance(hb200_ctx* c, hb200_covariance_info* info) {
   // commit: results, and the linearisation point they belong to
   c->cov_packed.swap(c->cov_packed_next);
   c->cov_lm.swap(c->cov_lm_next);
+  c->cov_blk.swap(c->cov_blk_next);
+  c->cov_blk_st.swap(c->cov_blk_st_next);
+  c->cov_blk_n = static_cast<int>(c->cov_req.size());
   c->cov_slot_committed = c->cov_slot_built;
   c->cov_valid = true;
   cov_info(c, info);
+  return 0;
+}
+
+int hb200_set_covariance_blocks(hb200_ctx* c, int n, const int* pairs) {
+  if (!c) return fail(-1, "null context");
+  static_assert(+HB200_COV_KNOT == +kCovKnot && +HB200_COV_GYRO_BIAS == +kCovGyroBias && +HB200_COV_ACCEL_BIAS == +kCovAccelBias &&
+                    +HB200_COV_GRAVITY == +kCovGravity && +HB200_COV_LANDMARK == +kCovLandmark,
+                "covariance block kinds");
+  if (n < 0 || (n > 0 && !pairs)) return fail(-1, "invalid argument");
+  c->cov_req.resize(n);
+  for (int q = 0; q < n; ++q) c->cov_req[q] = make_int4(pairs[4 * q], pairs[4 * q + 1], pairs[4 * q + 2], pairs[4 * q + 3]);
+  return 0;
+}
+
+int hb200_get_covariance_blocks(hb200_ctx* c, int n, double* out, int* status) {
+  if (!c) return fail(-1, "null context");
+  if (n < 0 || (n > 0 && !out)) return fail(-1, "invalid argument");
+  if (!c->cov_valid) return fail(-2, "no covariance computed (hb200_compute_covariance has not succeeded)");
+  if (n != c->cov_blk_n) return fail(-2, "the last successful compute had %d covariance blocks, not %d", c->cov_blk_n, n);
+  if (n == 0) return 0;
+  HB_CUDA(cudaSetDevice(c->device));
+  HB_CUDA(cudaMemcpyAsync(out, c->cov_blk.p, sizeof(double) * 36 * n, cudaMemcpyDeviceToHost, c->stream));
+  if (status) HB_CUDA(cudaMemcpyAsync(status, c->cov_blk_st.p, sizeof(int) * n, cudaMemcpyDeviceToHost, c->stream));
+  HB_CUDA(cudaStreamSynchronize(c->stream));
   return 0;
 }
 

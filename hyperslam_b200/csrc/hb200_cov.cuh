@@ -6,7 +6,9 @@
 //   cov_selinv_kernel     the entries of S^-1 on the block band, the arrow and the corner (selected inversion);
 //   cov_landmark_kernel   the 3 x 3 marginal of every landmark, Sigma_ll = L^-T (I + Y^T Sigma_pp Y) L^-1;
 //   cov_interpolate_kernel the 6 x 6 covariance of the interpolated pose at arbitrary stamps, J(t) Sigma J(t)^T;
-//   cov_state_interpolate_kernel the 18 x 18 joint covariance of pose, body velocity and IMU biases at arbitrary stamps.
+//   cov_state_interpolate_kernel the 18 x 18 joint covariance of pose, body velocity and IMU biases at arbitrary stamps;
+//   cov_far_column_kernel / cov_cross_landmark_kernel the requested blocks outside the pattern (ceres::Covariance::Compute's
+//                         list): knot pairs beyond the band and landmark cross-covariances.
 // All are deterministic: no atomics, every sum in a fixed order.
 #pragma once
 #include "hb200_solve.cuh"
@@ -348,26 +350,17 @@ __global__ void __launch_bounds__(kCovThreads) cov_selinv_kernel(const double* _
 // Unobserved landmarks get a zero block.  Nothing runs when the selected inversion failed.
 // Dynamic shared memory: kLmWarps * 3 * max_rows doubles.
 // ---------------------------------------------------------------------------------------------
+// Y = W L^-T of an observed landmark into the warp's buffer Y (rows x 3, rows = 6 x its control-point span; the
+// observations' first control points are ascending) and its packed factor into F.  Returns the span's first control point.
 template <int K>
-__global__ void __launch_bounds__(kLmWarps * 32) cov_landmark_kernel(int L, const int* __restrict__ lm_off, const int* __restrict__ lm_obs,
-                                                                     const int4* __restrict__ idx, const double* __restrict__ Jp,
-                                                                     const double* __restrict__ Jl, const double* __restrict__ wv,
-                                                                     const double* __restrict__ Vchol, const double* __restrict__ cov, SysLayout lay,
-                                                                     const CovStatus* __restrict__ status, double* __restrict__ out, int max_rows) {
+HB_DI int cov_landmark_Y(int o_lo, int o_hi, const int* __restrict__ lm_obs, const int4* __restrict__ idx, const double* __restrict__ Jp,
+                         const double* __restrict__ Jl, const double* __restrict__ wv, const double* __restrict__ Vl, double* Y, int* rows_out,
+                         double* F) {
   constexpr int NB = 6 * K;
-  extern __shared__ double s_lw[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int l = blockIdx.x * kLmWarps + warp;
-  if (status->status != 0 || l >= L) return;
-  double* Y = s_lw + static_cast<size_t>(warp) * 3 * max_rows;
-  double* o = out + 9 * static_cast<size_t>(l);
-  const int o_lo = lm_off[l], o_hi = lm_off[l + 1];
-  if (o_lo >= o_hi) {
-    if (lane < 9) o[lane] = 0.0;
-    return;
-  }
+  const int lane = threadIdx.x & 31;
   const int cp_lo = idx[lm_obs[o_lo]].x, cp_hi = idx[lm_obs[o_hi - 1]].x + K;
   const int rows = 6 * (cp_hi - cp_lo);
+  *rows_out = rows;
   for (int e = lane; e < 3 * rows; e += 32) Y[e] = 0.0;
   __syncwarp();
   for (int ob = o_lo; ob < o_hi; ++ob) {
@@ -385,15 +378,45 @@ __global__ void __launch_bounds__(kLmWarps * 32) cov_landmark_kernel(int L, cons
     }
     __syncwarp();
   }
-  double F[6];
 #pragma unroll
-  for (int i = 0; i < 6; ++i) F[i] = Vchol[9 * static_cast<size_t>(l) + i];
+  for (int i = 0; i < 6; ++i) F[i] = Vl[i];
   for (int r = lane; r < rows; r += 32) {
     double y[3];
     lm_lsolve(F, Y[3 * r], Y[3 * r + 1], Y[3 * r + 2], y);
     Y[3 * r] = y[0]; Y[3 * r + 1] = y[1]; Y[3 * r + 2] = y[2];
   }
   __syncwarp();
+  return cp_lo;
+}
+
+// L^-1 (row-major 3 x 3, lower) of a packed landmark factor, columns L^-1 e_c
+HB_DI void cov_landmark_Linv(const double* F, double* Li) {
+  double y[3];
+  lm_lsolve(F, 1.0, 0.0, 0.0, y); Li[0] = y[0]; Li[3] = y[1]; Li[6] = y[2];
+  lm_lsolve(F, 0.0, 1.0, 0.0, y); Li[1] = y[0]; Li[4] = y[1]; Li[7] = y[2];
+  lm_lsolve(F, 0.0, 0.0, 1.0, y); Li[2] = y[0]; Li[5] = y[1]; Li[8] = y[2];
+}
+
+template <int K>
+__global__ void __launch_bounds__(kLmWarps * 32) cov_landmark_kernel(int L, const int* __restrict__ lm_off, const int* __restrict__ lm_obs,
+                                                                     const int4* __restrict__ idx, const double* __restrict__ Jp,
+                                                                     const double* __restrict__ Jl, const double* __restrict__ wv,
+                                                                     const double* __restrict__ Vchol, const double* __restrict__ cov, SysLayout lay,
+                                                                     const CovStatus* __restrict__ status, double* __restrict__ out, int max_rows) {
+  extern __shared__ double s_lw[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int l = blockIdx.x * kLmWarps + warp;
+  if (status->status != 0 || l >= L) return;
+  double* Y = s_lw + static_cast<size_t>(warp) * 3 * max_rows;
+  double* o = out + 9 * static_cast<size_t>(l);
+  const int o_lo = lm_off[l], o_hi = lm_off[l + 1];
+  if (o_lo >= o_hi) {
+    if (lane < 9) o[lane] = 0.0;
+    return;
+  }
+  double F[6];
+  int rows;
+  const int cp_lo = cov_landmark_Y<K>(o_lo, o_hi, lm_obs, idx, Jp, Jl, wv, Vchol + 9 * static_cast<size_t>(l), Y, &rows, F);
   double M[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
   const int g0 = 6 * cp_lo;
   for (int r = lane; r < rows; r += 32) {
@@ -414,11 +437,8 @@ __global__ void __launch_bounds__(kLmWarps * 32) cov_landmark_kernel(int L, cons
 #pragma unroll
     for (int x = 16; x > 0; x >>= 1) M[i] += __shfl_xor_sync(0xffffffffu, M[i], x);
   if (lane == 0) {
-    // L^-1 (lower), columns L^-1 e_c
-    double Li[9], y[3];
-    lm_lsolve(F, 1.0, 0.0, 0.0, y); Li[0] = y[0]; Li[3] = y[1]; Li[6] = y[2];
-    lm_lsolve(F, 0.0, 1.0, 0.0, y); Li[1] = y[0]; Li[4] = y[1]; Li[7] = y[2];
-    lm_lsolve(F, 0.0, 0.0, 1.0, y); Li[2] = y[0]; Li[5] = y[1]; Li[8] = y[2];
+    double Li[9];
+    cov_landmark_Linv(F, Li);
     double A[9], T[9];
 #pragma unroll
     for (int i = 0; i < 9; ++i) A[i] = 0.5 * (M[i] + M[3 * (i % 3) + i / 3]) + ((i % 4 == 0) ? 1.0 : 0.0);
@@ -427,6 +447,255 @@ __global__ void __launch_bounds__(kLmWarps * 32) cov_landmark_kernel(int L, cons
     m3_tmul(Li, T, S);       // L^-T (I + M) L^-1
 #pragma unroll
     for (int i = 0; i < 9; ++i) o[i] = 0.5 * (S[i] + S[3 * (i % 3) + i / 3]);
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Covariance blocks outside the selected inverse's pattern (hb200_set_covariance_blocks), computed inside the compute
+// from its factor and its Sigma.  A request is a pair of parameter blocks (kind, index); kinds as HB200_COV_*.
+// ---------------------------------------------------------------------------------------------
+enum { kCovKnot = 0, kCovGyroBias = 1, kCovAccelBias = 2, kCovGravity = 3, kCovLandmark = 4 };
+constexpr int kFarThreads = 64;
+
+// First reduced-system dof and device tangent size of a non-landmark block.
+HB_DI void cov_block_dofs(int kind, int index, const SysLayout& lay, int Kbg, int* dof, int* t) {
+  if (kind == kCovKnot) { *dof = 6 * index; *t = 6; }
+  else if (kind == kCovGyroBias) { *dof = lay.np + 3 * index; *t = 3; }
+  else if (kind == kCovAccelBias) { *dof = lay.np + 3 * Kbg + 3 * index; *t = 3; }
+  else { *dof = lay.n - 2; *t = 2; }
+}
+
+// The far-column plan, one int array: slot[K] (column block -> slot, -1: none), then per slot its column block, its
+// lowest row block lo and its first scratch block; the scratch holds Sigma_ij of rows i = lo .. j - beta - 1 (6 x 6 each,
+// row-major, rows of block i) at block off + (i - lo).
+struct CovFarPlan {
+  const int* p;
+  int nc;
+  HB_DI int slot(int j) const { return p[j]; }
+};
+
+// Sigma entry (ga, gb) of two non-landmark dofs: the packed Sigma inside the band, the arrow and the corner, the far
+// scratch for knot pairs more than beta blocks apart (which the plan covers).
+HB_DI double cov_sigma(const double* __restrict__ cov, const double* __restrict__ far, const CovFarPlan& plan, const SysLayout& lay, int ga, int gb) {
+  const int hi = max(ga, gb), lo = min(ga, gb);
+  if (hi < lay.np) {
+    const int bh = hi / 6, bl = lo / 6;
+    if (bh - bl > lay.beta) {
+      const int s = plan.slot(bh);
+      const int blk = plan.p[lay.K + 2 * plan.nc + s] + (bl - plan.p[lay.K + plan.nc + s]);
+      return far[static_cast<size_t>(blk) * 36 + 6 * (lo - 6 * bl) + (hi - 6 * bh)];
+    }
+  }
+  return cov[sys_index(lay, hi, lo)];
+}
+
+// Control-point span [first, end) of the landmark on each side of every request, (-1, -1) for a non-landmark side or a
+// landmark without observations.  One thread per request.
+__global__ void cov_landmark_span_kernel(int n, const int4* __restrict__ req, const int* __restrict__ lm_off, const int* __restrict__ lm_obs,
+                                         const int4* __restrict__ idx, int k, int2* __restrict__ span) {
+  const int q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= n) return;
+  const int4 r = req[q];
+  const int kind[2] = {r.x, r.z}, index[2] = {r.y, r.w};
+  for (int s = 0; s < 2; ++s) {
+    int2 v = make_int2(-1, -1);
+    if (kind[s] == kCovLandmark) {
+      const int o_lo = lm_off[index[s]], o_hi = lm_off[index[s] + 1];
+      if (o_lo < o_hi) v = make_int2(idx[lm_obs[o_lo]].x, idx[lm_obs[o_hi - 1]].x + k);
+    }
+    span[2 * q + s] = v;
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Knot columns beyond the band, one CTA per planned column block j.  Z = A_hat^-1 (A_hat = D S D) satisfies
+// L^T Z = L^-1, whose column j is zero above block j, so for i < j - beta (L_ki = 0 for k > i + beta):
+//   Z_ij = -L_ii^-T ( sum_{k=i+1..i+beta} L_ki^T Z_kj + L_Ci^T Z_Cj ),
+// with L the factor cov_selinv_kernel left in the workspace.  Seeds: Z_kj (j - beta <= k < j) and the arrow Z_Cj,
+// unscaled from the packed Sigma just computed (constant dofs: Sigma = 0 = Z off the diagonal, and their factor rows
+// and columns are those of the identity).  The CTA marches i down to the plan's lo with a ring of beta blocks in
+// shared memory and writes Sigma_ij = D Z D (constant dofs 0) to the scratch.  Every sum in a fixed order.
+// Dynamic shared memory: 36 beta + 6 m + 36 doubles.
+// ---------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kFarThreads) cov_far_column_kernel(const double* __restrict__ ws, const double* __restrict__ cov, SysLayout lay,
+                                                                     const unsigned char* __restrict__ fixed, CovFarPlan plan,
+                                                                     const CovStatus* __restrict__ status, double* __restrict__ far) {
+  extern __shared__ double s_far[];
+  if (status->status != 0) return;
+  const int beta = lay.beta, m = lay.m, np = lay.np, h = lay.h;
+  const int s = blockIdx.x;
+  const int j = plan.p[lay.K + s], lo = plan.p[lay.K + plan.nc + s], off = plan.p[lay.K + 2 * plan.nc + s];
+  const double* Lf = ws;
+  const double* dv = ws + cov_packed_doubles(lay);
+  double* ring = s_far;            // [beta][6][6]: Z_kj in slot k mod beta
+  double* Zc = ring + 36 * beta;   // [m][6]
+  double* T = Zc + 6 * m;          // [6][6]
+  const int tid = threadIdx.x;
+  for (int e = tid; e < 36 * beta; e += kFarThreads) {
+    const int k = j - beta + e / 36, r = (e % 36) / 6, c = e % 6;
+    const int gi = 6 * k + r, gj = 6 * j + c;
+    ring[36 * (k % beta) + 6 * r + c] = cov[sys_index(lay, gj, gi)] / (dv[gi] * dv[gj]);
+  }
+  for (int e = tid; e < 6 * m; e += kFarThreads) {
+    const int p = e / 6, c = e % 6;
+    Zc[e] = cov[lay.oA + static_cast<size_t>(p) * np + 6 * j + c] / (dv[np + p] * dv[6 * j + c]);
+  }
+  __syncthreads();
+  for (int i = j - beta - 1; i >= lo; --i) {
+    const size_t col = static_cast<size_t>(i) * h * 6;   // column block i of the factor: row q of block k at (6 (k - i) + q) * 6
+    if (tid < 36) {
+      const int r = tid / 6, c = tid % 6;
+      double t = 0.0;
+      for (int k = i + 1; k <= i + beta; ++k) {
+        const double* Lk = Lf + col + 36 * (k - i);
+        const double* Zk = ring + 36 * (k % beta);
+#pragma unroll
+        for (int q = 0; q < 6; ++q) t += Lk[6 * q + r] * Zk[6 * q + c];
+      }
+      const double* LC = Lf + lay.oA + 6 * i + r;
+      for (int p = 0; p < m; ++p) t += LC[static_cast<size_t>(p) * np] * Zc[6 * p + c];
+      T[tid] = t;
+    }
+    __syncthreads();
+    if (tid < 6) {   // Z_ij = -L_ii^-T T, one column per thread (L_ii^T is upper triangular)
+      const double* Li = Lf + col;
+      double x[6];
+#pragma unroll
+      for (int r = 5; r >= 0; --r) {
+        double v = T[6 * r + tid];
+#pragma unroll
+        for (int q = r + 1; q < 6; ++q) v -= Li[6 * q + r] * x[q];
+        x[r] = v / Li[6 * r + r];
+      }
+      double* Zi = ring + 36 * (i % beta);
+#pragma unroll
+      for (int r = 0; r < 6; ++r) Zi[6 * r + tid] = -x[r];
+    }
+    __syncthreads();
+    if (tid < 36) {
+      const int gi = 6 * i + tid / 6, gj = 6 * j + tid % 6;
+      const double v = ring[36 * (i % beta) + tid];
+      far[(static_cast<size_t>(off) + (i - lo)) * 36 + tid] = (fixed[gi] || fixed[gj]) ? 0.0 : dv[gi] * v * dv[gj];
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
+// The requested blocks, one warp per request, written as t_a x t_b (row-major) into the top-left of a 6 x 6 slot, the
+// rest 0.  A request is taken in a canonical order -- a landmark first, the smaller landmark index first -- and written
+// transposed when it was given the other way round, so (b, a) is exactly the transpose of (a, b).
+//   non-landmark pairs: gathered from the packed Sigma (in the pattern: bit for bit) or the far scratch;
+//   landmark l with itself: its marginal, bit for bit;
+//   landmark l x knot / bias / gravity q: Sigma_lq = -V_l^-1 W_l^T Sigma_{span(l), q} = -L_l^-T Y_l^T Sigma_{span(l), q};
+//   landmarks l != m: Sigma_lm = V_l^-1 W_l^T Sigma_{span(l), span(m)} W_m V_m^-1 = L_l^-T Y_l^T Sigma Y_m L_m^-1;
+// with W_l, Y_l = W_l L_l^-T and the undamped factor V_l = L_l L_l^T of the build (cov_landmark_Y).  A landmark
+// without observations gives a zero block and status 2, or 1 on a sharded context (its observations are on its owner).
+// Lane sums are combined by a fixed butterfly.  Dynamic shared memory: kLmWarps * 6 * max_rows doubles.
+// ---------------------------------------------------------------------------------------------
+template <int K>
+__global__ void __launch_bounds__(kLmWarps * 32) cov_cross_landmark_kernel(
+    int n, const int4* __restrict__ req, const int* __restrict__ lm_off, const int* __restrict__ lm_obs, const int4* __restrict__ idx,
+    const double* __restrict__ Jp, const double* __restrict__ Jl, const double* __restrict__ wv, const double* __restrict__ Vchol,
+    const double* __restrict__ cov, const double* __restrict__ lmcov, const double* __restrict__ far, CovFarPlan plan, SysLayout lay, int Kbg,
+    int sharded, const CovStatus* __restrict__ status, int max_rows, double* __restrict__ out, int* __restrict__ out_status) {
+  extern __shared__ double s_cw[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int q = blockIdx.x * kLmWarps + warp;
+  if (status->status != 0 || q >= n) return;
+  double* o = out + 36 * static_cast<size_t>(q);
+  const int4 r = req[q];
+  int ka = r.x, ia = r.y, kb = r.z, ib = r.w;
+  if (ka != kCovLandmark && kb != kCovLandmark) {
+    int ga, ta, gb, tb;
+    cov_block_dofs(ka, ia, lay, Kbg, &ga, &ta);
+    cov_block_dofs(kb, ib, lay, Kbg, &gb, &tb);
+    for (int e = lane; e < 36; e += 32) {
+      const int a = e / 6, b = e % 6;
+      o[e] = (a < ta && b < tb) ? cov_sigma(cov, far, plan, lay, ga + a, gb + b) : 0.0;
+    }
+    if (lane == 0) out_status[q] = 0;
+    return;
+  }
+  const bool swap = ka != kCovLandmark || (kb == kCovLandmark && ib < ia);
+  if (swap) { const int k0 = ka, i0 = ia; ka = kb; ia = ib; kb = k0; ib = i0; }
+  // canonical: a is landmark ia; b is landmark ib or block (gb, tb)
+  const bool pair = kb == kCovLandmark;
+  const int oa_lo = lm_off[ia], oa_hi = lm_off[ia + 1];
+  const int ob_lo = pair ? lm_off[ib] : 0, ob_hi = pair ? lm_off[ib + 1] : 1;
+  double R[18];   // canonical block, 3 x tb (row stride 6)
+#pragma unroll
+  for (int i = 0; i < 18; ++i) R[i] = 0.0;
+  int tb = 3, st = 0;
+  if (oa_lo >= oa_hi || ob_lo >= ob_hi) {
+    st = sharded ? 1 : 2;
+    if (!pair) { int gb; cov_block_dofs(kb, ib, lay, Kbg, &gb, &tb); }
+  } else if (pair && ia == ib) {
+#pragma unroll
+    for (int i = 0; i < 9; ++i) R[6 * (i / 3) + i % 3] = lmcov[9 * static_cast<size_t>(ia) + i];
+  } else {
+    double* Ya = s_cw + static_cast<size_t>(warp) * 6 * max_rows;
+    double* Yb = Ya + 3 * max_rows;
+    double Fa[6], Fb[6];
+    int rows_a, rows_b = 0;
+    const int ga0 = 6 * cov_landmark_Y<K>(oa_lo, oa_hi, lm_obs, idx, Jp, Jl, wv, Vchol + 9 * static_cast<size_t>(ia), Ya, &rows_a, Fa);
+    int gb = 0;
+    if (pair) gb = 6 * cov_landmark_Y<K>(ob_lo, ob_hi, lm_obs, idx, Jp, Jl, wv, Vchol + 9 * static_cast<size_t>(ib), Yb, &rows_b, Fb);
+    else cov_block_dofs(kb, ib, lay, Kbg, &gb, &tb);
+    // M = Y_a^T Sigma_{span(a), b} (3 x tb), b = Y_b-weighted span(b) for a landmark pair (tb = 3)
+    double M[18];
+#pragma unroll
+    for (int i = 0; i < 18; ++i) M[i] = 0.0;
+    for (int rr = lane; rr < rows_a; rr += 32) {
+      const int gr = ga0 + rr;
+      double t[6] = {0, 0, 0, 0, 0, 0};
+      if (pair) {
+        for (int s = 0; s < rows_b; ++s) {
+          const double z = cov_sigma(cov, far, plan, lay, gr, gb + s);
+          t[0] += z * Yb[3 * s]; t[1] += z * Yb[3 * s + 1]; t[2] += z * Yb[3 * s + 2];
+        }
+      } else {
+#pragma unroll
+        for (int c = 0; c < 6; ++c) t[c] = c < tb ? cov_sigma(cov, far, plan, lay, gr, gb + c) : 0.0;
+      }
+#pragma unroll
+      for (int a = 0; a < 3; ++a)
+#pragma unroll
+        for (int c = 0; c < 6; ++c) M[6 * a + c] += Ya[3 * rr + a] * t[c];
+    }
+#pragma unroll
+    for (int i = 0; i < 18; ++i)
+#pragma unroll
+      for (int x = 16; x > 0; x >>= 1) M[i] += __shfl_xor_sync(0xffffffffu, M[i], x);
+    if (lane == 0) {
+      double La[9];
+      cov_landmark_Linv(Fa, La);
+      if (pair) {   // L_a^-T M L_b^-1
+        double Lb[9], Mm[9], T[9], S[9];
+#pragma unroll
+        for (int i = 0; i < 9; ++i) Mm[i] = M[6 * (i / 3) + i % 3];
+        cov_landmark_Linv(Fb, Lb);
+        m3_mul(Mm, Lb, T);
+        m3_tmul(La, T, S);
+#pragma unroll
+        for (int i = 0; i < 9; ++i) R[6 * (i / 3) + i % 3] = S[i];
+      } else {      // -L_a^-T M
+#pragma unroll
+        for (int a = 0; a < 3; ++a)
+#pragma unroll
+          for (int c = 0; c < 6; ++c) R[6 * a + c] = -(La[a] * M[c] + La[3 + a] * M[6 + c] + La[6 + a] * M[12 + c]);
+      }
+    }
+  }
+  if (lane == 0) {
+    out_status[q] = st;
+#pragma unroll
+    for (int e = 0; e < 36; ++e) {
+      const int a = e / 6, b = e % 6;
+      double v = 0.0;
+      if (!swap && a < 3 && b < tb) v = R[6 * a + b];
+      if (swap && b < 3 && a < tb) v = R[6 * b + a];
+      o[e] = v;
+    }
   }
 }
 

@@ -447,10 +447,20 @@ bool Covariance::Compute(const std::vector<std::pair<const double*, const double
   o.upload(o.dirty_);   // the device window == the host variables (as Ceres evaluates at the values it aliases)
   int beta = 0;
   check(hb200_get_bandwidth(o.ctx_, &beta), "hb200_get_bandwidth");
+  // pairs outside the pattern as hb200_set_covariance_blocks requests (kind, index, kind, index)
+  static constexpr int kKind[] = {HB200_COV_KNOT, HB200_COV_GYRO_BIAS, HB200_COV_ACCEL_BIAS, HB200_COV_GRAVITY, HB200_COV_LANDMARK};
+  std::vector<int> requests;
+  std::vector<std::pair<const double*, const double*>> outside;
   for (const auto& [pa, pb] : blocks) {
     Block a, b;
-    if (!locate(pa, &a) || !locate(pb, &b) || !inPattern(a, b, beta)) return false;
+    if (!locate(pa, &a) || !locate(pb, &b)) return false;
+    if (inPattern(a, b, beta)) continue;
+    if (!options_.full_pattern) return false;
+    requests.insert(requests.end(), {kKind[a.kind], a.index, kKind[b.kind], b.index});
+    outside.emplace_back(pa, pb);
   }
+  const int nreq = static_cast<int>(outside.size());
+  check(hb200_set_covariance_blocks(o.ctx_, nreq, requests.data()), "hb200_set_covariance_blocks");
   check(hb200_build_covariance(o.ctx_), "hb200_build_covariance");
   hb200_covariance_info info{};
   const int rc = hb200_compute_covariance(o.ctx_, &info);
@@ -460,6 +470,18 @@ bool Covariance::Compute(const std::vector<std::pair<const double*, const double
   packed_.assign(static_cast<size_t>(info.K) * (6 + 6 * info.beta) * 6 + static_cast<size_t>(info.m) * 6 * info.K + static_cast<size_t>(info.m) * info.m, 0.0);
   landmarks_.assign(9 * static_cast<size_t>(info.L), 0.0);
   check(hb200_get_covariance(o.ctx_, packed_.data(), landmarks_.empty() ? nullptr : landmarks_.data()), "hb200_get_covariance");
+  std::vector<double> slots(36 * static_cast<size_t>(nreq));
+  check(hb200_get_covariance_blocks(o.ctx_, nreq, slots.data(), nullptr), "hb200_get_covariance_blocks");
+  outside_.clear();
+  for (int q = 0; q < nreq; ++q) {   // (status 1, a landmark on another rank, cannot occur on one GPU; status 2 is a zero block)
+    Block a, b;
+    locate(outside[q].first, &a);
+    locate(outside[q].second, &b);
+    std::vector<double>& t = outside_[outside[q]];
+    t.resize(static_cast<size_t>(a.tangent) * b.tangent);
+    for (int i = 0; i < a.tangent; ++i)
+      for (int j = 0; j < b.tangent; ++j) t[static_cast<size_t>(i) * b.tangent + j] = slots[36 * static_cast<size_t>(q) + 6 * i + j];
+  }
   beta_ = info.beta; K_ = info.K; n_ = 6 * info.K + info.m;
   computed_ = blocks;
   values_.clear();
@@ -477,6 +499,17 @@ bool Covariance::tangentBlock(const double* pa, const double* pb, std::vector<do
   for (const auto& [x, y] : computed_) found = found || (x == pa && y == pb) || (x == pb && y == pa);
   if (!found || !locate(pa, a) || !locate(pb, b)) return false;
   out->assign(static_cast<size_t>(a->tangent) * b->tangent, 0.0);
+  // Ceres' quaternion tangent: delta = theta / 2
+  auto scale = [](const Block& bl, int i) { return (bl.kind == kState && i < 3) ? 0.5 : 1.0; };
+  const auto ab = outside_.find({pa, pb}), ba = outside_.find({pb, pa});
+  if (ab != outside_.end() || ba != outside_.end()) {   // outside the pattern: (b, a) is the transpose of (a, b)
+    for (int i = 0; i < a->tangent; ++i)
+      for (int j = 0; j < b->tangent; ++j) {
+        const double v = ab != outside_.end() ? ab->second[static_cast<size_t>(i) * b->tangent + j] : ba->second[static_cast<size_t>(j) * a->tangent + i];
+        (*out)[static_cast<size_t>(i) * b->tangent + j] = scale(*a, i) * v * scale(*b, j);
+      }
+    return true;
+  }
   if (a->kind == kLandmark) {   // (same landmark: the only landmark pair in the pattern)
     for (int i = 0; i < 9; ++i) (*out)[i] = landmarks_[9 * static_cast<size_t>(a->index) + i];
     return true;
@@ -489,8 +522,6 @@ bool Covariance::tangentBlock(const double* pa, const double* pb, std::vector<do
     if (c < np) return packed_[static_cast<size_t>(K_) * h * 6 + static_cast<size_t>(r - np) * np + c];
     return packed_[static_cast<size_t>(K_) * h * 6 + static_cast<size_t>(m) * np + static_cast<size_t>(r - np) * m + (c - np)];
   };
-  // Ceres' quaternion tangent: delta = theta / 2
-  auto scale = [](const Block& bl, int i) { return (bl.kind == kState && i < 3) ? 0.5 : 1.0; };
   for (int i = 0; i < a->tangent; ++i)
     for (int j = 0; j < b->tangent; ++j) (*out)[static_cast<size_t>(i) * b->tangent + j] = scale(*a, i) * at(a->dof + i, b->dof + j) * scale(*b, j);
   return true;

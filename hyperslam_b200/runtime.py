@@ -46,6 +46,9 @@ class CovarianceInfo(C.Structure):
 
 COV_NOT_POSITIVE_DEFINITE, COV_DEGENERATE_LANDMARKS = 40, 41
 STATE_COV_DIM = 18   # HB200_STATE_COV_DIM: [theta p | omega v | b_g b_a]
+# parameter-block kinds of set_covariance_blocks (HB200_COV_*) and their device tangent sizes
+COV_KNOT, COV_GYRO_BIAS, COV_ACCEL_BIAS, COV_GRAVITY, COV_LANDMARK = 0, 1, 2, 3, 4
+COV_TANGENT = {COV_KNOT: 6, COV_GYRO_BIAS: 3, COV_ACCEL_BIAS: 3, COV_GRAVITY: 2, COV_LANDMARK: 3}
 
 
 ALLREDUCE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p)
@@ -68,7 +71,7 @@ EXPORTS = [
     "hb200_append_bearing_factors", "hb200_append_manifold_factors", "hb200_append_stereo_tracks", "hb200_slide_landmark_map",
     "hb200_factor_counts", "hb200_build_covariance", "hb200_compute_covariance", "hb200_get_covariance", "hb200_interpolate_covariance",
     "hb200_append_bias_knots", "hb200_bias_knots", "hb200_set_deterministic", "hb200_get_deterministic",
-    "hb200_interpolate_state_covariance",
+    "hb200_interpolate_state_covariance", "hb200_set_covariance_blocks", "hb200_get_covariance_blocks",
 ]
 
 _lib = None
@@ -120,6 +123,7 @@ class Context:
         self.order = self.K = self.Kbg = self.Kba = self.L = self.Nv = self.Ni = self.Nb = self.Nm = 0
         self._slide_L = 0   # landmarks before the last slide (landmark_map)
         self._cov_shape = (0, 0, 0, 0)
+        self._cov_blocks = (0, 0)   # (pairs registered, pairs of the last successful compute)
         self.bias_order = 4
 
     def _check(self, rc: int):
@@ -408,7 +412,25 @@ class Context:
         if rc:
             out["message"] = self.lib.hb200_last_error_string().decode()
         self._cov_shape = (info.K, info.beta, info.m, info.L)
+        if rc == 0:
+            self._cov_blocks = (self._cov_blocks[0], self._cov_blocks[0])
         return out
+
+    def set_covariance_blocks(self, pairs):
+        """Registers pairs (kind_a, index_a, kind_b, index_b) (COV_* kinds) that every later compute_covariance also
+        computes, as ceres::Covariance::Compute(covariance_blocks); an empty list clears them."""
+        pairs = np.ascontiguousarray(np.asarray(pairs, dtype=np.int32).reshape(-1, 4))
+        self._check(self.lib.hb200_set_covariance_blocks(self.h, pairs.shape[0], _i(pairs)))
+        self._cov_blocks = (pairs.shape[0], self._cov_blocks[1])
+
+    def covariance_blocks(self):
+        """(blocks (n, 6, 6), status (n,)) of the last successful compute: Sigma_ab in the device tangents, t_a x t_b in
+        the top-left of each slot; status 0 computed, 1 landmark not observed on this rank, 2 unobserved landmark."""
+        n = self._cov_blocks[1]
+        out = np.zeros((n, 6, 6))
+        st = np.zeros(n, np.int32)
+        self._check(self.lib.hb200_get_covariance_blocks(self.h, n, _d(out), _i(st)))
+        return out, st
 
     def covariance_packed(self):
         """(packed P | A | C of Sigma, landmark blocks (L, 3, 3), (K, beta, m, L)) of the last successful compute."""

@@ -271,6 +271,27 @@ int hb200_get_covariance(hb200_ctx* ctx, double* packed /* P | A | C of SysLayou
 int hb200_interpolate_covariance(hb200_ctx* ctx, int n, const double* stamps, double* cov /* [n][6][6] */, int* num_invalid);
 enum { HB200_STATE_COV_DIM = 18 };
 int hb200_interpolate_state_covariance(hb200_ctx* ctx, int n, const double* stamps, double* cov /* [n][18][18] */, int* num_invalid);
+/* Blocks outside the selected inverse's pattern, the list of ceres::Covariance::Compute(covariance_blocks): knot pairs
+ * more than beta apart, landmark x knot / bias / gravity and landmark x landmark (any pair is accepted; pairs in the
+ * pattern are copied from Sigma and the landmark marginals bit for bit).
+ *   hb200_set_covariance_blocks: registers n pairs (kind_a, index_a, kind_b, index_b) that every later
+ *                             hb200_compute_covariance computes with Sigma (n = 0 clears the list; with no list the compute
+ *                             runs exactly as without this call).  Host-only: touches neither the build nor committed results.
+ *                             The compute checks the indices against the build's shapes (knots < K, bias knots < Kbg / Kba,
+ *                             gravity 0, landmarks < L of this context) and returns -1 without computing anything on a bad one.
+ *   hb200_get_covariance_blocks: Sigma_ab of the last successful compute, t_a x t_b row-major in the top-left of a 6 x 6
+ *                             slot (device tangents: knot 6, bias knot 3, gravity 2, landmark 3), the rest 0; (b, a) is the
+ *                             exact transpose of (a, b); constant dofs 0.  status[i] (may be NULL): 0 computed, 1 a landmark
+ *                             without observations on a sharded context (its owner computes the pair), 2 a landmark without
+ *                             observations (as its marginal); both with a zero block.  -2 before a successful compute and
+ *                             when n differs from the number of pairs that compute was given.  Like Sigma, the blocks are
+ *                             a snapshot: a failed compute, later iterations, appends and slides leave them as they are.
+ * Sharded contexts: no collective step is added.  Knot, bias and gravity pairs are bit-identical on every rank; a pair
+ * with landmarks is computed by the rank that observes them (status 1 elsewhere); two landmarks owned by different ranks
+ * are not supported (status 1 on both). */
+enum { HB200_COV_KNOT = 0, HB200_COV_GYRO_BIAS = 1, HB200_COV_ACCEL_BIAS = 2, HB200_COV_GRAVITY = 3, HB200_COV_LANDMARK = 4 };
+int hb200_set_covariance_blocks(hb200_ctx* ctx, int n, const int* pairs /* [n][4] */);
+int hb200_get_covariance_blocks(hb200_ctx* ctx, int n, double* out /* [n][6][6] */, int* status /* [n], may be NULL */);
 
 /* full LM iterations: evaluate -> build -> [allreduce] -> solve -> retract -> cost at trial ->
  * accept/reject, all on the device.  records may be NULL. */

@@ -3,8 +3,10 @@ landmark marginals), hb200_interpolate_covariance and hb200_interpolate_state_co
 events around each call (host copies included), on cfg1, cfg2 and a K = 500 window.  Prints the card and its power
 limit first; one JSON line per window.  --baseline-lib PATH alternates, round by round, with contexts of another build
 of libhyperb200.so (the calls it lacks are skipped) and prints its line (lib = "baseline") after each window's.
+--blocks times the compute alone with requested blocks outside the pattern (see blocks()), after the card, its power
+limit and SM clocks.
 
-    python tools/covariance_timing.py [--reps 5] [--baseline-lib PATH]
+    python tools/covariance_timing.py [--reps 5] [--baseline-lib PATH] [--blocks]
 """
 import argparse
 import json
@@ -43,11 +45,56 @@ def window(name):
     return win
 
 
+def blocks(reps):
+    """--blocks: hb200_compute_covariance with no requested blocks, with every far knot pair of cfg1 (all knot pairs more
+    than beta apart), and with 1000 landmark x knot plus 1000 landmark x landmark pairs on the K = 500 window."""
+    import torch
+    from hyperslam_b200 import runtime
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True,
+                       timeout=30)
+    print(f"# {q.stdout.strip().splitlines()[0]}")
+    rng = np.random.default_rng(7)
+    for name in ("cfg1", "K500"):
+        win = window(name)
+        ctx = runtime.Context(0)
+        ctx.load_window(win)
+        K, L, beta = win.knots.shape[0], win.landmarks.shape[0], ctx.bandwidth()
+        cases = {"none": np.zeros((0, 4), np.int32)}
+        if name == "cfg1":
+            cases["far_knot_pairs"] = np.array([(0, i, 0, j) for j in range(K) for i in range(j - beta)], np.int32)
+        else:
+            lk = np.stack([np.full(1000, 4), rng.integers(0, L, 1000), np.zeros(1000, int), rng.integers(0, K, 1000)], 1)
+            ll = np.stack([np.full(1000, 4), rng.integers(0, L, 1000), np.full(1000, 4), rng.integers(0, L, 1000)], 1)
+            cases["landmark_pairs"] = np.concatenate([lk, ll]).astype(np.int32)
+        stream = torch.cuda.ExternalStream(ctx.stream)
+        for case, req in cases.items():
+            ctx.set_covariance_blocks(req)
+            times, launches = [], 0
+            for r in range(reps + 1):
+                ctx.build_covariance()
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                l0 = ctx.launch_count
+                e0.record(stream)
+                info = ctx.compute_covariance()
+                e1.record(stream)
+                e1.synchronize()
+                launches = ctx.launch_count - l0
+                if r:   # first round: warm-up
+                    times.append(e0.elapsed_time(e1))
+            _, st = ctx.covariance_blocks()
+            print(json.dumps(dict(window=name, case=case, K=K, beta=beta, L=L, pairs=len(req), status=info["status"], launches=launches,
+                                  computed=int((st == 0).sum()), compute_ms=float(np.median(times)), reps=reps)))
+        ctx.close()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--baseline-lib", default=None)
+    ap.add_argument("--blocks", action="store_true", help="time the compute with requested blocks outside the pattern")
     args = ap.parse_args()
+    if args.blocks:
+        return blocks(args.reps)
     import ctypes
     import torch
     from hyperslam_b200 import runtime
