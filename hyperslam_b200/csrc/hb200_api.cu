@@ -300,6 +300,13 @@ struct hb200_ctx {
   DevBuf<int> cov_plan, cov_blk_st, cov_blk_st_next;
   DevBuf<double> cov_far, cov_blk, cov_blk_next;
   int cov_blk_n = 0;
+  // stamp pairs (hb200_set_covariance_stamp_pairs): the registered [t_a, t_b] per pair and their device copy (their
+  // control-point spans follow the requests' landmark spans in cov_span); cov_pair_joint / _rel / _st (cov_pair_n of
+  // them) are the committed blocks
+  std::vector<double> cov_pairs;
+  DevBuf<double> cov_pairs_d, cov_pair_joint, cov_pair_joint_next, cov_pair_rel, cov_pair_rel_next;
+  DevBuf<int> cov_pair_st, cov_pair_st_next;
+  int cov_pair_n = 0;
 
   hb200_allreduce_fn allreduce = nullptr;
   void* allreduce_user = nullptr;
@@ -2127,22 +2134,36 @@ bool cov_request_ok(const int4& r, const CovPoint& pt) {
   return ok(r.x, r.y) && ok(r.z, r.w);
 }
 
-// The requested blocks of a compute, after cov_landmark_kernel: the landmarks' control-point spans (one read-back, only
-// when a request has a landmark), the far-column plan -- for every knot pair more than beta blocks apart that a request
-// reads, directly or through a landmark's span, its column (the larger block) and the lowest row the march must reach --
-// then cov_far_column_kernel over the planned columns and cov_cross_landmark_kernel over the requests, into *_next.
+// The requested blocks and stamp pairs of a compute, after cov_landmark_kernel: the control-point spans of the requests'
+// landmarks and of the pairs' stamps (one read-back, only when a request has a landmark or a pair is registered), the
+// far-column plan -- for every knot pair more than beta blocks apart that a request or a pair reads, directly or through
+// a span, its column (the larger block) and the lowest row the march must reach -- then cov_far_column_kernel over the
+// planned columns, cov_cross_landmark_kernel over the requests and cov_pose_pair_kernel over the pairs, into *_next.
+// A column's values do not depend on its lowest row, so the requests' blocks are the same with or without pairs.
 int cov_blocks_enqueue(hb200_ctx* c, const CovPoint& pt) {
   const SysLayout& lay = pt.lay;
-  const int n = static_cast<int>(c->cov_req.size()), K = lay.K, beta = lay.beta;
-  HB_CUDA(c->cov_req_d.ensure(n));
-  HB_CUDA(cudaMemcpyAsync(c->cov_req_d.p, c->cov_req.data(), sizeof(int4) * n, cudaMemcpyHostToDevice, c->stream));
-  std::vector<int2> span(2 * static_cast<size_t>(n), make_int2(-1, -1));
+  const int n = static_cast<int>(c->cov_req.size()), npair = static_cast<int>(c->cov_pairs.size() / 2), K = lay.K, beta = lay.beta;
+  if (n) {
+    HB_CUDA(c->cov_req_d.ensure(n));
+    HB_CUDA(cudaMemcpyAsync(c->cov_req_d.p, c->cov_req.data(), sizeof(int4) * n, cudaMemcpyHostToDevice, c->stream));
+  }
+  // cov_span: [2n] landmark spans of the requests' sides, then [npair] (base_a, base_b) of the pairs
+  std::vector<int2> span(2 * static_cast<size_t>(n) + npair, make_int2(-1, -1));
   const bool landmarks = pt.Nv && std::any_of(c->cov_req.begin(), c->cov_req.end(), [](const int4& r) { return r.x == kCovLandmark || r.z == kCovLandmark; });
+  HB_CUDA(c->cov_span.ensure(span.size()));
   if (landmarks) {
-    HB_CUDA(c->cov_span.ensure(2 * static_cast<size_t>(n)));
     cov_landmark_span_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(n, c->cov_req_d.p, c->lm_off.p, c->lm_obs.p, c->v_idx.p, pt.k, c->cov_span.p);
     HB_LAUNCH(c, "cov_landmark_span_kernel");
-    HB_CUDA(cudaMemcpyAsync(span.data(), c->cov_span.p, sizeof(int2) * 2 * n, cudaMemcpyDeviceToHost, c->stream));
+  }
+  if (npair) {
+    HB_CUDA(c->cov_pairs_d.ensure(2 * static_cast<size_t>(npair)));
+    HB_CUDA(cudaMemcpyAsync(c->cov_pairs_d.p, c->cov_pairs.data(), sizeof(double) * 2 * npair, cudaMemcpyHostToDevice, c->stream));
+    cov_stamp_span_kernel<<<(npair + 127) / 128, 128, 0, c->stream>>>(npair, c->cov_pairs_d.p, pt.knots.p, K, pt.k, c->cov_span.p + 2 * n);
+    HB_LAUNCH(c, "cov_stamp_span_kernel");
+  }
+  if (landmarks || npair) {
+    const size_t first = landmarks ? 0 : 2 * static_cast<size_t>(n);
+    HB_CUDA(cudaMemcpyAsync(span.data() + first, c->cov_span.p + first, sizeof(int2) * (span.size() - first), cudaMemcpyDeviceToHost, c->stream));
     HB_CUDA(cudaStreamSynchronize(c->stream));
   }
   std::vector<int> need(K, K);   // lowest row block per column block (K: none)
@@ -2161,6 +2182,12 @@ int cov_blocks_enqueue(hb200_ctx* c, const CovPoint& pt) {
     if (kind[0] == kCovLandmark && kind[1] == kCovLandmark && index[0] == index[1]) continue;   // the marginal
     for (int a = lo[0]; a < hi[0]; ++a)
       for (int b = lo[1]; b < hi[1]; ++b) far(a, b);
+  }
+  for (int q = 0; q < npair; ++q) {
+    const int2 s = span[2 * static_cast<size_t>(n) + q];
+    if (s.x < 0 || s.y < 0) continue;
+    for (int a = s.x; a < s.x + pt.k; ++a)
+      for (int b = s.y; b < s.y + pt.k; ++b) far(a, b);
   }
   std::vector<int> plan(K, -1);
   int nc = 0, blocks = 0;
@@ -2184,13 +2211,25 @@ int cov_blocks_enqueue(hb200_ctx* c, const CovPoint& pt) {
     cov_far_column_kernel<<<nc, kFarThreads, smem, c->stream>>>(c->cov_ws.p, c->cov_packed_next.p, lay, c->fixed.p, fp, c->cov_status.p, c->cov_far.p);
     HB_LAUNCH(c, "cov_far_column_kernel");
   }
+  HB_CUDA(c->cov_pair_joint_next.ensure(144 * static_cast<size_t>(npair)));
+  HB_CUDA(c->cov_pair_rel_next.ensure(36 * static_cast<size_t>(npair)));
+  HB_CUDA(c->cov_pair_st_next.ensure(npair));
   const size_t smem = static_cast<size_t>(kLmWarps) * 6 * pt.max_rows * sizeof(double);
   return with_order(pt.k, [&](auto Kc) {
-    HB_CUDA(cudaFuncSetAttribute(cov_cross_landmark_kernel<Kc>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    cov_cross_landmark_kernel<Kc><<<(n + kLmWarps - 1) / kLmWarps, kLmWarps * 32, smem, c->stream>>>(
-        n, c->cov_req_d.p, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p, c->Vchol.p, c->cov_packed_next.p, c->cov_lm_next.p,
-        c->cov_far.p, fp, lay, pt.Kbg, c->multi() ? 1 : 0, c->cov_status.p, pt.max_rows, c->cov_blk_next.p, c->cov_blk_st_next.p);
-    return check_launch(c, "cov_cross_landmark_kernel");
+    if (n) {
+      HB_CUDA(cudaFuncSetAttribute(cov_cross_landmark_kernel<Kc>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+      cov_cross_landmark_kernel<Kc><<<(n + kLmWarps - 1) / kLmWarps, kLmWarps * 32, smem, c->stream>>>(
+          n, c->cov_req_d.p, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p, c->Vchol.p, c->cov_packed_next.p, c->cov_lm_next.p,
+          c->cov_far.p, fp, lay, pt.Kbg, c->multi() ? 1 : 0, c->cov_status.p, pt.max_rows, c->cov_blk_next.p, c->cov_blk_st_next.p);
+      if (const int rc = check_launch(c, "cov_cross_landmark_kernel")) return rc;
+    }
+    if (npair) {
+      cov_pose_pair_kernel<Kc><<<(npair + kPairWarps - 1) / kPairWarps, kPairWarps * 32, 0, c->stream>>>(
+          npair, c->cov_pairs_d.p, c->cov_span.p + 2 * n, pt.tab.p, pt.basis, c->cov_packed_next.p, c->cov_far.p, fp, lay, c->cov_status.p,
+          c->cov_pair_joint_next.p, c->cov_pair_rel_next.p, c->cov_pair_st_next.p);
+      if (const int rc = check_launch(c, "cov_pose_pair_kernel")) return rc;
+    }
+    return 0;
   });
 }
 }  // namespace
@@ -2298,9 +2337,9 @@ int hb200_compute_covariance(hb200_ctx* c, hb200_covariance_info* info) {
   } else if (L) {
     HB_CUDA(cudaMemsetAsync(c->cov_lm_next.p, 0, sizeof(double) * 9 * L, c->stream));
   }
-  // requested blocks: the landmark blocks need the build's factor outputs and the far columns the factor in cov_ws,
-  // both valid only until the next launch, so they are computed here (nothing runs without a request)
-  if (!c->cov_req.empty())
+  // requested blocks and stamp pairs: the landmark blocks need the build's factor outputs and the far columns the factor
+  // in cov_ws, both valid only until the next launch, so they are computed here (nothing runs without a request or pair)
+  if (!c->cov_req.empty() || !c->cov_pairs.empty())
     if (const int rc = cov_blocks_enqueue(c, pt)) return rc;
   CovStatus st{};
   HB_CUDA(cudaMemcpyAsync(&st, c->cov_status.p, sizeof(st), cudaMemcpyDeviceToHost, c->stream));
@@ -2320,6 +2359,10 @@ int hb200_compute_covariance(hb200_ctx* c, hb200_covariance_info* info) {
   c->cov_blk.swap(c->cov_blk_next);
   c->cov_blk_st.swap(c->cov_blk_st_next);
   c->cov_blk_n = static_cast<int>(c->cov_req.size());
+  c->cov_pair_joint.swap(c->cov_pair_joint_next);
+  c->cov_pair_rel.swap(c->cov_pair_rel_next);
+  c->cov_pair_st.swap(c->cov_pair_st_next);
+  c->cov_pair_n = static_cast<int>(c->cov_pairs.size() / 2);
   c->cov_slot_committed = c->cov_slot_built;
   c->cov_valid = true;
   cov_info(c, info);
@@ -2346,6 +2389,29 @@ int hb200_get_covariance_blocks(hb200_ctx* c, int n, double* out, int* status) {
   HB_CUDA(cudaSetDevice(c->device));
   HB_CUDA(cudaMemcpyAsync(out, c->cov_blk.p, sizeof(double) * 36 * n, cudaMemcpyDeviceToHost, c->stream));
   if (status) HB_CUDA(cudaMemcpyAsync(status, c->cov_blk_st.p, sizeof(int) * n, cudaMemcpyDeviceToHost, c->stream));
+  HB_CUDA(cudaStreamSynchronize(c->stream));
+  return 0;
+}
+
+int hb200_set_covariance_stamp_pairs(hb200_ctx* c, int n, const double* stamps) {
+  if (!c) return fail(-1, "null context");
+  if (n < 0 || (n > 0 && !stamps)) return fail(-1, "invalid argument");
+  for (size_t i = 0; i < 2 * static_cast<size_t>(n); ++i)
+    if (!std::isfinite(stamps[i])) return fail(-1, "stamp pair %zu: stamp %zu is not finite", i / 2, i % 2);
+  c->cov_pairs.assign(stamps, stamps + 2 * static_cast<size_t>(n));
+  return 0;
+}
+
+int hb200_get_pose_pair_covariance(hb200_ctx* c, int n, double* joint, double* relative, int* status) {
+  if (!c) return fail(-1, "null context");
+  if (n < 0) return fail(-1, "invalid argument");
+  if (!c->cov_valid) return fail(-2, "no covariance computed (hb200_compute_covariance has not succeeded)");
+  if (n != c->cov_pair_n) return fail(-2, "the last successful compute had %d stamp pairs, not %d", c->cov_pair_n, n);
+  if (n == 0) return 0;
+  HB_CUDA(cudaSetDevice(c->device));
+  if (joint) HB_CUDA(cudaMemcpyAsync(joint, c->cov_pair_joint.p, sizeof(double) * 144 * n, cudaMemcpyDeviceToHost, c->stream));
+  if (relative) HB_CUDA(cudaMemcpyAsync(relative, c->cov_pair_rel.p, sizeof(double) * 36 * n, cudaMemcpyDeviceToHost, c->stream));
+  if (status) HB_CUDA(cudaMemcpyAsync(status, c->cov_pair_st.p, sizeof(int) * n, cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
   return 0;
 }

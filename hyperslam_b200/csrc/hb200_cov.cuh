@@ -8,7 +8,8 @@
 //   cov_interpolate_kernel the 6 x 6 covariance of the interpolated pose at arbitrary stamps, J(t) Sigma J(t)^T;
 //   cov_state_interpolate_kernel the 18 x 18 joint covariance of pose, body velocity and IMU biases at arbitrary stamps;
 //   cov_far_column_kernel / cov_cross_landmark_kernel the requested blocks outside the pattern (ceres::Covariance::Compute's
-//                         list): knot pairs beyond the band and landmark cross-covariances.
+//                         list): knot pairs beyond the band and landmark cross-covariances;
+//   cov_pose_pair_kernel  the joint covariance of the poses at two stamps and the covariance of their relative pose.
 // All are deterministic: no atomics, every sum in a fixed order.
 #pragma once
 #include "hb200_solve.cuh"
@@ -957,6 +958,185 @@ __global__ void __launch_bounds__(kStateWarps * 32) cov_state_interpolate_kernel
     const int r = e / D, c = e - r * D;
     o[e] = 0.5 * (J[r * D + c] + J[c * D + r]);
   }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Joint and relative covariance of the poses at two stamps (hb200_set_covariance_stamp_pairs), computed inside the
+// compute from its Sigma and the far scratch, at the knots the build linearised at (the snapshot knot table).
+//   joint    (12 x 12) of [theta_a p_a | theta_b p_b]: blocks J_s Sigma_{span(s), span(s')} J_s'^T, J(t) the pose
+//            Jacobian of cov_interpolate_kernel (global rotation tangent, p <- p + rho);
+//   relative (6 x 6) of T_ab = T_a^-1 T_b (R_ab = R_a^T R_b, p_ab = R_a^T (p_b - p_a)) in the same split tangent in frame
+//            a: A joint A^T with A = Rb M, Rb = diag(R_a^T, R_a^T), M = [[-I, 0, I, 0], [hat(p_b - p_a), -I, 0, I]].
+// ---------------------------------------------------------------------------------------------
+constexpr int kPairWarps = 2;   // pairs per CTA (static shared memory: 2 x 21 KB at k = 6)
+
+// Control-point span bases (segment_base on the snapshot knots, -1 outside the valid span) of both stamps of each pair.
+__global__ void cov_stamp_span_kernel(int n, const double* __restrict__ stamps, const double* __restrict__ knots, int Kn, int k, int2* __restrict__ span) {
+  const int q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= n) return;
+  span[q] = make_int2(segment_base(knots, 8, 7, Kn, k, stamps[2 * q]), segment_base(knots, 8, 7, Kn, k, stamps[2 * q + 1]));
+}
+
+// J(t) (6 x 6K row-major, dense) of the pose at t over control points base .. base + K - 1 -- the operations of
+// cov_interpolate_kernel's builder in its order, so D_m = M_m - M_{m+1} rounds the same -- and the pose R (row-major), p.
+template <int K>
+HB_DI void cov_pose_jacobian(const double* __restrict__ tab, const Basis& B, int base, double t, double* J, double* R, double* p) {
+  constexpr int left = (K - 1) / 2, NC = 6 * K;
+  const double* row0 = tab + static_cast<size_t>(base) * kTabStride;
+  const double t0 = row0[left * kTabStride + 24], t1 = row0[(left + 1) * kTabStride + 24];
+  const double inv_dt = 1.0 / (t1 - t0);
+  double lam[K + 1];
+  basis_eval<K, false>(B, (t - t0) * inv_dt, inv_dt, lam, nullptr, nullptr);
+  for (int e = 0; e < 6 * NC; ++e) J[e] = 0.0;
+  for (int i = 0; i < 3; ++i) J[i * NC + i] = 1.0;   // M_0 = I
+  double P[9], pp[3] = {row0[9], row0[10], row0[11]};
+#pragma unroll
+  for (int i = 0; i < 9; ++i) P[i] = row0[i];
+#pragma unroll 1
+  for (int j = 1; j < K; ++j) {
+    const double* rj = row0 + j * kTabStride;
+    const double wj[3] = {lam[j] * rj[12], lam[j] * rj[13], lam[j] * rj[14]};
+    double A[9], Jr[9], Pn[9], G[9], JG[9], PJG[9];
+    so3_exp_and_Jr(wj, A, Jr);
+    m3_mul(P, A, Pn);
+#pragma unroll
+    for (int i = 0; i < 9; ++i) G[i] = rj[15 + i];
+    m3_mul(Jr, G, JG);
+    m3_mul(Pn, JG, PJG);
+#pragma unroll
+    for (int i = 0; i < 9; ++i) {
+      const double Mj = lam[j] * PJG[i];
+      J[(i / 3) * NC + 6 * j + i % 3] += Mj;
+      J[(i / 3) * NC + 6 * (j - 1) + i % 3] -= Mj;
+      P[i] = Pn[i];
+    }
+#pragma unroll
+    for (int c = 0; c < 3; ++c) pp[c] += lam[j] * (rj[9 + c] - rj[9 + c - kTabStride]);
+  }
+  for (int mm = 0; mm < K; ++mm) {
+    const double wm = lam[mm] - lam[mm + 1];
+    for (int i = 0; i < 3; ++i) J[(3 + i) * NC + 6 * mm + 3 + i] = wm;
+  }
+#pragma unroll
+  for (int i = 0; i < 9; ++i) R[i] = P[i];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) p[c] = pp[c];
+}
+
+// One warp per pair.  Lanes 0 and 1 build J_a and J_b; T = Z J^T over the 2 x 6k span dofs (row a of Z per lane, its
+// entries gathered through cov_sigma: band, arrow and the far scratch the plan filled), S = blockdiag(J_a, J_b) T,
+// joint = 0.5 (S + S^T); then E = M joint, F = E M^T, relative = 0.5 (Rb F Rb^T + (Rb F Rb^T)^T).  Swapping the stamps
+// relabels the blocks of every sum without reordering its terms, so (t_b, t_a) is exactly the permutation of
+// (t_a, t_b).  A stamp outside the valid span gives zero blocks and status 1.  No atomics, every sum in a fixed order.
+template <int K>
+__global__ void __launch_bounds__(kPairWarps * 32) cov_pose_pair_kernel(
+    int n, const double* __restrict__ stamps, const int2* __restrict__ span, const double* __restrict__ tab, Basis B, const double* __restrict__ cov,
+    const double* __restrict__ far, CovFarPlan plan, SysLayout lay, const CovStatus* __restrict__ status, double* __restrict__ joint,
+    double* __restrict__ rel, int* __restrict__ out_status) {
+  constexpr int NC = 6 * K;
+  __shared__ double s_J[kPairWarps][2][6 * NC];   // J_a, J_b
+  __shared__ double s_T[kPairWarps][2 * NC * 12];  // T; then S (144) and the joint (144)
+  __shared__ double s_E[kPairWarps][72 + 36 + 36]; // E (6 x 12), F, H = F Rb^T
+  __shared__ double s_P[kPairWarps][2][12];        // R (9) and p (3) of each stamp
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int q = blockIdx.x * kPairWarps + warp;
+  if (status->status != 0 || q >= n) return;
+  double* jo = joint + 144 * static_cast<size_t>(q);
+  double* ro = rel + 36 * static_cast<size_t>(q);
+  const int2 sp = span[q];
+  if (sp.x < 0 || sp.y < 0) {
+    for (int e = lane; e < 144; e += 32) jo[e] = 0.0;
+    for (int e = lane; e < 36; e += 32) ro[e] = 0.0;
+    if (lane == 0) out_status[q] = 1;
+    return;
+  }
+  const int base[2] = {sp.x, sp.y};
+  double* T = s_T[warp];
+  if (lane < 2) cov_pose_jacobian<K>(tab, B, base[lane], stamps[2 * static_cast<size_t>(q) + lane], s_J[warp][lane], s_P[warp][lane], s_P[warp][lane] + 9);
+  __syncwarp();
+  for (int a = lane; a < 2 * NC; a += 32) {
+    const int ga = 6 * base[a / NC] + a % NC;
+    double acc[12];
+#pragma unroll
+    for (int c = 0; c < 12; ++c) acc[c] = 0.0;
+#pragma unroll
+    for (int s = 0; s < 2; ++s) {
+      const double* Js = s_J[warp][s];
+#pragma unroll 2
+      for (int b = 0; b < NC; ++b) {
+        const double z = cov_sigma(cov, far, plan, lay, ga, 6 * base[s] + b);
+#pragma unroll
+        for (int r = 0; r < 6; ++r) acc[6 * s + r] += z * Js[r * NC + b];
+      }
+    }
+#pragma unroll
+    for (int c = 0; c < 12; ++c) T[a * 12 + c] = acc[c];
+  }
+  __syncwarp();
+  double sv[5];   // S = blockdiag(J_a, J_b) T, 144 entries over the lanes
+#pragma unroll
+  for (int u = 0; u < 5; ++u) {
+    const int e = lane + 32 * u;
+    double v = 0.0;
+    if (e < 144) {
+      const int r = e / 12, c = e % 12, s = r / 6;
+      const double* Jr = s_J[warp][s] + (r % 6) * NC;
+      const double* Tc = T + s * NC * 12 + c;
+      for (int b = 0; b < NC; ++b) v += Jr[b] * Tc[12 * b];
+    }
+    sv[u] = v;
+  }
+  __syncwarp();
+  double* S = T;
+  double* Jn = T + 144;
+#pragma unroll
+  for (int u = 0; u < 5; ++u)
+    if (lane + 32 * u < 144) S[lane + 32 * u] = sv[u];
+  __syncwarp();
+  for (int e = lane; e < 144; e += 32) {
+    const int r = e / 12, c = e % 12;
+    const double v = 0.5 * (S[e] + S[12 * c + r]);
+    Jn[e] = v;
+    jo[e] = v;
+  }
+  __syncwarp();
+  const double* Ra = s_P[warp][0];
+  const double dp[3] = {s_P[warp][1][9] - s_P[warp][0][9], s_P[warp][1][10] - s_P[warp][0][10], s_P[warp][1][11] - s_P[warp][0][11]};
+  const double hp[9] = {0.0, -dp[2], dp[1], dp[2], 0.0, -dp[0], -dp[1], dp[0], 0.0};   // hat(p_b - p_a)
+  double* E = s_E[warp];
+  double* F = E + 72;
+  double* H = F + 36;
+  for (int e = lane; e < 72; e += 32) {   // E = M joint
+    const int i = e / 12, c = e % 12;
+    double v;
+    if (i < 3) v = Jn[12 * (6 + i) + c] - Jn[12 * i + c];
+    else v = Jn[12 * (6 + i) + c] - Jn[12 * i + c] + (hp[3 * (i - 3)] * Jn[c] + hp[3 * (i - 3) + 1] * Jn[12 + c] + hp[3 * (i - 3) + 2] * Jn[24 + c]);
+    E[e] = v;
+  }
+  __syncwarp();
+  for (int e = lane; e < 36; e += 32) {   // F = E M^T
+    const int i = e / 6, j = e % 6;
+    const double* Ei = E + 12 * i;
+    double v;
+    if (j < 3) v = Ei[6 + j] - Ei[j];
+    else v = Ei[6 + j] - Ei[j] + (hp[3 * (j - 3)] * Ei[0] + hp[3 * (j - 3) + 1] * Ei[1] + hp[3 * (j - 3) + 2] * Ei[2]);
+    F[e] = v;
+  }
+  __syncwarp();
+  for (int e = lane; e < 36; e += 32) {   // H = F Rb^T: (R_a^T)^T = R_a, H_ij = sum_l F_{i, 3 bj + l} R_a[l][j % 3]
+    const int i = e / 6, j = e % 6, bj = 3 * (j / 3), jj = j % 3;
+    H[e] = F[6 * i + bj] * Ra[jj] + F[6 * i + bj + 1] * Ra[3 + jj] + F[6 * i + bj + 2] * Ra[6 + jj];
+  }
+  __syncwarp();
+  for (int e = lane; e < 36; e += 32) {   // Rb H, symmetrised in registers of the lane pair (e, e^T)
+    const int i = e / 6, j = e % 6;
+    auto rbh = [&](int r, int c) {
+      const int br = 3 * (r / 3), rr = r % 3;
+      return Ra[rr] * H[6 * br + c] + Ra[3 + rr] * H[6 * (br + 1) + c] + Ra[6 + rr] * H[6 * (br + 2) + c];
+    };
+    ro[e] = 0.5 * (rbh(i, j) + rbh(j, i));
+  }
+  if (lane == 0) out_status[q] = 0;
 }
 
 }  // namespace hb

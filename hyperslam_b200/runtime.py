@@ -72,6 +72,7 @@ EXPORTS = [
     "hb200_factor_counts", "hb200_build_covariance", "hb200_compute_covariance", "hb200_get_covariance", "hb200_interpolate_covariance",
     "hb200_append_bias_knots", "hb200_bias_knots", "hb200_set_deterministic", "hb200_get_deterministic",
     "hb200_interpolate_state_covariance", "hb200_set_covariance_blocks", "hb200_get_covariance_blocks",
+    "hb200_set_covariance_stamp_pairs", "hb200_get_pose_pair_covariance",
 ]
 
 _lib = None
@@ -124,6 +125,7 @@ class Context:
         self._slide_L = 0   # landmarks before the last slide (landmark_map)
         self._cov_shape = (0, 0, 0, 0)
         self._cov_blocks = (0, 0)   # (pairs registered, pairs of the last successful compute)
+        self._cov_pairs = (0, 0)    # the same for the stamp pairs
         self.bias_order = 4
 
     def _check(self, rc: int):
@@ -414,6 +416,7 @@ class Context:
         self._cov_shape = (info.K, info.beta, info.m, info.L)
         if rc == 0:
             self._cov_blocks = (self._cov_blocks[0], self._cov_blocks[0])
+            self._cov_pairs = (self._cov_pairs[0], self._cov_pairs[0])
         return out
 
     def set_covariance_blocks(self, pairs):
@@ -431,6 +434,22 @@ class Context:
         st = np.zeros(n, np.int32)
         self._check(self.lib.hb200_get_covariance_blocks(self.h, n, _d(out), _i(st)))
         return out, st
+
+    def set_covariance_stamp_pairs(self, stamps):
+        """Registers stamp pairs (t_a, t_b) whose joint and relative pose covariances every later compute_covariance also
+        computes; an empty list clears them."""
+        stamps = np.ascontiguousarray(np.asarray(stamps, dtype=np.float64).reshape(-1, 2))
+        self._check(self.lib.hb200_set_covariance_stamp_pairs(self.h, stamps.shape[0], _d(stamps)))
+        self._cov_pairs = (stamps.shape[0], self._cov_pairs[1])
+
+    def pose_pair_covariance(self):
+        """(joint (n, 12, 12), relative (n, 6, 6), status (n,)) of the last successful compute: the covariance of
+        [theta_a p_a | theta_b p_b] and of the relative pose T_a^-1 T_b in frame a (device tangent); status 0 computed, 1 a
+        stamp outside the valid span (zero blocks)."""
+        n = self._cov_pairs[1]
+        joint, rel, st = np.zeros((n, 12, 12)), np.zeros((n, 6, 6)), np.zeros(n, np.int32)
+        self._check(self.lib.hb200_get_pose_pair_covariance(self.h, n, _d(joint), _d(rel), _i(st)))
+        return joint, rel, st
 
     def covariance_packed(self):
         """(packed P | A | C of Sigma, landmark blocks (L, 3, 3), (K, beta, m, L)) of the last successful compute."""

@@ -292,6 +292,31 @@ int hb200_interpolate_state_covariance(hb200_ctx* ctx, int n, const double* stam
 enum { HB200_COV_KNOT = 0, HB200_COV_GYRO_BIAS = 1, HB200_COV_ACCEL_BIAS = 2, HB200_COV_GRAVITY = 3, HB200_COV_LANDMARK = 4 };
 int hb200_set_covariance_blocks(hb200_ctx* ctx, int n, const int* pairs /* [n][4] */);
 int hb200_get_covariance_blocks(hb200_ctx* ctx, int n, double* out /* [n][6][6] */, int* status /* [n], may be NULL */);
+/* Poses at two stamps: their joint covariance and the covariance of the relative pose between them (loop-closure gates,
+ * increment uncertainty).
+ *   hb200_set_covariance_stamp_pairs: registers n pairs (t_a, t_b) that every later hb200_compute_covariance computes with
+ *                             Sigma (n = 0 clears the list; with no list the compute runs exactly as without this call).
+ *                             Host-only: touches neither the build nor committed results.  -1 for n < 0, NULL stamps with
+ *                             n > 0 or a non-finite stamp (the previous list stays).
+ *   hb200_get_pose_pair_covariance: per pair, at the knots of the last successful compute --
+ *                             joint    [12][12]: covariance of [theta_a p_a | theta_b p_b] in the device tangent (R <- Exp(theta) R,
+ *                                      p <- p + rho).  Its diagonal blocks are hb200_interpolate_covariance at t_a and t_b, its
+ *                                      off-diagonal block J(t_a) Sigma_{span(a), span(b)} J(t_b)^T (knot pairs beyond the band
+ *                                      included); exactly symmetric, and (t_b, t_a) is exactly the permutation of (t_a, t_b).
+ *                             relative [6][6]: covariance of T_ab = T_a^-1 T_b (R_ab = R_a^T R_b, p_ab = R_a^T (p_b - p_a)) in
+ *                                      the same split tangent in frame a (R_ab <- Exp(dtheta) R_ab, p_ab <- p_ab + dp):
+ *                                      A joint A^T with A = [[-R_a^T, 0, R_a^T, 0], [R_a^T hat(p_b - p_a), -R_a^T, 0, R_a^T]],
+ *                                      R_a, p_a, p_b the interpolated poses; exactly symmetric.
+ *                             status [n]: 0 computed, 1 a stamp outside the pose spline's valid span (both blocks zero).
+ *                             joint, relative and status may each be NULL.  -2 before a successful compute and when n differs
+ *                             from the number of pairs that compute was given.  A snapshot like Sigma: a failed compute, a
+ *                             registration without a compute, later iterations, appends and slides leave the results as
+ *                             they are.
+ * Sharded contexts: no collective step is added; the pairs involve knots only, so the results are bit-identical on every
+ * rank. */
+int hb200_set_covariance_stamp_pairs(hb200_ctx* ctx, int n, const double* stamps /* [n][2]: t_a, t_b */);
+int hb200_get_pose_pair_covariance(hb200_ctx* ctx, int n, double* joint /* [n][12][12], may be NULL */, double* relative /* [n][6][6], may be NULL */,
+                                   int* status /* [n], may be NULL */);
 
 /* full LM iterations: evaluate -> build -> [allreduce] -> solve -> retract -> cost at trial ->
  * accept/reject, all on the device.  records may be NULL. */
@@ -320,6 +345,7 @@ int hb200_get_termination(hb200_ctx* ctx, int* type, int* iterations_performed, 
  *   - the packed buffer hb200_build_system leaves (hb200_system_device_ptr), hb200_get_system, hb200_solve / hb200_get_delta
  *   - hb200_iterate / hb200_optimize: records, termination and state
  *   - hb200_build_covariance + hb200_compute_covariance (hb200_get_covariance) and hb200_interpolate_covariance
+ *   - hb200_get_pose_pair_covariance (the stamp pairs of hb200_set_covariance_stamp_pairs)
  *   - sharded contexts: each rank's partial system; the peer-memory reduction sums the ranks in rank order.
  * Not covered: other GPU models or builds, the dense fallback solver (hb200_options.reserved bit 0) and the NCCL
  * all-reduce (as deterministic as NCCL's reduction).  It costs extra device memory for the slots and time for the
@@ -375,6 +401,8 @@ int hb200_ingest_stereo(hb200_ctx* ctx, int n, const double* stamp, const int* c
  *     and every rank must make the same sequence of hb200_iterate / hb200_optimize / hb200_build_system /
  *     hb200_build_covariance / hb200_compute_covariance calls.  The covariance build takes one system reduction
  *     (like hb200_build_system) and leaves the LM's trust-region state alone; the compute has no collective step.
+ *     Registered stamp pairs (hb200_set_covariance_stamp_pairs) need not be the same on every rank; a pair's results
+ *     are bit-identical on every rank that registered it.
  *     A rank that fails a call for a reason of its own (an invalid argument, a stale build) breaks the contract as
  *     in hb200_iterate; the peer reduction's timeout and the callback's error return keep the others from waiting
  *     forever.

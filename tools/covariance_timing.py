@@ -4,9 +4,10 @@ events around each call (host copies included), on cfg1, cfg2 and a K = 500 wind
 limit first; one JSON line per window.  --baseline-lib PATH alternates, round by round, with contexts of another build
 of libhyperb200.so (the calls it lacks are skipped) and prints its line (lib = "baseline") after each window's.
 --blocks times the compute alone with requested blocks outside the pattern (see blocks()), after the card, its power
-limit and SM clocks.
+limit and SM clocks.  --stamp-pairs N times the compute alone without and with N registered stamp pairs (see
+stamp_pairs()); with --baseline-lib the compute without pairs alternates with the other build's.
 
-    python tools/covariance_timing.py [--reps 5] [--baseline-lib PATH] [--blocks]
+    python tools/covariance_timing.py [--reps 5] [--baseline-lib PATH] [--blocks | --stamp-pairs N]
 """
 import argparse
 import json
@@ -87,25 +88,83 @@ def blocks(reps):
         ctx.close()
 
 
+def load_baseline(path):
+    import ctypes
+    base = ctypes.CDLL(os.path.abspath(path))   # RTLD_LOCAL: both builds' symbols stay apart
+    for fn, res in (("hb200_last_error_string", ctypes.c_char_p), ("hb200_stream", ctypes.c_void_p), ("hb200_launch_count", ctypes.c_longlong)):
+        getattr(base, fn).restype = res
+    base.hb200_launch_count.argtypes = [ctypes.c_void_p]
+    base.hb200_destroy.argtypes, base.hb200_destroy.restype = [ctypes.c_void_p], None
+    return base
+
+
+def stamp_pairs(reps, npairs, baseline_lib):
+    """--stamp-pairs N: hb200_compute_covariance on cfg1 and the K = 500 window without stamp pairs and with N pairs drawn
+    uniformly over the valid span (most of them more than beta knots apart, so the far-column march runs); with a
+    baseline build, its compute without pairs alternates round by round with this build's."""
+    import torch
+    from hyperslam_b200 import runtime
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True,
+                       timeout=30)
+    print(f"# {q.stdout.strip().splitlines()[0]}")
+    libs = dict(current=runtime.load_library())
+    if baseline_lib:
+        libs["baseline"] = load_baseline(baseline_lib)
+    for name in ("cfg1", "K500"):
+        win = window(name)
+        kt, k = win.knots[:, 7], win.order
+        left = (k - 1) // 2
+        pairs = np.random.default_rng(11).uniform(kt[left], kt[len(kt) - k + left + 1], (npairs, 2))
+        runs = []   # (lib, case, context)
+        for lib_name, lib in libs.items():
+            runtime._lib = lib          # a Context keeps the library it was created with
+            for case in (("none", "pairs") if lib_name == "current" else ("none",)):
+                ctx = runtime.Context(0)
+                ctx.load_window(win)
+                if case == "pairs":
+                    ctx.set_covariance_stamp_pairs(pairs)
+                runs.append((lib_name, case, ctx))
+        runtime._lib = libs["current"]
+        times = {(l, c): [] for l, c, _ in runs}
+        launches, info = {}, {}
+        for r in range(reps + 1):
+            for lib_name, case, ctx in runs:
+                stream = torch.cuda.ExternalStream(ctx.stream)
+                ctx.build_covariance()
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                l0 = ctx.launch_count
+                e0.record(stream)
+                info[lib_name, case] = ctx.compute_covariance()
+                e1.record(stream)
+                e1.synchronize()
+                launches[lib_name, case] = ctx.launch_count - l0
+                if r:   # first round: warm-up
+                    times[lib_name, case].append(e0.elapsed_time(e1))
+        for lib_name, case, ctx in runs:
+            computed = int((ctx.pose_pair_covariance()[2] == 0).sum()) if case == "pairs" else 0
+            print(json.dumps(dict(window=name, lib=lib_name, case=case, K=win.knots.shape[0], beta=info[lib_name, case]["beta"],
+                                  pairs=npairs if case == "pairs" else 0, computed=computed, status=info[lib_name, case]["status"],
+                                  launches=launches[lib_name, case], compute_ms=float(np.median(times[lib_name, case])),
+                                  spread_ms=float(np.ptp(times[lib_name, case])), reps=reps)))
+            ctx.close()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--baseline-lib", default=None)
     ap.add_argument("--blocks", action="store_true", help="time the compute with requested blocks outside the pattern")
+    ap.add_argument("--stamp-pairs", type=int, default=0, help="time the compute with this many registered stamp pairs")
     args = ap.parse_args()
     if args.blocks:
         return blocks(args.reps)
-    import ctypes
+    if args.stamp_pairs:
+        return stamp_pairs(args.reps, args.stamp_pairs, args.baseline_lib)
     import torch
     from hyperslam_b200 import runtime
     libs = dict(current=runtime.load_library())
     if args.baseline_lib:
-        base = ctypes.CDLL(os.path.abspath(args.baseline_lib))   # RTLD_LOCAL: both builds' symbols stay apart
-        for fn, res in (("hb200_last_error_string", ctypes.c_char_p), ("hb200_stream", ctypes.c_void_p), ("hb200_launch_count", ctypes.c_longlong)):
-            getattr(base, fn).restype = res
-        base.hb200_launch_count.argtypes = [ctypes.c_void_p]
-        base.hb200_destroy.argtypes, base.hb200_destroy.restype = [ctypes.c_void_p], None
-        libs["baseline"] = base
+        libs["baseline"] = load_baseline(args.baseline_lib)
     print(f"# {card()}")
     for name in ("cfg1", "cfg2", "K500"):
         win = window(name)
