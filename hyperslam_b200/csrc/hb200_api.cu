@@ -614,9 +614,8 @@ int launch_factors_merged(hb200_ctx* c, int sel, double* sys) {
   const PixelArgs pa = pixel_args<J>(c, sel, sys);
   const InertialArgs ia = inertial_args<J>(c, sel);
   const int blocks = c->n_pix_blocks + c->n_imu_blocks;
-  const size_t smem = J ? inertial_stash_bytes(K) : 0;
   return with_pixel_pass<J>(c, pa, [&](auto FUSE, auto DET) {
-    factor_eval_kernel<K, 4, J, FUSE, DET><<<blocks, kEvalThreads, smem, c->stream>>>(pa, ia, c->basis, c->bias_basis, c->n_pix_blocks, DET ? c->det_pix : DetOut{},
+    factor_eval_kernel<K, 4, J, FUSE, DET><<<blocks, kEvalThreads * factor_lanes(K), 0, c->stream>>>(pa, ia, c->basis, c->bias_basis, c->n_pix_blocks, DET ? c->det_pix : DetOut{},
                                                                                      DET ? c->det_seg_off.p : nullptr);
     return check_launch(c, DET ? "factor_eval_det_kernel" : "factor_eval_kernel");
   });
@@ -638,8 +637,9 @@ int launch_manifold(hb200_ctx* c, int sel) {
 int enqueue_factors(hb200_ctx* c, bool want_J, int sel, double* sys = nullptr) {
   int rc = 0;
   const bool J_any = want_J || sys;
-  // Small windows are latency-bound: one launch for both factor families.  Large windows are throughput-bound: the
-  // merged kernel would run the pixel CTAs at the inertial body's 255 registers, so the families stay separate.
+  // Small windows are latency-bound: one launch for both factor families, each factor on a lane group.  Large windows
+  // are throughput-bound: one factor per thread, the families in separate kernels (a lane group repeats the work that
+  // does not depend on the spline step on every lane, which costs issue slots there).
   if (c->Nv && c->Ni && c->n_pix_blocks + c->n_imu_blocks <= 4 * c->num_sms) {   // (also while profiling: same kernels as the graph)
     // visual and inertial factors side by side in one launch; pose factors (if any) on the side stream
     if (c->Nm && (rc = fork_side(c))) return rc;
@@ -1157,15 +1157,11 @@ int create_impl(const hb200_options* options, hb200_ctx* c) {
   if (rc) return rc;
   if (options && options->nccl_comm && (rc = hb200_set_nccl_comm(c, options->nccl_comm, options->nranks, options->rank))) return rc;
   HB_CUDA(cudaFuncSetAttribute(cholesky_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kCholSmem)));
-  // the Jacobian passes of the inertial factors park their forward-sweep state in dynamic shared memory (41.5 KB at
-  // order 4, 69 KB at order 6); together with the static scratch of the merged kernel that is above the 48 KB default
+  // the Jacobian pass of the large-window inertial kernel parks its forward-sweep state in dynamic shared memory (41.5 KB
+  // at order 4, 69 KB at order 6: above the 48 KB default)
   rc = for_each_order_mode([&](auto K, auto DET) {
-    const int stash = static_cast<int>(inertial_stash_bytes(K));
-    HB_CUDA(cudaFuncSetAttribute(factor_eval_kernel<K, 4, true, true, DET>, cudaFuncAttributeMaxDynamicSharedMemorySize, stash));
-    if constexpr (!DET) {   // the Jacobian passes without a fused J^T J have no deterministic instantiation
-      HB_CUDA(cudaFuncSetAttribute(factor_eval_kernel<K, 4, true, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, stash));
-      HB_CUDA(cudaFuncSetAttribute(inertial_eval_kernel<K, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, stash));
-    }
+    if constexpr (!DET)
+      HB_CUDA(cudaFuncSetAttribute(inertial_eval_kernel<K, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(inertial_stash_bytes(K))));
     return 0;
   });
   return rc ? rc : reset_solver_state(c);

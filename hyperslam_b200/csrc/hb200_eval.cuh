@@ -1,5 +1,6 @@
 // Factor evaluation kernels (sm_90a): knot table, index maps, stereo-pixel and inertial
-// residual + Jacobian.  One factor per thread; a CTA's knot-table tile is staged to shared memory
+// residual + Jacobian.  Large windows evaluate one factor per thread (pixel_eval_kernel, inertial_eval_kernel); small
+// windows one factor per lane group (factor_eval_kernel).  A CTA's knot-table tile is staged to shared memory
 // with one TMA bulk copy (cp.async.bulk + mbarrier).  Replaces, for a whole factor list at once,
 //   ExteroceptiveCost::Evaluate           reference internal/hyper/optimizers/ceres/costs/exteroceptive.cpp:101-160
 //   VisualPixelEvaluator<SE3>::evaluate   reference internal/hyper/optimizers/evaluators/pixel.cpp:16-146
@@ -95,6 +96,24 @@ HB_DI void block_min_max(int v_min, int v_max, int* s_red /*2 ints*/, int* out_m
   __syncthreads();
   *out_min = s_red[0];
   *out_max = s_red[1];
+}
+
+// Barrier of a CTA's first kEvalThreads threads (the whole CTA of the one-factor-per-thread kernels): the work that
+// follows the factor evaluation of a 64-factor tile -- cost sum, fused J^T J -- runs on those threads only.
+HB_DI void sync_tile() { asm volatile("bar.sync 1, %0;" ::"n"(kEvalThreads) : "memory"); }
+
+// Cost of a 64-factor tile, summed in a fixed order: thread t < kEvalThreads holds factor t's cost; thread 0 writes the
+// sum to *out.  Call from threads [0, kEvalThreads).
+HB_DI void tile_cost_sum(double cost, double* s_cost /*kEvalThreads / 32*/, double* out) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) cost += __shfl_xor_sync(0xffffffffu, cost, o);
+  if ((threadIdx.x & 31) == 0) s_cost[threadIdx.x >> 5] = cost;
+  sync_tile();
+  if (threadIdx.x == 0) {
+    double c = 0;
+    for (int w = 0; w < kEvalThreads / 32; ++w) c += s_cost[w];
+    *out = c;
+  }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -267,47 +286,46 @@ HB_DI void st_v4(double* p, double a, double b, double c, double d) {
   asm volatile("st.global.v2.f64 [%0], {%1, %2};\n\tst.global.v2.f64 [%0+16], {%3, %4};" ::"l"(p), "d"(a), "d"(b), "d"(c), "d"(d) : "memory");
 }
 
+// ---- per-step math, shared by the one-factor-per-thread bodies and the lane-group bodies of the small-window kernel ----
+// Step j of the forward sweep: A = Exp(lam_j d_j) and, with Jr, Jr(lam_j d_j)   (rj: knot-table row j of the factor)
+HB_DI void spline_step_exp(const double* rj, double lj, double* A, double* Jr) {
+  const double w[3] = {lj * rj[12], lj * rj[13], lj * rj[14]};
+  so3_exp_and_Jr(w, A, Jr);
+}
+// pixel block of step j: M_j = lam_j P_j Jr_j G_j   (P_j: pose rotation after step j)
+HB_DI void pixel_step_block(const double* rj, double lj, const double* Pj, const double* Jr, double* M) {
+  double G[9], JG[9], PJG[9];
+#pragma unroll
+  for (int i = 0; i < 9; ++i) G[i] = rj[15 + i];
+  m3_mul(Jr, G, JG);
+  m3_mul(Pj, JG, PJG);
+#pragma unroll
+  for (int i = 0; i < 9; ++i) M[i] = lj * PJG[i];
+}
+// EM = E M (2x3)
+HB_DI void pixel_em(const double* E, const double* M, double* EM) {
+#pragma unroll
+  for (int i = 0; i < 2; ++i)
+#pragma unroll
+    for (int c = 0; c < 3; ++c) EM[3 * i + c] = E[3 * i] * M[c] + E[3 * i + 1] * M[3 + c] + E[3 * i + 2] * M[6 + c];
+}
+// columns of control point m in Jacobian row i: rotation cur - nxt (E M_m - E M_{m+1}, E M_0 = E, E M_K = 0),
+// translation -(lam_m - lam_{m+1}) F
+HB_DI void pixel_row_block(const double* cur, const double* nxt, double dl, const double* F, int i, double* out) {
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    out[c] = cur[3 * i + c] - nxt[3 * i + c];
+    out[3 + c] = -dl * F[3 * i + c];
+  }
+}
+
 // kind 0: pixel residual (reference pixel.cpp:16-146 + CartesianMetric); kind 1: bearing residual
 // (reference bearing.cpp:14-79 + AngularMetric): r = [angle(p_s, z), 0], second Jacobian row zero, so a
 // bearing factor travels through the same compact [2][6K] / [2][3] layout and the same J^T J / Schur code.
-template <int K, bool WANT_J>
-HB_DI void pixel_factor(const double* __restrict__ T, const Basis& B, int base, double t, double zx, double zy, double zz, int kind,
-                        const double* __restrict__ cam, const double* __restrict__ lmk, double* r, double* __restrict__ Jp,
-                        double* __restrict__ Jl) {
-  constexpr int left = (K - 1) / 2;
-  const double* row0 = T + static_cast<size_t>(base) * kTabStride;
-  const double t0 = row0[left * kTabStride + 24], t1 = row0[(left + 1) * kTabStride + 24];
-  const double inv_dt = 1.0 / (t1 - t0);
-  const double u = (t - t0) * inv_dt;
-  double lam[K + 1];
-  basis_eval<K, false>(B, u, inv_dt, lam, nullptr, nullptr);
-
-  double P[9], p[3];
-#pragma unroll
-  for (int i = 0; i < 9; ++i) P[i] = row0[i];
-  p[0] = row0[9]; p[1] = row0[10]; p[2] = row0[11];
-  double M[(K - 1) * 9];
-#pragma unroll
-  for (int j = 1; j < K; ++j) {
-    const double* rj = row0 + j * kTabStride;
-    const double w[3] = {lam[j] * rj[12], lam[j] * rj[13], lam[j] * rj[14]};
-    double A[9], Jr[9], Pn[9];
-    so3_exp_and_Jr(w, A, WANT_J ? Jr : nullptr);
-    m3_mul(P, A, Pn);
-    if (WANT_J) {
-      double G[9], JG[9], PJG[9];
-#pragma unroll
-      for (int i = 0; i < 9; ++i) G[i] = rj[15 + i];
-      m3_mul(Jr, G, JG);
-      m3_mul(Pn, JG, PJG);
-#pragma unroll
-      for (int i = 0; i < 9; ++i) M[(j - 1) * 9 + i] = lam[j] * PJG[i];
-    }
-#pragma unroll
-    for (int i = 0; i < 9; ++i) P[i] = Pn[i];
-#pragma unroll
-    for (int c = 0; c < 3; ++c) p[c] += lam[j] * (rj[9 + c] - rj[9 + c - kTabStride]);
-  }
+// Residual at the pose (P, p) and, WANT_J, the landmark Jacobian F (2x3) and E = F hat(q).
+template <bool WANT_J>
+HB_DI void pixel_project(const double* P, const double* p, const double* __restrict__ lmk, const double* __restrict__ cam, double zx, double zy,
+                         double zz, int kind, double* r, double* E, double* F) {
   // p_s = R_sb (R^T (p_w - p) - t_bs)
   const double q[3] = {lmk[0] - p[0], lmk[1] - p[1], lmk[2] - p[2]};
   double pb[3], ps[3];
@@ -357,7 +375,7 @@ HB_DI void pixel_factor(const double* __restrict__ T, const Basis& B, int base, 
       for (int i = 0; i < 3; ++i) Jps[i] = (c * zn[i] - s * z[i]) * iden;
     }
   }
-  double Jpb[6], F[6], E[6];
+  double Jpb[6];
 #pragma unroll
   for (int i = 0; i < 2; ++i)
 #pragma unroll
@@ -372,30 +390,54 @@ HB_DI void pixel_factor(const double* __restrict__ T, const Basis& B, int base, 
     E[3 * i + 1] = F[3 * i + 2] * q[0] - F[3 * i] * q[2];
     E[3 * i + 2] = F[3 * i] * q[1] - F[3 * i + 1] * q[0];
   }
+}
+
+// One thread per factor.
+template <int K, bool WANT_J>
+HB_DI void pixel_factor(const double* __restrict__ T, const Basis& B, int base, double t, double zx, double zy, double zz, int kind,
+                        const double* __restrict__ cam, const double* __restrict__ lmk, double* r, double* __restrict__ Jp,
+                        double* __restrict__ Jl) {
+  constexpr int left = (K - 1) / 2;
+  const double* row0 = T + static_cast<size_t>(base) * kTabStride;
+  const double t0 = row0[left * kTabStride + 24], t1 = row0[(left + 1) * kTabStride + 24];
+  const double inv_dt = 1.0 / (t1 - t0);
+  const double u = (t - t0) * inv_dt;
+  double lam[K + 1];
+  basis_eval<K, false>(B, u, inv_dt, lam, nullptr, nullptr);
+
+  double P[9], p[3];
+#pragma unroll
+  for (int i = 0; i < 9; ++i) P[i] = row0[i];
+  p[0] = row0[9]; p[1] = row0[10]; p[2] = row0[11];
+  double M[(K - 1) * 9];
+#pragma unroll
+  for (int j = 1; j < K; ++j) {
+    const double* rj = row0 + j * kTabStride;
+    double A[9], Jr[9], Pn[9];
+    spline_step_exp(rj, lam[j], A, WANT_J ? Jr : nullptr);
+    m3_mul(P, A, Pn);
+    if (WANT_J) pixel_step_block(rj, lam[j], Pn, Jr, &M[(j - 1) * 9]);
+#pragma unroll
+    for (int i = 0; i < 9; ++i) P[i] = Pn[i];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) p[c] += lam[j] * (rj[9 + c] - rj[9 + c - kTabStride]);
+  }
+  double E[6], F[6];
+  pixel_project<WANT_J>(P, p, lmk, cam, zx, zy, zz, kind, r, E, F);
+  if (!WANT_J) return;
 #pragma unroll
   for (int i = 0; i < 6; ++i) Jl[i] = F[i];
   // E M_j (2x3 each)
-  double EM[(K - 1) * 6];
+  double EM[(K + 1) * 6];
 #pragma unroll
-  for (int j = 0; j < K - 1; ++j)
+  for (int i = 0; i < 6; ++i) { EM[i] = E[i]; EM[K * 6 + i] = 0.0; }
 #pragma unroll
-    for (int i = 0; i < 2; ++i)
-#pragma unroll
-      for (int c = 0; c < 3; ++c)
-        EM[j * 6 + 3 * i + c] = E[3 * i] * M[j * 9 + c] + E[3 * i + 1] * M[j * 9 + 3 + c] + E[3 * i + 2] * M[j * 9 + 6 + c];
+  for (int j = 1; j < K; ++j) pixel_em(E, &M[(j - 1) * 9], &EM[j * 6]);
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
     double row[6 * K];
 #pragma unroll
-    for (int m = 0; m < K; ++m) {
-#pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        const double cur = (m == 0) ? E[3 * i + c] : EM[(m - 1) * 6 + 3 * i + c];
-        const double nxt = (m + 1 < K) ? EM[m * 6 + 3 * i + c] : 0.0;
-        row[6 * m + c] = cur - nxt;
-        row[6 * m + 3 + c] = -(lam[m] - lam[m + 1]) * F[3 * i + c];
-      }
-    }
+    for (int m = 0; m < K; ++m) pixel_row_block(&EM[m * 6], &EM[(m + 1) * 6], lam[m] - lam[m + 1], F, i, &row[6 * m]);
     double* out = Jp + i * 6 * K;   // 32-byte aligned: rows are 192 B (K=4) / 288 B (K=6)
 #pragma unroll
     for (int g = 0; g < 6 * K / 4; ++g) st_v4(out + 4 * g, row[4 * g], row[4 * g + 1], row[4 * g + 2], row[4 * g + 3]);
@@ -532,7 +574,7 @@ HB_DI void cta_pixel_hessian(const PixelArgs& a, int f0, int cnt, double* sJ /*[
   const int prev = __shfl_up_sync(0xffffffffu, my_base, 1);
   __shared__ int s_edge[2], s_warp_cnt;
   if (lane == 31) s_edge[warp] = my_base;
-  __syncthreads();   // (also: previous use of the scratch is complete; s_sw is visible)
+  sync_tile();   // (also: previous use of the scratch is complete; s_sw is visible)
   // staging: the CTA's 2 * cnt Jacobian rows are one contiguous run of global memory (just written: L2 hits) -- copied
   // cooperatively with coalesced 128-bit loads, scaled by sqrt(w) of their factor, pitch LD in shared memory
   {
@@ -550,13 +592,13 @@ HB_DI void cta_pixel_hessian(const PixelArgs& a, int f0, int cnt, double* sJ /*[
   const bool start = tid < cnt && my_base != before;
   const unsigned mask = __ballot_sync(0xffffffffu, start);
   if (warp == 0 && lane == 0) s_warp_cnt = __popc(mask);
-  __syncthreads();
+  sync_tile();
   const int pos = __popc(mask & ((1u << lane) - 1u)) + (warp ? s_warp_cnt : 0);
   if (start) sseg[pos] = tid;
   if (tid == 0) sseg[65] = 0;
-  __syncthreads();
+  sync_tile();
   if (warp == 1 && lane == 0) { const int n = s_warp_cnt + __popc(mask); sseg[n] = cnt; sseg[65] = n; }
-  __syncthreads();
+  sync_tile();
   const int nseg = sseg[65];
   const int lm = lane >> 2, lk = lane & 3;
   for (int j = 0; j < nseg; ++j) {
@@ -622,19 +664,10 @@ HB_DI void pixel_eval_body(const PixelArgs& a, const Basis& B, int bid0, const D
     cost = 0.5 * huber_rho(r[0] * r[0] + r[1] * r[1], (id.w != 0) ? a.huber_bearing : a.huber, &wgt);
     if (WANT_J) a.w[f] = wgt;
   }
-  // deterministic block reduction of the cost
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) cost += __shfl_xor_sync(0xffffffffu, cost, o);
-  if ((threadIdx.x & 31) == 0) s_cost[threadIdx.x >> 5] = cost;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double c = 0;
-    for (int w = 0; w < kEvalThreads / 32; ++w) c += s_cost[w];
-    a.cost_partial[bid] = c;
-  }
+  tile_cost_sum(cost, s_cost, &a.cost_partial[bid]);
   if (FUSE && a.sys != nullptr) {
     // fused normal equations of this CTA's factors (residuals / Jacobians were written above; the barrier in the
-    // cost reduction ordered them for the whole CTA)
+    // cost sum ordered them for the whole CTA)
     const int f_lo = bid * kEvalThreads;
     cta_pixel_hessian<K, DET>(a, f_lo, min(kEvalThreads, a.n - f_lo), s_J, s_r, s_b, acc, det, DET ? seg_off[bid] : 0);
   }
@@ -702,6 +735,215 @@ HB_DI void sphere_plus_jacobian(const double* x, double* J /*3x2*/) {
     for (int r = 0; r < 3; ++r) J[2 * r + c] = nx * ((r == c ? 1.0 : 0.0) - beta * v[c] * v[r]);
 }
 
+// ---- per-step math, shared by the one-factor-per-thread body and the lane-group body of the small-window kernel ----
+// body-rate recursion of step j: aw = A_j^T w, awd = A_j^T wd, then w <- aw + lamd_j d_j, wd <- awd + lamd_j (w x d_j) + lamdd_j d_j
+HB_DI void inertial_rate_step(const double* A, const double* d, double ld, double ldd, double* w, double* wd, double* aw, double* awd) {
+  double wn[3], cr[3];
+  m3_tvec(A, w, aw);
+  m3_tvec(A, wd, awd);
+#pragma unroll
+  for (int c = 0; c < 3; ++c) wn[c] = aw[c] + ld * d[c];
+  cross(wn, d, cr);
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    wd[c] = awd[c] + ld * cr[c] + ldd * d[c];
+    w[c] = wn[c];
+  }
+}
+
+// Residual (reference inertial.cpp:62-79) from the pose rotation P, body rates w / wd and acceleration pdd at the stamp;
+// a_i = R^T (pdd - g) for the coefficient matrices.  wg_out / wa_out (or null): the bias splines' basis weights.
+template <int KB>
+HB_DI void inertial_residual(const double* P, const double* w, const double* wd, const double* pdd, const Basis& BB, int gb, int ab, double t,
+                             const double* __restrict__ z, const double* __restrict__ I, const double* __restrict__ bg, const double* __restrict__ ba,
+                             const double* __restrict__ grav, double* r, double* a_i, double* __restrict__ wg_out, double* __restrict__ wa_out) {
+  // ---- bias splines (value + basis weights) ----
+  double bgv[3] = {0, 0, 0}, bav[3] = {0, 0, 0};
+  {
+    constexpr int lb = (KB - 1) / 2;
+    double lb_[KB + 1];
+    const double* g0 = bg + 4 * static_cast<size_t>(gb);
+    const double s0 = g0[4 * lb + 3], s1 = g0[4 * (lb + 1) + 3];
+    basis_eval<KB, false>(BB, (t - s0) / (s1 - s0), 0.0, lb_, nullptr, nullptr);
+#pragma unroll
+    for (int m = 0; m < KB; ++m) {
+      const double wv = lb_[m] - lb_[m + 1];
+      if (wg_out) wg_out[m] = wv;
+#pragma unroll
+      for (int c = 0; c < 3; ++c) bgv[c] += wv * g0[4 * m + c];
+    }
+    const double* a0 = ba + 4 * static_cast<size_t>(ab);
+    const double u0 = a0[4 * lb + 3], u1 = a0[4 * (lb + 1) + 3];
+    basis_eval<KB, false>(BB, (t - u0) / (u1 - u0), 0.0, lb_, nullptr, nullptr);
+#pragma unroll
+    for (int m = 0; m < KB; ++m) {
+      const double wv = lb_[m] - lb_[m + 1];
+      if (wa_out) wa_out[m] = wv;
+#pragma unroll
+      for (int c = 0; c < 3; ++c) bav[c] += wv * a0[4 * m + c];
+    }
+  }
+  const double* IgR = I + 12;
+  const double* IaR = I + 21;
+  const double* Sg = I + 30;
+  const double* lever = I + 39;  // row i = c_i
+  const double gm[3] = {pdd[0] - grav[0], pdd[1] - grav[1], pdd[2] - grav[2]};
+  double a_m[3];
+  m3_tvec(P, gm, a_i);  // R^T (pdd - g) = A_lin - R_bw g
+  double Fa[9];
+  {
+    const double ww = w[0] * w[0] + w[1] * w[1] + w[2] * w[2];
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+#pragma unroll
+      for (int j = 0; j < 3; ++j) Fa[3 * i + j] = w[i] * w[j] - (i == j ? ww : 0.0);
+    Fa[1] -= wd[2]; Fa[2] += wd[1]; Fa[3] += wd[2]; Fa[5] -= wd[0]; Fa[6] -= wd[1]; Fa[7] += wd[0];
+  }
+#pragma unroll
+  for (int i = 0; i < 3; ++i) a_m[i] = a_i[i] + Fa[3 * i] * lever[3 * i] + Fa[3 * i + 1] * lever[3 * i + 1] + Fa[3 * i + 2] * lever[3 * i + 2];
+  double t1v[3], t2v[3], t3v[3];
+  m3_vec(IgR, w, t1v);
+  m3_vec(Sg, a_m, t2v);
+  m3_vec(IaR, a_m, t3v);
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    r[c] = t1v[c] + t2v[c] + bgv[c] - z[c];
+    r[3 + c] = t3v[c] + bav[c] - z[3 + c];
+  }
+}
+
+// Coefficient matrices (rows 0-2 gyro, 3-5 accel):  d a_m / d theta = hat(a_i) R^T = Bm ; d a_m / d omega = Kw ;
+// d a_m / d alpha = Kal ; d a_m / d pdd_w = R^T.
+HB_DI void inertial_coeffs(const double* P, const double* a_i, const double* w, const double* __restrict__ I, double* Bm, double* Kw, double* Kal) {
+  const double* leverJ = I + 66;
+  {
+    double Rt[9];
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+#pragma unroll
+      for (int j = 0; j < 3; ++j) Rt[3 * i + j] = P[3 * j + i];
+    hat_mul(a_i, Rt, Bm);
+  }
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+    const double* c = leverJ + 3 * i;
+    // row i of -(2 w^ c^ - c^ w^) ; (w^ c^) = c w^T - (w.c) I ; (c^ w^) = w c^T - (w.c) I
+    const double wc = w[0] * c[0] + w[1] * c[1] + w[2] * c[2];
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+      const double wxcx = c[i] * w[j] - (i == j ? wc : 0.0);
+      const double cxwx = w[i] * c[j] - (i == j ? wc : 0.0);
+      Kw[3 * i + j] = -(2.0 * wxcx - cxwx);
+    }
+    // row i of -c^
+    Kal[3 * i] = (i == 0) ? 0.0 : (i == 1 ? -c[2] : c[1]);
+    Kal[3 * i + 1] = (i == 0) ? c[2] : (i == 1 ? 0.0 : -c[0]);
+    Kal[3 * i + 2] = (i == 0) ? -c[1] : (i == 1 ? c[0] : 0.0);
+  }
+}
+// Translation coefficients Cp = [S_g R^T ; I_a R_sb R^T] (6x3) and, Jg non-null, the gravity Jacobian.
+HB_DI void inertial_trans(const double* P, const double* __restrict__ I, const double* __restrict__ grav, double* Cp, double* __restrict__ Jg) {
+  const double* IaR = I + 21;
+  const double* SgJ = I + 57;
+  m3_mult(SgJ, P, &Cp[0]);  // S_g R^T
+  m3_mult(IaR, P, &Cp[9]);  // I_a R_sb R^T (inertial.cpp:150,198 use I_a in every variant)
+  // gravity tangent Jacobian: -(Cp) * PlusJacobian_sphere(g)   (6x2)
+  if (Jg) {
+    double PJ[6];
+    sphere_plus_jacobian(grav, PJ);
+#pragma unroll
+    for (int i = 0; i < 6; ++i)
+#pragma unroll
+      for (int c = 0; c < 2; ++c) Jg[2 * i + c] = -(Cp[3 * i] * PJ[c] + Cp[3 * i + 1] * PJ[2 + c] + Cp[3 * i + 2] * PJ[4 + c]);
+  }
+}
+
+// Backward step j, first half: the step's frames TG_j, XG_j, YG_j from what the forward sweep left for it
+// (lj = lam_j Jr(lam_j d_j), atw = A_j^T w_{j-1}, atwd = A_j^T wd_{j-1}, wat = w_j) and the state (Pc, QT, Z) of the
+// backward steps after it.
+HB_DI void inertial_back_frames(const double* rj, const double* lj, const double* atw, const double* atwd, const double* wat, double ld, double ldd,
+                                const double* Pc, const double* QT, const double* Z, double* TG, double* XG, double* YG) {
+  const double d[3] = {rj[12], rj[13], rj[14]};
+  double X[9], Y[9], tmp[9], tmp2[9];
+  hat_mul(atw, lj, X);
+#pragma unroll
+  for (int i = 0; i < 3; ++i) X[4 * i] += ld;
+  hat_mul(atwd, lj, Y);
+  hat_mul(d, X, tmp);
+  hat(wat, tmp2);
+#pragma unroll
+  for (int i = 0; i < 9; ++i) Y[i] += ld * (tmp2[i] - tmp[i]);
+#pragma unroll
+  for (int i = 0; i < 3; ++i) Y[4 * i] += ldd;
+  double Xf[9], Yf[9], Tf[9];
+  m3_mul(QT, X, Xf);
+  m3_mul(Z, X, Yf);
+  m3_mul(QT, Y, tmp);
+#pragma unroll
+  for (int i = 0; i < 9; ++i) Yf[i] += tmp[i];
+  m3_mul(Pc, lj, Tf);
+  double G[9];
+#pragma unroll
+  for (int i = 0; i < 9; ++i) G[i] = rj[15 + i];
+  m3_mul(Tf, G, TG);
+  m3_mul(Xf, G, XG);
+  m3_mul(Yf, G, YG);
+}
+// Backward step j, second half: its rotation block D_j (6x3).  The 6 x 3 coefficient matrices [S_g ; I R_sb]
+// {Bm, Kw, Kal} (+ I_g R_sb for the rate) are NOT materialised: with
+//   M_j = Bm TG_j + Kw XG_j + Kal YG_j      the block of step j is   [S_g M_j + I_g R_sb XG_j ; I_lin R_sb M_j]
+// -- six 3x3 products per step instead of nine 6x3x3 ones.
+HB_DI void inertial_back_rows(const double* TG, const double* XG, const double* YG, const double* Bm, const double* Kw, const double* Kal,
+                              const double* __restrict__ I, double* D) {
+  const double* IgR = I + 12;
+  const double* IlinR = I + 48;  // Jacobian-side matrices (== IaR, Sg unless a reference quirk is switched on)
+  const double* SgJ = I + 57;
+  double M[9], t9[9];
+  m3_mul(Bm, TG, M);
+  m3_mul(Kw, XG, t9);
+#pragma unroll
+  for (int i = 0; i < 9; ++i) M[i] += t9[i];
+  m3_mul(Kal, YG, t9);
+#pragma unroll
+  for (int i = 0; i < 9; ++i) M[i] += t9[i];
+  m3_mul(SgJ, M, &D[0]);
+  m3_mul(IgR, XG, t9);
+#pragma unroll
+  for (int i = 0; i < 9; ++i) D[i] += t9[i];
+  m3_mul(IlinR, M, &D[9]);
+}
+// D_0 = [S_g ; I_lin R_sb] Bm: block 0's rotation is D_0 - D_1
+HB_DI void inertial_block0(const double* Bm, const double* __restrict__ I, double* D) {
+  m3_mul(I + 57, Bm, &D[0]);
+  m3_mul(I + 48, Bm, &D[9]);
+}
+// backward state past step j:  Pc <- Pc A_j^T ; Z <- (Z - lamd_j QT d_j^) A_j^T ; QT <- QT A_j^T
+HB_DI void inertial_suffix_step(const double* A, const double* d, double ld, double* Pc, double* QT, double* Z) {
+  double tmp[9], tmp2[9];
+  m3_mult(Pc, A, tmp);
+#pragma unroll
+  for (int i = 0; i < 9; ++i) Pc[i] = tmp[i];
+  mul_hat(QT, d, tmp);
+#pragma unroll
+  for (int i = 0; i < 9; ++i) tmp2[i] = Z[i] - ld * tmp[i];
+  m3_mult(tmp2, A, Z);
+  m3_mult(QT, A, tmp);
+#pragma unroll
+  for (int i = 0; i < 9; ++i) QT[i] = tmp[i];
+}
+// columns of control point m: rotation dD = D_m - D_{m+1}, translation (lamdd_m - lamdd_{m+1}) Cp
+template <int K>
+HB_DI void inertial_store_block(double* __restrict__ Jp, int m, const double* dD, double wdd, const double* Cp) {
+#pragma unroll
+  for (int i = 0; i < 6; ++i) {
+    double2* out = reinterpret_cast<double2*>(Jp + i * 6 * K + 6 * m);
+    out[0] = make_double2(dD[3 * i], dD[3 * i + 1]);
+    out[1] = make_double2(dD[3 * i + 2], wdd * Cp[3 * i]);
+    out[2] = make_double2(wdd * Cp[3 * i + 1], wdd * Cp[3 * i + 2]);
+  }
+}
+
+// One thread per factor.
 template <int K, int KB, bool WANT_J>
 HB_DI void inertial_factor(const double* __restrict__ T, const Basis& B, const Basis& BB, int base, int gb, int ab, double t,
                            const double* __restrict__ z, const double* __restrict__ I, const double* __restrict__ bg,
@@ -729,139 +971,29 @@ HB_DI void inertial_factor(const double* __restrict__ T, const Basis& B, const B
   for (int j = 1; j < K; ++j) {
     const double* rj = row0 + j * kTabStride;
     const double d[3] = {rj[12], rj[13], rj[14]};
-    const double lw[3] = {lam[j] * d[0], lam[j] * d[1], lam[j] * d[2]};
     double Aj[9], Jr[9], Pn[9];
-    so3_exp_and_Jr(lw, Aj, WANT_J ? Jr : nullptr);
+    spline_step_exp(rj, lam[j], Aj, WANT_J ? Jr : nullptr);
     m3_mul(P, Aj, Pn);
 #pragma unroll
     for (int i = 0; i < 9; ++i) P[i] = Pn[i];
-    double aw[3], awd[3], wn[3], cr[3];
-    m3_tvec(Aj, w, aw);
-    m3_tvec(Aj, wd, awd);
+    double aw[3], awd[3];
+    inertial_rate_step(Aj, d, lamd[j], lamdd[j], w, wd, aw, awd);
 #pragma unroll
-    for (int c = 0; c < 3; ++c) wn[c] = aw[c] + lamd[j] * d[c];
-    cross(wn, d, cr);
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-      wd[c] = awd[c] + lamd[j] * cr[c] + lamdd[j] * d[c];
-      w[c] = wn[c];
-      pdd[c] += lamdd[j] * (rj[9 + c] - rj[9 + c - kTabStride]);
-    }
+    for (int c = 0; c < 3; ++c) pdd[c] += lamdd[j] * (rj[9 + c] - rj[9 + c - kTabStride]);
     if (WANT_J) {
       double* sj = stash + (j - 1) * 27 * kEvalThreads;
 #pragma unroll
       for (int i = 0; i < 9; ++i) { sj[i * kEvalThreads] = Aj[i]; sj[(9 + i) * kEvalThreads] = lam[j] * Jr[i]; }
 #pragma unroll
-      for (int c = 0; c < 3; ++c) { sj[(18 + c) * kEvalThreads] = aw[c]; sj[(21 + c) * kEvalThreads] = awd[c]; sj[(24 + c) * kEvalThreads] = wn[c]; }
+      for (int c = 0; c < 3; ++c) { sj[(18 + c) * kEvalThreads] = aw[c]; sj[(21 + c) * kEvalThreads] = awd[c]; sj[(24 + c) * kEvalThreads] = w[c]; }
     }
   }
-  // ---- bias splines (value + basis weights) ----
-  double bgv[3] = {0, 0, 0}, bav[3] = {0, 0, 0};
-  {
-    constexpr int lb = (KB - 1) / 2;
-    double lb_[KB + 1];
-    const double* g0 = bg + 4 * static_cast<size_t>(gb);
-    const double s0 = g0[4 * lb + 3], s1 = g0[4 * (lb + 1) + 3];
-    basis_eval<KB, false>(BB, (t - s0) / (s1 - s0), 0.0, lb_, nullptr, nullptr);
-#pragma unroll
-    for (int m = 0; m < KB; ++m) {
-      const double wv = lb_[m] - lb_[m + 1];
-      if (WANT_J) wg_out[m] = wv;
-#pragma unroll
-      for (int c = 0; c < 3; ++c) bgv[c] += wv * g0[4 * m + c];
-    }
-    const double* a0 = ba + 4 * static_cast<size_t>(ab);
-    const double u0 = a0[4 * lb + 3], u1 = a0[4 * (lb + 1) + 3];
-    basis_eval<KB, false>(BB, (t - u0) / (u1 - u0), 0.0, lb_, nullptr, nullptr);
-#pragma unroll
-    for (int m = 0; m < KB; ++m) {
-      const double wv = lb_[m] - lb_[m + 1];
-      if (WANT_J) wa_out[m] = wv;
-#pragma unroll
-      for (int c = 0; c < 3; ++c) bav[c] += wv * a0[4 * m + c];
-    }
-  }
-  // ---- residual (reference inertial.cpp:62-79) ----
-  const double* Rsb = I;
-  const double* IgR = I + 12;
-  const double* IaR = I + 21;
-  const double* Sg = I + 30;
-  const double* lever = I + 39;  // row i = c_i
-  const double* IlinR = I + 48;  // Jacobian-side matrices (== IaR, Sg, lever unless a reference quirk is switched on)
-  const double* SgJ = I + 57;
-  const double* leverJ = I + 66;
-  const double gm[3] = {pdd[0] - grav[0], pdd[1] - grav[1], pdd[2] - grav[2]};
-  double a_i[3], a_m[3];
-  m3_tvec(P, gm, a_i);  // R^T (pdd - g) = A_lin - R_bw g
-  double Fa[9];
-  {
-    const double ww = w[0] * w[0] + w[1] * w[1] + w[2] * w[2];
-#pragma unroll
-    for (int i = 0; i < 3; ++i)
-#pragma unroll
-      for (int j = 0; j < 3; ++j) Fa[3 * i + j] = w[i] * w[j] - (i == j ? ww : 0.0);
-    Fa[1] -= wd[2]; Fa[2] += wd[1]; Fa[3] += wd[2]; Fa[5] -= wd[0]; Fa[6] -= wd[1]; Fa[7] += wd[0];
-  }
-#pragma unroll
-  for (int i = 0; i < 3; ++i) a_m[i] = a_i[i] + Fa[3 * i] * lever[3 * i] + Fa[3 * i + 1] * lever[3 * i + 1] + Fa[3 * i + 2] * lever[3 * i + 2];
-  {
-    double t1v[3], t2v[3], t3v[3];
-    m3_vec(IgR, w, t1v);
-    m3_vec(Sg, a_m, t2v);
-    m3_vec(IaR, a_m, t3v);
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-      r[c] = t1v[c] + t2v[c] + bgv[c] - z[c];
-      r[3 + c] = t3v[c] + bav[c] - z[3 + c];
-    }
-  }
+  double a_i[3];
+  inertial_residual<KB>(P, w, wd, pdd, BB, gb, ab, t, z, I, bg, ba, grav, r, a_i, wg_out, wa_out);
   if (!WANT_J) return;
-
-  // ---- coefficient matrices: rows 0-2 gyro, 3-5 accel ----
-  // d a_m / d theta = hat(a_i) R^T ; d a_m / d omega = Kw ; d a_m / d alpha = Kal ; d a_m / d pdd_w = R^T
-  double Bm[9];  // hat(a_i) R^T
-  {
-    double Rt[9];
-#pragma unroll
-    for (int i = 0; i < 3; ++i)
-#pragma unroll
-      for (int j = 0; j < 3; ++j) Rt[3 * i + j] = P[3 * j + i];
-    hat_mul(a_i, Rt, Bm);
-  }
-  double Kw[9], Kal[9];
-#pragma unroll
-  for (int i = 0; i < 3; ++i) {
-    const double* c = leverJ + 3 * i;
-    // row i of -(2 w^ c^ - c^ w^) ; (w^ c^) = c w^T - (w.c) I ; (c^ w^) = w c^T - (w.c) I
-    const double wc = w[0] * c[0] + w[1] * c[1] + w[2] * c[2];
-#pragma unroll
-    for (int j = 0; j < 3; ++j) {
-      const double wxcx = c[i] * w[j] - (i == j ? wc : 0.0);
-      const double cxwx = w[i] * c[j] - (i == j ? wc : 0.0);
-      Kw[3 * i + j] = -(2.0 * wxcx - cxwx);
-    }
-    // row i of -c^
-    Kal[3 * i] = (i == 0) ? 0.0 : (i == 1 ? -c[2] : c[1]);
-    Kal[3 * i + 1] = (i == 0) ? c[2] : (i == 1 ? 0.0 : -c[0]);
-    Kal[3 * i + 2] = (i == 0) ? -c[1] : (i == 1 ? c[0] : 0.0);
-  }
-  // The 6 x 3 coefficient matrices [S_g ; I R_sb] {Bm, Kw, Kal} (+ I_g R_sb for the rate) are NOT materialised: with
-  //   M_j = Bm TG_j + Kw XG_j + Kal YG_j      the block of step j is   [S_g M_j + I_g R_sb XG_j ; I_lin R_sb M_j]
-  // -- 54 fewer live doubles across the backward sweep (the calibration matrices sit in shared memory) and six 3x3
-  // products per step instead of nine 6x3x3 ones.
-  double Cp[18];
-  m3_mult(SgJ, P, &Cp[0]);  // S_g R^T
-  m3_mult(IaR, P, &Cp[9]);  // I_a R_sb R^T (inertial.cpp:150,198 use I_a in every variant)
-  (void)Rsb;
-  // gravity tangent Jacobian: -(Cp) * PlusJacobian_sphere(g)   (6x2)
-  {
-    double PJ[6];
-    sphere_plus_jacobian(grav, PJ);
-#pragma unroll
-    for (int i = 0; i < 6; ++i)
-#pragma unroll
-      for (int c = 0; c < 2; ++c) Jg[2 * i + c] = -(Cp[3 * i] * PJ[c] + Cp[3 * i + 1] * PJ[2 + c] + Cp[3 * i + 2] * PJ[4 + c]);
-  }
+  double Bm[9], Kw[9], Kal[9], Cp[18];
+  inertial_coeffs(P, a_i, w, I, Bm, Kw, Kal);
+  inertial_trans(P, I, grav, Cp, Jg);
   // ---- backward sweep over j = K-1 .. 1 ----
   double Pc[9], QT[9], Z[9], Dprev[18];
 #pragma unroll
@@ -871,98 +1003,35 @@ HB_DI void inertial_factor(const double* __restrict__ T, const Basis& B, const B
 #pragma unroll 1   // one step's live set at a time: fully unrolled, the scheduler interleaved the steps and spilled 2.4 KB per thread
   for (int j = K - 1; j >= 1; --j) {
     const double* rj = row0 + j * kTabStride;
-    const double d[3] = {rj[12], rj[13], rj[14]};
     const double* sj = stash + (j - 1) * 27 * kEvalThreads;
     double lj[9], atw[3], atwd[3], wat[3];
 #pragma unroll
     for (int i = 0; i < 9; ++i) lj[i] = sj[(9 + i) * kEvalThreads];
 #pragma unroll
     for (int c = 0; c < 3; ++c) { atw[c] = sj[(18 + c) * kEvalThreads]; atwd[c] = sj[(21 + c) * kEvalThreads]; wat[c] = sj[(24 + c) * kEvalThreads]; }
-    double X[9], Y[9], tmp[9], tmp2[9];
-    hat_mul(atw, lj, X);
-#pragma unroll
-    for (int i = 0; i < 3; ++i) X[4 * i] += lamd[j];
-    hat_mul(atwd, lj, Y);
-    hat_mul(d, X, tmp);
-    hat(wat, tmp2);
-#pragma unroll
-    for (int i = 0; i < 9; ++i) Y[i] += lamd[j] * (tmp2[i] - tmp[i]);
-#pragma unroll
-    for (int i = 0; i < 3; ++i) Y[4 * i] += lamdd[j];
-    double Xf[9], Yf[9], Tf[9];
-    m3_mul(QT, X, Xf);
-    m3_mul(Z, X, Yf);
-    m3_mul(QT, Y, tmp);
-#pragma unroll
-    for (int i = 0; i < 9; ++i) Yf[i] += tmp[i];
-    m3_mul(Pc, lj, Tf);
-    double G[9], TG[9], XG[9], YG[9];
-#pragma unroll
-    for (int i = 0; i < 9; ++i) G[i] = rj[15 + i];
-    m3_mul(Tf, G, TG);
-    m3_mul(Xf, G, XG);
-    m3_mul(Yf, G, YG);
     double D[18];
     {
-      double M[9], t9[9];
-      m3_mul(Bm, TG, M);
-      m3_mul(Kw, XG, t9);
-#pragma unroll
-      for (int i = 0; i < 9; ++i) M[i] += t9[i];
-      m3_mul(Kal, YG, t9);
-#pragma unroll
-      for (int i = 0; i < 9; ++i) M[i] += t9[i];
-      m3_mul(SgJ, M, &D[0]);
-      m3_mul(IgR, XG, t9);
-#pragma unroll
-      for (int i = 0; i < 9; ++i) D[i] += t9[i];
-      m3_mul(IlinR, M, &D[9]);
-    }
-    // block m = j : rotation = D_j - D_{j+1}, translation = (lamdd_m - lamdd_{m+1}) * Cp
-    {
-      const double wdd = lamdd[j] - lamdd[j + 1];
-#pragma unroll
-      for (int i = 0; i < 6; ++i) {
-        double2* out = reinterpret_cast<double2*>(Jp + i * 6 * K + 6 * j);
-        out[0] = make_double2(D[3 * i] - Dprev[3 * i], D[3 * i + 1] - Dprev[3 * i + 1]);
-        out[1] = make_double2(D[3 * i + 2] - Dprev[3 * i + 2], wdd * Cp[3 * i]);
-        out[2] = make_double2(wdd * Cp[3 * i + 1], wdd * Cp[3 * i + 2]);
-      }
+      double TG[9], XG[9], YG[9];
+      inertial_back_frames(rj, lj, atw, atwd, wat, lamd[j], lamdd[j], Pc, QT, Z, TG, XG, YG);
+      inertial_back_rows(TG, XG, YG, Bm, Kw, Kal, I, D);
     }
 #pragma unroll
-    for (int i = 0; i < 18; ++i) Dprev[i] = D[i];
-    // Pc <- Pc A_j^T ; Z <- (Z - lamd_j QT d^) A_j^T ; QT <- QT A_j^T
+    for (int i = 0; i < 18; ++i) { const double Di = D[i]; D[i] -= Dprev[i]; Dprev[i] = Di; }
+    inertial_store_block<K>(Jp, j, D, lamdd[j] - lamdd[j + 1], Cp);
     double Aj[9];
 #pragma unroll
     for (int i = 0; i < 9; ++i) Aj[i] = sj[i * kEvalThreads];
-    m3_mult(Pc, Aj, tmp);
-#pragma unroll
-    for (int i = 0; i < 9; ++i) Pc[i] = tmp[i];
-    mul_hat(QT, d, tmp);
-#pragma unroll
-    for (int i = 0; i < 9; ++i) tmp2[i] = Z[i] - lamd[j] * tmp[i];
-    m3_mult(tmp2, Aj, Z);
-    m3_mult(QT, Aj, tmp);
-#pragma unroll
-    for (int i = 0; i < 9; ++i) QT[i] = tmp[i];
+    const double d[3] = {rj[12], rj[13], rj[14]};
+    inertial_suffix_step(Aj, d, lamd[j], Pc, QT, Z);
   }
-  // block m = 0 : rotation = [S_g ; I_lin R_sb] Bm - D_1
-  {
-    double Cth[18];
-    m3_mul(SgJ, Bm, &Cth[0]);
-    m3_mul(IlinR, Bm, &Cth[9]);
-    const double wdd = lamdd[0] - lamdd[1];
+  double D0[18];
+  inertial_block0(Bm, I, D0);
 #pragma unroll
-    for (int i = 0; i < 6; ++i) {
-      double2* out = reinterpret_cast<double2*>(Jp + i * 6 * K);
-      out[0] = make_double2(Cth[3 * i] - Dprev[3 * i], Cth[3 * i + 1] - Dprev[3 * i + 1]);
-      out[1] = make_double2(Cth[3 * i + 2] - Dprev[3 * i + 2], wdd * Cp[3 * i]);
-      out[2] = make_double2(wdd * Cp[3 * i + 1], wdd * Cp[3 * i + 2]);
-    }
-  }
+  for (int i = 0; i < 18; ++i) D0[i] -= Dprev[i];
+  inertial_store_block<K>(Jp, 0, D0, lamdd[0] - lamdd[1], Cp);
 }
 
-// dynamic shared memory of the Jacobian pass of the inertial factors (the merged factor kernel carries it too)
+// dynamic shared memory of the Jacobian pass of the large-window inertial kernel
 constexpr size_t inertial_stash_bytes(int K) { return static_cast<size_t>(27) * (K - 1) * kEvalThreads * sizeof(double); }
 
 template <int K, int KB, bool WANT_J>
@@ -1014,30 +1083,326 @@ HB_DI void inertial_eval_body(const InertialArgs& a, const Basis& B, const Basis
       ro[0] = make_double2(r[0], r[1]); ro[1] = make_double2(r[2], r[3]); ro[2] = make_double2(r[4], r[5]);
     }
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) cost += __shfl_xor_sync(0xffffffffu, cost, o);
-  if ((threadIdx.x & 31) == 0) s_cost[threadIdx.x >> 5] = cost;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double c = 0;
-    for (int w = 0; w < kEvalThreads / 32; ++w) c += s_cost[w];
-    a.cost_partial[bid] = c;
-  }
+  tile_cost_sum(cost, s_cost, &a.cost_partial[bid]);
 }
 template <int K, int KB, bool WANT_J>
 __global__ void __launch_bounds__(kEvalThreads) inertial_eval_kernel(InertialArgs a, Basis B, Basis BB) { inertial_eval_body<K, KB, WANT_J>(a, B, BB, blockIdx.x); }
 
-// Visual and inertial factors in ONE launch (they are independent): CTAs [0, n_pix_blocks) run the pixel / bearing
-// body, the rest the inertial body.  At 12 k factors each of these kernels is a ~20 us latency-bound launch; side by
-// side they cost the longer of the two.
-template <int K, int KB, bool WANT_J, bool FUSE, bool DET>
-__global__ void __launch_bounds__(kEvalThreads) factor_eval_kernel(PixelArgs pa, InertialArgs ia, Basis B, Basis BB, int n_pix_blocks, DetOut det,
-                                                                   const int* __restrict__ seg_off) {
-  static_assert(!DET || (WANT_J && FUSE), "the deterministic assembly is a fused Jacobian pass");
-  if (static_cast<int>(blockIdx.x) < n_pix_blocks) pixel_eval_body<K, WANT_J, FUSE, DET>(pa, B, blockIdx.x, det, seg_off);
-  else inertial_eval_body<K, KB, WANT_J>(ia, B, BB, blockIdx.x - n_pix_blocks);
+// ---------------------------------------------------------------------------------------------
+// Lane-group bodies of the small-window factor kernel.  A small window is latency-bound: with one factor per thread a
+// pass lasts as long as one thread's serial walk over the spline steps.  Here G = factor_lanes(K) lanes evaluate one
+// factor.  Lane j (1 <= j < K) owns step j: its Exp / Jr (an FP64 sincos, sqrt and division), its pixel block, the
+// heavy part of its inertial backward step and the output block of control point j; lane 0 owns control point 0.
+// The cheap running products (pose rotation, body rates, backward state) need every A_j: each lane broadcasts its A_j
+// with __shfl_sync, and every lane runs those recursions in the one-thread order and keeps the state at its own step,
+// so it evaluates the one-thread body's expressions in the same order.  What does not depend on the step (projection,
+// distortion, residual, coefficient matrices) each lane of the group computes itself: the warp issues those
+// instructions once either way, and nothing has to be broadcast.  A CTA still holds one 64-factor tile (64 G
+// threads), so the CTA split, the cost partials and the pixel J^T J staging and slots are those of the
+// one-factor-per-thread kernels.
+// ---------------------------------------------------------------------------------------------
+__host__ __device__ constexpr int factor_lanes(int K) { return K <= 4 ? 4 : 8; }
+
+template <int N>
+HB_DI void shfl_group(unsigned mask, const double* v, double* out, int src, int G) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) out[i] = __shfl_sync(mask, v[i], src, G);
+}
+// v[i] for a lane-dependent i without indexing a register array (which would put the array in local memory)
+template <int N>
+HB_DI double pick(const double* v, int i) {
+  double r = v[0];
+#pragma unroll
+  for (int k = 1; k < N; ++k) r = (k == i) ? v[k] : r;
+  return r;
+}
+template <int N>
+HB_DI void keep_if(bool c, const double* v, double* out) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) out[i] = c ? v[i] : out[i];
 }
 
+struct LaneGroup {
+  int g;          // lane within the group; lane 0 leads
+  int j;          // spline step the lane evaluates: g clamped to [1, K-1] (lane 0 and lanes >= K repeat a step, unused)
+  unsigned mask;  // the group's lanes
+};
+template <int K>
+HB_DI LaneGroup lane_group() {
+  constexpr int G = factor_lanes(K);
+  const int g = threadIdx.x % G;
+  return LaneGroup{g, min(max(g, 1), K - 1), ((1u << G) - 1u) << ((threadIdx.x & 31) & ~(G - 1))};
+}
+
+template <int K, bool WANT_J>
+HB_DI void pixel_factor_lanes(const LaneGroup& lg, const double* T, const Basis& B, int base, double t, double zx, double zy, double zz, int kind,
+                              const double* __restrict__ cam, const double* __restrict__ lmk, double* r, double* __restrict__ Jp,
+                              double* __restrict__ Jl) {
+  constexpr int G = factor_lanes(K), left = (K - 1) / 2;
+  static_assert(K % 2 == 0, "the sector stores pair the blocks of control points 2p and 2p + 1");
+  const double* row0 = T + static_cast<size_t>(base) * kTabStride;
+  const double t0 = row0[left * kTabStride + 24], t1 = row0[(left + 1) * kTabStride + 24];
+  const double inv_dt = 1.0 / (t1 - t0);
+  const double u = (t - t0) * inv_dt;
+  double lam[K + 1];
+  basis_eval<K, false>(B, u, inv_dt, lam, nullptr, nullptr);
+  const double* rj = row0 + lg.j * kTabStride;
+  const double lj = pick<K>(lam, lg.j);
+  double A[9], Jr[9];
+  spline_step_exp(rj, lj, A, WANT_J ? Jr : nullptr);
+  double P[9], p[3], Pj[9];
+#pragma unroll
+  for (int i = 0; i < 9; ++i) P[i] = row0[i];
+  p[0] = row0[9]; p[1] = row0[10]; p[2] = row0[11];
+#pragma unroll
+  for (int s = 1; s < K; ++s) {
+    const double* rs = row0 + s * kTabStride;
+    double As[9];
+    shfl_group<9>(lg.mask, A, As, s, G);
+    double Pn[9];
+    m3_mul(P, As, Pn);
+#pragma unroll
+    for (int i = 0; i < 9; ++i) P[i] = Pn[i];
+    if (WANT_J) keep_if<9>(s == lg.j, P, Pj);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) p[c] += lam[s] * (rs[9 + c] - rs[9 + c - kTabStride]);
+  }
+  double E[6], F[6];
+  pixel_project<WANT_J>(P, p, lmk, cam, zx, zy, zz, kind, r, E, F);
+  if (!WANT_J) return;
+  if (lg.g == 0) {
+#pragma unroll
+    for (int i = 0; i < 6; ++i) Jl[i] = F[i];
+  }
+  // lane m holds E M_m (E for m = 0) and takes E M_{m+1} from lane m + 1
+  double M[9], cur[6], nxt[6];
+  pixel_step_block(rj, lj, Pj, Jr, M);
+  pixel_em(E, M, cur);
+  keep_if<6>(lg.g == 0, E, cur);
+#pragma unroll
+  for (int i = 0; i < 6; ++i) {
+    nxt[i] = __shfl_down_sync(lg.mask, cur[i], 1, G);
+    if (lg.g + 1 >= K) nxt[i] = 0.0;
+  }
+  const int m = min(lg.g, K - 1);
+  double r0[6], r1[6];
+  pixel_row_block(cur, nxt, pick<K>(lam, m) - pick<K + 1>(lam, m + 1), F, 0, r0);
+  pixel_row_block(cur, nxt, pick<K>(lam, m) - pick<K + 1>(lam, m + 1), F, 1, r1);
+  // Control points 2p and 2p + 1 cover 96 B of each row, three whole sectors: the even lane stores row 0's first and
+  // middle sector and row 1's first, the odd lane the rest; the middle sectors take two values from the partner lane.
+  const bool odd = lg.g & 1;
+  const double x0 = __shfl_xor_sync(lg.mask, odd ? r0[0] : r1[4], 1, G);
+  const double x1 = __shfl_xor_sync(lg.mask, odd ? r0[1] : r1[5], 1, G);
+  if (lg.g < K) {
+    double* q0 = Jp + 6 * (lg.g & ~1);   // 32-byte aligned: rows are 192 B (K=4) / 288 B (K=6)
+    double* q1 = q0 + 6 * K;
+    const int o = odd ? 8 : 0;
+    st_v4(q0 + o, odd ? r0[2] : r0[0], odd ? r0[3] : r0[1], odd ? r0[4] : r0[2], odd ? r0[5] : r0[3]);
+    st_v4(q1 + o, odd ? r1[2] : r1[0], odd ? r1[3] : r1[1], odd ? r1[4] : r1[2], odd ? r1[5] : r1[3]);
+    st_v4((odd ? q1 : q0) + 4, odd ? x0 : r0[4], odd ? x1 : r0[5], odd ? r1[0] : x0, odd ? r1[1] : x1);
+  }
+}
+
+// Returns |r|^2; the leader writes r to r_out (or null).  Two CTAs per SM leave 128 registers per thread at order 4, so
+// the lane keeps only w_{j-1}, wd_{j-1} of its step and evaluates Exp / Jr of the step again after the backward state,
+// instead of keeping A_j^T w_{j-1}, A_j^T wd_{j-1}, w_j and Jr_j live across it.
+template <int K, int KB, bool WANT_J>
+HB_DI double inertial_factor_lanes(const LaneGroup& lg, const double* T, const Basis& B, const Basis& BB, int base, int gb, int ab, double t,
+                                   const double* __restrict__ z, const double* __restrict__ I, const double* __restrict__ bg,
+                                   const double* __restrict__ ba, const double* __restrict__ grav, double* __restrict__ r_out,
+                                   double* __restrict__ Jp, double* __restrict__ wg_out, double* __restrict__ wa_out, double* __restrict__ Jg) {
+  constexpr int G = factor_lanes(K), left = (K - 1) / 2;
+  const double* row0 = T + static_cast<size_t>(base) * kTabStride;
+  const double t0 = row0[left * kTabStride + 24], t1 = row0[(left + 1) * kTabStride + 24];
+  const double inv_dt = 1.0 / (t1 - t0);
+  const double u = (t - t0) * inv_dt;
+  double lam[K + 1], lamd[K + 1], lamdd[K + 1];
+  basis_eval<K, true>(B, u, inv_dt, lam, lamd, lamdd);
+  const double* rj = row0 + lg.j * kTabStride;
+  const double lj = pick<K>(lam, lg.j);
+  double A[9];
+  spline_step_exp(rj, lj, A, nullptr);
+  // ---- forward sweep; the lane keeps w_{j-1}, wd_{j-1} of its own step ----
+  double P[9], pdd[3] = {0, 0, 0}, w[3] = {0, 0, 0}, wd[3] = {0, 0, 0}, wp[3], wdp[3];
+#pragma unroll
+  for (int i = 0; i < 9; ++i) P[i] = row0[i];
+#pragma unroll 1
+  for (int s = 1; s < K; ++s) {
+    const double* rs = row0 + s * kTabStride;
+    const double d[3] = {rs[12], rs[13], rs[14]};
+    double As[9], Pn[9], aw[3], awd[3];
+    shfl_group<9>(lg.mask, A, As, s, G);
+    m3_mul(P, As, Pn);
+#pragma unroll
+    for (int i = 0; i < 9; ++i) P[i] = Pn[i];
+    if (WANT_J) {
+      keep_if<3>(s == lg.j, w, wp);
+      keep_if<3>(s == lg.j, wd, wdp);
+    }
+    inertial_rate_step(As, d, lamd[s], lamdd[s], w, wd, aw, awd);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) pdd[c] += lamdd[s] * (rs[9 + c] - rs[9 + c - kTabStride]);
+  }
+  const bool lead = lg.g == 0;
+  double a_i[3], r[6], sq = 0.0;
+  inertial_residual<KB>(P, w, wd, pdd, BB, gb, ab, t, z, I, bg, ba, grav, r, a_i, lead ? wg_out : nullptr, lead ? wa_out : nullptr);
+#pragma unroll
+  for (int i = 0; i < 6; ++i) sq += r[i] * r[i];
+  if (lead && r_out) {
+    double2* ro = reinterpret_cast<double2*>(r_out);
+    ro[0] = make_double2(r[0], r[1]); ro[1] = make_double2(r[2], r[3]); ro[2] = make_double2(r[4], r[5]);
+  }
+  if (!WANT_J) return sq;
+  const double ld = pick<K>(lamd, lg.j), ldd = pick<K>(lamdd, lg.j), wdd = pick<K + 1>(lamdd, lg.g) - pick<K + 1>(lamdd, lg.g + 1);
+  // ---- backward state of steps K-1 .. j+1: the state the lane's own step j starts from ----
+  double Pc[9], QT[9], Z[9];
+#pragma unroll
+  for (int i = 0; i < 9; ++i) { Pc[i] = P[i]; QT[i] = (i % 4 == 0) ? 1.0 : 0.0; Z[i] = 0.0; }
+#pragma unroll 1
+  for (int s = K - 1; s > 1; --s) {
+    const double* rs = row0 + s * kTabStride;
+    const double d[3] = {rs[12], rs[13], rs[14]};
+    double As[9];
+    shfl_group<9>(lg.mask, A, As, s, G);
+    if (s > lg.j) inertial_suffix_step(As, d, lamd[s], Pc, QT, Z);
+  }
+  // ---- the lane's backward step; lane 0 takes D_0 instead ----
+  double D[18];
+  {
+    double Aj[9], Jr[9], lJr[9], atw[3], atwd[3], TG[9], XG[9], YG[9];
+    spline_step_exp(rj, lj, Aj, Jr);
+#pragma unroll
+    for (int i = 0; i < 9; ++i) lJr[i] = lj * Jr[i];
+    const double dj[3] = {rj[12], rj[13], rj[14]};
+    inertial_rate_step(Aj, dj, ld, ldd, wp, wdp, atw, atwd);   // wp <- w_j
+    inertial_back_frames(rj, lJr, atw, atwd, wp, ld, ldd, Pc, QT, Z, TG, XG, YG);
+    double Bm[9], Kw[9], Kal[9];
+    inertial_coeffs(P, a_i, w, I, Bm, Kw, Kal);
+    inertial_back_rows(TG, XG, YG, Bm, Kw, Kal, I, D);
+    if (lead) inertial_block0(Bm, I, D);
+  }
+  // block m = D_m - D_{m+1}: D_{m+1} from lane m + 1
+#pragma unroll
+  for (int i = 0; i < 18; ++i) {
+    const double Dn = __shfl_down_sync(lg.mask, D[i], 1, G);
+    D[i] -= (lg.g + 1 < K) ? Dn : 0.0;
+  }
+  double Cp[18];
+  inertial_trans(P, I, grav, Cp, lead ? Jg : nullptr);
+  if (lg.g < K) inertial_store_block<K>(Jp, lg.g, D, wdd, Cp);
+  return sq;
+}
+
+// One 64-factor tile per CTA, kEvalThreads * factor_lanes(K) threads: factor t of the tile on threads [G t, G t + G).
+// The tile's cost sum and fused J^T J run on the first kEvalThreads threads, as in pixel_eval_body.
+template <int K, bool WANT_J, bool FUSE, bool DET>
+HB_DI void pixel_lanes_body(const PixelArgs& a, const Basis& B, int bid, const DetOut& det, const int* seg_off) {
+  constexpr int G = factor_lanes(K);
+  __shared__ __align__(16) double s_tab[kTileRows * kTabStride];
+  __shared__ __align__(8) uint64_t s_bar;
+  __shared__ int s_red[2];
+  __shared__ double s_fcost[kEvalThreads];
+  __shared__ double s_cost[kEvalThreads / 32];
+  __shared__ double s_J[FUSE ? 128 * PixelHessAcc<K>::LD : 1];
+  __shared__ double s_r[FUSE ? 128 : 1];
+  __shared__ int s_b[FUSE ? 66 : 1];
+  const LaneGroup lg = lane_group<K>();
+  const int f = bid * kEvalThreads + threadIdx.x / G;
+  const bool active = f < a.n;
+  int4 id = make_int4(0, 0, 0, 0);
+  if (active) id = a.idx[f];
+  int bmin, bmax;
+  block_min_max(active ? id.x : 0x7fffffff, active ? id.x : -0x7fffffff, s_red, &bmin, &bmax);
+  const int rows = bmax - bmin + K;
+  const bool staged = rows <= kTileRows;
+  if (staged) stage_table(s_tab, &s_bar, a.tab, bmin, rows);
+  double cost = 0.0;
+  if (active) {
+    const double t = a.stamp[f];
+    const double2 z = a.pixel[f];
+    const double* cam = a.cam_tab + kCamStride * id.z;
+    const double* lmk = a.landmarks + 3 * static_cast<size_t>(id.y);
+    double r[2];
+    double* Jp = WANT_J ? a.Jp + static_cast<size_t>(f) * 12 * K : nullptr;
+    double* Jl = WANT_J ? a.Jl + static_cast<size_t>(f) * 6 : nullptr;
+    const double zz = (id.w != 0) ? a.meas_z[f] : 0.0;
+    const double* T = staged ? s_tab - static_cast<ptrdiff_t>(bmin) * kTabStride : a.tab;
+    pixel_factor_lanes<K, WANT_J>(lg, T, B, id.x, t, z.x, z.y, zz, id.w, cam, lmk, r, Jp, Jl);
+    double wgt;
+    cost = 0.5 * huber_rho(r[0] * r[0] + r[1] * r[1], (id.w != 0) ? a.huber_bearing : a.huber, &wgt);
+    if (lg.g == 0) {
+      if (a.r) reinterpret_cast<double2*>(a.r)[f] = make_double2(r[0], r[1]);
+      if (WANT_J) a.w[f] = wgt;
+    }
+  }
+  if (lg.g == 0) s_fcost[threadIdx.x / G] = cost;
+  __syncthreads();   // (also orders the tile's residuals and Jacobians before the fused J^T J reads them)
+  if (threadIdx.x >= kEvalThreads) return;
+  tile_cost_sum(s_fcost[threadIdx.x], s_cost, &a.cost_partial[bid]);
+  if (FUSE && a.sys != nullptr) {
+    const int f_lo = bid * kEvalThreads;
+    PixelHessAcc<K> acc;
+    pixel_hess_reset<K>(acc, -1);
+    cta_pixel_hessian<K, DET>(a, f_lo, min(kEvalThreads, a.n - f_lo), s_J, s_r, s_b, acc, det, DET ? seg_off[bid] : 0);
+    pixel_hess_flush<K, DET>(a, acc, det, DET ? seg_off[bid + 1] - 1 : 0);
+  }
+}
+
+template <int K, int KB, bool WANT_J>
+HB_DI void inertial_lanes_body(const InertialArgs& a, const Basis& B, const Basis& BB, int bid) {
+  constexpr int G = factor_lanes(K);
+  __shared__ __align__(16) double s_tab[kTileRows * kTabStride];
+  __shared__ __align__(8) uint64_t s_bar;
+  __shared__ int s_red[2];
+  __shared__ double s_fcost[kEvalThreads];
+  __shared__ double s_cost[kEvalThreads / 32];
+  __shared__ double s_imu[kImuStride];
+  __shared__ double s_grav[3];
+  for (int i = threadIdx.x; i < kImuStride; i += blockDim.x) s_imu[i] = a.imu_tab[i];
+  if (threadIdx.x < 3) s_grav[threadIdx.x] = a.gravity[threadIdx.x];
+  const LaneGroup lg = lane_group<K>();
+  const int f = bid * kEvalThreads + threadIdx.x / G;
+  const bool active = f < a.n;
+  int4 id = make_int4(0, 0, 0, 0);
+  if (active) id = a.idx[f];
+  int bmin, bmax;
+  block_min_max(active ? id.x : 0x7fffffff, active ? id.x : -0x7fffffff, s_red, &bmin, &bmax);
+  const int rows = bmax - bmin + K;
+  const bool staged = rows <= kTileRows;
+  if (staged) stage_table(s_tab, &s_bar, a.tab, bmin, rows);
+  double cost = 0.0;
+  if (active) {
+    const double t = a.stamp[f];
+    double z[6];
+    {
+      const double2* zp = reinterpret_cast<const double2*>(a.meas + 6 * static_cast<size_t>(f));
+      const double2 z0 = zp[0], z1 = zp[1], z2 = zp[2];
+      z[0] = z0.x; z[1] = z0.y; z[2] = z1.x; z[3] = z1.y; z[4] = z2.x; z[5] = z2.y;
+    }
+    double* Jp = WANT_J ? a.Jp + static_cast<size_t>(f) * 36 * K : nullptr;
+    double* wg = WANT_J ? a.wg + static_cast<size_t>(f) * KB : nullptr;
+    double* wa = WANT_J ? a.wa + static_cast<size_t>(f) * KB : nullptr;
+    double* Jg = WANT_J ? a.Jg + static_cast<size_t>(f) * 12 : nullptr;
+    double* r = a.r ? a.r + 6 * static_cast<size_t>(f) : nullptr;
+    const double* T = staged ? s_tab - static_cast<ptrdiff_t>(bmin) * kTabStride : a.tab;
+    const double s = inertial_factor_lanes<K, KB, WANT_J>(lg, T, B, BB, id.x, id.y, id.z, t, z, s_imu, a.bg, a.ba, s_grav, r, Jp, wg, wa, Jg);
+    cost = 0.5 * a.loss_scale * s;
+  }
+  if (lg.g == 0) s_fcost[threadIdx.x / G] = cost;
+  __syncthreads();
+  if (threadIdx.x >= kEvalThreads) return;
+  tile_cost_sum(s_fcost[threadIdx.x], s_cost, &a.cost_partial[bid]);
+}
+
+// Visual and inertial factors of a small window in ONE launch (they are independent): CTAs [0, n_pix_blocks) run the
+// pixel / bearing body, the rest the inertial body, both on lane groups.  A pass costs the longer of the two families.
+template <int K, int KB, bool WANT_J, bool FUSE, bool DET>
+__global__ void __launch_bounds__(kEvalThreads * factor_lanes(K), K == 4 ? 2 : 1)
+    factor_eval_kernel(PixelArgs pa, InertialArgs ia, Basis B, Basis BB, int n_pix_blocks, DetOut det, const int* __restrict__ seg_off) {
+  static_assert(!DET || (WANT_J && FUSE), "the deterministic assembly is a fused Jacobian pass");
+  if (static_cast<int>(blockIdx.x) < n_pix_blocks) pixel_lanes_body<K, WANT_J, FUSE, DET>(pa, B, blockIdx.x, det, seg_off);
+  else inertial_lanes_body<K, KB, WANT_J>(ia, B, BB, blockIdx.x - n_pix_blocks);
+}
 
 // ---------------------------------------------------------------------------------------------
 // Manifold (pose) factor: prediction T_ws = T_wb (+) T_bs (reference

@@ -13,7 +13,7 @@ constexpr int kMaxOrder = 6;
 //   [24]    stamp_j ; [25..27] pad  -> 28 doubles = 224 B (16 B multiple for cp.async.bulk)
 constexpr int kTabStride = 28;
 constexpr int kTileRows = 16;       // knot-table rows staged per CTA (3.6 KB); wider spans read the table from global/L2
-constexpr int kEvalThreads = 64;    // one factor per thread
+constexpr int kEvalThreads = 64;    // factors per CTA tile of the factor kernels (one per thread on large windows)
 
 constexpr int kCamStride = 20;      // R_sb(9) t_bs(3) intrinsics(4) distortion(4)
 // IMU derived table: R_sb(9) t_bs(3) IgRsb(9) IaRsb(9) Sg(9,row-major) lever arms c_r (3x3 rows) = 48, then the
