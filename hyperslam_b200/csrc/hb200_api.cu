@@ -2425,18 +2425,18 @@ int hb200_get_covariance(hb200_ctx* c, double* packed, double* landmark) {
 
 int hb200_interpolate_covariance(hb200_ctx* c, int n, const double* stamps, double* cov, int* num_invalid) {
   return cov_interpolate(c, n, stamps, cov, num_invalid, 36, [&](auto K, const CovPoint& pt) {
-    cov_interpolate_kernel<K><<<(n + 127) / 128, 128, 0, c->stream>>>(n, c->cov_t.p, pt.knots.p, pt.tab.p, pt.lay.K, pt.basis, c->cov_packed.p, pt.lay,
-                                                                     c->cov_o.p, c->cov_bad.p);
-    return check_launch(c, "cov_interpolate_kernel");
+    cov_stamp_kernel<K, 6><<<(n + kStateWarps - 1) / kStateWarps, kStateWarps * 32, 0, c->stream>>>(
+        n, c->cov_t.p, pt.knots.p, pt.tab.p, pt.lay.K, pt.basis, nullptr, 0, nullptr, 0, pt.bias_basis, c->cov_packed.p, pt.lay, c->cov_o.p, c->cov_bad.p);
+    return check_launch(c, "cov_stamp_kernel");
   });
 }
 
 int hb200_interpolate_state_covariance(hb200_ctx* c, int n, const double* stamps, double* cov, int* num_invalid) {
   static_assert(HB200_STATE_COV_DIM == kStateDim, "state covariance dimension");
   return cov_interpolate(c, n, stamps, cov, num_invalid, HB200_STATE_COV_DIM * HB200_STATE_COV_DIM, [&](auto K, const CovPoint& pt) {
-    cov_state_interpolate_kernel<K><<<(n + kStateWarps - 1) / kStateWarps, kStateWarps * 32, 0, c->stream>>>(
+    cov_stamp_kernel<K, kStateDim><<<(n + kStateWarps - 1) / kStateWarps, kStateWarps * 32, 0, c->stream>>>(
         n, c->cov_t.p, pt.knots.p, pt.tab.p, pt.lay.K, pt.basis, pt.bg.p, pt.Kbg, pt.ba.p, pt.Kba, pt.bias_basis, c->cov_packed.p, pt.lay, c->cov_o.p, c->cov_bad.p);
-    return check_launch(c, "cov_state_interpolate_kernel");
+    return check_launch(c, "cov_stamp_kernel");
   });
 }
 

@@ -23,32 +23,6 @@ enum {   // == oracle/ho_evaluators.h Quirks (SURVEY.md section 8a "Reference qu
   kQuirkAxesOffsetsIgnored = 8           // (v)  inertial.cpp:142,148 use t_bs only
 };
 
-// pose of the body at the factor's stamp (value only): R (row-major), p
-template <int K>
-HB_DI void pose_value(const double* __restrict__ T, const Basis& B, int base, double t, double* P, double* p) {
-  constexpr int left = (K - 1) / 2;
-  const double* row0 = T + static_cast<size_t>(base) * kTabStride;
-  const double t0 = row0[left * kTabStride + 24], t1 = row0[(left + 1) * kTabStride + 24];
-  const double inv_dt = 1.0 / (t1 - t0);
-  double lam[K + 1];
-  basis_eval<K, false>(B, (t - t0) * inv_dt, inv_dt, lam, nullptr, nullptr);
-#pragma unroll
-  for (int i = 0; i < 9; ++i) P[i] = row0[i];
-  p[0] = row0[9]; p[1] = row0[10]; p[2] = row0[11];
-#pragma unroll
-  for (int j = 1; j < K; ++j) {
-    const double* rj = row0 + j * kTabStride;
-    const double w[3] = {lam[j] * rj[12], lam[j] * rj[13], lam[j] * rj[14]};
-    double A[9], Pn[9];
-    so3_exp_and_Jr(w, A, nullptr);
-    m3_mul(P, A, Pn);
-#pragma unroll
-    for (int i = 0; i < 9; ++i) P[i] = Pn[i];
-#pragma unroll
-    for (int c = 0; c < 3; ++c) p[c] += lam[j] * (rj[9 + c] - rj[9 + c - kTabStride]);
-  }
-}
-
 // row (1x3) times [R_sb hat(v) | -R_sb]: the extrinsics tangent block of anything that depends on p_s = R_sb (p_b - t_bs)
 HB_DI void extrinsics_row(const double* a /* = d/dp_s * R_sb, 1x3 */, const double* v /* p_b - t_bs */, double* out /*6*/) {
   out[0] = a[1] * v[2] - a[2] * v[1];
@@ -67,8 +41,8 @@ __global__ void __launch_bounds__(kEvalThreads) pixel_calib_kernel(int n, const 
   const int4 id = idx[f];
   const double* cam = cam_tab + kCamStride * id.z;
   const double* lmk = landmarks + 3 * static_cast<size_t>(id.y);
-  double P[9], p[3];
-  pose_value<K>(tab, B, id.x, stamp[f], P, p);
+  double lam[K + 1], P[9], p[3];
+  spline_pose<K, false>(spline_segment<K>(tab, B, id.x, stamp[f], lam), lam, P, p, nullptr);
   const double q[3] = {lmk[0] - p[0], lmk[1] - p[1], lmk[2] - p[2]};
   double pb[3], ps[3];
   m3_tvec(P, q, pb);
@@ -134,8 +108,8 @@ __global__ void __launch_bounds__(kEvalThreads) manifold_calib_kernel(int n, con
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= n) return;
   const int2 id = idx[f];
-  double P[9], p[3];
-  pose_value<K>(tab, B, id.x, stamp[f], P, p);
+  double lam[K + 1], P[9], p[3];
+  spline_pose<K, false>(spline_segment<K>(tab, B, id.x, stamp[f], lam), lam, P, p, nullptr);
   const double* T_bs = sensors + 7 * static_cast<size_t>(id.y);
   const double* z = meas + 7 * static_cast<size_t>(f);
   double Rbs[9], Rz[9], Rws[9], Rerr[9], q[4], th[3];
@@ -167,12 +141,8 @@ __global__ void __launch_bounds__(kEvalThreads) inertial_calib_kernel(int n, con
                                                                       double* __restrict__ Jc /*[n][6][36]*/) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= n) return;
-  constexpr int left = (K - 1) / 2;
-  const double* row0 = tab + static_cast<size_t>(idx[f].x) * kTabStride;
-  const double t0 = row0[left * kTabStride + 24], t1 = row0[(left + 1) * kTabStride + 24];
-  const double inv_dt = 1.0 / (t1 - t0);
   double lam[K + 1], lamd[K + 1], lamdd[K + 1];
-  basis_eval<K, true>(B, (stamp[f] - t0) * inv_dt, inv_dt, lam, lamd, lamdd);
+  const double* row0 = spline_segment<K, true>(tab, B, idx[f].x, stamp[f], lam, lamd, lamdd);
   double P[9], pdd[3] = {0, 0, 0}, w[3] = {0, 0, 0}, wd[3] = {0, 0, 0};
 #pragma unroll
   for (int i = 0; i < 9; ++i) P[i] = row0[i];
@@ -180,23 +150,14 @@ __global__ void __launch_bounds__(kEvalThreads) inertial_calib_kernel(int n, con
   for (int j = 1; j < K; ++j) {
     const double* rj = row0 + j * kTabStride;
     const double d[3] = {rj[12], rj[13], rj[14]};
-    const double lw[3] = {lam[j] * d[0], lam[j] * d[1], lam[j] * d[2]};
-    double A[9], Pn[9], aw[3], awd[3], wn[3], cr[3];
-    so3_exp_and_Jr(lw, A, nullptr);
+    double A[9], Pn[9], aw[3], awd[3];
+    spline_step_exp(rj, lam[j], A, nullptr);
     m3_mul(P, A, Pn);
 #pragma unroll
     for (int i = 0; i < 9; ++i) P[i] = Pn[i];
-    m3_tvec(A, w, aw);
-    m3_tvec(A, wd, awd);
+    inertial_rate_step(A, d, lamd[j], lamdd[j], w, wd, aw, awd);
 #pragma unroll
-    for (int c = 0; c < 3; ++c) wn[c] = aw[c] + lamd[j] * d[c];
-    cross(wn, d, cr);
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-      wd[c] = awd[c] + lamd[j] * cr[c] + lamdd[j] * d[c];
-      w[c] = wn[c];
-      pdd[c] += lamdd[j] * (rj[9 + c] - rj[9 + c - kTabStride]);
-    }
+    for (int c = 0; c < 3; ++c) pdd[c] += lamdd[j] * (rj[9 + c] - rj[9 + c - kTabStride]);
   }
   // calibration (inertial.cpp:35-49,114-119)
   double Rbs[9], Rsb[9];

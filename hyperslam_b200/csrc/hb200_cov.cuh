@@ -5,8 +5,8 @@
 // buffer; the kernels here then produce, from S and the landmark factors of that build:
 //   cov_selinv_kernel     the entries of S^-1 on the block band, the arrow and the corner (selected inversion);
 //   cov_landmark_kernel   the 3 x 3 marginal of every landmark, Sigma_ll = L^-T (I + Y^T Sigma_pp Y) L^-1;
-//   cov_interpolate_kernel the 6 x 6 covariance of the interpolated pose at arbitrary stamps, J(t) Sigma J(t)^T;
-//   cov_state_interpolate_kernel the 18 x 18 joint covariance of pose, body velocity and IMU biases at arbitrary stamps;
+//   cov_stamp_kernel      at arbitrary stamps, J(t) Sigma J(t)^T of the interpolated pose (6 x 6) or of the joint pose,
+//                         body velocity and IMU biases (18 x 18);
 //   cov_far_column_kernel / cov_cross_landmark_kernel the requested blocks outside the pattern (ceres::Covariance::Compute's
 //                         list): knot pairs beyond the band and landmark cross-covariances;
 //   cov_pose_pair_kernel  the joint covariance of the poses at two stamps and the covariance of their relative pose.
@@ -701,106 +701,106 @@ __global__ void __launch_bounds__(kLmWarps * 32) cov_cross_landmark_kernel(
 }
 
 // ---------------------------------------------------------------------------------------------
-// Covariance of the interpolated pose at arbitrary stamps, one thread per stamp: J(t) (6 x 6k) is the Jacobian of the
-// pose [theta | p] at t (global rotation tangent, R <- Exp(theta) R, p <- p + rho) with respect to the tangents of its k
-// control points -- the pose-factor Jacobian of manifold_eval_kernel with an identity sensor at zero residual -- and
-// Sigma(t) = sum_ab J_a Z_ab J_b^T over the k x k control-point blocks (within the band).  knots / tab are the snapshot of
-// the last successful compute.  A stamp outside the valid span gives a zero block and invalid[f] = 1.
-// ---------------------------------------------------------------------------------------------
-template <int K>
-__global__ void cov_interpolate_kernel(int n, const double* __restrict__ stamps, const double* __restrict__ knots, const double* __restrict__ tab,
-                                       int Kn, Basis B, const double* __restrict__ cov, SysLayout lay, double* __restrict__ out,
-                                       int* __restrict__ invalid) {
-  const int f = blockIdx.x * blockDim.x + threadIdx.x;
-  if (f >= n) return;
-  double* o = out + 36 * static_cast<size_t>(f);
-  const int base = segment_base(knots, 8, 7, Kn, K, stamps[f]);
-  invalid[f] = base < 0 ? 1 : 0;
-  if (base < 0) {
-    for (int i = 0; i < 36; ++i) o[i] = 0.0;
-    return;
-  }
-  constexpr int left = (K - 1) / 2;
-  const double* row0 = tab + static_cast<size_t>(base) * kTabStride;
-  const double t0 = row0[left * kTabStride + 24], t1 = row0[(left + 1) * kTabStride + 24];
-  const double inv_dt = 1.0 / (t1 - t0);
-  double lam[K + 1];
-  basis_eval<K, false>(B, (stamps[f] - t0) * inv_dt, inv_dt, lam, nullptr, nullptr);
-  double P[9], M[(K - 1) * 9];
-#pragma unroll
-  for (int i = 0; i < 9; ++i) P[i] = row0[i];
-#pragma unroll
-  for (int j = 1; j < K; ++j) {
-    const double* rj = row0 + j * kTabStride;
-    const double wj[3] = {lam[j] * rj[12], lam[j] * rj[13], lam[j] * rj[14]};
-    double A[9], Jr[9], Pn[9], G[9], JG[9], PJG[9];
-    so3_exp_and_Jr(wj, A, Jr);
-    m3_mul(P, A, Pn);
-#pragma unroll
-    for (int i = 0; i < 9; ++i) G[i] = rj[15 + i];
-    m3_mul(Jr, G, JG);
-    m3_mul(Pn, JG, PJG);
-#pragma unroll
-    for (int i = 0; i < 9; ++i) { M[(j - 1) * 9 + i] = lam[j] * PJG[i]; P[i] = Pn[i]; }
-  }
-  // J_m = [D_m 0 ; 0 w_m I], D_m = d theta / d phi_m, w_m = lambda_m - lambda_{m+1}
-  auto Dm = [&](int mm, int i) { return ((mm == 0) ? ((i % 4 == 0) ? 1.0 : 0.0) : M[(mm - 1) * 9 + i]) - ((mm + 1 < K) ? M[mm * 9 + i] : 0.0); };
-  double S[36];
-#pragma unroll
-  for (int i = 0; i < 36; ++i) S[i] = 0.0;
-  for (int a = 0; a < K; ++a) {
-    double Da[9];
-    for (int i = 0; i < 9; ++i) Da[i] = Dm(a, i);
-    const double wa = lam[a] - lam[a + 1];
-    for (int b = 0; b < K; ++b) {
-      double Db[9];
-      for (int i = 0; i < 9; ++i) Db[i] = Dm(b, i);
-      const double wb = lam[b] - lam[b + 1];
-      double Z[36], T[36];
-      for (int r = 0; r < 6; ++r)
-        for (int s = 0; s < 6; ++s) {
-          const int gi = 6 * (base + a) + r, gj = 6 * (base + b) + s;
-          Z[r * 6 + s] = cov[sys_index(lay, max(gi, gj), min(gi, gj))];
-        }
-      for (int r = 0; r < 6; ++r) {   // T = Z_ab J_b^T
-        for (int c = 0; c < 3; ++c) T[r * 6 + c] = Z[r * 6] * Db[c * 3] + Z[r * 6 + 1] * Db[c * 3 + 1] + Z[r * 6 + 2] * Db[c * 3 + 2];
-        for (int c = 3; c < 6; ++c) T[r * 6 + c] = wb * Z[r * 6 + c];
-      }
-      for (int c = 0; c < 6; ++c) {   // S += J_a T
-        for (int i = 0; i < 3; ++i) S[i * 6 + c] += Da[i * 3] * T[c] + Da[i * 3 + 1] * T[6 + c] + Da[i * 3 + 2] * T[12 + c];
-        for (int i = 3; i < 6; ++i) S[i * 6 + c] += wa * T[i * 6 + c];
-      }
-    }
-  }
-  for (int i = 0; i < 6; ++i)
-    for (int c = 0; c < 6; ++c) o[i * 6 + c] = 0.5 * (S[i * 6 + c] + S[c * 6 + i]);
-}
-
-// ---------------------------------------------------------------------------------------------
-// Joint covariance of the interpolated state x(t) = [theta p | omega v | b_g b_a] (18 rows) at arbitrary stamps, one warp
-// per stamp.  J(t) (18 x NC, NC = 6k + 24) is taken with respect to the tangents [phi | rho] of the stamp's k control
-// points and the 4 knots of each bias spline (columns 6k + 3m + c gyro, 6k + 12 + 3m + c accel); Sigma(t) = J Z J^T with
-// Z the span of the packed Sigma (control-point pairs in the band, pose x bias in the arrow, bias x bias in the corner).
+// Covariance at arbitrary stamps, one warp per stamp: the pose [theta p] (ROWS = 6, hb200_interpolate_covariance) or
+// the joint state x(t) = [theta p | omega v | b_g b_a] (ROWS = 18, hb200_interpolate_state_covariance).  J(t)
+// (ROWS x NC) is taken with respect to the tangents [phi | rho] of the stamp's k control points (global rotation
+// tangent, R <- Exp(theta) R, p <- p + rho) and, for the state, the 4 knots of each bias spline (NC = 6k + 24, columns
+// 6k + 3m + c gyro, 6k + 12 + 3m + c accel; NC = 6k for the pose); Sigma(t) = J Z J^T with Z the span of the packed
+// Sigma (control-point pairs in the band, pose x bias in the arrow, bias x bias in the corner).
 // Jacobian blocks of control point m, with P_j = R_0 A_1 .. A_j, A_j = Exp(lambda_j d_j), G_j = Jr^-1(d_j) R_j^T:
-//   theta: D_m = M_m - M_{m+1},             M_j = lambda_j P_j Jr(lambda_j d_j) G_j   (cov_interpolate_kernel; M_0 = I)
+//   theta: D_m = M_m - M_{m+1},             M_j = lambda_j P_j Jr(lambda_j d_j) G_j   (M_0 = I);  p: (lambda_m - lambda_{m+1}) I on rho_m;
 //   omega: R^T (Y_m - Y_{m+1}),             Y_j = P_j X_j G_j, X_j = hat(A_j^T w_{j-1}) lambda_j Jr(lambda_j d_j) + lamd_j I
 //          -- inertial_factor's rate rows X -> XG, whose left factor A_{k-1}^T .. A_{j+1}^T is R^T P_j;
-//   v = R^T pdot: hat(v) R^T D_m on phi_m and (lamd_m - lamd_{m+1}) R^T on rho_m;  p: (lambda_m - lambda_{m+1}) I on rho_m;
+//   v = R^T pdot: hat(v) R^T D_m on phi_m and (lamd_m - lamd_{m+1}) R^T on rho_m;
 //   b_g / b_a: (lb_m - lb_{m+1}) I on knot gb + m / ab + m (the bias basis, as inertial_factor evaluates it).
-// Lane 0 builds J in shared memory (one forward sweep); each lane then forms rows a of T = Z J^T from the packed Sigma
-// and entries of J T; the output is 0.5 (S + S^T).  Sums run in a fixed order, no atomics.  A stamp outside the pose
+// Lane 0 builds J in shared memory (one forward sweep, cov_stamp_jacobian); each lane then forms rows a of T = Z J^T
+// from the packed Sigma and entries of J T; the output is 0.5 (S + S^T).  Sums run in a fixed order, no atomics.  The
+// pose rows of the state's J are the pose J, and its bias columns only add z * 0 terms to the pose block's sums, so
+// the pose block of the state covariance equals the pose covariance value for value.  A stamp outside the pose
 // spline's valid span, or outside the span of a bias spline that has knots, gives a zero block and invalid[f] = 1; a
 // spline without knots (Kbg or Kba = 0) gives zero rows and columns.  All inputs are the snapshot of the last compute.
 // ---------------------------------------------------------------------------------------------
 constexpr int kStateDim = 18;
-constexpr int kStateWarps = 2;   // stamps per CTA (static shared memory: 2 x 17.5 KB at k = 6)
+constexpr int kStateWarps = 2;   // stamps per CTA (static shared memory: 2 x 17.5 KB at k = 6, ROWS = 18)
 
-template <int K>
-__global__ void __launch_bounds__(kStateWarps * 32) cov_state_interpolate_kernel(
+// Rows 0 .. ROWS - 1 of J(t) (row stride NC, zero on entry) over control points base .. base + K - 1 -- every column
+// but the bias ones -- and the pose R (row-major), p at t.
+template <int K, int ROWS, int NC>
+HB_DI void cov_stamp_jacobian(const double* __restrict__ tab, const Basis& B, int base, double t, double* J, double* P, double* p) {
+  double lam[K + 1], lamd[K + 1], lamdd[K + 1];
+  const double* row0 = spline_segment<K, ROWS == kStateDim>(tab, B, base, t, lam, lamd, lamdd);
+  auto add3 = [&](double* b, const double* M, double s) {   // 3 x 3 block at b += s M
+    for (int i = 0; i < 3; ++i)
+      for (int c = 0; c < 3; ++c) b[i * NC + c] += s * M[3 * i + c];
+  };
+  for (int i = 0; i < 3; ++i) J[i * NC + i] = 1.0;   // M_0 = I
+  double w[3] = {0, 0, 0}, wdot[3] = {0, 0, 0}, pd[3] = {0, 0, 0};
+  for (int i = 0; i < 9; ++i) P[i] = row0[i];
+  p[0] = row0[9]; p[1] = row0[10]; p[2] = row0[11];
+#pragma unroll 1
+  for (int j = 1; j < K; ++j) {
+    const double* rj = row0 + j * kTabStride;
+    double A[9], Jr[9], Pn[9], M[9];
+    spline_step_exp(rj, lam[j], A, Jr);
+    m3_mul(P, A, Pn);
+    // theta rows: + M_j on phi_j, - M_j on phi_{j-1}
+    pixel_step_block(rj, lam[j], Pn, Jr, M);
+    add3(J + 6 * j, M, 1.0);
+    add3(J + 6 * (j - 1), M, -1.0);
+    if (ROWS == kStateDim) {   // omega rows (R^T applied below): + Y_j on phi_j, - Y_j on phi_{j-1}
+      const double d[3] = {rj[12], rj[13], rj[14]};
+      double G[9], lj[9], X[9], XG[9], aw[3], awd[3];
+      for (int i = 0; i < 9; ++i) { G[i] = rj[15 + i]; lj[i] = lam[j] * Jr[i]; }
+      inertial_rate_step(A, d, lamd[j], lamdd[j], w, wdot, aw, awd);   // the J rows need aw and w only; wdot, awd go unused
+      hat_mul(aw, lj, X);
+      for (int i = 0; i < 3; ++i) X[4 * i] += lamd[j];
+      m3_mul(X, G, XG);
+      m3_mul(Pn, XG, M);
+      add3(J + 6 * NC + 6 * j, M, 1.0);
+      add3(J + 6 * NC + 6 * (j - 1), M, -1.0);
+      for (int c = 0; c < 3; ++c) pd[c] += lamd[j] * (rj[9 + c] - rj[9 + c - kTabStride]);
+    }
+    for (int c = 0; c < 3; ++c) p[c] += lam[j] * (rj[9 + c] - rj[9 + c - kTabStride]);
+    for (int i = 0; i < 9; ++i) P[i] = Pn[i];
+  }
+  // P = R: p rows w_m I; omega rows R^T (Y_m - Y_{m+1}); v rows hat(v) R^T D_m and (lamd_m - lamd_{m+1}) R^T
+  double H[9];
+  if (ROWS == kStateDim) {
+    double v[3], Rt[9];
+    m3_tvec(P, pd, v);
+    for (int i = 0; i < 3; ++i)
+      for (int c = 0; c < 3; ++c) Rt[3 * i + c] = P[3 * c + i];
+    hat_mul(v, Rt, H);
+  }
+#pragma unroll 1
+  for (int m = 0; m < K; ++m) {
+    const double wm = lam[m] - lam[m + 1];
+    for (int i = 0; i < 3; ++i) J[(3 + i) * NC + 6 * m + 3 + i] = wm;
+    if (ROWS == kStateDim) {
+      double* Jo = J + 6 * NC + 6 * m;   // omega block, then the v blocks three rows below
+      double Y[9], Dm[9], Z[9];
+      for (int i = 0; i < 3; ++i)
+        for (int c = 0; c < 3; ++c) { Y[3 * i + c] = Jo[i * NC + c]; Dm[3 * i + c] = J[i * NC + 6 * m + c]; }
+      m3_tmul(P, Y, Z);
+      for (int i = 0; i < 3; ++i)
+        for (int c = 0; c < 3; ++c) Jo[i * NC + c] = Z[3 * i + c];
+      m3_mul(H, Dm, Z);
+      add3(Jo + 3 * NC, Z, 1.0);
+      const double wd = lamd[m] - lamd[m + 1];
+      for (int i = 0; i < 3; ++i)
+        for (int c = 0; c < 3; ++c) Jo[(3 + i) * NC + 3 + c] = wd * P[3 * c + i];
+    }
+  }
+}
+
+template <int K, int ROWS>
+__global__ void __launch_bounds__(kStateWarps * 32) cov_stamp_kernel(
     int n, const double* __restrict__ stamps, const double* __restrict__ knots, const double* __restrict__ tab, int Kn, Basis B,
     const double* __restrict__ bg, int Kbg, const double* __restrict__ ba, int Kba, Basis BB, const double* __restrict__ cov,
     SysLayout lay, double* __restrict__ out, int* __restrict__ invalid) {
-  constexpr int NC = 6 * K + 24, D = kStateDim, KB = 4;
+  static_assert(ROWS == 6 || ROWS == kStateDim, "pose or joint state rows");
+  constexpr bool STATE = ROWS == kStateDim;
+  constexpr int NC = 6 * K + (STATE ? 24 : 0), D = ROWS, KB = 4;
   __shared__ double s_J[kStateWarps][D * NC];   // J (row-major), then S
   __shared__ double s_T[kStateWarps][NC * D];   // T = Z J^T (row a of Z per row)
   __shared__ int s_dof[kStateWarps][NC];
@@ -813,8 +813,8 @@ __global__ void __launch_bounds__(kStateWarps * 32) cov_state_interpolate_kernel
   double* o = out + D * D * static_cast<size_t>(f);
   const double t = stamps[f];
   const int base = segment_base(knots, 8, 7, Kn, K, t);
-  const int gb = Kbg ? segment_base(bg, 4, 3, Kbg, KB, t) : 0;
-  const int ab = Kba ? segment_base(ba, 4, 3, Kba, KB, t) : 0;
+  const int gb = STATE && Kbg ? segment_base(bg, 4, 3, Kbg, KB, t) : 0;
+  const int ab = STATE && Kba ? segment_base(ba, 4, 3, Kba, KB, t) : 0;
   if (base < 0 || gb < 0 || ab < 0) {
     for (int e = lane; e < D * D; e += 32) o[e] = 0.0;
     if (lane == 0) invalid[f] = 1;
@@ -831,79 +831,12 @@ __global__ void __launch_bounds__(kStateWarps * 32) cov_state_interpolate_kernel
   }
   __syncwarp();
   if (lane == 0) {
-    constexpr int left = (K - 1) / 2;
-    const double* row0 = tab + static_cast<size_t>(base) * kTabStride;
-    const double t0 = row0[left * kTabStride + 24], t1 = row0[(left + 1) * kTabStride + 24];
-    const double inv_dt = 1.0 / (t1 - t0);
-    double lam[K + 1], lamd[K + 1], lamdd[K + 1];
-    basis_eval<K, true>(B, (t - t0) * inv_dt, inv_dt, lam, lamd, lamdd);
-    auto blk = [&](int r, int c) { return J + r * NC + c; };   // 3 x 3 block at row r, column c
-    auto add3 = [&](double* b, const double* M, double s) {
-      for (int i = 0; i < 3; ++i)
-        for (int c = 0; c < 3; ++c) b[i * NC + c] += s * M[3 * i + c];
-    };
-    for (int i = 0; i < 3; ++i) J[i * NC + i] = 1.0;   // M_0 = I
-    double P[9], w[3] = {0, 0, 0}, pd[3] = {0, 0, 0};
-    for (int i = 0; i < 9; ++i) P[i] = row0[i];
-#pragma unroll 1
-    for (int j = 1; j < K; ++j) {
-      const double* rj = row0 + j * kTabStride;
-      const double d[3] = {rj[12], rj[13], rj[14]};
-      const double lw[3] = {lam[j] * d[0], lam[j] * d[1], lam[j] * d[2]};
-      double A[9], Jr[9], Pn[9], G[9], lj[9], X[9], XG[9], M[9];
-      so3_exp_and_Jr(lw, A, Jr);
-      m3_mul(P, A, Pn);
-      for (int i = 0; i < 9; ++i) { G[i] = rj[15 + i]; lj[i] = lam[j] * Jr[i]; }
-      double aw[3];
-      m3_tvec(A, w, aw);
-      hat_mul(aw, lj, X);
-      for (int i = 0; i < 3; ++i) X[4 * i] += lamd[j];
-      // theta rows: + M_j on phi_j, - M_j on phi_{j-1} (the same roundings as cov_interpolate_kernel's D_m)
-      m3_mul(Jr, G, XG);
-      m3_mul(Pn, XG, M);
-      for (int i = 0; i < 9; ++i) M[i] *= lam[j];
-      add3(blk(0, 6 * j), M, 1.0);
-      add3(blk(0, 6 * (j - 1)), M, -1.0);
-      // omega rows (R^T applied below): + Y_j on phi_j, - Y_j on phi_{j-1}
-      m3_mul(X, G, XG);
-      m3_mul(Pn, XG, M);
-      add3(blk(6, 6 * j), M, 1.0);
-      add3(blk(6, 6 * (j - 1)), M, -1.0);
-      for (int c = 0; c < 3; ++c) {
-        w[c] = aw[c] + lamd[j] * d[c];
-        pd[c] += lamd[j] * (rj[9 + c] - rj[9 + c - kTabStride]);
-      }
-      for (int i = 0; i < 9; ++i) P[i] = Pn[i];
-    }
-    // P = R: omega rows R^T (Y_m - Y_{m+1}); v rows hat(v) R^T D_m and (lamd_m - lamd_{m+1}) R^T; p rows w_m I
-    double v[3], H[9];
-    m3_tvec(P, pd, v);
-    {
-      double Rt[9];
-      for (int i = 0; i < 3; ++i)
-        for (int c = 0; c < 3; ++c) Rt[3 * i + c] = P[3 * c + i];
-      hat_mul(v, Rt, H);
-    }
-#pragma unroll 1
-    for (int m = 0; m < K; ++m) {
-      double Y[9], Dm[9], Z[9];
-      for (int i = 0; i < 3; ++i)
-        for (int c = 0; c < 3; ++c) { Y[3 * i + c] = blk(6, 6 * m)[i * NC + c]; Dm[3 * i + c] = blk(0, 6 * m)[i * NC + c]; }
-      m3_tmul(P, Y, Z);
-      for (int i = 0; i < 3; ++i)
-        for (int c = 0; c < 3; ++c) blk(6, 6 * m)[i * NC + c] = Z[3 * i + c];
-      m3_mul(H, Dm, Z);
-      add3(blk(9, 6 * m), Z, 1.0);
-      const double wd = lamd[m] - lamd[m + 1], wm = lam[m] - lam[m + 1];
-      for (int i = 0; i < 3; ++i) {
-        blk(3, 6 * m + 3)[i * NC + i] = wm;
-        for (int c = 0; c < 3; ++c) blk(9, 6 * m + 3)[i * NC + c] = wd * P[3 * c + i];
-      }
-    }
+    double R[9], p[3];
+    cov_stamp_jacobian<K, ROWS, NC>(tab, B, base, t, J, R, p);
     // bias rows
     constexpr int lb = (KB - 1) / 2;
     double lbw[KB + 1];
-    for (int s = 0; s < 2; ++s) {
+    for (int s = 0; STATE && s < 2; ++s) {
       const int Kb = s ? Kba : Kbg;
       if (!Kb) continue;
       const double* b0 = (s ? ba + 4 * static_cast<size_t>(ab) : bg + 4 * static_cast<size_t>(gb));
@@ -964,7 +897,7 @@ __global__ void __launch_bounds__(kStateWarps * 32) cov_state_interpolate_kernel
 // Joint and relative covariance of the poses at two stamps (hb200_set_covariance_stamp_pairs), computed inside the
 // compute from its Sigma and the far scratch, at the knots the build linearised at (the snapshot knot table).
 //   joint    (12 x 12) of [theta_a p_a | theta_b p_b]: blocks J_s Sigma_{span(s), span(s')} J_s'^T, J(t) the pose
-//            Jacobian of cov_interpolate_kernel (global rotation tangent, p <- p + rho);
+//            Jacobian of cov_stamp_jacobian (global rotation tangent, p <- p + rho);
 //   relative (6 x 6) of T_ab = T_a^-1 T_b (R_ab = R_a^T R_b, p_ab = R_a^T (p_b - p_a)) in the same split tangent in frame
 //            a: A joint A^T with A = Rb M, Rb = diag(R_a^T, R_a^T), M = [[-I, 0, I, 0], [hat(p_b - p_a), -I, 0, I]].
 // ---------------------------------------------------------------------------------------------
@@ -977,53 +910,8 @@ __global__ void cov_stamp_span_kernel(int n, const double* __restrict__ stamps, 
   span[q] = make_int2(segment_base(knots, 8, 7, Kn, k, stamps[2 * q]), segment_base(knots, 8, 7, Kn, k, stamps[2 * q + 1]));
 }
 
-// J(t) (6 x 6K row-major, dense) of the pose at t over control points base .. base + K - 1 -- the operations of
-// cov_interpolate_kernel's builder in its order, so D_m = M_m - M_{m+1} rounds the same -- and the pose R (row-major), p.
-template <int K>
-HB_DI void cov_pose_jacobian(const double* __restrict__ tab, const Basis& B, int base, double t, double* J, double* R, double* p) {
-  constexpr int left = (K - 1) / 2, NC = 6 * K;
-  const double* row0 = tab + static_cast<size_t>(base) * kTabStride;
-  const double t0 = row0[left * kTabStride + 24], t1 = row0[(left + 1) * kTabStride + 24];
-  const double inv_dt = 1.0 / (t1 - t0);
-  double lam[K + 1];
-  basis_eval<K, false>(B, (t - t0) * inv_dt, inv_dt, lam, nullptr, nullptr);
-  for (int e = 0; e < 6 * NC; ++e) J[e] = 0.0;
-  for (int i = 0; i < 3; ++i) J[i * NC + i] = 1.0;   // M_0 = I
-  double P[9], pp[3] = {row0[9], row0[10], row0[11]};
-#pragma unroll
-  for (int i = 0; i < 9; ++i) P[i] = row0[i];
-#pragma unroll 1
-  for (int j = 1; j < K; ++j) {
-    const double* rj = row0 + j * kTabStride;
-    const double wj[3] = {lam[j] * rj[12], lam[j] * rj[13], lam[j] * rj[14]};
-    double A[9], Jr[9], Pn[9], G[9], JG[9], PJG[9];
-    so3_exp_and_Jr(wj, A, Jr);
-    m3_mul(P, A, Pn);
-#pragma unroll
-    for (int i = 0; i < 9; ++i) G[i] = rj[15 + i];
-    m3_mul(Jr, G, JG);
-    m3_mul(Pn, JG, PJG);
-#pragma unroll
-    for (int i = 0; i < 9; ++i) {
-      const double Mj = lam[j] * PJG[i];
-      J[(i / 3) * NC + 6 * j + i % 3] += Mj;
-      J[(i / 3) * NC + 6 * (j - 1) + i % 3] -= Mj;
-      P[i] = Pn[i];
-    }
-#pragma unroll
-    for (int c = 0; c < 3; ++c) pp[c] += lam[j] * (rj[9 + c] - rj[9 + c - kTabStride]);
-  }
-  for (int mm = 0; mm < K; ++mm) {
-    const double wm = lam[mm] - lam[mm + 1];
-    for (int i = 0; i < 3; ++i) J[(3 + i) * NC + 6 * mm + 3 + i] = wm;
-  }
-#pragma unroll
-  for (int i = 0; i < 9; ++i) R[i] = P[i];
-#pragma unroll
-  for (int c = 0; c < 3; ++c) p[c] = pp[c];
-}
-
-// One warp per pair.  Lanes 0 and 1 build J_a and J_b; T = Z J^T over the 2 x 6k span dofs (row a of Z per lane, its
+// One warp per pair.  Lanes 0 and 1 build J_a and J_b (cov_stamp_jacobian, as cov_stamp_kernel<K, 6> does, whose sums
+// the diagonal blocks repeat term for term); T = Z J^T over the 2 x 6k span dofs (row a of Z per lane, its
 // entries gathered through cov_sigma: band, arrow and the far scratch the plan filled), S = blockdiag(J_a, J_b) T,
 // joint = 0.5 (S + S^T); then E = M joint, F = E M^T, relative = 0.5 (Rb F Rb^T + (Rb F Rb^T)^T).  Swapping the stamps
 // relabels the blocks of every sum without reordering its terms, so (t_b, t_a) is exactly the permutation of
@@ -1052,7 +940,14 @@ __global__ void __launch_bounds__(kPairWarps * 32) cov_pose_pair_kernel(
   }
   const int base[2] = {sp.x, sp.y};
   double* T = s_T[warp];
-  if (lane < 2) cov_pose_jacobian<K>(tab, B, base[lane], stamps[2 * static_cast<size_t>(q) + lane], s_J[warp][lane], s_P[warp][lane], s_P[warp][lane] + 9);
+  for (int e = lane; e < 2 * 6 * NC; e += 32) s_J[warp][e / (6 * NC)][e % (6 * NC)] = 0.0;
+  __syncwarp();
+  if (lane < 2) {
+    double R[9], p[3];
+    cov_stamp_jacobian<K, 6, NC>(tab, B, base[lane], stamps[2 * static_cast<size_t>(q) + lane], s_J[warp][lane], R, p);
+    for (int i = 0; i < 9; ++i) s_P[warp][lane][i] = R[i];
+    for (int c = 0; c < 3; ++c) s_P[warp][lane][9 + c] = p[c];
+  }
   __syncwarp();
   for (int a = lane; a < 2 * NC; a += 32) {
     const int ga = 6 * base[a / NC] + a % NC;

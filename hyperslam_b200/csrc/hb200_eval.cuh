@@ -9,8 +9,7 @@
 // and projects Jacobians straight into the tangent space the Ceres manifolds would project them to
 // (reference include/hyper/optimizers/ceres/manifolds/variables/wrapper.hpp:36-42).
 #pragma once
-#include "hb200_math.cuh"
-#include "hb200_types.cuh"
+#include "hb200_spline.cuh"
 
 namespace hb {
 
@@ -250,26 +249,6 @@ __global__ void calib_kernel(int C, const double* __restrict__ cams, double* __r
   }
 }
 
-// ---------------------------------------------------------------------------------------------
-// Basis evaluation (Horner), lam[0] = 1, lam[K] = 0.
-// ---------------------------------------------------------------------------------------------
-template <int K, bool DERIV>
-HB_DI void basis_eval(const Basis& b, double u, double inv_dt, double* lam, double* lamd, double* lamdd) {
-  lam[0] = 1.0; lam[K] = 0.0;
-  if (DERIV) { lamd[0] = lamdd[0] = 0.0; lamd[K] = lamdd[K] = 0.0; }
-#pragma unroll
-  for (int j = 1; j < K; ++j) {
-    double v = 0, d1 = 0, d2 = 0;
-#pragma unroll
-    for (int n = K - 1; n >= 0; --n) {
-      if (DERIV) { d2 = d2 * u + 2.0 * d1; d1 = d1 * u + v; }
-      v = v * u + b.Mc[j * K + n];
-    }
-    lam[j] = v;
-    if (DERIV) { lamd[j] = d1 * inv_dt; lamdd[j] = d2 * inv_dt * inv_dt; }
-  }
-}
-
 HB_DI double huber_rho(double s, double delta, double* weight) {
   if (s <= delta * delta) { *weight = 1.0; return s; }
   const double rt = sqrt(s);
@@ -286,22 +265,8 @@ HB_DI void st_v4(double* p, double a, double b, double c, double d) {
   asm volatile("st.global.v2.f64 [%0], {%1, %2};\n\tst.global.v2.f64 [%0+16], {%3, %4};" ::"l"(p), "d"(a), "d"(b), "d"(c), "d"(d) : "memory");
 }
 
-// ---- per-step math, shared by the one-factor-per-thread bodies and the lane-group bodies of the small-window kernel ----
-// Step j of the forward sweep: A = Exp(lam_j d_j) and, with Jr, Jr(lam_j d_j)   (rj: knot-table row j of the factor)
-HB_DI void spline_step_exp(const double* rj, double lj, double* A, double* Jr) {
-  const double w[3] = {lj * rj[12], lj * rj[13], lj * rj[14]};
-  so3_exp_and_Jr(w, A, Jr);
-}
-// pixel block of step j: M_j = lam_j P_j Jr_j G_j   (P_j: pose rotation after step j)
-HB_DI void pixel_step_block(const double* rj, double lj, const double* Pj, const double* Jr, double* M) {
-  double G[9], JG[9], PJG[9];
-#pragma unroll
-  for (int i = 0; i < 9; ++i) G[i] = rj[15 + i];
-  m3_mul(Jr, G, JG);
-  m3_mul(Pj, JG, PJG);
-#pragma unroll
-  for (int i = 0; i < 9; ++i) M[i] = lj * PJG[i];
-}
+// ---- per-step pixel math, shared by the one-factor-per-thread bodies and the lane-group bodies of the small-window kernel
+// (the spline steps are in hb200_spline.cuh) ----
 // EM = E M (2x3)
 HB_DI void pixel_em(const double* E, const double* M, double* EM) {
 #pragma unroll
@@ -733,22 +698,6 @@ HB_DI void sphere_plus_jacobian(const double* x, double* J /*3x2*/) {
   for (int c = 0; c < 2; ++c)
 #pragma unroll
     for (int r = 0; r < 3; ++r) J[2 * r + c] = nx * ((r == c ? 1.0 : 0.0) - beta * v[c] * v[r]);
-}
-
-// ---- per-step math, shared by the one-factor-per-thread body and the lane-group body of the small-window kernel ----
-// body-rate recursion of step j: aw = A_j^T w, awd = A_j^T wd, then w <- aw + lamd_j d_j, wd <- awd + lamd_j (w x d_j) + lamdd_j d_j
-HB_DI void inertial_rate_step(const double* A, const double* d, double ld, double ldd, double* w, double* wd, double* aw, double* awd) {
-  double wn[3], cr[3];
-  m3_tvec(A, w, aw);
-  m3_tvec(A, wd, awd);
-#pragma unroll
-  for (int c = 0; c < 3; ++c) wn[c] = aw[c] + ld * d[c];
-  cross(wn, d, cr);
-#pragma unroll
-  for (int c = 0; c < 3; ++c) {
-    wd[c] = awd[c] + ld * cr[c] + ldd * d[c];
-    w[c] = wn[c];
-  }
 }
 
 // Residual (reference inertial.cpp:62-79) from the pose rotation P, body rates w / wd and acceleration pdd at the stamp;
@@ -1436,43 +1385,12 @@ __global__ void bind_manifold_kernel(int n, const double* __restrict__ stamp, co
 template <int K, bool WANT_J>
 __global__ void __launch_bounds__(kEvalThreads) manifold_eval_kernel(ManifoldArgs a, Basis B) {
   __shared__ double s_cost[kEvalThreads / 32];
-  constexpr int left = (K - 1) / 2;
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   double cost = 0.0;
   if (f < a.n) {
     const int2 id = a.idx[f];
-    const double* row0 = a.tab + static_cast<size_t>(id.x) * kTabStride;
-    const double t0 = row0[left * kTabStride + 24], t1 = row0[(left + 1) * kTabStride + 24];
-    const double inv_dt = 1.0 / (t1 - t0);
-    const double u = (a.stamp[f] - t0) * inv_dt;
-    double lam[K + 1];
-    basis_eval<K, false>(B, u, inv_dt, lam, nullptr, nullptr);
-    double P[9], p[3];
-#pragma unroll
-    for (int i = 0; i < 9; ++i) P[i] = row0[i];
-    p[0] = row0[9]; p[1] = row0[10]; p[2] = row0[11];
-    double M[(K - 1) * 9];
-#pragma unroll
-    for (int j = 1; j < K; ++j) {
-      const double* rj = row0 + j * kTabStride;
-      const double w[3] = {lam[j] * rj[12], lam[j] * rj[13], lam[j] * rj[14]};
-      double A[9], Jr[9], Pn[9];
-      so3_exp_and_Jr(w, A, WANT_J ? Jr : nullptr);
-      m3_mul(P, A, Pn);
-      if (WANT_J) {
-        double G[9], JG[9], PJG[9];
-#pragma unroll
-        for (int i = 0; i < 9; ++i) G[i] = rj[15 + i];
-        m3_mul(Jr, G, JG);
-        m3_mul(Pn, JG, PJG);
-#pragma unroll
-        for (int i = 0; i < 9; ++i) M[(j - 1) * 9 + i] = lam[j] * PJG[i];
-      }
-#pragma unroll
-      for (int i = 0; i < 9; ++i) P[i] = Pn[i];
-#pragma unroll
-      for (int c = 0; c < 3; ++c) p[c] += lam[j] * (rj[9 + c] - rj[9 + c - kTabStride]);
-    }
+    double lam[K + 1], P[9], p[3], M[(K - 1) * 9];
+    spline_pose<K, WANT_J>(spline_segment<K>(a.tab, B, id.x, a.stamp[f], lam), lam, P, p, M);
     const double* T_bs = a.sensors + 7 * static_cast<size_t>(id.y);
     const double* z = a.meas + 7 * static_cast<size_t>(f);
     double Rbs[9], Rz[9], Rws[9], Rerr[9], Rt[3], q[4], th[3];
@@ -1498,12 +1416,7 @@ __global__ void __launch_bounds__(kEvalThreads) manifold_eval_kernel(ManifoldArg
 #pragma unroll
       for (int m = 0; m < K; ++m) {
         double D[9], AD[9], HD[9];
-#pragma unroll
-        for (int i = 0; i < 9; ++i) {
-          const double cur = (m == 0) ? ((i % 4 == 0) ? 1.0 : 0.0) : M[(m - 1) * 9 + i];
-          const double nxt = (m + 1 < K) ? M[m * 9 + i] : 0.0;
-          D[i] = cur - nxt;   // d theta / d phi_m
-        }
+        pose_theta_block<K>(M, m, D);
         m3_mul(A, D, AD);
         m3_mul(H, D, HD);
         const double wm = lam[m] - lam[m + 1];
@@ -1550,12 +1463,8 @@ __global__ void interpolate_kernel(int n, const double* __restrict__ stamps, con
     if (acc) for (int i = 0; i < 6; ++i) acc[6 * static_cast<size_t>(f) + i] = 0.0;
     return;
   }
-  constexpr int left = (K - 1) / 2;
-  const double* row0 = tab + static_cast<size_t>(base) * kTabStride;
-  const double t0 = row0[left * kTabStride + 24], t1 = row0[(left + 1) * kTabStride + 24];
-  const double inv_dt = 1.0 / (t1 - t0);
   double lam[K + 1], lamd[K + 1], lamdd[K + 1];
-  basis_eval<K, true>(B, (t - t0) * inv_dt, inv_dt, lam, lamd, lamdd);
+  const double* row0 = spline_segment<K, true>(tab, B, base, t, lam, lamd, lamdd);
   const double* k0 = knots + 8 * static_cast<size_t>(base);
   double q[4] = {k0[0], k0[1], k0[2], k0[3]};
   double p[3] = {k0[4], k0[5], k0[6]}, pd[3] = {0, 0, 0}, pdd[3] = {0, 0, 0};
@@ -1565,21 +1474,15 @@ __global__ void interpolate_kernel(int n, const double* __restrict__ stamps, con
     const double* rj = row0 + j * kTabStride;
     const double d[3] = {rj[12], rj[13], rj[14]};
     const double lw[3] = {lam[j] * d[0], lam[j] * d[1], lam[j] * d[2]};
-    double qe[4], qn[4], A[9], aw[3], awd[3], wn[3], cr[3];
+    double qe[4], qn[4], A[9], aw[3], awd[3];
     quat_exp(lw, qe);
     quat_mul(q, qe, qn);
 #pragma unroll
     for (int i = 0; i < 4; ++i) q[i] = qn[i];
-    so3_exp_and_Jr(lw, A, nullptr);
-    m3_tvec(A, w, aw);
-    m3_tvec(A, wd, awd);
-#pragma unroll
-    for (int c = 0; c < 3; ++c) wn[c] = aw[c] + lamd[j] * d[c];
-    cross(wn, d, cr);
+    spline_step_exp(rj, lam[j], A, nullptr);
+    inertial_rate_step(A, d, lamd[j], lamdd[j], w, wd, aw, awd);
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
-      wd[c] = awd[c] + lamd[j] * cr[c] + lamdd[j] * d[c];
-      w[c] = wn[c];
       const double dp = rj[9 + c] - rj[9 + c - kTabStride];
       p[c] += lam[j] * dp; pd[c] += lamd[j] * dp; pdd[c] += lamdd[j] * dp;
     }
@@ -1643,28 +1546,8 @@ HB_DI int stereo_track(int f, const double* __restrict__ stamps, const int* __re
   const int c0 = cam0[f], c1 = cam1[f];
   if (base < 0 || c0 < 0 || c0 >= C || c1 < 0 || c1 >= C) return -1;
   // pose of the body at the stamp (value only)
-  constexpr int left = (K - 1) / 2;
-  const double* row0 = tab + static_cast<size_t>(base) * kTabStride;
-  const double t0 = row0[left * kTabStride + 24], t1 = row0[(left + 1) * kTabStride + 24];
-  const double inv_dt = 1.0 / (t1 - t0);
-  double lam[K + 1];
-  basis_eval<K, false>(B, (t - t0) * inv_dt, inv_dt, lam, nullptr, nullptr);
-  double R[9], p[3];
-#pragma unroll
-  for (int i = 0; i < 9; ++i) R[i] = row0[i];
-  p[0] = row0[9]; p[1] = row0[10]; p[2] = row0[11];
-#pragma unroll
-  for (int j = 1; j < K; ++j) {
-    const double* rj = row0 + j * kTabStride;
-    const double w[3] = {lam[j] * rj[12], lam[j] * rj[13], lam[j] * rj[14]};
-    double A[9], Rn[9];
-    so3_exp_and_Jr(w, A, nullptr);
-    m3_mul(R, A, Rn);
-#pragma unroll
-    for (int i = 0; i < 9; ++i) R[i] = Rn[i];
-#pragma unroll
-    for (int c = 0; c < 3; ++c) p[c] += lam[j] * (rj[9 + c] - rj[9 + c - kTabStride]);
-  }
+  double lam[K + 1], R[9], p[3];
+  spline_pose<K, false>(spline_segment<K>(tab, B, base, t, lam), lam, R, p, nullptr);
   const double* ca = cams + 15 * static_cast<size_t>(c0);
   const double* cb = cams + 15 * static_cast<size_t>(c1);
   pixel_to_bearing(ca, px0[2 * static_cast<size_t>(f)], px0[2 * static_cast<size_t>(f) + 1], b0);

@@ -5,7 +5,8 @@ hb200_set_covariance_stamp_pairs / hb200_get_pose_pair_covariance against tests/
   sysref.forward_bound(n, kappa) (the joint in covref's correlation metric, the relative normalised by |A| sqrt(diag joint)
   since it is a difference of the joint's blocks); the largest normalised reference entry among the pairs more than
   beta apart is >= 1e3 x the bound, so a march that returned zeros fails;
-* the diagonal blocks agree with hb200_interpolate_covariance within 1e-13 (correlation metric); (t_b, t_a) is exactly
+* the diagonal blocks are bit-identical to hb200_interpolate_covariance (the same Jacobian builder and the same sums,
+  term for term; their correlation-metric distance is recorded); (t_b, t_a) is exactly
   the permutation of (t_a, t_b); both blocks are exactly symmetric; constant knots give zero rows; an out-of-span stamp
   gives status 1 and zero blocks; a non-finite stamp is refused at registration;
 * launches: stamp pairs alone add the span kernel, one far-column launch and the pair kernel; block requests registered
@@ -112,6 +113,7 @@ def test_against_reference(built, record_property, case):
         if ok.any():
             err_rel = max(err_rel, float((np.abs(np.asarray(rel[q] - want_rel, np.float64))[ok] / np.outer(s, s)[ok]).max()))
         err_diag = max(err_diag, cr.cov_error(joint[q][:6, :6], pose[q, 0]), cr.cov_error(joint[q][6:, 6:], pose[q, 1]))
+        assert same_bits(joint[q][:6, :6], pose[q, 0]) and same_bits(joint[q][6:, 6:], pose[q, 1]), q
         ba, bb = pp.pose_value(knots, order, ta)[0], pp.pose_value(knots, order, tb)[0]
         if abs(ba - bb) + order - 1 > beta:   # the off-diagonal block reads far columns
             dg = np.sqrt(np.abs(np.diagonal(want)).astype(np.float64))
@@ -133,7 +135,6 @@ def test_against_reference(built, record_property, case):
     print(f"{case}: beta {beta}, joint err {err_joint:.3e}, relative err {err_rel:.3e}, diag err {err_diag:.3e}, bound {bound:.3e}, largest {biggest:.3e}")
     assert err_joint < bound, (err_joint, bound)
     assert err_rel < bound, (err_rel, bound)
-    assert err_diag < 1e-13, err_diag
     assert biggest >= 1e3 * bound, (biggest, bound)
 
 

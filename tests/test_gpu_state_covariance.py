@@ -4,8 +4,9 @@ covref.packed_to_dense), in covref's correlation metric.
 
 * end to end (orders 4 and 6, bias splines spaced unlike the pose knots and starting inside the pose span, as after a
   slide that dropped bias knots): valid blocks within 1e-11, invalid stamps (outside the pose span, before a bias span)
-  zero and counted, output exactly symmetric and positive semidefinite after equilibration; the pose block agrees with
-  hb200_interpolate_covariance within 1e-13; one launch per call, two calls bit-identical;
+  zero and counted, output exactly symmetric and positive semidefinite after equilibration; the pose block equals
+  hb200_interpolate_covariance value for value (one Jacobian builder; the bias columns only add z * 0 terms, so zeros
+  may differ in sign); one launch per call, two calls bit-identical;
 * omega and b_g against the device's own inertial factor (identity IMU calibration): Sigma_omega,omega + Sigma_omega,bg
   + Sigma_bg,omega + Sigma_bg,bg equals the sandwich of the factor's gyro rows of Jp and wg;
 * knot increments across the small-angle switches of the SO(3) coefficients; bias_const, constant knots, no bias splines;
@@ -113,9 +114,9 @@ def test_end_to_end(built, record_property, order):
     assert np.array_equal(cov.view(np.int64), cov2.view(np.int64))
     _, invalid = compare(cov, bad, stamps, snap, order, record_property)
     assert invalid == list(range(len(stamps) - 5, len(stamps)))
-    worst = max(cr.cov_error(cov[i][:6, :6], pose[i]) for i in range(len(stamps)) if i not in invalid)
-    record_property("err_pose_block", worst)
-    assert worst < 1e-13, worst
+    for i in range(len(stamps)):
+        if i not in invalid:
+            assert np.array_equal(cov[i][:6, :6], pose[i]), i
 
 
 def test_gyro_rows_against_inertial_factor(built, record_property):
