@@ -348,6 +348,18 @@ struct hb200_ctx {
   cudaGraphExec_t graph_exec = nullptr;
   bool graph_valid = false;
 
+  // family weight matrices (hb200_set_weights): which families have one, the device table the WT kernel instantiations
+  // read (kWtSize doubles, identity where a family has none) and its host copy
+  bool wt_set[4] = {false, false, false, false};
+  DevBuf<double> wt;
+  std::array<double, kWtSize> h_wt = [] {
+    std::array<double, kWtSize> t{};
+    const int sides[4] = {2, 6, 1, 6}, offs[4] = {kWtPixel, kWtInertial, kWtBearing, kWtManifold};   // indexed by HB200_PIXEL ...
+    for (int f = 0; f < 4; ++f) for (int i = 0; i < sides[f]; ++i) t[offs[f] + (sides[f] + 1) * i] = 1.0;
+    return t;
+  }();
+  bool wt_visual() const { return wt_set[HB200_PIXEL] || wt_set[HB200_BEARING]; }
+
   int o_bg() const { return 6 * K; }
   int o_ba() const { return 6 * K + 3 * Kbg; }
   int o_g() const { return 6 * K + 3 * Kbg + 3 * Kba; }
@@ -596,17 +608,21 @@ int launch_pixel(hb200_ctx* c, int sel, double* sys) {
   if (c->Nv == 0) return 0;
   const PixelArgs a = pixel_args<J>(c, sel, sys);
   return with_pixel_pass<J>(c, a, [&](auto FUSE, auto DET) {
-    pixel_eval_kernel<K, J, FUSE, DET><<<c->n_pix_blocks, kEvalThreads, 0, c->stream>>>(a, c->basis, DET ? c->det_pix : DetOut{}, DET ? c->det_seg_off.p : nullptr);
-    return check_launch(c, DET ? "pixel_eval_det_kernel" : "pixel_eval_kernel");
+    return with_flag(c->wt_visual(), [&](auto WT) {
+      pixel_eval_kernel<K, J, FUSE, DET, WT><<<c->n_pix_blocks, kEvalThreads, 0, c->stream>>>(a, c->basis, DET ? c->det_pix : DetOut{}, DET ? c->det_seg_off.p : nullptr,
+                                                                                            c->wt.p);
+      return check_launch(c, DET ? "pixel_eval_det_kernel" : "pixel_eval_kernel");
+    });
   });
 }
 template <int K, bool J>
 int launch_inertial(hb200_ctx* c, int sel) {
   if (c->Ni == 0) return 0;
   const InertialArgs a = inertial_args<J>(c, sel);
-  inertial_eval_kernel<K, 4, J><<<c->n_imu_blocks, kEvalThreads, J ? inertial_stash_bytes(K) : 0, side(c)>>>(a, c->basis, c->bias_basis);
-  HB_LAUNCH(c, "inertial_eval_kernel");
-  return 0;
+  return with_flag(c->wt_set[HB200_INERTIAL], [&](auto WT) {
+    inertial_eval_kernel<K, 4, J, WT><<<c->n_imu_blocks, kEvalThreads, J ? inertial_stash_bytes(K) : 0, side(c)>>>(a, c->basis, c->bias_basis, c->wt.p);
+    return check_launch(c, "inertial_eval_kernel");
+  });
 }
 // visual + inertial factors in one launch (both lists non-empty)
 template <int K, bool J>
@@ -615,9 +631,11 @@ int launch_factors_merged(hb200_ctx* c, int sel, double* sys) {
   const InertialArgs ia = inertial_args<J>(c, sel);
   const int blocks = c->n_pix_blocks + c->n_imu_blocks;
   return with_pixel_pass<J>(c, pa, [&](auto FUSE, auto DET) {
-    factor_eval_kernel<K, 4, J, FUSE, DET><<<blocks, kEvalThreads * factor_lanes(K), 0, c->stream>>>(pa, ia, c->basis, c->bias_basis, c->n_pix_blocks, DET ? c->det_pix : DetOut{},
-                                                                                     DET ? c->det_seg_off.p : nullptr);
-    return check_launch(c, DET ? "factor_eval_det_kernel" : "factor_eval_kernel");
+    return with_flag(c->wt_visual() || c->wt_set[HB200_INERTIAL], [&](auto WT) {
+      factor_eval_kernel<K, 4, J, FUSE, DET, WT><<<blocks, kEvalThreads * factor_lanes(K), 0, c->stream>>>(pa, ia, c->basis, c->bias_basis, c->n_pix_blocks,
+                                                                                           DET ? c->det_pix : DetOut{}, DET ? c->det_seg_off.p : nullptr, c->wt.p);
+      return check_launch(c, DET ? "factor_eval_det_kernel" : "factor_eval_kernel");
+    });
   });
 }
 template <int K, bool J>
@@ -626,9 +644,10 @@ int launch_manifold(hb200_ctx* c, int sel) {
   ManifoldArgs a{};
   a.n = c->Nm; a.stamp = c->m_stamp.p; a.meas = c->m_meas.p; a.idx = c->m_idx.p; a.tab = c->tab[sel].p; a.sensors = c->sensors.p;
   a.r = J ? c->m_r.p : nullptr; a.Jp = c->m_Jp.p; a.cost_partial = c->cp_imu[J ? 0 : 1].p + c->n_imu_blocks;
-  manifold_eval_kernel<K, J><<<c->n_man_blocks, kEvalThreads, 0, side(c)>>>(a, c->basis);
-  HB_LAUNCH(c, "manifold_eval_kernel");
-  return 0;
+  return with_flag(c->wt_set[HB200_MANIFOLD], [&](auto WT) {
+    manifold_eval_kernel<K, J, WT><<<c->n_man_blocks, kEvalThreads, 0, side(c)>>>(a, c->basis, c->wt.p);
+    return check_launch(c, "manifold_eval_kernel");
+  });
 }
 
 // The factor kernels of state `sel` (0: current, 1: trial) on its up-to-date knot table: residuals and cost partials,
@@ -684,9 +703,10 @@ int enqueue_evaluate(hb200_ctx* c, bool want_J, int sel) {
 // Inertial J^T J: large windows (>= 16 384 inertial factors) take the augmented product on the FP64 tensor cores, ~6 CTAs
 // per SM of 8-factor chunks; small windows the scalar block-by-block kernel on short runs (cfg1, ~9 factors per CTA), which
 // is faster there.  (Order 6 keeps 12-factor chunks at ~2 CTAs per SM, which beat 8-factor chunks at ~6 CTAs per SM on the
-// order-6 window.)  Returns the CTAs per run.
+// order-6 window.)  A set inertial weight matrix makes the bias columns dense, which only the augmented product covers: it
+// selects the tensor-core kernel at every size.  Returns the CTAs per run.
 int inertial_splits(const hb200_ctx* c, bool* scalar_hess) {
-  *scalar_hess = c->Ni < 16384;
+  *scalar_hess = c->Ni < 16384 && !c->wt_set[HB200_INERTIAL];
   return (*scalar_hess || c->k != 4) ? c->imu_splits : c->imu_splits_mma;
 }
 
@@ -706,10 +726,14 @@ int enqueue_build(hb200_ctx* c, const SolverState* st) {
         if (scalar_hess)
           inertial_hessian_kernel<K, 4, DET><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->i_idx.p, c->i_r.p, c->i_Jp.p, c->i_wg.p, c->i_wa.p, c->i_Jg.p,
                                                                                  c->imu_scale, c->assembly(), c->lay, c->o_bg(), c->o_ba(), c->o_g(), splits, d);
+        else if (c->wt_set[HB200_INERTIAL])
+          inertial_hessian_mma_kernel<K, 4, K == 4 ? 8 : 12, DET, true><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->i_idx.p, c->i_r.p, c->i_Jp.p, c->i_wg.p,
+                                                                                                           c->i_wa.p, c->i_Jg.p, c->imu_scale, c->assembly(), c->lay,
+                                                                                                           c->o_bg(), c->o_ba(), c->o_g(), splits, d, c->wt.p);
         else
-          inertial_hessian_mma_kernel<K, 4, K == 4 ? 8 : 12, DET><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->i_idx.p, c->i_r.p, c->i_Jp.p, c->i_wg.p, c->i_wa.p,
-                                                                                                     c->i_Jg.p, c->imu_scale, c->assembly(), c->lay, c->o_bg(), c->o_ba(),
-                                                                                                     c->o_g(), splits, d);
+          inertial_hessian_mma_kernel<K, 4, K == 4 ? 8 : 12, DET, false><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->i_idx.p, c->i_r.p, c->i_Jp.p, c->i_wg.p, c->i_wa.p,
+                                                                                                            c->i_Jg.p, c->imu_scale, c->assembly(), c->lay, c->o_bg(), c->o_ba(),
+                                                                                                            c->o_g(), splits, d, nullptr);
         return check_launch(c, scalar_hess ? (DET ? "inertial_hessian_det_kernel" : "inertial_hessian_kernel")
                                            : (DET ? "inertial_hessian_mma_det_kernel" : "inertial_hessian_mma_kernel"));
       });
@@ -1160,8 +1184,10 @@ int create_impl(const hb200_options* options, hb200_ctx* c) {
   // the Jacobian pass of the large-window inertial kernel parks its forward-sweep state in dynamic shared memory (41.5 KB
   // at order 4, 69 KB at order 6: above the 48 KB default)
   rc = for_each_order_mode([&](auto K, auto DET) {
-    if constexpr (!DET)
-      HB_CUDA(cudaFuncSetAttribute(inertial_eval_kernel<K, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(inertial_stash_bytes(K))));
+    if constexpr (!DET) {
+      HB_CUDA(cudaFuncSetAttribute(inertial_eval_kernel<K, 4, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(inertial_stash_bytes(K))));
+      HB_CUDA(cudaFuncSetAttribute(inertial_eval_kernel<K, 4, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(inertial_stash_bytes(K))));
+    }
     return 0;
   });
   return rc ? rc : reset_solver_state(c);
@@ -1467,6 +1493,27 @@ int hb200_set_pixel_factors(hb200_ctx* c, int n, const double* stamp, const int*
 int hb200_set_bearing_factors(hb200_ctx* c, int n, const double* stamp, const int* camera, const int* landmark, const double* bearing) {
   if (!c || n < 0 || (n > 0 && (!stamp || !camera || !landmark || !bearing))) return fail(-1, "invalid bearing factors");
   return set_visual_family(c, 1, n, stamp, camera, landmark, bearing);
+}
+
+int hb200_set_weights(hb200_ctx* c, int kind, const double* W) {
+  if (!c) return fail(-1, "null context");
+  if (kind < HB200_PIXEL || kind > HB200_MANIFOLD) return fail(-1, "unknown factor kind %d", kind);
+  const int sides[4] = {2, 6, 1, 6}, offs[4] = {kWtPixel, kWtInertial, kWtBearing, kWtManifold};
+  const int d = sides[kind], o = offs[kind];
+  if (W) for (int i = 0; i < d * d; ++i) if (!std::isfinite(W[i])) return fail(-1, "weight matrix entry %d is not finite", i);
+  std::array<double, kWtSize> next = c->h_wt;
+  for (int i = 0; i < d * d; ++i) next[o + i] = W ? W[i] : (i % (d + 1) == 0 ? 1.0 : 0.0);
+  const bool set = W != nullptr;
+  if (set == c->wt_set[kind] && (!set || next == c->h_wt)) return 0;   // the current value: nothing changes
+  HB_CUDA(cudaSetDevice(c->device));
+  HB_CUDA(cudaStreamSynchronize(c->stream));   // no launch still reading the table
+  HB_CUDA(c->wt.ensure(kWtSize));
+  HB_CUDA(cudaMemcpy(c->wt.p, next.data(), sizeof(double) * kWtSize, cudaMemcpyHostToDevice));
+  c->h_wt = next;
+  c->wt_set[kind] = set;
+  // the kernel instantiations (and the inertial J^T J kernel with its deterministic record regions) follow the flags
+  c->kernel_args_changed();
+  return 0;
 }
 
 int hb200_set_bearing_loss(hb200_ctx* c, double huber_bearing) {
@@ -1875,8 +1922,11 @@ int ensure_calib_mirror(hb200_ctx* c) {
     HB_CUDA(dv.ensure(28 * Nv));
     const int blocks = static_cast<int>((Nv + kEvalThreads - 1) / kEvalThreads);
     const int rc = with_order(c->k, [&](auto K) {
-      pixel_calib_kernel<K><<<blocks, kEvalThreads, 0, c->stream>>>(c->Nv, c->v_stamp.p, reinterpret_cast<const double2*>(c->v_pixel.p), c->v_z.p, c->v_idx.p, c->tab[0].p, c->cam_tab.p, c->lms[0].p, c->basis, dv.p);
-      return check_launch(c, "pixel_calib_kernel");
+      return with_flag(c->wt_visual(), [&](auto WT) {
+        pixel_calib_kernel<K, WT><<<blocks, kEvalThreads, 0, c->stream>>>(c->Nv, c->v_stamp.p, reinterpret_cast<const double2*>(c->v_pixel.p), c->v_z.p, c->v_idx.p, c->tab[0].p,
+                                                                          c->cam_tab.p, c->lms[0].p, c->basis, dv.p, c->wt.p);
+        return check_launch(c, "pixel_calib_kernel");
+      });
     });
     if (rc) return rc;
     HB_CUDA(cudaMemcpyAsync(tv.data(), dv.p, sizeof(double) * 28 * Nv, cudaMemcpyDeviceToHost, c->stream));
@@ -1885,8 +1935,11 @@ int ensure_calib_mirror(hb200_ctx* c) {
     HB_CUDA(di.ensure(216 * Ni));
     const int blocks = static_cast<int>((Ni + kEvalThreads - 1) / kEvalThreads);
     const int rc = with_order(c->k, [&](auto K) {
-      inertial_calib_kernel<K><<<blocks, kEvalThreads, 0, c->stream>>>(c->Ni, c->i_stamp.p, c->i_idx.p, c->tab[0].p, c->imu.p, c->grav[0].p, c->basis, c->quirks, di.p);
-      return check_launch(c, "inertial_calib_kernel");
+      return with_flag(c->wt_set[HB200_INERTIAL], [&](auto WT) {
+        inertial_calib_kernel<K, WT><<<blocks, kEvalThreads, 0, c->stream>>>(c->Ni, c->i_stamp.p, c->i_idx.p, c->tab[0].p, c->imu.p, c->grav[0].p, c->basis, c->quirks, di.p,
+                                                                             c->wt.p);
+        return check_launch(c, "inertial_calib_kernel");
+      });
     });
     if (rc) return rc;
     HB_CUDA(cudaMemcpyAsync(ti.data(), di.p, sizeof(double) * 216 * Ni, cudaMemcpyDeviceToHost, c->stream));
@@ -1895,8 +1948,10 @@ int ensure_calib_mirror(hb200_ctx* c) {
     HB_CUDA(dm.ensure(36 * Nm));
     const int blocks = static_cast<int>((Nm + kEvalThreads - 1) / kEvalThreads);
     const int rc = with_order(c->k, [&](auto K) {
-      manifold_calib_kernel<K><<<blocks, kEvalThreads, 0, c->stream>>>(c->Nm, c->m_stamp.p, c->m_meas.p, c->m_idx.p, c->tab[0].p, c->sensors.p, c->basis, dm.p);
-      return check_launch(c, "manifold_calib_kernel");
+      return with_flag(c->wt_set[HB200_MANIFOLD], [&](auto WT) {
+        manifold_calib_kernel<K, WT><<<blocks, kEvalThreads, 0, c->stream>>>(c->Nm, c->m_stamp.p, c->m_meas.p, c->m_idx.p, c->tab[0].p, c->sensors.p, c->basis, dm.p, c->wt.p);
+        return check_launch(c, "manifold_calib_kernel");
+      });
     });
     if (rc) return rc;
     HB_CUDA(cudaMemcpyAsync(c->m_m_Jc.data(), dm.p, sizeof(double) * 36 * Nm, cudaMemcpyDeviceToHost, c->stream));
@@ -1991,14 +2046,20 @@ int hb200_factor_evaluate(hb200_ctx* c, int kind, int index, const double* const
       if (b == 0) tangent_to_ambient_se3(Jc, 36, 6, parameters[k], o);
       else for (int row = 0; row < 6; ++row) for (int col = 0; col < sizes[b]; ++col) o[sizes[b] * row + col] = Jc[36 * row + coff[b] + col];
     }
+    // bias knot m: w_g[m] [I3 ; 0] / w_a[m] [0 ; I3], times the inertial weight matrix when one is set
+    const double* W = &c->h_wt[kWtInertial];
     for (int m = 0; m < kb; ++m) {
       if (double* o = jacobians[k + 5 + m]) {
         std::fill(o, o + 24, 0.0);
-        for (int a = 0; a < 3; ++a) o[4 * a + a] = c->m_i_wg[4 * static_cast<size_t>(index) + m];
+        const double wv = c->m_i_wg[4 * static_cast<size_t>(index) + m];
+        if (c->wt_set[HB200_INERTIAL]) { for (int row = 0; row < 6; ++row) for (int a = 0; a < 3; ++a) o[4 * row + a] = wv * W[6 * row + a]; }
+        else for (int a = 0; a < 3; ++a) o[4 * a + a] = wv;
       }
       if (double* o = jacobians[k + 5 + kb + m]) {
         std::fill(o, o + 24, 0.0);
-        for (int a = 0; a < 3; ++a) o[4 * (3 + a) + a] = c->m_i_wa[4 * static_cast<size_t>(index) + m];
+        const double wv = c->m_i_wa[4 * static_cast<size_t>(index) + m];
+        if (c->wt_set[HB200_INERTIAL]) { for (int row = 0; row < 6; ++row) for (int a = 0; a < 3; ++a) o[4 * row + a] = wv * W[6 * row + 3 + a]; }
+        else for (int a = 0; a < 3; ++a) o[4 * (3 + a) + a] = wv;
       }
     }
     if (double* o = jacobians[k + 5 + 2 * kb]) {

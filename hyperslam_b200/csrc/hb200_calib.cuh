@@ -10,7 +10,8 @@
 //   inertial(reference evaluators/inertial.cpp:155-194): extrinsics, gyroscope / accelerometer intrinsics,
 //           S_g, X_a, with the reference-quirk switches of the oracle                   -> Jc[n][6][36]
 // Tangent convention: R_bs <- Exp(theta) R_bs, t_bs <- t_bs + rho; the 6 -> 7 ambient adapter is applied by the
-// host copy-out exactly as for the control-point blocks.
+// host copy-out exactly as for the control-point blocks.  WT: the family's weight matrix (hb200_eval.cuh) multiplies
+// the rows, as it does every other block of the factor (reference exteroceptive.cpp:133,142).
 #pragma once
 #include "hb200_eval.cuh"
 
@@ -31,11 +32,12 @@ HB_DI void extrinsics_row(const double* a /* = d/dp_s * R_sb, 1x3 */, const doub
   out[3] = -a[0]; out[4] = -a[1]; out[5] = -a[2];
 }
 
-template <int K>
+template <int K, bool WT>
 __global__ void __launch_bounds__(kEvalThreads) pixel_calib_kernel(int n, const double* __restrict__ stamp, const double2* __restrict__ pixel,
                                                                    const double* __restrict__ meas_z, const int4* __restrict__ idx,
                                                                    const double* __restrict__ tab, const double* __restrict__ cam_tab,
-                                                                   const double* __restrict__ landmarks, Basis B, double* __restrict__ Jc /*[n][2][14]*/) {
+                                                                   const double* __restrict__ landmarks, Basis B, double* __restrict__ Jc /*[n][2][14]*/,
+                                                                   const double* __restrict__ wt) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= n) return;
   const int4 id = idx[f];
@@ -96,15 +98,22 @@ __global__ void __launch_bounds__(kEvalThreads) pixel_calib_kernel(int n, const 
     for (int j = 0; j < 3; ++j) a[j] = Jps[3 * i] * cam[j] + Jps[3 * i + 1] * cam[3 + j] + Jps[3 * i + 2] * cam[6 + j];
     extrinsics_row(a, pbt, &J[14 * i]);
   }
+  if constexpr (WT) {
+    double W[4];
+    if (id.w == 0) { W[0] = wt[kWtPixel]; W[1] = wt[kWtPixel + 1]; W[2] = wt[kWtPixel + 2]; W[3] = wt[kWtPixel + 3]; }
+    else { W[0] = wt[kWtBearing]; W[1] = 0.0; W[2] = 0.0; W[3] = 1.0; }
+    weigh_rows<2, 14>(W, J);
+  }
   double* out = Jc + 28 * static_cast<size_t>(f);
 #pragma unroll
   for (int i = 0; i < 28; ++i) out[i] = J[i];
 }
 
-template <int K>
+template <int K, bool WT>
 __global__ void __launch_bounds__(kEvalThreads) manifold_calib_kernel(int n, const double* __restrict__ stamp, const double* __restrict__ meas,
                                                                       const int2* __restrict__ idx, const double* __restrict__ tab,
-                                                                      const double* __restrict__ sensors, Basis B, double* __restrict__ Jc /*[n][6][6]*/) {
+                                                                      const double* __restrict__ sensors, Basis B, double* __restrict__ Jc /*[n][6][6]*/,
+                                                                      const double* __restrict__ wt) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= n) return;
   const int2 id = idx[f];
@@ -125,6 +134,20 @@ __global__ void __launch_bounds__(kEvalThreads) manifold_calib_kernel(int n, con
   m3_mul(A, P, AR);
   // manifold.cpp:57: J_metric * J(T_wb (+) T_bs wrt T_bs) = blockdiag(Jl^{-1} R_wb, R_wb)
   double* out = Jc + 36 * static_cast<size_t>(f);
+  if constexpr (WT) {
+    double J[36];
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        J[6 * i + c] = AR[3 * i + c]; J[6 * i + 3 + c] = 0.0;
+        J[6 * (3 + i) + c] = 0.0; J[6 * (3 + i) + 3 + c] = P[3 * i + c];
+      }
+    weigh_rows<6, 6>(wt + kWtManifold, J);
+#pragma unroll
+    for (int i = 0; i < 36; ++i) out[i] = J[i];
+    return;
+  }
 #pragma unroll
   for (int i = 0; i < 3; ++i)
 #pragma unroll
@@ -134,11 +157,11 @@ __global__ void __launch_bounds__(kEvalThreads) manifold_calib_kernel(int n, con
     }
 }
 
-template <int K>
+template <int K, bool WT>
 __global__ void __launch_bounds__(kEvalThreads) inertial_calib_kernel(int n, const double* __restrict__ stamp, const int4* __restrict__ idx,
                                                                       const double* __restrict__ tab, const double* __restrict__ imu /*raw 37*/,
                                                                       const double* __restrict__ gravity, Basis B, int quirks,
-                                                                      double* __restrict__ Jc /*[n][6][36]*/) {
+                                                                      double* __restrict__ Jc /*[n][6][36]*/, const double* __restrict__ wt) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= n) return;
   double lam[K + 1], lamd[K + 1], lamdd[K + 1];
@@ -260,6 +283,19 @@ __global__ void __launch_bounds__(kEvalThreads) inertial_calib_kernel(int n, con
         if (!q_sg) J[36 * i + 27 + 3 * r + j] = Sg[3 * i + r] * Fa[3 * r + j];
       }
   double* out = Jc + 216 * static_cast<size_t>(f);
+  if constexpr (WT) {   // column by column: W mixes the six rows of each of the 36 columns
+    const double* W = wt + kWtInertial;
+#pragma unroll 1
+    for (int col = 0; col < 36; ++col) {
+      double x[6];
+#pragma unroll
+      for (int i = 0; i < 6; ++i) x[i] = J[36 * i + col];
+      weigh_rows<6, 1>(W, x);
+#pragma unroll
+      for (int i = 0; i < 6; ++i) out[36 * i + col] = x[i];
+    }
+    return;
+  }
 #pragma unroll 1
   for (int i = 0; i < 216; ++i) out[i] = J[i];
 }

@@ -249,6 +249,47 @@ __global__ void calib_kernel(int C, const double* __restrict__ cams, double* __r
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// Family weight matrices (hb200_set_weights; reference exteroceptive.cpp:101-160, CostConfiguration::weights): one
+// row-major square matrix per factor family, applied in registers right after a factor's residual and Jacobian blocks
+// are formed, so every consumer -- cost, robust loss, J^T J, Schur complement, back-substitution, copy-outs -- reads
+// W r and W J.  The context keeps all four in one device table; a family without a matrix holds the identity there,
+// which a weighted kernel applies exactly (1 x + 0 y = x for finite y).  Kernels are instantiated weighted (template
+// flag WT) only while a family they evaluate has a matrix; the unweighted instantiations never read the table.
+// ---------------------------------------------------------------------------------------------
+constexpr int kWtPixel = 0, kWtBearing = 4, kWtInertial = 5, kWtManifold = 41, kWtSize = 77;
+
+// x <- W x for an N x COLS row-major block x (W row-major N x N)
+template <int N, int COLS>
+HB_DI void weigh_rows(const double* __restrict__ W, double* x) {
+  double y[N * COLS];
+#pragma unroll
+  for (int i = 0; i < N; ++i)
+#pragma unroll
+    for (int c = 0; c < COLS; ++c) {
+      double s = W[N * i] * x[c];
+#pragma unroll
+      for (int k = 1; k < N; ++k) s += W[N * i + k] * x[COLS * k + c];
+      y[COLS * i + c] = s;
+    }
+#pragma unroll
+  for (int i = 0; i < N * COLS; ++i) x[i] = y[i];
+}
+
+// A visual factor's residual and, WANT_J, its landmark Jacobian F and E = F hat(q) (from which every control-point block
+// follows linearly, row by row): pixel rows by the 2 x 2 pixel matrix, the bearing's one angular row by the 1 x 1 one
+// (its second row is zero).
+template <bool WANT_J>
+HB_DI void weigh_visual(const double* __restrict__ wt, int kind, double* r, double* E, double* F) {
+  double W[4];
+  if (kind == 0) { W[0] = wt[kWtPixel]; W[1] = wt[kWtPixel + 1]; W[2] = wt[kWtPixel + 2]; W[3] = wt[kWtPixel + 3]; }
+  else { W[0] = wt[kWtBearing]; W[1] = 0.0; W[2] = 0.0; W[3] = 1.0; }
+  weigh_rows<2, 1>(W, r);
+  if (!WANT_J) return;
+  weigh_rows<2, 3>(W, E);
+  weigh_rows<2, 3>(W, F);
+}
+
 HB_DI double huber_rho(double s, double delta, double* weight) {
   if (s <= delta * delta) { *weight = 1.0; return s; }
   const double rt = sqrt(s);
@@ -358,10 +399,10 @@ HB_DI void pixel_project(const double* P, const double* p, const double* __restr
 }
 
 // One thread per factor.
-template <int K, bool WANT_J>
+template <int K, bool WANT_J, bool WT>
 HB_DI void pixel_factor(const double* __restrict__ T, const Basis& B, int base, double t, double zx, double zy, double zz, int kind,
                         const double* __restrict__ cam, const double* __restrict__ lmk, double* r, double* __restrict__ Jp,
-                        double* __restrict__ Jl) {
+                        double* __restrict__ Jl, const double* __restrict__ wt) {
   constexpr int left = (K - 1) / 2;
   const double* row0 = T + static_cast<size_t>(base) * kTabStride;
   const double t0 = row0[left * kTabStride + 24], t1 = row0[(left + 1) * kTabStride + 24];
@@ -389,6 +430,7 @@ HB_DI void pixel_factor(const double* __restrict__ T, const Basis& B, int base, 
   }
   double E[6], F[6];
   pixel_project<WANT_J>(P, p, lmk, cam, zx, zy, zz, kind, r, E, F);
+  if constexpr (WT) weigh_visual<WANT_J>(wt, kind, r, E, F);
   if (!WANT_J) return;
 #pragma unroll
   for (int i = 0; i < 6; ++i) Jl[i] = F[i];
@@ -583,8 +625,8 @@ HB_DI void cta_pixel_hessian(const PixelArgs& a, int f0, int cnt, double* sJ /*[
 
 // bid: the CTA's index within the pixel grid (the merged factor kernel offsets it).  DET (fused pass, one tile per CTA):
 // the J^T J goes to the slots of the tile's segments, seg_off[bid] .. seg_off[bid + 1] - 1
-template <int K, bool WANT_J, bool FUSE, bool DET>
-HB_DI void pixel_eval_body(const PixelArgs& a, const Basis& B, int bid0, const DetOut& det, const int* seg_off) {
+template <int K, bool WANT_J, bool FUSE, bool DET, bool WT>
+HB_DI void pixel_eval_body(const PixelArgs& a, const Basis& B, int bid0, const DetOut& det, const int* seg_off, const double* __restrict__ wt) {
   __shared__ __align__(16) double s_tab[kTileRows * kTabStride];
   __shared__ __align__(8) uint64_t s_bar;
   __shared__ int s_red[2];
@@ -622,8 +664,8 @@ HB_DI void pixel_eval_body(const PixelArgs& a, const Basis& B, int bid0, const D
     double* Jp = WANT_J ? a.Jp + static_cast<size_t>(f) * 12 * K : nullptr;
     double* Jl = WANT_J ? a.Jl + static_cast<size_t>(f) * 6 : nullptr;
     const double zz = (id.w != 0) ? a.meas_z[f] : 0.0;
-    if (staged) pixel_factor<K, WANT_J>(s_tab - static_cast<ptrdiff_t>(bmin) * kTabStride, B, id.x, t, z.x, z.y, zz, id.w, cam, lmk, r, Jp, Jl);
-    else pixel_factor<K, WANT_J>(a.tab, B, id.x, t, z.x, z.y, zz, id.w, cam, lmk, r, Jp, Jl);
+    if (staged) pixel_factor<K, WANT_J, WT>(s_tab - static_cast<ptrdiff_t>(bmin) * kTabStride, B, id.x, t, z.x, z.y, zz, id.w, cam, lmk, r, Jp, Jl, wt);
+    else pixel_factor<K, WANT_J, WT>(a.tab, B, id.x, t, z.x, z.y, zz, id.w, cam, lmk, r, Jp, Jl, wt);
     if (a.r) reinterpret_cast<double2*>(a.r)[f] = make_double2(r[0], r[1]);
     double wgt;
     cost = 0.5 * huber_rho(r[0] * r[0] + r[1] * r[1], (id.w != 0) ? a.huber_bearing : a.huber, &wgt);
@@ -640,11 +682,12 @@ HB_DI void pixel_eval_body(const PixelArgs& a, const Basis& B, int bid0, const D
   if (FUSE && a.sys != nullptr) pixel_hess_flush<K, DET>(a, acc, det, DET ? seg_off[bid0 + 1] - 1 : 0);
 }
 
-// DET: the fused pass of the deterministic assembly
-template <int K, bool WANT_J, bool FUSE, bool DET>
-__global__ void __launch_bounds__(kEvalThreads, (K == 4 && FUSE) ? 6 : 1) pixel_eval_kernel(PixelArgs a, Basis B, DetOut det, const int* __restrict__ seg_off) {
+// DET: the fused pass of the deterministic assembly; WT: the visual families' weight matrices applied
+template <int K, bool WANT_J, bool FUSE, bool DET, bool WT>
+__global__ void __launch_bounds__(kEvalThreads, (K == 4 && FUSE) ? 6 : 1) pixel_eval_kernel(PixelArgs a, Basis B, DetOut det, const int* __restrict__ seg_off,
+                                                                                           const double* __restrict__ wt) {
   static_assert(!DET || (WANT_J && FUSE), "the deterministic assembly is a fused Jacobian pass");
-  pixel_eval_body<K, WANT_J, FUSE, DET>(a, B, blockIdx.x, det, seg_off);
+  pixel_eval_body<K, WANT_J, FUSE, DET, WT>(a, B, blockIdx.x, det, seg_off, wt);
 }
 
 // segments (runs of equal knot base) of every 64-factor tile of the visual list: the slots of the deterministic fused pass
@@ -790,20 +833,33 @@ HB_DI void inertial_coeffs(const double* P, const double* a_i, const double* w, 
     Kal[3 * i + 2] = (i == 0) ? -c[1] : (i == 1 ? c[0] : 0.0);
   }
 }
+// gravity tangent Jacobian: -(Cp) * PlusJacobian_sphere(g)   (6x2)
+HB_DI void inertial_gravity_jacobian(const double* __restrict__ grav, const double* Cp, double* __restrict__ Jg) {
+  double PJ[6];
+  sphere_plus_jacobian(grav, PJ);
+#pragma unroll
+  for (int i = 0; i < 6; ++i)
+#pragma unroll
+    for (int c = 0; c < 2; ++c) Jg[2 * i + c] = -(Cp[3 * i] * PJ[c] + Cp[3 * i + 1] * PJ[2 + c] + Cp[3 * i + 2] * PJ[4 + c]);
+}
 // Translation coefficients Cp = [S_g R^T ; I_a R_sb R^T] (6x3) and, Jg non-null, the gravity Jacobian.
 HB_DI void inertial_trans(const double* P, const double* __restrict__ I, const double* __restrict__ grav, double* Cp, double* __restrict__ Jg) {
   const double* IaR = I + 21;
   const double* SgJ = I + 57;
   m3_mult(SgJ, P, &Cp[0]);  // S_g R^T
   m3_mult(IaR, P, &Cp[9]);  // I_a R_sb R^T (inertial.cpp:150,198 use I_a in every variant)
-  // gravity tangent Jacobian: -(Cp) * PlusJacobian_sphere(g)   (6x2)
-  if (Jg) {
-    double PJ[6];
-    sphere_plus_jacobian(grav, PJ);
-#pragma unroll
-    for (int i = 0; i < 6; ++i)
-#pragma unroll
-      for (int c = 0; c < 2; ++c) Jg[2 * i + c] = -(Cp[3 * i] * PJ[c] + Cp[3 * i + 1] * PJ[2 + c] + Cp[3 * i + 2] * PJ[4 + c]);
+  if (Jg) inertial_gravity_jacobian(grav, Cp, Jg);
+}
+// WT: Cp <- W Cp before the gravity Jacobian is formed from it, so Jg and the translation columns are both W-weighted
+template <bool WT>
+HB_DI void inertial_trans_w(const double* P, const double* __restrict__ I, const double* __restrict__ grav, double* Cp, double* __restrict__ Jg,
+                            const double* __restrict__ W) {
+  if constexpr (WT) {
+    inertial_trans(P, I, grav, Cp, nullptr);
+    weigh_rows<6, 3>(W, Cp);
+    if (Jg) inertial_gravity_jacobian(grav, Cp, Jg);
+  } else {
+    inertial_trans(P, I, grav, Cp, Jg);
   }
 }
 
@@ -893,12 +949,14 @@ HB_DI void inertial_store_block(double* __restrict__ Jp, int m, const double* dD
 }
 
 // One thread per factor.
-template <int K, int KB, bool WANT_J>
+// WT: W (6 x 6, row-major) weighs the residual and every Jacobian block
+template <int K, int KB, bool WANT_J, bool WT>
 HB_DI void inertial_factor(const double* __restrict__ T, const Basis& B, const Basis& BB, int base, int gb, int ab, double t,
                            const double* __restrict__ z, const double* __restrict__ I, const double* __restrict__ bg,
                            const double* __restrict__ ba, const double* __restrict__ grav, double* r, double* __restrict__ Jp,
                            double* __restrict__ wg_out, double* __restrict__ wa_out, double* __restrict__ Jg,
-                           double* __restrict__ stash /* shared memory, kInertialStash(K) doubles per thread, or null when !WANT_J */) {
+                           double* __restrict__ stash /* shared memory, kInertialStash(K) doubles per thread, or null when !WANT_J */,
+                           const double* __restrict__ W) {
   constexpr int left = (K - 1) / 2;
   const double* row0 = T + static_cast<size_t>(base) * kTabStride;
   const double t0 = row0[left * kTabStride + 24], t1 = row0[(left + 1) * kTabStride + 24];
@@ -939,10 +997,11 @@ HB_DI void inertial_factor(const double* __restrict__ T, const Basis& B, const B
   }
   double a_i[3];
   inertial_residual<KB>(P, w, wd, pdd, BB, gb, ab, t, z, I, bg, ba, grav, r, a_i, wg_out, wa_out);
+  if constexpr (WT) weigh_rows<6, 1>(W, r);
   if (!WANT_J) return;
   double Bm[9], Kw[9], Kal[9], Cp[18];
   inertial_coeffs(P, a_i, w, I, Bm, Kw, Kal);
-  inertial_trans(P, I, grav, Cp, Jg);
+  inertial_trans_w<WT>(P, I, grav, Cp, Jg, W);
   // ---- backward sweep over j = K-1 .. 1 ----
   double Pc[9], QT[9], Z[9], Dprev[18];
 #pragma unroll
@@ -966,6 +1025,7 @@ HB_DI void inertial_factor(const double* __restrict__ T, const Basis& B, const B
     }
 #pragma unroll
     for (int i = 0; i < 18; ++i) { const double Di = D[i]; D[i] -= Dprev[i]; Dprev[i] = Di; }
+    if constexpr (WT) weigh_rows<6, 3>(W, D);
     inertial_store_block<K>(Jp, j, D, lamdd[j] - lamdd[j + 1], Cp);
     double Aj[9];
 #pragma unroll
@@ -977,14 +1037,15 @@ HB_DI void inertial_factor(const double* __restrict__ T, const Basis& B, const B
   inertial_block0(Bm, I, D0);
 #pragma unroll
   for (int i = 0; i < 18; ++i) D0[i] -= Dprev[i];
+  if constexpr (WT) weigh_rows<6, 3>(W, D0);
   inertial_store_block<K>(Jp, 0, D0, lamdd[0] - lamdd[1], Cp);
 }
 
 // dynamic shared memory of the Jacobian pass of the large-window inertial kernel
 constexpr size_t inertial_stash_bytes(int K) { return static_cast<size_t>(27) * (K - 1) * kEvalThreads * sizeof(double); }
 
-template <int K, int KB, bool WANT_J>
-HB_DI void inertial_eval_body(const InertialArgs& a, const Basis& B, const Basis& BB, int bid) {
+template <int K, int KB, bool WANT_J, bool WT>
+HB_DI void inertial_eval_body(const InertialArgs& a, const Basis& B, const Basis& BB, int bid, const double* __restrict__ wt) {
   extern __shared__ double s_dyn_eval[];
   double* stash = WANT_J ? s_dyn_eval + threadIdx.x : nullptr;
   __shared__ __align__(16) double s_tab[kTileRows * kTabStride];
@@ -993,8 +1054,10 @@ HB_DI void inertial_eval_body(const InertialArgs& a, const Basis& B, const Basis
   __shared__ double s_cost[kEvalThreads / 32];
   __shared__ double s_imu[kImuStride];
   __shared__ double s_grav[3];
+  __shared__ double s_w[WT ? 36 : 1];
   for (int i = threadIdx.x; i < kImuStride; i += kEvalThreads) s_imu[i] = a.imu_tab[i];
   if (threadIdx.x < 3) s_grav[threadIdx.x] = a.gravity[threadIdx.x];
+  if constexpr (WT) { if (threadIdx.x < 36) s_w[threadIdx.x] = wt[kWtInertial + threadIdx.x]; }
   const int f = bid * kEvalThreads + threadIdx.x;
   const bool active = f < a.n;
   int4 id = make_int4(0, 0, 0, 0);
@@ -1019,10 +1082,10 @@ HB_DI void inertial_eval_body(const InertialArgs& a, const Basis& B, const Basis
     double* wa = WANT_J ? a.wa + static_cast<size_t>(f) * KB : nullptr;
     double* Jg = WANT_J ? a.Jg + static_cast<size_t>(f) * 12 : nullptr;
     if (staged)
-      inertial_factor<K, KB, WANT_J>(s_tab - static_cast<ptrdiff_t>(bmin) * kTabStride, B, BB, id.x, id.y, id.z, t, z, s_imu, a.bg, a.ba,
-                                     s_grav, r, Jp, wg, wa, Jg, stash);
+      inertial_factor<K, KB, WANT_J, WT>(s_tab - static_cast<ptrdiff_t>(bmin) * kTabStride, B, BB, id.x, id.y, id.z, t, z, s_imu, a.bg, a.ba,
+                                         s_grav, r, Jp, wg, wa, Jg, stash, s_w);
     else
-      inertial_factor<K, KB, WANT_J>(a.tab, B, BB, id.x, id.y, id.z, t, z, s_imu, a.bg, a.ba, s_grav, r, Jp, wg, wa, Jg, stash);
+      inertial_factor<K, KB, WANT_J, WT>(a.tab, B, BB, id.x, id.y, id.z, t, z, s_imu, a.bg, a.ba, s_grav, r, Jp, wg, wa, Jg, stash, s_w);
     double s = 0;
 #pragma unroll
     for (int i = 0; i < 6; ++i) s += r[i] * r[i];
@@ -1034,8 +1097,10 @@ HB_DI void inertial_eval_body(const InertialArgs& a, const Basis& B, const Basis
   }
   tile_cost_sum(cost, s_cost, &a.cost_partial[bid]);
 }
-template <int K, int KB, bool WANT_J>
-__global__ void __launch_bounds__(kEvalThreads) inertial_eval_kernel(InertialArgs a, Basis B, Basis BB) { inertial_eval_body<K, KB, WANT_J>(a, B, BB, blockIdx.x); }
+template <int K, int KB, bool WANT_J, bool WT>
+__global__ void __launch_bounds__(kEvalThreads) inertial_eval_kernel(InertialArgs a, Basis B, Basis BB, const double* __restrict__ wt) {
+  inertial_eval_body<K, KB, WANT_J, WT>(a, B, BB, blockIdx.x, wt);
+}
 
 // ---------------------------------------------------------------------------------------------
 // Lane-group bodies of the small-window factor kernel.  A small window is latency-bound: with one factor per thread a
@@ -1083,10 +1148,10 @@ HB_DI LaneGroup lane_group() {
   return LaneGroup{g, min(max(g, 1), K - 1), ((1u << G) - 1u) << ((threadIdx.x & 31) & ~(G - 1))};
 }
 
-template <int K, bool WANT_J>
+template <int K, bool WANT_J, bool WT>
 HB_DI void pixel_factor_lanes(const LaneGroup& lg, const double* T, const Basis& B, int base, double t, double zx, double zy, double zz, int kind,
                               const double* __restrict__ cam, const double* __restrict__ lmk, double* r, double* __restrict__ Jp,
-                              double* __restrict__ Jl) {
+                              double* __restrict__ Jl, const double* __restrict__ wt) {
   constexpr int G = factor_lanes(K), left = (K - 1) / 2;
   static_assert(K % 2 == 0, "the sector stores pair the blocks of control points 2p and 2p + 1");
   const double* row0 = T + static_cast<size_t>(base) * kTabStride;
@@ -1118,6 +1183,7 @@ HB_DI void pixel_factor_lanes(const LaneGroup& lg, const double* T, const Basis&
   }
   double E[6], F[6];
   pixel_project<WANT_J>(P, p, lmk, cam, zx, zy, zz, kind, r, E, F);
+  if constexpr (WT) weigh_visual<WANT_J>(wt, kind, r, E, F);
   if (!WANT_J) return;
   if (lg.g == 0) {
 #pragma unroll
@@ -1155,11 +1221,12 @@ HB_DI void pixel_factor_lanes(const LaneGroup& lg, const double* T, const Basis&
 // Returns |r|^2; the leader writes r to r_out (or null).  Two CTAs per SM leave 128 registers per thread at order 4, so
 // the lane keeps only w_{j-1}, wd_{j-1} of its step and evaluates Exp / Jr of the step again after the backward state,
 // instead of keeping A_j^T w_{j-1}, A_j^T wd_{j-1}, w_j and Jr_j live across it.
-template <int K, int KB, bool WANT_J>
+template <int K, int KB, bool WANT_J, bool WT>
 HB_DI double inertial_factor_lanes(const LaneGroup& lg, const double* T, const Basis& B, const Basis& BB, int base, int gb, int ab, double t,
                                    const double* __restrict__ z, const double* __restrict__ I, const double* __restrict__ bg,
                                    const double* __restrict__ ba, const double* __restrict__ grav, double* __restrict__ r_out,
-                                   double* __restrict__ Jp, double* __restrict__ wg_out, double* __restrict__ wa_out, double* __restrict__ Jg) {
+                                   double* __restrict__ Jp, double* __restrict__ wg_out, double* __restrict__ wa_out, double* __restrict__ Jg,
+                                   const double* __restrict__ W) {
   constexpr int G = factor_lanes(K), left = (K - 1) / 2;
   const double* row0 = T + static_cast<size_t>(base) * kTabStride;
   const double t0 = row0[left * kTabStride + 24], t1 = row0[(left + 1) * kTabStride + 24];
@@ -1195,6 +1262,7 @@ HB_DI double inertial_factor_lanes(const LaneGroup& lg, const double* T, const B
   const bool lead = lg.g == 0;
   double a_i[3], r[6], sq = 0.0;
   inertial_residual<KB>(P, w, wd, pdd, BB, gb, ab, t, z, I, bg, ba, grav, r, a_i, lead ? wg_out : nullptr, lead ? wa_out : nullptr);
+  if constexpr (WT) weigh_rows<6, 1>(W, r);
 #pragma unroll
   for (int i = 0; i < 6; ++i) sq += r[i] * r[i];
   if (lead && r_out) {
@@ -1236,16 +1304,17 @@ HB_DI double inertial_factor_lanes(const LaneGroup& lg, const double* T, const B
     const double Dn = __shfl_down_sync(lg.mask, D[i], 1, G);
     D[i] -= (lg.g + 1 < K) ? Dn : 0.0;
   }
+  if constexpr (WT) weigh_rows<6, 3>(W, D);
   double Cp[18];
-  inertial_trans(P, I, grav, Cp, lead ? Jg : nullptr);
+  inertial_trans_w<WT>(P, I, grav, Cp, lead ? Jg : nullptr, W);
   if (lg.g < K) inertial_store_block<K>(Jp, lg.g, D, wdd, Cp);
   return sq;
 }
 
 // One 64-factor tile per CTA, kEvalThreads * factor_lanes(K) threads: factor t of the tile on threads [G t, G t + G).
 // The tile's cost sum and fused J^T J run on the first kEvalThreads threads, as in pixel_eval_body.
-template <int K, bool WANT_J, bool FUSE, bool DET>
-HB_DI void pixel_lanes_body(const PixelArgs& a, const Basis& B, int bid, const DetOut& det, const int* seg_off) {
+template <int K, bool WANT_J, bool FUSE, bool DET, bool WT>
+HB_DI void pixel_lanes_body(const PixelArgs& a, const Basis& B, int bid, const DetOut& det, const int* seg_off, const double* __restrict__ wt) {
   constexpr int G = factor_lanes(K);
   __shared__ __align__(16) double s_tab[kTileRows * kTabStride];
   __shared__ __align__(8) uint64_t s_bar;
@@ -1276,7 +1345,7 @@ HB_DI void pixel_lanes_body(const PixelArgs& a, const Basis& B, int bid, const D
     double* Jl = WANT_J ? a.Jl + static_cast<size_t>(f) * 6 : nullptr;
     const double zz = (id.w != 0) ? a.meas_z[f] : 0.0;
     const double* T = staged ? s_tab - static_cast<ptrdiff_t>(bmin) * kTabStride : a.tab;
-    pixel_factor_lanes<K, WANT_J>(lg, T, B, id.x, t, z.x, z.y, zz, id.w, cam, lmk, r, Jp, Jl);
+    pixel_factor_lanes<K, WANT_J, WT>(lg, T, B, id.x, t, z.x, z.y, zz, id.w, cam, lmk, r, Jp, Jl, wt);
     double wgt;
     cost = 0.5 * huber_rho(r[0] * r[0] + r[1] * r[1], (id.w != 0) ? a.huber_bearing : a.huber, &wgt);
     if (lg.g == 0) {
@@ -1297,8 +1366,8 @@ HB_DI void pixel_lanes_body(const PixelArgs& a, const Basis& B, int bid, const D
   }
 }
 
-template <int K, int KB, bool WANT_J>
-HB_DI void inertial_lanes_body(const InertialArgs& a, const Basis& B, const Basis& BB, int bid) {
+template <int K, int KB, bool WANT_J, bool WT>
+HB_DI void inertial_lanes_body(const InertialArgs& a, const Basis& B, const Basis& BB, int bid, const double* __restrict__ wt) {
   constexpr int G = factor_lanes(K);
   __shared__ __align__(16) double s_tab[kTileRows * kTabStride];
   __shared__ __align__(8) uint64_t s_bar;
@@ -1307,8 +1376,10 @@ HB_DI void inertial_lanes_body(const InertialArgs& a, const Basis& B, const Basi
   __shared__ double s_cost[kEvalThreads / 32];
   __shared__ double s_imu[kImuStride];
   __shared__ double s_grav[3];
+  __shared__ double s_w[WT ? 36 : 1];
   for (int i = threadIdx.x; i < kImuStride; i += blockDim.x) s_imu[i] = a.imu_tab[i];
   if (threadIdx.x < 3) s_grav[threadIdx.x] = a.gravity[threadIdx.x];
+  if constexpr (WT) { if (threadIdx.x < 36) s_w[threadIdx.x] = wt[kWtInertial + threadIdx.x]; }
   const LaneGroup lg = lane_group<K>();
   const int f = bid * kEvalThreads + threadIdx.x / G;
   const bool active = f < a.n;
@@ -1334,7 +1405,7 @@ HB_DI void inertial_lanes_body(const InertialArgs& a, const Basis& B, const Basi
     double* Jg = WANT_J ? a.Jg + static_cast<size_t>(f) * 12 : nullptr;
     double* r = a.r ? a.r + 6 * static_cast<size_t>(f) : nullptr;
     const double* T = staged ? s_tab - static_cast<ptrdiff_t>(bmin) * kTabStride : a.tab;
-    const double s = inertial_factor_lanes<K, KB, WANT_J>(lg, T, B, BB, id.x, id.y, id.z, t, z, s_imu, a.bg, a.ba, s_grav, r, Jp, wg, wa, Jg);
+    const double s = inertial_factor_lanes<K, KB, WANT_J, WT>(lg, T, B, BB, id.x, id.y, id.z, t, z, s_imu, a.bg, a.ba, s_grav, r, Jp, wg, wa, Jg, s_w);
     cost = 0.5 * a.loss_scale * s;
   }
   if (lg.g == 0) s_fcost[threadIdx.x / G] = cost;
@@ -1345,12 +1416,14 @@ HB_DI void inertial_lanes_body(const InertialArgs& a, const Basis& B, const Basi
 
 // Visual and inertial factors of a small window in ONE launch (they are independent): CTAs [0, n_pix_blocks) run the
 // pixel / bearing body, the rest the inertial body, both on lane groups.  A pass costs the longer of the two families.
-template <int K, int KB, bool WANT_J, bool FUSE, bool DET>
+// WT: the weight matrices of both (a family without one holds the identity in the table).
+template <int K, int KB, bool WANT_J, bool FUSE, bool DET, bool WT>
 __global__ void __launch_bounds__(kEvalThreads * factor_lanes(K), K == 4 ? 2 : 1)
-    factor_eval_kernel(PixelArgs pa, InertialArgs ia, Basis B, Basis BB, int n_pix_blocks, DetOut det, const int* __restrict__ seg_off) {
+    factor_eval_kernel(PixelArgs pa, InertialArgs ia, Basis B, Basis BB, int n_pix_blocks, DetOut det, const int* __restrict__ seg_off,
+                       const double* __restrict__ wt) {
   static_assert(!DET || (WANT_J && FUSE), "the deterministic assembly is a fused Jacobian pass");
-  if (static_cast<int>(blockIdx.x) < n_pix_blocks) pixel_lanes_body<K, WANT_J, FUSE, DET>(pa, B, blockIdx.x, det, seg_off);
-  else inertial_lanes_body<K, KB, WANT_J>(ia, B, BB, blockIdx.x - n_pix_blocks);
+  if (static_cast<int>(blockIdx.x) < n_pix_blocks) pixel_lanes_body<K, WANT_J, FUSE, DET, WT>(pa, B, blockIdx.x, det, seg_off, wt);
+  else inertial_lanes_body<K, KB, WANT_J, WT>(ia, B, BB, blockIdx.x - n_pix_blocks, wt);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1382,8 +1455,9 @@ __global__ void bind_manifold_kernel(int n, const double* __restrict__ stamp, co
   if (base < 0 || s < 0 || s >= P) atomicAdd(num_invalid, 1);
 }
 
-template <int K, bool WANT_J>
-__global__ void __launch_bounds__(kEvalThreads) manifold_eval_kernel(ManifoldArgs a, Basis B) {
+// WT: the pose family's 6 x 6 weight matrix applied to the residual and each control point's 6 x 6 block
+template <int K, bool WANT_J, bool WT>
+__global__ void __launch_bounds__(kEvalThreads) manifold_eval_kernel(ManifoldArgs a, Basis B, const double* __restrict__ wt) {
   __shared__ double s_cost[kEvalThreads / 32];
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   double cost = 0.0;
@@ -1402,6 +1476,7 @@ __global__ void __launch_bounds__(kEvalThreads) manifold_eval_kernel(ManifoldArg
     rot_to_quat(Rerr, q);
     quat_log(q, th);
     double r[6] = {th[0], th[1], th[2], p[0] + Rt[0] - z[4], p[1] + Rt[1] - z[5], p[2] + Rt[2] - z[6]};
+    if constexpr (WT) weigh_rows<6, 1>(wt + kWtManifold, r);
     if (a.r) {
 #pragma unroll
       for (int i = 0; i < 6; ++i) a.r[6 * static_cast<size_t>(f) + i] = r[i];
@@ -1420,15 +1495,33 @@ __global__ void __launch_bounds__(kEvalThreads) manifold_eval_kernel(ManifoldArg
         m3_mul(A, D, AD);
         m3_mul(H, D, HD);
         const double wm = lam[m] - lam[m + 1];
+        if constexpr (WT) {
+          double blk[36];
 #pragma unroll
-        for (int i = 0; i < 3; ++i)
+          for (int i = 0; i < 3; ++i)
 #pragma unroll
-          for (int c = 0; c < 3; ++c) {
-            out[i * 6 * K + 6 * m + c] = AD[3 * i + c];
-            out[i * 6 * K + 6 * m + 3 + c] = 0.0;
-            out[(3 + i) * 6 * K + 6 * m + c] = -HD[3 * i + c];
-            out[(3 + i) * 6 * K + 6 * m + 3 + c] = (i == c) ? wm : 0.0;
-          }
+            for (int c = 0; c < 3; ++c) {
+              blk[6 * i + c] = AD[3 * i + c];
+              blk[6 * i + 3 + c] = 0.0;
+              blk[6 * (3 + i) + c] = -HD[3 * i + c];
+              blk[6 * (3 + i) + 3 + c] = (i == c) ? wm : 0.0;
+            }
+          weigh_rows<6, 6>(wt + kWtManifold, blk);
+#pragma unroll
+          for (int i = 0; i < 6; ++i)
+#pragma unroll
+            for (int c = 0; c < 6; ++c) out[i * 6 * K + 6 * m + c] = blk[6 * i + c];
+        } else {
+#pragma unroll
+          for (int i = 0; i < 3; ++i)
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+              out[i * 6 * K + 6 * m + c] = AD[3 * i + c];
+              out[i * 6 * K + 6 * m + 3 + c] = 0.0;
+              out[(3 + i) * 6 * K + 6 * m + c] = -HD[3 * i + c];
+              out[(3 + i) * 6 * K + 6 * m + 3 + c] = (i == c) ? wm : 0.0;
+            }
+        }
       }
     }
   }

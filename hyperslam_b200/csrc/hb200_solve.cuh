@@ -266,6 +266,10 @@ __global__ void __launch_bounds__(kHessThreads) inertial_hessian_kernel(const in
 // are zero except one entry per row, written once per chunk; the zero pattern of the product (gyro-bias x accel-bias,
 // bias components c != c') is skipped at the flush.  k-step-outer loop as in the fused pixel J^T J: the NT column
 // fragments of a step are loaded once and feed every tile the warp owns.
+// WT (an inertial weight matrix W is set): the bias Jacobian is W [w_g[m] I3 ; 0] / W [0 ; w_a[m] I3], so the bias
+// columns are dense -- gyro column 3m+c = w_g[m] W[:, c], accel column 3m+c = w_a[m] W[:, 3+c] over all six rows --
+// and the product has no zero pattern: every entry is flushed, the gyro-accel coupling included.  The scalar kernel
+// above relies on the unweighted structure, so a set inertial matrix always selects this one (inertial_splits).
 // ---------------------------------------------------------------------------------------------
 template <int K, int KB>
 struct ImuHess {
@@ -301,10 +305,10 @@ template <int K, int KB>
 __host__ __device__ constexpr int imu_hess_mma_det_writes() { return 4 * ImuHess<K, KB>::PER_WARP; }
 
 // CH: factors per chunk (static shared memory: 6 CH rows of pitch 60 / 68 doubles, <= 48 KB -> 16 / 12 at most)
-template <int K, int KB, int CH, bool DET>
+template <int K, int KB, int CH, bool DET, bool WT>
 HB_DI void inertial_hessian_mma_body(const int* __restrict__ run_off, const int4* __restrict__ idx, const double* __restrict__ r, const double* __restrict__ Jp,
                                      const double* __restrict__ wg, const double* __restrict__ wa, const double* __restrict__ Jg, double loss_scale, double* sys,
-                                     SysLayout lay, int o_bg, int o_ba, int o_g, int splits, const DetOut& det) {
+                                     SysLayout lay, int o_bg, int o_ba, int o_g, int splits, const DetOut& det, const double* __restrict__ wt) {
   using H = ImuHess<K, KB>;
   constexpr int NP = H::NP, NBG = H::NBG, NA = H::NA, NT = H::NT, NTL = H::NTL, LD = ImuHessLD<K, KB>::value;
   static_assert(LD >= 8 * NT && (LD % 16 == 4 || LD % 16 == 12), "row pitch: conflict-free fragment loads");
@@ -334,10 +338,18 @@ HB_DI void inertial_hessian_mma_body(const int* __restrict__ run_off, const int4
         sJ[row * LD + col] = v.x; sJ[row * LD + col + 1] = v.y;
       }
     }
-    for (int e = tid; e < cnt * KB * 3; e += kHessThreads) {   // bias entries: factor ff, knot m, component c
-      const int ff = e / (KB * 3), rem = e - ff * KB * 3, m = rem / 3, c = rem - 3 * m;
-      sJ[(6 * ff + c) * LD + NP + 3 * m + c] = wg[static_cast<size_t>(f0 + ff) * KB + m];
-      sJ[(6 * ff + 3 + c) * LD + NP + NBG + 3 * m + c] = wa[static_cast<size_t>(f0 + ff) * KB + m];
+    if constexpr (WT) {
+      for (int e = tid; e < cnt * KB * 18; e += kHessThreads) {   // bias columns: factor ff, knot m, component c, row
+        const int ff = e / (KB * 18), rem = e - ff * KB * 18, m = rem / 18, rc = rem - 18 * m, c = rc / 6, row = rc - 6 * c;
+        sJ[(6 * ff + row) * LD + NP + 3 * m + c] = wg[static_cast<size_t>(f0 + ff) * KB + m] * wt[kWtInertial + 6 * row + c];
+        sJ[(6 * ff + row) * LD + NP + NBG + 3 * m + c] = wa[static_cast<size_t>(f0 + ff) * KB + m] * wt[kWtInertial + 6 * row + 3 + c];
+      }
+    } else {
+      for (int e = tid; e < cnt * KB * 3; e += kHessThreads) {   // bias entries: factor ff, knot m, component c
+        const int ff = e / (KB * 3), rem = e - ff * KB * 3, m = rem / 3, c = rem - 3 * m;
+        sJ[(6 * ff + c) * LD + NP + 3 * m + c] = wg[static_cast<size_t>(f0 + ff) * KB + m];
+        sJ[(6 * ff + 3 + c) * LD + NP + NBG + 3 * m + c] = wa[static_cast<size_t>(f0 + ff) * KB + m];
+      }
     }
     for (int e = tid; e < cnt * 12; e += kHessThreads) {       // gravity: Jg[ff][row][gm]
       const int ff = e / 12, rem = e - 12 * ff, row = rem >> 1, gm = rem & 1;
@@ -369,9 +381,11 @@ HB_DI void inertial_hessian_mma_body(const int* __restrict__ run_off, const int4
       if (b < NA - 1) add(gv + dof(b), ls * v);
       return;
     }
-    if (a >= NP && a < NP + 2 * NBG && b >= NP) {   // bias x bias: only equal components of the same sensor
-      if ((a >= NP + NBG) != (b >= NP + NBG)) return;
-      if ((a - NP) % 3 != (b - NP) % 3) return;
+    if constexpr (!WT) {
+      if (a >= NP && a < NP + 2 * NBG && b >= NP) {   // bias x bias: only equal components of the same sensor
+        if ((a >= NP + NBG) != (b >= NP + NBG)) return;
+        if ((a - NP) % 3 != (b - NP) % 3) return;
+      }
     }
     const int da = dof(a), db = dof(b);
     add(sys_index(lay, da, db), ls * v);
@@ -388,14 +402,15 @@ HB_DI void inertial_hessian_mma_body(const int* __restrict__ run_off, const int4
     }
   }
 }
-// DET: slot = CTA
-template <int K, int KB, int CH, bool DET>
+// DET: slot = CTA; WT: wt is the context's weight table
+template <int K, int KB, int CH, bool DET, bool WT>
 __global__ void __launch_bounds__(kHessThreads) inertial_hessian_mma_kernel(const int* __restrict__ run_off, const int4* __restrict__ idx,
                                                                             const double* __restrict__ r, const double* __restrict__ Jp,
                                                                             const double* __restrict__ wg, const double* __restrict__ wa,
                                                                             const double* __restrict__ Jg, double loss_scale, double* sys,
-                                                                            SysLayout lay, int o_bg, int o_ba, int o_g, int splits, DetOut det) {
-  inertial_hessian_mma_body<K, KB, CH, DET>(run_off, idx, r, Jp, wg, wa, Jg, loss_scale, sys, lay, o_bg, o_ba, o_g, splits, det);
+                                                                            SysLayout lay, int o_bg, int o_ba, int o_g, int splits, DetOut det,
+                                                                            const double* __restrict__ wt) {
+  inertial_hessian_mma_body<K, KB, CH, DET, WT>(run_off, idx, r, Jp, wg, wa, Jg, loss_scale, sys, lay, o_bg, o_ba, o_g, splits, det, wt);
 }
 
 // J^T J / J^T r of the manifold (pose) factors: one warp per factor, lower triangle of its 6K x 6K block.

@@ -97,6 +97,11 @@ class Optimizer {   // OptimizerSuite::H100
   // problem is solved again on the same GPU model with the same build, as the reference's single-threaded solve does
   // (reference optimizer.cpp:38-54).  Off by default.
   void setDeterministic(bool deterministic);
+  // CostConfiguration::weights of one family (reference exteroceptive.cpp:101-178), one matrix per family as the reference's
+  // per-family configuration: row-major d x d with d = 2 (pixel), 1 (bearing), 6 (inertial, pose); empty clears it (the
+  // reference's weights = nullptr, the default).  ExteroceptiveCost::Evaluate then returns W r and W J for every block
+  // (hb200_set_weights); the losses see W r.
+  void setWeights(ExteroceptiveCost::Kind kind, const std::vector<double>& weights);
   // summary.termination_type of the last optimize(): 0 iteration limit, 1 function, 2 parameter, 3 gradient tolerance, 4 radius, 5 invalid steps
   int terminationType() const;
 

@@ -209,6 +209,14 @@ void Optimizer::setSolverTolerances(double function_tolerance, double gradient_t
   check(hb200_set_termination(ctx_, function_tolerance, gradient_tolerance, parameter_tolerance, min_trust_region_radius), "hb200_set_termination");
 }
 void Optimizer::setDeterministic(bool deterministic) { check(hb200_set_deterministic(ctx_, deterministic ? 1 : 0), "hb200_set_deterministic"); }
+void Optimizer::setWeights(ExteroceptiveCost::Kind kind, const std::vector<double>& weights) {
+  static constexpr size_t kSide[] = {2, 6, 1, 6};   // indexed by ExteroceptiveCost::Kind (== HB200_PIXEL ...)
+  const int k = static_cast<int>(kind);
+  if (k < 0 || k > 3) throw std::invalid_argument("setWeights: unknown factor kind " + std::to_string(k));
+  const size_t d = kSide[k];
+  if (!weights.empty() && weights.size() != d * d) throw std::invalid_argument("setWeights: the matrix of this family is " + std::to_string(d) + " x " + std::to_string(d));
+  check(hb200_set_weights(ctx_, static_cast<int>(kind), weights.empty() ? nullptr : weights.data()), "hb200_set_weights");
+}
 int Optimizer::terminationType() const {
   int type = 0;
   hb200_get_termination(ctx_, &type, nullptr, nullptr, nullptr, nullptr);

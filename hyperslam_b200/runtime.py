@@ -72,7 +72,7 @@ EXPORTS = [
     "hb200_factor_counts", "hb200_build_covariance", "hb200_compute_covariance", "hb200_get_covariance", "hb200_interpolate_covariance",
     "hb200_append_bias_knots", "hb200_bias_knots", "hb200_set_deterministic", "hb200_get_deterministic",
     "hb200_interpolate_state_covariance", "hb200_set_covariance_blocks", "hb200_get_covariance_blocks",
-    "hb200_set_covariance_stamp_pairs", "hb200_get_pose_pair_covariance",
+    "hb200_set_covariance_stamp_pairs", "hb200_get_pose_pair_covariance", "hb200_set_weights",
 ]
 
 _lib = None
@@ -177,6 +177,20 @@ class Context:
     def set_options(self, huber_pixel=0.5, imu_loss_scale=1.6e-5, radius=1e4):
         self._check(self.lib.hb200_set_options(self.h, C.c_double(huber_pixel), C.c_double(imu_loss_scale), C.c_double(radius)))
 
+    WEIGHT_SIDES = {PIXEL: 2, INERTIAL: 6, BEARING: 1, MANIFOLD: 6}
+
+    def set_weights(self, kind: int, W=None):
+        """Family weight matrix (hb200_set_weights): residual W r and Jacobians W J for every factor of `kind`;
+        W is (d, d) with d = WEIGHT_SIDES[kind], None clears it."""
+        if W is None:
+            self._check(self.lib.hb200_set_weights(self.h, int(kind), None))
+            return
+        W = _f64(W)
+        d = self.WEIGHT_SIDES.get(int(kind))
+        if d is None or W.size != d * d:
+            raise ValueError(f"weight matrix of kind {kind} must be {d} x {d}, got shape {W.shape}")
+        self._check(self.lib.hb200_set_weights(self.h, int(kind), _d(W.reshape(d, d))))
+
     def set_reference_quirks(self, quirks: int):
         self._check(self.lib.hb200_set_reference_quirks(self.h, int(quirks)))
 
@@ -232,6 +246,8 @@ class Context:
         self.set_manifold_factors(w.m_stamp, w.m_sensor, w.m_pose)
         self.bind()
         self.set_constant(w.knot_const, w.gravity_const, w.bias_const)
+        for kind, W in (w.weights or {}).items():
+            self.set_weights(kind, W)
 
     # ---- device-side sliding-window bookkeeping ------------------------------------------------------
     def _refresh_sizes(self):

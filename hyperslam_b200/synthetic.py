@@ -67,6 +67,9 @@ class Window:
     m_stamp: np.ndarray = dataclasses.field(default_factory=lambda: np.zeros(0))
     m_sensor: np.ndarray = dataclasses.field(default_factory=lambda: np.zeros(0, dtype=np.int32))
     m_pose: np.ndarray = dataclasses.field(default_factory=lambda: np.zeros((0, 7)))         # (Nm, 7) measured T_ws
+    # family weight matrices (CostConfiguration::weights, reference exteroceptive.cpp:162-178): {kind: (d, d) array} with
+    # kind runtime.PIXEL (2x2) / BEARING (1x1) / INERTIAL (6x6) / MANIFOLD (6x6); None (the reference default) sets none
+    weights: dict | None = None
 
     @property
     def num_factors(self) -> int:

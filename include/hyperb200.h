@@ -75,6 +75,22 @@ int hb200_set_constant(hb200_ctx* ctx, const unsigned char* knot_constant, int g
 /* losses: HuberLoss(huber_pixel) (reference optimizer.cpp:226), ScaledLoss(NULL, imu_loss_scale)
  * (:267-268); radius = initial trust-region radius (Ceres default 1e4). */
 int hb200_set_options(hb200_ctx* ctx, double huber_pixel, double imu_loss_scale, double radius);
+/* Family weight matrix: the weights branch of ExteroceptiveCost::Evaluate (reference exteroceptive.cpp:101-160), set in
+ * place of CostConfiguration::weights (:162-178), one matrix per family as the reference's per-family configuration
+ * (optimizer.cpp:191,214,236,255).  Wf is row-major d x d: d = 2 for HB200_PIXEL, 1 for HB200_BEARING (the one angular
+ * row), 6 for HB200_INERTIAL (rows gyro | accel) and HB200_MANIFOLD (rows [theta | p]); any finite matrix is accepted (it
+ * need not be triangular or positive definite; a singular one shows up as a failed covariance or a damped LM step).
+ * NULL clears the family's matrix, which is the default (the reference's weights = nullptr): without a matrix every
+ * output is what it is without this call, bit for bit.  With one, each factor of the family has residual Wf r and every
+ * Jacobian block Wf J; the loss sees the weighted residual (Huber on |Wf r|^2, ScaledLoss times |Wf r|^2), and the cost,
+ * J^T J, the Schur complement, the LM step and the covariances all follow from the weighted r and J.  So the copy-outs
+ * (hb200_get_*_outputs, hb200_factor_evaluate, calibration blocks included) return weighted residuals and Jacobians --
+ * except the inertial wg / wa outputs, which stay the bias splines' basis weights: with a matrix set the bias Jacobian
+ * of gyro knot m is wg[m] Wf[:, 0:3] and that of accel knot m is wa[m] Wf[:, 3:6] (without one, wg[m] [I3 ; 0] and
+ * wa[m] [0 ; I3]).  Returns -1 for an unknown kind or a non-finite entry (nothing changes).  Setting the value a family
+ * already has changes nothing; a change drops a built system and a pending covariance build (-2 until rebuilt), like
+ * every setter, and the next iteration is captured again with the new matrix. */
+int hb200_set_weights(hb200_ctx* ctx, int kind, const double* Wf);
 
 /* HYPER_REFERENCE_QUIRKS (SURVEY.md section 8a): 0 (default) = the mathematically consistent inertial Jacobians;
  * bits switch on the in-tree formulas verbatim -- 1: gyroscope intrinsics in the accelerometer rows (reference
@@ -195,7 +211,7 @@ int hb200_get_bearing_outputs(hb200_ctx* ctx, double* r, double* Jp, double* Jl)
 int hb200_get_manifold_outputs(hb200_ctx* ctx, double* r, double* Jp);
 /* Ceres-shaped copy-out of one factor after hb200_evaluate(JACOBIANS): same signature, block order
  * and row-major ambient Jacobians as ExteroceptiveCost::Evaluate (reference exteroceptive.hpp:31,
- * exteroceptive.cpp:149-156).  parameters must be the blocks the window was uploaded from.  Every block is served,
+ * exteroceptive.cpp:149-156), weighted by the family's matrix when one is set (hb200_set_weights).  parameters must be the blocks the window was uploaded from.  Every block is served,
  * the calibration blocks too (extrinsics, intrinsics, distortion; i_g, i_a, S_g, X_a -- reference pixel.cpp:91-135,141,
  * inertial.cpp:155-194): they are constant in the live configuration (optimizer.cpp:59-63), so their Jacobians are
  * computed by separate kernels the first time one is requested after an evaluation, not on the iteration path. */
@@ -212,7 +228,8 @@ int hb200_solve(hb200_ctx* ctx);
 int hb200_get_delta(hb200_ctx* ctx, double* delta_pose /* n */, double* delta_landmark /* 3L */);
 /* ---- marginal covariances: the replacement of ceres::Covariance (default options: apply_loss_function, constant
  * blocks get zero covariance) -----------------------------------------------------------------------------------------
- * Sigma = (J^T W J)^-1 over the non-constant dofs at the current state, W the loss weights of the LM build (Huber rho' of
+ * Sigma = (J^T W J)^-1 over the non-constant dofs at the current state, J the Jacobian of the (family-matrix weighted,
+ * hb200_set_weights) residuals, W the loss weights of the LM build (Huber rho' of
  * pixel / bearing factors, the inertial ScaledLoss, none for pose factors), no damping anywhere (mu = 0, also inside the
  * landmark elimination).  Constant knots, bias_const and gravity_const dofs get exact zeros.  Tangent convention of the
  * device: rotation global (R <- Exp(theta) R), SE3 split [theta | rho] with p <- p + rho, gravity the 2-dof sphere tangent.
@@ -397,7 +414,8 @@ int hb200_ingest_stereo(hb200_ctx* ctx, int n, const double* stamp, const int* c
  *     complements) and only the owner updates the landmark, so non-owned landmarks of a replica are stale;
  *     read each landmark back from its owner.
  *   - inertial and manifold factors may be split arbitrarily; every factor lives on exactly one rank.
- *   - knots, bias splines, gravity, calibration, constancy flags and options must be identical on all ranks,
+ *   - knots, bias splines, gravity, calibration, constancy flags, options and family weight matrices
+ *     (hb200_set_weights: replicated configuration, no collective step) must be identical on all ranks,
  *     and every rank must make the same sequence of hb200_iterate / hb200_optimize / hb200_build_system /
  *     hb200_build_covariance / hb200_compute_covariance calls.  The covariance build takes one system reduction
  *     (like hb200_build_system) and leaves the LM's trust-region state alone; the compute has no collective step.
