@@ -9,6 +9,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <initializer_list>
 #include <numeric>
 #include <string>
 #include <type_traits>
@@ -76,6 +77,37 @@ struct DevBuf {
   DevBuf(const DevBuf&) = delete;
   DevBuf& operator=(const DevBuf&) = delete;
   ~DevBuf() { release(); }   // scratch buffers of the API calls do not leak on early error returns
+};
+
+// The first failure of a series of calls, all of which run.
+cudaError_t first_error(std::initializer_list<cudaError_t> es) {
+  for (cudaError_t e : es) if (e != cudaSuccess) return e;
+  return cudaSuccess;
+}
+
+// The factor lists on the device, one buffer per field.  grow: capacity for n factors, the first `keep` preserved
+// (DevBuf::grow on every field); swap: switch with another copy of the list.
+struct VisualList {
+  DevBuf<double> stamp, z;   // z: a bearing's third component (x, y are in `pixel`)
+  DevBuf<double2> pixel;
+  DevBuf<int4> idx;
+  cudaError_t grow(size_t n, size_t keep, cudaStream_t s) { return first_error({stamp.grow(n, keep, s), z.grow(n, keep, s), pixel.grow(n, keep, s), idx.grow(n, keep, s)}); }
+  void swap(VisualList& o) { stamp.swap(o.stamp); z.swap(o.z); pixel.swap(o.pixel); idx.swap(o.idx); }
+};
+struct InertialList {
+  DevBuf<double> stamp, meas;   // meas: [gyro | accel] per factor
+  DevBuf<int4> idx;
+  cudaError_t grow(size_t n, size_t keep, cudaStream_t s) { return first_error({stamp.grow(n, keep, s), meas.grow(6 * n, 6 * keep, s), idx.grow(n, keep, s)}); }
+  void swap(InertialList& o) { stamp.swap(o.stamp); meas.swap(o.meas); idx.swap(o.idx); }
+};
+struct ManifoldList {
+  DevBuf<double> stamp, meas;   // meas: a pose [7] per factor
+  DevBuf<int> sensor;
+  DevBuf<int2> idx;
+  cudaError_t grow(size_t n, size_t keep, cudaStream_t s) {
+    return first_error({stamp.grow(n, keep, s), meas.grow(7 * n, 7 * keep, s), sensor.grow(n, keep, s), idx.grow(n, keep, s)});
+  }
+  void swap(ManifoldList& o) { stamp.swap(o.stamp); meas.swap(o.meas); sensor.swap(o.sensor); idx.swap(o.idx); }
 };
 
 void compute_basis(Basis* b, int k) {
@@ -190,14 +222,16 @@ struct hb200_ctx {
 
   // factor lists, on the device only (the setters write them in user order, hb200_bind sorts them into bound order):
   // the visual list holds pixel and bearing factors (kind flag in idx.w), which travel through the same kernels and the
-  // same compact layout; inertial and manifold (pose) factors have their own lists.
+  // same compact layout; inertial and manifold (pose) factors have their own lists.  A compaction writes a list's spare
+  // copy and switches it in.  Spares grow as the live lists do, since the next append grows what was the spare, and
+  // hold at least one factor, as every list.
   int Nv = 0, Ni = 0, Np = 0, Nb = 0, Nm = 0, P = 0;
   std::vector<double> h_sensors;
-  DevBuf<double> v_stamp, v_pixel, v_z, v_w, i_stamp, i_meas, m_stamp, m_meas, sensors;
-  DevBuf<int> m_sensor;
-  DevBuf<int2> m_idx;
+  VisualList visual, visual_spare;
+  InertialList inertial, inertial_spare;
+  ManifoldList manifold, manifold_spare;
+  DevBuf<double> v_w, sensors;
   double huber_bearing = 1.6e-3;   // reference optimizer.cpp:204
-  DevBuf<int4> v_idx, i_idx;
   // list position -> user index (visual: pixel factors 0 .. Np-1, bearing factors Np .. Nv-1); appends and slides clear
   // them, ensure_perms rebuilds them
   std::vector<int> v_perm, i_perm;
@@ -226,14 +260,9 @@ struct hb200_ctx {
   DevBuf<long long> band_dbg;   // optional phase timings of band_solve_kernel (HB200_BAND_TIMING=1)
   bool bound = false;
 
-  // device-side window bookkeeping (hb200_append_* / hb200_slide) and the compactions / permutations of the factor lists
-  DevBuf<double> alt_stamp, alt_meas, alt_z, alt_lms, alt_knots;
-  DevBuf<double2> alt_pixel;
-  DevBuf<int4> alt_idx;
-  DevBuf<int2> alt_midx;
-  DevBuf<int> alt_sensor;
-  // w_lkeep / w_lpos: landmark keep flags and new positions of the last hb200_slide (slide_L landmarks before it; -1:
-  // none yet), kept until the next slide for hb200_slide_landmark_map
+  // device-side window bookkeeping (hb200_append_* / hb200_slide).  w_lkeep / w_lpos: landmark keep flags and new
+  // positions of the last hb200_slide (slide_L landmarks before it; -1: none yet), kept until the next slide for
+  // hb200_slide_landmark_map
   DevBuf<int> w_keep, w_pos, w_lkeep, w_lpos, w_cnt, w_scal;
   DevBuf<double> w_vote;   // sharded contexts: the agreement payload of a collective sliding-window call (agree_round)
   int slide_L = -1;
@@ -376,7 +405,8 @@ struct hb200_ctx {
   void kernel_args_changed() { outputs_changed(); graph_valid = false; det_ready = false; }
 
   // The variable blocks in their canonical order (knots, gyroscope bias, accelerometer bias, gravity, landmarks): the
-  // current state, the trial state, the snapshot and the block's length in doubles.
+  // current state, the trial state, the snapshot and the block's length in doubles.  Every LM step rewrites the whole
+  // trial state before reading it, so hb200_slide compacts the current state into the trial copy and switches the two.
   struct StateBlock { DevBuf<double>* cur; DevBuf<double>* trial; DevBuf<double>* snap; size_t count; };
   std::array<StateBlock, 5> state_blocks() {
     return {{{&knots[0], &knots[1], &snap[0], 8 * static_cast<size_t>(K)},
@@ -580,7 +610,7 @@ template <bool J>
 PixelArgs pixel_args(hb200_ctx* c, int sel, double* sys) {
   PixelArgs a{};
   a.sys = sys; a.lay = c->lay; a.tiles_per_cta = 1;
-  a.n = c->Nv; a.stamp = c->v_stamp.p; a.pixel = reinterpret_cast<const double2*>(c->v_pixel.p); a.meas_z = c->v_z.p; a.idx = c->v_idx.p;
+  a.n = c->Nv; a.stamp = c->visual.stamp.p; a.pixel = c->visual.pixel.p; a.meas_z = c->visual.z.p; a.idx = c->visual.idx.p;
   a.tab = c->tab[sel].p; a.cam_tab = c->cam_tab.p; a.landmarks = c->lms[sel].p;
   a.r = J ? c->v_r.p : nullptr; a.Jp = c->v_Jp.p; a.Jl = c->v_Jl.p; a.w = c->v_w.p; a.cost_partial = c->cp_pix[J ? 0 : 1].p; a.huber = c->huber; a.huber_bearing = c->huber_bearing; a.K_knots = c->K;
   return a;
@@ -588,7 +618,7 @@ PixelArgs pixel_args(hb200_ctx* c, int sel, double* sys) {
 template <bool J>
 InertialArgs inertial_args(hb200_ctx* c, int sel) {
   InertialArgs a{};
-  a.n = c->Ni; a.stamp = c->i_stamp.p; a.meas = c->i_meas.p; a.idx = c->i_idx.p; a.tab = c->tab[sel].p; a.imu_tab = c->imu_tab.p;
+  a.n = c->Ni; a.stamp = c->inertial.stamp.p; a.meas = c->inertial.meas.p; a.idx = c->inertial.idx.p; a.tab = c->tab[sel].p; a.imu_tab = c->imu_tab.p;
   a.bg = c->bg[sel].p; a.ba = c->ba[sel].p; a.gravity = c->grav[sel].p;
   a.r = J ? c->i_r.p : nullptr; a.Jp = c->i_Jp.p; a.wg = c->i_wg.p; a.wa = c->i_wa.p; a.Jg = c->i_Jg.p;
   a.cost_partial = c->cp_imu[J ? 0 : 1].p; a.loss_scale = c->imu_scale;
@@ -642,7 +672,7 @@ template <int K, bool J>
 int launch_manifold(hb200_ctx* c, int sel) {
   if (c->Nm == 0) return 0;
   ManifoldArgs a{};
-  a.n = c->Nm; a.stamp = c->m_stamp.p; a.meas = c->m_meas.p; a.idx = c->m_idx.p; a.tab = c->tab[sel].p; a.sensors = c->sensors.p;
+  a.n = c->Nm; a.stamp = c->manifold.stamp.p; a.meas = c->manifold.meas.p; a.idx = c->manifold.idx.p; a.tab = c->tab[sel].p; a.sensors = c->sensors.p;
   a.r = J ? c->m_r.p : nullptr; a.Jp = c->m_Jp.p; a.cost_partial = c->cp_imu[J ? 0 : 1].p + c->n_imu_blocks;
   return with_flag(c->wt_set[HB200_MANIFOLD], [&](auto WT) {
     manifold_eval_kernel<K, J, WT><<<c->n_man_blocks, kEvalThreads, 0, side(c)>>>(a, c->basis, c->wt.p);
@@ -724,14 +754,14 @@ int enqueue_build(hb200_ctx* c, const SolverState* st) {
       return with_flag(det, [&](auto DET) {
         const DetOut d = DET ? c->det_imu : DetOut{};
         if (scalar_hess)
-          inertial_hessian_kernel<K, 4, DET><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->i_idx.p, c->i_r.p, c->i_Jp.p, c->i_wg.p, c->i_wa.p, c->i_Jg.p,
+          inertial_hessian_kernel<K, 4, DET><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->inertial.idx.p, c->i_r.p, c->i_Jp.p, c->i_wg.p, c->i_wa.p, c->i_Jg.p,
                                                                                  c->imu_scale, c->assembly(), c->lay, c->o_bg(), c->o_ba(), c->o_g(), splits, d);
         else if (c->wt_set[HB200_INERTIAL])
-          inertial_hessian_mma_kernel<K, 4, K == 4 ? 8 : 12, DET, true><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->i_idx.p, c->i_r.p, c->i_Jp.p, c->i_wg.p,
+          inertial_hessian_mma_kernel<K, 4, K == 4 ? 8 : 12, DET, true><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->inertial.idx.p, c->i_r.p, c->i_Jp.p, c->i_wg.p,
                                                                                                            c->i_wa.p, c->i_Jg.p, c->imu_scale, c->assembly(), c->lay,
                                                                                                            c->o_bg(), c->o_ba(), c->o_g(), splits, d, c->wt.p);
         else
-          inertial_hessian_mma_kernel<K, 4, K == 4 ? 8 : 12, DET, false><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->i_idx.p, c->i_r.p, c->i_Jp.p, c->i_wg.p, c->i_wa.p,
+          inertial_hessian_mma_kernel<K, 4, K == 4 ? 8 : 12, DET, false><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->inertial.idx.p, c->i_r.p, c->i_Jp.p, c->i_wg.p, c->i_wa.p,
                                                                                                             c->i_Jg.p, c->imu_scale, c->assembly(), c->lay, c->o_bg(), c->o_ba(),
                                                                                                             c->o_g(), splits, d, nullptr);
         return check_launch(c, scalar_hess ? (DET ? "inertial_hessian_det_kernel" : "inertial_hessian_kernel")
@@ -744,7 +774,7 @@ int enqueue_build(hb200_ctx* c, const SolverState* st) {
     const int blocks = (c->Nm + kManWarps - 1) / kManWarps;
     const int rc = with_order(c->k, [&](auto K) {
       return with_flag(det, [&](auto DET) {
-        manifold_hessian_kernel<K, DET><<<blocks, kManWarps * 32, 0, side(c)>>>(c->Nm, c->m_idx.p, c->m_r.p, c->m_Jp.p, c->assembly(), c->lay,
+        manifold_hessian_kernel<K, DET><<<blocks, kManWarps * 32, 0, side(c)>>>(c->Nm, c->manifold.idx.p, c->m_r.p, c->m_Jp.p, c->assembly(), c->lay,
                                                                                DET ? c->det_man : DetOut{});
         return check_launch(c, DET ? "manifold_hessian_det_kernel" : "manifold_hessian_kernel");
       });
@@ -761,7 +791,7 @@ int enqueue_build(hb200_ctx* c, const SolverState* st) {
     const size_t smem = (3 * static_cast<size_t>(kSchurGroup) * (c->schur_rt + 1) + 3 * kSchurGroup + 4 * 3 * static_cast<size_t>(c->schur_rt)) * sizeof(double);
     const int rc = with_order(c->k, [&](auto K) {
       return with_flag(det, [&](auto DET) {
-        schur_group_kernel<K, DET><<<c->n_lm_groups, kSchurGThreads, smem, c->stream>>>(c->lm_group_off.p, c->lm_order.p, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p,
+        schur_group_kernel<K, DET><<<c->n_lm_groups, kSchurGThreads, smem, c->stream>>>(c->lm_group_off.p, c->lm_order.p, c->lm_off.p, c->lm_obs.p, c->visual.idx.p, c->v_r.p,
                                                                                         c->v_Jp.p, c->v_Jl.p, c->v_w.p, st, c->assembly(), c->lay, c->Vchol.p, c->gl.p,
                                                                                         c->Dl.p, c->schur_rt, DET ? c->det_schur : DetOut{});
         return check_launch(c, DET ? "schur_group_det_kernel" : "schur_group_kernel");
@@ -772,7 +802,7 @@ int enqueue_build(hb200_ctx* c, const SolverState* st) {
     const size_t smem = 2 * 3 * static_cast<size_t>(c->max_rows) * sizeof(double);
     const int rc = with_order(c->k, [&](auto K) {
       return with_flag(det, [&](auto DET) {
-        schur_kernel<K, DET><<<c->L, kSchurThreads, smem, c->stream>>>(c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p, st,
+        schur_kernel<K, DET><<<c->L, kSchurThreads, smem, c->stream>>>(c->lm_off.p, c->lm_obs.p, c->visual.idx.p, c->v_r.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p, st,
                                                                        c->assembly(), c->lay, c->Vchol.p, c->gl.p, c->Dl.p, c->max_rows, DET ? c->det_schur : DetOut{});
         return check_launch(c, DET ? "schur_det_kernel" : "schur_kernel");
       });
@@ -821,7 +851,7 @@ int prepare_det(hb200_ctx* c) {
       HB_CUDA(c->det_seg_off.ensure(2 * (static_cast<size_t>(tiles) + 1)));   // offsets | counts
       int* counts = c->det_seg_off.p + tiles + 1;
       HB_CUDA(cudaMemsetAsync(counts, 0, sizeof(int) * (static_cast<size_t>(tiles) + 1), c->stream));
-      det_pixel_segments_kernel<<<(tiles + 127) / 128, 128, 0, c->stream>>>(c->Nv, c->v_idx.p, counts);
+      det_pixel_segments_kernel<<<(tiles + 127) / 128, 128, 0, c->stream>>>(c->Nv, c->visual.idx.p, counts);
       HB_LAUNCH(c, "det_pixel_segments_kernel");
       HB_CUDA(c->w_scal.ensure(8));
       scan_kernel<<<1, 1024, 0, c->stream>>>(counts, tiles + 1, c->det_seg_off.p, c->w_scal.p);
@@ -918,7 +948,7 @@ int enqueue_solve(hb200_ctx* c, bool fuse_retract = false, bool* fused = nullptr
         if (fused) *fused = true;
       }
       const int rc = with_order(c->k, [&](auto K) {
-        lm_backsub_kernel<K><<<c->n_lm_blocks + extra, kLmWarps * 32, 0, c->stream>>>(c->L, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_r.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p,
+        lm_backsub_kernel<K><<<c->n_lm_blocks + extra, kLmWarps * 32, 0, c->stream>>>(c->L, c->lm_off.p, c->lm_obs.p, c->visual.idx.p, c->v_r.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p,
                                                                                  c->Vchol.p, c->gl.p, c->Dl.p, c->dp.p, c->dl.p, c->lm_part.p, c->lms[0].p, c->lms[1].p, c->n_lm_blocks, ra);
         return check_launch(c, "lm_backsub_kernel");
       });
@@ -1144,10 +1174,9 @@ int ensure_placeholders(hb200_ctx* c) {
     HB_CUDA(c->cp_pix[s].ensure(1)); HB_CUDA(c->cp_imu[s].ensure(1));
   }
   HB_CUDA(c->imu_tab.ensure(kImuStride)); HB_CUDA(c->cam_tab.ensure(kCamStride));
-  HB_CUDA(c->v_z.ensure(1)); HB_CUDA(c->v_w.ensure(1)); HB_CUDA(c->sensors.ensure(7)); HB_CUDA(c->m_idx.ensure(1));
-  HB_CUDA(c->v_stamp.ensure(1)); HB_CUDA(c->v_pixel.ensure(2)); HB_CUDA(c->v_idx.ensure(1));
-  HB_CUDA(c->i_stamp.ensure(1)); HB_CUDA(c->i_meas.ensure(6)); HB_CUDA(c->i_idx.ensure(1));
-  HB_CUDA(c->m_stamp.ensure(1)); HB_CUDA(c->m_meas.ensure(7)); HB_CUDA(c->m_sensor.ensure(1));
+  HB_CUDA(c->v_w.ensure(1)); HB_CUDA(c->sensors.ensure(7));
+  HB_CUDA(c->visual.grow(1, 0, c->stream)); HB_CUDA(c->inertial.grow(1, 0, c->stream)); HB_CUDA(c->manifold.grow(1, 0, c->stream));
+  HB_CUDA(c->visual_spare.grow(1, 0, c->stream)); HB_CUDA(c->inertial_spare.grow(1, 0, c->stream)); HB_CUDA(c->manifold_spare.grow(1, 0, c->stream));
   return 0;
 }
 
@@ -1397,20 +1426,12 @@ int ensure_perms(hb200_ctx* c) {
   if (c->v_perm.size() != Nv) {
     std::vector<int4> id(Nv);
     HB_CUDA(cudaSetDevice(c->device));
-    HB_CUDA(cudaMemcpyAsync(id.data(), c->v_idx.p, sizeof(int4) * Nv, cudaMemcpyDeviceToHost, c->stream));
+    HB_CUDA(cudaMemcpyAsync(id.data(), c->visual.idx.p, sizeof(int4) * Nv, cudaMemcpyDeviceToHost, c->stream));
     HB_CUDA(cudaStreamSynchronize(c->stream));
     c->v_perm.resize(Nv);
     for (size_t f = 0, p = 0, b = c->Np; f < Nv; ++f) c->v_perm[f] = static_cast<int>(id[f].w == 0 ? p++ : b++);
   }
   if (c->i_perm.size() != Ni) { c->i_perm.resize(Ni); std::iota(c->i_perm.begin(), c->i_perm.end(), 0); }
-  return 0;
-}
-
-// capacity for N visual factors, the current ones preserved
-int grow_visual(hb200_ctx* c, size_t N) {
-  const size_t Nv = c->Nv;
-  HB_CUDA(c->v_stamp.grow(N, Nv, c->stream)); HB_CUDA(c->v_pixel.grow(2 * N, 2 * Nv, c->stream));
-  HB_CUDA(c->v_z.grow(N, Nv, c->stream)); HB_CUDA(c->v_idx.grow(N, Nv, c->stream));
   return 0;
 }
 
@@ -1422,40 +1443,44 @@ int upload_visual(hb200_ctx* c, int at, int n, const double* stamp, const int* c
   for (int f = 0; f < static_cast<int>(z.size()); ++f) { xy[2 * f] = meas[3 * f]; xy[2 * f + 1] = meas[3 * f + 1]; z[f] = meas[3 * f + 2]; }
   std::vector<int4> id(n);
   for (int f = 0; f < n; ++f) id[f] = make_int4(0, landmark[f], camera[f], kind);
-  HB_CUDA(cudaMemcpyAsync(c->v_stamp.p + at, stamp, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
-  HB_CUDA(cudaMemcpyAsync(c->v_pixel.p + 2 * static_cast<size_t>(at), kind ? xy.data() : meas, sizeof(double) * 2 * n, cudaMemcpyHostToDevice, c->stream));
-  if (kind) HB_CUDA(cudaMemcpyAsync(c->v_z.p + at, z.data(), sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
-  HB_CUDA(cudaMemcpyAsync(c->v_idx.p + at, id.data(), sizeof(int4) * n, cudaMemcpyHostToDevice, c->stream));
+  HB_CUDA(cudaMemcpyAsync(c->visual.stamp.p + at, stamp, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
+  HB_CUDA(cudaMemcpyAsync(c->visual.pixel.p + at, kind ? xy.data() : meas, sizeof(double2) * n, cudaMemcpyHostToDevice, c->stream));
+  if (kind) HB_CUDA(cudaMemcpyAsync(c->visual.z.p + at, z.data(), sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
+  HB_CUDA(cudaMemcpyAsync(c->visual.idx.p + at, id.data(), sizeof(int4) * n, cudaMemcpyHostToDevice, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
   return 0;
 }
 
-// Moves the visual factors with keep[f] (nullptr: all n) to positions pos[f] of the alternate buffers -- knot base less
-// knot_shift, landmark through lm_pos (nullptr: unchanged) -- and copies positions [at, at + count) back.
-int compact_visual(hb200_ctx* c, int n, const int* keep, const int* pos, const int* lm_pos, int knot_shift, int at, int count) {
-  const size_t end = std::max(at + count, 1);
-  HB_CUDA(c->alt_stamp.ensure(end)); HB_CUDA(c->alt_pixel.ensure(end)); HB_CUDA(c->alt_z.ensure(end)); HB_CUDA(c->alt_idx.ensure(end));
-  compact_visual_kernel<<<(n + 255) / 256, 256, 0, c->stream>>>(n, keep, pos, lm_pos, knot_shift, c->v_stamp.p, reinterpret_cast<const double2*>(c->v_pixel.p),
-                                                                c->v_z.p, c->v_idx.p, c->alt_stamp.p, c->alt_pixel.p, c->alt_z.p, c->alt_idx.p);
+// The compactions of the factor lists: the factors with keep[f] (nullptr: all n) move to positions pos[f] of the spare
+// list, which then replaces the live one and holds `count` factors.  Knot bases drop by the shifts, landmarks go
+// through lm_pos (nullptr: unchanged).  The switch moves the buffers the captured iteration points at.
+int compact_visual(hb200_ctx* c, int n, const int* keep, const int* pos, const int* lm_pos, int knot_shift, int count) {
+  HB_CUDA(c->visual_spare.grow(std::max(count, 1), 0, c->stream));
+  compact_visual_kernel<<<(n + 255) / 256, 256, 0, c->stream>>>(n, keep, pos, lm_pos, knot_shift, c->visual.stamp.p, c->visual.pixel.p, c->visual.z.p, c->visual.idx.p,
+                                                                c->visual_spare.stamp.p, c->visual_spare.pixel.p, c->visual_spare.z.p, c->visual_spare.idx.p);
   HB_LAUNCH(c, "compact_visual_kernel");
-  // (v_pixel is a DevBuf<double>: copy the compacted pairs back instead of swapping differently typed buffers)
-  HB_CUDA(cudaMemcpyAsync(c->v_pixel.p + 2 * static_cast<size_t>(at), c->alt_pixel.p + at, sizeof(double2) * count, cudaMemcpyDeviceToDevice, c->stream));
-  HB_CUDA(cudaMemcpyAsync(c->v_stamp.p + at, c->alt_stamp.p + at, sizeof(double) * count, cudaMemcpyDeviceToDevice, c->stream));
-  HB_CUDA(cudaMemcpyAsync(c->v_z.p + at, c->alt_z.p + at, sizeof(double) * count, cudaMemcpyDeviceToDevice, c->stream));
-  HB_CUDA(cudaMemcpyAsync(c->v_idx.p + at, c->alt_idx.p + at, sizeof(int4) * count, cudaMemcpyDeviceToDevice, c->stream));
+  c->visual.swap(c->visual_spare);
+  c->kernel_args_changed();
   return 0;
 }
 
-// The inertial counterpart of compact_visual: positions [0, count) come back, bases less the three shifts.
 int compact_inertial(hb200_ctx* c, int n, const int* keep, const int* pos, int knot_shift, int gyro_shift, int accel_shift, int count) {
-  const size_t end = std::max(count, 1);
-  HB_CUDA(c->alt_stamp.ensure(end)); HB_CUDA(c->alt_meas.ensure(6 * end)); HB_CUDA(c->alt_idx.ensure(end));
-  compact_inertial_kernel<<<(n + 255) / 256, 256, 0, c->stream>>>(n, keep, pos, knot_shift, gyro_shift, accel_shift, c->i_stamp.p, c->i_meas.p, c->i_idx.p, c->alt_stamp.p,
-                                                                  c->alt_meas.p, c->alt_idx.p);
+  HB_CUDA(c->inertial_spare.grow(std::max(count, 1), 0, c->stream));
+  compact_inertial_kernel<<<(n + 255) / 256, 256, 0, c->stream>>>(n, keep, pos, knot_shift, gyro_shift, accel_shift, c->inertial.stamp.p, c->inertial.meas.p, c->inertial.idx.p,
+                                                                  c->inertial_spare.stamp.p, c->inertial_spare.meas.p, c->inertial_spare.idx.p);
   HB_LAUNCH(c, "compact_inertial_kernel");
-  HB_CUDA(cudaMemcpyAsync(c->i_stamp.p, c->alt_stamp.p, sizeof(double) * count, cudaMemcpyDeviceToDevice, c->stream));
-  HB_CUDA(cudaMemcpyAsync(c->i_meas.p, c->alt_meas.p, sizeof(double) * 6 * count, cudaMemcpyDeviceToDevice, c->stream));
-  HB_CUDA(cudaMemcpyAsync(c->i_idx.p, c->alt_idx.p, sizeof(int4) * count, cudaMemcpyDeviceToDevice, c->stream));
+  c->inertial.swap(c->inertial_spare);
+  c->kernel_args_changed();
+  return 0;
+}
+
+int compact_manifold(hb200_ctx* c, int n, const int* keep, const int* pos, int knot_shift, int count) {
+  HB_CUDA(c->manifold_spare.grow(std::max(count, 1), 0, c->stream));
+  compact_manifold_kernel<<<(n + 255) / 256, 256, 0, c->stream>>>(n, keep, pos, knot_shift, c->manifold.stamp.p, c->manifold.meas.p, c->manifold.sensor.p, c->manifold.idx.p,
+                                                                  c->manifold_spare.stamp.p, c->manifold_spare.meas.p, c->manifold_spare.sensor.p, c->manifold_spare.idx.p);
+  HB_LAUNCH(c, "compact_manifold_kernel");
+  c->manifold.swap(c->manifold_spare);
+  c->kernel_args_changed();
   return 0;
 }
 
@@ -1467,14 +1492,14 @@ int set_visual_family(hb200_ctx* c, int kind, int n, const double* stamp, const 
   if (rc) return rc;
   const int Nv = c->Nv, Np = kind ? c->Np : n, Nb = kind ? n : c->Nb;
   const int kept = kind ? Np : Nb, kept_at = kind ? 0 : n, kept_from = kind ? 0 : c->Np;   // the other family: count, new position, old user index
-  if ((rc = grow_visual(c, Np + Nb))) return rc;
+  if (!kept) HB_CUDA(c->visual.grow(n, 0, c->stream));
   if (kept) {
     std::vector<int> keep(Nv), pos(Nv);
     for (int f = 0; f < Nv; ++f) { const int u = c->v_perm[f]; keep[f] = (u < c->Np) == (kind == 1); pos[f] = kept_at + u - kept_from; }
     HB_CUDA(c->w_keep.ensure(Nv)); HB_CUDA(c->w_pos.ensure(Nv));
     HB_CUDA(cudaMemcpyAsync(c->w_keep.p, keep.data(), sizeof(int) * Nv, cudaMemcpyHostToDevice, c->stream));
     HB_CUDA(cudaMemcpyAsync(c->w_pos.p, pos.data(), sizeof(int) * Nv, cudaMemcpyHostToDevice, c->stream));
-    if ((rc = compact_visual(c, Nv, c->w_keep.p, c->w_pos.p, nullptr, 0, kept_at, kept))) return rc;
+    if ((rc = compact_visual(c, Nv, c->w_keep.p, c->w_pos.p, nullptr, 0, Np + Nb))) return rc;
   }
   if (n && (rc = upload_visual(c, kind ? Np : 0, n, stamp, camera, landmark, meas, kind))) return rc;
   HB_CUDA(cudaStreamSynchronize(c->stream));
@@ -1542,11 +1567,11 @@ int hb200_set_manifold_factors(hb200_ctx* c, int n, const double* stamp, const i
   if (!c || n < 0 || (n > 0 && (!stamp || !sensor || !pose))) return fail(-1, "invalid manifold factors");
   HB_CUDA(cudaSetDevice(c->device));
   const size_t N = n;
-  HB_CUDA(c->m_stamp.ensure(N)); HB_CUDA(c->m_meas.ensure(7 * N)); HB_CUDA(c->m_sensor.ensure(N)); HB_CUDA(c->m_idx.ensure(N));
+  HB_CUDA(c->manifold.grow(N, 0, c->stream));
   if (N) {
-    HB_CUDA(cudaMemcpyAsync(c->m_stamp.p, stamp, sizeof(double) * N, cudaMemcpyHostToDevice, c->stream));
-    HB_CUDA(cudaMemcpyAsync(c->m_meas.p, pose, sizeof(double) * 7 * N, cudaMemcpyHostToDevice, c->stream));
-    HB_CUDA(cudaMemcpyAsync(c->m_sensor.p, sensor, sizeof(int) * N, cudaMemcpyHostToDevice, c->stream));
+    HB_CUDA(cudaMemcpyAsync(c->manifold.stamp.p, stamp, sizeof(double) * N, cudaMemcpyHostToDevice, c->stream));
+    HB_CUDA(cudaMemcpyAsync(c->manifold.meas.p, pose, sizeof(double) * 7 * N, cudaMemcpyHostToDevice, c->stream));
+    HB_CUDA(cudaMemcpyAsync(c->manifold.sensor.p, sensor, sizeof(int) * N, cudaMemcpyHostToDevice, c->stream));
   }
   HB_CUDA(cudaStreamSynchronize(c->stream));
   c->Nm = n;
@@ -1558,10 +1583,10 @@ int hb200_set_inertial_factors(hb200_ctx* c, int n, const double* stamp, const d
   if (!c || n < 0 || (n > 0 && (!stamp || !meas))) return fail(-1, "invalid inertial factors");
   HB_CUDA(cudaSetDevice(c->device));
   const size_t N = n;
-  HB_CUDA(c->i_stamp.ensure(N)); HB_CUDA(c->i_meas.ensure(6 * N)); HB_CUDA(c->i_idx.ensure(N));
+  HB_CUDA(c->inertial.grow(N, 0, c->stream));
   if (N) {
-    HB_CUDA(cudaMemcpyAsync(c->i_stamp.p, stamp, sizeof(double) * N, cudaMemcpyHostToDevice, c->stream));
-    HB_CUDA(cudaMemcpyAsync(c->i_meas.p, meas, sizeof(double) * 6 * N, cudaMemcpyHostToDevice, c->stream));
+    HB_CUDA(cudaMemcpyAsync(c->inertial.stamp.p, stamp, sizeof(double) * N, cudaMemcpyHostToDevice, c->stream));
+    HB_CUDA(cudaMemcpyAsync(c->inertial.meas.p, meas, sizeof(double) * 6 * N, cudaMemcpyHostToDevice, c->stream));
   }
   HB_CUDA(cudaStreamSynchronize(c->stream));
   c->Ni = n;
@@ -1590,19 +1615,19 @@ int derive_window(hb200_ctx* c, int kind = 0) {
   HB_CUDA(c->w_keep.ensure(std::max(std::max(Nv, Ni), 1))); HB_CUDA(c->w_pos.ensure(std::max(std::max(Nv, Ni), 1)));
   // landmark CSR
   HB_CUDA(cudaMemsetAsync(c->w_cnt.p, 0, sizeof(int) * (static_cast<size_t>(L) + 1), c->stream));
-  if (Nv) { count_kernel<<<(Nv + 255) / 256, 256, 0, c->stream>>>(Nv, c->v_idx.p, c->w_cnt.p); HB_LAUNCH(c, "count_kernel"); }
+  if (Nv) { count_kernel<<<(Nv + 255) / 256, 256, 0, c->stream>>>(Nv, c->visual.idx.p, c->w_cnt.p); HB_LAUNCH(c, "count_kernel"); }
   scan_kernel<<<1, 1024, 0, c->stream>>>(c->w_cnt.p, L + 1, c->lm_off.p, c->w_scal.p + 0);
   HB_LAUNCH(c, "scan_kernel");
   HB_CUDA(cudaMemsetAsync(c->w_cnt.p, 0, sizeof(int) * (static_cast<size_t>(L) + 1), c->stream));
   if (Nv) {
-    csr_fill_kernel<<<(Nv + 255) / 256, 256, 0, c->stream>>>(Nv, c->v_idx.p, c->lm_off.p, c->w_cnt.p, c->lm_obs.p);
+    csr_fill_kernel<<<(Nv + 255) / 256, 256, 0, c->stream>>>(Nv, c->visual.idx.p, c->lm_off.p, c->w_cnt.p, c->lm_obs.p);
     HB_LAUNCH(c, "csr_fill_kernel");
-    csr_sort_kernel<<<(L + 127) / 128, 128, 0, c->stream>>>(L, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->k, c->w_scal.p + 1);
+    csr_sort_kernel<<<(L + 127) / 128, 128, 0, c->stream>>>(L, c->lm_off.p, c->lm_obs.p, c->visual.idx.p, c->k, c->w_scal.p + 1);
     HB_LAUNCH(c, "csr_sort_kernel");
   }
   // inertial runs
   if (Ni) {
-    run_flag_kernel<<<(Ni + 255) / 256, 256, 0, c->stream>>>(Ni, c->i_idx.p, c->w_keep.p);
+    run_flag_kernel<<<(Ni + 255) / 256, 256, 0, c->stream>>>(Ni, c->inertial.idx.p, c->w_keep.p);
     HB_LAUNCH(c, "run_flag_kernel");
     scan_kernel<<<1, 1024, 0, c->stream>>>(c->w_keep.p, Ni, c->w_pos.p, c->w_scal.p + 3);
     HB_LAUNCH(c, "scan_kernel");
@@ -1629,7 +1654,7 @@ int derive_window(hb200_ctx* c, int kind = 0) {
   if (2 * 3 * static_cast<size_t>(rows) * sizeof(double) > 200 * 1024) return fail(-6, "landmark track spans %d control-point dofs; exceeds the Schur kernel's shared-memory tile", rows);
   // outputs and launch shapes
   const size_t k = c->k;
-  HB_CUDA(c->v_z.ensure(std::max(Nv, 1))); HB_CUDA(c->v_w.ensure(std::max(Nv, 1)));
+  HB_CUDA(c->visual.grow(std::max(Nv, 1), Nv, c->stream)); HB_CUDA(c->v_w.ensure(std::max(Nv, 1)));
   HB_CUDA(c->v_r.ensure(2 * static_cast<size_t>(std::max(Nv, 1)))); HB_CUDA(c->v_Jp.ensure(12 * k * std::max(Nv, 1))); HB_CUDA(c->v_Jl.ensure(6 * static_cast<size_t>(std::max(Nv, 1))));
   HB_CUDA(c->i_r.ensure(6 * static_cast<size_t>(std::max(Ni, 1)))); HB_CUDA(c->i_Jp.ensure(36 * k * std::max(Ni, 1)));
   HB_CUDA(c->i_wg.ensure(4 * static_cast<size_t>(std::max(Ni, 1)))); HB_CUDA(c->i_wa.ensure(4 * static_cast<size_t>(std::max(Ni, 1)))); HB_CUDA(c->i_Jg.ensure(12 * static_cast<size_t>(std::max(Ni, 1))));
@@ -1657,15 +1682,15 @@ int derive_window(hb200_ctx* c, int kind = 0) {
 
 // Binds the visual factors at list positions [at, at + n) in place; factors that fail to bind are counted in d_invalid[0].
 int bind_pixel_range(hb200_ctx* c, int at, int n) {
-  bind_pixel_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(n, c->v_stamp.p + at, c->knots[0].p, c->K, c->k, c->C, c->L, c->v_idx.p + at, c->d_invalid.p);
+  bind_pixel_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(n, c->visual.stamp.p + at, c->knots[0].p, c->K, c->k, c->C, c->L, c->visual.idx.p + at, c->d_invalid.p);
   HB_LAUNCH(c, "bind_pixel_kernel");
   return 0;
 }
 
 // Binds the inertial factors at list positions [at, at + n) in place; factors that fail to bind are counted in d_invalid[0].
 int bind_inertial_range(hb200_ctx* c, int at, int n) {
-  bind_inertial_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(n, c->i_stamp.p + at, c->knots[0].p, c->K, c->k, c->bg[0].p, c->Kbg, c->ba[0].p, c->Kba, c->kb,
-                                                             c->i_idx.p + at, c->d_invalid.p);
+  bind_inertial_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(n, c->inertial.stamp.p + at, c->knots[0].p, c->K, c->k, c->bg[0].p, c->Kbg, c->ba[0].p, c->Kba, c->kb,
+                                                             c->inertial.idx.p + at, c->d_invalid.p);
   HB_LAUNCH(c, "bind_inertial_kernel");
   return 0;
 }
@@ -1703,13 +1728,13 @@ int hb200_bind(hb200_ctx* c, int* num_invalid) {
   if (Nv && (rc = bind_pixel_range(c, 0, Nv))) return rc;
   if (Ni && (rc = bind_inertial_range(c, 0, Ni))) return rc;
   if (Nm) {
-    bind_manifold_kernel<<<(Nm + 127) / 128, 128, 0, c->stream>>>(Nm, c->m_stamp.p, c->m_sensor.p, c->knots[0].p, c->K, c->k, c->P, c->m_idx.p, c->d_invalid.p);
+    bind_manifold_kernel<<<(Nm + 127) / 128, 128, 0, c->stream>>>(Nm, c->manifold.stamp.p, c->manifold.sensor.p, c->knots[0].p, c->K, c->k, c->P, c->manifold.idx.p, c->d_invalid.p);
     HB_LAUNCH(c, "bind_manifold_kernel");
   }
   std::vector<int4> vi(Nv), ii(Ni);
   int invalid = 0;
-  if (Nv) HB_CUDA(cudaMemcpyAsync(vi.data(), c->v_idx.p, sizeof(int4) * Nv, cudaMemcpyDeviceToHost, c->stream));
-  if (Ni) HB_CUDA(cudaMemcpyAsync(ii.data(), c->i_idx.p, sizeof(int4) * Ni, cudaMemcpyDeviceToHost, c->stream));
+  if (Nv) HB_CUDA(cudaMemcpyAsync(vi.data(), c->visual.idx.p, sizeof(int4) * Nv, cudaMemcpyDeviceToHost, c->stream));
+  if (Ni) HB_CUDA(cudaMemcpyAsync(ii.data(), c->inertial.idx.p, sizeof(int4) * Ni, cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaMemcpyAsync(&invalid, c->d_invalid.p, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
   if (num_invalid) *num_invalid = invalid;
@@ -1724,7 +1749,7 @@ int hb200_bind(hb200_ctx* c, int* num_invalid) {
   if (!std::is_sorted(vi.begin(), vi.end(), by_base)) {
     v_inv = bound_order(vi, c->v_perm, by_base);
     HB_CUDA(cudaMemcpyAsync(c->w_pos.p, v_inv.data(), sizeof(int) * Nv, cudaMemcpyHostToDevice, c->stream));
-    if ((rc = compact_visual(c, Nv, nullptr, c->w_pos.p, nullptr, 0, 0, Nv))) return rc;
+    if ((rc = compact_visual(c, Nv, nullptr, c->w_pos.p, nullptr, 0, Nv))) return rc;
   }
   if (!std::is_sorted(ii.begin(), ii.end(), by_bases)) {
     i_inv = bound_order(ii, c->i_perm, by_bases);
@@ -1790,8 +1815,8 @@ int hb200_get_index_maps(hb200_ctx* c, int* pixel_base, int* inertial_base, int*
   if (rc) return rc;
   const int Nv = pixel_base ? c->Nv : 0, Ni = (inertial_base || gyro_bias_base || accel_bias_base) ? c->Ni : 0;
   std::vector<int4> vi(Nv), ii(Ni);
-  if (Nv) HB_CUDA(cudaMemcpyAsync(vi.data(), c->v_idx.p, sizeof(int4) * Nv, cudaMemcpyDeviceToHost, c->stream));
-  if (Ni) HB_CUDA(cudaMemcpyAsync(ii.data(), c->i_idx.p, sizeof(int4) * Ni, cudaMemcpyDeviceToHost, c->stream));
+  if (Nv) HB_CUDA(cudaMemcpyAsync(vi.data(), c->visual.idx.p, sizeof(int4) * Nv, cudaMemcpyDeviceToHost, c->stream));
+  if (Ni) HB_CUDA(cudaMemcpyAsync(ii.data(), c->inertial.idx.p, sizeof(int4) * Ni, cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
   for (int p = 0; p < Nv; ++p) if (c->v_perm[p] < c->Np) pixel_base[c->v_perm[p]] = vi[p].x;
   for (int p = 0; p < Ni; ++p) {
@@ -1923,7 +1948,7 @@ int ensure_calib_mirror(hb200_ctx* c) {
     const int blocks = static_cast<int>((Nv + kEvalThreads - 1) / kEvalThreads);
     const int rc = with_order(c->k, [&](auto K) {
       return with_flag(c->wt_visual(), [&](auto WT) {
-        pixel_calib_kernel<K, WT><<<blocks, kEvalThreads, 0, c->stream>>>(c->Nv, c->v_stamp.p, reinterpret_cast<const double2*>(c->v_pixel.p), c->v_z.p, c->v_idx.p, c->tab[0].p,
+        pixel_calib_kernel<K, WT><<<blocks, kEvalThreads, 0, c->stream>>>(c->Nv, c->visual.stamp.p, c->visual.pixel.p, c->visual.z.p, c->visual.idx.p, c->tab[0].p,
                                                                           c->cam_tab.p, c->lms[0].p, c->basis, dv.p, c->wt.p);
         return check_launch(c, "pixel_calib_kernel");
       });
@@ -1936,7 +1961,7 @@ int ensure_calib_mirror(hb200_ctx* c) {
     const int blocks = static_cast<int>((Ni + kEvalThreads - 1) / kEvalThreads);
     const int rc = with_order(c->k, [&](auto K) {
       return with_flag(c->wt_set[HB200_INERTIAL], [&](auto WT) {
-        inertial_calib_kernel<K, WT><<<blocks, kEvalThreads, 0, c->stream>>>(c->Ni, c->i_stamp.p, c->i_idx.p, c->tab[0].p, c->imu.p, c->grav[0].p, c->basis, c->quirks, di.p,
+        inertial_calib_kernel<K, WT><<<blocks, kEvalThreads, 0, c->stream>>>(c->Ni, c->inertial.stamp.p, c->inertial.idx.p, c->tab[0].p, c->imu.p, c->grav[0].p, c->basis, c->quirks, di.p,
                                                                              c->wt.p);
         return check_launch(c, "inertial_calib_kernel");
       });
@@ -1949,7 +1974,7 @@ int ensure_calib_mirror(hb200_ctx* c) {
     const int blocks = static_cast<int>((Nm + kEvalThreads - 1) / kEvalThreads);
     const int rc = with_order(c->k, [&](auto K) {
       return with_flag(c->wt_set[HB200_MANIFOLD], [&](auto WT) {
-        manifold_calib_kernel<K, WT><<<blocks, kEvalThreads, 0, c->stream>>>(c->Nm, c->m_stamp.p, c->m_meas.p, c->m_idx.p, c->tab[0].p, c->sensors.p, c->basis, dm.p, c->wt.p);
+        manifold_calib_kernel<K, WT><<<blocks, kEvalThreads, 0, c->stream>>>(c->Nm, c->manifold.stamp.p, c->manifold.meas.p, c->manifold.idx.p, c->tab[0].p, c->sensors.p, c->basis, dm.p, c->wt.p);
         return check_launch(c, "manifold_calib_kernel");
       });
     });
@@ -2209,7 +2234,7 @@ int cov_blocks_enqueue(hb200_ctx* c, const CovPoint& pt) {
   const bool landmarks = pt.Nv && std::any_of(c->cov_req.begin(), c->cov_req.end(), [](const int4& r) { return r.x == kCovLandmark || r.z == kCovLandmark; });
   HB_CUDA(c->cov_span.ensure(span.size()));
   if (landmarks) {
-    cov_landmark_span_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(n, c->cov_req_d.p, c->lm_off.p, c->lm_obs.p, c->v_idx.p, pt.k, c->cov_span.p);
+    cov_landmark_span_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(n, c->cov_req_d.p, c->lm_off.p, c->lm_obs.p, c->visual.idx.p, pt.k, c->cov_span.p);
     HB_LAUNCH(c, "cov_landmark_span_kernel");
   }
   if (npair) {
@@ -2276,7 +2301,7 @@ int cov_blocks_enqueue(hb200_ctx* c, const CovPoint& pt) {
     if (n) {
       HB_CUDA(cudaFuncSetAttribute(cov_cross_landmark_kernel<Kc>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
       cov_cross_landmark_kernel<Kc><<<(n + kLmWarps - 1) / kLmWarps, kLmWarps * 32, smem, c->stream>>>(
-          n, c->cov_req_d.p, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p, c->Vchol.p, c->cov_packed_next.p, c->cov_lm_next.p,
+          n, c->cov_req_d.p, c->lm_off.p, c->lm_obs.p, c->visual.idx.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p, c->Vchol.p, c->cov_packed_next.p, c->cov_lm_next.p,
           c->cov_far.p, fp, lay, pt.Kbg, c->multi() ? 1 : 0, c->cov_status.p, pt.max_rows, c->cov_blk_next.p, c->cov_blk_st_next.p);
       if (const int rc = check_launch(c, "cov_cross_landmark_kernel")) return rc;
     }
@@ -2386,7 +2411,7 @@ int hb200_compute_covariance(hb200_ctx* c, hb200_covariance_info* info) {
     const int blocks = (L + kLmWarps - 1) / kLmWarps;
     const size_t lsmem = static_cast<size_t>(kLmWarps) * 3 * max_rows * sizeof(double);
     const int rc = with_order(k, [&](auto K) {
-      cov_landmark_kernel<K><<<blocks, kLmWarps * 32, lsmem, c->stream>>>(L, c->lm_off.p, c->lm_obs.p, c->v_idx.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p, c->Vchol.p,
+      cov_landmark_kernel<K><<<blocks, kLmWarps * 32, lsmem, c->stream>>>(L, c->lm_off.p, c->lm_obs.p, c->visual.idx.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p, c->Vchol.p,
                                                                          c->cov_packed_next.p, lay, c->cov_status.p, c->cov_lm_next.p, max_rows);
       return check_launch(c, "cov_landmark_kernel");
     });
@@ -2967,14 +2992,14 @@ int check_device_window(hb200_ctx* c) {
 int append_visual(hb200_ctx* c, int n, const double* stamp, const int* camera, const int* landmark, const double* meas, int kind) {
   HB_CUDA(cudaSetDevice(c->device));
   const size_t Nv = c->Nv;
-  int rc = grow_visual(c, Nv + n);
-  if (rc) return rc;
+  HB_CUDA(c->visual.grow(Nv + n, Nv, c->stream));
   HB_CUDA(c->d_invalid.ensure(2 + kAgreeOut));   // [bad index, arrival order | agreement]
   HB_CUDA(cudaMemsetAsync(c->d_invalid.p, 0, (2 + kAgreeOut) * sizeof(int), c->stream));
+  int rc = 0;
   if (n) {
     if ((rc = upload_visual(c, static_cast<int>(Nv), n, stamp, camera, landmark, meas, kind))) return rc;
     if ((rc = bind_pixel_range(c, static_cast<int>(Nv), n))) return rc;
-    tail_sorted_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(static_cast<int>(Nv), n, c->v_idx.p, c->d_invalid.p + 1);
+    tail_sorted_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(static_cast<int>(Nv), n, c->visual.idx.p, c->d_invalid.p + 1);
     HB_LAUNCH(c, "tail_sorted_kernel");
   }
   const int call = kind ? kCallBearing : kCallPixel;
@@ -3138,14 +3163,13 @@ int hb200_append_manifold_factors(hb200_ctx* c, int n, const double* stamp, cons
   if (c->P == 0) return fail(-2, "pose sensors not set");
   HB_CUDA(cudaSetDevice(c->device));
   const size_t Nm = c->Nm;
-  HB_CUDA(c->m_stamp.grow(Nm + n, Nm, c->stream)); HB_CUDA(c->m_meas.grow(7 * (Nm + n), 7 * Nm, c->stream));
-  HB_CUDA(c->m_sensor.grow(Nm + n, Nm, c->stream)); HB_CUDA(c->m_idx.grow(Nm + n, Nm, c->stream));
+  HB_CUDA(c->manifold.grow(Nm + n, Nm, c->stream));
   HB_CUDA(c->d_invalid.ensure(1));
   HB_CUDA(cudaMemsetAsync(c->d_invalid.p, 0, sizeof(int), c->stream));
-  HB_CUDA(cudaMemcpyAsync(c->m_stamp.p + Nm, stamp, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
-  HB_CUDA(cudaMemcpyAsync(c->m_meas.p + 7 * Nm, pose, sizeof(double) * 7 * n, cudaMemcpyHostToDevice, c->stream));
-  HB_CUDA(cudaMemcpyAsync(c->m_sensor.p + Nm, sensor, sizeof(int) * n, cudaMemcpyHostToDevice, c->stream));
-  bind_manifold_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(n, c->m_stamp.p + Nm, c->m_sensor.p + Nm, c->knots[0].p, c->K, c->k, c->P, c->m_idx.p + Nm, c->d_invalid.p);
+  HB_CUDA(cudaMemcpyAsync(c->manifold.stamp.p + Nm, stamp, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
+  HB_CUDA(cudaMemcpyAsync(c->manifold.meas.p + 7 * Nm, pose, sizeof(double) * 7 * n, cudaMemcpyHostToDevice, c->stream));
+  HB_CUDA(cudaMemcpyAsync(c->manifold.sensor.p + Nm, sensor, sizeof(int) * n, cudaMemcpyHostToDevice, c->stream));
+  bind_manifold_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(n, c->manifold.stamp.p + Nm, c->manifold.sensor.p + Nm, c->knots[0].p, c->K, c->k, c->P, c->manifold.idx.p + Nm, c->d_invalid.p);
   HB_LAUNCH(c, "bind_manifold_kernel");
   int bad = 0;
   HB_CUDA(cudaMemcpyAsync(&bad, c->d_invalid.p, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
@@ -3175,7 +3199,7 @@ int hb200_append_stereo_tracks(hb200_ctx* c, int n, const double* stamp, const i
     hi[f] = camera0[f]; hi[N + f] = camera1[f]; hi[2 * N + f] = landmark[f]; hi[3 * N + f] = landmark[f] < 0;
     fresh += landmark[f] < 0;
   }
-  if ((rc = grow_visual(c, Nv + 2 * N))) return rc;
+  HB_CUDA(c->visual.grow(Nv + 2 * N, Nv, c->stream));
   for (int s2 = 0; s2 < 2; ++s2) HB_CUDA(c->lms[s2].grow(3 * (L + fresh), s2 == 0 ? 3 * L : 0, c->stream));
   HB_CUDA(c->d_invalid.ensure(3 + kAgreeOut));   // [bad tracks, order violations, new landmarks | agreement]
   HB_CUDA(cudaMemsetAsync(c->d_invalid.p, 0, (3 + kAgreeOut) * sizeof(int), c->stream));
@@ -3190,15 +3214,14 @@ int hb200_append_stereo_tracks(hb200_ctx* c, int n, const double* stamp, const i
     HB_LAUNCH(c, "scan_kernel");
     prep_kernel<<<(c->K + 63) / 64, 64, 0, c->stream>>>(c->K, c->knots[0].p, c->tab[0].p, nullptr, 0);   // knot table of the current state
     HB_LAUNCH(c, "prep_kernel");
-    double2* v_pixel = reinterpret_cast<double2*>(c->v_pixel.p);
     rc = with_order(c->k, [&](auto K) {
       stereo_track_kernel<K><<<(n + 127) / 128, 128, 0, c->stream>>>(n, d_t, c->trk_i.p, c->trk_i.p + N, d_t + N, d_t + 3 * N, d_lm, d_rank, c->knots[0].p, c->tab[0].p, c->K,
-                                                                    c->basis, c->cams.p, c->C, static_cast<int>(L), static_cast<int>(Nv), c->v_stamp.p, v_pixel, c->v_z.p,
-                                                                    c->v_idx.p, c->lms[0].p, c->d_invalid.p);
+                                                                    c->basis, c->cams.p, c->C, static_cast<int>(L), static_cast<int>(Nv), c->visual.stamp.p, c->visual.pixel.p, c->visual.z.p,
+                                                                    c->visual.idx.p, c->lms[0].p, c->d_invalid.p);
       return check_launch(c, "stereo_track_kernel");
     });
     if (rc) return rc;
-    tail_sorted_kernel<<<(2 * n + 127) / 128, 128, 0, c->stream>>>(static_cast<int>(Nv), 2 * n, c->v_idx.p, c->d_invalid.p + 1);
+    tail_sorted_kernel<<<(2 * n + 127) / 128, 128, 0, c->stream>>>(static_cast<int>(Nv), 2 * n, c->visual.idx.p, c->d_invalid.p + 1);
     HB_LAUNCH(c, "tail_sorted_kernel");
   }
   if (c->multi() && (rc = agree_round(c, vote_header(c, kCallStereo), VoteSrc{c->d_invalid.p, {nullptr, nullptr, nullptr}, nullptr, nullptr}, c->d_invalid.p + 3))) return rc;
@@ -3224,13 +3247,13 @@ int hb200_append_inertial_factors(hb200_ctx* c, int n, const double* stamp, cons
   if (!c->have_imu || c->Kbg == 0 || c->Kba == 0) return fail(-2, "inertial factors need IMU calibration and bias splines");
   HB_CUDA(cudaSetDevice(c->device));
   const size_t Ni = c->Ni;
-  HB_CUDA(c->i_stamp.grow(Ni + n, Ni, c->stream)); HB_CUDA(c->i_meas.grow(6 * (Ni + n), 6 * Ni, c->stream)); HB_CUDA(c->i_idx.grow(Ni + n, Ni, c->stream));
+  HB_CUDA(c->inertial.grow(Ni + n, Ni, c->stream));
   HB_CUDA(c->d_invalid.ensure(2));
   HB_CUDA(cudaMemsetAsync(c->d_invalid.p, 0, 2 * sizeof(int), c->stream));
-  HB_CUDA(cudaMemcpyAsync(c->i_stamp.p + Ni, stamp, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
-  HB_CUDA(cudaMemcpyAsync(c->i_meas.p + 6 * Ni, meas, sizeof(double) * 6 * n, cudaMemcpyHostToDevice, c->stream));
+  HB_CUDA(cudaMemcpyAsync(c->inertial.stamp.p + Ni, stamp, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
+  HB_CUDA(cudaMemcpyAsync(c->inertial.meas.p + 6 * Ni, meas, sizeof(double) * 6 * n, cudaMemcpyHostToDevice, c->stream));
   if ((rc = bind_inertial_range(c, static_cast<int>(Ni), n))) return rc;
-  tail_sorted_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(static_cast<int>(Ni), n, c->i_idx.p, c->d_invalid.p + 1);
+  tail_sorted_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(static_cast<int>(Ni), n, c->inertial.idx.p, c->d_invalid.p + 1);
   HB_LAUNCH(c, "tail_sorted_kernel");
   int bad[2] = {0, 0};
   HB_CUDA(cudaMemcpyAsync(bad, c->d_invalid.p, 2 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
@@ -3265,7 +3288,7 @@ int hb200_slide(hb200_ctx* c, double lower_bound, int flags, hb200_slide_stats* 
   HB_CUDA(f_keep.ensure(std::max(Ni + Nm, 1))); HB_CUDA(f_pos.ensure(std::max(Ni + Nm, 1)));
   int* i_keep = f_keep.p; int* i_pos = f_pos.p; int* m_keep = f_keep.p + Ni; int* m_pos = f_pos.p + Ni;
   HB_CUDA(cudaMemsetAsync(c->w_last.p, 0, sizeof(unsigned long long) * std::max(L, 1), c->stream));
-  if (Nv) { landmark_last_stamp_kernel<<<(Nv + 255) / 256, 256, 0, c->stream>>>(Nv, c->v_stamp.p, c->v_idx.p, c->w_last.p); HB_LAUNCH(c, "landmark_last_stamp_kernel"); }
+  if (Nv) { landmark_last_stamp_kernel<<<(Nv + 255) / 256, 256, 0, c->stream>>>(Nv, c->visual.stamp.p, c->visual.idx.p, c->w_last.p); HB_LAUNCH(c, "landmark_last_stamp_kernel"); }
   if (L) {
     landmark_keep_kernel<<<(L + 255) / 256, 256, 0, c->stream>>>(L, c->w_last.p, lower_bound, c->w_lkeep.p);
     HB_LAUNCH(c, "landmark_keep_kernel");
@@ -3273,20 +3296,20 @@ int hb200_slide(hb200_ctx* c, double lower_bound, int flags, hb200_slide_stats* 
     HB_LAUNCH(c, "scan_kernel");
   }
   if (Nv) {
-    visual_keep_kernel<<<(Nv + 255) / 256, 256, 0, c->stream>>>(Nv, c->v_idx.p, c->w_lkeep.p, c->w_keep.p, c->w_scal.p + 3, c->w_scal.p + 7);
+    visual_keep_kernel<<<(Nv + 255) / 256, 256, 0, c->stream>>>(Nv, c->visual.idx.p, c->w_lkeep.p, c->w_keep.p, c->w_scal.p + 3, c->w_scal.p + 7);
     HB_LAUNCH(c, "visual_keep_kernel");
     scan_kernel<<<1, 1024, 0, c->stream>>>(c->w_keep.p, Nv, c->w_pos.p, c->w_scal.p + 1);
     HB_LAUNCH(c, "scan_kernel");
   }
   if (Ni) {
-    inertial_keep_kernel<<<(Ni + 255) / 256, 256, 0, c->stream>>>(Ni, c->i_idx.p, c->k, (flags & HB200_SLIDE_DROP_INERTIAL) ? last_const : -1, i_keep, c->w_scal.p + 4,
+    inertial_keep_kernel<<<(Ni + 255) / 256, 256, 0, c->stream>>>(Ni, c->inertial.idx.p, c->k, (flags & HB200_SLIDE_DROP_INERTIAL) ? last_const : -1, i_keep, c->w_scal.p + 4,
                                                                   drop_bias ? c->w_scal.p + 8 : nullptr);
     HB_LAUNCH(c, "inertial_keep_kernel");
     scan_kernel<<<1, 1024, 0, c->stream>>>(i_keep, Ni, i_pos, c->w_scal.p + 2);
     HB_LAUNCH(c, "scan_kernel");
   }
   if (Nm) {   // the reference never removes pose residuals either: same rule as the inertial ones, its own flag
-    inertial_keep_kernel<<<(Nm + 255) / 256, 256, 0, c->stream>>>(Nm, c->m_idx.p, c->k, (flags & HB200_SLIDE_DROP_MANIFOLD) ? last_const : -1, m_keep, c->w_scal.p + 6);
+    inertial_keep_kernel<<<(Nm + 255) / 256, 256, 0, c->stream>>>(Nm, c->manifold.idx.p, c->k, (flags & HB200_SLIDE_DROP_MANIFOLD) ? last_const : -1, m_keep, c->w_scal.p + 6);
     HB_LAUNCH(c, "manifold_keep_kernel");
     scan_kernel<<<1, 1024, 0, c->stream>>>(m_keep, Nm, m_pos, c->w_scal.p + 5);
     HB_LAUNCH(c, "scan_kernel");
@@ -3320,46 +3343,22 @@ int hb200_slide(hb200_ctx* c, double lower_bound, int flags, hb200_slide_stats* 
   };
   const int g_shift = drop_bias ? bias_shift(c->h_bg_stamp, gyro_min) : 0, a_shift = drop_bias ? bias_shift(c->h_ba_stamp, accel_min) : 0;
   const int Kbg_new = c->Kbg - g_shift, Kba_new = c->Kba - a_shift;
-  // compaction into the alternate buffers, then swap
-  const int n_alt = std::max(std::max(std::max(Nv_new, Ni_new), Nm_new), 1);
-  HB_CUDA(c->alt_stamp.ensure(n_alt)); HB_CUDA(c->alt_idx.ensure(n_alt));
-  if (Nv && (rc = compact_visual(c, Nv, c->w_keep.p, c->w_pos.p, c->w_lpos.p, shift, 0, Nv_new))) return rc;
-  HB_CUDA(c->alt_meas.ensure(std::max(6 * static_cast<size_t>(Ni_new), 7 * static_cast<size_t>(Nm_new)) + 1));
+  // compaction of the factor lists into their spare copies and of the state into its trial copy, each then switched in
+  if (Nv && (rc = compact_visual(c, Nv, c->w_keep.p, c->w_pos.p, c->w_lpos.p, shift, Nv_new))) return rc;
   if (Ni && (rc = compact_inertial(c, Ni, i_keep, i_pos, shift, g_shift, a_shift, Ni_new))) return rc;
-  if (Nm) {
-    HB_CUDA(c->alt_midx.ensure(std::max(Nm_new, 1))); HB_CUDA(c->alt_sensor.ensure(std::max(Nm_new, 1)));
-    compact_manifold_kernel<<<(Nm + 255) / 256, 256, 0, c->stream>>>(Nm, m_keep, m_pos, shift, c->m_stamp.p, c->m_meas.p, c->m_sensor.p, c->m_idx.p, c->alt_stamp.p, c->alt_meas.p,
-                                                                    c->alt_sensor.p, c->alt_midx.p);
-    HB_LAUNCH(c, "compact_manifold_kernel");
-    HB_CUDA(cudaMemcpyAsync(c->m_stamp.p, c->alt_stamp.p, sizeof(double) * Nm_new, cudaMemcpyDeviceToDevice, c->stream));
-    HB_CUDA(cudaMemcpyAsync(c->m_meas.p, c->alt_meas.p, sizeof(double) * 7 * Nm_new, cudaMemcpyDeviceToDevice, c->stream));
-    HB_CUDA(cudaMemcpyAsync(c->m_sensor.p, c->alt_sensor.p, sizeof(int) * Nm_new, cudaMemcpyDeviceToDevice, c->stream));
-    HB_CUDA(cudaMemcpyAsync(c->m_idx.p, c->alt_midx.p, sizeof(int2) * Nm_new, cudaMemcpyDeviceToDevice, c->stream));
-  }
+  if (Nm && (rc = compact_manifold(c, Nm, m_keep, m_pos, shift, Nm_new))) return rc;
+  c->kernel_args_changed();   // (the state switches below move buffers the captured iteration points at)
   if (L) {
-    HB_CUDA(c->alt_lms.ensure(3 * static_cast<size_t>(std::max(L_new, 1))));
-    compact_landmarks_kernel<<<(L + 255) / 256, 256, 0, c->stream>>>(L, c->w_lkeep.p, c->w_lpos.p, c->lms[0].p, c->alt_lms.p);
+    compact_landmarks_kernel<<<(L + 255) / 256, 256, 0, c->stream>>>(L, c->w_lkeep.p, c->w_lpos.p, c->lms[0].p, c->lms[1].p);
     HB_LAUNCH(c, "compact_landmarks_kernel");
-    HB_CUDA(cudaMemcpyAsync(c->lms[0].p, c->alt_lms.p, sizeof(double) * 3 * L_new, cudaMemcpyDeviceToDevice, c->stream));
+    c->lms[0].swap(c->lms[1]);
   }
-  // (one scratch buffer for the three splines: the copies back are ordered on the stream)
-  const size_t alt_need = std::max(shift ? 8 * static_cast<size_t>(K_new) : 0,
-                                   std::max(g_shift ? 4 * static_cast<size_t>(Kbg_new) : 0, a_shift ? 4 * static_cast<size_t>(Kba_new) : 0));
-  if (alt_need) HB_CUDA(c->alt_knots.ensure(alt_need));
-  if (shift) {
-    shift_knots_kernel<<<(8 * K_new + 255) / 256, 256, 0, c->stream>>>(K_new, shift, 8, c->knots[0].p, c->alt_knots.p);
+  const struct { DevBuf<double>* copies; int shift, stride, count; } splines[3] = {{c->knots, shift, 8, K_new}, {c->bg, g_shift, 4, Kbg_new}, {c->ba, a_shift, 4, Kba_new}};
+  for (const auto& s : splines) {
+    if (!s.shift) continue;
+    shift_knots_kernel<<<(s.stride * s.count + 255) / 256, 256, 0, c->stream>>>(s.count, s.shift, s.stride, s.copies[0].p, s.copies[1].p);
     HB_LAUNCH(c, "shift_knots_kernel");
-    HB_CUDA(cudaMemcpyAsync(c->knots[0].p, c->alt_knots.p, sizeof(double) * 8 * K_new, cudaMemcpyDeviceToDevice, c->stream));
-  }
-  if (g_shift) {
-    shift_knots_kernel<<<(4 * Kbg_new + 255) / 256, 256, 0, c->stream>>>(Kbg_new, g_shift, 4, c->bg[0].p, c->alt_knots.p);
-    HB_LAUNCH(c, "shift_knots_kernel");
-    HB_CUDA(cudaMemcpyAsync(c->bg[0].p, c->alt_knots.p, sizeof(double) * 4 * Kbg_new, cudaMemcpyDeviceToDevice, c->stream));
-  }
-  if (a_shift) {
-    shift_knots_kernel<<<(4 * Kba_new + 255) / 256, 256, 0, c->stream>>>(Kba_new, a_shift, 4, c->ba[0].p, c->alt_knots.p);
-    HB_LAUNCH(c, "shift_knots_kernel");
-    HB_CUDA(cudaMemcpyAsync(c->ba[0].p, c->alt_knots.p, sizeof(double) * 4 * Kba_new, cudaMemcpyDeviceToDevice, c->stream));
+    s.copies[0].swap(s.copies[1]);
   }
   HB_CUDA(cudaStreamSynchronize(c->stream));
   // host bookkeeping: sizes, stamps, constancy (elements at or before the lower bound: reference optimizer.cpp:322-328;
