@@ -182,6 +182,50 @@ struct CovPoint {
   DevBuf<double> knots, tab, bg, ba;
 };
 
+// The results of hb200_compute_covariance: the packed selected inverse, the landmark marginals, and the requested blocks
+// (blk_n) and stamp-pair blocks (pair_n), each with its status.  swap: switch with another copy.
+struct CovResults {
+  DevBuf<double> packed, lm, blk, pair_joint, pair_rel;
+  DevBuf<int> blk_st, pair_st;
+  int blk_n = 0, pair_n = 0;
+  void swap(CovResults& o) {
+    packed.swap(o.packed); lm.swap(o.lm); blk.swap(o.blk); pair_joint.swap(o.pair_joint); pair_rel.swap(o.pair_rel);
+    blk_st.swap(o.blk_st); pair_st.swap(o.pair_st); std::swap(blk_n, o.blk_n); std::swap(pair_n, o.pair_n);
+  }
+};
+
+// The factor kernels' outputs, one buffer per field.  ensure: room for n factors (at least one) at spline order k.
+struct VisualOut {
+  DevBuf<double> r, Jp, Jl, w;   // per factor: [2] residual, [2][6k] state and [2][3] landmark Jacobians, robust-loss weight
+  cudaError_t ensure(size_t n, size_t k) { n = std::max<size_t>(n, 1); return first_error({r.ensure(2 * n), Jp.ensure(12 * k * n), Jl.ensure(6 * n), w.ensure(n)}); }
+};
+struct InertialOut {
+  DevBuf<double> r, Jp, wg, wa, Jg;   // per factor: [6] residual, [6][6k] state Jacobian, [4] + [4] bias weights, [6][2] gravity
+  cudaError_t ensure(size_t n, size_t k) {
+    n = std::max<size_t>(n, 1);
+    return first_error({r.ensure(6 * n), Jp.ensure(36 * k * n), wg.ensure(4 * n), wa.ensure(4 * n), Jg.ensure(12 * n)});
+  }
+};
+struct ManifoldOut {
+  DevBuf<double> r, Jp;   // per factor: [6] residual, [6][6k] state Jacobian
+  cudaError_t ensure(size_t n, size_t k) { n = std::max<size_t>(n, 1); return first_error({r.ensure(6 * n), Jp.ensure(36 * k * n)}); }
+};
+
+// Host mirror of the factor outputs for hb200_factor_evaluate in user order, indexed by factor kind (HB200_PIXEL ...):
+// residuals, state, landmark and calibration Jacobians (the last on demand: calib_valid), inertial bias weights and gravity.
+struct OutputMirror {
+  std::vector<double> r[4], Jp[4], Jl[4], Jc[4], wg, wa, Jg;
+  bool valid = false, calib_valid = false;
+};
+
+// One capture of the LM iteration.  release: destroy both handles and mark it stale.
+struct IterationGraph {
+  cudaGraph_t graph = nullptr;
+  cudaGraphExec_t exec = nullptr;
+  bool valid = false;
+  void release() { if (exec) cudaGraphExecDestroy(exec); if (graph) cudaGraphDestroy(graph); exec = nullptr; graph = nullptr; valid = false; }
+};
+
 }  // namespace
 
 struct hb200_ctx {
@@ -230,7 +274,7 @@ struct hb200_ctx {
   VisualList visual, visual_spare;
   InertialList inertial, inertial_spare;
   ManifoldList manifold, manifold_spare;
-  DevBuf<double> v_w, sensors;
+  DevBuf<double> sensors;
   double huber_bearing = 1.6e-3;   // reference optimizer.cpp:204
   // list position -> user index (visual: pixel factors 0 .. Np-1, bearing factors Np .. Nv-1); appends and slides clear
   // them, ensure_perms rebuilds them
@@ -271,18 +315,15 @@ struct hb200_ctx {
   DevBuf<double> trk_d;
   DevBuf<int> trk_i;
   DevBuf<unsigned long long> w_last;
-  // outputs
-  DevBuf<double> v_r, v_Jp, v_Jl, i_r, i_Jp, i_wg, i_wa, i_Jg, m_r, m_Jp;
+  // outputs, in list order (derive_window sizes them), and their host mirror in user order (hb200_factor_evaluate)
+  VisualOut v_out;
+  InertialOut i_out;
+  ManifoldOut m_out;
   DevBuf<double> cp_pix[2], cp_imu[2];
   int n_pix_blocks = 0, n_imu_blocks = 0, n_man_blocks = 0;   // manifold cost partials follow the inertial ones in cp_imu
   bool evaluated_J = false;
-  // calibration-block Jacobians (on demand, hb200_factor_evaluate) and the reference-quirk switches
-  int quirks = 0;
-  bool calib_valid = false;
-  std::vector<double> m_v_Jc, m_i_Jc, m_m_Jc;   // user order: [Np + Nb][2][14], [Ni][6][36], [Nm][6][6]
-  // host mirror for hb200_factor_evaluate
-  bool mirror_valid = false;
-  std::vector<double> m_v_r, m_v_Jp, m_v_Jl, m_i_r, m_i_Jp, m_i_wg, m_i_wa, m_i_Jg, m_grav, m_b_r, m_b_Jp, m_b_Jl, m_m_r, m_m_Jp;
+  OutputMirror mirror;
+  int quirks = 0;   // the reference-quirk switches
 
   // system (band-only packed storage, see SysLayout)
   int n = 0;
@@ -308,10 +349,12 @@ struct hb200_ctx {
   // covariance call -- any other launch since (an evaluation, an iteration, a slide) rewrote what the compute reads.
   // cov_pt: two linearisation points.  The build freezes one into the slot that is not committed (cov_slot_built); a
   // successful compute commits it by index (cov_slot_committed, meaningful while cov_valid), so a failed compute or a
-  // build not yet computed leaves every reader on the committed point.  *_next: what the next compute writes, swapped
-  // with the unsuffixed results on success only.
+  // build not yet computed leaves every reader on the committed point.  cov_res: the committed results; a compute writes
+  // cov_next and a successful one switches the two.  The results are not part of a point: a second compute with no build
+  // in between writes results while the built point is the committed one.
   DevBuf<SolverState> cov_st;
-  DevBuf<double> cov_ws, cov_packed, cov_packed_next, cov_lm, cov_lm_next;
+  DevBuf<double> cov_ws;
+  CovResults cov_res, cov_next;
   DevBuf<int> cov_counts;
   DevBuf<CovStatus> cov_status;
   bool cov_built = false, cov_valid = false;
@@ -322,20 +365,16 @@ struct hb200_ctx {
   DevBuf<double> cov_t, cov_o;   // hb200_interpolate_covariance / hb200_interpolate_state_covariance staging
   DevBuf<int> cov_bad;
   // requested blocks (hb200_set_covariance_blocks): the registered list, its device copy, the landmark spans and the
-  // far-column plan and scratch of a compute; cov_blk / cov_blk_st (cov_blk_n of them) are the committed blocks
+  // far-column plan and scratch of a compute
   std::vector<int4> cov_req;
   DevBuf<int4> cov_req_d;
   DevBuf<int2> cov_span;
-  DevBuf<int> cov_plan, cov_blk_st, cov_blk_st_next;
-  DevBuf<double> cov_far, cov_blk, cov_blk_next;
-  int cov_blk_n = 0;
+  DevBuf<int> cov_plan;
+  DevBuf<double> cov_far;
   // stamp pairs (hb200_set_covariance_stamp_pairs): the registered [t_a, t_b] per pair and their device copy (their
-  // control-point spans follow the requests' landmark spans in cov_span); cov_pair_joint / _rel / _st (cov_pair_n of
-  // them) are the committed blocks
+  // control-point spans follow the requests' landmark spans in cov_span)
   std::vector<double> cov_pairs;
-  DevBuf<double> cov_pairs_d, cov_pair_joint, cov_pair_joint_next, cov_pair_rel, cov_pair_rel_next;
-  DevBuf<int> cov_pair_st, cov_pair_st_next;
-  int cov_pair_n = 0;
+  DevBuf<double> cov_pairs_d;
 
   hb200_allreduce_fn allreduce = nullptr;
   void* allreduce_user = nullptr;
@@ -352,9 +391,6 @@ struct hb200_ctx {
   bool peer_reduce_wanted = true;
   DevBuf<unsigned long long> red_round;
   DevBuf<unsigned int> red_arrive;
-  cudaGraph_t graph_b = nullptr;            // second capture of the iteration (arena half B)
-  cudaGraphExec_t graph_exec_b = nullptr;
-  bool graph_b_valid = false;
   bool peer_reduce() const { return nccl && peers_open && peer_reduce_wanted && lay.total <= arena_cap; }
   double* assembly() { return peer_reduce() ? mbox.p + kArenaParts + static_cast<long long>(peer_par) * arena_cap : sys.p; }
   DevBuf<unsigned long long> mbox_seq;
@@ -373,9 +409,8 @@ struct hb200_ctx {
   DevBuf<SolverState> snap_st;
   bool have_snapshot = false;
 
-  cudaGraph_t graph = nullptr;
-  cudaGraphExec_t graph_exec = nullptr;
-  bool graph_valid = false;
+  // the captured iteration, by the arena half it assembles into (peer_par; without the peer-memory reduction only half A)
+  IterationGraph graphs[2];
 
   // family weight matrices (hb200_set_weights): which families have one, the device table the WT kernel instantiations
   // read (kWtSize doubles, identity where a family has none) and its host copy
@@ -400,9 +435,11 @@ struct hb200_ctx {
   // constants or the state changed: the built system and the covariance build no longer match them
   void system_changed() { system_built = false; cov_built = false; }
   // the factor outputs changed or no longer match the state
-  void outputs_changed() { system_changed(); evaluated_J = false; mirror_valid = false; calib_valid = false; }
+  void outputs_changed() { system_changed(); evaluated_J = false; mirror.valid = false; mirror.calib_valid = false; }
+  // something the captured iterations were recorded with changed (a kernel argument, the communicator, the peers)
+  void iterations_changed() { for (IterationGraph& g : graphs) g.valid = false; }
   // shapes or buffers the captured iteration was recorded with changed
-  void kernel_args_changed() { outputs_changed(); graph_valid = false; det_ready = false; }
+  void kernel_args_changed() { outputs_changed(); iterations_changed(); det_ready = false; }
 
   // The variable blocks in their canonical order (knots, gyroscope bias, accelerometer bias, gravity, landmarks): the
   // current state, the trial state, the snapshot and the block's length in doubles.  Every LM step rewrites the whole
@@ -612,7 +649,7 @@ PixelArgs pixel_args(hb200_ctx* c, int sel, double* sys) {
   a.sys = sys; a.lay = c->lay; a.tiles_per_cta = 1;
   a.n = c->Nv; a.stamp = c->visual.stamp.p; a.pixel = c->visual.pixel.p; a.meas_z = c->visual.z.p; a.idx = c->visual.idx.p;
   a.tab = c->tab[sel].p; a.cam_tab = c->cam_tab.p; a.landmarks = c->lms[sel].p;
-  a.r = J ? c->v_r.p : nullptr; a.Jp = c->v_Jp.p; a.Jl = c->v_Jl.p; a.w = c->v_w.p; a.cost_partial = c->cp_pix[J ? 0 : 1].p; a.huber = c->huber; a.huber_bearing = c->huber_bearing; a.K_knots = c->K;
+  a.r = J ? c->v_out.r.p : nullptr; a.Jp = c->v_out.Jp.p; a.Jl = c->v_out.Jl.p; a.w = c->v_out.w.p; a.cost_partial = c->cp_pix[J ? 0 : 1].p; a.huber = c->huber; a.huber_bearing = c->huber_bearing; a.K_knots = c->K;
   return a;
 }
 template <bool J>
@@ -620,7 +657,7 @@ InertialArgs inertial_args(hb200_ctx* c, int sel) {
   InertialArgs a{};
   a.n = c->Ni; a.stamp = c->inertial.stamp.p; a.meas = c->inertial.meas.p; a.idx = c->inertial.idx.p; a.tab = c->tab[sel].p; a.imu_tab = c->imu_tab.p;
   a.bg = c->bg[sel].p; a.ba = c->ba[sel].p; a.gravity = c->grav[sel].p;
-  a.r = J ? c->i_r.p : nullptr; a.Jp = c->i_Jp.p; a.wg = c->i_wg.p; a.wa = c->i_wa.p; a.Jg = c->i_Jg.p;
+  a.r = J ? c->i_out.r.p : nullptr; a.Jp = c->i_out.Jp.p; a.wg = c->i_out.wg.p; a.wa = c->i_out.wa.p; a.Jg = c->i_out.Jg.p;
   a.cost_partial = c->cp_imu[J ? 0 : 1].p; a.loss_scale = c->imu_scale;
   return a;
 }
@@ -673,7 +710,7 @@ int launch_manifold(hb200_ctx* c, int sel) {
   if (c->Nm == 0) return 0;
   ManifoldArgs a{};
   a.n = c->Nm; a.stamp = c->manifold.stamp.p; a.meas = c->manifold.meas.p; a.idx = c->manifold.idx.p; a.tab = c->tab[sel].p; a.sensors = c->sensors.p;
-  a.r = J ? c->m_r.p : nullptr; a.Jp = c->m_Jp.p; a.cost_partial = c->cp_imu[J ? 0 : 1].p + c->n_imu_blocks;
+  a.r = J ? c->m_out.r.p : nullptr; a.Jp = c->m_out.Jp.p; a.cost_partial = c->cp_imu[J ? 0 : 1].p + c->n_imu_blocks;
   return with_flag(c->wt_set[HB200_MANIFOLD], [&](auto WT) {
     manifold_eval_kernel<K, J, WT><<<c->n_man_blocks, kEvalThreads, 0, side(c)>>>(a, c->basis, c->wt.p);
     return check_launch(c, "manifold_eval_kernel");
@@ -754,15 +791,15 @@ int enqueue_build(hb200_ctx* c, const SolverState* st) {
       return with_flag(det, [&](auto DET) {
         const DetOut d = DET ? c->det_imu : DetOut{};
         if (scalar_hess)
-          inertial_hessian_kernel<K, 4, DET><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->inertial.idx.p, c->i_r.p, c->i_Jp.p, c->i_wg.p, c->i_wa.p, c->i_Jg.p,
+          inertial_hessian_kernel<K, 4, DET><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->inertial.idx.p, c->i_out.r.p, c->i_out.Jp.p, c->i_out.wg.p, c->i_out.wa.p, c->i_out.Jg.p,
                                                                                  c->imu_scale, c->assembly(), c->lay, c->o_bg(), c->o_ba(), c->o_g(), splits, d);
         else if (c->wt_set[HB200_INERTIAL])
-          inertial_hessian_mma_kernel<K, 4, K == 4 ? 8 : 12, DET, true><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->inertial.idx.p, c->i_r.p, c->i_Jp.p, c->i_wg.p,
-                                                                                                           c->i_wa.p, c->i_Jg.p, c->imu_scale, c->assembly(), c->lay,
+          inertial_hessian_mma_kernel<K, 4, K == 4 ? 8 : 12, DET, true><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->inertial.idx.p, c->i_out.r.p, c->i_out.Jp.p, c->i_out.wg.p,
+                                                                                                           c->i_out.wa.p, c->i_out.Jg.p, c->imu_scale, c->assembly(), c->lay,
                                                                                                            c->o_bg(), c->o_ba(), c->o_g(), splits, d, c->wt.p);
         else
-          inertial_hessian_mma_kernel<K, 4, K == 4 ? 8 : 12, DET, false><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->inertial.idx.p, c->i_r.p, c->i_Jp.p, c->i_wg.p, c->i_wa.p,
-                                                                                                            c->i_Jg.p, c->imu_scale, c->assembly(), c->lay, c->o_bg(), c->o_ba(),
+          inertial_hessian_mma_kernel<K, 4, K == 4 ? 8 : 12, DET, false><<<grid, kHessThreads, 0, side(c)>>>(c->run_off.p, c->inertial.idx.p, c->i_out.r.p, c->i_out.Jp.p, c->i_out.wg.p, c->i_out.wa.p,
+                                                                                                            c->i_out.Jg.p, c->imu_scale, c->assembly(), c->lay, c->o_bg(), c->o_ba(),
                                                                                                             c->o_g(), splits, d, nullptr);
         return check_launch(c, scalar_hess ? (DET ? "inertial_hessian_det_kernel" : "inertial_hessian_kernel")
                                            : (DET ? "inertial_hessian_mma_det_kernel" : "inertial_hessian_mma_kernel"));
@@ -774,7 +811,7 @@ int enqueue_build(hb200_ctx* c, const SolverState* st) {
     const int blocks = (c->Nm + kManWarps - 1) / kManWarps;
     const int rc = with_order(c->k, [&](auto K) {
       return with_flag(det, [&](auto DET) {
-        manifold_hessian_kernel<K, DET><<<blocks, kManWarps * 32, 0, side(c)>>>(c->Nm, c->manifold.idx.p, c->m_r.p, c->m_Jp.p, c->assembly(), c->lay,
+        manifold_hessian_kernel<K, DET><<<blocks, kManWarps * 32, 0, side(c)>>>(c->Nm, c->manifold.idx.p, c->m_out.r.p, c->m_out.Jp.p, c->assembly(), c->lay,
                                                                                DET ? c->det_man : DetOut{});
         return check_launch(c, DET ? "manifold_hessian_det_kernel" : "manifold_hessian_kernel");
       });
@@ -791,8 +828,8 @@ int enqueue_build(hb200_ctx* c, const SolverState* st) {
     const size_t smem = (3 * static_cast<size_t>(kSchurGroup) * (c->schur_rt + 1) + 3 * kSchurGroup + 4 * 3 * static_cast<size_t>(c->schur_rt)) * sizeof(double);
     const int rc = with_order(c->k, [&](auto K) {
       return with_flag(det, [&](auto DET) {
-        schur_group_kernel<K, DET><<<c->n_lm_groups, kSchurGThreads, smem, c->stream>>>(c->lm_group_off.p, c->lm_order.p, c->lm_off.p, c->lm_obs.p, c->visual.idx.p, c->v_r.p,
-                                                                                        c->v_Jp.p, c->v_Jl.p, c->v_w.p, st, c->assembly(), c->lay, c->Vchol.p, c->gl.p,
+        schur_group_kernel<K, DET><<<c->n_lm_groups, kSchurGThreads, smem, c->stream>>>(c->lm_group_off.p, c->lm_order.p, c->lm_off.p, c->lm_obs.p, c->visual.idx.p, c->v_out.r.p,
+                                                                                        c->v_out.Jp.p, c->v_out.Jl.p, c->v_out.w.p, st, c->assembly(), c->lay, c->Vchol.p, c->gl.p,
                                                                                         c->Dl.p, c->schur_rt, DET ? c->det_schur : DetOut{});
         return check_launch(c, DET ? "schur_group_det_kernel" : "schur_group_kernel");
       });
@@ -802,7 +839,7 @@ int enqueue_build(hb200_ctx* c, const SolverState* st) {
     const size_t smem = 2 * 3 * static_cast<size_t>(c->max_rows) * sizeof(double);
     const int rc = with_order(c->k, [&](auto K) {
       return with_flag(det, [&](auto DET) {
-        schur_kernel<K, DET><<<c->L, kSchurThreads, smem, c->stream>>>(c->lm_off.p, c->lm_obs.p, c->visual.idx.p, c->v_r.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p, st,
+        schur_kernel<K, DET><<<c->L, kSchurThreads, smem, c->stream>>>(c->lm_off.p, c->lm_obs.p, c->visual.idx.p, c->v_out.r.p, c->v_out.Jp.p, c->v_out.Jl.p, c->v_out.w.p, st,
                                                                        c->assembly(), c->lay, c->Vchol.p, c->gl.p, c->Dl.p, c->max_rows, DET ? c->det_schur : DetOut{});
         return check_launch(c, DET ? "schur_det_kernel" : "schur_kernel");
       });
@@ -948,7 +985,7 @@ int enqueue_solve(hb200_ctx* c, bool fuse_retract = false, bool* fused = nullptr
         if (fused) *fused = true;
       }
       const int rc = with_order(c->k, [&](auto K) {
-        lm_backsub_kernel<K><<<c->n_lm_blocks + extra, kLmWarps * 32, 0, c->stream>>>(c->L, c->lm_off.p, c->lm_obs.p, c->visual.idx.p, c->v_r.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p,
+        lm_backsub_kernel<K><<<c->n_lm_blocks + extra, kLmWarps * 32, 0, c->stream>>>(c->L, c->lm_off.p, c->lm_obs.p, c->visual.idx.p, c->v_out.r.p, c->v_out.Jp.p, c->v_out.Jl.p, c->v_out.w.p,
                                                                                  c->Vchol.p, c->gl.p, c->Dl.p, c->dp.p, c->dl.p, c->lm_part.p, c->lms[0].p, c->lms[1].p, c->n_lm_blocks, ra);
         return check_launch(c, "lm_backsub_kernel");
       });
@@ -1174,7 +1211,7 @@ int ensure_placeholders(hb200_ctx* c) {
     HB_CUDA(c->cp_pix[s].ensure(1)); HB_CUDA(c->cp_imu[s].ensure(1));
   }
   HB_CUDA(c->imu_tab.ensure(kImuStride)); HB_CUDA(c->cam_tab.ensure(kCamStride));
-  HB_CUDA(c->v_w.ensure(1)); HB_CUDA(c->sensors.ensure(7));
+  HB_CUDA(c->v_out.w.ensure(1)); HB_CUDA(c->sensors.ensure(7));
   HB_CUDA(c->visual.grow(1, 0, c->stream)); HB_CUDA(c->inertial.grow(1, 0, c->stream)); HB_CUDA(c->manifold.grow(1, 0, c->stream));
   HB_CUDA(c->visual_spare.grow(1, 0, c->stream)); HB_CUDA(c->inertial_spare.grow(1, 0, c->stream)); HB_CUDA(c->manifold_spare.grow(1, 0, c->stream));
   return 0;
@@ -1247,11 +1284,7 @@ void hb200_destroy(hb200_ctx* c) {
     if (c->peer_ptrs[p] && c->peer_ptrs[p] != c->mbox.p) cudaIpcCloseMemHandle(c->peer_ptrs[p]);
   c->peer_ptrs.clear();
   // the captured iteration references the communicator: NCCL waits in ncclCommDestroy until such graphs are gone
-  if (c->graph_exec) cudaGraphExecDestroy(c->graph_exec);
-  if (c->graph) cudaGraphDestroy(c->graph);
-  if (c->graph_exec_b) cudaGraphExecDestroy(c->graph_exec_b);
-  if (c->graph_b) cudaGraphDestroy(c->graph_b);
-  c->graph_exec = nullptr; c->graph = nullptr; c->graph_exec_b = nullptr; c->graph_b = nullptr;
+  for (IterationGraph& g : c->graphs) g.release();
   if (c->nccl && c->own_nccl && g_nccl.CommDestroy) g_nccl.CommDestroy(c->nccl);
   c->nccl = nullptr;
   for (cudaEvent_t e : c->prof_events) cudaEventDestroy(e);
@@ -1412,7 +1445,7 @@ int hb200_set_options(hb200_ctx* c, double huber_pixel, double imu_loss_scale, d
   if (!c) return fail(-1, "null context");
   if (!(huber_pixel > 0) || !(imu_loss_scale > 0) || !(radius > 0)) return fail(-1, "options must be positive");
   HB_CUDA(cudaSetDevice(c->device));
-  if (huber_pixel != c->huber || imu_loss_scale != c->imu_scale) c->graph_valid = false;  // baked into kernel arguments
+  if (huber_pixel != c->huber || imu_loss_scale != c->imu_scale) c->iterations_changed();  // baked into kernel arguments
   c->huber = huber_pixel; c->imu_scale = imu_loss_scale; c->radius0 = radius;
   c->outputs_changed();
   return reset_solver_state(c);
@@ -1544,7 +1577,7 @@ int hb200_set_weights(hb200_ctx* c, int kind, const double* W) {
 int hb200_set_bearing_loss(hb200_ctx* c, double huber_bearing) {
   if (!c) return fail(-1, "null context");
   if (!(huber_bearing > 0)) return fail(-1, "options must be positive");
-  if (huber_bearing != c->huber_bearing) c->graph_valid = false;
+  if (huber_bearing != c->huber_bearing) c->iterations_changed();
   c->huber_bearing = huber_bearing;
   c->outputs_changed();
   return 0;
@@ -1653,12 +1686,8 @@ int derive_window(hb200_ctx* c, int kind = 0) {
   const int rows = agree ? std::max(c->max_rows, 6 * (c->agreed_beta + 1)) : c->max_rows;
   if (2 * 3 * static_cast<size_t>(rows) * sizeof(double) > 200 * 1024) return fail(-6, "landmark track spans %d control-point dofs; exceeds the Schur kernel's shared-memory tile", rows);
   // outputs and launch shapes
-  const size_t k = c->k;
-  HB_CUDA(c->visual.grow(std::max(Nv, 1), Nv, c->stream)); HB_CUDA(c->v_w.ensure(std::max(Nv, 1)));
-  HB_CUDA(c->v_r.ensure(2 * static_cast<size_t>(std::max(Nv, 1)))); HB_CUDA(c->v_Jp.ensure(12 * k * std::max(Nv, 1))); HB_CUDA(c->v_Jl.ensure(6 * static_cast<size_t>(std::max(Nv, 1))));
-  HB_CUDA(c->i_r.ensure(6 * static_cast<size_t>(std::max(Ni, 1)))); HB_CUDA(c->i_Jp.ensure(36 * k * std::max(Ni, 1)));
-  HB_CUDA(c->i_wg.ensure(4 * static_cast<size_t>(std::max(Ni, 1)))); HB_CUDA(c->i_wa.ensure(4 * static_cast<size_t>(std::max(Ni, 1)))); HB_CUDA(c->i_Jg.ensure(12 * static_cast<size_t>(std::max(Ni, 1))));
-  HB_CUDA(c->m_r.ensure(6 * static_cast<size_t>(std::max(Nm, 1)))); HB_CUDA(c->m_Jp.ensure(36 * k * std::max(Nm, 1)));
+  HB_CUDA(c->visual.grow(std::max(Nv, 1), Nv, c->stream));
+  HB_CUDA(c->v_out.ensure(Nv, c->k)); HB_CUDA(c->i_out.ensure(Ni, c->k)); HB_CUDA(c->m_out.ensure(Nm, c->k));
   c->n_pix_blocks = (Nv + kEvalThreads - 1) / kEvalThreads;
   c->n_imu_blocks = (Ni + kEvalThreads - 1) / kEvalThreads;
   c->n_man_blocks = (Nm + kEvalThreads - 1) / kEvalThreads;
@@ -1841,56 +1870,46 @@ int hb200_evaluate(hb200_ctx* c, int flags) {
   return 0;
 }
 
-int hb200_get_pixel_outputs(hb200_ctx* c, double* r, double* Jp, double* Jl) {
+namespace {
+// Where read_visual_outputs writes one visual kind's outputs in user order (null: not wanted).
+struct VisualDest { double *r, *Jp, *Jl; };
+// The outputs of the pixel factors (dst[0]) and the bearing factors (dst[1]) from one read-back of the visual list.  A
+// bearing factor fills the first row of its 2-row slot.
+int read_visual_outputs(hb200_ctx* c, const VisualDest (&dst)[2]) {
   if (!c || !c->bound) return fail(-2, "not bound");
   { const int rs = ensure_perms(c); if (rs) return rs; }
   HB_CUDA(cudaSetDevice(c->device));
-  const size_t N = c->Nv, w = 12 * static_cast<size_t>(c->k);
-  std::vector<double> tr(2 * N), tJ(Jp ? w * N : 0), tl(Jl ? 6 * N : 0);
-  if (N) {
-    HB_CUDA(cudaMemcpyAsync(tr.data(), c->v_r.p, sizeof(double) * 2 * N, cudaMemcpyDeviceToHost, c->stream));
-    if (Jp) HB_CUDA(cudaMemcpyAsync(tJ.data(), c->v_Jp.p, sizeof(double) * w * N, cudaMemcpyDeviceToHost, c->stream));
-    if (Jl) HB_CUDA(cudaMemcpyAsync(tl.data(), c->v_Jl.p, sizeof(double) * 6 * N, cudaMemcpyDeviceToHost, c->stream));
-  }
+  const size_t N = c->Nv, w = 6 * static_cast<size_t>(c->k);   // w: one row of a state Jacobian
+  if (N == 0) return 0;
+  const bool Jp = dst[0].Jp || dst[1].Jp, Jl = dst[0].Jl || dst[1].Jl;
+  std::vector<double> tr(2 * N), tJ(Jp ? 2 * w * N : 0), tl(Jl ? 6 * N : 0);
+  HB_CUDA(cudaMemcpyAsync(tr.data(), c->v_out.r.p, sizeof(double) * 2 * N, cudaMemcpyDeviceToHost, c->stream));
+  if (Jp) HB_CUDA(cudaMemcpyAsync(tJ.data(), c->v_out.Jp.p, sizeof(double) * 2 * w * N, cudaMemcpyDeviceToHost, c->stream));
+  if (Jl) HB_CUDA(cudaMemcpyAsync(tl.data(), c->v_out.Jl.p, sizeof(double) * 6 * N, cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
   for (size_t p = 0; p < N; ++p) {
-    const size_t u = c->v_perm[p];
-    if (u >= static_cast<size_t>(c->Np)) continue;   // bearing factor
-    if (r) { r[2 * u] = tr[2 * p]; r[2 * u + 1] = tr[2 * p + 1]; }
-    if (Jp) std::memcpy(Jp + w * u, tJ.data() + w * p, sizeof(double) * w);
-    if (Jl) std::memcpy(Jl + 6 * u, tl.data() + 6 * p, sizeof(double) * 6);
+    const int b = c->v_perm[p] >= c->Np ? 1 : 0;   // pixel factors 0 .. Np-1, bearing factors after
+    const size_t u = c->v_perm[p] - b * c->Np, rows = 2 - b;
+    const VisualDest& d = dst[b];
+    if (d.r) std::memcpy(d.r + rows * u, tr.data() + 2 * p, sizeof(double) * rows);
+    if (d.Jp) std::memcpy(d.Jp + rows * w * u, tJ.data() + 2 * w * p, sizeof(double) * rows * w);
+    if (d.Jl) std::memcpy(d.Jl + 3 * rows * u, tl.data() + 6 * p, sizeof(double) * 3 * rows);
   }
   return 0;
 }
+}  // namespace
 
-int hb200_get_bearing_outputs(hb200_ctx* c, double* r, double* Jp, double* Jl) {
-  if (!c || !c->bound) return fail(-2, "not bound");
-  { const int rs = ensure_perms(c); if (rs) return rs; }
-  HB_CUDA(cudaSetDevice(c->device));
-  const size_t N = c->Nv, w = 12 * static_cast<size_t>(c->k);
-  if (c->Nb == 0) return 0;
-  std::vector<double> tr(2 * N), tJ(Jp ? w * N : 0), tl(Jl ? 6 * N : 0);
-  HB_CUDA(cudaMemcpyAsync(tr.data(), c->v_r.p, sizeof(double) * 2 * N, cudaMemcpyDeviceToHost, c->stream));
-  if (Jp) HB_CUDA(cudaMemcpyAsync(tJ.data(), c->v_Jp.p, sizeof(double) * w * N, cudaMemcpyDeviceToHost, c->stream));
-  if (Jl) HB_CUDA(cudaMemcpyAsync(tl.data(), c->v_Jl.p, sizeof(double) * 6 * N, cudaMemcpyDeviceToHost, c->stream));
-  HB_CUDA(cudaStreamSynchronize(c->stream));
-  for (size_t p = 0; p < N; ++p) {
-    if (c->v_perm[p] < c->Np) continue;
-    const size_t u = c->v_perm[p] - c->Np;   // first row of the 2-row slot carries the angular residual
-    if (r) r[u] = tr[2 * p];
-    if (Jp) std::memcpy(Jp + (w / 2) * u, tJ.data() + w * p, sizeof(double) * (w / 2));
-    if (Jl) std::memcpy(Jl + 3 * u, tl.data() + 6 * p, sizeof(double) * 3);
-  }
-  return 0;
-}
+int hb200_get_pixel_outputs(hb200_ctx* c, double* r, double* Jp, double* Jl) { return read_visual_outputs(c, {{r, Jp, Jl}, {}}); }
+
+int hb200_get_bearing_outputs(hb200_ctx* c, double* r, double* Jp, double* Jl) { return read_visual_outputs(c, {{}, {r, Jp, Jl}}); }
 
 int hb200_get_manifold_outputs(hb200_ctx* c, double* r, double* Jp) {
   if (!c || !c->bound) return fail(-2, "not bound");
   HB_CUDA(cudaSetDevice(c->device));
   const size_t N = c->Nm, w = 36 * static_cast<size_t>(c->k);
   if (N == 0) return 0;
-  if (r) HB_CUDA(cudaMemcpyAsync(r, c->m_r.p, sizeof(double) * 6 * N, cudaMemcpyDeviceToHost, c->stream));
-  if (Jp) HB_CUDA(cudaMemcpyAsync(Jp, c->m_Jp.p, sizeof(double) * w * N, cudaMemcpyDeviceToHost, c->stream));
+  if (r) HB_CUDA(cudaMemcpyAsync(r, c->m_out.r.p, sizeof(double) * 6 * N, cudaMemcpyDeviceToHost, c->stream));
+  if (Jp) HB_CUDA(cudaMemcpyAsync(Jp, c->m_out.Jp.p, sizeof(double) * w * N, cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
   return 0;
 }
@@ -1900,14 +1919,13 @@ int hb200_get_inertial_outputs(hb200_ctx* c, double* r, double* Jp, double* wg, 
   { const int rs = ensure_perms(c); if (rs) return rs; }
   HB_CUDA(cudaSetDevice(c->device));
   const size_t N = c->Ni, w = 36 * static_cast<size_t>(c->k);
+  if (N == 0) return 0;
   std::vector<double> tr(6 * N), tJ(Jp ? w * N : 0), tg(wg ? 4 * N : 0), ta(wa ? 4 * N : 0), tG(Jg ? 12 * N : 0);
-  if (N) {
-    HB_CUDA(cudaMemcpyAsync(tr.data(), c->i_r.p, sizeof(double) * 6 * N, cudaMemcpyDeviceToHost, c->stream));
-    if (Jp) HB_CUDA(cudaMemcpyAsync(tJ.data(), c->i_Jp.p, sizeof(double) * w * N, cudaMemcpyDeviceToHost, c->stream));
-    if (wg) HB_CUDA(cudaMemcpyAsync(tg.data(), c->i_wg.p, sizeof(double) * 4 * N, cudaMemcpyDeviceToHost, c->stream));
-    if (wa) HB_CUDA(cudaMemcpyAsync(ta.data(), c->i_wa.p, sizeof(double) * 4 * N, cudaMemcpyDeviceToHost, c->stream));
-    if (Jg) HB_CUDA(cudaMemcpyAsync(tG.data(), c->i_Jg.p, sizeof(double) * 12 * N, cudaMemcpyDeviceToHost, c->stream));
-  }
+  HB_CUDA(cudaMemcpyAsync(tr.data(), c->i_out.r.p, sizeof(double) * 6 * N, cudaMemcpyDeviceToHost, c->stream));
+  if (Jp) HB_CUDA(cudaMemcpyAsync(tJ.data(), c->i_out.Jp.p, sizeof(double) * w * N, cudaMemcpyDeviceToHost, c->stream));
+  if (wg) HB_CUDA(cudaMemcpyAsync(tg.data(), c->i_out.wg.p, sizeof(double) * 4 * N, cudaMemcpyDeviceToHost, c->stream));
+  if (wa) HB_CUDA(cudaMemcpyAsync(ta.data(), c->i_out.wa.p, sizeof(double) * 4 * N, cudaMemcpyDeviceToHost, c->stream));
+  if (Jg) HB_CUDA(cudaMemcpyAsync(tG.data(), c->i_out.Jg.p, sizeof(double) * 12 * N, cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
   for (size_t p = 0; p < N; ++p) {
     const size_t u = c->i_perm[p];
@@ -1924,15 +1942,17 @@ int hb200_get_inertial_outputs(hb200_ctx* c, double* r, double* Jp, double* wg, 
 
 namespace {
 // rows of a tangent-space SE3 Jacobian [d/dtheta | d/drho] -> ambient [q(4) | p(3)] through the SE3JacobianAdapter
-// (reference pixel.cpp:141, inertial.cpp:161): J_theta A_q(q) | J_rho
-void tangent_to_ambient_se3(const double* Jt, int ld, int rows, const double* T, double* out /*rows x 7*/) {
+// (reference pixel.cpp:141, inertial.cpp:161): J_theta A_q(q) | J_rho, in output rows of ld_out >= 7 doubles (zero after
+// the seventh)
+void tangent_to_ambient_se3(const double* Jt, int ld, int rows, const double* T, double* out, int ld_out = 7) {
   const double* q = T;
   const double Aq[12] = {2 * q[3], -2 * q[2], 2 * q[1], -2 * q[0], 2 * q[2], 2 * q[3], -2 * q[0], -2 * q[1], -2 * q[1], 2 * q[0], 2 * q[3], -2 * q[2]};
   for (int row = 0; row < rows; ++row) {
     const double* jt = Jt + static_cast<size_t>(ld) * row;
-    double* o = out + 7 * row;
+    double* o = out + static_cast<size_t>(ld_out) * row;
     for (int col = 0; col < 4; ++col) o[col] = jt[0] * Aq[col] + jt[1] * Aq[4 + col] + jt[2] * Aq[8 + col];
     o[4] = jt[3]; o[5] = jt[4]; o[6] = jt[5];
+    std::fill(o + 7, o + ld_out, 0.0);
   }
 }
 
@@ -1942,7 +1962,9 @@ int ensure_calib_mirror(hb200_ctx* c) {
   const size_t Nv = c->Nv, Ni = c->Ni, Nm = c->Nm;
   DevBuf<double> dv, di, dm;
   std::vector<double> tv(28 * Nv), ti(216 * Ni);
-  c->m_v_Jc.assign(28 * Nv, 0.0); c->m_i_Jc.assign(216 * Ni, 0.0); c->m_m_Jc.assign(36 * Nm, 0.0);
+  std::vector<double>* Jc = c->mirror.Jc;   // user order: [Np], [Nb] ([2][14] each), [Ni][6][36], [Nm][6][6]
+  Jc[HB200_PIXEL].assign(28 * static_cast<size_t>(c->Np), 0.0); Jc[HB200_BEARING].assign(28 * static_cast<size_t>(c->Nb), 0.0);
+  Jc[HB200_INERTIAL].assign(216 * Ni, 0.0); Jc[HB200_MANIFOLD].assign(36 * Nm, 0.0);
   if (Nv) {
     HB_CUDA(dv.ensure(28 * Nv));
     const int blocks = static_cast<int>((Nv + kEvalThreads - 1) / kEvalThreads);
@@ -1979,12 +2001,13 @@ int ensure_calib_mirror(hb200_ctx* c) {
       });
     });
     if (rc) return rc;
-    HB_CUDA(cudaMemcpyAsync(c->m_m_Jc.data(), dm.p, sizeof(double) * 36 * Nm, cudaMemcpyDeviceToHost, c->stream));
+    HB_CUDA(cudaMemcpyAsync(Jc[HB200_MANIFOLD].data(), dm.p, sizeof(double) * 36 * Nm, cudaMemcpyDeviceToHost, c->stream));
   }
   HB_CUDA(cudaStreamSynchronize(c->stream));
-  for (size_t p = 0; p < Nv; ++p) std::memcpy(&c->m_v_Jc[28 * static_cast<size_t>(c->v_perm[p])], &tv[28 * p], 28 * sizeof(double));   // pixel [0, Np), bearing after
-  for (size_t p = 0; p < Ni; ++p) std::memcpy(&c->m_i_Jc[216 * static_cast<size_t>(c->i_perm[p])], &ti[216 * p], 216 * sizeof(double));
-  c->calib_valid = true;
+  for (size_t p = 0; p < Nv; ++p)   // pixel factors 0 .. Np-1, bearing factors after
+    std::memcpy(c->v_perm[p] < c->Np ? &Jc[HB200_PIXEL][28 * c->v_perm[p]] : &Jc[HB200_BEARING][28 * (c->v_perm[p] - c->Np)], &tv[28 * p], 28 * sizeof(double));
+  for (size_t p = 0; p < Ni; ++p) std::memcpy(&Jc[HB200_INERTIAL][216 * static_cast<size_t>(c->i_perm[p])], &ti[216 * p], 216 * sizeof(double));
+  c->mirror.calib_valid = true;
   return 0;
 }
 }  // namespace
@@ -1996,60 +2019,47 @@ int hb200_factor_evaluate(hb200_ctx* c, int kind, int index, const double* const
   if (!c->evaluated_J) return fail(-2, "call hb200_evaluate(HB200_EVAL_JACOBIANS) first");
   if (!parameters || !residuals) return fail(-1, "null argument");
   { const int rs = ensure_perms(c); if (rs) return rs; }
-  if (!c->mirror_valid) {
-    const size_t k = c->k;
-    c->m_v_r.resize(2 * static_cast<size_t>(c->Np)); c->m_v_Jp.resize(12 * k * c->Np); c->m_v_Jl.resize(6 * static_cast<size_t>(c->Np));
-    c->m_b_r.resize(c->Nb); c->m_b_Jp.resize(6 * k * c->Nb); c->m_b_Jl.resize(3 * static_cast<size_t>(c->Nb));
-    c->m_m_r.resize(6 * static_cast<size_t>(c->Nm)); c->m_m_Jp.resize(36 * k * c->Nm);
-    c->m_i_r.resize(6 * static_cast<size_t>(c->Ni)); c->m_i_Jp.resize(36 * k * c->Ni); c->m_i_wg.resize(4 * static_cast<size_t>(c->Ni));
-    c->m_i_wa.resize(4 * static_cast<size_t>(c->Ni)); c->m_i_Jg.resize(12 * static_cast<size_t>(c->Ni)); c->m_grav.resize(3);
-    int rc = hb200_get_pixel_outputs(c, c->m_v_r.data(), c->m_v_Jp.data(), c->m_v_Jl.data());
+  OutputMirror& mir = c->mirror;
+  const int nrs[4] = {2, 6, 1, 6};
+  const int Ns[4] = {c->Np, c->Ni, c->Nb, c->Nm};
+  if (!mir.valid) {
+    const size_t k = c->k, Ni = c->Ni;
+    for (int f = HB200_PIXEL; f <= HB200_MANIFOLD; ++f) {
+      mir.r[f].resize(static_cast<size_t>(nrs[f]) * Ns[f]);
+      mir.Jp[f].resize(6 * k * nrs[f] * Ns[f]);
+    }
+    for (int f : {HB200_PIXEL, HB200_BEARING}) mir.Jl[f].resize(3 * static_cast<size_t>(nrs[f]) * Ns[f]);
+    mir.wg.resize(4 * Ni); mir.wa.resize(4 * Ni); mir.Jg.resize(12 * Ni);
+    auto visual = [&](int f) { return VisualDest{mir.r[f].data(), mir.Jp[f].data(), mir.Jl[f].data()}; };
+    int rc = read_visual_outputs(c, {visual(HB200_PIXEL), visual(HB200_BEARING)});
+    if (!rc) rc = hb200_get_inertial_outputs(c, mir.r[HB200_INERTIAL].data(), mir.Jp[HB200_INERTIAL].data(), mir.wg.data(), mir.wa.data(), mir.Jg.data());
+    if (!rc) rc = hb200_get_manifold_outputs(c, mir.r[HB200_MANIFOLD].data(), mir.Jp[HB200_MANIFOLD].data());
     if (rc) return rc;
-    rc = hb200_get_inertial_outputs(c, c->m_i_r.data(), c->m_i_Jp.data(), c->m_i_wg.data(), c->m_i_wa.data(), c->m_i_Jg.data());
-    if (rc) return rc;
-    rc = hb200_get_bearing_outputs(c, c->m_b_r.data(), c->m_b_Jp.data(), c->m_b_Jl.data());
-    if (rc) return rc;
-    rc = hb200_get_manifold_outputs(c, c->m_m_r.data(), c->m_m_Jp.data());
-    if (rc) return rc;
-    HB_CUDA(cudaMemcpy(c->m_grav.data(), c->grav[0].p, 3 * sizeof(double), cudaMemcpyDeviceToHost));
-    c->mirror_valid = true;
+    mir.valid = true;
   }
   const int k = c->k, kb = c->kb;
   if (kind < HB200_PIXEL || kind > HB200_MANIFOLD) return fail(-1, "unknown factor kind %d", kind);
-  if (jacobians && !c->calib_valid) {
+  if (jacobians && !mir.calib_valid) {
     // calibration blocks requested?  (constant in the live configuration, so they are produced on demand only)
     const int first = k, count = (kind == HB200_INERTIAL) ? 5 : (kind == HB200_MANIFOLD ? 1 : 3);
     bool want = false;
     for (int b = 0; b < count; ++b) want = want || jacobians[first + b] != nullptr;
     if (want) { const int rc = ensure_calib_mirror(c); if (rc) return rc; }
   }
-  const int nrs[4] = {2, 6, 1, 6};
-  const int Ns[4] = {c->Np, c->Ni, c->Nb, c->Nm};
   const int nr = nrs[kind], N = Ns[kind];
   if (index < 0 || index >= N) return fail(-1, "factor index %d out of range", index);
-  const double* rs[4] = {c->m_v_r.data(), c->m_i_r.data(), c->m_b_r.data(), c->m_m_r.data()};
-  const double* Js[4] = {c->m_v_Jp.data(), c->m_i_Jp.data(), c->m_b_Jp.data(), c->m_m_Jp.data()};
-  const double* r = rs[kind] + static_cast<size_t>(nr) * index;
+  const double* r = mir.r[kind].data() + static_cast<size_t>(nr) * index;
   for (int i = 0; i < nr; ++i) residuals[i] = r[i];
   if (!jacobians) return 0;
-  const double* Jp = Js[kind] + static_cast<size_t>(nr) * 6 * k * index;
+  const double* Jp = mir.Jp[kind].data() + static_cast<size_t>(nr) * 6 * k * index;
   // state blocks: [J_theta * A_q(q_m) | J_rho | 0]  (ambient 8, row-major nr x 8)
-  for (int m = 0; m < k; ++m) {
-    if (!jacobians[m]) continue;
-    const double* q = parameters[m];
-    const double Aq[12] = {2 * q[3], -2 * q[2], 2 * q[1], -2 * q[0], 2 * q[2], 2 * q[3], -2 * q[0], -2 * q[1], -2 * q[1], 2 * q[0], 2 * q[3], -2 * q[2]};
-    for (int row = 0; row < nr; ++row) {
-      const double* jt = Jp + row * 6 * k + 6 * m;
-      double* o = jacobians[m] + 8 * row;
-      for (int col = 0; col < 4; ++col) o[col] = jt[0] * Aq[col] + jt[1] * Aq[4 + col] + jt[2] * Aq[8 + col];
-      o[4] = jt[3]; o[5] = jt[4]; o[6] = jt[5]; o[7] = 0.0;
-    }
-  }
+  for (int m = 0; m < k; ++m)
+    if (jacobians[m]) tangent_to_ambient_se3(Jp + 6 * m, 6 * k, nr, parameters[m], jacobians[m], 8);
   if (kind == HB200_PIXEL || kind == HB200_BEARING) {
     const int sizes[4] = {7, 4, 4, 3};
-    const double* Jl = (kind == HB200_PIXEL) ? &c->m_v_Jl[6 * static_cast<size_t>(index)] : &c->m_b_Jl[3 * static_cast<size_t>(index)];
+    const double* Jl = mir.Jl[kind].data() + 3 * static_cast<size_t>(nr) * index;
     // calibration blocks (reference pixel.cpp:91-135,141; bearing.cpp:76): rows of [T_bs tangent 6 | intrinsics 4 | distortion 4]
-    const double* Jc = &c->m_v_Jc[28 * static_cast<size_t>(kind == HB200_PIXEL ? index : c->Np + index)];
+    const double* Jc = mir.Jc[kind].data() + 28 * static_cast<size_t>(index);
     const int coff[3] = {0, 6, 10};
     for (int b = 0; b < 4; ++b) {
       double* o = jacobians[k + b];
@@ -2059,12 +2069,12 @@ int hb200_factor_evaluate(hb200_ctx* c, int kind, int index, const double* const
       else std::memcpy(o, Jl, 3 * nr * sizeof(double));
     }
   } else if (kind == HB200_MANIFOLD) {
-    if (jacobians[k]) tangent_to_ambient_se3(&c->m_m_Jc[36 * static_cast<size_t>(index)], 6, 6, parameters[k], jacobians[k]);   // reference manifold.cpp:57
+    if (jacobians[k]) tangent_to_ambient_se3(mir.Jc[kind].data() + 36 * static_cast<size_t>(index), 6, 6, parameters[k], jacobians[k]);   // reference manifold.cpp:57
   } else {
     // reference inertial.cpp:155-194: rows of [T_bs tangent 6 | i_g 6 | i_a 6 | S_g 9 | X_a 9]
     const int sizes[5] = {7, 6, 6, 9, 9};
     const int coff[5] = {0, 6, 12, 18, 27};
-    const double* Jc = &c->m_i_Jc[216 * static_cast<size_t>(index)];
+    const double* Jc = mir.Jc[kind].data() + 216 * static_cast<size_t>(index);
     for (int b = 0; b < 5; ++b) {
       double* o = jacobians[k + b];
       if (!o) continue;
@@ -2076,13 +2086,13 @@ int hb200_factor_evaluate(hb200_ctx* c, int kind, int index, const double* const
     for (int m = 0; m < kb; ++m) {
       if (double* o = jacobians[k + 5 + m]) {
         std::fill(o, o + 24, 0.0);
-        const double wv = c->m_i_wg[4 * static_cast<size_t>(index) + m];
+        const double wv = mir.wg[4 * static_cast<size_t>(index) + m];
         if (c->wt_set[HB200_INERTIAL]) { for (int row = 0; row < 6; ++row) for (int a = 0; a < 3; ++a) o[4 * row + a] = wv * W[6 * row + a]; }
         else for (int a = 0; a < 3; ++a) o[4 * a + a] = wv;
       }
       if (double* o = jacobians[k + 5 + kb + m]) {
         std::fill(o, o + 24, 0.0);
-        const double wv = c->m_i_wa[4 * static_cast<size_t>(index) + m];
+        const double wv = mir.wa[4 * static_cast<size_t>(index) + m];
         if (c->wt_set[HB200_INERTIAL]) { for (int row = 0; row < 6; ++row) for (int a = 0; a < 3; ++a) o[4 * row + a] = wv * W[6 * row + 3 + a]; }
         else for (int a = 0; a < 3; ++a) o[4 * (3 + a) + a] = wv;
       }
@@ -2102,7 +2112,7 @@ int hb200_factor_evaluate(hb200_ctx* c, int kind, int index, const double* const
       const double nx = std::sqrt(sigma + x[2] * x[2]);
       double PJ[6];
       for (int cc = 0; cc < 2; ++cc) for (int rr = 0; rr < 3; ++rr) PJ[2 * rr + cc] = nx * ((rr == cc ? 1.0 : 0.0) - beta * v[cc] * v[rr]);
-      const double* Jg = &c->m_i_Jg[12 * static_cast<size_t>(index)];
+      const double* Jg = &mir.Jg[12 * static_cast<size_t>(index)];
       for (int row = 0; row < 6; ++row)
         for (int col = 0; col < 3; ++col) o[3 * row + col] = (Jg[2 * row] * PJ[2 * col] + Jg[2 * row + 1] * PJ[2 * col + 1]) / (nx * nx);
     }
@@ -2220,7 +2230,7 @@ bool cov_request_ok(const int4& r, const CovPoint& pt) {
 // landmarks and of the pairs' stamps (one read-back, only when a request has a landmark or a pair is registered), the
 // far-column plan -- for every knot pair more than beta blocks apart that a request or a pair reads, directly or through
 // a span, its column (the larger block) and the lowest row the march must reach -- then cov_far_column_kernel over the
-// planned columns, cov_cross_landmark_kernel over the requests and cov_pose_pair_kernel over the pairs, into *_next.
+// planned columns, cov_cross_landmark_kernel over the requests and cov_pose_pair_kernel over the pairs, into cov_next.
 // A column's values do not depend on its lowest row, so the requests' blocks are the same with or without pairs.
 int cov_blocks_enqueue(hb200_ctx* c, const CovPoint& pt) {
   const SysLayout& lay = pt.lay;
@@ -2285,30 +2295,31 @@ int cov_blocks_enqueue(hb200_ctx* c, const CovPoint& pt) {
   HB_CUDA(c->cov_plan.ensure(plan.size()));
   HB_CUDA(cudaMemcpyAsync(c->cov_plan.p, plan.data(), sizeof(int) * plan.size(), cudaMemcpyHostToDevice, c->stream));
   HB_CUDA(c->cov_far.ensure(36 * static_cast<size_t>(blocks)));
-  HB_CUDA(c->cov_blk_next.ensure(36 * static_cast<size_t>(n)));
-  HB_CUDA(c->cov_blk_st_next.ensure(n));
+  CovResults& next = c->cov_next;
+  HB_CUDA(next.blk.ensure(36 * static_cast<size_t>(n)));
+  HB_CUDA(next.blk_st.ensure(n));
   const CovFarPlan fp{c->cov_plan.p, nc};
   if (nc) {
     const size_t smem = (36 * static_cast<size_t>(beta) + 6 * lay.m + 36) * sizeof(double);
-    cov_far_column_kernel<<<nc, kFarThreads, smem, c->stream>>>(c->cov_ws.p, c->cov_packed_next.p, lay, c->fixed.p, fp, c->cov_status.p, c->cov_far.p);
+    cov_far_column_kernel<<<nc, kFarThreads, smem, c->stream>>>(c->cov_ws.p, next.packed.p, lay, c->fixed.p, fp, c->cov_status.p, c->cov_far.p);
     HB_LAUNCH(c, "cov_far_column_kernel");
   }
-  HB_CUDA(c->cov_pair_joint_next.ensure(144 * static_cast<size_t>(npair)));
-  HB_CUDA(c->cov_pair_rel_next.ensure(36 * static_cast<size_t>(npair)));
-  HB_CUDA(c->cov_pair_st_next.ensure(npair));
+  HB_CUDA(next.pair_joint.ensure(144 * static_cast<size_t>(npair)));
+  HB_CUDA(next.pair_rel.ensure(36 * static_cast<size_t>(npair)));
+  HB_CUDA(next.pair_st.ensure(npair));
   const size_t smem = static_cast<size_t>(kLmWarps) * 6 * pt.max_rows * sizeof(double);
   return with_order(pt.k, [&](auto Kc) {
     if (n) {
       HB_CUDA(cudaFuncSetAttribute(cov_cross_landmark_kernel<Kc>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
       cov_cross_landmark_kernel<Kc><<<(n + kLmWarps - 1) / kLmWarps, kLmWarps * 32, smem, c->stream>>>(
-          n, c->cov_req_d.p, c->lm_off.p, c->lm_obs.p, c->visual.idx.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p, c->Vchol.p, c->cov_packed_next.p, c->cov_lm_next.p,
-          c->cov_far.p, fp, lay, pt.Kbg, c->multi() ? 1 : 0, c->cov_status.p, pt.max_rows, c->cov_blk_next.p, c->cov_blk_st_next.p);
+          n, c->cov_req_d.p, c->lm_off.p, c->lm_obs.p, c->visual.idx.p, c->v_out.Jp.p, c->v_out.Jl.p, c->v_out.w.p, c->Vchol.p, next.packed.p, next.lm.p,
+          c->cov_far.p, fp, lay, pt.Kbg, c->multi() ? 1 : 0, c->cov_status.p, pt.max_rows, next.blk.p, next.blk_st.p);
       if (const int rc = check_launch(c, "cov_cross_landmark_kernel")) return rc;
     }
     if (npair) {
       cov_pose_pair_kernel<Kc><<<(npair + kPairWarps - 1) / kPairWarps, kPairWarps * 32, 0, c->stream>>>(
-          npair, c->cov_pairs_d.p, c->cov_span.p + 2 * n, pt.tab.p, pt.basis, c->cov_packed_next.p, c->cov_far.p, fp, lay, c->cov_status.p,
-          c->cov_pair_joint_next.p, c->cov_pair_rel_next.p, c->cov_pair_st_next.p);
+          npair, c->cov_pairs_d.p, c->cov_span.p + 2 * n, pt.tab.p, pt.basis, next.packed.p, c->cov_far.p, fp, lay, c->cov_status.p,
+          next.pair_joint.p, next.pair_rel.p, next.pair_st.p);
       if (const int rc = check_launch(c, "cov_pose_pair_kernel")) return rc;
     }
     return 0;
@@ -2400,24 +2411,27 @@ int hb200_compute_covariance(hb200_ctx* c, hb200_covariance_info* info) {
   const SysLayout& lay = pt.lay;
   const size_t smem = cov_smem_doubles(lay.beta, lay.m) * sizeof(double);
   HB_CUDA(c->cov_ws.ensure(static_cast<size_t>(cov_workspace_doubles(lay))));
-  HB_CUDA(c->cov_packed_next.ensure(static_cast<size_t>(cov_packed_doubles(lay))));
   const int L = pt.L, k = pt.k, max_rows = pt.max_rows;   // (the build's shapes)
-  HB_CUDA(c->cov_lm_next.ensure(9 * static_cast<size_t>(std::max(L, 1))));
+  CovResults& next = c->cov_next;
+  HB_CUDA(next.packed.ensure(static_cast<size_t>(cov_packed_doubles(lay))));
+  HB_CUDA(next.lm.ensure(9 * static_cast<size_t>(std::max(L, 1))));
+  next.blk_n = static_cast<int>(c->cov_req.size());
+  next.pair_n = static_cast<int>(c->cov_pairs.size() / 2);
   HB_CUDA(c->cov_status.ensure(1));
   HB_CUDA(cudaFuncSetAttribute(cov_selinv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-  cov_selinv_kernel<<<1, kCovThreads, smem, c->stream>>>(c->sys.p, lay, c->fixed.p, c->cov_ws.p, c->cov_packed_next.p, c->cov_status.p);
+  cov_selinv_kernel<<<1, kCovThreads, smem, c->stream>>>(c->sys.p, lay, c->fixed.p, c->cov_ws.p, next.packed.p, c->cov_status.p);
   HB_LAUNCH(c, "cov_selinv_kernel");
   if (L && pt.Nv) {
     const int blocks = (L + kLmWarps - 1) / kLmWarps;
     const size_t lsmem = static_cast<size_t>(kLmWarps) * 3 * max_rows * sizeof(double);
     const int rc = with_order(k, [&](auto K) {
-      cov_landmark_kernel<K><<<blocks, kLmWarps * 32, lsmem, c->stream>>>(L, c->lm_off.p, c->lm_obs.p, c->visual.idx.p, c->v_Jp.p, c->v_Jl.p, c->v_w.p, c->Vchol.p,
-                                                                         c->cov_packed_next.p, lay, c->cov_status.p, c->cov_lm_next.p, max_rows);
+      cov_landmark_kernel<K><<<blocks, kLmWarps * 32, lsmem, c->stream>>>(L, c->lm_off.p, c->lm_obs.p, c->visual.idx.p, c->v_out.Jp.p, c->v_out.Jl.p, c->v_out.w.p, c->Vchol.p,
+                                                                         next.packed.p, lay, c->cov_status.p, next.lm.p, max_rows);
       return check_launch(c, "cov_landmark_kernel");
     });
     if (rc) return rc;
   } else if (L) {
-    HB_CUDA(cudaMemsetAsync(c->cov_lm_next.p, 0, sizeof(double) * 9 * L, c->stream));
+    HB_CUDA(cudaMemsetAsync(next.lm.p, 0, sizeof(double) * 9 * L, c->stream));
   }
   // requested blocks and stamp pairs: the landmark blocks need the build's factor outputs and the far columns the factor
   // in cov_ws, both valid only until the next launch, so they are computed here (nothing runs without a request or pair)
@@ -2436,15 +2450,7 @@ int hb200_compute_covariance(hb200_ctx* c, hb200_covariance_info* info) {
                 st.min_pivot, st.bad_dof, kCovMinPivot);
   }
   // commit: results, and the linearisation point they belong to
-  c->cov_packed.swap(c->cov_packed_next);
-  c->cov_lm.swap(c->cov_lm_next);
-  c->cov_blk.swap(c->cov_blk_next);
-  c->cov_blk_st.swap(c->cov_blk_st_next);
-  c->cov_blk_n = static_cast<int>(c->cov_req.size());
-  c->cov_pair_joint.swap(c->cov_pair_joint_next);
-  c->cov_pair_rel.swap(c->cov_pair_rel_next);
-  c->cov_pair_st.swap(c->cov_pair_st_next);
-  c->cov_pair_n = static_cast<int>(c->cov_pairs.size() / 2);
+  c->cov_res.swap(next);
   c->cov_slot_committed = c->cov_slot_built;
   c->cov_valid = true;
   cov_info(c, info);
@@ -2466,11 +2472,11 @@ int hb200_get_covariance_blocks(hb200_ctx* c, int n, double* out, int* status) {
   if (!c) return fail(-1, "null context");
   if (n < 0 || (n > 0 && !out)) return fail(-1, "invalid argument");
   if (!c->cov_valid) return fail(-2, "no covariance computed (hb200_compute_covariance has not succeeded)");
-  if (n != c->cov_blk_n) return fail(-2, "the last successful compute had %d covariance blocks, not %d", c->cov_blk_n, n);
+  if (n != c->cov_res.blk_n) return fail(-2, "the last successful compute had %d covariance blocks, not %d", c->cov_res.blk_n, n);
   if (n == 0) return 0;
   HB_CUDA(cudaSetDevice(c->device));
-  HB_CUDA(cudaMemcpyAsync(out, c->cov_blk.p, sizeof(double) * 36 * n, cudaMemcpyDeviceToHost, c->stream));
-  if (status) HB_CUDA(cudaMemcpyAsync(status, c->cov_blk_st.p, sizeof(int) * n, cudaMemcpyDeviceToHost, c->stream));
+  HB_CUDA(cudaMemcpyAsync(out, c->cov_res.blk.p, sizeof(double) * 36 * n, cudaMemcpyDeviceToHost, c->stream));
+  if (status) HB_CUDA(cudaMemcpyAsync(status, c->cov_res.blk_st.p, sizeof(int) * n, cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
   return 0;
 }
@@ -2488,12 +2494,12 @@ int hb200_get_pose_pair_covariance(hb200_ctx* c, int n, double* joint, double* r
   if (!c) return fail(-1, "null context");
   if (n < 0) return fail(-1, "invalid argument");
   if (!c->cov_valid) return fail(-2, "no covariance computed (hb200_compute_covariance has not succeeded)");
-  if (n != c->cov_pair_n) return fail(-2, "the last successful compute had %d stamp pairs, not %d", c->cov_pair_n, n);
+  if (n != c->cov_res.pair_n) return fail(-2, "the last successful compute had %d stamp pairs, not %d", c->cov_res.pair_n, n);
   if (n == 0) return 0;
   HB_CUDA(cudaSetDevice(c->device));
-  if (joint) HB_CUDA(cudaMemcpyAsync(joint, c->cov_pair_joint.p, sizeof(double) * 144 * n, cudaMemcpyDeviceToHost, c->stream));
-  if (relative) HB_CUDA(cudaMemcpyAsync(relative, c->cov_pair_rel.p, sizeof(double) * 36 * n, cudaMemcpyDeviceToHost, c->stream));
-  if (status) HB_CUDA(cudaMemcpyAsync(status, c->cov_pair_st.p, sizeof(int) * n, cudaMemcpyDeviceToHost, c->stream));
+  if (joint) HB_CUDA(cudaMemcpyAsync(joint, c->cov_res.pair_joint.p, sizeof(double) * 144 * n, cudaMemcpyDeviceToHost, c->stream));
+  if (relative) HB_CUDA(cudaMemcpyAsync(relative, c->cov_res.pair_rel.p, sizeof(double) * 36 * n, cudaMemcpyDeviceToHost, c->stream));
+  if (status) HB_CUDA(cudaMemcpyAsync(status, c->cov_res.pair_st.p, sizeof(int) * n, cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
   return 0;
 }
@@ -2503,8 +2509,8 @@ int hb200_get_covariance(hb200_ctx* c, double* packed, double* landmark) {
   if (!c->cov_valid) return fail(-2, "no covariance computed (hb200_compute_covariance has not succeeded)");
   HB_CUDA(cudaSetDevice(c->device));
   const CovPoint& pt = c->cov_pt[c->cov_slot_committed];
-  if (packed) HB_CUDA(cudaMemcpyAsync(packed, c->cov_packed.p, sizeof(double) * cov_packed_doubles(pt.lay), cudaMemcpyDeviceToHost, c->stream));
-  if (landmark && pt.L) HB_CUDA(cudaMemcpyAsync(landmark, c->cov_lm.p, sizeof(double) * 9 * pt.L, cudaMemcpyDeviceToHost, c->stream));
+  if (packed) HB_CUDA(cudaMemcpyAsync(packed, c->cov_res.packed.p, sizeof(double) * cov_packed_doubles(pt.lay), cudaMemcpyDeviceToHost, c->stream));
+  if (landmark && pt.L) HB_CUDA(cudaMemcpyAsync(landmark, c->cov_res.lm.p, sizeof(double) * 9 * pt.L, cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
   return 0;
 }
@@ -2512,7 +2518,7 @@ int hb200_get_covariance(hb200_ctx* c, double* packed, double* landmark) {
 int hb200_interpolate_covariance(hb200_ctx* c, int n, const double* stamps, double* cov, int* num_invalid) {
   return cov_interpolate(c, n, stamps, cov, num_invalid, 36, [&](auto K, const CovPoint& pt) {
     cov_stamp_kernel<K, 6><<<(n + kStateWarps - 1) / kStateWarps, kStateWarps * 32, 0, c->stream>>>(
-        n, c->cov_t.p, pt.knots.p, pt.tab.p, pt.lay.K, pt.basis, nullptr, 0, nullptr, 0, pt.bias_basis, c->cov_packed.p, pt.lay, c->cov_o.p, c->cov_bad.p);
+        n, c->cov_t.p, pt.knots.p, pt.tab.p, pt.lay.K, pt.basis, nullptr, 0, nullptr, 0, pt.bias_basis, c->cov_res.packed.p, pt.lay, c->cov_o.p, c->cov_bad.p);
     return check_launch(c, "cov_stamp_kernel");
   });
 }
@@ -2521,7 +2527,7 @@ int hb200_interpolate_state_covariance(hb200_ctx* c, int n, const double* stamps
   static_assert(HB200_STATE_COV_DIM == kStateDim, "state covariance dimension");
   return cov_interpolate(c, n, stamps, cov, num_invalid, HB200_STATE_COV_DIM * HB200_STATE_COV_DIM, [&](auto K, const CovPoint& pt) {
     cov_stamp_kernel<K, kStateDim><<<(n + kStateWarps - 1) / kStateWarps, kStateWarps * 32, 0, c->stream>>>(
-        n, c->cov_t.p, pt.knots.p, pt.tab.p, pt.lay.K, pt.basis, pt.bg.p, pt.Kbg, pt.ba.p, pt.Kba, pt.bias_basis, c->cov_packed.p, pt.lay, c->cov_o.p, c->cov_bad.p);
+        n, c->cov_t.p, pt.knots.p, pt.tab.p, pt.lay.K, pt.basis, pt.bg.p, pt.Kbg, pt.ba.p, pt.Kba, pt.bias_basis, c->cov_res.packed.p, pt.lay, c->cov_o.p, c->cov_bad.p);
     return check_launch(c, "cov_stamp_kernel");
   });
 }
@@ -2540,18 +2546,14 @@ int iterate_enqueue(hb200_ctx* c, int iterations) {
     const bool graph_ok = c->use_graph && !c->allreduce && (!c->nccl || c->comm_warm || c->peer_reduce());
     if (graph_ok) {
       const bool slot_b = c->peer_reduce() && c->peer_par == 1;
-      cudaGraph_t& graph = slot_b ? c->graph_b : c->graph;
-      cudaGraphExec_t& exec = slot_b ? c->graph_exec_b : c->graph_exec;
-      bool& valid = slot_b ? c->graph_b_valid : c->graph_valid;
-      if (!c->graph_valid) c->graph_b_valid = false;   // (kernel_args_changed() only knows the first slot)
-      if (!valid) {
-        if (exec) { cudaGraphExecDestroy(exec); exec = nullptr; }
-        if (graph) { cudaGraphDestroy(graph); graph = nullptr; }
+      IterationGraph& g = c->graphs[slot_b];
+      if (!g.valid) {
+        g.release();
         const int par_before = c->peer_par;
         HB_CUDA(cudaStreamBeginCapture(c->stream, c->nccl ? cudaStreamCaptureModeRelaxed : cudaStreamCaptureModeThreadLocal));
         const long long before = c->launches, nccl_before = c->nccl_calls;
         rc = enqueue_iteration(c);
-        cudaError_t e = cudaStreamEndCapture(c->stream, &graph);
+        cudaError_t e = cudaStreamEndCapture(c->stream, &g.graph);
         c->launches = before;  // capture does not execute
         c->nccl_calls_per_iteration = c->nccl_calls - nccl_before;
         c->nccl_calls = nccl_before;
@@ -2561,28 +2563,28 @@ int iterate_enqueue(hb200_ctx* c, int iterations) {
           if (!c->nccl) return fail(100 + static_cast<int>(e), "graph capture: %s", cudaGetErrorString(e));
           // a communicator that cannot be captured: fall back to direct launches for this context
           cudaGetLastError();
-          c->use_graph = false; graph = nullptr;
+          c->use_graph = false; g.graph = nullptr;
           --it;
           continue;
         }
-        HB_CUDA(cudaGraphInstantiate(&exec, graph, 0));
-        valid = true;
+        HB_CUDA(cudaGraphInstantiate(&g.exec, g.graph, 0));
+        g.valid = true;
         c->launches_per_iteration = 0;
         size_t nodes = 0;
-        HB_CUDA(cudaGraphGetNodes(graph, nullptr, &nodes));
+        HB_CUDA(cudaGraphGetNodes(g.graph, nullptr, &nodes));
         cudaGraphNode_t* nd = new cudaGraphNode_t[nodes];
-        HB_CUDA(cudaGraphGetNodes(graph, nd, &nodes));
+        HB_CUDA(cudaGraphGetNodes(g.graph, nd, &nodes));
         for (size_t i = 0; i < nodes; ++i) { cudaGraphNodeType t; if (cudaGraphNodeGetType(nd[i], &t) == cudaSuccess && t == cudaGraphNodeTypeKernel) c->launches_per_iteration += 1; }
         delete[] nd;
         c->launches_per_iteration -= c->nccl_calls_per_iteration;   // NCCL's kernel nodes are not this library's launches
         if (getenv("HB200_GRAPH_DEBUG")) {
           size_t edges = 0;
-          cudaGraphGetEdges(graph, nullptr, nullptr, &edges);
+          cudaGraphGetEdges(g.graph, nullptr, nullptr, &edges);
           std::fprintf(stderr, "[hb200] iteration graph%s: %zu nodes (%lld own kernels, %lld NCCL), %zu edges\n", slot_b ? " (arena half B)" : "", nodes,
                        c->launches_per_iteration, c->nccl_calls_per_iteration, edges);
         }
       }
-      HB_CUDA(cudaGraphLaunch(exec, c->stream));
+      HB_CUDA(cudaGraphLaunch(g.exec, c->stream));
       if (c->peer_reduce()) c->peer_par ^= 1;
       c->launches += c->launches_per_iteration;
       c->nccl_calls += c->nccl_calls_per_iteration;
@@ -2754,7 +2756,7 @@ int hb200_set_termination(hb200_ctx* c, double function_tolerance, double gradie
   if (!c) return fail(-1, "null context");
   c->term_ftol = function_tolerance; c->term_gtol = gradient_tolerance; c->term_ptol = parameter_tolerance; c->term_min_radius = min_trust_region_radius;
   c->term_enabled = function_tolerance > 0 || gradient_tolerance > 0 || parameter_tolerance > 0 || min_trust_region_radius > 0;
-  c->graph_valid = false;   // baked into kernel arguments
+  c->iterations_changed();   // baked into kernel arguments
   return 0;
 }
 
@@ -3415,7 +3417,7 @@ int hb200_set_allreduce(hb200_ctx* c, hb200_allreduce_fn fn, void* user) {
   if (fn && c->nccl) return fail(-2, "a NCCL communicator is attached; the callback hook is its replacement, not an addition");
   const bool detach = !fn && c->allreduce;
   c->allreduce = fn; c->allreduce_user = user;
-  c->graph_valid = false;
+  c->iterations_changed();
   return detach ? forget_agreement(c) : 0;
 }
 
@@ -3436,15 +3438,11 @@ int hb200_set_nccl_comm(hb200_ctx* c, void* comm, int nranks, int rank) {
   if (comm) { int rc = load_nccl(); if (rc) return rc; }
   HB_CUDA(cudaSetDevice(c->device));
   HB_CUDA(cudaStreamSynchronize(c->stream));
-  if (c->graph_exec) { cudaGraphExecDestroy(c->graph_exec); c->graph_exec = nullptr; }   // it references the old communicator
-  if (c->graph) { cudaGraphDestroy(c->graph); c->graph = nullptr; }
-  if (c->graph_exec_b) { cudaGraphExecDestroy(c->graph_exec_b); c->graph_exec_b = nullptr; }
-  if (c->graph_b) { cudaGraphDestroy(c->graph_b); c->graph_b = nullptr; }
-  c->graph_valid = false; c->graph_b_valid = false;
+  for (IterationGraph& g : c->graphs) g.release();   // they reference the old communicator
   if (c->nccl && c->own_nccl) g_nccl.CommDestroy(c->nccl);
   c->nccl = comm; c->own_nccl = false;
   c->nranks = comm ? nranks : 1; c->rank = comm ? rank : 0;
-  c->comm_warm = false; c->graph_valid = false;
+  c->comm_warm = false;
   const int rc = forget_agreement(c);   // a new communicator agrees afresh; none leaves a single context
   return rc ? rc : sync_layout(c);
 }
@@ -3524,7 +3522,7 @@ int hb200_peer_connect(hb200_ctx* c, int nranks, int rank, const char* handles) 
   HB_CUDA(cudaMemcpyAsync(c->d_peers.p, host.data(), sizeof(double*) * kMaxRanks, cudaMemcpyHostToDevice, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
   c->peers_open = true;
-  c->graph_valid = false;
+  c->iterations_changed();
   return 0;
 }
 
@@ -3568,7 +3566,7 @@ int hb200_peer_disconnect(hb200_ctx* c) {
   HB_CUDA(cudaSetDevice(c->device));
   HB_CUDA(cudaStreamSynchronize(c->stream));
   close_peers(c);
-  c->graph_valid = false;
+  c->iterations_changed();
   return 0;
 }
 
@@ -3578,7 +3576,7 @@ int hb200_comm_info(hb200_ctx* c, int* nranks, int* rank, int* nccl, int* peer_m
   if (rank) *rank = c->rank;
   if (nccl) *nccl = c->nccl ? 1 : 0;
   if (peer_mailbox) *peer_mailbox = (c->nccl && c->peers_open) ? (c->peer_reduce() ? 2 : 1) : 0;   // 2: the system reduction runs over peer memory too
-  if (graph) *graph = (c->use_graph && !c->allreduce && c->graph_valid) ? 1 : 0;
+  if (graph) *graph = (c->use_graph && !c->allreduce && c->graphs[0].valid) ? 1 : 0;
   if (payload_doubles) *payload_doubles = c->bound ? c->lay.total : 0;
   return 0;
 }
