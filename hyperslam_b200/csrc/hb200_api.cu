@@ -135,6 +135,94 @@ void compute_basis(Basis* b, int k) {
     }
 }
 
+// One of the window's uniform B-splines: the pose knots (stride 8) or a bias spline (stride 4), each knot's stamp last.
+// val: the current and trial state; stamp: the host mirror of the stamps hb200_bind computed its index maps from, and
+// the knot count; dropped: the leading knots the last hb200_slide removed.  Launching helpers take the context.
+struct Spline {
+  int order = 0;
+  const int stride;
+  Basis basis{};
+  DevBuf<double> val[2];
+  std::vector<double> stamp;
+  int dropped = 0;
+  explicit Spline(int stride) : stride(stride) {}
+  int n() const { return static_cast<int>(stamp.size()); }
+  size_t doubles() const { return static_cast<size_t>(stride) * stamp.size(); }
+  double stamp_of(const double* knots, int j) const { return knots[static_cast<size_t>(stride) * j + stride - 1]; }
+  // Knots fit for set: at least k of them, stamps strictly increasing and each step within 1e-6 of the first (the
+  // reference only ever creates uniformly separated knots, abstract.cpp:89,128), so all finite.  `what` names a knot.
+  int check(int k, int count, const double* knots, const char* what) const {
+    if (count < k) return fail(-1, "need at least %d %ss, got %d", k, what, count);
+    for (int j = 1; j < count; ++j)
+      if (!(stamp_of(knots, j) > stamp_of(knots, j - 1))) return fail(-1, "%s stamps must be strictly increasing (%s %d)", what, what, j);
+    const double dt0 = stamp_of(knots, 1) - stamp_of(knots, 0);
+    for (int j = 1; j < count; ++j)
+      if (!(std::fabs((stamp_of(knots, j) - stamp_of(knots, j - 1)) - dt0) <= 1e-6 * dt0)) return fail(-1, "%s stamps must be uniformly spaced (%s %d)", what, what, j);
+    return 0;
+  }
+  // checked knots as the current state; *changed: the order, the count or a stamp changed: the index maps no longer hold
+  int set(int k, int count, const double* knots, cudaStream_t s, bool* changed) {
+    std::vector<double> t(count);
+    for (int j = 0; j < count; ++j) t[j] = stamp_of(knots, j);
+    *changed = k != order || t != stamp;
+    stamp.swap(t); order = k;
+    compute_basis(&basis, k);
+    for (DevBuf<double>& v : val) HB_CUDA(v.ensure(doubles()));
+    HB_CUDA(cudaMemcpyAsync(val[0].p, knots, sizeof(double) * doubles(), cudaMemcpyHostToDevice, s));
+    HB_CUDA(cudaStreamSynchronize(s));
+    return 0;
+  }
+  // room for `count` more knots in both copies, the current knots kept
+  int reserve(int count, cudaStream_t s) {
+    for (int i = 0; i < 2; ++i) HB_CUDA(val[i].grow(static_cast<size_t>(stride) * (n() + count), i == 0 ? doubles() : 0, s));
+    return 0;
+  }
+  int append(hb200_ctx* c, int count);   // append_knots_kernel, the new stamps read back into the mirror
+  int upper(double t) const { return static_cast<int>(std::upper_bound(stamp.begin(), stamp.end(), t) - stamp.begin()); }
+  // Leading knots a slide to lower_bound drops: those before the (order - 1) / 2 knots of padding in front of the lower
+  // bound's interval (reference optimizer.cpp:289,331-341), none from min_base (a kept factor's base) on, `order` kept.
+  int drop_count(double lower_bound, int min_base) const {
+    const int sh = std::min(std::max(0, upper(lower_bound) - 1 - (order - 1) / 2), min_base);
+    return std::max(0, std::min(sh, n() - order));
+  }
+  int shift(hb200_ctx* c, int count);   // the rest shifted into the trial copy (shift_knots_kernel), which is switched in
+  int mismatch(const double* knots) const {   // the first knot whose stamp differs from the mirror, or -1
+    for (int j = 0; j < n(); ++j) if (stamp_of(knots, j) != stamp[j]) return j;
+    return -1;
+  }
+  // a covariance build's copy of s: its order, basis, stamps and current knots
+  int freeze(const Spline& s, cudaStream_t st) {
+    order = s.order; basis = s.basis; stamp = s.stamp;
+    HB_CUDA(val[0].ensure(doubles()));
+    if (n()) HB_CUDA(cudaMemcpyAsync(val[0].p, s.val[0].p, sizeof(double) * doubles(), cudaMemcpyDeviceToDevice, st));
+    return 0;
+  }
+};
+
+// Fewest knots append_knots_kernel must append to a bias spline (stamps s, order kb) so that segment_base accepts t:
+// s[left] <= t < s'[K' - right] (left = (kb-1)/2, right = kb-1-left) over the K' extended stamps s', where new stamp
+// K - 1 + i is fma(i, dt, s[K-1]) with dt = s[K-1] - s[K-2].  0 on success, 2 for t before the span, -1 past HB200_BIAS_APPEND_MAX.
+int bias_append_count(const Spline& spline, double t, int* count) {
+  const std::vector<double>& s = spline.stamp;
+  const int K = spline.n(), kb = spline.order, left = (kb - 1) / 2, right = kb - 1 - left;
+  const double dt = s[K - 1] - s[K - 2];
+  auto end_of = [&](int added) {   // the valid span's end with `added` knots appended: stamp of knot K + added - right
+    const int j = K + added - right;
+    return j < K ? s[j] : std::fma(static_cast<double>(j - (K - 1)), dt, s[K - 1]);
+  };
+  *count = 0;
+  if (t < s[left]) return 2;
+  if (t < end_of(0)) return 0;
+  const double est = std::floor((t - s[K - 1]) / dt) + right;   // first guess; the loops below decide
+  if (!(est <= HB200_BIAS_APPEND_MAX + 1.0)) return -1;
+  int n = std::max(1, static_cast<int>(est));
+  while (n > 1 && t < end_of(n - 1)) --n;
+  while (!(t < end_of(n)) && n <= HB200_BIAS_APPEND_MAX) ++n;
+  if (n > HB200_BIAS_APPEND_MAX) return -1;
+  *count = n;
+  return 0;
+}
+
 // ---- NCCL, bound at run time ----------------------------------------------------------------------
 // libnccl.so.2 is resolved with dlopen when the first communicator call is made: inside a torch process this is
 // the copy torch already loaded (same SONAME), in a plain C++ host the system library.  Only the five entry
@@ -173,13 +261,12 @@ int load_nccl() {
     if (r__ != 0) return fail(300 + r__, "%s: %s", #expr, g_nccl.GetErrorString ? g_nccl.GetErrorString(r__) : "nccl error"); \
   } while (0)
 
-// The linearisation point hb200_build_covariance froze: the shapes its outputs were written with, and copies of the
-// knots, the knot table and both bias splines (knot values and stamps) for the interpolated covariances.
+// The linearisation point hb200_build_covariance froze: its output shapes, and copies of the splines and the knot table.
 struct CovPoint {
   SysLayout lay{};
-  Basis basis{}, bias_basis{};
-  int L = 0, k = 0, Nv = 0, max_rows = 0, Kbg = 0, Kba = 0;
-  DevBuf<double> knots, tab, bg, ba;
+  int L = 0, Nv = 0, max_rows = 0;
+  Spline pose{8}, gyro{4}, accel{4};   // the current copy only
+  DevBuf<double> tab;
 };
 
 // The results of hb200_compute_covariance: the packed selected inverse, the landmark marginals, and the requested blocks
@@ -249,14 +336,17 @@ struct hb200_ctx {
   int last_terminated = 0, last_performed = 0;     // outcome of the last hb200_iterate / hb200_optimize that fetched records
   double last_gmax = 0, last_step_norm = 0, last_x_norm = 0;
 
-  // window state (index 0 = current, 1 = trial)
-  int k = 0, K = 0, kb = 4, Kbg = 0, Kba = 0, C = 0, L = 0;
-  Basis basis{}, bias_basis{};
-  DevBuf<double> knots[2], bg[2], ba[2], grav[2], lms[2], tab[2];
+  // window state (index 0 = current, 1 = trial): the pose knots and their table, and the two bias splines of one order
+  Spline pose{8}, gyro{4}, accel{4};
+  int C = 0, L = 0;
+  DevBuf<double> grav[2], lms[2], tab[2];
   DevBuf<double> cams, imu, cam_tab, imu_tab;
   DevBuf<unsigned char> fixed;
   std::vector<unsigned char> h_knot_const;
-  std::vector<double> h_knot_stamp, h_bg_stamp, h_ba_stamp;   // stamps the index maps of hb200_bind were computed from
+  int k() const { return pose.order; }
+  int K() const { return pose.n(); }
+  int Kbg() const { return gyro.n(); }
+  int Kba() const { return accel.n(); }
   int gravity_const = 0, bias_const = 0;
   bool have_imu = false, have_gravity = false;
   double huber = 0.5, imu_scale = 1.6e-5, radius0 = 1e4;
@@ -310,7 +400,6 @@ struct hb200_ctx {
   DevBuf<int> w_keep, w_pos, w_lkeep, w_lpos, w_cnt, w_scal;
   DevBuf<double> w_vote;   // sharded contexts: the agreement payload of a collective sliding-window call (agree_round)
   int slide_L = -1;
-  int bg_dropped = 0, ba_dropped = 0;   // leading gyro / accel bias knots the last hb200_slide removed (HB200_SLIDE_DROP_BIAS)
   // hb200_append_stereo_tracks inputs: [stamp | pixel0 | pixel1] and [camera0 | camera1 | landmark | new flag | rank]
   DevBuf<double> trk_d;
   DevBuf<int> trk_i;
@@ -424,9 +513,9 @@ struct hb200_ctx {
   }();
   bool wt_visual() const { return wt_set[HB200_PIXEL] || wt_set[HB200_BEARING]; }
 
-  int o_bg() const { return 6 * K; }
-  int o_ba() const { return 6 * K + 3 * Kbg; }
-  int o_g() const { return 6 * K + 3 * Kbg + 3 * Kba; }
+  int o_bg() const { return 6 * K(); }
+  int o_ba() const { return 6 * K() + 3 * Kbg(); }
+  int o_g() const { return 6 * K() + 3 * Kbg() + 3 * Kba(); }
 
   // What a change makes stale, from the narrowest to the widest.  The calibration and output mirrors are only read
   // while evaluated_J holds, so dropping them with it never refuses a valid call.  `bound` and `have_snapshot` are
@@ -446,9 +535,8 @@ struct hb200_ctx {
   // trial state before reading it, so hb200_slide compacts the current state into the trial copy and switches the two.
   struct StateBlock { DevBuf<double>* cur; DevBuf<double>* trial; DevBuf<double>* snap; size_t count; };
   std::array<StateBlock, 5> state_blocks() {
-    return {{{&knots[0], &knots[1], &snap[0], 8 * static_cast<size_t>(K)},
-             {&bg[0], &bg[1], &snap[1], 4 * static_cast<size_t>(Kbg)},
-             {&ba[0], &ba[1], &snap[2], 4 * static_cast<size_t>(Kba)},
+    auto spline = [&](Spline& s, int i) { return StateBlock{&s.val[0], &s.val[1], &snap[i], s.doubles()}; };
+    return {{spline(pose, 0), spline(gyro, 1), spline(accel, 2),
              {&grav[0], &grav[1], &snap[3], 3},
              {&lms[0], &lms[1], &snap[4], 3 * static_cast<size_t>(L)}}};
   }
@@ -478,6 +566,26 @@ int check_launch(hb200_ctx* c, const char* what) {
     if (rc__) return rc__;                         \
   } while (0)
 
+int Spline::append(hb200_ctx* c, int count) {
+  if (const int rc = reserve(count, c->stream)) return rc;
+  append_knots_kernel<<<1, 32, 0, c->stream>>>(n(), count, stride, stride - 1, val[0].p);
+  HB_LAUNCH(c, "append_knots_kernel");
+  std::vector<double> tail(static_cast<size_t>(stride) * count);
+  HB_CUDA(cudaMemcpyAsync(tail.data(), val[0].p + doubles(), sizeof(double) * tail.size(), cudaMemcpyDeviceToHost, c->stream));
+  HB_CUDA(cudaStreamSynchronize(c->stream));
+  for (int i = 0; i < count; ++i) stamp.push_back(stamp_of(tail.data(), i));
+  return 0;
+}
+int Spline::shift(hb200_ctx* c, int count) {
+  dropped = count;
+  if (!count) return 0;
+  shift_knots_kernel<<<(stride * (n() - count) + 255) / 256, 256, 0, c->stream>>>(n() - count, count, stride, val[0].p, val[1].p);
+  HB_LAUNCH(c, "shift_knots_kernel");
+  val[0].swap(val[1]);
+  stamp.erase(stamp.begin(), stamp.begin() + count);
+  return 0;
+}
+
 // The kernels are instantiated per spline order: f(std::integral_constant<int, K>) for K = k.
 template <typename F>
 int with_order(int k, F&& f) {
@@ -503,7 +611,7 @@ int for_each_order_mode(F&& f) {
 // stream, each chain's workspace in its CTA's shared memory.  at: storage for the cluster-dimension attribute.
 void band_cluster_config(hb200_ctx* c, cudaLaunchConfig_t* cfg, cudaLaunchAttribute* at) {
   cfg->gridDim = dim3(2); cfg->blockDim = dim3(kBandThreads); cfg->stream = c->stream;
-  cfg->dynamicSmemBytes = band_cluster_doubles(c->K, c->beta, c->n - 6 * c->K) * sizeof(double);
+  cfg->dynamicSmemBytes = band_cluster_doubles(c->K(), c->beta, c->n - 6 * c->K()) * sizeof(double);
   at[0].id = cudaLaunchAttributeClusterDimension;
   at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
   cfg->attrs = at; cfg->numAttrs = 1;
@@ -526,9 +634,9 @@ int join_side(hb200_ctx* c) {
 }
 
 int update_fixed(hb200_ctx* c) {
-  c->n = 6 * c->K + 3 * c->Kbg + 3 * c->Kba + 2;
+  c->n = 6 * c->K() + 3 * c->Kbg() + 3 * c->Kba() + 2;
   std::vector<unsigned char> f(c->n, 0);
-  for (int j = 0; j < c->K && j < static_cast<int>(c->h_knot_const.size()); ++j)
+  for (int j = 0; j < c->K() && j < static_cast<int>(c->h_knot_const.size()); ++j)
     if (c->h_knot_const[j]) for (int a = 0; a < 6; ++a) f[6 * j + a] = 1;
   if (c->bias_const) for (int a = c->o_bg(); a < c->o_g(); ++a) f[a] = 1;
   if (c->gravity_const) { f[c->o_g()] = 1; f[c->o_g() + 1] = 1; }
@@ -550,9 +658,9 @@ int ensure_dense(hb200_ctx* c) {
 int ensure_system(hb200_ctx* c) {
   const size_t n = c->n;
   // block half-bandwidth of the reduced pose system = longest landmark track in control points (>= k - 1)
-  c->beta = std::max(std::max(c->k - 1, c->max_rows / 6 - 1), std::max(c->min_beta, c->agreed_beta));
-  c->beta = std::min(c->beta, std::max(c->K - 1, 0));
-  c->lay = sys_layout(c->K, c->beta, c->n - 6 * c->K);
+  c->beta = std::max(std::max(c->k() - 1, c->max_rows / 6 - 1), std::max(c->min_beta, c->agreed_beta));
+  c->beta = std::min(c->beta, std::max(c->K() - 1, 0));
+  c->lay = sys_layout(c->K(), c->beta, c->n - 6 * c->K());
   HB_CUDA(c->sys.ensure(static_cast<size_t>(c->lay.total)));
   HB_CUDA(c->D.ensure(n));
   HB_CUDA(c->dp.ensure(n));
@@ -566,16 +674,16 @@ int ensure_system(hb200_ctx* c) {
   HB_CUDA(c->spd.ensure(1));
   HB_CUDA(c->records.ensure(c->max_records));
   // solver selection: block-banded + arrowhead unless the band is wide on a large system
-  const size_t ws = band_workspace_doubles(c->K, c->beta, c->n - 6 * c->K) * sizeof(double);
-  c->band_solver = !c->force_dense && ((c->n <= 512) || (12 * (c->beta + 1) <= 6 * c->K));
+  const size_t ws = band_workspace_doubles(c->K(), c->beta, c->n - 6 * c->K()) * sizeof(double);
+  c->band_solver = !c->force_dense && ((c->n <= 512) || (12 * (c->beta + 1) <= 6 * c->K()));
   c->band_smem = ws <= kBandSmemBytes;
   c->use_bcr = false;
-  if (c->band_solver && !c->band_smem && 6 * c->beta <= kBcrMaxNb && c->n - 6 * c->K <= 54) {
+  if (c->band_solver && !c->band_smem && 6 * c->beta <= kBcrMaxNb && c->n - 6 * c->K() <= 54) {
     // the band does not fit one CTA's shared memory: cyclic reduction over super-blocks of beta control points
-    const int m = c->n - 6 * c->K;
-    const int nsb = (c->K + c->beta - 1) / c->beta;
+    const int m = c->n - 6 * c->K();
+    const int nsb = (c->K() + c->beta - 1) / c->beta;
     const int nctas = std::max(1, std::min(c->num_sms, (nsb + 1) / 2));
-    const BcrPlan pl = bcr_plan(c->K, c->beta, m, nctas);
+    const BcrPlan pl = bcr_plan(c->K(), c->beta, m, nctas);
     const size_t nb = pl.nb;
     const size_t p1 = nb * (nb | 1) + nb + 1 + nb * (((2 * nb + m + 1 + 11) / 16) * 16 + 4) + static_cast<size_t>(m + 1) * m;
     const size_t p2 = 3 * nb * nb + 2 * nb * m + 2 * nb;
@@ -607,13 +715,13 @@ int ensure_system(hb200_ctx* c) {
     } else {
       HB_CUDA(c->band_ws.ensure(ws / sizeof(double)));
       // chunked factorisation: two shared-memory views of band_chunk_cols block columns (band + arrow + LI)
-      const size_t colbytes = (static_cast<size_t>(6 + 6 * c->beta) * 6 + 6 * static_cast<size_t>(c->n - 6 * c->K + 1) + 48) * sizeof(double);
+      const size_t colbytes = (static_cast<size_t>(6 + 6 * c->beta) * 6 + 6 * static_cast<size_t>(c->n - 6 * c->K() + 1) + 48) * sizeof(double);
       const int fit = static_cast<int>((200 * 1024) / (2 * colbytes));
-      c->band_chunk_cols = std::max(c->beta + 2, std::min(fit, c->K + c->beta));
+      c->band_chunk_cols = std::max(c->beta + 2, std::min(fit, c->K() + c->beta));
       // after the factorisation the corner system [m + 1][m | 1], its solution and factor diagonal (2m) and the
       // 6-double block scratch behind them move into the same shared memory (band_solve_kernel<false>): a wide
       // arrowhead needs more than the two chunk views
-      const int m = c->n - 6 * c->K;
+      const int m = c->n - 6 * c->K();
       const size_t corner = (static_cast<size_t>(m + 1) * (m | 1) + 2 * static_cast<size_t>(m) + 6) * sizeof(double);
       c->band_chunk_smem = std::max(2 * colbytes * c->band_chunk_cols, corner);
       if (c->band_chunk_smem > 220 * 1024) return fail(-6, "band solver: a chunk of %d block columns or the %d x %d corner does not fit shared memory (arrow too wide)", c->band_chunk_cols, m, m);
@@ -649,14 +757,14 @@ PixelArgs pixel_args(hb200_ctx* c, int sel, double* sys) {
   a.sys = sys; a.lay = c->lay; a.tiles_per_cta = 1;
   a.n = c->Nv; a.stamp = c->visual.stamp.p; a.pixel = c->visual.pixel.p; a.meas_z = c->visual.z.p; a.idx = c->visual.idx.p;
   a.tab = c->tab[sel].p; a.cam_tab = c->cam_tab.p; a.landmarks = c->lms[sel].p;
-  a.r = J ? c->v_out.r.p : nullptr; a.Jp = c->v_out.Jp.p; a.Jl = c->v_out.Jl.p; a.w = c->v_out.w.p; a.cost_partial = c->cp_pix[J ? 0 : 1].p; a.huber = c->huber; a.huber_bearing = c->huber_bearing; a.K_knots = c->K;
+  a.r = J ? c->v_out.r.p : nullptr; a.Jp = c->v_out.Jp.p; a.Jl = c->v_out.Jl.p; a.w = c->v_out.w.p; a.cost_partial = c->cp_pix[J ? 0 : 1].p; a.huber = c->huber; a.huber_bearing = c->huber_bearing; a.K_knots = c->K();
   return a;
 }
 template <bool J>
 InertialArgs inertial_args(hb200_ctx* c, int sel) {
   InertialArgs a{};
   a.n = c->Ni; a.stamp = c->inertial.stamp.p; a.meas = c->inertial.meas.p; a.idx = c->inertial.idx.p; a.tab = c->tab[sel].p; a.imu_tab = c->imu_tab.p;
-  a.bg = c->bg[sel].p; a.ba = c->ba[sel].p; a.gravity = c->grav[sel].p;
+  a.bg = c->gyro.val[sel].p; a.ba = c->accel.val[sel].p; a.gravity = c->grav[sel].p;
   a.r = J ? c->i_out.r.p : nullptr; a.Jp = c->i_out.Jp.p; a.wg = c->i_out.wg.p; a.wa = c->i_out.wa.p; a.Jg = c->i_out.Jg.p;
   a.cost_partial = c->cp_imu[J ? 0 : 1].p; a.loss_scale = c->imu_scale;
   return a;
@@ -676,7 +784,7 @@ int launch_pixel(hb200_ctx* c, int sel, double* sys) {
   const PixelArgs a = pixel_args<J>(c, sel, sys);
   return with_pixel_pass<J>(c, a, [&](auto FUSE, auto DET) {
     return with_flag(c->wt_visual(), [&](auto WT) {
-      pixel_eval_kernel<K, J, FUSE, DET, WT><<<c->n_pix_blocks, kEvalThreads, 0, c->stream>>>(a, c->basis, DET ? c->det_pix : DetOut{}, DET ? c->det_seg_off.p : nullptr,
+      pixel_eval_kernel<K, J, FUSE, DET, WT><<<c->n_pix_blocks, kEvalThreads, 0, c->stream>>>(a, c->pose.basis, DET ? c->det_pix : DetOut{}, DET ? c->det_seg_off.p : nullptr,
                                                                                             c->wt.p);
       return check_launch(c, DET ? "pixel_eval_det_kernel" : "pixel_eval_kernel");
     });
@@ -687,7 +795,7 @@ int launch_inertial(hb200_ctx* c, int sel) {
   if (c->Ni == 0) return 0;
   const InertialArgs a = inertial_args<J>(c, sel);
   return with_flag(c->wt_set[HB200_INERTIAL], [&](auto WT) {
-    inertial_eval_kernel<K, 4, J, WT><<<c->n_imu_blocks, kEvalThreads, J ? inertial_stash_bytes(K) : 0, side(c)>>>(a, c->basis, c->bias_basis, c->wt.p);
+    inertial_eval_kernel<K, 4, J, WT><<<c->n_imu_blocks, kEvalThreads, J ? inertial_stash_bytes(K) : 0, side(c)>>>(a, c->pose.basis, c->gyro.basis, c->wt.p);
     return check_launch(c, "inertial_eval_kernel");
   });
 }
@@ -699,7 +807,7 @@ int launch_factors_merged(hb200_ctx* c, int sel, double* sys) {
   const int blocks = c->n_pix_blocks + c->n_imu_blocks;
   return with_pixel_pass<J>(c, pa, [&](auto FUSE, auto DET) {
     return with_flag(c->wt_visual() || c->wt_set[HB200_INERTIAL], [&](auto WT) {
-      factor_eval_kernel<K, 4, J, FUSE, DET, WT><<<blocks, kEvalThreads * factor_lanes(K), 0, c->stream>>>(pa, ia, c->basis, c->bias_basis, c->n_pix_blocks,
+      factor_eval_kernel<K, 4, J, FUSE, DET, WT><<<blocks, kEvalThreads * factor_lanes(K), 0, c->stream>>>(pa, ia, c->pose.basis, c->gyro.basis, c->n_pix_blocks,
                                                                                            DET ? c->det_pix : DetOut{}, DET ? c->det_seg_off.p : nullptr, c->wt.p);
       return check_launch(c, DET ? "factor_eval_det_kernel" : "factor_eval_kernel");
     });
@@ -712,7 +820,7 @@ int launch_manifold(hb200_ctx* c, int sel) {
   a.n = c->Nm; a.stamp = c->manifold.stamp.p; a.meas = c->manifold.meas.p; a.idx = c->manifold.idx.p; a.tab = c->tab[sel].p; a.sensors = c->sensors.p;
   a.r = J ? c->m_out.r.p : nullptr; a.Jp = c->m_out.Jp.p; a.cost_partial = c->cp_imu[J ? 0 : 1].p + c->n_imu_blocks;
   return with_flag(c->wt_set[HB200_MANIFOLD], [&](auto WT) {
-    manifold_eval_kernel<K, J, WT><<<c->n_man_blocks, kEvalThreads, 0, side(c)>>>(a, c->basis, c->wt.p);
+    manifold_eval_kernel<K, J, WT><<<c->n_man_blocks, kEvalThreads, 0, side(c)>>>(a, c->pose.basis, c->wt.p);
     return check_launch(c, "manifold_eval_kernel");
   });
 }
@@ -729,7 +837,7 @@ int enqueue_factors(hb200_ctx* c, bool want_J, int sel, double* sys = nullptr) {
   if (c->Nv && c->Ni && c->n_pix_blocks + c->n_imu_blocks <= 4 * c->num_sms) {   // (also while profiling: same kernels as the graph)
     // visual and inertial factors side by side in one launch; pose factors (if any) on the side stream
     if (c->Nm && (rc = fork_side(c))) return rc;
-    rc = with_order(c->k, [&](auto K) {
+    rc = with_order(c->k(), [&](auto K) {
       return with_flag(J_any, [&](auto J) {
         const int r = launch_factors_merged<K, J>(c, sel, sys);
         return r ? r : launch_manifold<K, J>(c, sel);
@@ -743,7 +851,7 @@ int enqueue_factors(hb200_ctx* c, bool want_J, int sel, double* sys = nullptr) {
   // visual factors on the main stream, inertial + manifold factors concurrently on the side stream
   if (c->Nv && (c->Ni || c->Nm) && (rc = fork_side(c))) return rc;
   // sys (fused path): the pixel J^T J is accumulated by the factor kernel itself
-  rc = with_order(c->k, [&](auto K) {
+  rc = with_order(c->k(), [&](auto K) {
     return with_flag(J_any, [&](auto J) {
       int r = launch_pixel<K, J>(c, sel, sys);
       if (!r) r = launch_inertial<K, J>(c, sel);
@@ -756,7 +864,7 @@ int enqueue_factors(hb200_ctx* c, bool want_J, int sel, double* sys = nullptr) {
 
 // Knot table of state `sel`, then its factor sweep
 int enqueue_evaluate(hb200_ctx* c, bool want_J, int sel) {
-  prep_kernel<<<(c->K + 255) / 256, 256, 0, c->stream>>>(c->K, c->knots[sel].p, c->tab[sel].p, nullptr, 0);
+  prep_kernel<<<(c->K() + 255) / 256, 256, 0, c->stream>>>(c->K(), c->pose.val[sel].p, c->tab[sel].p, nullptr, 0);
   HB_LAUNCH(c, "prep_kernel");
   return enqueue_factors(c, want_J, sel);
 }
@@ -774,7 +882,7 @@ int enqueue_evaluate(hb200_ctx* c, bool want_J, int sel) {
 // selects the tensor-core kernel at every size.  Returns the CTAs per run.
 int inertial_splits(const hb200_ctx* c, bool* scalar_hess) {
   *scalar_hess = c->Ni < 16384 && !c->wt_set[HB200_INERTIAL];
-  return (*scalar_hess || c->k != 4) ? c->imu_splits : c->imu_splits_mma;
+  return (*scalar_hess || c->k() != 4) ? c->imu_splits : c->imu_splits_mma;
 }
 
 // DET instantiations (deterministic assembly) write the records of their region of the context's DetOut instead of
@@ -787,7 +895,7 @@ int enqueue_build(hb200_ctx* c, const SolverState* st) {
     bool scalar_hess = false;
     const int splits = inertial_splits(c, &scalar_hess);
     const int grid = c->nruns * splits;
-    const int rc = with_order(c->k, [&](auto K) {
+    const int rc = with_order(c->k(), [&](auto K) {
       return with_flag(det, [&](auto DET) {
         const DetOut d = DET ? c->det_imu : DetOut{};
         if (scalar_hess)
@@ -809,7 +917,7 @@ int enqueue_build(hb200_ctx* c, const SolverState* st) {
   }
   if (c->Nm) {
     const int blocks = (c->Nm + kManWarps - 1) / kManWarps;
-    const int rc = with_order(c->k, [&](auto K) {
+    const int rc = with_order(c->k(), [&](auto K) {
       return with_flag(det, [&](auto DET) {
         manifold_hessian_kernel<K, DET><<<blocks, kManWarps * 32, 0, side(c)>>>(c->Nm, c->manifold.idx.p, c->m_out.r.p, c->m_out.Jp.p, c->assembly(), c->lay,
                                                                                DET ? c->det_man : DetOut{});
@@ -826,7 +934,7 @@ int enqueue_build(hb200_ctx* c, const SolverState* st) {
   HB_LAUNCH(c, "cost_kernel");
   if (c->Nv && c->L && c->schur_groups) {
     const size_t smem = (3 * static_cast<size_t>(kSchurGroup) * (c->schur_rt + 1) + 3 * kSchurGroup + 4 * 3 * static_cast<size_t>(c->schur_rt)) * sizeof(double);
-    const int rc = with_order(c->k, [&](auto K) {
+    const int rc = with_order(c->k(), [&](auto K) {
       return with_flag(det, [&](auto DET) {
         schur_group_kernel<K, DET><<<c->n_lm_groups, kSchurGThreads, smem, c->stream>>>(c->lm_group_off.p, c->lm_order.p, c->lm_off.p, c->lm_obs.p, c->visual.idx.p, c->v_out.r.p,
                                                                                         c->v_out.Jp.p, c->v_out.Jl.p, c->v_out.w.p, st, c->assembly(), c->lay, c->Vchol.p, c->gl.p,
@@ -837,7 +945,7 @@ int enqueue_build(hb200_ctx* c, const SolverState* st) {
     if (rc) return rc;
   } else if (c->Nv && c->L) {
     const size_t smem = 2 * 3 * static_cast<size_t>(c->max_rows) * sizeof(double);
-    const int rc = with_order(c->k, [&](auto K) {
+    const int rc = with_order(c->k(), [&](auto K) {
       return with_flag(det, [&](auto DET) {
         schur_kernel<K, DET><<<c->L, kSchurThreads, smem, c->stream>>>(c->lm_off.p, c->lm_obs.p, c->visual.idx.p, c->v_out.r.p, c->v_out.Jp.p, c->v_out.Jl.p, c->v_out.w.p, st,
                                                                        c->assembly(), c->lay, c->Vchol.p, c->gl.p, c->Dl.p, c->max_rows, DET ? c->det_schur : DetOut{});
@@ -868,7 +976,7 @@ int enqueue_build(hb200_ctx* c, const SolverState* st) {
 int enqueue_assembly(hb200_ctx* c, const SolverState* st) {
   const size_t nclear = static_cast<size_t>(c->lay.total);
   const int blocks = static_cast<int>(std::min<size_t>((nclear / 4 + 255) / 256, static_cast<size_t>(c->num_sms) * 4));
-  prep_kernel<<<std::max(blocks, (c->K + 255) / 256), 256, 0, c->stream>>>(c->K, c->knots[0].p, c->tab[0].p, c->assembly(), nclear);
+  prep_kernel<<<std::max(blocks, (c->K() + 255) / 256), 256, 0, c->stream>>>(c->K(), c->pose.val[0].p, c->tab[0].p, c->assembly(), nclear);
   HB_LAUNCH(c, "prep_kernel");
   const int rc = enqueue_factors(c, true, 0, c->assembly());
   return rc ? rc : enqueue_build(c, st);
@@ -882,7 +990,7 @@ int prepare_det(hb200_ctx* c) {
   long long off = 0;
   auto region = [&](DetOut& d, long long slots, long long per_slot) { d.off = off; d.per_slot = per_slot; off += slots * per_slot; };
   c->det_pix = c->det_imu = c->det_man = c->det_schur = DetOut{};
-  const int rc = with_order(c->k, [&](auto K) {
+  const int rc = with_order(c->k(), [&](auto K) {
     if (c->Nv) {   // pixel: one slot per (64-factor tile, knot-base segment)
       const int tiles = c->n_pix_blocks;
       HB_CUDA(c->det_seg_off.ensure(2 * (static_cast<size_t>(tiles) + 1)));   // offsets | counts
@@ -981,10 +1089,10 @@ int enqueue_solve(hb200_ctx* c, bool fuse_retract = false, bool* fused = nullptr
       int extra = 0;
       if (fuse_retract) {
         ra = retract_args(c);
-        extra = (std::max(std::max(c->K, 1), std::max(c->Kbg, c->Kba)) + kLmWarps * 32 - 1) / (kLmWarps * 32);
+        extra = (std::max(std::max(c->K(), 1), std::max(c->Kbg(), c->Kba())) + kLmWarps * 32 - 1) / (kLmWarps * 32);
         if (fused) *fused = true;
       }
-      const int rc = with_order(c->k, [&](auto K) {
+      const int rc = with_order(c->k(), [&](auto K) {
         lm_backsub_kernel<K><<<c->n_lm_blocks + extra, kLmWarps * 32, 0, c->stream>>>(c->L, c->lm_off.p, c->lm_obs.p, c->visual.idx.p, c->v_out.r.p, c->v_out.Jp.p, c->v_out.Jl.p, c->v_out.w.p,
                                                                                  c->Vchol.p, c->gl.p, c->Dl.p, c->dp.p, c->dl.p, c->lm_part.p, c->lms[0].p, c->lms[1].p, c->n_lm_blocks, ra);
         return check_launch(c, "lm_backsub_kernel");
@@ -1000,14 +1108,14 @@ int enqueue_solve(hb200_ctx* c, bool fuse_retract = false, bool* fused = nullptr
 
 RetractArgs retract_args(hb200_ctx* c) {
   RetractArgs ra{};
-  ra.K = c->K; ra.Kbg = c->Kbg; ra.Kba = c->Kba; ra.L = c->L;
-  ra.dp = c->dp.p; ra.dl = c->dl.p; ra.knots = c->knots[0].p; ra.bg = c->bg[0].p; ra.ba = c->ba[0].p; ra.grav = c->grav[0].p; ra.lms = c->lms[0].p;
-  ra.knots_t = c->knots[1].p; ra.bg_t = c->bg[1].p; ra.ba_t = c->ba[1].p; ra.grav_t = c->grav[1].p; ra.lms_t = c->lms[1].p; ra.tab_t = c->tab[1].p;
+  ra.K = c->K(); ra.Kbg = c->Kbg(); ra.Kba = c->Kba(); ra.L = c->L;
+  ra.dp = c->dp.p; ra.dl = c->dl.p; ra.knots = c->pose.val[0].p; ra.bg = c->gyro.val[0].p; ra.ba = c->accel.val[0].p; ra.grav = c->grav[0].p; ra.lms = c->lms[0].p;
+  ra.knots_t = c->pose.val[1].p; ra.bg_t = c->gyro.val[1].p; ra.ba_t = c->accel.val[1].p; ra.grav_t = c->grav[1].p; ra.lms_t = c->lms[1].p; ra.tab_t = c->tab[1].p;
   ra.retract_landmarks = (c->L && !c->Nv) ? 1 : 0;
   return ra;
 }
 int enqueue_retract(hb200_ctx* c) {
-  const int m = std::max(std::max(c->K, c->L), std::max(std::max(c->Kbg, c->Kba), 1));
+  const int m = std::max(std::max(c->K(), c->L), std::max(std::max(c->Kbg(), c->Kba()), 1));
   retract_kernel<<<(m + 127) / 128, 128, 0, c->stream>>>(retract_args(c));
   HB_LAUNCH(c, "retract_kernel");
   return 0;
@@ -1024,8 +1132,8 @@ TermArgs term_args(hb200_ctx* c) {
   TermArgs t{};
   t.enabled = c->term_enabled ? 1 : 0;
   t.function_tolerance = c->term_ftol; t.gradient_tolerance = c->term_gtol; t.parameter_tolerance = c->term_ptol; t.min_radius = c->term_min_radius;
-  t.K = c->K; t.Kbg = c->Kbg; t.Kba = c->Kba;
-  t.knots = c->knots[0].p; t.knots_t = c->knots[1].p; t.bg = c->bg[0].p; t.bg_t = c->bg[1].p; t.ba = c->ba[0].p; t.ba_t = c->ba[1].p;
+  t.K = c->K(); t.Kbg = c->Kbg(); t.Kba = c->Kba();
+  t.knots = c->pose.val[0].p; t.knots_t = c->pose.val[1].p; t.bg = c->gyro.val[0].p; t.bg_t = c->gyro.val[1].p; t.ba = c->accel.val[0].p; t.ba_t = c->accel.val[1].p;
   t.grav = c->grav[0].p; t.grav_t = c->grav[1].p;
   return t;
 }
@@ -1141,7 +1249,7 @@ int sync_layout(hb200_ctx* c) {
 enum { kCallPixel = 1, kCallBearing = 2, kCallStereo = 3, kCallSlide = 4 };
 
 VoteHeader vote_header(const hb200_ctx* c, int kind, int flags = 0, int ub = 0, int ubg = 0, int uba = 0) {
-  return VoteHeader{{1.0, double(c->K), double(c->Kbg), double(c->Kba), double(kind), double(flags), double(ub), double(ubg), double(uba)}};
+  return VoteHeader{{1.0, double(c->K()), double(c->Kbg()), double(c->Kba()), double(kind), double(flags), double(ub), double(ubg), double(uba)}};
 }
 
 // One agreement round: this rank's payload (window_vote_kernel), its sum over the ranks through the channel the context
@@ -1149,9 +1257,9 @@ VoteHeader vote_header(const hb200_ctx* c, int kind, int flags = 0, int ub = 0, 
 // written to out[kAgreeOut] on the device (window_agree_kernel).  Enqueued on the context's stream: the caller's
 // existing read-back brings the result home, so a round adds no host synchronisation.
 int agree_round(hb200_ctx* c, const VoteHeader& h, const VoteSrc& src, int* out) {
-  const int len = vote_payload_len(c->K, c->Kbg, c->Kba);
+  const int len = vote_payload_len(c->K(), c->Kbg(), c->Kba());
   if (static_cast<size_t>(len) > c->w_vote.cap) HB_CUDA(c->w_vote.ensure(2 * static_cast<size_t>(len)));   // (the window grows by a knot a frame)
-  window_vote_kernel<<<1, 256, 0, c->stream>>>(c->w_vote.p, c->K, c->Kbg, c->Kba, c->k, h, src);
+  window_vote_kernel<<<1, 256, 0, c->stream>>>(c->w_vote.p, c->K(), c->Kbg(), c->Kba(), c->k(), h, src);
   HB_LAUNCH(c, "window_vote_kernel");
   if (c->nccl) {
     HB_NCCL(g_nccl.AllReduce(c->w_vote.p, c->w_vote.p, static_cast<size_t>(len), /*ncclDouble*/ 8, /*ncclSum*/ 0, c->nccl, c->stream));
@@ -1163,7 +1271,7 @@ int agree_round(hb200_ctx* c, const VoteHeader& h, const VoteSrc& src, int* out)
     if (rc) return fail(200 + rc, "all-reduce callback failed (%d)", rc);
     prof_mark(c, "allreduce_callback(window)");
   }
-  window_agree_kernel<<<1, 256, 0, c->stream>>>(c->w_vote.p, c->K, c->Kbg, c->Kba, h, out);
+  window_agree_kernel<<<1, 256, 0, c->stream>>>(c->w_vote.p, c->K(), c->Kbg(), c->Kba(), h, out);
   HB_LAUNCH(c, "window_agree_kernel");
   return 0;
 }
@@ -1196,9 +1304,9 @@ int window_outcome(hb200_ctx* c, const int* agreed, int own) {
 
 int check_ready(hb200_ctx* c) {
   if (!c) return fail(-1, "null context");
-  if (c->K == 0) return fail(-2, "spline not set");
+  if (c->K() == 0) return fail(-2, "spline not set");
   if (!c->bound) return fail(-2, "factors not bound (call hb200_bind)");
-  if (c->Ni && (!c->have_imu || !c->have_gravity || c->Kbg == 0 || c->Kba == 0)) return fail(-2, "inertial factors need IMU calibration, bias splines and gravity");
+  if (c->Ni && (!c->have_imu || !c->have_gravity || c->Kbg() == 0 || c->Kba() == 0)) return fail(-2, "inertial factors need IMU calibration, bias splines and gravity");
   if (c->Nv && (c->C == 0 || c->L == 0)) return fail(-2, "pixel / bearing factors need cameras and landmarks");
   if (c->Nm && c->P == 0) return fail(-2, "manifold factors need pose sensors");
   return 0;
@@ -1207,7 +1315,7 @@ int check_ready(hb200_ctx* c) {
 int ensure_placeholders(hb200_ctx* c) {
   // Kernels take these pointers even when a factor family is absent.
   for (int s = 0; s < 2; ++s) {
-    HB_CUDA(c->bg[s].ensure(4)); HB_CUDA(c->ba[s].ensure(4)); HB_CUDA(c->grav[s].ensure(4)); HB_CUDA(c->lms[s].ensure(3));
+    HB_CUDA(c->gyro.val[s].ensure(4)); HB_CUDA(c->accel.val[s].ensure(4)); HB_CUDA(c->grav[s].ensure(4)); HB_CUDA(c->lms[s].ensure(3));
     HB_CUDA(c->cp_pix[s].ensure(1)); HB_CUDA(c->cp_imu[s].ensure(1));
   }
   HB_CUDA(c->imu_tab.ensure(kImuStride)); HB_CUDA(c->cam_tab.ensure(kCamStride));
@@ -1310,26 +1418,14 @@ long long hb200_launch_count(hb200_ctx* c) { return c ? c->launches : 0; }
 int hb200_set_spline(hb200_ctx* c, int order, int K, const double* knots) {
   if (!c || !knots) return fail(-1, "null argument");
   if (order != 4 && order != 6) return fail(-4, "spline order %d not supported (4 or 6)", order);
-  if (K < order) return fail(-1, "need at least %d knots, got %d", order, K);
-  for (int j = 1; j < K; ++j)
-    if (!(knots[8 * j + 7] > knots[8 * (j - 1) + 7])) return fail(-1, "knot stamps must be strictly increasing (knot %d)", j);
-  {   // uniform B-spline (the reference only ever creates uniformly separated knots, abstract.cpp:89,128)
-    const double dt0 = knots[8 + 7] - knots[7];
-    for (int j = 2; j < K; ++j)
-      if (std::fabs((knots[8 * j + 7] - knots[8 * (j - 1) + 7]) - dt0) > 1e-6 * dt0) return fail(-1, "knot stamps must be uniformly spaced (knot %d)", j);
-  }
+  int rc = c->pose.check(order, K, knots, "knot");
+  if (rc) return rc;
   HB_CUDA(cudaSetDevice(c->device));
-  bool reshape = (order != c->k) || (K != c->K);
+  bool reshape = false;
+  if ((rc = c->pose.set(order, K, knots, c->stream, &reshape))) return rc;
+  for (DevBuf<double>& t : c->tab) HB_CUDA(t.ensure(static_cast<size_t>(K) * kTabStride));
   // the index maps of hb200_bind follow from the stamps: a window shifted by one knot keeps K but needs a re-bind
-  if (!reshape) for (int j = 0; j < K && !reshape; ++j) if (c->h_knot_stamp[j] != knots[8 * j + 7]) reshape = true;
-  c->h_knot_stamp.resize(K);
-  for (int j = 0; j < K; ++j) c->h_knot_stamp[j] = knots[8 * j + 7];
-  c->k = order; c->K = K;
-  compute_basis(&c->basis, order);
-  for (int s = 0; s < 2; ++s) { HB_CUDA(c->knots[s].ensure(8 * static_cast<size_t>(K))); HB_CUDA(c->tab[s].ensure(static_cast<size_t>(K) * kTabStride)); }
-  HB_CUDA(cudaMemcpyAsync(c->knots[0].p, knots, 8 * sizeof(double) * K, cudaMemcpyHostToDevice, c->stream));
-  HB_CUDA(cudaStreamSynchronize(c->stream));
-  if (reshape) { c->h_knot_const.assign(K, 0); c->bound = false; c->kernel_args_changed(); c->have_snapshot = false; int rc = update_fixed(c); if (rc) return rc; }
+  if (reshape) { c->h_knot_const.assign(K, 0); c->bound = false; c->kernel_args_changed(); c->have_snapshot = false; if ((rc = update_fixed(c))) return rc; }
   c->outputs_changed();
   return 0;
 }
@@ -1337,31 +1433,12 @@ int hb200_set_spline(hb200_ctx* c, int order, int K, const double* knots) {
 int hb200_set_bias_splines(hb200_ctx* c, int order, int Kg, const double* gyro, int Ka, const double* accel) {
   if (!c || !gyro || !accel) return fail(-1, "null argument");
   if (order != 4) return fail(-4, "bias spline order %d not supported (4)", order);
-  if (Kg < order || Ka < order) return fail(-1, "need at least %d bias knots", order);
-  for (int w = 0; w < 2; ++w) {
-    const double* b = w ? accel : gyro;
-    const int Kb = w ? Ka : Kg;
-    const double dt0 = b[4 + 3] - b[3];
-    if (!(dt0 > 0)) return fail(-1, "bias knot stamps must be strictly increasing");
-    for (int j = 2; j < Kb; ++j)
-      if (std::fabs((b[4 * j + 3] - b[4 * (j - 1) + 3]) - dt0) > 1e-6 * dt0) return fail(-1, "bias knot stamps must be uniformly spaced (knot %d)", j);
-  }
+  int rc = 0;
+  if ((rc = c->gyro.check(order, Kg, gyro, "gyroscope bias knot")) || (rc = c->accel.check(order, Ka, accel, "accelerometer bias knot"))) return rc;
   HB_CUDA(cudaSetDevice(c->device));
-  bool reshape = (Kg != c->Kbg) || (Ka != c->Kba);
-  if (!reshape) {
-    for (int j = 0; j < Kg && !reshape; ++j) if (c->h_bg_stamp[j] != gyro[4 * j + 3]) reshape = true;
-    for (int j = 0; j < Ka && !reshape; ++j) if (c->h_ba_stamp[j] != accel[4 * j + 3]) reshape = true;
-  }
-  c->h_bg_stamp.resize(Kg); c->h_ba_stamp.resize(Ka);
-  for (int j = 0; j < Kg; ++j) c->h_bg_stamp[j] = gyro[4 * j + 3];
-  for (int j = 0; j < Ka; ++j) c->h_ba_stamp[j] = accel[4 * j + 3];
-  c->kb = order; c->Kbg = Kg; c->Kba = Ka;
-  compute_basis(&c->bias_basis, order);
-  for (int s = 0; s < 2; ++s) { HB_CUDA(c->bg[s].ensure(4 * static_cast<size_t>(Kg))); HB_CUDA(c->ba[s].ensure(4 * static_cast<size_t>(Ka))); }
-  HB_CUDA(cudaMemcpyAsync(c->bg[0].p, gyro, 4 * sizeof(double) * Kg, cudaMemcpyHostToDevice, c->stream));
-  HB_CUDA(cudaMemcpyAsync(c->ba[0].p, accel, 4 * sizeof(double) * Ka, cudaMemcpyHostToDevice, c->stream));
-  HB_CUDA(cudaStreamSynchronize(c->stream));
-  if (reshape) { c->bound = false; c->kernel_args_changed(); c->have_snapshot = false; int rc = update_fixed(c); if (rc) return rc; }
+  bool reshape[2] = {false, false};
+  if ((rc = c->gyro.set(order, Kg, gyro, c->stream, &reshape[0])) || (rc = c->accel.set(order, Ka, accel, c->stream, &reshape[1]))) return rc;
+  if (reshape[0] || reshape[1]) { c->bound = false; c->kernel_args_changed(); c->have_snapshot = false; if ((rc = update_fixed(c))) return rc; }
   c->outputs_changed();
   return 0;
 }
@@ -1418,10 +1495,10 @@ int hb200_set_landmarks(hb200_ctx* c, int L, const double* xyz) {
 
 int hb200_set_constant(hb200_ctx* c, const unsigned char* knot_constant, int gravity_constant, int bias_constant) {
   if (!c) return fail(-1, "null context");
-  if (c->K == 0) return fail(-2, "spline not set");
+  if (c->K() == 0) return fail(-2, "spline not set");
   HB_CUDA(cudaSetDevice(c->device));
-  if (knot_constant) c->h_knot_const.assign(knot_constant, knot_constant + c->K);
-  else c->h_knot_const.assign(c->K, 0);
+  if (knot_constant) c->h_knot_const.assign(knot_constant, knot_constant + c->K());
+  else c->h_knot_const.assign(c->K(), 0);
   c->gravity_const = gravity_constant; c->bias_const = bias_constant;
   c->system_changed();
   return update_fixed(c);
@@ -1655,7 +1732,7 @@ int derive_window(hb200_ctx* c, int kind = 0) {
   if (Nv) {
     csr_fill_kernel<<<(Nv + 255) / 256, 256, 0, c->stream>>>(Nv, c->visual.idx.p, c->lm_off.p, c->w_cnt.p, c->lm_obs.p);
     HB_LAUNCH(c, "csr_fill_kernel");
-    csr_sort_kernel<<<(L + 127) / 128, 128, 0, c->stream>>>(L, c->lm_off.p, c->lm_obs.p, c->visual.idx.p, c->k, c->w_scal.p + 1);
+    csr_sort_kernel<<<(L + 127) / 128, 128, 0, c->stream>>>(L, c->lm_off.p, c->lm_obs.p, c->visual.idx.p, c->k(), c->w_scal.p + 1);
     HB_LAUNCH(c, "csr_sort_kernel");
   }
   // inertial runs
@@ -1677,7 +1754,7 @@ int derive_window(hb200_ctx* c, int kind = 0) {
     if (h[8 + kAgreeMismatch]) return fail(-2, "sharded window calls out of step at the band agreement: the ranks made different calls or hold different knot / bias knot counts");
     c->agreed_beta = h[8 + kAgreeBeta];
   }
-  c->max_rows = std::max(6 * c->k, h[1]);
+  c->max_rows = std::max(6 * c->k(), h[1]);
   c->schur_groups = false;   // the landmark groups are cut by hb200_bind, after this
   c->nruns = Ni ? h[3] : 0;
   if (Ni) { run_fill_kernel<<<(Ni + 255) / 256, 256, 0, c->stream>>>(Ni, c->w_keep.p, c->w_pos.p, c->nruns, c->run_off.p); HB_LAUNCH(c, "run_fill_kernel"); }
@@ -1687,7 +1764,7 @@ int derive_window(hb200_ctx* c, int kind = 0) {
   if (2 * 3 * static_cast<size_t>(rows) * sizeof(double) > 200 * 1024) return fail(-6, "landmark track spans %d control-point dofs; exceeds the Schur kernel's shared-memory tile", rows);
   // outputs and launch shapes
   HB_CUDA(c->visual.grow(std::max(Nv, 1), Nv, c->stream));
-  HB_CUDA(c->v_out.ensure(Nv, c->k)); HB_CUDA(c->i_out.ensure(Ni, c->k)); HB_CUDA(c->m_out.ensure(Nm, c->k));
+  HB_CUDA(c->v_out.ensure(Nv, c->k())); HB_CUDA(c->i_out.ensure(Ni, c->k())); HB_CUDA(c->m_out.ensure(Nm, c->k()));
   c->n_pix_blocks = (Nv + kEvalThreads - 1) / kEvalThreads;
   c->n_imu_blocks = (Ni + kEvalThreads - 1) / kEvalThreads;
   c->n_man_blocks = (Nm + kEvalThreads - 1) / kEvalThreads;
@@ -1711,14 +1788,14 @@ int derive_window(hb200_ctx* c, int kind = 0) {
 
 // Binds the visual factors at list positions [at, at + n) in place; factors that fail to bind are counted in d_invalid[0].
 int bind_pixel_range(hb200_ctx* c, int at, int n) {
-  bind_pixel_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(n, c->visual.stamp.p + at, c->knots[0].p, c->K, c->k, c->C, c->L, c->visual.idx.p + at, c->d_invalid.p);
+  bind_pixel_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(n, c->visual.stamp.p + at, c->pose.val[0].p, c->K(), c->k(), c->C, c->L, c->visual.idx.p + at, c->d_invalid.p);
   HB_LAUNCH(c, "bind_pixel_kernel");
   return 0;
 }
 
 // Binds the inertial factors at list positions [at, at + n) in place; factors that fail to bind are counted in d_invalid[0].
 int bind_inertial_range(hb200_ctx* c, int at, int n) {
-  bind_inertial_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(n, c->inertial.stamp.p + at, c->knots[0].p, c->K, c->k, c->bg[0].p, c->Kbg, c->ba[0].p, c->Kba, c->kb,
+  bind_inertial_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(n, c->inertial.stamp.p + at, c->pose.val[0].p, c->K(), c->k(), c->gyro.val[0].p, c->Kbg(), c->accel.val[0].p, c->Kba(), c->gyro.order,
                                                              c->inertial.idx.p + at, c->d_invalid.p);
   HB_LAUNCH(c, "bind_inertial_kernel");
   return 0;
@@ -1743,8 +1820,8 @@ extern "C" {
 
 int hb200_bind(hb200_ctx* c, int* num_invalid) {
   if (!c) return fail(-1, "null context");
-  if (c->K == 0) return fail(-2, "spline not set");
-  if (c->Ni && (c->Kbg == 0 || c->Kba == 0)) return fail(-2, "bias splines not set");
+  if (c->K() == 0) return fail(-2, "spline not set");
+  if (c->Ni && (c->Kbg() == 0 || c->Kba() == 0)) return fail(-2, "bias splines not set");
   if (c->Nv && (c->C == 0 || c->L == 0)) return fail(-2, "cameras / landmarks not set");
   if (c->Nm && c->P == 0) return fail(-2, "pose sensors not set");
   HB_CUDA(cudaSetDevice(c->device));
@@ -1757,7 +1834,7 @@ int hb200_bind(hb200_ctx* c, int* num_invalid) {
   if (Nv && (rc = bind_pixel_range(c, 0, Nv))) return rc;
   if (Ni && (rc = bind_inertial_range(c, 0, Ni))) return rc;
   if (Nm) {
-    bind_manifold_kernel<<<(Nm + 127) / 128, 128, 0, c->stream>>>(Nm, c->manifold.stamp.p, c->manifold.sensor.p, c->knots[0].p, c->K, c->k, c->P, c->manifold.idx.p, c->d_invalid.p);
+    bind_manifold_kernel<<<(Nm + 127) / 128, 128, 0, c->stream>>>(Nm, c->manifold.stamp.p, c->manifold.sensor.p, c->pose.val[0].p, c->K(), c->k(), c->P, c->manifold.idx.p, c->d_invalid.p);
     HB_LAUNCH(c, "bind_manifold_kernel");
   }
   std::vector<int4> vi(Nv), ii(Ni);
@@ -1809,7 +1886,7 @@ int hb200_bind(hb200_ctx* c, int* num_invalid) {
       int glo = 0;
       for (size_t i = 0; i < order.size(); ++i) {
         const int l = order[i];
-        const int lo = first[l], hi = last[l] + c->k;
+        const int lo = first[l], hi = last[l] + c->k();
         if (goff.empty() || static_cast<int>(i) - goff.back() >= kSchurGroup || hi - glo > win) { goff.push_back(static_cast<int>(i)); glo = lo; }
       }
       c->n_lm_groups = static_cast<int>(goff.size());
@@ -1879,7 +1956,7 @@ int read_visual_outputs(hb200_ctx* c, const VisualDest (&dst)[2]) {
   if (!c || !c->bound) return fail(-2, "not bound");
   { const int rs = ensure_perms(c); if (rs) return rs; }
   HB_CUDA(cudaSetDevice(c->device));
-  const size_t N = c->Nv, w = 6 * static_cast<size_t>(c->k);   // w: one row of a state Jacobian
+  const size_t N = c->Nv, w = 6 * static_cast<size_t>(c->k());   // w: one row of a state Jacobian
   if (N == 0) return 0;
   const bool Jp = dst[0].Jp || dst[1].Jp, Jl = dst[0].Jl || dst[1].Jl;
   std::vector<double> tr(2 * N), tJ(Jp ? 2 * w * N : 0), tl(Jl ? 6 * N : 0);
@@ -1906,7 +1983,7 @@ int hb200_get_bearing_outputs(hb200_ctx* c, double* r, double* Jp, double* Jl) {
 int hb200_get_manifold_outputs(hb200_ctx* c, double* r, double* Jp) {
   if (!c || !c->bound) return fail(-2, "not bound");
   HB_CUDA(cudaSetDevice(c->device));
-  const size_t N = c->Nm, w = 36 * static_cast<size_t>(c->k);
+  const size_t N = c->Nm, w = 36 * static_cast<size_t>(c->k());
   if (N == 0) return 0;
   if (r) HB_CUDA(cudaMemcpyAsync(r, c->m_out.r.p, sizeof(double) * 6 * N, cudaMemcpyDeviceToHost, c->stream));
   if (Jp) HB_CUDA(cudaMemcpyAsync(Jp, c->m_out.Jp.p, sizeof(double) * w * N, cudaMemcpyDeviceToHost, c->stream));
@@ -1918,7 +1995,7 @@ int hb200_get_inertial_outputs(hb200_ctx* c, double* r, double* Jp, double* wg, 
   if (!c || !c->bound) return fail(-2, "not bound");
   { const int rs = ensure_perms(c); if (rs) return rs; }
   HB_CUDA(cudaSetDevice(c->device));
-  const size_t N = c->Ni, w = 36 * static_cast<size_t>(c->k);
+  const size_t N = c->Ni, w = 36 * static_cast<size_t>(c->k());
   if (N == 0) return 0;
   std::vector<double> tr(6 * N), tJ(Jp ? w * N : 0), tg(wg ? 4 * N : 0), ta(wa ? 4 * N : 0), tG(Jg ? 12 * N : 0);
   HB_CUDA(cudaMemcpyAsync(tr.data(), c->i_out.r.p, sizeof(double) * 6 * N, cudaMemcpyDeviceToHost, c->stream));
@@ -1968,10 +2045,10 @@ int ensure_calib_mirror(hb200_ctx* c) {
   if (Nv) {
     HB_CUDA(dv.ensure(28 * Nv));
     const int blocks = static_cast<int>((Nv + kEvalThreads - 1) / kEvalThreads);
-    const int rc = with_order(c->k, [&](auto K) {
+    const int rc = with_order(c->k(), [&](auto K) {
       return with_flag(c->wt_visual(), [&](auto WT) {
         pixel_calib_kernel<K, WT><<<blocks, kEvalThreads, 0, c->stream>>>(c->Nv, c->visual.stamp.p, c->visual.pixel.p, c->visual.z.p, c->visual.idx.p, c->tab[0].p,
-                                                                          c->cam_tab.p, c->lms[0].p, c->basis, dv.p, c->wt.p);
+                                                                          c->cam_tab.p, c->lms[0].p, c->pose.basis, dv.p, c->wt.p);
         return check_launch(c, "pixel_calib_kernel");
       });
     });
@@ -1981,9 +2058,9 @@ int ensure_calib_mirror(hb200_ctx* c) {
   if (Ni) {
     HB_CUDA(di.ensure(216 * Ni));
     const int blocks = static_cast<int>((Ni + kEvalThreads - 1) / kEvalThreads);
-    const int rc = with_order(c->k, [&](auto K) {
+    const int rc = with_order(c->k(), [&](auto K) {
       return with_flag(c->wt_set[HB200_INERTIAL], [&](auto WT) {
-        inertial_calib_kernel<K, WT><<<blocks, kEvalThreads, 0, c->stream>>>(c->Ni, c->inertial.stamp.p, c->inertial.idx.p, c->tab[0].p, c->imu.p, c->grav[0].p, c->basis, c->quirks, di.p,
+        inertial_calib_kernel<K, WT><<<blocks, kEvalThreads, 0, c->stream>>>(c->Ni, c->inertial.stamp.p, c->inertial.idx.p, c->tab[0].p, c->imu.p, c->grav[0].p, c->pose.basis, c->quirks, di.p,
                                                                              c->wt.p);
         return check_launch(c, "inertial_calib_kernel");
       });
@@ -1994,9 +2071,9 @@ int ensure_calib_mirror(hb200_ctx* c) {
   if (Nm) {
     HB_CUDA(dm.ensure(36 * Nm));
     const int blocks = static_cast<int>((Nm + kEvalThreads - 1) / kEvalThreads);
-    const int rc = with_order(c->k, [&](auto K) {
+    const int rc = with_order(c->k(), [&](auto K) {
       return with_flag(c->wt_set[HB200_MANIFOLD], [&](auto WT) {
-        manifold_calib_kernel<K, WT><<<blocks, kEvalThreads, 0, c->stream>>>(c->Nm, c->manifold.stamp.p, c->manifold.meas.p, c->manifold.idx.p, c->tab[0].p, c->sensors.p, c->basis, dm.p, c->wt.p);
+        manifold_calib_kernel<K, WT><<<blocks, kEvalThreads, 0, c->stream>>>(c->Nm, c->manifold.stamp.p, c->manifold.meas.p, c->manifold.idx.p, c->tab[0].p, c->sensors.p, c->pose.basis, dm.p, c->wt.p);
         return check_launch(c, "manifold_calib_kernel");
       });
     });
@@ -2023,7 +2100,7 @@ int hb200_factor_evaluate(hb200_ctx* c, int kind, int index, const double* const
   const int nrs[4] = {2, 6, 1, 6};
   const int Ns[4] = {c->Np, c->Ni, c->Nb, c->Nm};
   if (!mir.valid) {
-    const size_t k = c->k, Ni = c->Ni;
+    const size_t k = c->k(), Ni = c->Ni;
     for (int f = HB200_PIXEL; f <= HB200_MANIFOLD; ++f) {
       mir.r[f].resize(static_cast<size_t>(nrs[f]) * Ns[f]);
       mir.Jp[f].resize(6 * k * nrs[f] * Ns[f]);
@@ -2037,7 +2114,7 @@ int hb200_factor_evaluate(hb200_ctx* c, int kind, int index, const double* const
     if (rc) return rc;
     mir.valid = true;
   }
-  const int k = c->k, kb = c->kb;
+  const int k = c->k(), kb = c->gyro.order;
   if (kind < HB200_PIXEL || kind > HB200_MANIFOLD) return fail(-1, "unknown factor kind %d", kind);
   if (jacobians && !mir.calib_valid) {
     // calibration blocks requested?  (constant in the live configuration, so they are produced on demand only)
@@ -2120,7 +2197,7 @@ int hb200_factor_evaluate(hb200_ctx* c, int kind, int index, const double* const
   return 0;
 }
 
-int hb200_reduced_size(hb200_ctx* c) { return c ? 6 * c->K + 3 * c->Kbg + 3 * c->Kba + 2 : -1; }
+int hb200_reduced_size(hb200_ctx* c) { return c ? 6 * c->K() + 3 * c->Kbg() + 3 * c->Kba() + 2 : -1; }
 
 int hb200_build_system(hb200_ctx* c) {
   int rc = check_ready(c);
@@ -2173,16 +2250,11 @@ void cov_info(hb200_ctx* c, hb200_covariance_info* info) {
 
 // the current state as the linearisation point of a build
 int freeze_point(hb200_ctx* c, CovPoint& pt) {
-  pt.lay = c->lay; pt.basis = c->basis; pt.bias_basis = c->bias_basis;
-  pt.L = c->L; pt.k = c->k; pt.Nv = c->Nv; pt.max_rows = c->max_rows; pt.Kbg = c->Kbg; pt.Kba = c->Kba;
-  HB_CUDA(pt.knots.ensure(8 * static_cast<size_t>(c->K)));
-  HB_CUDA(pt.tab.ensure(static_cast<size_t>(kTabStride) * c->K));
-  HB_CUDA(cudaMemcpyAsync(pt.knots.p, c->knots[0].p, sizeof(double) * 8 * c->K, cudaMemcpyDeviceToDevice, c->stream));
-  HB_CUDA(cudaMemcpyAsync(pt.tab.p, c->tab[0].p, sizeof(double) * kTabStride * c->K, cudaMemcpyDeviceToDevice, c->stream));
-  HB_CUDA(pt.bg.ensure(4 * static_cast<size_t>(c->Kbg)));
-  HB_CUDA(pt.ba.ensure(4 * static_cast<size_t>(c->Kba)));
-  if (c->Kbg) HB_CUDA(cudaMemcpyAsync(pt.bg.p, c->bg[0].p, sizeof(double) * 4 * c->Kbg, cudaMemcpyDeviceToDevice, c->stream));
-  if (c->Kba) HB_CUDA(cudaMemcpyAsync(pt.ba.p, c->ba[0].p, sizeof(double) * 4 * c->Kba, cudaMemcpyDeviceToDevice, c->stream));
+  pt.lay = c->lay; pt.L = c->L; pt.Nv = c->Nv; pt.max_rows = c->max_rows;
+  int rc = 0;
+  if ((rc = pt.pose.freeze(c->pose, c->stream)) || (rc = pt.gyro.freeze(c->gyro, c->stream)) || (rc = pt.accel.freeze(c->accel, c->stream))) return rc;
+  HB_CUDA(pt.tab.ensure(static_cast<size_t>(kTabStride) * c->K()));
+  HB_CUDA(cudaMemcpyAsync(pt.tab.p, c->tab[0].p, sizeof(double) * kTabStride * c->K(), cudaMemcpyDeviceToDevice, c->stream));
   return 0;
 }
 
@@ -2200,7 +2272,7 @@ int cov_interpolate(hb200_ctx* c, int n, const double* stamps, double* cov, int*
   HB_CUDA(c->cov_t.ensure(n)); HB_CUDA(c->cov_o.ensure(block * n)); HB_CUDA(c->cov_bad.ensure(n));
   HB_CUDA(cudaMemcpyAsync(c->cov_t.p, stamps, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
   const CovPoint& pt = c->cov_pt[c->cov_slot_committed];
-  const int rc = with_order(pt.basis.k, [&](auto K) { return launch(K, pt); });
+  const int rc = with_order(pt.pose.order, [&](auto K) { return launch(K, pt); });
   if (rc) return rc;
   std::vector<int> bad(n);
   HB_CUDA(cudaMemcpyAsync(cov, c->cov_o.p, sizeof(double) * block * n, cudaMemcpyDeviceToHost, c->stream));
@@ -2216,8 +2288,8 @@ bool cov_request_ok(const int4& r, const CovPoint& pt) {
   auto ok = [&](int kind, int i) {
     switch (kind) {
       case kCovKnot: return i >= 0 && i < pt.lay.K;
-      case kCovGyroBias: return i >= 0 && i < pt.Kbg;
-      case kCovAccelBias: return i >= 0 && i < pt.Kba;
+      case kCovGyroBias: return i >= 0 && i < pt.gyro.n();
+      case kCovAccelBias: return i >= 0 && i < pt.accel.n();
       case kCovGravity: return i == 0;
       case kCovLandmark: return i >= 0 && i < pt.L;
       default: return false;
@@ -2244,13 +2316,13 @@ int cov_blocks_enqueue(hb200_ctx* c, const CovPoint& pt) {
   const bool landmarks = pt.Nv && std::any_of(c->cov_req.begin(), c->cov_req.end(), [](const int4& r) { return r.x == kCovLandmark || r.z == kCovLandmark; });
   HB_CUDA(c->cov_span.ensure(span.size()));
   if (landmarks) {
-    cov_landmark_span_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(n, c->cov_req_d.p, c->lm_off.p, c->lm_obs.p, c->visual.idx.p, pt.k, c->cov_span.p);
+    cov_landmark_span_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(n, c->cov_req_d.p, c->lm_off.p, c->lm_obs.p, c->visual.idx.p, pt.pose.order, c->cov_span.p);
     HB_LAUNCH(c, "cov_landmark_span_kernel");
   }
   if (npair) {
     HB_CUDA(c->cov_pairs_d.ensure(2 * static_cast<size_t>(npair)));
     HB_CUDA(cudaMemcpyAsync(c->cov_pairs_d.p, c->cov_pairs.data(), sizeof(double) * 2 * npair, cudaMemcpyHostToDevice, c->stream));
-    cov_stamp_span_kernel<<<(npair + 127) / 128, 128, 0, c->stream>>>(npair, c->cov_pairs_d.p, pt.knots.p, K, pt.k, c->cov_span.p + 2 * n);
+    cov_stamp_span_kernel<<<(npair + 127) / 128, 128, 0, c->stream>>>(npair, c->cov_pairs_d.p, pt.pose.val[0].p, K, pt.pose.order, c->cov_span.p + 2 * n);
     HB_LAUNCH(c, "cov_stamp_span_kernel");
   }
   if (landmarks || npair) {
@@ -2278,8 +2350,8 @@ int cov_blocks_enqueue(hb200_ctx* c, const CovPoint& pt) {
   for (int q = 0; q < npair; ++q) {
     const int2 s = span[2 * static_cast<size_t>(n) + q];
     if (s.x < 0 || s.y < 0) continue;
-    for (int a = s.x; a < s.x + pt.k; ++a)
-      for (int b = s.y; b < s.y + pt.k; ++b) far(a, b);
+    for (int a = s.x; a < s.x + pt.pose.order; ++a)
+      for (int b = s.y; b < s.y + pt.pose.order; ++b) far(a, b);
   }
   std::vector<int> plan(K, -1);
   int nc = 0, blocks = 0;
@@ -2308,17 +2380,17 @@ int cov_blocks_enqueue(hb200_ctx* c, const CovPoint& pt) {
   HB_CUDA(next.pair_rel.ensure(36 * static_cast<size_t>(npair)));
   HB_CUDA(next.pair_st.ensure(npair));
   const size_t smem = static_cast<size_t>(kLmWarps) * 6 * pt.max_rows * sizeof(double);
-  return with_order(pt.k, [&](auto Kc) {
+  return with_order(pt.pose.order, [&](auto Kc) {
     if (n) {
       HB_CUDA(cudaFuncSetAttribute(cov_cross_landmark_kernel<Kc>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
       cov_cross_landmark_kernel<Kc><<<(n + kLmWarps - 1) / kLmWarps, kLmWarps * 32, smem, c->stream>>>(
           n, c->cov_req_d.p, c->lm_off.p, c->lm_obs.p, c->visual.idx.p, c->v_out.Jp.p, c->v_out.Jl.p, c->v_out.w.p, c->Vchol.p, next.packed.p, next.lm.p,
-          c->cov_far.p, fp, lay, pt.Kbg, c->multi() ? 1 : 0, c->cov_status.p, pt.max_rows, next.blk.p, next.blk_st.p);
+          c->cov_far.p, fp, lay, pt.gyro.n(), c->multi() ? 1 : 0, c->cov_status.p, pt.max_rows, next.blk.p, next.blk_st.p);
       if (const int rc = check_launch(c, "cov_cross_landmark_kernel")) return rc;
     }
     if (npair) {
       cov_pose_pair_kernel<Kc><<<(npair + kPairWarps - 1) / kPairWarps, kPairWarps * 32, 0, c->stream>>>(
-          npair, c->cov_pairs_d.p, c->cov_span.p + 2 * n, pt.tab.p, pt.basis, next.packed.p, c->cov_far.p, fp, lay, c->cov_status.p,
+          npair, c->cov_pairs_d.p, c->cov_span.p + 2 * n, pt.tab.p, pt.pose.basis, next.packed.p, c->cov_far.p, fp, lay, c->cov_status.p,
           next.pair_joint.p, next.pair_rel.p, next.pair_st.p);
       if (const int rc = check_launch(c, "cov_pose_pair_kernel")) return rc;
     }
@@ -2394,7 +2466,7 @@ int hb200_compute_covariance(hb200_ctx* c, hb200_covariance_info* info) {
   // every setter that changes shapes, constants or the state clears cov_built; any other launch since the build (an
   // evaluation, an iteration, a slide) rewrote the factor outputs or the packed buffer the compute reads
   const CovPoint& pt = c->cov_pt[c->cov_slot_built];
-  if (!c->cov_built || c->cov_at != c->launches || c->L != pt.L || c->k != pt.k || c->Nv != pt.Nv ||
+  if (!c->cov_built || c->cov_at != c->launches || c->L != pt.L || c->k() != pt.pose.order || c->Nv != pt.Nv ||
       c->max_rows != pt.max_rows || c->lay.total != pt.lay.total || c->lay.beta != pt.lay.beta)
     return fail(-2, "call hb200_build_covariance first (the window was evaluated, iterated or changed since)");
   HB_CUDA(cudaSetDevice(c->device));
@@ -2411,7 +2483,7 @@ int hb200_compute_covariance(hb200_ctx* c, hb200_covariance_info* info) {
   const SysLayout& lay = pt.lay;
   const size_t smem = cov_smem_doubles(lay.beta, lay.m) * sizeof(double);
   HB_CUDA(c->cov_ws.ensure(static_cast<size_t>(cov_workspace_doubles(lay))));
-  const int L = pt.L, k = pt.k, max_rows = pt.max_rows;   // (the build's shapes)
+  const int L = pt.L, k = pt.pose.order, max_rows = pt.max_rows;   // (the build's shapes)
   CovResults& next = c->cov_next;
   HB_CUDA(next.packed.ensure(static_cast<size_t>(cov_packed_doubles(lay))));
   HB_CUDA(next.lm.ensure(9 * static_cast<size_t>(std::max(L, 1))));
@@ -2518,7 +2590,7 @@ int hb200_get_covariance(hb200_ctx* c, double* packed, double* landmark) {
 int hb200_interpolate_covariance(hb200_ctx* c, int n, const double* stamps, double* cov, int* num_invalid) {
   return cov_interpolate(c, n, stamps, cov, num_invalid, 36, [&](auto K, const CovPoint& pt) {
     cov_stamp_kernel<K, 6><<<(n + kStateWarps - 1) / kStateWarps, kStateWarps * 32, 0, c->stream>>>(
-        n, c->cov_t.p, pt.knots.p, pt.tab.p, pt.lay.K, pt.basis, nullptr, 0, nullptr, 0, pt.bias_basis, c->cov_res.packed.p, pt.lay, c->cov_o.p, c->cov_bad.p);
+        n, c->cov_t.p, pt.pose.val[0].p, pt.tab.p, pt.lay.K, pt.pose.basis, nullptr, 0, nullptr, 0, pt.gyro.basis, c->cov_res.packed.p, pt.lay, c->cov_o.p, c->cov_bad.p);
     return check_launch(c, "cov_stamp_kernel");
   });
 }
@@ -2527,7 +2599,7 @@ int hb200_interpolate_state_covariance(hb200_ctx* c, int n, const double* stamps
   static_assert(HB200_STATE_COV_DIM == kStateDim, "state covariance dimension");
   return cov_interpolate(c, n, stamps, cov, num_invalid, HB200_STATE_COV_DIM * HB200_STATE_COV_DIM, [&](auto K, const CovPoint& pt) {
     cov_stamp_kernel<K, kStateDim><<<(n + kStateWarps - 1) / kStateWarps, kStateWarps * 32, 0, c->stream>>>(
-        n, c->cov_t.p, pt.knots.p, pt.tab.p, pt.lay.K, pt.basis, pt.bg.p, pt.Kbg, pt.ba.p, pt.Kba, pt.bias_basis, c->cov_res.packed.p, pt.lay, c->cov_o.p, c->cov_bad.p);
+        n, c->cov_t.p, pt.pose.val[0].p, pt.tab.p, pt.lay.K, pt.pose.basis, pt.gyro.val[0].p, pt.gyro.n(), pt.accel.val[0].p, pt.accel.n(), pt.gyro.basis, c->cov_res.packed.p, pt.lay, c->cov_o.p, c->cov_bad.p);
     return check_launch(c, "cov_stamp_kernel");
   });
 }
@@ -2681,9 +2753,10 @@ int hb200_optimize(hb200_ctx* c, int iterations, double* knots, double* gyro, do
   HB_CUDA(cudaSetDevice(c->device));
   // the blocks alias the caller's variables, stamps included: the bound index maps are only valid for the stamps
   // they were computed from (a slid window needs hb200_set_spline / hb200_slide + hb200_bind first)
-  if (knots) for (int j = 0; j < c->K; ++j) if (knots[8 * j + 7] != c->h_knot_stamp[j]) return fail(-2, "knot %d: stamp differs from the bound window (re-bind after changing stamps)", j);
-  if (gyro) for (int j = 0; j < c->Kbg; ++j) if (gyro[4 * j + 3] != c->h_bg_stamp[j]) return fail(-2, "gyroscope bias knot %d: stamp differs from the bound window", j);
-  if (accel) for (int j = 0; j < c->Kba; ++j) if (accel[4 * j + 3] != c->h_ba_stamp[j]) return fail(-2, "accelerometer bias knot %d: stamp differs from the bound window", j);
+  int j = -1;
+  if (knots && (j = c->pose.mismatch(knots)) >= 0) return fail(-2, "knot %d: stamp differs from the bound window (re-bind after changing stamps)", j);
+  if (gyro && (j = c->gyro.mismatch(gyro)) >= 0) return fail(-2, "gyroscope bias knot %d: stamp differs from the bound window", j);
+  if (accel && (j = c->accel.mismatch(accel)) >= 0) return fail(-2, "accelerometer bias knot %d: stamp differs from the bound window", j);
   const auto blocks = c->state_blocks();
   double* host[5] = {knots, gyro, accel, gravity, landmarks};
   double* dev[5];
@@ -2870,7 +2943,7 @@ int hb200_profile_iteration(hb200_ctx* c, int reps, int max_entries, char* names
 
 int hb200_interpolate(hb200_ctx* c, int n, const double* stamps, double* pose, double* velocity, double* acceleration, int* num_invalid) {
   if (!c || n < 0 || (n > 0 && (!stamps || !pose))) return fail(-1, "invalid argument");
-  if (c->K == 0) return fail(-2, "spline not set");
+  if (c->K() == 0) return fail(-2, "spline not set");
   HB_CUDA(cudaSetDevice(c->device));
   if (num_invalid) *num_invalid = 0;
   if (n == 0) return 0;
@@ -2881,10 +2954,10 @@ int hb200_interpolate(hb200_ctx* c, int n, const double* stamps, double* pose, d
   HB_CUDA(c->d_invalid.ensure(1));
   HB_CUDA(cudaMemsetAsync(c->d_invalid.p, 0, sizeof(int), c->stream));
   HB_CUDA(cudaMemcpyAsync(d_t.p, stamps, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
-  prep_kernel<<<(c->K + 63) / 64, 64, 0, c->stream>>>(c->K, c->knots[0].p, c->tab[0].p, nullptr, 0);
+  prep_kernel<<<(c->K() + 63) / 64, 64, 0, c->stream>>>(c->K(), c->pose.val[0].p, c->tab[0].p, nullptr, 0);
   HB_LAUNCH(c, "prep_kernel");
-  const int rc = with_order(c->k, [&](auto K) {
-    interpolate_kernel<K><<<(n + 127) / 128, 128, 0, c->stream>>>(n, d_t.p, c->knots[0].p, c->tab[0].p, c->K, c->basis, d_p.p, d_v.p, d_a.p, c->d_invalid.p);
+  const int rc = with_order(c->k(), [&](auto K) {
+    interpolate_kernel<K><<<(n + 127) / 128, 128, 0, c->stream>>>(n, d_t.p, c->pose.val[0].p, c->tab[0].p, c->K(), c->pose.basis, d_p.p, d_v.p, d_a.p, c->d_invalid.p);
     return check_launch(c, "interpolate_kernel");
   });
   if (rc) return rc;
@@ -2907,7 +2980,7 @@ int hb200_debug_band_timing(hb200_ctx* c, long long* cycles /*[144]: per CTA, 8 
 }
 
 int hb200_snapshot(hb200_ctx* c) {
-  if (!c || c->K == 0) return fail(-2, "spline not set");
+  if (!c || c->K() == 0) return fail(-2, "spline not set");
   HB_CUDA(cudaSetDevice(c->device));
   const auto blocks = c->state_blocks();
   for (const auto& b : blocks) HB_CUDA(b.snap->ensure(std::max<size_t>(b.count, 1)));
@@ -2934,7 +3007,7 @@ int hb200_restore(hb200_ctx* c) {
 int hb200_ingest_stereo(hb200_ctx* c, int n, const double* stamp, const int* camera0, const int* camera1, const double* pixel0,
                         const double* pixel1, double* bearing0, double* bearing1, double* landmark, int* num_invalid) {
   if (!c || n < 0) return fail(-1, "invalid arguments");
-  if (c->K == 0 || c->C == 0) return fail(-2, "spline / cameras not set");
+  if (c->K() == 0 || c->C == 0) return fail(-2, "spline / cameras not set");
   if (n > 0 && (!stamp || !camera0 || !camera1 || !pixel0 || !pixel1 || !bearing0 || !bearing1 || !landmark)) return fail(-1, "null argument");
   if (num_invalid) *num_invalid = 0;
   if (n == 0) return 0;
@@ -2951,10 +3024,10 @@ int hb200_ingest_stereo(hb200_ctx* c, int n, const double* stamp, const int* cam
   HB_CUDA(cudaMemcpyAsync(d_c1.p, camera1, sizeof(int) * N, cudaMemcpyHostToDevice, c->stream));
   HB_CUDA(cudaMemcpyAsync(d_p0.p, pixel0, sizeof(double) * 2 * N, cudaMemcpyHostToDevice, c->stream));
   HB_CUDA(cudaMemcpyAsync(d_p1.p, pixel1, sizeof(double) * 2 * N, cudaMemcpyHostToDevice, c->stream));
-  prep_kernel<<<(c->K + 63) / 64, 64, 0, c->stream>>>(c->K, c->knots[0].p, c->tab[0].p, nullptr, 0);
+  prep_kernel<<<(c->K() + 63) / 64, 64, 0, c->stream>>>(c->K(), c->pose.val[0].p, c->tab[0].p, nullptr, 0);
   HB_LAUNCH(c, "prep_kernel");
-  const int rc = with_order(c->k, [&](auto K) {
-    ingest_stereo_kernel<K><<<(n + 127) / 128, 128, 0, c->stream>>>(n, d_t.p, d_c0.p, d_c1.p, d_p0.p, d_p1.p, c->knots[0].p, c->tab[0].p, c->K, c->basis, c->cams.p, c->C, d_b0.p, d_b1.p, d_lm.p, c->d_invalid.p);
+  const int rc = with_order(c->k(), [&](auto K) {
+    ingest_stereo_kernel<K><<<(n + 127) / 128, 128, 0, c->stream>>>(n, d_t.p, d_c0.p, d_c1.p, d_p0.p, d_p1.p, c->pose.val[0].p, c->tab[0].p, c->K(), c->pose.basis, c->cams.p, c->C, d_b0.p, d_b1.p, d_lm.p, c->d_invalid.p);
     return check_launch(c, "ingest_stereo_kernel");
   });
   if (rc) return rc;
@@ -3029,18 +3102,9 @@ int hb200_append_knots(hb200_ctx* c, int count) {
   if (rc) return rc;
   if (count <= 0) return fail(-1, "count must be positive");
   HB_CUDA(cudaSetDevice(c->device));
-  const int K = c->K;
-  for (int s2 = 0; s2 < 2; ++s2) {
-    HB_CUDA(c->knots[s2].grow(8 * static_cast<size_t>(K + count), s2 == 0 ? 8 * static_cast<size_t>(K) : 0, c->stream));
-    HB_CUDA(c->tab[s2].ensure(static_cast<size_t>(K + count) * kTabStride));
-  }
-  append_knots_kernel<<<1, 32, 0, c->stream>>>(K, count, 8, 7, c->knots[0].p);
-  HB_LAUNCH(c, "append_knots_kernel");
-  std::vector<double> tail(8 * static_cast<size_t>(count));
-  HB_CUDA(cudaMemcpyAsync(tail.data(), c->knots[0].p + 8 * static_cast<size_t>(K), sizeof(double) * tail.size(), cudaMemcpyDeviceToHost, c->stream));
-  HB_CUDA(cudaStreamSynchronize(c->stream));
-  for (int i = 0; i < count; ++i) { c->h_knot_stamp.push_back(tail[8 * i + 7]); c->h_knot_const.push_back(0); }
-  c->K = K + count;
+  for (DevBuf<double>& t : c->tab) HB_CUDA(t.ensure(static_cast<size_t>(c->K() + count) * kTabStride));
+  if ((rc = c->pose.append(c, count))) return rc;
+  c->h_knot_const.insert(c->h_knot_const.end(), count, 0);
   if ((rc = update_fixed(c))) return rc;
   if ((rc = ensure_system(c))) return rc;
   HB_CUDA(cudaStreamSynchronize(c->stream));
@@ -3048,70 +3112,27 @@ int hb200_append_knots(hb200_ctx* c, int count) {
   return 0;   // replicated: every rank appends the same knots, the agreed band half-width stays what it was
 }
 
-}  // extern "C"
-
-namespace {
-// Fewest knots append_knots_kernel must append to a bias spline (stamps s, order kb) so that segment_base accepts t:
-// s[left] <= t < s'[K' - right] (left = (kb-1)/2, right = kb-1-left) over the K' extended stamps s', where new stamp
-// K - 1 + i is fma(i, dt, s[K-1]) with dt = s[K-1] - s[K-2].  0 on success, 2 for t before the span, -1 past HB200_BIAS_APPEND_MAX.
-int bias_append_count(const std::vector<double>& s, int kb, double t, int* count) {
-  const int K = static_cast<int>(s.size()), left = (kb - 1) / 2, right = kb - 1 - left;
-  const double dt = s[K - 1] - s[K - 2];
-  auto end_of = [&](int added) {   // the valid span's end with `added` knots appended: stamp of knot K + added - right
-    const int j = K + added - right;
-    return j < K ? s[j] : std::fma(static_cast<double>(j - (K - 1)), dt, s[K - 1]);
-  };
-  *count = 0;
-  if (t < s[left]) return 2;
-  if (t < end_of(0)) return 0;
-  const double est = std::floor((t - s[K - 1]) / dt) + right;   // first guess; the loops below decide
-  if (!(est <= HB200_BIAS_APPEND_MAX + 1.0)) return -1;
-  int n = std::max(1, static_cast<int>(est));
-  while (n > 1 && t < end_of(n - 1)) --n;
-  while (!(t < end_of(n)) && n <= HB200_BIAS_APPEND_MAX) ++n;
-  if (n > HB200_BIAS_APPEND_MAX) return -1;
-  *count = n;
-  return 0;
-}
-}  // namespace
-
-extern "C" {
-
 int hb200_append_bias_knots(hb200_ctx* c, double stamp, int* gyro_added, int* accel_added) {
   if (gyro_added) *gyro_added = 0;
   if (accel_added) *accel_added = 0;
   if (!c) return fail(-1, "null context");
-  if (c->Kbg == 0 || c->Kba == 0) return fail(-2, "bias splines not set");
+  if (c->Kbg() == 0 || c->Kba() == 0) return fail(-2, "bias splines not set");
   int rc = check_device_window(c);
   if (rc) return rc;
   if (!std::isfinite(stamp)) return fail(-1, "stamp is not finite");
   int add[2] = {0, 0};
+  Spline* bias[2] = {&c->gyro, &c->accel};
   for (int w = 0; w < 2; ++w) {
-    rc = bias_append_count(w ? c->h_ba_stamp : c->h_bg_stamp, c->kb, stamp, &add[w]);
+    rc = bias_append_count(*bias[w], stamp, &add[w]);
     if (rc == 2) return fail(2, "stamp %.17g lies before the %s bias spline's valid span (bias knots are never prepended)", stamp, w ? "accelerometer" : "gyroscope");
     if (rc) return fail(-1, "stamp %.17g needs more than %d new %s bias knots", stamp, HB200_BIAS_APPEND_MAX, w ? "accelerometer" : "gyroscope");
   }
   if (add[0] == 0 && add[1] == 0) return 0;
   HB_CUDA(cudaSetDevice(c->device));
-  DevBuf<double>* bias[2] = {c->bg, c->ba};
-  const int Kb[2] = {c->Kbg, c->Kba};
-  for (int w = 0; w < 2; ++w)   // both state copies, contents kept, before anything changes
-    for (int s2 = 0; s2 < 2 && add[w]; ++s2) HB_CUDA(bias[w][s2].grow(4 * static_cast<size_t>(Kb[w] + add[w]), 4 * static_cast<size_t>(Kb[w]), c->stream));
-  for (int w = 0; w < 2; ++w) {
-    if (!add[w]) continue;
-    append_knots_kernel<<<1, 32, 0, c->stream>>>(Kb[w], add[w], 4, 3, bias[w][0].p);
-    HB_LAUNCH(c, "append_knots_kernel");
-  }
-  // the host stamp mirrors (hb200_optimize checks bias stamps against them) from the device's own results
-  for (int w = 0; w < 2; ++w) {
-    if (!add[w]) continue;
-    std::vector<double> tail(4 * static_cast<size_t>(add[w]));
-    HB_CUDA(cudaMemcpyAsync(tail.data(), bias[w][0].p + 4 * static_cast<size_t>(Kb[w]), sizeof(double) * tail.size(), cudaMemcpyDeviceToHost, c->stream));
-    HB_CUDA(cudaStreamSynchronize(c->stream));
-    std::vector<double>& hs = w ? c->h_ba_stamp : c->h_bg_stamp;
-    for (int i = 0; i < add[w]; ++i) hs.push_back(tail[4 * i + 3]);
-  }
-  c->Kbg = static_cast<int>(c->h_bg_stamp.size()); c->Kba = static_cast<int>(c->h_ba_stamp.size());
+  for (int w = 0; w < 2; ++w)   // both splines' copies, contents kept, before anything changes
+    if ((rc = bias[w]->reserve(add[w], c->stream))) return rc;
+  for (int w = 0; w < 2; ++w)
+    if (add[w] && (rc = bias[w]->append(c, add[w]))) return rc;
   if (gyro_added) *gyro_added = add[0];
   if (accel_added) *accel_added = add[1];
   if ((rc = update_fixed(c))) return rc;
@@ -3123,10 +3144,10 @@ int hb200_append_bias_knots(hb200_ctx* c, double stamp, int* gyro_added, int* ac
 
 int hb200_bias_knots(hb200_ctx* c, int* num_gyro, int* num_accel, int* gyro_dropped, int* accel_dropped) {
   if (!c) return fail(-1, "null context");
-  if (num_gyro) *num_gyro = c->Kbg;
-  if (num_accel) *num_accel = c->Kba;
-  if (gyro_dropped) *gyro_dropped = c->bg_dropped;
-  if (accel_dropped) *accel_dropped = c->ba_dropped;
+  if (num_gyro) *num_gyro = c->Kbg();
+  if (num_accel) *num_accel = c->Kba();
+  if (gyro_dropped) *gyro_dropped = c->gyro.dropped;
+  if (accel_dropped) *accel_dropped = c->accel.dropped;
   return 0;
 }
 
@@ -3171,7 +3192,7 @@ int hb200_append_manifold_factors(hb200_ctx* c, int n, const double* stamp, cons
   HB_CUDA(cudaMemcpyAsync(c->manifold.stamp.p + Nm, stamp, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
   HB_CUDA(cudaMemcpyAsync(c->manifold.meas.p + 7 * Nm, pose, sizeof(double) * 7 * n, cudaMemcpyHostToDevice, c->stream));
   HB_CUDA(cudaMemcpyAsync(c->manifold.sensor.p + Nm, sensor, sizeof(int) * n, cudaMemcpyHostToDevice, c->stream));
-  bind_manifold_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(n, c->manifold.stamp.p + Nm, c->manifold.sensor.p + Nm, c->knots[0].p, c->K, c->k, c->P, c->manifold.idx.p + Nm, c->d_invalid.p);
+  bind_manifold_kernel<<<(n + 127) / 128, 128, 0, c->stream>>>(n, c->manifold.stamp.p + Nm, c->manifold.sensor.p + Nm, c->pose.val[0].p, c->K(), c->k(), c->P, c->manifold.idx.p + Nm, c->d_invalid.p);
   HB_LAUNCH(c, "bind_manifold_kernel");
   int bad = 0;
   HB_CUDA(cudaMemcpyAsync(&bad, c->d_invalid.p, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
@@ -3214,11 +3235,11 @@ int hb200_append_stereo_tracks(hb200_ctx* c, int n, const double* stamp, const i
     int* d_rank = c->trk_i.p + 4 * N;
     scan_kernel<<<1, 1024, 0, c->stream>>>(c->trk_i.p + 3 * N, n, d_rank, c->d_invalid.p + 2);
     HB_LAUNCH(c, "scan_kernel");
-    prep_kernel<<<(c->K + 63) / 64, 64, 0, c->stream>>>(c->K, c->knots[0].p, c->tab[0].p, nullptr, 0);   // knot table of the current state
+    prep_kernel<<<(c->K() + 63) / 64, 64, 0, c->stream>>>(c->K(), c->pose.val[0].p, c->tab[0].p, nullptr, 0);   // knot table of the current state
     HB_LAUNCH(c, "prep_kernel");
-    rc = with_order(c->k, [&](auto K) {
-      stereo_track_kernel<K><<<(n + 127) / 128, 128, 0, c->stream>>>(n, d_t, c->trk_i.p, c->trk_i.p + N, d_t + N, d_t + 3 * N, d_lm, d_rank, c->knots[0].p, c->tab[0].p, c->K,
-                                                                    c->basis, c->cams.p, c->C, static_cast<int>(L), static_cast<int>(Nv), c->visual.stamp.p, c->visual.pixel.p, c->visual.z.p,
+    rc = with_order(c->k(), [&](auto K) {
+      stereo_track_kernel<K><<<(n + 127) / 128, 128, 0, c->stream>>>(n, d_t, c->trk_i.p, c->trk_i.p + N, d_t + N, d_t + 3 * N, d_lm, d_rank, c->pose.val[0].p, c->tab[0].p, c->K(),
+                                                                    c->pose.basis, c->cams.p, c->C, static_cast<int>(L), static_cast<int>(Nv), c->visual.stamp.p, c->visual.pixel.p, c->visual.z.p,
                                                                     c->visual.idx.p, c->lms[0].p, c->d_invalid.p);
       return check_launch(c, "stereo_track_kernel");
     });
@@ -3246,7 +3267,7 @@ int hb200_append_inertial_factors(hb200_ctx* c, int n, const double* stamp, cons
   int rc = check_device_window(c);
   if (rc) return rc;
   if (n <= 0 || !stamp || !meas) return fail(-1, "invalid inertial factors");
-  if (!c->have_imu || c->Kbg == 0 || c->Kba == 0) return fail(-2, "inertial factors need IMU calibration and bias splines");
+  if (!c->have_imu || c->Kbg() == 0 || c->Kba() == 0) return fail(-2, "inertial factors need IMU calibration and bias splines");
   HB_CUDA(cudaSetDevice(c->device));
   const size_t Ni = c->Ni;
   HB_CUDA(c->inertial.grow(Ni + n, Ni, c->stream));
@@ -3271,14 +3292,11 @@ int hb200_slide(hb200_ctx* c, double lower_bound, int flags, hb200_slide_stats* 
   int rc = check_device_window(c);
   if (rc) return rc;
   HB_CUDA(cudaSetDevice(c->device));
-  const int Nv = c->Nv, Ni = c->Ni, Nm = c->Nm, L = c->L, K = c->K;
-  // knot index of the last state element at or before the lower bound; the window keeps `left padding` elements in
-  // front of the one that starts the lower bound's interval (reference optimizer.cpp:289: prev(upper_bound(lower), left_padding))
-  int ub = static_cast<int>(std::upper_bound(c->h_knot_stamp.begin(), c->h_knot_stamp.end(), lower_bound) - c->h_knot_stamp.begin());
-  const int begin = std::max(0, ub - 1 - (c->k - 1) / 2);
+  const int Nv = c->Nv, Ni = c->Ni, Nm = c->Nm, L = c->L;
+  const int ub = c->pose.upper(lower_bound);
   const int last_const = ub - 1;   // knots 0 .. last_const have stamp <= lower bound
   // leading bias knots go only with the inertial factors that reached them: without DROP_INERTIAL nothing is dropped
-  const bool drop_bias = (flags & HB200_SLIDE_DROP_BIAS) && (flags & HB200_SLIDE_DROP_INERTIAL) && c->Kbg && c->Kba;
+  const bool drop_bias = (flags & HB200_SLIDE_DROP_BIAS) && (flags & HB200_SLIDE_DROP_INERTIAL) && c->Kbg() && c->Kba();
   HB_CUDA(c->w_scal.ensure(10 + kAgreeOut));
   // [L_new, Nv_new, Ni_new, min base visual, min base inertial, Nm_new, min base manifold, kept bearing factors,
   //  min gyro bias base, min accel bias base (kept inertial factors) | agreement (sharded contexts)]
@@ -3304,23 +3322,22 @@ int hb200_slide(hb200_ctx* c, double lower_bound, int flags, hb200_slide_stats* 
     HB_LAUNCH(c, "scan_kernel");
   }
   if (Ni) {
-    inertial_keep_kernel<<<(Ni + 255) / 256, 256, 0, c->stream>>>(Ni, c->inertial.idx.p, c->k, (flags & HB200_SLIDE_DROP_INERTIAL) ? last_const : -1, i_keep, c->w_scal.p + 4,
+    inertial_keep_kernel<<<(Ni + 255) / 256, 256, 0, c->stream>>>(Ni, c->inertial.idx.p, c->k(), (flags & HB200_SLIDE_DROP_INERTIAL) ? last_const : -1, i_keep, c->w_scal.p + 4,
                                                                   drop_bias ? c->w_scal.p + 8 : nullptr);
     HB_LAUNCH(c, "inertial_keep_kernel");
     scan_kernel<<<1, 1024, 0, c->stream>>>(i_keep, Ni, i_pos, c->w_scal.p + 2);
     HB_LAUNCH(c, "scan_kernel");
   }
   if (Nm) {   // the reference never removes pose residuals either: same rule as the inertial ones, its own flag
-    inertial_keep_kernel<<<(Nm + 255) / 256, 256, 0, c->stream>>>(Nm, c->manifold.idx.p, c->k, (flags & HB200_SLIDE_DROP_MANIFOLD) ? last_const : -1, m_keep, c->w_scal.p + 6);
+    inertial_keep_kernel<<<(Nm + 255) / 256, 256, 0, c->stream>>>(Nm, c->manifold.idx.p, c->k(), (flags & HB200_SLIDE_DROP_MANIFOLD) ? last_const : -1, m_keep, c->w_scal.p + 6);
     HB_LAUNCH(c, "manifold_keep_kernel");
     scan_kernel<<<1, 1024, 0, c->stream>>>(m_keep, Nm, m_pos, c->w_scal.p + 5);
     HB_LAUNCH(c, "scan_kernel");
   }
   // sharded: round A of the agreement -- the smallest kept knot and bias bases over the ranks, before anything moves
-  auto ub_of = [&](const std::vector<double>& s) { return static_cast<int>(std::upper_bound(s.begin(), s.end(), lower_bound) - s.begin()); };
   if (c->multi()) {
     int* w = c->w_scal.p;
-    rc = agree_round(c, vote_header(c, kCallSlide, flags, ub, ub_of(c->h_bg_stamp), ub_of(c->h_ba_stamp)),
+    rc = agree_round(c, vote_header(c, kCallSlide, flags, ub, c->gyro.upper(lower_bound), c->accel.upper(lower_bound)),
                      VoteSrc{nullptr, {w + 3, w + 4, w + 6}, drop_bias ? w + 8 : nullptr, nullptr}, w + 10);
     if (rc) return rc;
   }
@@ -3334,17 +3351,9 @@ int hb200_slide(hb200_ctx* c, double lower_bound, int flags, hb200_slide_stats* 
   const int L_new = L ? h[0] : 0, Nv_new = Nv ? h[1] : 0, Ni_new = Ni ? h[2] : 0, Nm_new = Nm ? h[5] : 0, Nb_new = Nv ? h[7] : 0;
   const int knot_min = c->multi() ? h[10 + kAgreeKnotMin] : std::min(h[6], std::min(h[3], h[4]));
   const int gyro_min = c->multi() ? h[10 + kAgreeGyroMin] : h[8], accel_min = c->multi() ? h[10 + kAgreeAccelMin] : h[9];
-  // state elements in front of `begin` go once no residual touches them (reference optimizer.cpp:331-341)
-  int shift = std::min(begin, knot_min);
-  shift = std::max(0, std::min(shift, K - c->k));
-  const int K_new = K - shift;
-  // the same rule on each bias spline, with the smallest bias base of the kept inertial factors
-  auto bias_shift = [&](const std::vector<double>& s, int min_base) {
-    const int sh = std::min(std::max(0, ub_of(s) - 1 - (c->kb - 1) / 2), min_base);
-    return std::max(0, std::min(sh, static_cast<int>(s.size()) - c->kb));
-  };
-  const int g_shift = drop_bias ? bias_shift(c->h_bg_stamp, gyro_min) : 0, a_shift = drop_bias ? bias_shift(c->h_ba_stamp, accel_min) : 0;
-  const int Kbg_new = c->Kbg - g_shift, Kba_new = c->Kba - a_shift;
+  // leading knots go once no kept factor touches them (the smallest bases of the kept factors)
+  const int shift = c->pose.drop_count(lower_bound, knot_min);
+  const int g_shift = drop_bias ? c->gyro.drop_count(lower_bound, gyro_min) : 0, a_shift = drop_bias ? c->accel.drop_count(lower_bound, accel_min) : 0;
   // compaction of the factor lists into their spare copies and of the state into its trial copy, each then switched in
   if (Nv && (rc = compact_visual(c, Nv, c->w_keep.p, c->w_pos.p, c->w_lpos.p, shift, Nv_new))) return rc;
   if (Ni && (rc = compact_inertial(c, Ni, i_keep, i_pos, shift, g_shift, a_shift, Ni_new))) return rc;
@@ -3355,29 +3364,19 @@ int hb200_slide(hb200_ctx* c, double lower_bound, int flags, hb200_slide_stats* 
     HB_LAUNCH(c, "compact_landmarks_kernel");
     c->lms[0].swap(c->lms[1]);
   }
-  const struct { DevBuf<double>* copies; int shift, stride, count; } splines[3] = {{c->knots, shift, 8, K_new}, {c->bg, g_shift, 4, Kbg_new}, {c->ba, a_shift, 4, Kba_new}};
-  for (const auto& s : splines) {
-    if (!s.shift) continue;
-    shift_knots_kernel<<<(s.stride * s.count + 255) / 256, 256, 0, c->stream>>>(s.count, s.shift, s.stride, s.copies[0].p, s.copies[1].p);
-    HB_LAUNCH(c, "shift_knots_kernel");
-    s.copies[0].swap(s.copies[1]);
-  }
+  if ((rc = c->pose.shift(c, shift)) || (rc = c->gyro.shift(c, g_shift)) || (rc = c->accel.shift(c, a_shift))) return rc;
   HB_CUDA(cudaStreamSynchronize(c->stream));
-  // host bookkeeping: sizes, stamps, constancy (elements at or before the lower bound: reference optimizer.cpp:322-328;
-  // gravity once the window no longer covers the whole state range: reference abstract.cpp:57-61)
-  c->h_knot_stamp.erase(c->h_knot_stamp.begin(), c->h_knot_stamp.begin() + shift);
-  c->h_bg_stamp.erase(c->h_bg_stamp.begin(), c->h_bg_stamp.begin() + g_shift);
-  c->h_ba_stamp.erase(c->h_ba_stamp.begin(), c->h_ba_stamp.begin() + a_shift);
-  c->Kbg = Kbg_new; c->Kba = Kba_new; c->bg_dropped = g_shift; c->ba_dropped = a_shift;
-  c->h_knot_const.assign(K_new, 0);
-  for (int j = 0; j < K_new; ++j) c->h_knot_const[j] = c->h_knot_stamp[j] <= lower_bound ? 1 : 0;
+  // host bookkeeping: constancy (elements at or before the lower bound: reference optimizer.cpp:322-328; gravity once
+  // the window no longer covers the whole state range: reference abstract.cpp:57-61) and sizes
+  c->h_knot_const.assign(c->K(), 0);
+  for (int j = 0; j < c->K(); ++j) c->h_knot_const[j] = c->pose.stamp[j] <= lower_bound ? 1 : 0;
   if (ub > 0) c->gravity_const = 1;
-  c->K = K_new; c->L = L_new; c->Nv = Nv_new; c->Np = Nv_new - Nb_new; c->Nb = Nb_new; c->Ni = Ni_new; c->Nm = Nm_new;
+  c->L = L_new; c->Nv = Nv_new; c->Np = Nv_new - Nb_new; c->Nb = Nb_new; c->Ni = Ni_new; c->Nm = Nm_new;
   c->slide_L = L;
   if (stats) {
     stats->knots_dropped = shift; stats->knots_constant = std::max(0, ub - shift); stats->landmarks_dropped = L - L_new;
     stats->visual_factors_dropped = Nv - Nv_new; stats->inertial_factors_dropped = Ni - Ni_new;
-    stats->knots = K_new; stats->landmarks = L_new; stats->visual_factors = Nv_new; stats->inertial_factors = Ni_new;
+    stats->knots = c->K(); stats->landmarks = L_new; stats->visual_factors = Nv_new; stats->inertial_factors = Ni_new;
   }
   c->v_perm.clear(); c->i_perm.clear(); c->have_snapshot = false;
   return derive_window(c, kCallSlide);
@@ -3385,7 +3384,7 @@ int hb200_slide(hb200_ctx* c, double lower_bound, int flags, hb200_slide_stats* 
 
 int hb200_window_sizes(hb200_ctx* c, int* knots, int* landmarks, int* visual_factors, int* inertial_factors) {
   if (!c) return fail(-1, "null context");
-  if (knots) *knots = c->K;
+  if (knots) *knots = c->K();
   if (landmarks) *landmarks = c->L;
   if (visual_factors) *visual_factors = c->Nv;
   if (inertial_factors) *inertial_factors = c->Ni;
